@@ -54,8 +54,10 @@ def parse_args():
     ap.add_argument("--faces", type=int, default=0)
     ap.add_argument("--repeats", type=int, default=0, help="config5: sampled recursive strategies in total (0 = 4097)")
     ap.add_argument("--net", default="auto", choices=["auto", "fp32", "tc", "tcx2"],
-                    help="value-net kernel: tcx2 (default) = tcgen05 fp16 operands with the fast fp32 tanh GELU, tc = the same with the logistic fp32 GELU, fp32 = SIMT parity net")
+                    help="value-net kernel: tcx2 (default) = wgmma fp16 operands with the fast fp32 tanh GELU, tc = the same with the logistic fp32 GELU, fp32 = SIMT parity net")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--cpu-sample", type=int, default=0, help="subgames in the CPU-baseline sample (0 = auto)")
     return ap.parse_args()
 
@@ -80,7 +82,17 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured (MEASURED_PEAKS.json, sustained bf16)"}
-    return {"hbm_gbs": 6650.0, "tflops": 1590.0, "src": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "src": "NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth, dense fp16 tensor rate; not reached"}
+
+
+def dump_outputs(d, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array, float64 kept, everything else as float32."""
+    if not d:
+        return
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
 
 
 class ClockSampler:
@@ -152,6 +164,14 @@ def effective_cores():
 _SCRIPT = {}
 
 
+PORT_FALLBACK = ("oracle/_ref is not built (build() compiles it where a checkout of the original project exists): this baseline is "
+                 "the C port on one thread, NOT the reference's own multi-threaded CPU path")
+
+
+def port_fallback_warning():
+    print("[bench] WARNING: " + PORT_FALLBACK, file=sys.stderr, flush=True)
+
+
 def script_net_file(D, F):
     if (D, F) in _SCRIPT:
         return _SCRIPT[(D, F)]
@@ -187,6 +207,7 @@ def cpu_reference_rate(D, F, iters, n, beliefs, threads=None):
     else:
         import torch  # noqa: F401
         from rebel_b200.models import flatten_state_dict, make_selfplay_net
+        port_fallback_warning()
         port = Oracle("port")
         w = flatten_state_dict(make_selfplay_net(D, F, seed=0).state_dict())
         secs = port.bench_solve(D, F, n, net_w=w, num_iters=iters, beliefs=beliefs[:n])
@@ -195,7 +216,10 @@ def cpu_reference_rate(D, F, iters, n, beliefs, threads=None):
     sample = (f"{n} of the workload's root subgames x {iters} iters, build_solver+multistep with TorchScript Net2 on CPU, {threads} solver "
               f"threads on {cores} usable cores (os.cpu_count()={os.cpu_count()}), {secs:.1f} s wall" if kind == "reference"
               else f"{n} root subgames x {iters} iters, C port, 1 thread, {secs:.1f} s wall")
-    return rate, {"value": rate, "unit": UNIT, "cores": cores if kind == "reference" else 1, "threads": threads, "kind": kind, "sample": sample}
+    info = {"value": rate, "unit": UNIT, "cores": cores if kind == "reference" else 1, "threads": threads, "kind": kind, "sample": sample}
+    if kind == "port":
+        info["warning"] = PORT_FALLBACK
+    return rate, info
 
 
 def run_reference(args):
@@ -223,7 +247,7 @@ def run_reference(args):
         "impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": 1e3 * wall / max(args.steps, 1), "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f64 (CFR) / f32 (value net)", "data": "synthetic",
-        # the workload is the B200 arm's (args.subgames concurrent subgames); each step times a bounded sample of it (cpu_baseline.sample)
+        # the workload is the GPU arm's (args.subgames concurrent subgames); each step times a bounded sample of it (cpu_baseline.sample)
         "config": workload_config(args, args.subgames), "impl_config": {"parallelism": "cpu threads"}, "cpu_baseline": info,
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
@@ -317,7 +341,7 @@ def run_solve(args):
     t_pl = pin((K,), torch.int32); t_pl.zero_()
     t_act = pin((K,), torch.int32); t_act.numpy()[:] = np.random.RandomState(rank).randint(0, iters + 1, size=K)
     stream = torch.cuda.current_stream().cuda_stream
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > the 50 MB L2 of an H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -361,6 +385,8 @@ def run_solve(args):
     launches = S.kernel_launches - launches0
     S.set_profiling(False)
     value = world * K * iters * args.steps / (ms * 1e-3)
+    if rank == 0:                           # the last timed step's root value means, [K][2][H]
+        dump_outputs(args.dump_outputs, {"root_value_means": S.fetch(("root_means",))["root_means"]})
 
     # ================= end to end through the host-buffer C ABI (`e2e`) =================
     ex_all = None
@@ -394,13 +420,7 @@ def run_solve(args):
     n_net = args.steps * iters
     flops_launch = 2.0 * rows * (256 * Q + 256 * 256 + 256 * H)
     avg_net_ms = net_ms / max(n_net, 1)
-    traffic = None   # DRAM bytes per launch of the value-net kernel from the committed ncu --set full capture (same workload only)
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        if is_tc and (D, F, K) == (1, 6, 8192):
-            traffic = [v["dram_bytes_per_launch"] for k, v in tj.items() if "leaf_mlp_tc_kernel" in k][0]
-    except Exception:
-        traffic = None
+    traffic = None   # DRAM bytes per launch: not measured (no hardware-counter profiler on the measuring machines)
     achieved = flops_launch / (avg_net_ms * 1e-3) / 1e12 if avg_net_ms > 0 else 0.0
     roofline = {"bound": "tensor", "kernel": "leaf value net (Net2 forward over all pseudo-leaf rows of the wave)",
                 "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops"],
@@ -413,7 +433,7 @@ def run_solve(args):
     out = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f64 (CFR tables) / " + ("f16 operands, f32 accumulate + LayerNorm, " + ("f32 tanh" if mode == rb.NET_TC_F16X2 else "f32 logistic") + " GELU (value net, tcgen05)" if is_tc else "f32 (value net)"),
+        "dtype": "f64 (CFR tables) / " + ("f16 operands, f32 accumulate + LayerNorm, " + ("f32 tanh" if mode == rb.NET_TC_F16X2 else "f32 logistic") + " GELU (value net, wgmma)" if is_tc else "f32 (value net)"),
         "data": "synthetic", "config": workload_config(args, K),
         "impl_config": {"value_net_kernel": mode_name, "parallelism": f"dp{world}", "l2": "256 MiB memset between steps, inside the timed region"},
         "clocks": clocks,
@@ -481,13 +501,14 @@ def datagen_cpu_baseline(args, seconds=9.0, threads=None):
     if not available("ref_fast"):
         import torch  # noqa: F401
         from rebel_b200.models import flatten_state_dict, make_selfplay_net
+        port_fallback_warning()
         port = Oracle("port")
         w = flatten_state_dict(make_selfplay_net(D, F, seed=0).state_dict())
         t0 = time.time()
         q, v = port.rl_runner(D, F, 0, n_games=4, num_iters=iters, net_w=w, cap=4096)
         dt = time.time() - t0
         rate = len(q) / 2 * iters / dt
-        return {"value": rate, "unit": UNIT, "cores": 1, "threads": 1, "kind": "port",
+        return {"value": rate, "unit": UNIT, "cores": 1, "threads": 1, "kind": "port", "warning": PORT_FALLBACK,
                 "sample": f"4 self-play games ({len(q) // 2} subgames x {iters} iters) of the C port's RlRunner loop, 1 thread, {dt:.1f} s wall"}
     ref = Oracle("ref_fast")
     out = None
@@ -586,7 +607,7 @@ def run_datagen(args):
     if rank == 0 and os.environ.get("BENCH_NO_SAMPLER") != "1":
         sampler.start()
     # warm-up: eager run, CUDA-graph capture, replay — and the start-up transient of a generator: all games begin at the initial state
-    # together, so wave times oscillate (211 / 89 / 190 / 93 ... ms) and settle after ~20 waves (profiles/r2_wave_trend.log); the
+    # together, so the first wave times oscillate (long and short waves alternate) and settle after ~20 waves; the
     # timed steps measure the stationary loop whatever --warmup / --steps are
     for i in range(max(args.warmup, WARMUP_WAVES)):
         S.l2_flush()
@@ -605,6 +626,10 @@ def run_datagen(args):
     finish_and_start(False, True)
     S.mark(1)
     ms = S.elapsed_ms(0, 1)
+    if args.dump_outputs:                           # the last timed wave's training examples, [K][2][Q] and [K][2][H]
+        q_last, v_last = S.selfplay_examples()
+        if rank == 0:
+            dump_outputs(args.dump_outputs, {"examples_query": q_last, "examples_values": v_last})
     barrier()
     if rank == 0:
         sampler.window(t_region0, time.perf_counter())
@@ -716,14 +741,8 @@ def run_datagen(args):
             bytes_subgame += cnt * (4 * H * (E + 6 * E / 2) + 4 * L * (Q + H) + 8 * H)      # SURVEY 8(d), fp32-equivalent algorithmic bytes
     bytes_launch = bytes_subgame / len(prof)
     achieved = flops_launch / (net_us * 1e-6) / 1e12 if net_us > 0 else 0.0
-    traffic = cfr_traffic = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        traffic = tj.get(f"datagen_{D}x{F}_{K}", {}).get("value_net_dram_bytes_per_launch")
-        cfr_traffic = tj.get(f"datagen_{D}x{F}_{K}", {}).get("cfr_dram_bytes_per_launch")
-    except Exception:
-        traffic = cfr_traffic = None
-    roofline = {"bound": "tensor", "kernel": "leaf value net (Net2 forward over all pseudo-leaf rows of the wave, tcgen05)",
+    traffic = cfr_traffic = None    # DRAM bytes per launch: not measured (no hardware-counter profiler on the measuring machines)
+    roofline = {"bound": "tensor", "kernel": "leaf value net (Net2 forward over all pseudo-leaf rows of the wave, wgmma)",
                 "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops"], "traffic": traffic,
                 "traffic_unit": "bytes/launch (ncu dram__bytes_read.sum + dram__bytes_write.sum)", "peak_source": peaks["src"],
                 "avg_launch_ms": net_us * 1e-3, "rows_per_launch": float(rows.mean()), "flops_per_launch": flops_launch,
@@ -739,7 +758,7 @@ def run_datagen(args):
     out = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": steps, "warmup": args.warmup,
         "ms_per_step": ms / steps, "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None,
-        "dtype": "f64 (CFR tables, beliefs) / " + ("f16 operands, f32 accumulate + LayerNorm, " + ("f32 tanh" if mode == rb.NET_TC_F16X2 else "f32 logistic") + " GELU (value net, tcgen05)" if is_tc else "f32 (value net)"),
+        "dtype": "f64 (CFR tables, beliefs) / " + ("f16 operands, f32 accumulate + LayerNorm, " + ("f32 tanh" if mode == rb.NET_TC_F16X2 else "f32 logistic") + " GELU (value net, wgmma)" if is_tc else "f32 (value net)"),
         "data": "synthetic", "config": workload_config(args),
         "impl_config": {"value_net_kernel": mode_name, "parallelism": f"dp{world}", "games_per_gpu": K, "walk": "device (mt19937 streams in HBM)",
                         "replay": "device-resident rows", "l2": "256 MiB memset between steps, inside the timed region; every wave re-initialises its solver tables"},
@@ -827,6 +846,7 @@ def run_config5(args):
             dist.destroy_process_group()
         return
     final = (acc_s / (acc_r + 1e-6)).double().cpu()
+    dump_outputs(args.dump_outputs, {"final_strategy": final.numpy()})   # the averaged strategy the evaluation returns
     e0, e1 = rela.exploitability_of_strategy(D, F, final)
     value = tot_iters / (ms * 1e-3)
     out = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
@@ -848,6 +868,8 @@ def run_reference_config5(args):
     from rebel_b200.models import flatten_state_dict, make_selfplay_net
     D, F, iters = args.dice, args.faces, args.iters
     kind = "ref_fast" if available("ref_fast") else "port"
+    if kind == "port":
+        port_fallback_warning()
     lib = Oracle(kind)
     w = flatten_state_dict(make_selfplay_net(D, F, seed=0).state_dict())
     cores = effective_cores()

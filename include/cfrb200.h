@@ -1,5 +1,5 @@
 /*
- * cfrb200 — C ABI of the B200-native CFR subgame-wave solver (libcfrb200.so).
+ * cfrb200 — C ABI of the H100-native CFR subgame-wave solver (libcfrb200.so).
  *
  * This is the drop-in boundary beneath the reference's pybind11 module `cfvpy.rela`
  * (csrc/liars_dice/rela/pybind.cc:119-213): host orchestration (rebel_b200/csrc/rela/*.cc, the
@@ -61,7 +61,7 @@ enum {
 enum {
   CFRB_NET_ZERO = 0,      /* leaf values are 0 (reference: create_zero_net, real_net.cc:30-55) */
   CFRB_NET_FP32 = 1,      /* fp32 SIMT kernel: parity path, matches libtorch fp32 to ~1e-6 */
-  CFRB_NET_TC_F16 = 2,    /* tcgen05 tensor-core kernel: fp16 operands, fp32 accumulate/LayerNorm/GELU
+  CFRB_NET_TC_F16 = 2,    /* wgmma tensor-core kernel: fp16 operands, fp32 accumulate/LayerNorm/GELU
                              (the reference's own `half_inference` option, selfplay.py:42-43,211) */
   CFRB_NET_TC_F16X2 = 3   /* same kernel with the fast GELU: y/2 (1 + tanh(poly)) with packed f32x2 FMAs and tanh.approx.f32, one
                              rounding to fp16 at the end (same accuracy as mode 2, 1 instead of 2 MUFU operations per element).
@@ -188,8 +188,8 @@ int cfrb_debug_leaf_io(cfrb_handle* h, float* queries, float* net_out, double* s
 /* Debug taps of the tensor-core value net (CFRB_NET_TC_F16 only): re-runs it on the current query tiles and returns
  * the raw fp32 accumulators of layer 1 and layer 2 for the first 128 rows, each [128][256]. */
 int cfrb_debug_net_taps(cfrb_handle* h, float* d1, float* d2);
-/* Development aid: re-runs the tensor-core value net once with clock64() stamps of CTA 0 (out[2048]: epilogue thread 0 at
- * [iter*16 + e], MMA-issuing thread at [1024 + iter*8 + m]; see leaf_mlp_tc.cuh). */
+/* Development aid: re-runs the tensor-core value net once with clock64() stamps of CTA 0 (out[2048]: thread 0 of warpgroup w
+ * at [w*1024 + tile*8 + phase]; see TcArgs in leaf_mlp_tc.cuh). */
 int cfrb_debug_net_trace(cfrb_handle* h, long long* out, int n);
 
 /* Exploitability (best-response values of both players, compute_exploitability2) of a full-tree strategy
@@ -205,7 +205,7 @@ int cfrb_mark(cfrb_handle* h, int32_t slot, void* cuda_stream);
 int cfrb_mark_elapsed_ms(cfrb_handle* h, int32_t a, int32_t b, float* ms);
 int cfrb_mark_wait(cfrb_handle* h, int32_t slot);          /* block until the mark has been reached */
 void* cfrb_handle_stream(cfrb_handle* h);                  /* the handle's own cudaStream_t (what NULL stream arguments mean) */
-/* Overwrite a scratch buffer of `bytes` on the stream (pass more than the 126 MB of L2 to evict it between timed steps). */
+/* Overwrite a scratch buffer of `bytes` on the stream (pass more than the 50 MB of an H100's L2 to evict it between timed steps). */
 int cfrb_l2_flush(cfrb_handle* h, size_t bytes, void* cuda_stream);
 /* Device time in ms of the most recent cfrb_run, and of its value-net kernels only (CUDA events on
  * the launching stream; valid after cfrb_sync). */

@@ -9,7 +9,7 @@
  * Parity status: PINNED.  tests/test_oracle.py checks this file against (a) every known-answer
  * value in the reference's own gtests for this path (tree_test.cc, liars_dice_test.cc,
  * subgame_solving_test.cc thresholds) and (b) outputs of the reference itself compiled from
- * /root/reference (oracle/_ref, see oracle/Makefile + ref_harness.cc) — bit-exact for the zero-net
+ * a checkout of the original project (oracle/_ref, see oracle/Makefile + ref_harness.cc) — bit-exact for the zero-net
  * CFR trajectories when both are built with -ffp-contract=off — and against the committed
  * fixtures in tests/golden/ that were generated from oracle/_ref by oracle/make_golden.py.
  * Covered: game, tree, CFR (linear / vanilla / DCFR), fictitious play (linear / optimistic), terminal
@@ -19,7 +19,7 @@
  * the zero net (eval_net's float32 mean: 1e-7 relative).
  *
  * Every function cites the reference file:line it follows (paths relative to
- * /root/reference/csrc/liars_dice/).
+ * csrc/liars_dice/ of the original project).
  */
 #include <math.h>
 #include <stdint.h>

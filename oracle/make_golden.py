@@ -1,9 +1,9 @@
-"""TEST INFRASTRUCTURE — generates tests/golden/*.npz from the REFERENCE itself (oracle/_ref, built from
-/root/reference by oracle/Makefile).  Run in the build container only:
+"""TEST INFRASTRUCTURE — generates tests/golden/*.npz from the REFERENCE itself (oracle/_ref, built from a checkout of
+the original project by oracle/Makefile).  Run where that checkout exists:
 
-    make -C oracle ref && python oracle/make_golden.py
+    make -C oracle ref REF=<checkout> && python oracle/make_golden.py [live]
 
-The fixtures are what travels to the GPU box (where /root/reference does not exist).  Net weights are NOT stored:
+The fixtures make the tests self-contained: they run without the original project.  Net weights are NOT stored:
 they are re-created from the seed with rebel_b200.models.make_selfplay_net and pinned by a checksum in the fixture.
 """
 import os
@@ -206,5 +206,31 @@ def main():
         print(f, os.path.getsize(os.path.join(OUT, f)))
 
 
+def reference_live():
+    """tests/golden/reference_live.npz: what tests/test_oracle.py compares the C port with — the compiled reference's
+    synthetic beliefs, 40-iteration CFR solves and RlRunner streams, and its Net2 evaluated in the kernels' arithmetic."""
+    R = Oracle("ref_nofma")
+    out = {}
+    for (D, F) in SHAPES:
+        A, H, Q = game_dims(D, F)
+        out[f"beliefs11_{D}x{F}"] = R.synthetic_beliefs(H, 11)
+        b = R.synthetic_beliefs(H, 5)
+        for lb, pl in [(-1, 0), (4, 1)]:
+            y = R.cfr_solve(D, F, b, [0, 1, 5, 40], lb, pl, num_iters=40)
+            for k in ("regrets", "last", "sum", "avg", "root_means", "traverser_values"):
+                out[f"{k}_{lb}_{pl}_{D}x{F}"] = y[k]
+        out[f"q_{D}x{F}"], out[f"v_{D}x{F}"] = R.rl_runner(D, F, seed=3, n_games=2, num_iters=24)
+    D, F = 1, 6
+    A, H, Q = game_dims(D, F)
+    b = R.synthetic_beliefs(H, 3)
+    for model in (0, 1, 2):        # ref_set_net_emulation: 0 = ATen fp32, 1 / 2 = the tensor-core kernels' arithmetic models
+        R.set_net_emulation(model)
+        r = R.cfr_solve(D, F, b, [1], last_bid=-1, player_id=0, num_iters=1, net_w=weights(D, F), want=("avg",))
+        out[f"emulation{model}_leaf_values"] = r["leaf_values"][0]
+        out["emulation_queries"] = r["queries"][0]
+    R.set_net_emulation(0)
+    np.savez_compressed(os.path.join(OUT, "reference_live.npz"), **out)
+
+
 if __name__ == "__main__":
-    main()
+    reference_live() if sys.argv[1:] == ["live"] else main()

@@ -1,6 +1,7 @@
-"""TEST INFRASTRUCTURE — round-2 fixtures generated from the REFERENCE itself (oracle/_ref), build container only:
+"""TEST INFRASTRUCTURE — round-2 fixtures generated from the REFERENCE itself (oracle/_ref), where a checkout of the
+original project exists:
 
-    make -C oracle ref && python oracle/make_golden_r2.py [datagen] [config5] [band]
+    make -C oracle ref REF=<checkout> && python oracle/make_golden_r2.py [datagen] [config5] [band]
 
   datagen_stats.npz   P5 (SURVEY appendix B): the statistic cfvpy/selfplay.py:158-169 logs — per last action (and "initial")
                       the example count, the sum of the targets and the sum of the per-example MSE of the seed-0 Net2 — over
@@ -10,7 +11,7 @@
                       recursive_eval.cc:117-191,343-369) with the seed-0 Net2 evaluated in fp32 by ATen, 1x4f, 1024 iterations:
                       exploitability at powers of two.
   net_band.npz        derived tolerance of the tensor-core value nets: root value means after 1024 iterations when the
-                      REFERENCE's own net is perturbed the way the tcgen05 kernels perturb it — weights rounded to fp16 (fixed),
+                      REFERENCE's own net is perturbed the way the tensor-core kernels perturb it — weights rounded to fp16 (fixed),
                       and on top of that outputs multiplied by 1 + sigma N(0,1), sigma = the measured relative output noise of the
                       kernels (5.4e-4 fp32-GELU, 7.7e-4 packed-half GELU), 8 noise seeds per root.
 """
@@ -74,7 +75,7 @@ def datagen(R, threads=8):
 def datagen_models(R, threads=8):
     """The reference's RlRunner loops with the ARITHMETIC MODEL of the tensor-core value-net kernels inside the reference's own net
     (ref_set_net_emulation: fp16 operands, and for model 2 the packed-half GELU) — what the reference itself generates when its
-    net is evaluated the way the tcgen05 kernels evaluate it.  Added to datagen_stats.npz as count_m{1,2}_* etc."""
+    net is evaluated the way the tensor-core kernels evaluate it.  Added to datagen_stats.npz as count_m{1,2}_* etc."""
     import torch
     torch.set_num_threads(1)
     from rebel_b200.models import make_selfplay_net
@@ -120,7 +121,7 @@ def config5(R, RF=None):
 def band(R):
     """Three perturbations of the reference's own value net, each a model of what the tensor-core kernels do to it:
     w16       the weights of the three Linear layers rounded to fp16 (a FIXED perturbation, identical on every iteration — the
-              dominant, systematic part of the tcgen05 kernels' error),
+              dominant, systematic part of the tensor-core kernels' error),
     pert{0,1} w16 plus independent relative gaussian noise of sigma = 5.4e-4 / 7.7e-4 on every output (the per-call part:
               fp16 activations, approximate GELU), 8 noise seeds."""
     out = {"sigmas": np.array([5.4e-4, 7.7e-4]), "seeds": np.arange(8)}

@@ -36,7 +36,7 @@ def build_port():
 
 
 def build_ref():
-    """Only possible where /root/reference exists (this container, not the GPU box)."""
+    """Only possible where a checkout of the original project exists (REBEL_REFERENCE, default in oracle/Makefile)."""
     subprocess.check_call(["make", "-s", "-j8", "-C", _HERE, "ref"])
 
 
@@ -188,7 +188,7 @@ class Oracle:
         f(float(rel), int(seed))
 
     def set_net_emulation(self, model):
-        """Reference builds only: 0 = the reference's fp32 ATen net, 1 / 2 = arithmetic model of the tcgen05 value-net kernels
+        """Reference builds only: 0 = the reference's fp32 ATen net, 1 / 2 = arithmetic model of the tensor-core value-net kernels
         (fp16 operands; fp32 GELU / packed-half GELU) inside the reference's net, for cfr_solve and rl_runner on this thread."""
         assert self.kind != "port"
         f = self.lib.ref_set_net_emulation

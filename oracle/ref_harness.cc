@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — NOT PRODUCT CODE.
 //
 // Thin extern "C" harness around the UNMODIFIED reference sources compiled where they
-// lie under /root/reference (recipe: oracle/Makefile, output: oracle/_ref/).  It exists so
+// lie in a checkout of the original project (recipe: oracle/Makefile, output: oracle/_ref/).  It exists so
 // that (1) the plain-C restatement in oracle/cfr_oracle.c can be pinned against the real
 // reference, (2) golden fixtures under tests/golden/ can be generated (oracle/make_golden.py)
 // and (3) bench.py's `--impl reference` / `cpu_baseline` leg can time the reference's own
@@ -55,7 +55,7 @@ namespace {
 thread_local std::string g_err;
 thread_local double g_noise_rel = 0;       // ref_set_net_noise: relative gaussian noise on the Net2 outputs of ref_cfr_solve
 thread_local uint64_t g_noise_seed = 0;
-thread_local int g_net_emulation = 0;      // ref_set_net_emulation: 0 fp32 ATen (the reference), 1 / 2 arithmetic model of the tcgen05 kernels
+thread_local int g_net_emulation = 0;      // ref_set_net_emulation: 0 fp32 ATen (the reference), 1 / 2 arithmetic model of the tensor-core kernels
 
 SubgameSolvingParams make_params(int num_iters, int max_depth, int linear_update, int dcfr,
                                  double dcfr_alpha, double dcfr_beta, double dcfr_gamma) {
@@ -88,7 +88,7 @@ class FlatNet2 : public IValueNet {
     w3 = take({H, hidden}); b3 = take({H});
     hidden_ = hidden;
   }
-  // Arithmetic model of the tensor-core value-net kernels (rebel_b200/csrc/leaf_mlp_tc3.cuh) inside the reference's own net, used
+  // Arithmetic model of the tensor-core value-net kernels (rebel_b200/csrc/leaf_mlp_tc.cuh) inside the reference's own net, used
   // to derive parity bands (make_golden_r2.py): query columns, weights and both hidden activations rounded to fp16 (fp32
   // accumulation, fp32 LayerNorm), GELU either in fp32 (model 1, CFRB_NET_TC_F16: the 3-term logistic form) or in packed-half
   // arithmetic with one rounding per HMUL2 / HFMA2 / tanh (model 2, CFRB_NET_TC_F16X2).
@@ -99,7 +99,7 @@ class FlatNet2 : public IValueNet {
       auto p = y2 * (y2 * 1.014244e-3f - 1.0677588e-1f) - 2.3011216f;
       return h16(y / (1.f + torch::exp2(y * p)));
     }
-    // gelu_hy_x2 (leaf_mlp_tc3.cuh): hy = y / 2 rounded to fp16, then HMUL2 / HFMA2 / tanh.approx.f16x2 with one rounding each
+    // gelu_hy_x2 (leaf_mlp_tc.cuh): hy = y / 2 rounded to fp16, then HMUL2 / HFMA2 / tanh.approx.f16x2 with one rounding each
     // (the fp32 product of two fp16 values is exact, so rounding the fp32 result of a*b+c once models the fused HFMA2)
     const float c2 = (float)(at::Half)(-1.124832e-2f), c1 = (float)(at::Half)(2.960456e-1f), c0 = (float)(at::Half)(1.594992f);
     auto hy = h16(0.5f * y);

@@ -1,4 +1,4 @@
-"""rebel_b200 — B200-native CFR self-play data generation for ReBeL / Liar's Dice (hot path only).
+"""rebel_b200 — H100-native CFR self-play data generation for ReBeL / Liar's Dice (hot path only).
 
 Layers: CUDA kernels + C ABI (csrc/, libcfrb200.so, include/cfrb200.h) -> ctypes binding (capi.py) and the C++
 `rela` pybind module mirroring the reference's cfvpy.rela surface -> models.py (PyTorch Net2, Python side only).

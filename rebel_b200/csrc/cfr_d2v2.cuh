@@ -3,8 +3,8 @@
 // Same arithmetic as cfr_backward_d2 / cfr_forward_d2 (cfr_kernels.cuh) — every fp64 operation of the reference's CFR::step
 // (subgame_solving.cc:577-664), update_regrets (:538-575), compute_reach_probabilities (:54-78), write_query_to (:104-123),
 // query_value_net scaling (:253-269) and compute_expected_terminal_values / compute_win_probability (:80-98, :765-789) in the
-// reference's order, so the results are bit-identical — but re-organised around what the ncu profile of generation 1 showed
-// (profiles/r2b_*: 45 % issue-active, 7.4 warps per issue stalled on long_scoreboard, 43 M warp instructions per launch):
+// reference's order, so the results are bit-identical — but re-organised around the long-scoreboard stalls (dependent loads) that
+// limit generation 1:
 //
 //  * STAGING BY THE BULK-COPY ENGINE.  Everything a subgame reads in one launch is contiguous in HBM: its strategy table
 //    (all edges), the regret / sum-strategy rows of the traverser's level, its value-net output rows, scalers and terminal
@@ -303,7 +303,7 @@ __global__ void __launch_bounds__(GT, 8) cfr_iter_d2v2_kernel(CfrDev<real> p, in
     }
   }
   group_sync();
-  // ---- query rows (write_query_to :104-123), fp16 tile in UMMA K-major core-matrix order, one 16-byte store per (row, 8
+  // ---- query rows (write_query_to :104-123), fp16 tile in wgmma K-major core-matrix order, one 16-byte store per (row, 8
   // columns): constant columns from the per-template table, flags, and the two belief blocks from the fp16 values above
   const int leaf_player = rp ^ ((t.levels - 1) & 1);
   const int Qp = p.Qpad;

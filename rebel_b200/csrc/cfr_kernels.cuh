@@ -1,4 +1,4 @@
-// CFR wave kernels (sm_100a): regret matching, strategy averaging, reach / counterfactual-value traversal
+// CFR wave kernels (sm_90a): regret matching, strategy averaging, reach / counterfactual-value traversal
 // for thousands of concurrent Liar's Dice subgames.  Replaces, per iteration and per subgame, the CPU loops
 // of the reference's CFR::step (subgame_solving.cc:577-664), update_regrets (:538-575),
 // compute_reach_probabilities (:54-78), write_query_to (:104-123), query_value_net scaling (:253-269) and
@@ -134,7 +134,7 @@ __device__ void cfr_forward(const CfrDev<real>& p, int k, int trav, real* reach0
   const int leaf_player = rp ^ ((t.levels - 1) & 1);
   const int Qp = p.Qpad;
   if (p.Xh != nullptr) {
-    // fp16 tile in UMMA K-major core-matrix order (leaf_mlp_tc.cuh umma_kmajor_offset_halves, R = 128): one lane produces
+    // fp16 tile in wgmma K-major core-matrix order (leaf_mlp_tc.cuh umma_kmajor_offset_halves, R = 128): one lane produces
     // the 8 contiguous halves of a (row, k-chunk) and stores them with a single 16-byte write; consecutive lanes ->
     // consecutive rows -> contiguous chunks
     const int kc = Qp >> 3;
@@ -850,7 +850,7 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
   const int leaf_player = rp ^ ((t.levels - 1) & 1);
   const int Qp = p.Qpad;
   if (p.Xh != nullptr) {
-    // fp16 tile in UMMA K-major core-matrix order, one 16-byte store per (row, 8 columns).  The constant columns (one-hot of
+    // fp16 tile in wgmma K-major core-matrix order, one 16-byte store per (row, 8 columns).  The constant columns (one-hot of
     // the leaf's last bid, the 1 at column Q, zero padding) come from the per-template table qconst, the acting player /
     // traverser flags are set here, the 2H belief columns are copied from the fp16 rows above.
     const int kc = Qp >> 3;

@@ -33,7 +33,7 @@ struct CfrDev {
   int table_stride;
   real* vterm; int vterm_stride;  // [K][Tmax*H] terminal payoffs of the current iteration
   float* X;                       // [rows][Qpad] fp32 query rows (SIMT net) -- or nullptr
-  __half* Xh;                     // fp16 query tiles in UMMA core-matrix order (tensor-core net) -- or nullptr
+  __half* Xh;                     // fp16 query tiles in wgmma core-matrix order (tensor-core net) -- or nullptr
   const float* net_out;           // [rows][Hout] raw net outputs
   real* scaler;                   // [rows] sum of opponent reach at the pseudo-leaf
   real* scratch; size_t scratch_stride;   // global scratch (CTA groups), reals per subgame

@@ -1,4 +1,4 @@
-// libcfrb200.so — C ABI implementation (include/cfrb200.h) of the B200 CFR wave solver.
+// libcfrb200.so — C ABI implementation (include/cfrb200.h) of the H100 CFR wave solver.
 // Plain CUDA runtime; no torch, no CPU fallback: every entry point that computes needs the device.
 #include "../../include/cfrb200.h"
 
@@ -17,7 +17,6 @@
 #include "cfr_tree.h"
 #include "leaf_mlp_simt.cuh"
 #include "leaf_mlp_tc.cuh"
-#include "leaf_mlp_tc3.cuh"
 
 namespace {
 inline bool is_tc(int net_mode) { return net_mode == CFRB_NET_TC_F16 || net_mode == CFRB_NET_TC_F16X2; }
@@ -114,8 +113,7 @@ struct cfrb_handle {
   DevBuf<int> d_sg_tmpl, d_sg_player, d_sg_row_off, d_sg_act, d_steps;
   DevBuf<float> d_X, d_out, d_dbg;
   long long* dbg_trace = nullptr;   // set only inside cfrb_debug_net_trace
-  int x2_gelu = 2;                  // GELU variant of CFRB_NET_TC_F16X2 (leaf_mlp_tc3.cuh kGelu): 2 = fp32 tanh, 1 = packed half
-  bool tc_gen1 = false;             // CFRB_TC_GEN=1: the round-1 one-tile kernel (leaf_mlp_tc.cuh) instead of leaf_mlp_tc3.cuh
+  int x2_gelu = 2;                  // GELU variant of CFRB_NET_TC_F16X2 (leaf_mlp_tc.cuh kGelu): 2 = fp32 tanh, 1 = packed half
   DevBuf<__half> d_Xh;
   WaveState<float> sf;
   WaveState<double> sd;
@@ -190,7 +188,7 @@ static int alloc_state(cfrb_handle* h, int max_optin) {
     const char* no_d2 = std::getenv("CFRB_NO_D2");
     if (h->max_levels <= 3 && h->tpk_stride > 0 && !(no_d2 && *no_d2 == '1')) {
       // 32 warps per SM (register file: 64 registers x 32 warps) as 8 CTAs of 4 warps: small CTAs even out the last round
-      // (8192 subgames on 4736 warp slots = 1.73 rounds); each CTA has 1 KB of shared memory reserved by the runtime
+      // (8192 subgames on the 4224 warp slots of a 132-SM H100 = 1.94 rounds); each CTA has 1 KB of shared memory reserved by the runtime
       h->d2 = true;
       h->d2_scratch_per_group = cfrb::cfr_scratch_reals_d2((int)sizeof(real), h->Nmax, h->g.H, h->Lmax, h->Tmax, h->n1max);
       const size_t d2_bytes = (size_t)h->d2_scratch_per_group * sizeof(real) + h->tpk_stride;
@@ -199,7 +197,7 @@ static int alloc_state(cfrb_handle* h, int max_optin) {
       if (const char* e = std::getenv("CFRB_D2_GROUPS")) h->d2_groups_per_cta = std::max(1, std::min(h->d2_groups_per_cta, std::atoi(e)));
       h->d2_smem = d2_bytes * h->d2_groups_per_cta;
       // CFRB_D2_CTAS_PER_SM=n: pad the CTA's shared memory so that exactly n CTAs fit an SM (resident warps = n x warps per CTA);
-      // e.g. 7 x 4 = 28 warps make 8192 subgames 1.98 rounds on 148 SMs instead of 1.73 rounds of 32 warps executed as 2
+      // e.g. 7 x 4 = 28 warps per SM
       if (const char* e = std::getenv("CFRB_D2_CTAS_PER_SM")) {
         const int n = std::atoi(e);
         if (n >= 1 && n <= 8) h->d2_smem = std::max(h->d2_smem, ((size_t)227 * 1024 - (size_t)n * 1024) / n / 16 * 16);
@@ -643,24 +641,14 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
     CK(h->d_dbg.alloc(2 * cfrb::tc::kTileM * cfrb::tc::kHid));
     const cfrb::tc::BlobLayout L(h->Qpad);
     if (L.smem_bytes > max_optin) return fail(CFRB_EINVAL, "tensor-core value net does not fit shared memory for this game shape");
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    {
-      const char* gen = std::getenv("CFRB_TC_GEN");
-      h->tc_gen1 = gen && *gen == '1';
-      const cfrb::tc::Tc3Layout T3(h->Qpad);
-      if (T3.smem_bytes > max_optin) return fail(CFRB_EINVAL, "tensor-core value net does not fit shared memory for this game shape");
-      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc3_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3.smem_bytes));
-      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc3_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3.smem_bytes));
-      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc3_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3.smem_bytes));
-      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc3_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3.smem_bytes));
-      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc3_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3.smem_bytes));
-      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc3_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3.smem_bytes));
-      // CFRB_NET_TC_F16X2's GELU: fp32 tanh (default) or the packed-half evaluation (CFRB_X2_GELU=half), see leaf_mlp_tc3.cuh
-      if (const char* e = std::getenv("CFRB_X2_GELU")) h->x2_gelu = std::string(e) == "half" ? 1 : 2;
-    }
+    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
+    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
+    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
+    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
+    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
+    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
+    // CFRB_NET_TC_F16X2's GELU: fp32 tanh (default) or the packed-half evaluation (CFRB_X2_GELU=half), see leaf_mlp_tc.cuh
+    if (const char* e = std::getenv("CFRB_X2_GELU")) h->x2_gelu = std::string(e) == "half" ? 1 : 2;
   }
   CK(cudaFuncSetAttribute(cfrb::leaf_mlp_fp32_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                           (int)cfrb::leaf_mlp_fp32_smem(256)));
@@ -750,39 +738,34 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
   CK(cudaEventSynchronize(h->w_ev[slot]));        // the copy that last used this staging buffer (two uploads ago) is long done
   std::memset(h->w_stage[slot], 0, need);
   if (is_tc(h->cfg.net_mode)) {
-    // tensor-core blob: fp16 weights in UMMA K-major core-matrix order + fp32 {bias, gamma, beta} per feature
+    // tensor-core blob: fp16 weights in wgmma K-major core-matrix order + fp32 {bias, gamma, beta} per feature
     const cfrb::tc::BlobLayout L(Qp);
     struct { uint8_t* p; uint8_t* data() { return p; } } blob{h->w_stage[slot]};
     __half* hw1 = reinterpret_cast<__half*>(blob.data() + L.off_w1);
     __half* hw2 = reinterpret_cast<__half*>(blob.data() + L.off_w2);
     __half* hw3 = reinterpret_cast<__half*>(blob.data() + L.off_w3);
-    // Generation 3 (leaf_mlp_tc3.cuh): LayerNorm without the mean.  Subtracting from every column of W (and from the bias) its
+    // LayerNorm without the mean (leaf_mlp_tc.cuh).  Subtracting from every column of W (and from the bias) its
     // mean over the 256 output features makes the features of y = W x + b sum to zero for every x, which is all the mean
     // subtraction of LayerNorm does; the epilogue then only needs sum y^2.  Done in double, before the fp16 rounding.
-    const bool gen1 = h->tc_gen1;
     std::vector<double> m1(Q + 1, 0.0), m2(hid + 1, 0.0);
-    if (!gen1) {
-      for (int k = 0; k < Q; ++k) { for (int j = 0; j < hid; ++j) m1[k] += w1[(size_t)j * Q + k]; m1[k] /= hid; }
-      for (int j = 0; j < hid; ++j) m1[Q] += b1[j];
-      m1[Q] /= hid;
-      for (int k = 0; k < hid; ++k) { for (int j = 0; j < hid; ++j) m2[k] += w2[(size_t)j * hid + k]; m2[k] /= hid; }
-      for (int j = 0; j < hid; ++j) m2[hid] += b2[j];
-      m2[hid] /= hid;
-    }
+    for (int k = 0; k < Q; ++k) { for (int j = 0; j < hid; ++j) m1[k] += w1[(size_t)j * Q + k]; m1[k] /= hid; }
+    for (int j = 0; j < hid; ++j) m1[Q] += b1[j];
+    m1[Q] /= hid;
+    for (int k = 0; k < hid; ++k) { for (int j = 0; j < hid; ++j) m2[k] += w2[(size_t)j * hid + k]; m2[k] /= hid; }
+    for (int j = 0; j < hid; ++j) m2[hid] += b2[j];
+    m2[hid] /= hid;
     for (int j = 0; j < hid; ++j) for (int k = 0; k < Q; ++k) hw1[cfrb::tc::umma_kmajor_offset_halves(j, k, hid)] = __float2half_rn((float)(w1[(size_t)j * Q + k] - m1[k]));
     for (int j = 0; j < hid; ++j) hw1[cfrb::tc::umma_kmajor_offset_halves(j, Q, hid)] = __float2half_rn((float)(b1[j] - m1[Q]));   // bias 1 x constant-1 column
-    __half* hones = reinterpret_cast<__half*>(blob.data() + L.off_ones);
-    __half* hb2 = reinterpret_cast<__half*>(blob.data() + L.off_bias2);
-    for (int r = 0; r < cfrb::tc::kTileM; ++r) hones[cfrb::tc::umma_kmajor_offset_halves(r, 0, cfrb::tc::kTileM)] = __float2half_rn(1.f);
-    for (int j = 0; j < hid; ++j) hb2[cfrb::tc::umma_kmajor_offset_halves(j, 0, hid)] = __float2half_rn((float)(b2[j] - m2[hid]));
+    float* fb2 = reinterpret_cast<float*>(blob.data() + L.off_b2);      // bias 2, rounded to fp16 like bias 1 in W1
+    for (int j = 0; j < hid; ++j) fb2[j] = __half2float(__float2half_rn((float)(b2[j] - m2[hid])));
     for (int j = 0; j < hid; ++j) for (int k = 0; k < hid; ++k) hw2[cfrb::tc::umma_kmajor_offset_halves(j, k, hid)] = __float2half_rn((float)(w2[(size_t)j * hid + k] - m2[k]));
     for (int j = 0; j < H; ++j) for (int k = 0; k < hid; ++k) hw3[cfrb::tc::umma_kmajor_offset_halves(j, k, cfrb::tc::kNout)] = __float2half_rn(w3[(size_t)j * hid + k]);
     float* ln1 = reinterpret_cast<float*>(blob.data() + L.off_ln1);
     float* ln2 = reinterpret_cast<float*>(blob.data() + L.off_ln2);
-    // generation 3 with the packed-half GELU evaluates the activation from y / 2: gamma / 2 and beta / 2 are stored
-    const float lnscale = (!gen1 && h->cfg.net_mode == CFRB_NET_TC_F16X2) ? 0.5f : 1.f;
+    // the GELU of CFRB_NET_TC_F16X2 evaluates the activation from y / 2: gamma / 2 and beta / 2 are stored
+    const float lnscale = h->cfg.net_mode == CFRB_NET_TC_F16X2 ? 0.5f : 1.f;
     for (int j = 0; j < hid; ++j) {
-      // per feature pair (j even): {gamma_j, gamma_j+1, beta_j, beta_j+1} — the packed operands of the epilogue's fma.f32x2
+      // per feature pair (j even): {gamma_j, gamma_j+1, beta_j, beta_j+1}: one 16-byte load per column pair of the epilogue
       const int o = (j >> 1) * 4 + (j & 1);
       ln1[o] = lnscale * g1[j]; ln1[o + 2] = lnscale * be1[j];
       ln2[o] = lnscale * g2[j]; ln2[o + 2] = lnscale * be2[j];
@@ -889,30 +872,22 @@ static int launch_net(cfrb_handle* h, cudaStream_t st, float* dbg1, float* dbg2)
     const int grid = (h->capturing || h->rows_on_device) ? h->num_sms : std::min(tiles, h->num_sms);   // surplus CTAs return at once
     const bool x2 = h->cfg.net_mode == CFRB_NET_TC_F16X2;
     a.trace = h->dbg_trace;
-    const cfrb::tc::Tc3Layout T3(h->Qpad);
     const bool dbg = dbg1 || dbg2 || a.trace;
     // programmatic dependent launch: the kernel fetches its weights while the CFR kernel before it drains
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(grid); lc.blockDim = dim3(cfrb::tc::kThreads); lc.stream = st;
-    lc.dynamicSmemBytes = h->tc_gen1 ? L.smem_bytes : T3.smem_bytes;
+    lc.dynamicSmemBytes = L.smem_bytes;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     lc.attrs = at; lc.numAttrs = dbg ? 0 : 1;
-    if (h->tc_gen1) {
-      if (dbg && x2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, true>, a));
-      else if (dbg) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, false>, a));
-      else if (x2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<false, true>, a));
-      else CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<false, false>, a));
-    } else {
-      const int gelu = x2 ? h->x2_gelu : 0;
-      if (dbg && gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc3_kernel<true, 1>, a));
-      else if (dbg && gelu == 2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc3_kernel<true, 2>, a));
-      else if (dbg) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc3_kernel<true, 0>, a));
-      else if (gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc3_kernel<false, 1>, a));
-      else if (gelu == 2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc3_kernel<false, 2>, a));
-      else CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc3_kernel<false, 0>, a));
-    }
+    const int gelu = x2 ? h->x2_gelu : 0;
+    if (dbg && gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 1>, a));
+    else if (dbg && gelu == 2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 2>, a));
+    else if (dbg) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 0>, a));
+    else if (gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<false, 1>, a));
+    else if (gelu == 2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<false, 2>, a));
+    else CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<false, 0>, a));
   } else {
     // a wave built on the device: worst-case grid, CTAs beyond the device-side row count return at once
     const int64_t rows_host = h->rows_on_device ? (int64_t)h->n * std::max(h->Lmax, 1) : h->rows;
@@ -1253,7 +1228,7 @@ int cfrb_mark_elapsed_ms(cfrb_handle* h, int32_t a, int32_t b, float* ms) {
   CK(cudaEventElapsedTime(ms, h->marks[a], h->marks[b]));
   return CFRB_OK;
 }
-// Evict the L2 cache: overwrite a scratch buffer of `bytes` (> 126 MB) on the stream, for benchmarks' timed loops.
+// Evict the L2 cache: overwrite a scratch buffer of `bytes` (> the 50 MB L2 of an H100) on the stream, for benchmarks' timed loops.
 int cfrb_l2_flush(cfrb_handle* h, size_t bytes, void* cuda_stream) {
   if (!h || bytes == 0) return fail(CFRB_EINVAL, "cfrb_l2_flush: bad argument");
   CK(cudaSetDevice(h->cfg.device));
@@ -1399,7 +1374,7 @@ int cfrb_debug_div_check(cfrb_handle* h, uint64_t seed, int32_t blocks, uint64_t
 }
 
 // Development / test aid: what the packed-half GELU of the value-net epilogue computes, for every fp16 input.  what = 0:
-// tanh.approx.f16x2 itself; 1 / 2: gelu_hy_x2 / gelu_hy_t32 with hy = the input (leaf_mlp_tc3.cuh).  out[i] = fp16 bits of f(fp16 with bits i).
+// tanh.approx.f16x2 itself; 1 / 2: gelu_hy_x2 / gelu_hy_t32 with hy = the input (leaf_mlp_tc.cuh).  out[i] = fp16 bits of f(fp16 with bits i).
 namespace {
 __global__ void gelu_table_kernel(int what, unsigned short* out) {
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;

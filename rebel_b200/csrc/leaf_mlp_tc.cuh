@@ -1,22 +1,23 @@
 // Tensor-core evaluation of the leaf value net (Net2: Linear -> LayerNorm -> GELU -> Linear -> LayerNorm -> GELU -> Linear,
 // cfvpy/models.py:64-94) for all pseudo-leaf query rows of a wave — the one dense contraction of the CFR hot path and,
-// at 148k FLOP per row, its dominant cost.  Blackwell-native: tcgen05.mma (kind::f16, fp16 operands, fp32 accumulation in
-// TMEM), weights resident in shared memory for the lifetime of a persistent CTA, activations never leave the SM:
+// at 148k FLOP per row, its dominant cost.  Hopper-native: wgmma.mma_async (fp16 operands, fp32 accumulation in registers),
+// weights resident in shared memory for the lifetime of a persistent CTA, activations never leave the registers:
 //
-//   X tile [128 x Kp] fp16 (smem, UMMA K-major core-matrix order, written in that order by the CFR forward kernel)
-//     --tcgen05.mma SS-->  D1 [128 x 256] fp32 in TMEM cols [0,256)
-//     --epilogue (tcgen05.ld, +bias, LayerNorm, GELU, ->fp16, tcgen05.st)-->  A2 [128 x 256] fp16 in TMEM cols [256,384)
-//     --tcgen05.mma TS (A from TMEM, W2 from smem)-->  D2 in TMEM cols [0,256)   (reuses D1's columns)
-//     --epilogue-->  A3 in TMEM cols [256,384)
-//     --tcgen05.mma TS (N = 16)-->  D3 [128 x 16] in TMEM cols [384,400)  --epilogue (+bias)-->  out[rows][H] fp32
+//   X tile [128 x Kp] fp16 (smem, K-major core-matrix order, written in that order by the CFR forward kernel; bulk-copied,
+//   double-buffered)
+//     --wgmma SS-->  D1 [64 x 256] fp32 per warpgroup (two m64n128k16 halves, 128 registers per thread)
+//     --epilogue (LayerNorm, GELU, -> fp16 A fragments in registers)-->
+//     --wgmma RS (A from registers, W2 from smem; accumulators preloaded with bias 2)-->  D2 [64 x 256]
+//     --epilogue-->  --wgmma RS (N = 16)-->  D3 [64 x 16]  --(+ bias 3)-->  out[rows][Hout] fp32
 //
-// Warp roles (544 threads): warps 0-15 = epilogue — warp w owns TMEM lanes 32*(w&3).. (one row per thread) and the column
-// quarter (w>>2), so a thread keeps its 64 accumulators in registers, reads TMEM once per layer and exchanges its LayerNorm
-// partial sums with the three partner warps through shared memory; warp 16 = TMEM allocator + single-thread MMA issuer.
-// The biases ride on the tensor cores: layer 1 through a constant-1 query column (written by the CFR kernel) against a bias
-// column in W1, layer 2 through one extra K=16 MMA of a constant "ones" tile against a bias tile.
-// mbarriers: x (query tile staged), d1/d2/d3 (accumulator ready, via tcgen05.commit), a2/a3 (A operand ready).
-// Each barrier completes exactly once per tile, so one parity bit per tile iteration serves all of them.
+// CTA = two warpgroups; warpgroup w owns rows 64w..64w+63 of every 128-row tile and runs all three layers of them on its own,
+// so the tensor cores work for one warpgroup while the other one is in its epilogue.  The fp32 accumulator fragment of a
+// wgmma is, converted to fp16, exactly the A-register fragment of the next one (a thread holds two rows and, per 8 columns, a
+// column pair), so LayerNorm is a reduction over the four threads of a quad and nothing goes through shared memory.
+// Bias 1 rides on the tensor cores through a constant-1 query column (written by the CFR kernel) against a bias column in W1.
+//
+// LayerNorm without the mean: the rows of W1 / W2 and the biases are centred over the 256 output features on the host
+// (W'[j][k] = W[j][k] - mean_j W[j][k]), so sum_j y_j = 0 by construction and LayerNorm needs only sum_j y_j^2.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -26,37 +27,33 @@ namespace cfrb {
 namespace tc {
 
 constexpr int kHid = 256;
-constexpr int kTileM = 128;
-constexpr int kNout = 16;                 // output features padded to the minimum UMMA N
-constexpr int kParts = 4;                    // column quarters per row
-constexpr int kColsPerThread = kHid / kParts;   // 64
-constexpr int kEpiThreads = 128 * kParts;    // 16 epilogue warps
-constexpr int kSubChunks = 4;                // A-operand hand-over granularity: 16 features per thread
-constexpr int kThreads = kEpiThreads + 32;   // + allocator / MMA-issuer warp
-constexpr uint32_t kColD = 0, kColA = 256, kColD3 = 384, kTmemCols = 512;
+constexpr int kTileM = 128;               // rows of a query tile (the CFR kernel writes tiles of this height)
+constexpr int kWgRows = 64;               // rows per warpgroup (wgmma M)
+constexpr int kNout = 16;                 // output features padded to a wgmma N
+constexpr int kThreads = 2 * 128;         // two warpgroups
 
-// ---- shared-memory / weight-blob layout (bytes).  The blob in global memory has exactly the smem layout up to kOffX.
+// ---- shared-memory / weight-blob layout (bytes).  The blob in global memory has exactly the smem layout up to off_x.
 struct BlobLayout {
   int Kp;            // padded query width (multiple of 16, with at least one spare column for the constant 1)
-  int off_w1, off_w2, off_w3, off_ones, off_bias2, off_ln1, off_ln2, off_b3, blob_bytes, off_x, off_part, off_bar, smem_bytes;
+  int off_w1, off_w2, off_w3, off_b2, off_ln1, off_ln2, off_b3, blob_bytes, x_bytes, off_x, off_xcnt, off_bar, smem_bytes;
   __host__ __device__ explicit BlobLayout(int kp) : Kp(kp) {
     off_w1 = 0;                               // [256 x Kp]  fp16, column Q holds bias 1
     off_w2 = off_w1 + kHid * kp * 2;          // [256 x 256] fp16
     off_w3 = off_w2 + kHid * kHid * 2;        // [16 x 256]  fp16
-    off_ones = off_w3 + kNout * kHid * 2;     // [128 x 16]  fp16, column 0 = 1
-    off_bias2 = off_ones + kTileM * 16 * 2;   // [256 x 16]  fp16, column 0 = bias 2
-    off_ln1 = off_bias2 + kHid * 16 * 2;      // float4 {gamma_j, gamma_j+1, beta_j, beta_j+1} per feature pair
+    off_b2 = off_w3 + kNout * kHid * 2;       // float [256]: bias 2 (rounded to fp16 like the weights)
+    off_ln1 = off_b2 + kHid * 4;              // float4 {gamma_j, gamma_j+1, beta_j, beta_j+1} per feature pair
     off_ln2 = off_ln1 + kHid * 8;
     off_b3 = off_ln2 + kHid * 8;
     blob_bytes = off_b3 + kNout * 4;
-    off_x = (blob_bytes + 127) / 128 * 128;
-    off_part = off_x + kTileM * kp * 2;       // LayerNorm partial sums: [2 layers][kParts][128 rows] float2
-    off_bar = off_part + 2 * kParts * kTileM * 8;
-    smem_bytes = off_bar + 192;            // 16 mbarriers + TMEM base slot
+    x_bytes = kTileM * kp * 2;
+    off_x = (blob_bytes + 127) / 128 * 128;   // two query-tile buffers
+    off_xcnt = off_x + 2 * x_bytes;           // per buffer: warpgroups done with it (monotonic)
+    off_bar = off_xcnt + 16;                  // mbarriers: weights, x[0], x[1]
+    smem_bytes = off_bar + 3 * 8;
   }
 };
 
-// Element (row r, col k) of a K-major [R x K] fp16 operand in UMMA "no swizzle" core-matrix order:
+// Element (row r, col k) of a K-major [R x K] fp16 operand in the no-swizzle core-matrix order of wgmma:
 // 8x8 core matrices of 128 contiguous bytes; row-groups are 128 B apart (SBO), K-chunks R/8*128 B apart (LBO).
 __host__ __device__ inline int umma_kmajor_offset_halves(int r, int k, int R) {
   return (k >> 3) * (R >> 3) * 64 + (r >> 3) * 64 + (r & 7) * 8 + (k & 7);
@@ -68,9 +65,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -80,88 +74,58 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "bra WAIT_LOOP;\n\t"
       "WAIT_DONE:\n\t}" ::"r"(bar), "r"(parity) : "memory");
 }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc),
-      "r"(accumulate) : "memory");
+// Bulk copy global -> shared (the TMA engine without a tensor map); completion is signalled on the mbarrier as transaction bytes.
+__device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_dst), "l"(gsrc),
+               "r"(bytes), "r"(bar) : "memory");
 }
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc),
-      "r"(accumulate) : "memory");
-}
-// UMMA shared-memory descriptor, K-major, SWIZZLE_NONE (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type=0 [61,64).
+
+// wgmma shared-memory matrix descriptor, K-major, no swizzle: start>>4 [0,14), LBO>>4 [16,30) (between the two K core
+// matrices of a K=16 step), SBO>>4 [32,46) (between 8-row groups), layout type 0 [62,64).
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A/B format f16=0 [7,10),[10,13), both K-major,
-// N>>3 at [17,23), M>>4 at [24,29).
-__device__ __forceinline__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Keeps the compiler from moving register reads / writes across the asynchronous wgmma (issue ... wait) window.
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
-#define CFRB_TMEM_LD32(taddr, v)                                                                                          \
-  asm volatile(                                                                                                           \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                           \
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, " \
-      "[%32];"                                                                                                            \
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),      \
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),            \
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),           \
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])                         \
-      : "r"(taddr))
-
-#define CFRB_TMEM_LD16(taddr, v)                                                                                          \
-  asm volatile(                                                                                                           \
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"           \
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),      \
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])                          \
-      : "r"(taddr))
-
-#define CFRB_TMEM_ST16(taddr, v)                                                                                          \
-  asm volatile(                                                                                                           \
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr), \
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),       \
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])                                              \
-      : "memory")
-
-#define CFRB_TMEM_ST8(taddr, v)                                                                                           \
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),  \
-               "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])                                           \
-               : "memory")
-
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// Packed fp32 pairs (Blackwell FFMA2 / FADD2): one issue slot for two lanes' worth of LayerNorm arithmetic.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, A and B in shared memory (descriptors); scale_d = 0 overwrites D.
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
-__device__ __forceinline__ void unpack2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+// D[64 x 128] += A[64 x 16] * B[128 x 16]^T, A in registers (the accumulator layout of the previous layer, packed to fp16).
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t* a, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1u));
 }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+// D[64 x 16] += A[64 x 16] * B[16 x 16]^T, A in registers.
+__device__ __forceinline__ void wgmma_rs_n16(float (&d)[8], const uint32_t* a, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1u));
 }
 
 // GELU(y) = y * Phi(y), Phi(y) = 0.5 (1 + erf(y / sqrt 2)).  erf(z) = tanh(z (a + b z^2 + c z^4)) to 1.0e-4 (fitted, max error
@@ -178,106 +142,79 @@ __device__ __forceinline__ float gelu_tc(float y) {
   return y * r;
 }
 
-// The same function on a packed pair of fp16 values: y * Phi(y) = hy + hy * tanh(y (c0 + c1 y^2 + c2 y^4)), hy = y / 2, with
-// HFMA2 arithmetic and one tanh.approx.f16x2 per pair (a quarter of the MUFU work and ~40 % of the instructions of gelu_tc).
-// The fp16 evaluation adds ~1.8e-4 rms (N(0,1) inputs) to the 1.4e-4 rms of rounding the activation to fp16 at all.
-__device__ __forceinline__ uint32_t gelu_tc_x2(float y0, float y1) {
-  const __half2 y = __floats2half2_rn(y0, y1);
-  const __half2 y2 = __hmin2(__hmul2(y, y), __float2half2_rn(52.f));
-  const __half2 p = __hfma2(y2, __hfma2(y2, __float2half2_rn(-3.5151e-4f), __float2half2_rn(3.70057e-2f)), __float2half2_rn(0.797496f));
-  const __half2 u = __hmul2(y, p);
+// GELU(y) for a packed pair given hy = y / 2:  hy + hy * tanh(hy (c0 + c1 hy^2 + c2 hy^4)) (clamp hy^2 <= 13), with HFMA2
+// arithmetic and one tanh.approx.f16x2 per pair.
+__device__ __forceinline__ uint32_t gelu_hy_x2(float hy0, float hy1) {
+  const __half2 hy = __floats2half2_rn(hy0, hy1);
+  const __half2 s = __hmin2(__hmul2(hy, hy), __float2half2_rn(13.f));
+  const __half2 p = __hfma2(s, __hfma2(s, __float2half2_rn(-1.124832e-2f), __float2half2_rn(2.960456e-1f)), __float2half2_rn(1.594992f));
+  const __half2 u = __hmul2(hy, p);
   uint32_t t;
   asm("tanh.approx.f16x2 %0, %1;" : "=r"(t) : "r"(*reinterpret_cast<const uint32_t*>(&u)));
-  const __half2 hy = __hmul2(y, __float2half2_rn(0.5f));
   const __half2 g = __hfma2(hy, *reinterpret_cast<const __half2*>(&t), hy);
   return *reinterpret_cast<const uint32_t*>(&g);
 }
 
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+// The same function with fp32 arithmetic (tanh.approx.f32) and ONE rounding to fp16 at the end.  tanh.approx.f16x2 truncates
+// towards zero (mean error -2.4e-4 sign(u) on 0.25 <= |u| < 4, one fp16 ulp at most), which gives gelu_hy_x2 a coherent
+// negative bias of 1.6e-4 .. 3.9e-4 on every activation with |y| > 0.5; the data-generation statistics of the self-play loop
+// respond to that bias (tests/test_rela_module.py P5), not to the rounding noise.
+__device__ __forceinline__ float gelu_hy_f32(float hy) {
+  const float s = fminf(__fmul_rn(hy, hy), 13.f);
+  const float p = __fmaf_rn(s, __fmaf_rn(s, -1.124832e-2f, 2.960456e-1f), 1.594992f);
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(__fmul_rn(hy, p)));
+  return __fmaf_rn(hy, t, hy);
+}
+__device__ __forceinline__ uint32_t gelu_hy_t32(float hy0, float hy1) {
+  const __half2 g = __floats2half2_rn(gelu_hy_f32(hy0), gelu_hy_f32(hy1));
+  return *reinterpret_cast<const uint32_t*>(&g);
+}
 
-// LayerNorm(eps 1e-5) + GELU of this thread's quarter row: 64 fp32 accumulators (TMEM lane = row, columns part*64..),
-// bias already added by the tensor cores, kept in registers; the four threads of a row exchange (sum, sum of squares)
-// through `part`.  Result as fp16 into the A-operand columns.  ln: float2 {gamma, beta} per feature in smem (broadcast reads).
-template <bool kDebug, bool kGeluX2>
-__device__ __forceinline__ void epilogue_ln_gelu(uint32_t tmem_row, int part_id, int row, const float2* __restrict__ ln, float2* part,
-                                                 uint32_t bar_a0, uint32_t bar_dfree, float* dbg_row, long long* tr) {
-  uint32_t xr[kColsPerThread];
-  float sum, sumsq;
-  {
-    // the second half of the quarter row is still arriving from TMEM while the first half is summed
-    uint32_t* lo = xr; uint32_t* hi = xr + 32;
-    CFRB_TMEM_LD32(tmem_row + kColD + part_id * kColsPerThread, lo);
-    tmem_wait_ld();
-    CFRB_TMEM_LD32(tmem_row + kColD + part_id * kColsPerThread + 32, hi);
-    if (kDebug && tr) tr[0] = clock64();
-    // two independent accumulator pairs: 2 x 2 interleaved chains of 16 packed adds / fmas instead of one chain of 32
-    f32x2 s2[2], q2[2];
+// kGelu: 0 = fp32 logistic GELU of y (CFRB_NET_TC_F16); 1 = packed-half GELU, 2 = fp32 tanh GELU (both CFRB_NET_TC_F16X2:
+// the LayerNorm parameters in the blob are gamma / 2, beta / 2, so the affine yields hy = y / 2)
+template <int kGelu>
+__device__ __forceinline__ uint32_t act_pair(float y0, float y1) {
+  if (kGelu == 1) return gelu_hy_x2(y0, y1);
+  if (kGelu == 2) return gelu_hy_t32(y0, y1);
+  const __half2 h = __floats2half2_rn(gelu_tc(y0), gelu_tc(y1));
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// LayerNorm (eps 1e-5, mean-free, see above) + GELU of a warpgroup's 64 x 256 accumulators, packed to fp16 as the A fragments of
+// the next layer's wgmma: K-step kk = 8h + i/2 takes act[4kk .. 4kk+3].  A thread holds rows r and r + 8 (d[4i], d[4i+1] and
+// d[4i+2], d[4i+3]) at columns 128h + 8i + 2q + {0, 1}, q = lane & 3; the four threads of a quad share the rows.
+// ln: float4 {gamma_j, gamma_j+1, beta_j, beta_j+1} per feature pair.
+template <int kGelu>
+__device__ __forceinline__ void ln_gelu(const float (&acc)[2][64], const float4* __restrict__ ln, int q, uint32_t (&act)[64]) {
+  float s[4] = {0.f, 0.f, 0.f, 0.f};        // (row r, row r + 8) x two independent chains
 #pragma unroll
-    for (int u = 0; u < 2; ++u) { s2[u] = pack2(0.f, 0.f); q2[u] = pack2(0.f, 0.f); }
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      if (half == 1) tmem_wait_ld();
-#pragma unroll
-      for (int i = half * 32; i < half * 32 + 32; i += 2) {
-        if (kDebug && dbg_row) {
-          dbg_row[part_id * kColsPerThread + i] = __uint_as_float(xr[i]);
-          dbg_row[part_id * kColsPerThread + i + 1] = __uint_as_float(xr[i + 1]);
-        }
-        const f32x2 x2 = pack2(__uint_as_float(xr[i]), __uint_as_float(xr[i + 1]));
-        s2[(i >> 1) & 1] = add2(s2[(i >> 1) & 1], x2);
-        q2[(i >> 1) & 1] = fma2(x2, x2, q2[(i >> 1) & 1]);
-      }
+    for (int i = 0; i < 16; ++i) {
+      const int c = (i & 1) * 2;
+      s[c] = fmaf(acc[h][4 * i], acc[h][4 * i], s[c]);
+      s[c] = fmaf(acc[h][4 * i + 1], acc[h][4 * i + 1], s[c]);
+      s[c + 1] = fmaf(acc[h][4 * i + 2], acc[h][4 * i + 2], s[c + 1]);
+      s[c + 1] = fmaf(acc[h][4 * i + 3], acc[h][4 * i + 3], s[c + 1]);
     }
-    const f32x2 st = add2(s2[0], s2[1]), qt = add2(q2[0], q2[1]);
-    float a0, a1, b0, b1;
-    unpack2(st, a0, a1); unpack2(qt, b0, b1);
-    sum = a0 + a1; sumsq = b0 + b1;
-  }
-  part[part_id * kTileM + row] = make_float2(sum, sumsq);
-  if (kDebug && tr) tr[1] = clock64();
-  named_bar_sync(1, kEpiThreads);
-  // every accumulator of the tile now lives in registers: the D columns may be overwritten (next tile's layer 1)
-  if (bar_dfree) {
-    tc_fence_before();
-    mbar_arrive(bar_dfree);
-  }
-  if (kDebug && tr) tr[2] = clock64();
-  sum = 0.f; sumsq = 0.f;
+  float lo = s[0] + s[2], hi = s[1] + s[3];
+  lo += __shfl_xor_sync(0xffffffffu, lo, 1);
+  hi += __shfl_xor_sync(0xffffffffu, hi, 1);
+  lo += __shfl_xor_sync(0xffffffffu, lo, 2);
+  hi += __shfl_xor_sync(0xffffffffu, hi, 2);
+  // the rows of W and the biases are centred over the features on the host: the mean of the 256 accumulators is zero
+  const float rstd_lo = rsqrtf(lo * (1.f / kHid) + 1e-5f), rstd_hi = rsqrtf(hi * (1.f / kHid) + 1e-5f);
 #pragma unroll
-  for (int p = 0; p < kParts; ++p) {          // fixed order: all four threads of a row get bit-identical statistics
-    const float2 o = part[p * kTileM + row];
-    sum += o.x; sumsq += o.y;
-  }
-  const float mean = sum * (1.f / kHid);
-  const float var = fmaxf(sumsq * (1.f / kHid) - mean * mean, 0.f);
-  const float rstd = rsqrtf(var + 1e-5f);
-  const float shift = -mean * rstd;
-  const f32x2 rstd2 = pack2(rstd, rstd), shift2 = pack2(shift, shift);
-  // Four sub-chunks of 16 features: sub-chunk s of column quarter q is K-step 4q+s of the next layer's MMA, so after the
-  // s-th arrival of all epilogue threads the issuer can run K-steps {s, 4+s, 8+s, 12+s} while the rest is still being
-  // normalised (only the last quarter of the MMA stays exposed).
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-  for (int c = 0; c < kSubChunks; ++c) {
-    uint32_t pk[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int j = c * 16 + 2 * i;
-      const float4 pp = *reinterpret_cast<const float4*>(ln + part_id * kColsPerThread + j);   // {gamma_j, gamma_j+1, beta_j, beta_j+1}
-      float y0, y1;
-      unpack2(fma2(fma2(pack2(__uint_as_float(xr[j]), __uint_as_float(xr[j + 1])), rstd2, shift2), pack2(pp.x, pp.y), pack2(pp.z, pp.w)), y0, y1);
-      if (kGeluX2) {
-        pk[i] = gelu_tc_x2(y0, y1);
-      } else {
-        const __half2 h = __floats2half2_rn(gelu_tc(y0), gelu_tc(y1));
-        pk[i] = *reinterpret_cast<const uint32_t*>(&h);
-      }
+    for (int i = 0; i < 16; ++i) {
+      const float4 pp = ln[h * 64 + i * 4 + q];
+      act[h * 32 + 2 * i] = act_pair<kGelu>(__fmaf_rn(__fmul_rn(acc[h][4 * i], rstd_lo), pp.x, pp.z),
+                                            __fmaf_rn(__fmul_rn(acc[h][4 * i + 1], rstd_lo), pp.y, pp.w));
+      act[h * 32 + 2 * i + 1] = act_pair<kGelu>(__fmaf_rn(__fmul_rn(acc[h][4 * i + 2], rstd_hi), pp.x, pp.z),
+                                                __fmaf_rn(__fmul_rn(acc[h][4 * i + 3], rstd_hi), pp.y, pp.w));
     }
-    CFRB_TMEM_ST8(tmem_row + kColA + part_id * (kColsPerThread / 2) + c * 8, pk);
-    tmem_wait_st();
-    tc_fence_before();
-    mbar_arrive(bar_a0 + 8 * c);
-  }
-  if (kDebug && tr) tr[3] = clock64();
 }
 
 struct TcArgs {
@@ -288,194 +225,152 @@ struct TcArgs {
   int Kp, H, Hout;
   float* dbg_d1;            // optional [128][256] raw layer-1 accumulators of tile 0
   float* dbg_d2;            // optional [128][256] raw layer-2 accumulators of tile 0
-  long long* trace;         // optional (debug build only): SM clock stamps of CTA 0, [2048]: epilogue thread 0 at
-                            // [iter*16 + e], MMA thread at [1024 + iter*8 + m]
+  long long* trace;         // optional (debug build only): SM clock stamps of CTA 0, [2048]: thread 0 of warpgroup w at
+                            // [w * 1024 + j * 8 + e] for its j-th tile (j < 64): e = 0 query tile ready, 1 layer 1 done,
+                            // 2 epilogue 1 done, 3 layer 2 done, 4 epilogue 2 done, 5 outputs written
 };
 
-#define CFRB_TRACE(slot)                                                      \
-  do {                                                                        \
-    if (kDebug && a.trace && blockIdx.x == 0 && it_no < 60) a.trace[slot] = clock64(); \
-  } while (0)
-
-template <bool kDebug, bool kGeluX2>
+template <bool kDebug, int kGelu>
 __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_kernel(TcArgs a) {
-  constexpr int kMmaWarp = kEpiThreads / 32;
-  extern __shared__ __align__(1024) uint8_t smem[];
+  extern __shared__ __align__(128) uint8_t smem[];
   const BlobLayout L(a.Kp);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, lt = tid & 127, warp = lt >> 5, lane = tid & 31;
   const int rows = *a.rows_ptr;
   const int ntiles = (rows + kTileM - 1) / kTileM;
   if ((int)blockIdx.x >= ntiles) return;
+  const int J = (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1;      // tiles of this CTA: blockIdx.x + j * gridDim.x
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bar);
-  // bars: 0 x, 1 d1, 2 d2, 3 d3, 4 dfree, 8..11 a2[sub-chunk], 12..15 a3[sub-chunk]
-  const uint32_t bar_x = smem_u32(bars + 0), bar_d1 = smem_u32(bars + 1), bar_d2 = smem_u32(bars + 2), bar_d3 = smem_u32(bars + 3),
-                 bar_dfree = smem_u32(bars + 4), bar_a2 = smem_u32(bars + 8), bar_a3 = smem_u32(bars + 12);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-
-  // ---- one-time setup: weights -> smem, barriers, TMEM
-  {
-    const int4* src = reinterpret_cast<const int4*>(a.blob);
-    int4* dst = reinterpret_cast<int4*>(smem);
-    for (int i = tid; i < L.blob_bytes / 16; i += kThreads) dst[i] = __ldg(src + i);
-  }
+  const uint32_t bar_w = smem_u32(bars + 0), bar_x = smem_u32(bars + 1);   // x buffer b: bar_x + 8 b
+  int* xcnt = reinterpret_cast<int*>(smem + L.off_xcnt);
   if (tid == 0) {
-    mbar_init(bar_x, kEpiThreads); mbar_init(bar_d1, 1); mbar_init(bar_d2, 1); mbar_init(bar_d3, 1);
-    mbar_init(bar_dfree, kEpiThreads);
-    for (int c = 0; c < kSubChunks; ++c) { mbar_init(bar_a2 + 8 * c, kEpiThreads); mbar_init(bar_a3 + 8 * c, kEpiThreads); }
+    mbar_init(bar_w, 1); mbar_init(bar_x, 1); mbar_init(bar_x + 8, 1);
+    xcnt[0] = 0; xcnt[1] = 0;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_proxy_async_smem();          // generic-proxy weight stores -> visible to the tensor-core (async) proxy
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Everything above (weights -> shared memory, barriers, TMEM) is independent of the CFR kernel that precedes this launch:
-  // with programmatic dependent launch it runs while that kernel drains.  From here on its query tiles are read.
+  // weights: independent of the CFR kernel that precedes this launch -> fetched while that kernel drains (programmatic
+  // dependent launch); the query tiles are read only after griddepcontrol.wait
+  if (tid == 0) {
+    mbar_expect_tx(bar_w, (uint32_t)L.blob_bytes);
+    for (int o = 0; o < L.blob_bytes; o += 32768)
+      bulk_g2s(smem_u32(smem + o), a.blob + o, (uint32_t)min(32768, L.blob_bytes - o), bar_w);
+  }
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;");
 
   const uint32_t sx = smem_u32(smem + L.off_x), sw1 = smem_u32(smem + L.off_w1), sw2 = smem_u32(smem + L.off_w2),
-                 sw3 = smem_u32(smem + L.off_w3), sones = smem_u32(smem + L.off_ones), sbias2 = smem_u32(smem + L.off_bias2);
-  const int x_tile_int4 = kTileM * a.Kp * 2 / 16;
+                 sw3 = smem_u32(smem + L.off_w3);
+  const uint8_t* xg = reinterpret_cast<const uint8_t*>(a.Xh);
+  auto tile_of = [&](int j) { return (int)blockIdx.x + j * (int)gridDim.x; };
+  auto fetch_x = [&](int j) {                   // query tile of the CTA's j-th tile -> x buffer j & 1
+    const uint32_t b = bar_x + 8 * (j & 1);
+    mbar_expect_tx(b, (uint32_t)L.x_bytes);
+    bulk_g2s(sx + (j & 1) * (uint32_t)L.x_bytes, xg + (size_t)tile_of(j) * L.x_bytes, (uint32_t)L.x_bytes, b);
+  };
+  if (tid == 0) {
+    fetch_x(0);
+    if (J > 1) fetch_x(1);
+  }
+  mbar_wait(bar_w, 0);
 
-  if (warp == kMmaWarp) {
-    // ===================== MMA issuer (one thread) =====================
-    if (lane == 0) {
-      const uint32_t idesc256 = make_idesc(kTileM, kHid), idesc16 = make_idesc(kTileM, kNout);
-      const uint32_t lbo_x = (kTileM / 8) * 128, lbo_w = (kHid / 8) * 128, lbo_w3 = (kNout / 8) * 128;
-      // Layer 1 of tile n+1 is issued inside iteration n, as soon as the epilogue warps hold tile n's layer-2 accumulators in
-      // registers (dfree) — the D columns are free then and the tensor pipe would otherwise idle through epilogue 2.
-      mbar_wait(bar_x, 0);
-      tc_fence_after();
-      for (int k = 0; k < a.Kp / 16; ++k)
-        mma_ss(tmem_base + kColD, make_desc(sx + k * 2 * lbo_x, lbo_x, 128), make_desc(sw1 + k * 2 * lbo_w, lbo_w, 128), idesc256, k > 0);
-      tc_commit(bar_d1);
-      uint32_t parity = 0;
-      int it_no = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, parity ^= 1, ++it_no) {
-        // layer 2: D2 = ones * bias2^T + A2 * W2^T  (A from TMEM: 16 fp16 = 8 columns per K step), K-steps in the order the
-        // epilogue hands them over
-        for (int c = 0; c < kSubChunks; ++c) {
-          mbar_wait(bar_a2 + 8 * c, parity);
-          tc_fence_after();
-          if (c == 0) {
-            CFRB_TRACE(1024 + it_no * 8 + 2);
-            mma_ss(tmem_base + kColD, make_desc(sones, lbo_x, 128), make_desc(sbias2, lbo_w, 128), idesc256, 0);
-          }
-          for (int q = 0; q < kParts; ++q) {
-            const int k = q * kSubChunks + c;
-            mma_ts(tmem_base + kColD, tmem_base + kColA + k * 8, make_desc(sw2 + k * 2 * lbo_w, lbo_w, 128), idesc256, 1);
-          }
-        }
-        tc_commit(bar_d2);
-        CFRB_TRACE(1024 + it_no * 8 + 3);
-        // layer 1 of the next tile
-        if (tile + (int)gridDim.x < ntiles) {
-          mbar_wait(bar_dfree, parity);
-          mbar_wait(bar_x, parity ^ 1);
-          tc_fence_after();
-          CFRB_TRACE(1024 + it_no * 8 + 0);
-          for (int k = 0; k < a.Kp / 16; ++k)
-            mma_ss(tmem_base + kColD, make_desc(sx + k * 2 * lbo_x, lbo_x, 128), make_desc(sw1 + k * 2 * lbo_w, lbo_w, 128), idesc256, k > 0);
-          tc_commit(bar_d1);
-          CFRB_TRACE(1024 + it_no * 8 + 1);
-        }
-        // layer 3: D3 = A3 * W3^T  (N = 16)
-        for (int c = 0; c < kSubChunks; ++c) {
-          mbar_wait(bar_a3 + 8 * c, parity);
-          tc_fence_after();
-          if (c == 0) CFRB_TRACE(1024 + it_no * 8 + 4);
-          for (int q = 0; q < kParts; ++q) {
-            const int k = q * kSubChunks + c;
-            mma_ts(tmem_base + kColD3, tmem_base + kColA + k * 8, make_desc(sw3 + k * 2 * lbo_w3, lbo_w3, 128), idesc16, (c | q) != 0);
-          }
-        }
-        tc_commit(bar_d3);
-        CFRB_TRACE(1024 + it_no * 8 + 5);
-      }
-    }
-  } else {
-    // ===================== epilogue warps: thread == (row, column quarter) =====================
-    const int quad = warp & 3, part_id = warp >> 2;
-    const int row_in_tile = quad * 32 + lane;                      // 0..127 == TMEM lane
-    const uint32_t tmem_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const float2* ln1 = reinterpret_cast<const float2*>(smem + L.off_ln1);
-    const float2* ln2 = reinterpret_cast<const float2*>(smem + L.off_ln2);
-    const float* b3 = reinterpret_cast<const float*>(smem + L.off_b3);
-    float2* part1 = reinterpret_cast<float2*>(smem + L.off_part);
-    float2* part2 = part1 + kParts * kTileM;
-    int4* xdst = reinterpret_cast<int4*>(smem + L.off_x);
-    const int x_items = x_tile_int4;                               // 512 or 768 int4 per tile: <= 2 per thread
-    int4 xr0, xr1;
-    {
-      const int4* xsrc = reinterpret_cast<const int4*>(a.Xh) + (size_t)blockIdx.x * x_tile_int4;
-      for (int i = tid; i < x_items; i += kEpiThreads) xdst[i] = __ldg(xsrc + i);
-      fence_proxy_async_smem();
-      mbar_arrive(bar_x);
-    }
-    uint32_t parity = 0;
-    int it_no = tid == 0 ? 0 : 1 << 20;     // only thread 0 leaves trace stamps
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, parity ^= 1, ++it_no) {
-      const int next = tile + gridDim.x;
-      const bool dbg = (tile == 0);
-      // ---- layer-1 accumulators ready; the query tile in smem is free again -> start fetching the next one
-      mbar_wait(bar_d1, parity);
-      tc_fence_after();
-      CFRB_TRACE(it_no * 16 + 0);
-      if (next < ntiles) {
-        const int4* xsrc = reinterpret_cast<const int4*>(a.Xh) + (size_t)next * x_tile_int4;
-        xr0 = __ldg(xsrc + tid);
-        if (tid + kEpiThreads < x_items) xr1 = __ldg(xsrc + tid + kEpiThreads);
-      }
-      epilogue_ln_gelu<kDebug, kGeluX2>(tmem_row, part_id, row_in_tile, ln1, part1, bar_a2, 0u, (dbg && a.dbg_d1) ? a.dbg_d1 + row_in_tile * kHid : nullptr,
-                                        (kDebug && a.trace && blockIdx.x == 0 && it_no < 60) ? a.trace + it_no * 16 + 7 : nullptr);
-      CFRB_TRACE(it_no * 16 + 1);
-      if (next < ntiles) {
-        xdst[tid] = xr0;
-        if (tid + kEpiThreads < x_items) xdst[tid + kEpiThreads] = xr1;
-        fence_proxy_async_smem();
-        mbar_arrive(bar_x);
-      }
-      // ---- layer 2
-      CFRB_TRACE(it_no * 16 + 2);
-      mbar_wait(bar_d2, parity);
-      tc_fence_after();
-      CFRB_TRACE(it_no * 16 + 3);
-      epilogue_ln_gelu<kDebug, kGeluX2>(tmem_row, part_id, row_in_tile, ln2, part2, bar_a3, next < ntiles ? bar_dfree : 0u,
-                                        (dbg && a.dbg_d2) ? a.dbg_d2 + row_in_tile * kHid : nullptr,
-                                        (kDebug && a.trace && blockIdx.x == 0 && it_no < 60) ? a.trace + it_no * 16 + 11 : nullptr);
-      CFRB_TRACE(it_no * 16 + 4);
-      // ---- layer 3: raw net outputs (the CFR backward kernel multiplies by the opponent-reach scaler)
-      mbar_wait(bar_d3, parity);
-      tc_fence_after();
-      CFRB_TRACE(it_no * 16 + 5);
-      if (part_id == 0) {
-        uint32_t v[16];
-        CFRB_TMEM_LD16(tmem_row + kColD3, v);
-        tmem_wait_ld();
-        const int row = tile * kTileM + row_in_tile;
-        if (row < rows) {
-          float* o = a.out + (size_t)row * a.Hout;
+  const float4* ln1 = reinterpret_cast<const float4*>(smem + L.off_ln1);
+  const float4* ln2 = reinterpret_cast<const float4*>(smem + L.off_ln2);
+  const float* b2 = reinterpret_cast<const float*>(smem + L.off_b2);
+  const float* b3 = reinterpret_cast<const float*>(smem + L.off_b3);
+  const int q = lane & 3;
+  const int r_lo = warp * 16 + (lane >> 2);     // this thread's rows within the warpgroup's 64: r_lo and r_lo + 8
+  // K-major core-matrix strides: LBO = next 8 columns of K, SBO = next 8 rows
+  const uint32_t lbo_x = (kTileM / 8) * 128, lbo_w = (kHid / 8) * 128, lbo_w3 = (kNout / 8) * 128;
+  float acc[2][64];
+  uint32_t act[64];
+
+#define CFRB_TRACE(e)                                                                                 \
+  do {                                                                                                \
+    if (kDebug && a.trace && blockIdx.x == 0 && lt == 0 && j < 64) a.trace[wg * 1024 + j * 8 + (e)] = clock64(); \
+  } while (0)
+  auto tap = [&](float* dbg, int tile) {        // raw accumulators of tile 0 (debug build)
+    if (kDebug && dbg && tile == 0) {
 #pragma unroll
-          for (int h = 0; h < kNout; ++h) if (h < a.H) o[h] = __uint_as_float(v[h]) + b3[h];
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            dbg[(wg * kWgRows + r_lo + (e >> 1) * 8) * kHid + h * 128 + i * 8 + 2 * q + (e & 1)] = acc[h][4 * i + e];
+    }
+  };
+
+  for (int j = 0; j < J; ++j) {
+    const int tile = tile_of(j), buf = j & 1;
+    const uint32_t xb = sx + buf * (uint32_t)L.x_bytes + wg * (kWgRows / 8) * 128;
+    mbar_wait(bar_x + 8 * buf, (j >> 1) & 1);
+    CFRB_TRACE(0);
+    // ---- layer 1: D1 = X W1'^T (bias 1 through the constant-1 query column)
+    wgmma_fence();
+#pragma unroll 1
+    for (int kk = 0; kk < a.Kp / 16; ++kk) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        wgmma_ss_n128(acc[h], make_desc(xb + kk * 2 * lbo_x, lbo_x, 128), make_desc(sw1 + kk * 2 * lbo_w + h * 2048, lbo_w, 128), kk > 0);
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_regs(acc[0]); fence_regs(acc[1]);
+    // wgmma.wait_group covers only the calling warp's reads of the buffer: all four warps of the warpgroup meet first (named
+    // barrier 1 + wg), then the second warpgroup to get here refills the buffer with the tile two ahead
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    if (lt == 0 && (atomicAdd(&xcnt[buf], 1) & 1) && j + 2 < J) fetch_x(j + 2);
+    tap(a.dbg_d1, tile);
+    CFRB_TRACE(1);
+    ln_gelu<kGelu>(acc, ln1, q, act);
+    CFRB_TRACE(2);
+    // ---- layer 2: D2 = bias2 + A2 W2'^T, A2 from registers
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float2 bb = *reinterpret_cast<const float2*>(b2 + h * 128 + i * 8 + 2 * q);
+        acc[h][4 * i] = bb.x; acc[h][4 * i + 1] = bb.y; acc[h][4 * i + 2] = bb.x; acc[h][4 * i + 3] = bb.y;
+      }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kHid / 16; ++kk) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) wgmma_rs_n128(acc[h], act + 4 * kk, make_desc(sw2 + kk * 2 * lbo_w + h * 2048, lbo_w, 128));
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_regs(acc[0]); fence_regs(acc[1]); fence_regs(act);
+    tap(a.dbg_d2, tile);
+    CFRB_TRACE(3);
+    ln_gelu<kGelu>(acc, ln2, q, act);
+    CFRB_TRACE(4);
+    // ---- layer 3: raw net outputs (the CFR backward kernel multiplies by the opponent-reach scaler)
+    float o[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kHid / 16; ++kk) wgmma_rs_n16(o, act + 4 * kk, make_desc(sw3 + kk * 2 * lbo_w3, lbo_w3, 128));
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_regs(o); fence_regs(act);
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int row = tile * kTileM + wg * kWgRows + r_lo + 8 * e;
+      if (row < rows) {                         // rows are Hout floats apart, Hout a multiple of 4
+        float* orow = a.out + (size_t)row * a.Hout;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int c = i * 8 + 2 * q;
+          if (c < a.Hout) *reinterpret_cast<float2*>(orow + c) = make_float2(o[4 * i + 2 * e] + b3[c], o[4 * i + 2 * e + 1] + b3[c + 1]);
         }
       }
-      CFRB_TRACE(it_no * 16 + 6);
-      tc_fence_before();   // order this tile's TMEM reads before the next tile's MMAs (via the a2/a3/x arrivals that follow)
     }
+    CFRB_TRACE(5);
   }
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
-  }
+#undef CFRB_TRACE
 }
 
 }  // namespace tc

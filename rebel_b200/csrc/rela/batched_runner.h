@@ -1,4 +1,4 @@
-// BatchedRlRunner: self-play of K Liar's Dice games in lock-step on one GPU — the B200 counterpart of the reference's
+// BatchedRlRunner: self-play of K Liar's Dice games in lock-step on one GPU — the GPU counterpart of the reference's
 // RlRunner (recursive_solving.h:40-86, recursive_solving.cc:160-275), which plays ONE game per CPU thread.
 //
 // A "wave" solves the current subgame of every game at once through the C ABI (include/cfrb200.h).  Two drivers:

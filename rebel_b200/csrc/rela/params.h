@@ -1,7 +1,7 @@
 // Parameter structs mirrored to Python by the `rela` module, field for field like the reference's
 // liars_dice::SubgameSolvingParams (subgame_solving.h:43-58) and RecursiveSolvingParams (recursive_solving.h:31-38).
 // cfvpy/selfplay.py fills them with setattr from cfg.env (selfplay.py:587-610) and raises on unknown keys, so the
-// B200-specific knobs below are ordinary extra fields with defaults: they can be set as `env.concurrent_games=...`
+// GPU-specific knobs below are ordinary extra fields with defaults: they can be set as `env.concurrent_games=...`
 // without touching selfplay.py, and are invisible to configs that do not mention them.
 #pragma once
 #include <cstdlib>
@@ -33,7 +33,7 @@ struct RecursiveSolvingParams {
   SubgameSolvingParams subgame_params;
   // ---- rebel_b200 extensions
   int concurrent_games = env_int("CFRB_CONCURRENT_GAMES", 1024);   // self-play games advanced in lock-step per thread loop
-  int net_mode = env_int("CFRB_NET_MODE", 3);                      // include/cfrb200.h CFRB_NET_*: 3 = tcgen05 fp16 operands, fast tanh GELU
+  int net_mode = env_int("CFRB_NET_MODE", 3);                      // include/cfrb200.h CFRB_NET_*: 3 = wgmma fp16 operands, fast tanh GELU
   int state_dtype = env_int("CFRB_STATE_DTYPE", 0);                // CFRB_STATE_*: 0 = fp64 tables
   int host_walk = env_int("CFRB_HOST_WALK", 0);                    // 1 = per-game sampling on the host (parity mode of the device walk)
 };

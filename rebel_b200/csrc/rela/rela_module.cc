@@ -25,7 +25,7 @@ namespace {
 
 // One process per GPU (torchrun): NCCL communicator of libcfrb200 (cfrb_comm_*, include/cfrb200.h).  The reference has no
 // multi-process mode — its generator threads share the trainer's replay and model replicas inside one process — so this is the
-// B200 counterpart of those two shared objects: ModelLocker.update_model becomes a broadcast from the trainer's rank, and a
+// GPU counterpart of those two shared objects: ModelLocker.update_model becomes a broadcast from the trainer's rank, and a
 // generator loop hands every wave's examples to the trainer rank's device-resident replay with grouped send / recv.
 class Comm {
  public:

@@ -50,7 +50,7 @@ def main(argv=None):
     ap.add_argument("--no_full_tree", action="store_true", help="skip the full-tree solve the reference binary always starts with")
     ap.add_argument("--batch_repeats", type=int, default=64)
     ap.add_argument("--wave_capacity", type=int, default=8192)
-    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 tcgen05 fp16, 3 tcgen05 fp16 + packed-half GELU (default with --net)")
+    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast fp32-tanh GELU (default with --net)")
     ap.add_argument("--random_net_seed", type=int, default=None, help="use a random-init Net2 (benchmarks)")
     args = ap.parse_args(argv)
 

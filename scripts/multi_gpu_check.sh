@@ -1,7 +1,8 @@
 #!/bin/bash
-# 2-GPU box: bench under torchrun, the recursive-evaluation CLI under torchrun, data generation with one locker per GPU.
+# N-GPU machine (bash scripts/multi_gpu_check.sh [N] [output dir]): bench under torchrun, the recursive-evaluation CLI under
+# torchrun, data generation with one locker per GPU.
 N=${1:-2}
-O=gpurun_out; mkdir -p $O
+O=${2:-multi_gpu_check_out}; mkdir -p $O
 timeout 400 python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1 --master-port 29531 bench.py --gpus $N --steps 3 --warmup 3 --no-cpu-baseline > $O/bench_n$N.json 2> $O/bench_n$N.err
 python - <<PY
 import json

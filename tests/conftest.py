@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _has_cuda():
@@ -24,7 +24,7 @@ def _has_cuda():
 
 
 def pytest_collection_modifyitems(config, items):
-    # GPU tests are selected with -m gpu on the GPU box.  When somebody runs the whole suite on a CPU-only
+    # GPU tests are selected with -m gpu on a GPU machine.  When somebody runs the whole suite on a CPU-only
     # machine they are skipped (not silently passed); on a GPU machine a missing CUDA library is a hard failure.
     if _has_cuda():
         return

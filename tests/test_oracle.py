@@ -1,14 +1,13 @@
 """CPU tests (no GPU): pin the plain-C oracle (oracle/cfr_oracle.c) against
- (a) the known answers in the reference's own gtests (cited file:line, /root/reference/csrc/liars_dice/),
- (b) golden fixtures generated from the compiled reference (oracle/make_golden.py), and
- (c) the compiled reference itself when oracle/_ref is present (this container only).
+ (a) the known answers in the reference's own gtests (cited file:line, csrc/liars_dice/ of the original project), and
+ (b) golden fixtures generated from the compiled reference (oracle/make_golden.py).
 """
 import os
 
 import numpy as np
 import pytest
 
-from oracle.oracle import Oracle, available, game_dims
+from oracle.oracle import game_dims
 
 SHAPES = [(1, 4), (1, 6), (2, 3)]
 
@@ -194,22 +193,21 @@ def test_selfplay_walk_bit_exact_vs_golden(port, golden):
             assert np.array_equal(q, g[f"q_{D}x{F}_{sl}"]) and np.array_equal(v, g[f"v_{D}x{F}_{sl}"])
 
 
-# ---------------------------------------------------------------- live cross-check with the compiled reference
-@pytest.mark.skipif(not available("ref_nofma"), reason="oracle/_ref not built (needs /root/reference)")
-def test_port_vs_compiled_reference_live():
-    P, R = Oracle("port"), Oracle("ref_nofma")
+# ---------------------------------------------------------------- cross-check with the compiled reference's stored outputs
+def test_port_vs_compiled_reference_live(port, golden):
+    """The port against the compiled reference (fixture reference_live.npz, oracle/make_golden.py live): synthetic beliefs,
+    40-iteration CFR solves from two roots and RlRunner example streams, bit for bit."""
+    P, g = port, golden("reference_live.npz")
     for (D, F) in SHAPES:
         A, H, Q = game_dims(D, F)
-        assert np.array_equal(P.synthetic_beliefs(H, 11), R.synthetic_beliefs(H, 11))
+        assert np.array_equal(P.synthetic_beliefs(H, 11), g[f"beliefs11_{D}x{F}"])
         b = P.synthetic_beliefs(H, 5)
         for lb, pl in [(-1, 0), (4, 1)]:
             x = P.cfr_solve(D, F, b, [0, 1, 5, 40], lb, pl, num_iters=40)
-            y = R.cfr_solve(D, F, b, [0, 1, 5, 40], lb, pl, num_iters=40)
             for k in ("regrets", "last", "sum", "avg", "root_means", "traverser_values"):
-                assert np.array_equal(x[k], y[k]), (D, F, lb, k)
+                assert np.array_equal(x[k], g[f"{k}_{lb}_{pl}_{D}x{F}"]), (D, F, lb, k)
         qa, va = P.rl_runner(D, F, seed=3, n_games=2, num_iters=24)
-        qb, vb = R.rl_runner(D, F, seed=3, n_games=2, num_iters=24)
-        assert np.array_equal(qa, qb) and np.array_equal(va, vb)
+        assert np.array_equal(qa, g[f"q_{D}x{F}"]) and np.array_equal(va, g[f"v_{D}x{F}"])
 
 
 @pytest.mark.parametrize("D,F", SHAPES)
@@ -246,28 +244,9 @@ def test_port_evaluation_entry_points_vs_golden(port, golden, use_cfr, netname):
         assert np.array_equal(r["strategy_to_leaf"], g[f"strategy_to_leaf_{tag}"])
 
 
-@pytest.mark.skipif(not available("ref_nofma"), reason="oracle/_ref not built (needs /root/reference)")
-def test_recursive_eval_golden_reproducible_live(golden):
-    """The recursive-evaluation fixture (BASELINE config 5 path) is what the compiled reference produces here: its own
-    compute_sampled_strategy_recursive_to_leaf + compute_stategy_stats + compute_exploitability2 under the accumulation loop
-    of recursive_eval.cc:343-369."""
-    from oracle.make_golden import recursive_eval_reference
-    g = golden("recursive_eval_zero.npz")
-    D, F = 1, 4
-    iters, reps = (int(x) for x in g[f"cfg_{D}x{F}"])
-    r = recursive_eval_reference(Oracle("ref_nofma"), D, F, iters, reps)
-    for k in ("summed_strategy", "summed_reach", "checkpoints", "exploitability", "first_strategies"):
-        assert np.array_equal(r[k], g[f"{k}_{D}x{F}"]), k
-    # the sampled strategies are proper strategies on every non-terminal node of the full tree
-    s = r["first_strategies"][0]
-    tree = Oracle("ref_nofma").unroll_tree(D, F)
-    inner = tree[:, 2] != tree[:, 3]
-    assert np.allclose(s[inner].sum(-1), 1.0, atol=1e-12) and np.all(s[~inner] == 0)
-
-
-@pytest.mark.skipif(not available("ref_nofma"), reason="oracle/_ref not built (needs /root/reference)")
-def test_reference_net_in_the_kernels_arithmetic(net_weights):
-    """ref_set_net_emulation (oracle/ref_harness.cc) evaluates the reference's own Net2 with the arithmetic of the tcgen05 kernels —
+def test_reference_net_in_the_kernels_arithmetic(net_weights, golden):
+    """ref_set_net_emulation (oracle/ref_harness.cc) evaluates the reference's own Net2 with the arithmetic of the tensor-core
+    kernels (outputs stored in reference_live.npz) —
     the model behind the P5 comparison sets m1 / m2 of datagen_stats.npz.  Pinned here against an independent numpy restatement
     (fp16 operands, fp32 accumulation and LayerNorm, GELU of model 1 / 2 with one fp16 rounding per operation), and its error level
     against the fp32 net must be the kernels' measured one (5.0e-4 / 6.3e-4 relative rms)."""
@@ -275,15 +254,9 @@ def test_reference_net_in_the_kernels_arithmetic(net_weights):
     D, F = 1, 6
     A, H, Q = game_dims(D, F)
     w = net_weights(D, F)
-    R = Oracle("ref_nofma")
-    b = R.synthetic_beliefs(H, 3)
-    outs = {}
-    for model in (0, 1, 2):
-        R.set_net_emulation(model)
-        r = R.cfr_solve(D, F, b, [1], last_bid=-1, player_id=0, num_iters=1, net_w=w, want=("avg",))
-        outs[model] = r["leaf_values"][0].astype(np.float64)
-        q = r["queries"][0].astype(np.float64)
-    R.set_net_emulation(0)
+    g = golden("reference_live.npz")
+    outs = {model: g[f"emulation{model}_leaf_values"].astype(np.float64) for model in (0, 1, 2)}
+    q = g["emulation_queries"].astype(np.float64)
     for model, lo, hi in ((1, 3.5e-4, 7e-4), (2, 4.5e-4, 9e-4)):
         rel = np.sqrt(((outs[model] - outs[0]) ** 2).mean() / (outs[0] ** 2).mean())
         assert lo < rel < hi, (model, rel)

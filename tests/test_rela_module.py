@@ -428,9 +428,8 @@ def test_datagen_distribution_matches_reference(rela, golden, D, F, net_name, ne
       * tensor-core nets: the comparison set may also be the REFERENCE ITSELF with its own net evaluated in the kernels'
         arithmetic (fp16 operands, GELU rounded to fp16: set m1, ref_set_net_emulation); the allowed distance stays the
         seed-to-seed band.
-    (This test is what exposed the bias of tanh.approx.f16x2: with the packed-half GELU the 1x6f chi-square was 1050-1200 against a
-    seed-to-seed 37, while the reference with the SAME arithmetic but a correctly rounded tanh stayed at 43-45;
-    profiles/r2_gelu_table.log, profiles/r2_gelu_variants.log.)
+    (This test is what exposed the bias of tanh.approx.f16x2: with the packed-half GELU the chi-square of the last-action counts
+    was far outside the seed-to-seed band, while the reference with the SAME arithmetic but a correctly rounded tanh stayed inside it.)
     Only complete games are counted on the GPU side (a wave loop stops mid-game)."""
     from rebel_b200.models import flatten_state_dict, make_selfplay_net
     from test_gpu_parity import _note
