@@ -184,9 +184,14 @@ __device__ __forceinline__ uint32_t act_pair(float y0, float y1) {
 // LayerNorm (eps 1e-5, mean-free, see above) + GELU of a warpgroup's 64 x 256 accumulators, packed to fp16 as the A fragments of
 // the next layer's wgmma: K-step kk = 8h + i/2 takes act[4kk .. 4kk+3].  A thread holds rows r and r + 8 (d[4i], d[4i+1] and
 // d[4i+2], d[4i+3]) at columns 128h + 8i + 2q + {0, 1}, q = lane & 3; the four threads of a quad share the rows.
-// ln: float4 {gamma_j, gamma_j+1, beta_j, beta_j+1} per feature pair.
-template <int kGelu>
-__device__ __forceinline__ void ln_gelu(const float (&acc)[2][64], const float4* __restrict__ ln, int q, uint32_t (&act)[64]) {
+// ln: float4 {gamma_j, gamma_j+1, beta_j, beta_j+1} per feature pair.  half_ready(h) runs as soon as act[32h .. 32h+31] (K-steps
+// 8h .. 8h+7) are written: layer 3 issues its first eight K-steps there, so they run under the second half of the GELU.
+struct NoHalf {
+  __device__ __forceinline__ void operator()(int) const {}
+};
+template <int kGelu, typename Half = NoHalf>
+__device__ __forceinline__ void ln_gelu(const float (&acc)[2][64], const float4* __restrict__ ln, int q, uint32_t (&act)[64],
+                                        Half half_ready = Half()) {
   float s[4] = {0.f, 0.f, 0.f, 0.f};        // (row r, row r + 8) x two independent chains
 #pragma unroll
   for (int h = 0; h < 2; ++h)
@@ -206,7 +211,7 @@ __device__ __forceinline__ void ln_gelu(const float (&acc)[2][64], const float4*
   // the rows of W and the biases are centred over the features on the host: the mean of the 256 accumulators is zero
   const float rstd_lo = rsqrtf(lo * (1.f / kHid) + 1e-5f), rstd_hi = rsqrtf(hi * (1.f / kHid) + 1e-5f);
 #pragma unroll
-  for (int h = 0; h < 2; ++h)
+  for (int h = 0; h < 2; ++h) {
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const float4 pp = ln[h * 64 + i * 4 + q];
@@ -215,6 +220,8 @@ __device__ __forceinline__ void ln_gelu(const float (&acc)[2][64], const float4*
       act[h * 32 + 2 * i + 1] = act_pair<kGelu>(__fmaf_rn(__fmul_rn(acc[h][4 * i + 2], rstd_hi), pp.x, pp.z),
                                                 __fmaf_rn(__fmul_rn(acc[h][4 * i + 3], rstd_hi), pp.y, pp.w));
     }
+    half_ready(h);
+  }
 }
 
 struct TcArgs {
@@ -227,15 +234,24 @@ struct TcArgs {
   float* dbg_d2;            // optional [128][256] raw layer-2 accumulators of tile 0
   long long* trace;         // optional (debug build only): SM clock stamps of CTA 0, [2048]: thread 0 of warpgroup w at
                             // [w * 1024 + j * 8 + e] for its j-th tile (j < 64): e = 0 query tile ready, 1 layer 1 done,
-                            // 2 epilogue 1 done, 3 layer 2 done, 4 epilogue 2 done, 5 outputs written
+                            // 2 epilogue 1 done, 3 turn taken, 4 layer 2 issued, 5 layer 2 done, 6 epilogue 2 done (layer 3
+                            // issued under it), 7 outputs written.  Warpgroup 1 takes its first turn between stamps 1 and 2
+                            // of its tile 0.
 };
+
+// Named barriers (0 is __syncthreads): kBarWg + w gathers the four warps of warpgroup w; kBarTurn + w is warpgroup w's turn
+// to issue its layer-2 chain (bar.sync by w, bar.arrive by the other warpgroup: 256 threads).
+constexpr int kBarWg = 1;
+constexpr int kBarTurn = 3;
 
 template <bool kDebug, int kGelu>
 __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_kernel(TcArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
   const BlobLayout L(a.Kp);
-  const int tid = threadIdx.x, wg = tid >> 7, lt = tid & 127, warp = lt >> 5, lane = tid & 31;
-  const int rows = *a.rows_ptr;
+  // wg and rows through a shuffle: ptxas then knows they are warp-uniform, and the branches on them (the turns below) do not
+  // make it serialise the wgmmas (C7520) or spill
+  const int tid = threadIdx.x, wg = __shfl_sync(0xffffffffu, tid >> 7, 0), lt = tid & 127, warp = lt >> 5, lane = tid & 31;
+  const int rows = __shfl_sync(0xffffffffu, *a.rows_ptr, 0);
   const int ntiles = (rows + kTileM - 1) / kTileM;
   if ((int)blockIdx.x >= ntiles) return;
   const int J = (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1;      // tiles of this CTA: blockIdx.x + j * gridDim.x
@@ -301,6 +317,18 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_kernel(TcArgs a) {
     }
   };
 
+  // Ping-pong: the layer-2 chains of the two warpgroups take turns on the tensor cores.  A warpgroup takes its turn before it
+  // issues layer 2 and passes it on as soon as the chain is issued.  Warpgroup 0 has the first turn; warpgroup 1 takes its
+  // first turn already before epilogue 1 of its first tile, so that it starts one phase behind, its first epilogue under
+  // warpgroup 0's first layer 2.  (Holding the turn through epilogue 1 on every tile, which keeps the two epilogues apart, was
+  // slower: an epilogue is bound by the latency of its own dependent instructions, not by issue slots, and two of them side by
+  // side, one warp of each warpgroup per SM sub-partition, cover each other's latency.)  Both warpgroups run the same J tiles;
+  // warpgroup 0 takes J - 1 turns (none at j = 0) and passes J, warpgroup 1 takes J and passes J - 1 (none after its last
+  // chain), so every bar.arrive meets its bar.sync before exit, and neither warpgroup can arrive twice before the other has
+  // synchronised once.
+  auto take_turn = [&] { asm volatile("bar.sync %0, 256;" ::"r"(kBarTurn + wg) : "memory"); };
+  auto pass_turn = [&] { asm volatile("bar.arrive %0, 256;" ::"r"(kBarTurn + (wg ^ 1)) : "memory"); };
+
   for (int j = 0; j < J; ++j) {
     const int tile = tile_of(j), buf = j & 1;
     const uint32_t xb = sx + buf * (uint32_t)L.x_bytes + wg * (kWgRows / 8) * 128;
@@ -318,11 +346,14 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_kernel(TcArgs a) {
     wgmma_wait_all();
     fence_regs(acc[0]); fence_regs(acc[1]);
     // wgmma.wait_group covers only the calling warp's reads of the buffer: all four warps of the warpgroup meet first (named
-    // barrier 1 + wg), then the second warpgroup to get here refills the buffer with the tile two ahead
-    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    // barrier kBarWg + wg), then the second warpgroup to get here refills the buffer with the tile two ahead.  The layer-2
+    // issues of the two warpgroups alternate, so neither gets more than two tiles ahead of the other: a warpgroup waits for
+    // tile j + 2 only after both have passed layer 1 of tile j, never for tile j + 4 of the same buffer.
+    asm volatile("bar.sync %0, 128;" ::"r"(kBarWg + wg) : "memory");
     if (lt == 0 && (atomicAdd(&xcnt[buf], 1) & 1) && j + 2 < J) fetch_x(j + 2);
     tap(a.dbg_d1, tile);
     CFRB_TRACE(1);
+    if (wg == 1 && j == 0) take_turn();
     ln_gelu<kGelu>(acc, ln1, q, act);
     CFRB_TRACE(2);
     // ---- layer 2: D2 = bias2 + A2 W2'^T, A2 from registers
@@ -333,6 +364,8 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_kernel(TcArgs a) {
         const float2 bb = *reinterpret_cast<const float2*>(b2 + h * 128 + i * 8 + 2 * q);
         acc[h][4 * i] = bb.x; acc[h][4 * i + 1] = bb.y; acc[h][4 * i + 2] = bb.x; acc[h][4 * i + 3] = bb.y;
       }
+    if (j > 0) take_turn();
+    CFRB_TRACE(3);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < kHid / 16; ++kk) {
@@ -340,20 +373,26 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_kernel(TcArgs a) {
       for (int h = 0; h < 2; ++h) wgmma_rs_n128(acc[h], act + 4 * kk, make_desc(sw2 + kk * 2 * lbo_w + h * 2048, lbo_w, 128));
     }
     wgmma_commit();
+    if (wg == 0 || j + 1 < J) pass_turn();
+    CFRB_TRACE(4);
     wgmma_wait_all();
     fence_regs(acc[0]); fence_regs(acc[1]); fence_regs(act);
     tap(a.dbg_d2, tile);
-    CFRB_TRACE(3);
-    ln_gelu<kGelu>(acc, ln2, q, act);
-    CFRB_TRACE(4);
-    // ---- layer 3: raw net outputs (the CFR backward kernel multiplies by the opponent-reach scaler)
+    CFRB_TRACE(5);
+    // ---- epilogue 2 and layer 3 (raw net outputs; the CFR backward kernel multiplies by the opponent-reach scaler): each half
+    // of the m64n16k16 chain is issued as soon as epilogue 2 has produced its A fragments; the steps still accumulate in K order.
+    // (A fence per K-step, i.e. issuing each step as soon as its four registers exist, splits the GELU into sixteen short
+    // scheduling windows and made epilogue 2 about twice as long.)
     float o[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) o[i] = 0.f;
-    wgmma_fence();
+    ln_gelu<kGelu>(acc, ln2, q, act, [&](int h) {
+      wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < kHid / 16; ++kk) wgmma_rs_n16(o, act + 4 * kk, make_desc(sw3 + kk * 2 * lbo_w3, lbo_w3, 128));
+      for (int kk = 8 * h; kk < 8 * h + 8; ++kk) wgmma_rs_n16(o, act + 4 * kk, make_desc(sw3 + kk * 2 * lbo_w3, lbo_w3, 128));
+    });
     wgmma_commit();
+    CFRB_TRACE(6);
     wgmma_wait_all();
     fence_regs(o); fence_regs(act);
 #pragma unroll
@@ -368,7 +407,7 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_kernel(TcArgs a) {
         }
       }
     }
-    CFRB_TRACE(5);
+    CFRB_TRACE(7);
   }
 #undef CFRB_TRACE
 }
