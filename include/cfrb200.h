@@ -18,6 +18,8 @@
  *   cfrb_examples                   <-  CFR::update_value_network      (subgame_solving.cc:672-676, 220-226)
  *   cfrb_tree_template              <-  unroll_tree, for bit-exact infoset-index checks (tree_test.cc)
  *   cfrb_exploitability             <-  compute_exploitability2        (subgame_solving.cc:802-816)
+ *   cfrb_ev2                        <-  compute_ev2                    (subgame_solving.cc:931-982)
+ *   cfrb_regrets_*                  <-  compute_immediate_regrets      (subgame_solving.cc:984-1050)
  *
  * Conventions: plain C, no exceptions across the boundary; every function returns 0 on success or a
  * negative CFRB_E* code (cfrb_last_error() gives the message for the calling thread); all buffers are
@@ -195,6 +197,27 @@ int cfrb_debug_net_trace(cfrb_handle* h, long long* out, int n);
 /* Exploitability (best-response values of both players, compute_exploitability2) of a full-tree strategy
  * given as dense [N_full][H][A] fp64, evaluated on the GPU. out2 = {br0, br1}. */
 int cfrb_exploitability(cfrb_handle* h, const double* full_strategy, double* out2);
+
+/* Expected values of two full-tree strategies against each other, compute_ev2 (subgame_solving.cc:931-982): out2 = {ev0, ev1}
+ * with ev0 = player 0 playing s1 against player 1 playing s2, ev1 = -(player 0 playing s2 against s1).  Dense [N_full][H][A]
+ * fp64, evaluated on the GPU. */
+int cfrb_ev2(cfrb_handle* h, const double* s1_dense, const double* s2_dense, double* out2);
+/* Node count N_full of the full game tree (the tree cfrb_exploitability / cfrb_ev2 / cfrb_regrets_* index). */
+int cfrb_full_tree_nodes(cfrb_handle* h);
+
+/* Immediate-regret accumulator on the handle's device, compute_immediate_regrets (subgame_solving.cc:984-1050) split so that a
+ * list of strategies can be added in pieces: adding strategies in batches of any size gives the bits of one pass over the whole
+ * list.  Reset zeroes the sums [N_full][H][A] and the count (and must precede the first add). */
+int cfrb_regrets_reset(cfrb_handle* h);
+/* Add n full-tree strategies, fp32 compact [n][N_full - 1][H] with entry (child_node - 1) * H + hand (the repeats of
+ * recursive_eval go through a float32 tensor, recursive_eval.cc:358). */
+int cfrb_regrets_add(cfrb_handle* h, const float* compact, int32_t n);
+/* Add the handle's current sampling strategy (get_sampling_strategy, read in place on the device).  Subgame 0 of the wave must be
+ * the full game tree (max_depth covering the whole game, rooted at the initial state); otherwise CFRB_EINVAL. */
+int cfrb_regrets_add_current(cfrb_handle* h);
+/* immediate [N_full][H] = max over the A actions of the sums / count (0 at leaves); sums [N_full][H][A] raw, for reductions over
+ * processes; count = strategies added.  Any pointer may be NULL.  Synchronises. */
+int cfrb_regrets_fetch(cfrb_handle* h, double* immediate, double* sums, int64_t* count);
 
 /* Counters for bench.py: kernels launched by this handle since creation, and leaf rows of the wave. */
 int64_t cfrb_kernel_launches(const cfrb_handle* h);

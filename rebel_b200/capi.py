@@ -68,6 +68,12 @@ def lib():
     L.cfrb_load_state.argtypes = [vp, _dp, _dp, _dp, _dp, _ip, C.c_int32]
     L.cfrb_debug_leaf_io.argtypes = [vp, _fp, _fp, _dp, C.c_int32]
     L.cfrb_exploitability.argtypes = [vp, _dp, _dp]
+    L.cfrb_ev2.argtypes = [vp, _dp, _dp, _dp]
+    L.cfrb_full_tree_nodes.argtypes = [vp]
+    L.cfrb_regrets_reset.argtypes = [vp]
+    L.cfrb_regrets_add.argtypes = [vp, _fp, C.c_int32]
+    L.cfrb_regrets_add_current.argtypes = [vp]
+    L.cfrb_regrets_fetch.argtypes = [vp, _dp, _dp, C.POINTER(C.c_int64)]
     L.cfrb_debug_net_taps.argtypes = [vp, _fp, _fp]
     L.cfrb_debug_net_trace.argtypes = [vp, C.POINTER(C.c_longlong), C.c_int]
     L.cfrb_kernel_launches.argtypes = [vp]

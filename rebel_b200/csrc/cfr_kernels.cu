@@ -5,6 +5,7 @@
 
 #include "cfr_kernels.cuh"
 #include "br_kernel.cuh"
+#include "ev_regret_kernels.cuh"
 #include "selfplay_kernels.cuh"
 #include "cfr_d2v2.cuh"
 
@@ -52,6 +53,17 @@ void cfr_launch_iter(const CfrDev<real>& p, int group, int blocks, int threads, 
 }
 
 void br_launch(const BrDev& p, cudaStream_t st) { br_kernel<<<2, 1024, 0, st>>>(p); }
+
+void ev_launch(const BrDev& p, const double* s1, const double* s2, cudaStream_t st) { ev_kernel<<<2, 1024, 0, st>>>(p, s1, s2); }
+
+void regret_launch(const RegretDev& r, const float* s32, const double* s64, int S, cudaStream_t st) {
+  if (S <= 0) return;
+  if (s32) regret_values_kernel<float><<<2 * S, 1024, 0, st>>>(r, s32);
+  else regret_values_kernel<double><<<2 * S, 1024, 0, st>>>(r, s64);
+  const size_t nh = (size_t)r.tree.N * r.tree.H;
+  const int blocks = (int)std::min<size_t>((nh + 255) / 256, 132 * 8);
+  regret_accumulate_kernel<<<blocks, 256, 0, st>>>(r, S);
+}
 
 template <typename real>
 cudaError_t cfr_configure_d2(int smem_bytes) {

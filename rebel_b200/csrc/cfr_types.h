@@ -79,6 +79,21 @@ struct BrDev {
 };
 void br_launch(const BrDev& p, cudaStream_t st);
 
+// compute_ev2 of two compact full-tree strategies (ev_regret_kernels.cuh); scratch per CTA: reach1[N*H] | val[N*H] | hist[10*T].
+void ev_launch(const BrDev& p, const double* s1, const double* s2, cudaStream_t st);
+// Immediate-regret accumulator (ev_regret_kernels.cuh).  tree.scratch: per (strategy, traverser) reach0[N*H] | reach1[N*H] |
+// hist[10*T].
+struct RegretDev {
+  BrDev tree;
+  const int* depth; const int* act_lo;   // [N]
+  int A;
+  size_t s_stride;                // elements between two strategies of a batch
+  double* val;                    // [S][2][N][H] traverser values
+  double* acc;                    // [N][H][A] regret sums
+};
+// Adds S strategies (compact [S][s_stride], fp32 or fp64) to the regret sums, in order.
+void regret_launch(const RegretDev& r, const float* s32, const double* s64, int S, cudaStream_t st);
+
 // Device-resident self-play (selfplay_kernels.cuh): per-game state of K games advanced in lock-step.
 constexpr int kSpMaxH = 64;       // per-thread belief copies live in local memory: larger games use the host walk
 constexpr int kSpMaxPath = 16;

@@ -97,14 +97,22 @@ struct cfrb_handle {
   DevBuf<cfrb::TemplateDev> d_tmpl;
   DevBuf<int> d_parent, d_child_begin, d_nchild, d_last_bid, d_level_begin, d_pleaf_node, d_term_node;
   DevBuf<unsigned char> d_matches;
-  // full-depth tree for cfrb_exploitability, built on first use
+  // full-depth tree for cfrb_exploitability / cfrb_ev2 / the regret accumulator, built on first use
   struct BrState {
     bool ready = false;
     cfrb::TreeTemplate t;
-    DevBuf<int> parent, child_begin, nchild, level_begin, term_node;
-    DevBuf<double> strategy, scratch, out;
+    DevBuf<int> parent, child_begin, nchild, level_begin, term_node, depth, act_lo;
+    DevBuf<double> strategy, strategy2, scratch, out;
     size_t scratch_stride = 0;
   } br;
+  // immediate-regret accumulator (cfrb_regrets_*): sums [N_full][H][A] and the number of strategies added
+  struct RegretState {
+    bool ready = false;
+    int cap = 0;                     // strategies per batch
+    DevBuf<double> acc, val, scratch;
+    DevBuf<float> s32;
+    int64_t count = 0;
+  } rg;
   DevBuf<__half> d_qconst;
   DevBuf<unsigned char> d_tpk;   // byte-packed templates for the depth <= 2 kernel
   int tpk_stride = 0;
@@ -496,6 +504,8 @@ int cfrb_destroy(cfrb_handle* h) {
   h->d_tmpl.release(); h->d_parent.release(); h->d_child_begin.release(); h->d_nchild.release(); h->d_last_bid.release();
   h->br.parent.release(); h->br.child_begin.release(); h->br.nchild.release(); h->br.level_begin.release(); h->br.term_node.release();
   h->br.strategy.release(); h->br.scratch.release(); h->br.out.release();
+  h->br.depth.release(); h->br.act_lo.release(); h->br.strategy2.release();
+  h->rg.acc.release(); h->rg.val.release(); h->rg.scratch.release(); h->rg.s32.release();
   h->d_tpk.release();
   h->d_level_begin.release(); h->d_pleaf_node.release(); h->d_term_node.release(); h->d_matches.release(); h->d_qconst.release();
   h->d_wave.release(); h->d_sg_tmpl.release(); h->d_sg_player.release(); h->d_sg_row_off.release(); h->d_sg_act.release();
@@ -1147,49 +1157,200 @@ int cfrb_debug_net_taps(cfrb_handle* h, float* d1, float* d2) {
   return CFRB_OK;
 }
 
-int cfrb_exploitability(cfrb_handle* h, const double* full_strategy, double* out2) {
-  if (!h || !full_strategy || !out2) return fail(CFRB_EINVAL, "cfrb_exploitability: null argument");
-  CK(cudaSetDevice(h->cfg.device));
+// The full-depth tree rooted at the initial state (unroll_tree(game), tree.h:51-70) on the device, built on first use.
+static int full_tree_setup(cfrb_handle* h, const char* who) {
   auto& b = h->br;
   const auto& g = h->g;
-  if (!b.ready) {
-    if (g.A > 26) return fail(CFRB_EINVAL, "cfrb_exploitability: full tree too large (2^A - 1 nodes)");
-    b.t = cfrb::build_template(g, -1, 1 << 30);
-    const auto& t = b.t;
-    std::vector<int> term(t.term_node.begin(), t.term_node.end());
-    for (int n : t.term_node) term.push_back(t.last_bid[t.parent[n]]);   // challenged bid (:287)
-    for (int n : t.term_node) term.push_back(t.depth[n]);
-    auto up = [&](auto& buf, const auto& v) -> cudaError_t {
-      cudaError_t e = buf.alloc(v.size());
-      if (e != cudaSuccess) return e;
-      return cudaMemcpy(buf.p, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
-    };
-    CK(up(b.parent, t.parent)); CK(up(b.child_begin, t.child_begin)); CK(up(b.nchild, t.nchild));
-    CK(up(b.level_begin, t.level_begin)); CK(up(b.term_node, term));
-    b.scratch_stride = (size_t)3 * t.N * g.H + (size_t)10 * std::max(t.T, 1);
-    CK(b.scratch.alloc(2 * b.scratch_stride));
-    CK(b.strategy.alloc((size_t)std::max(t.N - 1, 1) * g.H));
-    CK(b.out.alloc(2));
-    b.ready = true;
-  }
+  if (b.ready) return CFRB_OK;
+  if (g.A > 26) return fail(CFRB_EINVAL, std::string(who) + ": full tree too large (2^A - 1 nodes)");
+  b.t = cfrb::build_template(g, -1, 1 << 30);
   const auto& t = b.t;
-  // dense [n][h][a] -> compact [edge = child - 1][h]
+  std::vector<int> term(t.term_node.begin(), t.term_node.end());
+  for (int n : t.term_node) term.push_back(t.last_bid[t.parent[n]]);   // challenged bid (:287)
+  for (int n : t.term_node) term.push_back(t.depth[n]);
+  auto up = [&](auto& buf, const auto& v) -> cudaError_t {
+    cudaError_t e = buf.alloc(v.size());
+    if (e != cudaSuccess) return e;
+    return cudaMemcpy(buf.p, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
+  };
+  CK(up(b.parent, t.parent)); CK(up(b.child_begin, t.child_begin)); CK(up(b.nchild, t.nchild));
+  CK(up(b.level_begin, t.level_begin)); CK(up(b.term_node, term)); CK(up(b.depth, t.depth)); CK(up(b.act_lo, t.act_lo));
+  b.scratch_stride = (size_t)3 * t.N * g.H + (size_t)10 * std::max(t.T, 1);
+  CK(b.scratch.alloc(2 * b.scratch_stride));
+  CK(b.strategy.alloc((size_t)std::max(t.N - 1, 1) * g.H));
+  CK(b.strategy2.alloc((size_t)std::max(t.N - 1, 1) * g.H));
+  CK(b.out.alloc(2));
+  b.ready = true;
+  return CFRB_OK;
+}
+
+static cfrb::BrDev full_tree_dev(cfrb_handle* h) {
+  const auto& b = h->br;
+  const auto& t = b.t;
+  cfrb::BrDev d{};
+  d.N = t.N; d.T = t.T; d.levels = t.levels; d.H = h->g.H; d.F = h->g.F;
+  d.parent = b.parent.p; d.child_begin = b.child_begin.p; d.nchild = b.nchild.p; d.level_begin = b.level_begin.p;
+  d.term_node = b.term_node.p; d.matches = h->d_matches.p; d.strategy = b.strategy.p;
+  d.scratch = b.scratch.p; d.scratch_stride = b.scratch_stride; d.out = b.out.p;
+  return d;
+}
+
+// dense full-tree [n][h][a] -> compact [edge = child - 1][h] on the device
+static int upload_compact(cfrb_handle* h, const double* dense, double* dst) {
+  const auto& t = h->br.t;
+  const auto& g = h->g;
   std::vector<double> compact((size_t)std::max(t.N - 1, 1) * g.H, 0.0);
   for (int n = 0; n < t.N; ++n)
     for (int j = 0; j < t.nchild[n]; ++j)
       for (int hd = 0; hd < g.H; ++hd)
-        compact[(size_t)(t.child_begin[n] + j - 1) * g.H + hd] = full_strategy[((size_t)n * g.H + hd) * g.A + t.act_lo[n] + j];
-  CK(cudaMemcpyAsync(b.strategy.p, compact.data(), compact.size() * sizeof(double), cudaMemcpyHostToDevice, h->own_stream));
-  cfrb::BrDev d{};
-  d.N = t.N; d.T = t.T; d.levels = t.levels; d.H = g.H; d.F = g.F;
-  d.parent = b.parent.p; d.child_begin = b.child_begin.p; d.nchild = b.nchild.p; d.level_begin = b.level_begin.p;
-  d.term_node = b.term_node.p; d.matches = h->d_matches.p; d.strategy = b.strategy.p;
-  d.scratch = b.scratch.p; d.scratch_stride = b.scratch_stride; d.out = b.out.p;
-  cfrb::br_launch(d, h->own_stream);
+        compact[(size_t)(t.child_begin[n] + j - 1) * g.H + hd] = dense[((size_t)n * g.H + hd) * g.A + t.act_lo[n] + j];
+  CK(cudaMemcpyAsync(dst, compact.data(), compact.size() * sizeof(double), cudaMemcpyHostToDevice, h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));   // `compact` goes out of scope
+  return CFRB_OK;
+}
+
+int cfrb_exploitability(cfrb_handle* h, const double* full_strategy, double* out2) {
+  if (!h || !full_strategy || !out2) return fail(CFRB_EINVAL, "cfrb_exploitability: null argument");
+  CK(cudaSetDevice(h->cfg.device));
+  int rc = full_tree_setup(h, "cfrb_exploitability");
+  if (!rc) rc = upload_compact(h, full_strategy, h->br.strategy.p);
+  if (rc) return rc;
+  cfrb::br_launch(full_tree_dev(h), h->own_stream);
   ++h->launches;
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out2, b.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, h->own_stream));
+  CK(cudaMemcpyAsync(out2, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, h->own_stream));
   CK(cudaStreamSynchronize(h->own_stream));
+  return CFRB_OK;
+}
+
+int cfrb_ev2(cfrb_handle* h, const double* s1_dense, const double* s2_dense, double* out2) {
+  if (!h || !s1_dense || !s2_dense || !out2) return fail(CFRB_EINVAL, "cfrb_ev2: null argument");
+  CK(cudaSetDevice(h->cfg.device));
+  int rc = full_tree_setup(h, "cfrb_ev2");
+  if (!rc) rc = upload_compact(h, s1_dense, h->br.strategy.p);
+  if (!rc) rc = upload_compact(h, s2_dense, h->br.strategy2.p);
+  if (rc) return rc;
+  cfrb::ev_launch(full_tree_dev(h), h->br.strategy.p, h->br.strategy2.p, h->own_stream);
+  ++h->launches;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out2, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  return CFRB_OK;
+}
+
+int cfrb_full_tree_nodes(cfrb_handle* h) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  CK(cudaSetDevice(h->cfg.device));
+  int rc = full_tree_setup(h, "cfrb_full_tree_nodes");
+  return rc ? rc : h->br.t.N;
+}
+
+int cfrb_regrets_reset(cfrb_handle* h) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  CK(cudaSetDevice(h->cfg.device));
+  int rc = full_tree_setup(h, "cfrb_regrets_reset");
+  if (rc) return rc;
+  auto& r = h->rg;
+  const auto& t = h->br.t;
+  if (!r.ready) {
+    CK(r.acc.alloc((size_t)t.N * h->g.H * h->g.A));
+    r.ready = true;
+  }
+  CK(cudaMemsetAsync(r.acc.p, 0, r.acc.n * sizeof(double), h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  r.count = 0;
+  return CFRB_OK;
+}
+
+// Room for `S` strategies per batch: traverser values [S][2][N][H], reach scratch per (strategy, traverser), fp32 staging.
+static int regrets_reserve(cfrb_handle* h, int S) {
+  auto& r = h->rg;
+  if (S <= r.cap) return CFRB_OK;
+  const auto& t = h->br.t;
+  const size_t NH = (size_t)t.N * h->g.H;
+  r.val.release(); r.scratch.release(); r.s32.release();
+  CK(r.val.alloc((size_t)S * 2 * NH));
+  CK(r.scratch.alloc((size_t)S * 2 * (2 * NH + (size_t)10 * std::max(t.T, 1))));
+  CK(r.s32.alloc((size_t)S * std::max(t.N - 1, 1) * h->g.H));
+  r.cap = S;
+  return CFRB_OK;
+}
+
+static int regrets_launch(cfrb_handle* h, const float* s32, const double* s64, int S) {
+  auto& r = h->rg;
+  const auto& t = h->br.t;
+  cfrb::RegretDev d{};
+  d.tree = full_tree_dev(h);
+  d.tree.scratch = r.scratch.p;
+  d.tree.scratch_stride = 2 * (size_t)t.N * h->g.H + (size_t)10 * std::max(t.T, 1);
+  d.depth = h->br.depth.p; d.act_lo = h->br.act_lo.p; d.A = h->g.A;
+  d.s_stride = (size_t)std::max(t.N - 1, 1) * h->g.H;
+  d.val = r.val.p; d.acc = r.acc.p;
+  cfrb::regret_launch(d, s32, s64, S, h->own_stream);
+  h->launches += 2;
+  CK(cudaGetLastError());
+  r.count += S;
+  return CFRB_OK;
+}
+
+static constexpr int kRegretBatch = 64;
+
+int cfrb_regrets_add(cfrb_handle* h, const float* compact, int32_t n) {
+  if (!h || n < 0 || (n > 0 && !compact)) return fail(CFRB_EINVAL, "cfrb_regrets_add: bad argument");
+  if (!h->rg.ready) return fail(CFRB_ESTATE, "cfrb_regrets_add: cfrb_regrets_reset has not been called");
+  CK(cudaSetDevice(h->cfg.device));
+  const size_t stride = (size_t)std::max(h->br.t.N - 1, 1) * h->g.H;
+  for (int off = 0; off < n; off += kRegretBatch) {
+    const int S = std::min(kRegretBatch, n - off);
+    int rc = regrets_reserve(h, S);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(h->rg.s32.p, compact + (size_t)off * stride, (size_t)S * stride * sizeof(float), cudaMemcpyHostToDevice,
+                       h->own_stream));
+    if ((rc = regrets_launch(h, h->rg.s32.p, nullptr, S))) return rc;
+    CK(cudaStreamSynchronize(h->own_stream));   // the host buffer and the staging area are reused
+  }
+  return CFRB_OK;
+}
+
+int cfrb_regrets_add_current(cfrb_handle* h) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  if (!h->rg.ready) return fail(CFRB_ESTATE, "cfrb_regrets_add_current: cfrb_regrets_reset has not been called");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());   // runs enqueued on other streams have finished before the table is read
+  { int rc = sync_mirror(h); if (rc) return rc; }
+  const auto& t = h->br.t;
+  // subgame 0 must be the whole game: rooted at the initial state, player 0, with the full tree's node order
+  if (h->n < 1 || h->h_tmpl[0] != 0 || h->h_player[0] != 0 || h->tmpl[0].N != t.N || h->tmpl[0].L != 0)
+    return fail(CFRB_EINVAL, "cfrb_regrets_add_current: subgame 0 of the wave is not the full game tree");
+  int rc = regrets_reserve(h, 1);
+  if (rc) return rc;
+  // the sampling strategy (CFR: last_strategies, FP: average_strategies) is the Sg table in both solvers, read in place
+  if (h->f64) rc = regrets_launch(h, nullptr, h->sd.Sg.p, 1);
+  else rc = regrets_launch(h, h->sf.Sg.p, nullptr, 1);
+  return rc;
+}
+
+int cfrb_regrets_fetch(cfrb_handle* h, double* immediate, double* sums, int64_t* count) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  if (!h->rg.ready) return fail(CFRB_ESTATE, "cfrb_regrets_fetch: cfrb_regrets_reset has not been called");
+  CK(cudaSetDevice(h->cfg.device));
+  const int N = h->br.t.N, H = h->g.H, A = h->g.A;
+  std::vector<double> acc((size_t)N * H * A);
+  CK(cudaMemcpyAsync(acc.data(), h->rg.acc.p, acc.size() * sizeof(double), cudaMemcpyDeviceToHost, h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  if (sums) std::memcpy(sums, acc.data(), acc.size() * sizeof(double));
+  if (count) *count = h->rg.count;
+  if (immediate) {
+    // max over all A actions (illegal ones stay 0) / number of strategies; 0 at leaves (subgame_solving.cc:1035-1048)
+    const double cnt = (double)h->rg.count;
+    for (int n = 0; n < N; ++n)
+      for (int hd = 0; hd < H; ++hd) {
+        const double* r = acc.data() + ((size_t)n * H + hd) * A;
+        double m = r[0];
+        for (int a = 1; a < A; ++a) if (m < r[a]) m = r[a];
+        immediate[(size_t)n * H + hd] = h->br.t.nchild[n] ? m / cnt : 0.0;
+      }
+  }
   return CFRB_OK;
 }
 

@@ -91,6 +91,8 @@ class FullTreeSolver {
     if (cfrb_exploitability(h_, s.data(), e.data()) < 0) throw std::runtime_error(cfrb_last_error());
     return e;
   }
+  cfrb_handle* handle() const { return h_; }
+  int numNodes() const { return N_; }
 
  private:
   cfrb_handle* h_ = nullptr;

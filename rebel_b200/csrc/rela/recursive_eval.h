@@ -28,12 +28,41 @@
 
 namespace rela {
 
+// Immediate regrets read out of a handle's accumulator (cfrb_regrets_fetch): [N][H], raw sums [N][H][A] and the count.
+struct ImmediateRegrets {
+  std::vector<double> immediate, sums;
+  int64_t count = 0;
+};
+inline ImmediateRegrets fetch_regrets(cfrb_handle* h, int H, int A) {
+  const int N = cfrb_full_tree_nodes(h);
+  if (N < 0) throw std::runtime_error(cfrb_last_error());
+  ImmediateRegrets r;
+  r.immediate.resize((size_t)N * H);
+  r.sums.resize((size_t)N * H * A);
+  if (cfrb_regrets_fetch(h, r.immediate.data(), r.sums.data(), &r.count) < 0) throw std::runtime_error(cfrb_last_error());
+  return r;
+}
+// report_regrets' summary (recursive_eval.cc:41-52): sum of the immediate regrets of the nodes above `depth`, and of the rest.
+inline std::array<double, 2> regret_summary(const std::vector<cfrb_node>& tree, const std::vector<double>& immediate, int H, int depth) {
+  double top = 0, bottom = 0;
+  for (size_t n = 0; n < tree.size(); ++n) {
+    double s = 0;
+    for (int h = 0; h < H; ++h) s += immediate[n * H + h];
+    if (tree[n].depth < depth) top += s;
+    else bottom += s;
+  }
+  return {top, bottom};
+}
+
 struct RecursiveEvalResult {
   std::vector<float> summed_strategy;   // [N][H][A]
   std::vector<float> summed_reach;      // [N][H]
   std::vector<float> final_strategy;    // summed_strategy / (summed_reach + 1e-6)   (recursive_eval.cc:362-363)
   std::vector<int> checkpoints;         // number of repeats at which exploitability was evaluated (powers of two + last)
   std::vector<std::array<double, 2>> exploitability;
+  std::vector<std::array<double, 2>> ev_of_full;        // compute_ev2(full_strategy, final_strategy) per checkpoint (:368)
+  std::vector<std::array<double, 2>> regret_summary;    // report_regrets' (depth < mdp_depth, rest) per checkpoint (:374-377)
+  ImmediateRegrets regrets;                             // of the sampled strategies of all repeats (CFR, track_regrets)
   int num_nodes = 0;
   int64_t subgames_solved = 0;
   int64_t subgame_iters = 0;   // CFR iterations the reference would run for these subgames: the sum of their act_iterations
@@ -148,19 +177,31 @@ class RecursiveEvaluator {
     return out;
   }
 
-  RecursiveEvalResult run(int num_repeats, int seed0, int batch_repeats) {
+  // full_strategy (dense [N][H][A], may be null): EV of the final strategy against it at every checkpoint.  track_regrets (CFR
+  // only, like the reference): immediate regrets of the sampled strategies, added to the handle's accumulator batch by batch in
+  // repeat order.
+  RecursiveEvalResult run(int num_repeats, int seed0, int batch_repeats, const std::vector<double>* full_strategy = nullptr,
+                          bool track_regrets = false) {
     const int N = (int)full_.size();
     RecursiveEvalResult res;
     res.num_nodes = N;
     res.summed_strategy.assign((size_t)N * H_ * A_, 0.f);
     res.summed_reach.assign((size_t)N * H_, 0.f);
+    if (full_strategy && full_strategy->size() != (size_t)N * H_ * A_) throw std::runtime_error("full_strategy must be [N_full][H][A]");
+    track_regrets = track_regrets && cfg_.subgame_params.use_cfr;
+    if (track_regrets && cfrb_regrets_reset(h_) < 0) throw std::runtime_error(cfrb_last_error());
     int done = 0;
     while (done < num_repeats) {
       // batches end at powers of two so that the exploitability curve of the reference (:364-369) can be reported
       int next_cp = 1;
       while (next_cp <= done) next_cp <<= 1;
       const int hi = std::min({num_repeats, done + std::max(1, batch_repeats), next_cp});
+      if (track_regrets) sampled_.assign((size_t)(hi - done) * (N - 1) * H_, 0.f);
       runBatch(seed0 + done, hi - done, res);
+      if (track_regrets) {
+        if (cfrb_regrets_add(h_, sampled_.data(), hi - done) < 0) throw std::runtime_error(cfrb_last_error());
+        sampled_.clear();
+      }
       done = hi;
       if ((done & (done - 1)) == 0 || done == num_repeats) {
         finalize(res);
@@ -169,6 +210,15 @@ class RecursiveEvaluator {
         std::array<double, 2> e{};   // best response of both players on the GPU (cfrb_exploitability = compute_exploitability2)
         if (cfrb_exploitability(h_, s.data(), e.data()) < 0) throw std::runtime_error(cfrb_last_error());
         res.exploitability.push_back(e);
+        if (full_strategy) {
+          std::array<double, 2> ev{};   // compute_ev2(full_strategy, final_strategy) (:368)
+          if (cfrb_ev2(h_, full_strategy->data(), s.data(), ev.data()) < 0) throw std::runtime_error(cfrb_last_error());
+          res.ev_of_full.push_back(ev);
+        }
+        if (track_regrets) {
+          res.regrets = fetch_regrets(h_, H_, A_);
+          res.regret_summary.push_back(regret_summary(full_, res.regrets.immediate, H_, cfg_.subgame_params.max_depth));
+        }
       }
     }
     return res;
@@ -341,8 +391,11 @@ class RecursiveEvaluator {
         double* cr = &rch[(size_t)pc * W];
         std::copy(nb, nb + W, cb);
         std::copy(nr, nr + W, cr);
+        // the repeat's sampled strategy as the float32 tensor of recursive_eval.cc:138-139, compact [edge = child - 1][h]
+        float* samp = sampled_.empty() ? nullptr : sampled_.data() + ((size_t)P.repeat * (full_.size() - 1) + full_id[pc] - 1) * H_;
         for (int h = 0; h < H_; ++h) {
           const double s = sigma[(size_t)(pc - 1) * H_ + h];
+          if (samp) samp[h] = (float)s;
           if (strategy_out_) strategy_out_[((size_t)fn * H_ + h) * A_ + action] = s;
           else res.summed_strategy[((size_t)fn * H_ + h) * A_ + action] += (float)s * (float)nr[(size_t)pid * H_ + h];
           cb[(size_t)pid * H_ + h] *= s;
@@ -364,6 +417,7 @@ class RecursiveEvaluator {
   const liars_dice::RecursiveSolvingParams cfg_;
   const int K_;
   double* strategy_out_ = nullptr;   // set while strategyToLeaf() runs
+  mutable std::vector<float> sampled_;   // run(track_regrets): sampled strategies of the batch's repeats, [count][N - 1][H]
   cfrb_handle* h_ = nullptr;
   int A_ = 0, H_ = 0, stride_ = 0;
   std::vector<cfrb_node> full_;

@@ -333,12 +333,36 @@ std::tuple<torch::Tensor, torch::Tensor> run_selfplay_waves(const RecursiveSolvi
 
 // BASELINE config 5 (`recursive_eval --cfr --num_repeats R`, recursive_eval.cc:331-369): R sampled recursive strategies,
 // float32 reach-weighted average, exploitability of the average.  Returns a dict of tensors.
+torch::Tensor pairs_tensor(const std::vector<std::array<double, 2>>& v) {
+  auto t = torch::empty({(int64_t)v.size(), 2}, torch::kFloat64);
+  for (size_t i = 0; i < v.size(); ++i) {
+    t[i][0] = v[i][0];
+    t[i][1] = v[i][1];
+  }
+  return t;
+}
+torch::Tensor f64_tensor(const std::vector<double>& v, std::vector<int64_t> shape) {
+  auto t = torch::empty(shape, torch::kFloat64);
+  std::copy(v.begin(), v.end(), t.data_ptr<double>());
+  return t;
+}
+void put_regrets(py::dict& d, const ImmediateRegrets& r, int64_t N, int64_t H, int64_t A) {
+  d["immediate_regrets"] = f64_tensor(r.immediate, {N, H});
+  d["regret_sums"] = f64_tensor(r.sums, {N, H, A});
+  d["regret_count"] = r.count;
+}
+
 py::dict recursive_eval_sampled(const RecursiveSolvingParams& cfg, int device, int num_repeats, int seed0, int batch_repeats,
-                                int wave_capacity, py::object flat_weights) {
+                                int wave_capacity, py::object flat_weights, py::object full_strategy, bool track_regrets) {
   std::vector<float> w;
   if (!flat_weights.is_none()) {
     auto t = flat_weights.cast<torch::Tensor>().to(torch::kCPU, torch::kFloat32).contiguous();
     w.assign(t.data_ptr<float>(), t.data_ptr<float>() + t.numel());
+  }
+  std::vector<double> full;
+  if (!full_strategy.is_none()) {
+    auto t = full_strategy.cast<torch::Tensor>().to(torch::kCPU, torch::kFloat64).contiguous();
+    full.assign(t.data_ptr<double>(), t.data_ptr<double>() + t.numel());
   }
   RecursiveEvalResult r;
   int A = 0, H = 0;
@@ -346,7 +370,7 @@ py::dict recursive_eval_sampled(const RecursiveSolvingParams& cfg, int device, i
     py::gil_scoped_release nogil;
     RecursiveEvaluator ev(cfg, device, wave_capacity);
     if (!w.empty()) ev.setWeights(w);
-    r = ev.run(num_repeats, seed0, batch_repeats);
+    r = ev.run(num_repeats, seed0, batch_repeats, full_strategy.is_none() ? nullptr : &full, track_regrets);
     A = ev.numActions(); H = ev.numHands();
   }
   const int64_t N = r.num_nodes;
@@ -363,6 +387,122 @@ py::dict recursive_eval_sampled(const RecursiveSolvingParams& cfg, int device, i
   d["summed_strategy"] = ss; d["summed_reach"] = sr; d["final_strategy"] = fs;
   d["checkpoints"] = r.checkpoints; d["exploitability"] = ex; d["subgames_solved"] = r.subgames_solved; d["subgame_iters"] = r.subgame_iters;
   d["gpu_seconds"] = r.gpu_seconds;
+  if (!full_strategy.is_none()) d["ev_of_full"] = pairs_tensor(r.ev_of_full);
+  if (!r.regret_summary.empty()) {
+    d["regret_summary"] = pairs_tensor(r.regret_summary);
+    put_regrets(d, r.regrets, N, H, A);
+  }
+  return d;
+}
+
+// A handle that only serves the full-tree kernels (best response, EV, regrets) of one game.
+struct FullTreeHandle {
+  cfrb_handle* h = nullptr;
+  int A = 0, H = 0, N = 0;
+  FullTreeHandle(int num_dice, int num_faces) {
+    cfrb_config c{};
+    c.num_dice = num_dice; c.num_faces = num_faces; c.max_depth = 2; c.num_iters = 1; c.max_subgames = 1; c.device = eval_device();
+    c.net_mode = CFRB_NET_ZERO; c.hidden = 256;
+    if (cfrb_create(&c, &h) < 0) throw std::runtime_error(std::string("cfrb_create: ") + cfrb_last_error());
+    A = cfrb_num_actions(h); H = cfrb_num_hands(h);
+    N = cfrb_full_tree_nodes(h);
+    if (N < 0) {
+      const std::string err = cfrb_last_error();
+      cfrb_destroy(h);
+      throw std::runtime_error(err);
+    }
+  }
+  ~FullTreeHandle() { if (h) cfrb_destroy(h); }
+  FullTreeHandle(const FullTreeHandle&) = delete;
+  FullTreeHandle& operator=(const FullTreeHandle&) = delete;
+  torch::Tensor dense(torch::Tensor s, const char* who) const {
+    auto t = s.to(torch::kCPU, torch::kFloat64).contiguous();
+    if (t.dim() != 3 || t.size(0) != N || t.size(1) != H || t.size(2) != A)
+      throw std::runtime_error(std::string(who) + ": strategy must be [num_full_tree_nodes, H, A]");
+    return t;
+  }
+};
+
+// compute_ev2 (subgame_solving.cc:975-982) of two dense full-tree strategies on the GPU: (ev0, ev1).
+std::tuple<double, double> ev_of_strategies(int num_dice, int num_faces, torch::Tensor s1, torch::Tensor s2) {
+  FullTreeHandle f(num_dice, num_faces);
+  auto a = f.dense(s1, "ev_of_strategies"), b = f.dense(s2, "ev_of_strategies");
+  std::array<double, 2> e{};
+  if (cfrb_ev2(f.h, a.data_ptr<double>(), b.data_ptr<double>(), e.data()) < 0) throw std::runtime_error(cfrb_last_error());
+  return std::make_tuple(e[0], e[1]);
+}
+
+// compute_immediate_regrets (subgame_solving.cc:984-1050) of dense strategies [S][N][H][A] on the GPU, [N][H].  The strategies
+// are read as float32, like the repeats recursive_eval passes through a float32 tensor (recursive_eval.cc:358); `batch` strategies
+// are uploaded at a time (any batch size gives the same bits).
+torch::Tensor immediate_regrets(int num_dice, int num_faces, torch::Tensor strategies, int batch) {
+  FullTreeHandle f(num_dice, num_faces);
+  auto s = strategies.to(torch::kCPU, torch::kFloat32).contiguous();
+  if (s.dim() != 4 || s.size(1) != f.N || s.size(2) != f.H || s.size(3) != f.A)
+    throw std::runtime_error("immediate_regrets: strategies must be [S, num_full_tree_nodes, H, A]");
+  std::vector<cfrb_node> tree(f.N);
+  if (cfrb_unroll_tree(num_dice, num_faces, -1, 0, 1 << 30, tree.data(), f.N) != f.N) throw std::runtime_error(cfrb_last_error());
+  const int64_t S = s.size(0), E = (int64_t)(f.N - 1) * f.H;
+  const float* dense = s.data_ptr<float>();
+  if (cfrb_regrets_reset(f.h) < 0) throw std::runtime_error(cfrb_last_error());
+  std::vector<float> compact;
+  batch = std::max(1, batch);
+  for (int64_t off = 0; off < S; off += batch) {
+    const int n = (int)std::min<int64_t>(batch, S - off);
+    compact.assign((size_t)n * E, 0.f);
+    for (int k = 0; k < n; ++k)
+      for (int c = 1; c < f.N; ++c) {
+        const int par = tree[c].parent;
+        for (int h = 0; h < f.H; ++h)
+          compact[(size_t)k * E + (size_t)(c - 1) * f.H + h] = dense[(((off + k) * f.N + par) * f.H + h) * f.A + tree[c].last_bid];
+      }
+    if (cfrb_regrets_add(f.h, compact.data(), n) < 0) throw std::runtime_error(cfrb_last_error());
+  }
+  return f64_tensor(fetch_regrets(f.h, f.H, f.A).immediate, {f.N, f.H});
+}
+
+// The full-tree solve of recursive_eval (recursive_eval.cc:270-309): build_solver(game, params) with max_depth 100000, the
+// exploitability of get_strategy() at powers of two (printed like compute_exploitability_fp) and the final get_strategy().  With
+// track_regrets (CFR only), the sampling strategy after every step with an even iteration index goes into the immediate-regret
+// accumulator on the device, without a host round trip.
+py::dict solve_full_tree(RecursiveSolvingParams cfg, int device, bool track_regrets) {
+  std::vector<int> cps;
+  std::vector<std::array<double, 2>> expl;
+  std::vector<double> strategy;
+  ImmediateRegrets reg;
+  int N = 0, H = 0, A = 0;
+  const int iters = cfg.subgame_params.num_iters;
+  track_regrets = track_regrets && cfg.subgame_params.use_cfr;
+  {
+    py::gil_scoped_release nogil;
+    FullTreeSolver solver(cfg, device, 100000);
+    cfrb_handle* h = solver.handle();
+    N = solver.numNodes(); H = cfrb_num_hands(h); A = cfrb_num_actions(h);
+    if (track_regrets && cfrb_regrets_reset(h) < 0) throw std::runtime_error(cfrb_last_error());
+    int done = 0;
+    for (int iter = 0; iter < iters; ++iter) {
+      const bool cp = ((iter + 1) & iter) == 0 || iter + 1 == iters;
+      if (track_regrets || cp) {   // without regrets the solver runs in one piece per checkpoint
+        solver.step(iter + 1 - done);
+        done = iter + 1;
+      }
+      if (track_regrets && iter % 2 == 0 && cfrb_regrets_add_current(h) < 0) throw std::runtime_error(cfrb_last_error());
+      if (cp) {
+        auto v = solver.exploitability(solver.strategy());
+        std::printf("Iter=%8d exploitabilities=(%.3e, %.3e) sum=%.3e\n", iter + 1, v[0], v[1], (v[0] + v[1]) / 2.);
+        std::fflush(stdout);
+        cps.push_back(iter + 1);
+        expl.push_back(v);
+      }
+    }
+    strategy = solver.strategy();
+    if (track_regrets) reg = fetch_regrets(h, H, A);
+  }
+  py::dict d;
+  d["checkpoints"] = cps;
+  d["exploitability"] = pairs_tensor(expl);
+  d["strategy"] = f64_tensor(strategy, {N, H, A});
+  if (track_regrets) put_regrets(d, reg, N, H, A);
   return d;
 }
 
@@ -485,6 +625,20 @@ PYBIND11_MODULE(rela, m) {
         "rebel_b200 extension: compute_exploitability2 of a dense full-tree strategy (GPU best-response kernel).");
   m.def("recursive_eval_sampled", &recursive_eval_sampled, py::arg("cfg"), py::arg("device"), py::arg("num_repeats"), py::arg("seed") = 0,
         py::arg("batch_repeats") = 64, py::arg("wave_capacity") = 8192, py::arg("flat_weights") = py::none(),
+        py::arg("full_strategy") = py::none(), py::arg("track_regrets") = false,
         "rebel_b200 extension: the reference's `recursive_eval --cfr --num_repeats R` (sampled recursive strategies, float32 "
-        "reach-weighted average, exploitability at powers of two) with the subgame solves batched on the GPU.");
+        "reach-weighted average, exploitability at powers of two) with the subgame solves batched on the GPU.  full_strategy "
+        "(dense [N, H, A]) adds ev_of_full [checkpoints, 2] (compute_ev2 against it); track_regrets (CFR only) adds "
+        "immediate_regrets [N, H], regret_summary [checkpoints, 2] (depth < max_depth, rest), regret_sums [N, H, A] and "
+        "regret_count.");
+  m.def("ev_of_strategies", &ev_of_strategies, py::arg("num_dice"), py::arg("num_faces"), py::arg("s1"), py::arg("s2"),
+        "rebel_b200 extension: compute_ev2 of two dense full-tree strategies (GPU kernel): (ev0, ev1).");
+  m.def("immediate_regrets", &immediate_regrets, py::arg("num_dice"), py::arg("num_faces"), py::arg("strategies"),
+        py::arg("batch") = 64,
+        "rebel_b200 extension: compute_immediate_regrets of dense full-tree strategies [S, N, H, A] read as float32 (GPU "
+        "kernels, `batch` strategies per upload): [N, H].");
+  m.def("solve_full_tree", &solve_full_tree, py::arg("cfg"), py::arg("device") = 0, py::arg("track_regrets") = false,
+        "rebel_b200 extension: recursive_eval's full-tree solve — dict with checkpoints, exploitability [C, 2], the final "
+        "get_strategy() [N, H, A] and, with track_regrets (CFR), the immediate regrets of the sampling strategies of the "
+        "even iterations (immediate_regrets, regret_sums, regret_count).");
 }
