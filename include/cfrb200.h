@@ -64,7 +64,10 @@ enum {
   CFRB_NET_ZERO = 0,      /* leaf values are 0 (reference: create_zero_net, real_net.cc:30-55) */
   CFRB_NET_FP32 = 1,      /* fp32 SIMT kernel: parity path, matches libtorch fp32 to ~1e-6 */
   CFRB_NET_TC_F16 = 2,    /* wgmma tensor-core kernel: fp16 operands, fp32 accumulate/LayerNorm/GELU
-                             (the reference's own `half_inference` option, selfplay.py:42-43,211) */
+                             (the reference's own `half_inference` option, selfplay.py:42-43,211).  Games of up to 16 hands
+                             whose weights and two query tiles fit shared memory run the resident kernel; larger ones
+                             (2x5f, 3x3f, 5x2f, 2x6f, 1x17f .. 1x32f) a kernel with the weights alone in shared memory;
+                             cfrb_tc_net_supported() tells which games have one (CFRB_TC_WIDE=1 forces the second) */
   CFRB_NET_TC_F16X2 = 3   /* same kernel with the fast GELU: y/2 (1 + tanh(poly)) with packed f32x2 FMAs and tanh.approx.f32, one
                              rounding to fp16 at the end (same accuracy as mode 2, 1 instead of 2 MUFU operations per element).
                              CFRB_X2_GELU=half selects the packed-fp16 evaluation (HFMA2 + tanh.approx.f16x2): 6 % faster, but
@@ -113,6 +116,10 @@ int cfrb_device_count(void);
 
 int cfrb_create(const cfrb_config* cfg, cfrb_handle** out);
 int cfrb_destroy(cfrb_handle* h);
+
+/* Host-only (no device needed): 1 if a tensor-core value net (CFRB_NET_TC_F16 / CFRB_NET_TC_F16X2) with `hidden` units fits the
+ * game on an sm_90 device, else 0 (cfrb_create then fails with CFRB_EINVAL for those modes; CFRB_NET_FP32 serves every game). */
+int cfrb_tc_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden);
 
 /* Shape queries. */
 int cfrb_num_actions(const cfrb_handle* h);   /* A */
@@ -187,7 +194,7 @@ int cfrb_load_state(cfrb_handle* h, const double* regrets, const double* last_st
  * writes at most cap_rows. */
 int cfrb_debug_leaf_io(cfrb_handle* h, float* queries, float* net_out, double* scalers, int32_t cap_rows);
 
-/* Debug taps of the tensor-core value net (CFRB_NET_TC_F16 only): re-runs it on the current query tiles and returns
+/* Debug taps of the tensor-core value net (either tensor-core mode, either kernel): re-runs it on the current query tiles and returns
  * the raw fp32 accumulators of layer 1 and layer 2 for the first 128 rows, each [128][256]. */
 int cfrb_debug_net_taps(cfrb_handle* h, float* d1, float* d2);
 /* Development aid: re-runs the tensor-core value net once with clock64() stamps of CTA 0 (out[2048]: thread 0 of warpgroup w

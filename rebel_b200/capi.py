@@ -53,6 +53,7 @@ def lib():
               "cfrb_sync"):
         getattr(L, f).argtypes = [vp]
     L.cfrb_unroll_tree.argtypes = [C.c_int32] * 5 + [_ip, C.c_int32]
+    L.cfrb_tc_net_supported.argtypes = [C.c_int32] * 3
     L.cfrb_tree_template.argtypes = [vp, C.c_int32, C.c_int32, _ip, C.c_int32]
     L.cfrb_set_weights.argtypes = [vp, _fp, C.c_size_t, C.c_uint64]
     L.cfrb_weights_version.argtypes = [vp]
@@ -121,6 +122,11 @@ def unroll_tree(num_dice, num_faces, last_bid=-1, player_id=0, max_depth=1000000
     out = np.zeros((cap, 6), np.int32)
     n = _check(lib().cfrb_unroll_tree(num_dice, num_faces, last_bid, player_id, max_depth, _p(out, _ip), cap))
     return out[:n].copy()
+
+
+def tc_net_supported(num_dice, num_faces, hidden=256):
+    """Host-only: does a tensor-core value net (NET_TC_F16 / NET_TC_F16X2) fit this game?  Otherwise NET_FP32 serves it."""
+    return bool(lib().cfrb_tc_net_supported(num_dice, num_faces, hidden))
 
 
 class WaveSolver:

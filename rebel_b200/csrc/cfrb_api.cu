@@ -17,6 +17,7 @@
 #include "cfr_tree.h"
 #include "leaf_mlp_simt.cuh"
 #include "leaf_mlp_tc.cuh"
+#include "leaf_mlp_tc_wide.cuh"
 
 namespace {
 inline bool is_tc(int net_mode) { return net_mode == CFRB_NET_TC_F16 || net_mode == CFRB_NET_TC_F16X2; }
@@ -48,6 +49,32 @@ struct DevBuf {
 };
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// Which tensor-core value net serves a game: the resident kernel (leaf_mlp_tc.cuh: weights and two query tiles in shared
+// memory, at most 16 outputs) where it fits and is not overridden, else the wide kernel (leaf_mlp_tc_wide.cuh: weights only,
+// query fragments loaded from global memory, nout = roundup(H, 16) outputs).  Returns false when neither fits; `why` then
+// holds the byte arithmetic.  `smem_limit` is the device's opt-in shared memory per block.
+struct TcPlan { bool wide = false; int nout = cfrb::tc::kNout, smem_bytes = 0; };
+bool tc_plan(int H, int Qpad, int smem_limit, bool force_wide, TcPlan* plan, std::string* why) {
+  const cfrb::tc::BlobLayout R(Qpad);
+  if (!force_wide && H <= cfrb::tc::kNout && R.smem_bytes <= smem_limit) {
+    plan->wide = false; plan->nout = cfrb::tc::kNout; plan->smem_bytes = R.smem_bytes;
+    return true;
+  }
+  const int nout = round_up(H, 16);
+  const cfrb::tc::WideLayout W(Qpad, nout);
+  if (nout <= 48 && Qpad / 16 <= cfrb::tc::kWideMaxKSteps && W.smem_bytes <= smem_limit) {
+    plan->wide = true; plan->nout = nout; plan->smem_bytes = W.smem_bytes;
+    return true;
+  }
+  if (why)
+    *why = "tensor-core value net does not fit this game: num_hands " + std::to_string(H) + ", padded query width " +
+           std::to_string(Qpad) + ", output layer " + std::to_string(nout) + " (at most 48); weights W1 256 x " +
+           std::to_string(Qpad) + " x 2 B + W2 131072 B + W3 " + std::to_string(nout) + " x 256 x 2 B + biases / LayerNorm " +
+           std::to_string(W.blob_bytes - W.off_b2) + " B = " + std::to_string(W.smem_bytes) + " B of shared memory (with the "
+           "mbarrier) > " + std::to_string(smem_limit) + " B per block; use CFRB_NET_FP32";
+  return false;
+}
 
 // Typed (fp32 / fp64) part of the solver state.
 template <typename real>
@@ -122,6 +149,7 @@ struct cfrb_handle {
   DevBuf<float> d_X, d_out, d_dbg;
   long long* dbg_trace = nullptr;   // set only inside cfrb_debug_net_trace
   int x2_gelu = 2;                  // GELU variant of CFRB_NET_TC_F16X2 (leaf_mlp_tc.cuh kGelu): 2 = fp32 tanh, 1 = packed half
+  TcPlan tc;                        // which tensor-core kernel serves the game (tc_plan)
   DevBuf<__half> d_Xh;
   WaveState<float> sf;
   WaveState<double> sd;
@@ -644,19 +672,25 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   CK(cudaMemset(h->d_wave.p, 0, 2 * sizeof(int)));
   CK(cudaMemset(h->d_out.p, 0, rows_cap * h->Hout * sizeof(float)));
   if (is_tc(cfg->net_mode)) {
-    if (g.H > cfrb::tc::kNout) return fail(CFRB_EINVAL, "CFRB_NET_TC_F16 supports num_hands <= 16");
+    // CFRB_TC_WIDE=1: the wide kernel also on games the resident kernel serves (tests, measurements)
+    const char* fw = std::getenv("CFRB_TC_WIDE");
+    std::string why;
+    if (!tc_plan(g.H, h->Qpad, max_optin, fw && *fw == '1', &h->tc, &why)) return fail(CFRB_EINVAL, why);
     const size_t tiles = (rows_cap + cfrb::tc::kTileM - 1) / cfrb::tc::kTileM;
     CK(h->d_Xh.alloc(tiles * cfrb::tc::kTileM * h->Qpad));
     CK(cudaMemset(h->d_Xh.p, 0, tiles * cfrb::tc::kTileM * h->Qpad * sizeof(__half)));
     CK(h->d_dbg.alloc(2 * cfrb::tc::kTileM * cfrb::tc::kHid));
-    const cfrb::tc::BlobLayout L(h->Qpad);
-    if (L.smem_bytes > max_optin) return fail(CFRB_EINVAL, "tensor-core value net does not fit shared memory for this game shape");
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-    CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
+    if (h->tc.wide) {
+      CK(cfrb::tc::wide_configure(h->tc.nout, h->tc.smem_bytes));
+    } else {
+      const int sm = h->tc.smem_bytes;
+      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+      CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+    }
     // CFRB_NET_TC_F16X2's GELU: fp32 tanh (default) or the packed-half evaluation (CFRB_X2_GELU=half), see leaf_mlp_tc.cuh
     if (const char* e = std::getenv("CFRB_X2_GELU")) h->x2_gelu = std::string(e) == "half" ? 1 : 2;
   }
@@ -682,6 +716,16 @@ int cfrb_create(const cfrb_config* cfg, cfrb_handle** out) {
   }
   *out = h;
   return CFRB_OK;
+}
+
+int cfrb_tc_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden) {
+  if (num_dice < 1 || num_faces < 1 || hidden != 256) return 0;
+  long hands = 1;
+  for (int i = 0; i < num_dice && hands <= 4096; ++i) hands *= num_faces;
+  if (hands > 4096 || 2L * num_dice * num_faces + 1 > 1024) return 0;     // beyond what cfrb_create accepts at all
+  const cfrb::GameShape g(num_dice, num_faces);
+  TcPlan plan;
+  return tc_plan(g.H, round_up(g.Q + 1, 16), cfrb::tc::kSmemOptinSm90, false, &plan, nullptr) ? 1 : 0;
 }
 
 int cfrb_num_actions(const cfrb_handle* h) { return h->g.A; }
@@ -732,7 +776,9 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
   // after the waves already enqueued there (ModelLocker::updateModel waits for in-flight forwards; here nothing waits — the
   // generator's software pipeline keeps running) and before everything enqueued later.
   const size_t total_fp32 = (size_t)Qp * hid + 3 * hid + (size_t)hid * hid + 3 * hid + (size_t)hid * h->Hout + h->Hout;
-  const size_t need = is_tc(h->cfg.net_mode) ? (size_t)cfrb::tc::BlobLayout(Qp).blob_bytes : total_fp32 * sizeof(float);
+  // tensor-core blob: the resident kernel's layout, or the wide kernel's (W3 with tc.nout rows); with 16 outputs the two agree
+  const cfrb::tc::WideLayout L(Qp, h->tc.nout);
+  const size_t need = is_tc(h->cfg.net_mode) ? (size_t)L.blob_bytes : total_fp32 * sizeof(float);
   if (h->w_stage_bytes < need) {
     CK(cudaStreamSynchronize(h->own_stream));
     for (int i = 0; i < 2; ++i) {
@@ -749,7 +795,6 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
   std::memset(h->w_stage[slot], 0, need);
   if (is_tc(h->cfg.net_mode)) {
     // tensor-core blob: fp16 weights in wgmma K-major core-matrix order + fp32 {bias, gamma, beta} per feature
-    const cfrb::tc::BlobLayout L(Qp);
     struct { uint8_t* p; uint8_t* data() { return p; } } blob{h->w_stage[slot]};
     __half* hw1 = reinterpret_cast<__half*>(blob.data() + L.off_w1);
     __half* hw2 = reinterpret_cast<__half*>(blob.data() + L.off_w2);
@@ -769,7 +814,7 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
     float* fb2 = reinterpret_cast<float*>(blob.data() + L.off_b2);      // bias 2, rounded to fp16 like bias 1 in W1
     for (int j = 0; j < hid; ++j) fb2[j] = __half2float(__float2half_rn((float)(b2[j] - m2[hid])));
     for (int j = 0; j < hid; ++j) for (int k = 0; k < hid; ++k) hw2[cfrb::tc::umma_kmajor_offset_halves(j, k, hid)] = __float2half_rn((float)(w2[(size_t)j * hid + k] - m2[k]));
-    for (int j = 0; j < H; ++j) for (int k = 0; k < hid; ++k) hw3[cfrb::tc::umma_kmajor_offset_halves(j, k, cfrb::tc::kNout)] = __float2half_rn(w3[(size_t)j * hid + k]);
+    for (int j = 0; j < H; ++j) for (int k = 0; k < hid; ++k) hw3[cfrb::tc::umma_kmajor_offset_halves(j, k, h->tc.nout)] = __float2half_rn(w3[(size_t)j * hid + k]);
     float* ln1 = reinterpret_cast<float*>(blob.data() + L.off_ln1);
     float* ln2 = reinterpret_cast<float*>(blob.data() + L.off_ln2);
     // the GELU of CFRB_NET_TC_F16X2 evaluates the activation from y / 2: gamma / 2 and beta / 2 are stored
@@ -876,7 +921,6 @@ static int launch_net(cfrb_handle* h, cudaStream_t st, float* dbg1, float* dbg2)
     CK(record_event(h, h->net_ev[h->net_ev_used], st));
   }
   if (is_tc(h->cfg.net_mode)) {
-    const cfrb::tc::BlobLayout L(h->Qpad);
     cfrb::tc::TcArgs a{h->d_blob.p, h->d_Xh.p, h->d_wave.p + 1, h->d_out.p, h->Qpad, h->g.H, h->Hout, dbg1, dbg2, nullptr};
     const int tiles = (h->rows + cfrb::tc::kTileM - 1) / cfrb::tc::kTileM;
     const int grid = (h->capturing || h->rows_on_device) ? h->num_sms : std::min(tiles, h->num_sms);   // surplus CTAs return at once
@@ -886,13 +930,14 @@ static int launch_net(cfrb_handle* h, cudaStream_t st, float* dbg1, float* dbg2)
     // programmatic dependent launch: the kernel fetches its weights while the CFR kernel before it drains
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(grid); lc.blockDim = dim3(cfrb::tc::kThreads); lc.stream = st;
-    lc.dynamicSmemBytes = L.smem_bytes;
+    lc.dynamicSmemBytes = h->tc.smem_bytes;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     lc.attrs = at; lc.numAttrs = dbg ? 0 : 1;
     const int gelu = x2 ? h->x2_gelu : 0;
-    if (dbg && gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 1>, a));
+    if (h->tc.wide) CK(cfrb::tc::wide_launch(lc, a, h->tc.nout, gelu, dbg));
+    else if (dbg && gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 1>, a));
     else if (dbg && gelu == 2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 2>, a));
     else if (dbg) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 0>, a));
     else if (gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<false, 1>, a));
@@ -1141,7 +1186,7 @@ int cfrb_debug_net_trace(cfrb_handle* h, long long* out, int n) {
 }
 
 int cfrb_debug_net_taps(cfrb_handle* h, float* d1, float* d2) {
-  if (!h || !is_tc(h->cfg.net_mode)) return fail(CFRB_EINVAL, "taps exist only for CFRB_NET_TC_F16");
+  if (!h || !is_tc(h->cfg.net_mode)) return fail(CFRB_EINVAL, "taps exist only for the tensor-core value net");
   if (!h->have_weights || h->rows == 0) return fail(CFRB_ESTATE, "no weights or no leaf rows");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaDeviceSynchronize());

@@ -6,6 +6,8 @@
 #pragma once
 #include <cstdlib>
 
+#include "../../../include/cfrb200.h"
+
 namespace liars_dice {
 
 struct SubgameSolvingParams {
@@ -38,11 +40,10 @@ struct RecursiveSolvingParams {
   int host_walk = env_int("CFRB_HOST_WALK", 0);                    // 1 = per-game sampling on the host (parity mode of the device walk)
 };
 
-// The tensor-core value net packs at most 16 output features (num_hands <= 16); larger games run the fp32 SIMT net.
+// A tensor-core net mode falls back to the fp32 SIMT net only on games whose Net2 weights do not fit a tensor-core kernel
+// (cfrb_tc_net_supported: 2x7f, 3x4f, 6x2f, 2x8f, one-die games from 1x33f on, ...).
 inline int effective_net_mode(const RecursiveSolvingParams& p) {
-  long hands = 1;
-  for (int i = 0; i < p.num_dice; ++i) hands *= p.num_faces;
-  return (p.net_mode >= 2 && hands > 16) ? 1 : p.net_mode;
+  return (p.net_mode >= 2 && !cfrb_tc_net_supported(p.num_dice, p.num_faces, 256)) ? 1 : p.net_mode;
 }
 
 }  // namespace liars_dice
