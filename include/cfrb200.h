@@ -20,6 +20,8 @@
  *   cfrb_exploitability             <-  compute_exploitability2        (subgame_solving.cc:802-816)
  *   cfrb_ev2                        <-  compute_ev2                    (subgame_solving.cc:931-982)
  *   cfrb_regrets_*                  <-  compute_immediate_regrets      (subgame_solving.cc:984-1050)
+ *   cfrb_match_*                    <-  compute_[sampled_]strategy_recursive_to_leaf restricted to the path two agents play
+ *                                       (recursive_solving.cc:76-134, 301-327); no counterpart in the reference
  *
  * Conventions: plain C, no exceptions across the boundary; every function returns 0 on success or a
  * negative CFRB_E* code (cfrb_last_error() gives the message for the calling thread); all buffers are
@@ -270,6 +272,48 @@ int cfrb_debug_gelu_table(cfrb_handle* h, int32_t what, uint16_t* out);
 int cfrb_wave_roots(cfrb_handle* h, int32_t* last_bid, int32_t* player_id, int32_t cap);
 /* Block until the work enqueued on `cuda_stream` (NULL = the handle's stream) has finished. */
 int cfrb_stream_wait(cfrb_handle* h, void* cuda_stream);
+
+/* ---- Head-to-head matches: two agents (an agent = one handle: its solver, iterations, CFR/FP settings and value net) play
+ * n_games games of the handles' game against each other on the device, n_slots at a time, one thread per game between waves.
+ * Each agent plays its recursive to-leaf strategy restricted to the path played: compute_strategy_recursive_to_leaf
+ * (recursive_solving.cc:76-134, policy AVERAGE: all num_iters iterations, get_strategy() acts and propagates beliefs) or
+ * compute_sampled_strategy_recursive_to_leaf without root_only (:301-327, policy SAMPLED: per subgame act_iteration ~ weight
+ * i/2 + 1 on even i < num_iters, the sampling strategy snapshotted at act_iteration acts and propagates beliefs).  It solves
+ * the subgame rooted at the current public node from its own beliefs at the game root and at every pseudo-leaf of its previous
+ * subgame, acts for the hand dealt to its seat, and updates both players' beliefs with its own strategy at every node
+ * (unnormalised inside a subgame, normalize_beliefs_inplace at its leaves, :41-44).
+ * Deals: each seat's hand uniform over the H hands; games 2i and 2i+1 share the hands and swap the agents' seats (agent A sits
+ * in seat 0 in even games).  Payoff to A: +1 / -1 at the liar call (the bidder wins iff both hands hold at least the bid's
+ * quantity of its face, the last face being wild).  Every draw of game g comes from mt19937 streams keyed by (seed, g) (the
+ * deal by (seed, g / 2)), so results do not depend on n_slots.  Slot s plays games s, s + n_slots, ... to their ends.
+ * While a match is live its handles serve only the match; afterwards a handle's "current wave" (cfrb_fetch, cfrb_wave_roots,
+ * ...) is the last wave the match enqueued, which is empty once every game had finished before it. */
+enum {
+  CFRB_MATCH_AVERAGE = 0,
+  CFRB_MATCH_SAMPLED = 1
+};
+enum { CFRB_MATCH_TRACE_GAMES = 256 };   /* games < min(n_games, this) are traced (cfrb_match_trace) */
+typedef struct cfrb_match cfrb_match;
+/* a, b: two distinct handles with the same game, max_depth, device and state dtype, max_subgames >= n_slots, no live self-play
+ * session or match.  n_games even.  Each violation returns CFRB_EINVAL with a message. */
+int cfrb_match_create(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out);
+/* Enqueue max_rounds rounds on `cuda_stream` (NULL = a's stream); a round is one wave of num_iters iterations per agent (the
+ * subgames of every running game, built on the device) and one walk.  Returns max_rounds, or 0 once every game has finished
+ * (learned from the previous call's rounds, without further work). */
+int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream);
+/* Synchronises.  payoff_a [n_games] (0 for a game not finished yet), plies [n_games]; solves = subgames solved by both agents;
+ * subgame_iters = CFR / FP iterations run for them.  Any pointer may be NULL. */
+int cfrb_match_results(cfrb_match* m, float* payoff_a, int32_t* plies, int64_t* solves, int64_t* subgame_iters);
+/* Synchronises.  Trace of one game < min(n_games, CFRB_MATCH_TRACE_GAMES); returns its number of plies P (<= A).
+ *   ply_records [A][6]  per ply: agent that acted (0 = a), last bid before the action, acting player (seat), its hand, action,
+ *                       subgame (round) index within the game
+ *   probs [A]           fp64 probability of that action in the acting agent's strategy
+ *   act_iterations [A][2], root_beliefs [A][2][2][H]: per subgame r < *n_rounds, each agent's act_iteration (-1 = AVERAGE) and
+ *                       root beliefs [player][hand] (fp64, before the conversion to the state dtype)
+ * Any pointer may be NULL. */
+int cfrb_match_trace(cfrb_match* m, int32_t game, int32_t* ply_records, double* probs, int32_t* act_iterations, double* root_beliefs,
+                     int32_t* n_rounds);
+int cfrb_match_destroy(cfrb_match* m);
 
 /* ---- Device-resident example rows: storage of the replay buffer (rela/prioritized_replay.h:224-506 keeps one pair of host
  * tensors per example; here the rows of the ring live in HBM as two [capacity][dim] fp32 matrices and never visit the host on

@@ -102,6 +102,11 @@ def lib():
     L.cfrb_rows_write.argtypes = [vp, C.c_int64, C.c_int32, vp, vp, C.c_int32, C.c_int32]
     L.cfrb_rows_read.argtypes = [vp, C.c_int64, C.c_int32, _fp, _fp]
     L.cfrb_rows_gather.argtypes = [vp, _ip, C.c_int32, vp, vp, C.c_int32, vp]
+    L.cfrb_match_create.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_uint64, C.c_int32, C.POINTER(vp)]
+    L.cfrb_match_run.argtypes = [vp, C.c_int32, vp]
+    L.cfrb_match_results.argtypes = [vp, _fp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    L.cfrb_match_trace.argtypes = [vp, C.c_int32, _ip, _dp, _ip, _dp, _ip]
+    L.cfrb_match_destroy.argtypes = [vp]
     _lib = L
     return L
 
@@ -326,3 +331,55 @@ class WaveSolver:
         a, b = C.c_float(0), C.c_float(0)
         _check(lib().cfrb_last_run_ms(self._h, C.byref(a), C.byref(b)))
         return a.value, b.value
+
+
+MATCH_AVERAGE, MATCH_SAMPLED = 0, 1
+MATCH_TRACE_GAMES = 256
+
+
+class Match:
+    """A head-to-head match between the agents of two WaveSolvers (cfrb_match_*): n_games games, n_slots at a time."""
+
+    def __init__(self, a, b, n_slots, n_games, seed=0, policy=MATCH_SAMPLED):
+        self.a, self.b, self.G = a, b, n_games
+        self._m = C.c_void_p()
+        _check(lib().cfrb_match_create(a._h, b._h, n_slots, n_games, seed, policy, C.byref(self._m)))
+
+    def close(self):
+        if self._m:
+            lib().cfrb_match_destroy(self._m)
+            self._m = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def run(self, max_rounds=8, stream=None):
+        """Enqueue rounds; 0 once every game has finished."""
+        return _check(lib().cfrb_match_run(self._m, max_rounds, C.c_void_p(stream) if stream else None))
+
+    def play(self):
+        while self.run() > 0:
+            pass
+        return self.results()
+
+    def results(self):
+        pay = np.zeros(self.G, np.float32)
+        plies = np.zeros(self.G, np.int32)
+        solves, iters = C.c_int64(0), C.c_int64(0)
+        _check(lib().cfrb_match_results(self._m, _p(pay, _fp), _p(plies, _ip), C.byref(solves), C.byref(iters)))
+        return {"payoff_a": pay, "plies": plies, "solves": solves.value, "subgame_iters": iters.value}
+
+    def trace(self, game):
+        """dict: plies [P, 6] (agent, last bid, player, hand, action, round), prob [P], act_iteration [R, 2], root_beliefs [R, 2, 2, H]."""
+        A, H = self.a.A, self.a.H
+        rec = np.zeros((A, 6), np.int32)
+        prob = np.zeros(A, np.float64)
+        act = np.zeros((A, 2), np.int32)
+        bel = np.zeros((A, 2, 2, H), np.float64)
+        nr = C.c_int32(0)
+        n = _check(lib().cfrb_match_trace(self._m, game, _p(rec, _ip), _p(prob, _dp), _p(act, _ip), _p(bel, _dp), C.byref(nr)))
+        r = nr.value
+        return {"plies": rec[:n], "prob": prob[:n], "act_iteration": act[:r], "root_beliefs": bel[:r]}

@@ -7,6 +7,7 @@
 #include "br_kernel.cuh"
 #include "ev_regret_kernels.cuh"
 #include "selfplay_kernels.cuh"
+#include "match_kernels.cuh"
 #include "cfr_d2v2.cuh"
 
 namespace cfrb {
@@ -109,6 +110,16 @@ void sp_launch_finish(const SpDev& p, const real* mu, const real* snap, float* e
   if (ex_q) sp_examples_kernel<real><<<(2 * p.K + 127) / 128, 128, 0, st>>>(p, mu, ex_q, ex_v);
   sp_advance_kernel<real><<<(p.K + 127) / 128, 128, 0, st>>>(p, snap);
 }
+void match_launch_deal(const MatchDev& p, cudaStream_t st) { match_deal_kernel<<<(p.S + 127) / 128, 128, 0, st>>>(p); }
+template <typename real>
+void match_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
+  match_scan_kernel<<<1, 1024, 0, st>>>(p);
+  match_begin_kernel<real><<<(p.S + 127) / 128, 128, 0, st>>>(p, t);
+}
+template <typename real>
+void match_launch_advance(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
+  match_advance_kernel<real><<<(p.S + 127) / 128, 128, 0, st>>>(p, t);
+}
 __global__ void rows_gather_kernel(const float* __restrict__ src, int width, const int* __restrict__ ids, int n, float* __restrict__ out) {
   const size_t total = (size_t)n * width;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -186,7 +197,9 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template int cfr_d2v2_smem_bytes<real>(int, int, int, int, int, int, int);                                                \
   template void cfr_launch_iter_d2v2<real>(const CfrDev<real>&, int, int, size_t, cudaStream_t, int, int, int, int);             \
   template void sp_launch_begin<real>(const SpDev&, real*, cudaStream_t);                                                  \
-  template void sp_launch_finish<real>(const SpDev&, const real*, const real*, float*, float*, cudaStream_t);
+  template void sp_launch_finish<real>(const SpDev&, const real*, const real*, float*, float*, cudaStream_t);              \
+  template void match_launch_begin<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                           \
+  template void match_launch_advance<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);
 CFRB_INSTANTIATE(float)
 CFRB_INSTANTIATE(double)
 

@@ -116,6 +116,45 @@ void sp_launch_seed(const SpDev& p, const uint32_t* dev_seeds, cudaStream_t st);
 template <typename real> void sp_launch_begin(const SpDev& p, real* wave_beliefs, cudaStream_t st);
 // training examples of the finished wave (skipped when ex_q == nullptr) and the sampling step of every game
 template <typename real> void sp_launch_finish(const SpDev& p, const real* mu, const real* snap, float* ex_q, float* ex_v, cudaStream_t st);
+// Head-to-head matches (match_kernels.cuh): S game slots playing G games between two handles (agent 0 = A, 1 = B).
+struct MatchDev {
+  int S, G, A, H, F, max_depth, sampled, iters[2];
+  uint64_t seed;
+  // per slot
+  int* game;                          // [S] game being played, -1 = quota done
+  int* last_bid; int* player;         // [S] public node at the root of the slot's next subgames
+  int* hands;                         // [S][2] dealt hand of each seat
+  int* ply; int* round;               // [S] plies / subgames so far in the current game
+  int* widx;                          // [S] wave index of the slot in this round (-1 = not running)
+  int* act;                           // [S][2] act_iteration of each agent's current subgame
+  double* bel;                        // [S][2 agents][2 players][H] fp64 beliefs
+  uint32_t* mt; int* mt_idx;          // [624][S], [S]
+  int* running;                       // [1] slots in this round's wave
+  int* left;                          // [1] slots still holding a game after this round's walk
+  // per game
+  float* payoff; int* plies; int* rounds;   // [G]
+  // trace of games < trace_games: per ply {agent, last bid, player, hand, action, round} and the probability of the action, per
+  // subgame both agents' act_iteration and root beliefs
+  int trace_games;
+  int* tr_ply; double* tr_prob; int* tr_plies;             // [T][A][6], [T][A], [T]
+  int* tr_act; double* tr_bel; int* tr_rounds;             // [T][A][2], [T][A][2][2][H], [T]
+  // tree templates (read-only; both handles index the same ones)
+  const TemplateDev* tmpl; const int* child_begin; const int* nchild;
+  const unsigned char* matches;       // [H][F]
+  int table_stride;
+  // each agent's wave descriptors and CFR step counters
+  int* wave[2]; int* sg_tmpl[2]; int* sg_player[2]; int* sg_row_off[2]; int* sg_act[2]; const int* steps[2];
+};
+template <typename real>
+struct MatchTabs {
+  real* wave_beliefs[2];              // each handle's [K][2][H] root beliefs
+  const real* table[2];               // the table each agent acts with: S (CFR average, normalised), Sg (FP average) or Snap
+  int normalise[2];
+};
+void match_launch_deal(const MatchDev& p, cudaStream_t st);
+// scan + subgame descriptors of the next round
+template <typename real> void match_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st);
+template <typename real> void match_launch_advance(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st);
 // rows [ids[i]] of a [*, width] fp32 matrix -> out[i]  (replay sampling)
 void rows_launch_gather(const float* src, int width, const int* ids, int n, float* out, cudaStream_t st);
 

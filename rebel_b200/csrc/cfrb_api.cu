@@ -187,6 +187,7 @@ struct cfrb_handle {
   void* flush_buf = nullptr; size_t flush_bytes = 0;                                                 // cfrb_l2_flush
   bool rows_on_device = false;   // the wave was built on the device: its row count / roots exist only there
   bool mirror_stale = false;     // ... and the host mirror (h_tmpl, h_beliefs, rows) has not been pulled yet
+  bool in_match = false;         // an agent of a live cfrb_match: its waves are built by the match
 };
 
 template <typename real> static WaveState<real>& state_of(cfrb_handle* h);
@@ -1617,6 +1618,225 @@ int cfrb_stream_wait(cfrb_handle* h, void* cuda_stream) {
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream));
   return CFRB_OK;
+}
+
+}  // extern "C"
+
+// ============================================================================================ head-to-head matches
+struct cfrb_match {
+  cfrb_handle* h[2] = {nullptr, nullptr};
+  int S = 0, G = 0, T = 0;
+  DevBuf<int> game, last_bid, player, hands, ply, round, widx, act, mt_idx, running, left, plies, rounds;
+  DevBuf<int> tr_ply, tr_plies, tr_act, tr_rounds;
+  DevBuf<double> bel, tr_prob, tr_bel;
+  DevBuf<float> payoff;
+  DevBuf<uint32_t> mt;
+  cfrb::MatchDev dev{};
+  int* pin_left = nullptr;            // slots with a game left, copied behind the last round of every cfrb_match_run
+  cudaEvent_t ev_left = nullptr;
+  bool ev_recorded = false;
+  void release() {
+    for (auto* b : {&game, &last_bid, &player, &hands, &ply, &round, &widx, &act, &mt_idx, &running, &left, &plies, &rounds, &tr_ply,
+                    &tr_plies, &tr_act, &tr_rounds})
+      b->release();
+    bel.release(); tr_prob.release(); tr_bel.release(); payoff.release(); mt.release();
+    if (pin_left) cudaFreeHost(pin_left);
+    if (ev_left) cudaEventDestroy(ev_left);
+    pin_left = nullptr; ev_left = nullptr;
+  }
+};
+
+template <typename real>
+static cfrb::MatchTabs<real> match_tabs(cfrb_match* m, int policy_sampled) {
+  cfrb::MatchTabs<real> t{};
+  for (int k = 0; k < 2; ++k) {
+    cfrb_handle* h = m->h[k];
+    auto& s = state_of<real>(h);
+    const bool fp = h->cfg.solver == CFRB_SOLVER_FP;
+    t.wave_beliefs[k] = s.beliefs.p;
+    t.table[k] = policy_sampled ? s.Snap.p : fp ? s.Sg.p : s.S.p;
+    t.normalise[k] = !policy_sampled && !fp;
+  }
+  return t;
+}
+template <typename real>
+static int match_begin_t(cfrb_match* m, cudaStream_t st) {
+  cfrb::match_launch_begin<real>(m->dev, match_tabs<real>(m, m->dev.sampled), st);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+template <typename real>
+static int match_advance_t(cfrb_match* m, cudaStream_t st) {
+  cfrb::match_launch_advance<real>(m->dev, match_tabs<real>(m, m->dev.sampled), st);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+
+// Everything enqueued has finished: each handle's current wave becomes the match's last wave (its size lives on the device).
+static int match_settle(cfrb_match* m) {
+  CK(cudaSetDevice(m->h[0]->cfg.device));
+  CK(cudaDeviceSynchronize());
+  for (cfrb_handle* h : m->h) {
+    int wave[2] = {0, 0};
+    CK(cudaMemcpy(wave, h->d_wave.p, sizeof(wave), cudaMemcpyDeviceToHost));
+    h->n = wave[0];
+    h->mirror_stale = true;
+  }
+  return CFRB_OK;
+}
+
+extern "C" {
+
+int cfrb_match_destroy(cfrb_match* m) {
+  if (!m) return CFRB_OK;
+  int rc = CFRB_OK;
+  if (m->h[0]) {
+    rc = match_settle(m);
+    for (cfrb_handle* h : m->h) h->in_match = false;
+  }
+  m->release();
+  delete m;
+  return rc;
+}
+
+static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed,
+                             int32_t policy) {
+  if (!a || !b) return fail(CFRB_EINVAL, "cfrb_match_create: null handle");
+  if (a == b) return fail(CFRB_EINVAL, "cfrb_match_create: the two agents need two handles (create a second one with the same config)");
+  if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_SAMPLED) return fail(CFRB_EINVAL, "cfrb_match_create: bad policy");
+  if (n_slots < 1) return fail(CFRB_EINVAL, "cfrb_match_create: n_slots must be >= 1");
+  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, "cfrb_match_create: n_games must be even and >= 2 (seat-swapped pairs)");
+  const auto &ca = a->cfg, &cb = b->cfg;
+  if (ca.num_dice != cb.num_dice || ca.num_faces != cb.num_faces)
+    return fail(CFRB_EINVAL, "cfrb_match_create: the agents play different games (" + std::to_string(ca.num_dice) + "x" +
+                                 std::to_string(ca.num_faces) + "f vs " + std::to_string(cb.num_dice) + "x" + std::to_string(cb.num_faces) + "f)");
+  if (ca.max_depth != cb.max_depth)
+    return fail(CFRB_EINVAL, "cfrb_match_create: the agents have different max_depth (" + std::to_string(ca.max_depth) + " vs " +
+                                 std::to_string(cb.max_depth) + ")");
+  if (ca.device != cb.device) return fail(CFRB_EINVAL, "cfrb_match_create: the agents are on different devices");
+  if (ca.state_dtype != cb.state_dtype) return fail(CFRB_EINVAL, "cfrb_match_create: the agents have different state dtypes");
+  for (cfrb_handle* h : {a, b}) {
+    if (h->cfg.max_subgames < n_slots)
+      return fail(CFRB_EINVAL, "cfrb_match_create: a handle's capacity (max_subgames " + std::to_string(h->cfg.max_subgames) +
+                                   ") is smaller than n_slots " + std::to_string(n_slots));
+    if (h->sp.ready) return fail(CFRB_EINVAL, "cfrb_match_create: a handle has a live self-play session");
+    if (h->in_match) return fail(CFRB_EINVAL, "cfrb_match_create: a handle already plays in a live match");
+  }
+  CK(cudaSetDevice(ca.device));
+  CK(cudaDeviceSynchronize());
+  const int S = n_slots, G = n_games, H = a->g.H, A = a->g.A, T = std::min(G, (int)CFRB_MATCH_TRACE_GAMES);
+  m->S = S; m->G = G; m->T = T;
+  for (auto* p : {&m->game, &m->last_bid, &m->player, &m->ply, &m->round, &m->widx, &m->mt_idx}) CK(p->alloc(S));
+  CK(m->hands.alloc((size_t)2 * S)); CK(m->act.alloc((size_t)2 * S));
+  CK(m->running.alloc(1)); CK(m->left.alloc(1));
+  CK(m->bel.alloc((size_t)S * 4 * H)); CK(m->mt.alloc((size_t)624 * S));
+  CK(m->payoff.alloc(G)); CK(m->plies.alloc(G)); CK(m->rounds.alloc(G));
+  CK(cudaMemset(m->payoff.p, 0, (size_t)G * sizeof(float)));
+  CK(cudaMemset(m->plies.p, 0, (size_t)G * sizeof(int)));
+  CK(cudaMemset(m->rounds.p, 0, (size_t)G * sizeof(int)));
+  CK(m->tr_ply.alloc((size_t)T * A * 6)); CK(m->tr_prob.alloc((size_t)T * A)); CK(m->tr_plies.alloc(T));
+  CK(m->tr_act.alloc((size_t)T * A * 2)); CK(m->tr_bel.alloc((size_t)T * A * 4 * H)); CK(m->tr_rounds.alloc(T));
+  CK(cudaMemset(m->tr_plies.p, 0, (size_t)T * sizeof(int)));
+  CK(cudaMemset(m->tr_rounds.p, 0, (size_t)T * sizeof(int)));
+  CK(cudaMallocHost((void**)&m->pin_left, sizeof(int)));
+  CK(cudaEventCreateWithFlags(&m->ev_left, cudaEventDisableTiming));
+  cfrb::MatchDev& d = m->dev;
+  d.S = S; d.G = G; d.A = A; d.H = H; d.F = a->g.F; d.max_depth = ca.max_depth; d.sampled = policy == CFRB_MATCH_SAMPLED;
+  d.iters[0] = ca.num_iters; d.iters[1] = cb.num_iters; d.seed = seed;
+  d.game = m->game.p; d.last_bid = m->last_bid.p; d.player = m->player.p; d.hands = m->hands.p; d.ply = m->ply.p; d.round = m->round.p;
+  d.widx = m->widx.p; d.act = m->act.p; d.bel = m->bel.p; d.mt = m->mt.p; d.mt_idx = m->mt_idx.p; d.running = m->running.p;
+  d.left = m->left.p;
+  d.payoff = m->payoff.p; d.plies = m->plies.p; d.rounds = m->rounds.p;
+  d.trace_games = T; d.tr_ply = m->tr_ply.p; d.tr_prob = m->tr_prob.p; d.tr_plies = m->tr_plies.p; d.tr_act = m->tr_act.p;
+  d.tr_bel = m->tr_bel.p; d.tr_rounds = m->tr_rounds.p;
+  d.tmpl = a->d_tmpl.p; d.child_begin = a->d_child_begin.p; d.nchild = a->d_nchild.p; d.matches = a->d_matches.p;
+  d.table_stride = a->table_stride;
+  cfrb_handle* hs[2] = {a, b};
+  for (int k = 0; k < 2; ++k) {
+    cfrb_handle* h = hs[k];
+    d.wave[k] = h->d_wave.p; d.sg_tmpl[k] = h->d_sg_tmpl.p; d.sg_player[k] = h->d_sg_player.p; d.sg_row_off[k] = h->d_sg_row_off.p;
+    d.sg_act[k] = h->d_sg_act.p; d.steps[k] = h->d_steps.p;
+  }
+  cfrb::match_launch_deal(d, a->own_stream);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(a->own_stream));
+  m->h[0] = a; m->h[1] = b;
+  a->in_match = b->in_match = true;
+  return CFRB_OK;
+}
+
+int cfrb_match_create(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out) {
+  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create: null argument");
+  *out = nullptr;
+  cfrb_match* m = new cfrb_match();
+  const int rc = match_create_impl(m, a, b, n_slots, n_games, seed, policy);
+  if (rc != CFRB_OK) {
+    m->release();
+    delete m;
+    return rc;
+  }
+  *out = m;
+  return CFRB_OK;
+}
+
+int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
+  if (!m || max_rounds < 1) return fail(CFRB_EINVAL, "cfrb_match_run: bad argument");
+  CK(cudaSetDevice(m->h[0]->cfg.device));
+  if (m->ev_recorded) {
+    CK(cudaEventSynchronize(m->ev_left));
+    if (*m->pin_left == 0) return 0;
+  }
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->h[0]->own_stream;
+  for (int r = 0; r < max_rounds; ++r) {
+    int rc = DISPATCH_REAL(m->h[0], match_begin_t, m, st);
+    if (rc) return rc;
+    for (cfrb_handle* h : m->h) {
+      h->n = m->S; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
+      if ((rc = DISPATCH_REAL(h, launch_init_t, h, st))) return rc;
+      if ((rc = cfrb_run(h, h->cfg.num_iters, st))) return rc;
+    }
+    CK(cudaMemsetAsync(m->left.p, 0, sizeof(int), st));
+    if ((rc = DISPATCH_REAL(m->h[0], match_advance_t, m, st))) return rc;
+    m->h[0]->launches += 3;
+  }
+  CK(cudaMemcpyAsync(m->pin_left, m->left.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(m->ev_left, st));
+  m->ev_recorded = true;
+  return max_rounds;
+}
+
+int cfrb_match_results(cfrb_match* m, float* payoff_a, int32_t* plies, int64_t* solves, int64_t* subgame_iters) {
+  if (!m) return fail(CFRB_EINVAL, "cfrb_match_results: null match");
+  int rc = match_settle(m);
+  if (rc) return rc;
+  const int G = m->G;
+  std::vector<int> rounds(G);
+  CK(cudaMemcpy(rounds.data(), m->rounds.p, (size_t)G * sizeof(int), cudaMemcpyDeviceToHost));
+  if (payoff_a) CK(cudaMemcpy(payoff_a, m->payoff.p, (size_t)G * sizeof(float), cudaMemcpyDeviceToHost));
+  if (plies) CK(cudaMemcpy(plies, m->plies.p, (size_t)G * sizeof(int), cudaMemcpyDeviceToHost));
+  int64_t r = 0;
+  for (int x : rounds) r += x;
+  if (solves) *solves = 2 * r;
+  if (subgame_iters) *subgame_iters = r * ((int64_t)m->dev.iters[0] + m->dev.iters[1]);
+  return CFRB_OK;
+}
+
+int cfrb_match_trace(cfrb_match* m, int32_t game, int32_t* ply_records, double* probs, int32_t* act_iterations, double* root_beliefs,
+                     int32_t* n_rounds) {
+  if (!m) return fail(CFRB_EINVAL, "cfrb_match_trace: null match");
+  if (game < 0 || game >= m->T) return fail(CFRB_EINVAL, "cfrb_match_trace: only games < min(n_games, CFRB_MATCH_TRACE_GAMES) are traced");
+  int rc = match_settle(m);
+  if (rc) return rc;
+  const size_t A = m->dev.A, H = m->dev.H;
+  int np = 0, nr = 0;
+  CK(cudaMemcpy(&np, m->tr_plies.p + game, sizeof(int), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(&nr, m->tr_rounds.p + game, sizeof(int), cudaMemcpyDeviceToHost));
+  if (ply_records) CK(cudaMemcpy(ply_records, m->tr_ply.p + game * A * 6, A * 6 * sizeof(int), cudaMemcpyDeviceToHost));
+  if (probs) CK(cudaMemcpy(probs, m->tr_prob.p + game * A, A * sizeof(double), cudaMemcpyDeviceToHost));
+  if (act_iterations) CK(cudaMemcpy(act_iterations, m->tr_act.p + game * A * 2, A * 2 * sizeof(int), cudaMemcpyDeviceToHost));
+  if (root_beliefs) CK(cudaMemcpy(root_beliefs, m->tr_bel.p + game * A * 4 * H, A * 4 * H * sizeof(double), cudaMemcpyDeviceToHost));
+  if (n_rounds) *n_rounds = nr;
+  return np;
 }
 
 // ============================================================================================ device-resident example rows

@@ -46,4 +46,17 @@ inline int effective_net_mode(const RecursiveSolvingParams& p) {
   return (p.net_mode >= 2 && !cfrb_tc_net_supported(p.num_dice, p.num_faces, 256)) ? 1 : p.net_mode;
 }
 
+// The handle configuration of a recursive solver with these parameters and `capacity` subgames per wave.
+inline cfrb_config solver_config(const RecursiveSolvingParams& cfg, int device, int capacity) {
+  const auto& sp = cfg.subgame_params;
+  cfrb_config c{};
+  c.solver = sp.use_cfr ? CFRB_SOLVER_CFR : CFRB_SOLVER_FP;
+  c.optimistic = sp.optimistic;
+  c.num_dice = cfg.num_dice; c.num_faces = cfg.num_faces; c.max_depth = sp.max_depth; c.num_iters = sp.num_iters;
+  c.linear_update = sp.linear_update; c.dcfr = sp.dcfr; c.dcfr_alpha = sp.dcfr_alpha; c.dcfr_beta = sp.dcfr_beta;
+  c.dcfr_gamma = sp.dcfr_gamma; c.max_subgames = capacity; c.device = device; c.net_mode = effective_net_mode(cfg); c.hidden = 256;
+  c.state_dtype = cfg.state_dtype;
+  return c;
+}
+
 }  // namespace liars_dice

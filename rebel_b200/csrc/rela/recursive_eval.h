@@ -74,13 +74,7 @@ class RecursiveEvaluator {
   RecursiveEvaluator(const liars_dice::RecursiveSolvingParams& cfg, int device, int wave_capacity)
       : cfg_(cfg), K_(std::max(1, wave_capacity)) {
     const auto& sp = cfg.subgame_params;
-    cfrb_config c{};
-    c.solver = sp.use_cfr ? CFRB_SOLVER_CFR : CFRB_SOLVER_FP;
-    c.optimistic = sp.optimistic;
-    c.num_dice = cfg.num_dice; c.num_faces = cfg.num_faces; c.max_depth = sp.max_depth; c.num_iters = sp.num_iters;
-    c.linear_update = sp.linear_update; c.dcfr = sp.dcfr; c.dcfr_alpha = sp.dcfr_alpha; c.dcfr_beta = sp.dcfr_beta;
-    c.dcfr_gamma = sp.dcfr_gamma; c.max_subgames = K_; c.device = device; c.net_mode = liars_dice::effective_net_mode(cfg); c.hidden = 256;
-    c.state_dtype = cfg.state_dtype;
+    const cfrb_config c = liars_dice::solver_config(cfg, device, K_);
     if (cfrb_create(&c, &h_) < 0) throw std::runtime_error(std::string("cfrb_create: ") + cfrb_last_error());
     A_ = cfrb_num_actions(h_); H_ = cfrb_num_hands(h_); stride_ = cfrb_table_stride(h_);
     // full tree + the order in which the reference's recursion creates subgame solvers (= order of its RNG draws)

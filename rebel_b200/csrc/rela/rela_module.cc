@@ -13,6 +13,7 @@
 #include "params.h"
 #include "recursive_eval.h"
 #include "evaluation.h"
+#include "match.h"
 #include "replay.h"
 #include "runtime.h"
 
@@ -525,6 +526,61 @@ std::tuple<double, double> exploitability_of_strategy(int num_dice, int num_face
   return std::make_tuple(e[0], e[1]);
 }
 
+std::vector<float> flat_of(py::object w) {
+  std::vector<float> v;
+  if (!w.is_none()) {
+    auto t = w.cast<torch::Tensor>().to(torch::kCPU, torch::kFloat32).contiguous();
+    v.assign(t.data_ptr<float>(), t.data_ptr<float>() + t.numel());
+  }
+  return v;
+}
+
+py::dict stats_dict(const std::vector<float>& payoff) {
+  const MatchStats s = match_stats(payoff);
+  py::dict d;
+  d["mean"] = s.mean; d["stderr"] = s.stderr_; d["seat_means"] = std::vector<double>{s.seat[0], s.seat[1]};
+  return d;
+}
+
+py::dict play_match_py(const RecursiveSolvingParams& cfg_a, const RecursiveSolvingParams& cfg_b, int device, int games, uint64_t seed,
+                       const std::string& policy, py::object flat_weights_a, py::object flat_weights_b, int concurrent_games) {
+  if (policy != "sampled" && policy != "average") throw std::runtime_error("play_match: policy must be 'sampled' or 'average'");
+  const std::vector<float> wa = flat_of(flat_weights_a), wb = flat_of(flat_weights_b);
+  MatchResult r;
+  {
+    py::gil_scoped_release nogil;
+    r = play_match(cfg_a, cfg_b, device, games, seed, policy == "sampled" ? CFRB_MATCH_SAMPLED : CFRB_MATCH_AVERAGE, wa, wb,
+                   concurrent_games);
+  }
+  py::dict d = stats_dict(r.payoff);
+  auto p = torch::empty({(int64_t)games}, torch::kFloat32);
+  std::copy(r.payoff.begin(), r.payoff.end(), p.data_ptr<float>());
+  auto pl = torch::empty({(int64_t)games}, torch::kInt32);
+  std::copy(r.plies.begin(), r.plies.end(), pl.data_ptr<int32_t>());
+  d["payoff_a"] = p; d["plies"] = pl; d["solves"] = r.solves; d["subgame_iters"] = r.subgame_iters; d["seconds"] = r.seconds;
+  return d;
+}
+
+py::dict match_stats_py(torch::Tensor payoff) {
+  auto t = payoff.to(torch::kCPU, torch::kFloat32).contiguous();
+  return stats_dict(std::vector<float>(t.data_ptr<float>(), t.data_ptr<float>() + t.numel()));
+}
+
+// compute_strategy_recursive_to_leaf (recursive_solving.cc:76-134) of one agent: dense [N, H, A] fp64.
+torch::Tensor strategy_recursive_to_leaf(const RecursiveSolvingParams& cfg, int device, py::object flat_weights) {
+  const std::vector<float> w = flat_of(flat_weights);
+  std::vector<double> s;
+  int64_t N = 0, H = 0, A = 0;
+  {
+    py::gil_scoped_release nogil;
+    RecursiveEvaluator ev(cfg, device, 8192);
+    if (!w.empty()) ev.setWeights(w);
+    s = ev.strategyToLeaf();
+    N = ev.numNodes(); H = ev.numHands(); A = ev.numActions();
+  }
+  return f64_tensor(s, {N, H, A});
+}
+
 }  // namespace
 
 PYBIND11_MODULE(rela, m) {
@@ -641,4 +697,17 @@ PYBIND11_MODULE(rela, m) {
         "rebel_b200 extension: recursive_eval's full-tree solve — dict with checkpoints, exploitability [C, 2], the final "
         "get_strategy() [N, H, A] and, with track_regrets (CFR), the immediate regrets of the sampling strategies of the "
         "even iterations (immediate_regrets, regret_sums, regret_count).");
+  m.def("play_match", &play_match_py, py::arg("cfg_a"), py::arg("cfg_b"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
+        py::arg("policy") = "sampled", py::arg("flat_weights_a") = py::none(), py::arg("flat_weights_b") = py::none(),
+        py::arg("concurrent_games") = 8192,
+        "rebel_b200 extension: `games` head-to-head games (seat-swapped pairs) of agent A (cfg_a + net A) against agent B on the GPU, "
+        "each re-solving subgames along the path played with its recursive to-leaf policy ('average' or 'sampled').  dict: payoff_a "
+        "[games] (to A), plies [games], mean, stderr (over pairs), seat_means [2] (A in seat 0 / seat 1), solves, subgame_iters, "
+        "seconds.");
+  m.def("match_stats", &match_stats_py, py::arg("payoff_a"),
+        "rebel_b200 extension: play_match's mean, stderr (over the pairs 2i, 2i+1) and seat_means of a payoff vector.");
+  m.def("strategy_recursive_to_leaf", &strategy_recursive_to_leaf, py::arg("cfg"), py::arg("device") = 0,
+        py::arg("flat_weights") = py::none(),
+        "rebel_b200 extension: compute_strategy_recursive_to_leaf (every subgame solved for num_iters iterations, get_strategy) as a "
+        "dense full-tree strategy [N, H, A] fp64 (games whose full tree has at most 2^20 nodes).");
 }
