@@ -315,6 +315,29 @@ int cfrb_match_trace(cfrb_match* m, int32_t game, int32_t* ply_records, double* 
                      int32_t* n_rounds);
 int cfrb_match_destroy(cfrb_match* m);
 
+/* ---- Local best response (Lisy & Bowling, 2017): a lower bound on one agent's exploitability on any game.  The agent (one
+ * handle) plays as in a CFRB_MATCH_AVERAGE match against LBR, which best-responds one decision at a time: with its fp64 belief
+ * beta over the agent's hand (uniform, times the agent's strategy after every agent action, renormalised) it plays the argmax
+ * (ties: the smallest action) of
+ *   liar (b >= 0):  sum_h beta[h] (b true ? -1 : +1)
+ *   raise a:        sum_h beta[h] sum_{a' legal after a, liar last} sigma(child(a), h, a') (a' liar ? (a true ? +1 : -1)
+ *                                                                                     : (a' true ? -1 : +1))
+ * (a bid is true for agent hand h when LBR's and h's matches of its face reach its quantity; every raise of the agent is
+ * assumed to be called).  sigma(child(a)) comes from the agent's current subgame, or, when child(a) is a pseudo-leaf of it,
+ * from the root of the agent's subgame at child(a) solved from its beliefs propagated through its own strategy ("what-if"
+ * solves, one per raise; the chosen one is the agent's next subgame).  Seats, deals and the agent's draws are those of
+ * cfrb_match_create: the agent sits in seat 0 in even games.  A round solves at most max_subgames subgames: running games ask
+ * for 1 subgame (game start, pseudo-leaf) or m (an LBR decision with m raises) and are admitted round-robin; the others wait.
+ * cfrb_match_run / _results / _trace / _destroy apply: payoff_a is the agent's payoff (LBR's is its negative), solves counts
+ * every subgame solved, what-if ones included; in the trace agent 1 is LBR (probability 1, act_iteration and root beliefs 0).
+ * agent: max_subgames >= A - 1, no live self-play session or match; n_games even.  Each violation returns CFRB_EINVAL. */
+int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out);
+/* Synchronises.  For a traced game: per ply where LBR acted, values [A][A] (fp64 value of every action, NaN where illegal and on
+ * the agent's plies) and beliefs [A][H] (beta before the decision, 0 on the agent's plies).  Returns the number of plies. */
+int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* beliefs);
+/* Synchronises.  what-if subgames solved, and running slots that waited a round for capacity (summed over rounds). */
+int cfrb_match_lbr_counts(cfrb_match* m, int64_t* whatif_solves, int64_t* deferred_slot_rounds);
+
 /* ---- Device-resident example rows: storage of the replay buffer (rela/prioritized_replay.h:224-506 keeps one pair of host
  * tensors per example; here the rows of the ring live in HBM as two [capacity][dim] fp32 matrices and never visit the host on
  * their way from the generator kernels to the trainer's batch).  Bookkeeping (head, size, priorities, blocking) stays with the

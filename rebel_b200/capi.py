@@ -107,6 +107,9 @@ def lib():
     L.cfrb_match_results.argtypes = [vp, _fp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.cfrb_match_trace.argtypes = [vp, C.c_int32, _ip, _dp, _ip, _dp, _ip]
     L.cfrb_match_destroy.argtypes = [vp]
+    L.cfrb_match_create_lbr.argtypes = [vp, C.c_int32, C.c_int32, C.c_uint64, C.POINTER(vp)]
+    L.cfrb_match_lbr_trace.argtypes = [vp, C.c_int32, _dp, _dp]
+    L.cfrb_match_lbr_counts.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     _lib = L
     return L
 
@@ -383,3 +386,29 @@ class Match:
         n = _check(lib().cfrb_match_trace(self._m, game, _p(rec, _ip), _p(prob, _dp), _p(act, _ip), _p(bel, _dp), C.byref(nr)))
         r = nr.value
         return {"plies": rec[:n], "prob": prob[:n], "act_iteration": act[:r], "root_beliefs": bel[:r]}
+
+
+class LbrMatch(Match):
+    """Local best response against the agent of one WaveSolver (cfrb_match_create_lbr): n_games games, n_slots at a time, at
+    most the solver's max_subgames subgames per round.  results()["payoff_a"] is the agent's payoff; in trace() agent 1 is LBR."""
+
+    def __init__(self, agent, n_slots, n_games, seed=0):
+        self.a, self.b, self.G = agent, None, n_games
+        self._m = C.c_void_p()
+        _check(lib().cfrb_match_create_lbr(agent._h, n_slots, n_games, seed, C.byref(self._m)))
+
+    def results(self):
+        r = super().results()
+        w, d = C.c_int64(0), C.c_int64(0)
+        _check(lib().cfrb_match_lbr_counts(self._m, C.byref(w), C.byref(d)))
+        r["whatif_solves"], r["deferred_slot_rounds"] = w.value, d.value
+        return r
+
+    def lbr_trace(self, game):
+        """dict: values [P, A] (value of each of LBR's actions at ply i, NaN where illegal or on the agent's plies), beliefs [P, H]
+        (LBR's belief over the agent's hand before the decision)."""
+        A, H = self.a.A, self.a.H
+        val = np.zeros((A, A), np.float64)
+        bel = np.zeros((A, H), np.float64)
+        n = _check(lib().cfrb_match_lbr_trace(self._m, game, _p(val, _dp), _p(bel, _dp)))
+        return {"values": val[:n], "beliefs": bel[:n]}

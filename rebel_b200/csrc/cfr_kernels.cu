@@ -8,6 +8,7 @@
 #include "ev_regret_kernels.cuh"
 #include "selfplay_kernels.cuh"
 #include "match_kernels.cuh"
+#include "lbr_kernels.cuh"
 #include "cfr_d2v2.cuh"
 
 namespace cfrb {
@@ -120,6 +121,15 @@ template <typename real>
 void match_launch_advance(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
   match_advance_kernel<real><<<(p.S + 127) / 128, 128, 0, st>>>(p, t);
 }
+template <typename real>
+void lbr_launch_begin(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st) {
+  lbr_scan_kernel<<<1, 1024, 0, st>>>(p);
+  lbr_begin_kernel<real><<<(p.m.S + 127) / 128, 128, 0, st>>>(p, t);
+}
+template <typename real>
+void lbr_launch_advance(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st) {
+  lbr_advance_kernel<real><<<(p.m.S + 127) / 128, 128, 0, st>>>(p, t);
+}
 __global__ void rows_gather_kernel(const float* __restrict__ src, int width, const int* __restrict__ ids, int n, float* __restrict__ out) {
   const size_t total = (size_t)n * width;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -199,7 +209,9 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void sp_launch_begin<real>(const SpDev&, real*, cudaStream_t);                                                  \
   template void sp_launch_finish<real>(const SpDev&, const real*, const real*, float*, float*, cudaStream_t);              \
   template void match_launch_begin<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                           \
-  template void match_launch_advance<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);
+  template void match_launch_advance<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                         \
+  template void lbr_launch_begin<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                               \
+  template void lbr_launch_advance<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);
 CFRB_INSTANTIATE(float)
 CFRB_INSTANTIATE(double)
 

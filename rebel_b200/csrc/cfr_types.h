@@ -155,6 +155,22 @@ void match_launch_deal(const MatchDev& p, cudaStream_t st);
 // scan + subgame descriptors of the next round
 template <typename real> void match_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st);
 template <typename real> void match_launch_advance(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st);
+// Local best response against one agent (lbr_kernels.cuh): the match's slots and games with handle 0 as the agent; index 1 of
+// m's per-agent arrays is unused.  m.bel holds per slot the agent's beliefs [player][hand] (rows 0, 1) and LBR's belief over the
+// agent's hand (row 2).
+struct LbrDev {
+  MatchDev m;
+  int K;                              // subgames per round (the agent's max_subgames)
+  int* nsg;                           // [S] subgames the slot holds in this round's wave (0 = waiting or done)
+  int* pend;                          // [S] 1: LBR's decision at (last_bid, player) waits for the solves of its raises' children
+  double* sigx;                       // [S][A][H] the agent's strategy for LBR's seat at that node, per raise
+  int* rr;                            // [1] rotated slot position where the next round's admission starts
+  unsigned long long* deferred;       // [1] running slots left out of a round, summed over rounds
+  int* solves; int* whatif;           // [G] subgames solved for game g, and how many of them were what-if solves
+  double* tr_val; double* tr_beta;    // [T][A][A] LBR's action values (NaN = illegal / not LBR's ply), [T][A][H] its belief
+};
+template <typename real> void lbr_launch_begin(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st);
+template <typename real> void lbr_launch_advance(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st);
 // rows [ids[i]] of a [*, width] fp32 matrix -> out[i]  (replay sampling)
 void rows_launch_gather(const float* src, int width, const int* ids, int n, float* out, cudaStream_t st);
 

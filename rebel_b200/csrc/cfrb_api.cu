@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <array>
 #include <cstring>
+#include <limits>
 #include <string>
 #include <vector>
 
@@ -1635,11 +1636,18 @@ struct cfrb_match {
   int* pin_left = nullptr;            // slots with a game left, copied behind the last round of every cfrb_match_run
   cudaEvent_t ev_left = nullptr;
   bool ev_recorded = false;
+  // local best response (cfrb_match_create_lbr): h[1] is null, agent 1 is LBR
+  bool lbr = false;
+  cfrb::LbrDev ldev{};
+  DevBuf<int> nsg, pend, rr, solves_g, whatif_g;
+  DevBuf<double> sigx, tr_val, tr_beta;
+  DevBuf<unsigned long long> deferred;
   void release() {
     for (auto* b : {&game, &last_bid, &player, &hands, &ply, &round, &widx, &act, &mt_idx, &running, &left, &plies, &rounds, &tr_ply,
-                    &tr_plies, &tr_act, &tr_rounds})
+                    &tr_plies, &tr_act, &tr_rounds, &nsg, &pend, &rr, &solves_g, &whatif_g})
       b->release();
     bel.release(); tr_prob.release(); tr_bel.release(); payoff.release(); mt.release();
+    sigx.release(); tr_val.release(); tr_beta.release(); deferred.release();
     if (pin_left) cudaFreeHost(pin_left);
     if (ev_left) cudaEventDestroy(ev_left);
     pin_left = nullptr; ev_left = nullptr;
@@ -1672,11 +1680,37 @@ static int match_advance_t(cfrb_match* m, cudaStream_t st) {
   return CFRB_OK;
 }
 
+// LBR matches: the agent's table is read as in an AVERAGE match (normalise(S) for CFR, Sg for FP).
+template <typename real>
+static cfrb::MatchTabs<real> lbr_tabs(cfrb_match* m) {
+  cfrb::MatchTabs<real> t{};
+  cfrb_handle* h = m->h[0];
+  auto& s = state_of<real>(h);
+  const bool fp = h->cfg.solver == CFRB_SOLVER_FP;
+  t.wave_beliefs[0] = s.beliefs.p;
+  t.table[0] = fp ? s.Sg.p : s.S.p;
+  t.normalise[0] = !fp;
+  return t;
+}
+template <typename real>
+static int lbr_begin_t(cfrb_match* m, cudaStream_t st) {
+  cfrb::lbr_launch_begin<real>(m->ldev, lbr_tabs<real>(m), st);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+template <typename real>
+static int lbr_advance_t(cfrb_match* m, cudaStream_t st) {
+  cfrb::lbr_launch_advance<real>(m->ldev, lbr_tabs<real>(m), st);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+
 // Everything enqueued has finished: each handle's current wave becomes the match's last wave (its size lives on the device).
 static int match_settle(cfrb_match* m) {
   CK(cudaSetDevice(m->h[0]->cfg.device));
   CK(cudaDeviceSynchronize());
   for (cfrb_handle* h : m->h) {
+    if (!h) continue;
     int wave[2] = {0, 0};
     CK(cudaMemcpy(wave, h->d_wave.p, sizeof(wave), cudaMemcpyDeviceToHost));
     h->n = wave[0];
@@ -1692,12 +1726,15 @@ int cfrb_match_destroy(cfrb_match* m) {
   int rc = CFRB_OK;
   if (m->h[0]) {
     rc = match_settle(m);
-    for (cfrb_handle* h : m->h) h->in_match = false;
+    for (cfrb_handle* h : m->h)
+      if (h) h->in_match = false;
   }
   m->release();
   delete m;
   return rc;
 }
+
+static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed);
 
 static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed,
                              int32_t policy) {
@@ -1722,6 +1759,28 @@ static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int3
     if (h->sp.ready) return fail(CFRB_EINVAL, "cfrb_match_create: a handle has a live self-play session");
     if (h->in_match) return fail(CFRB_EINVAL, "cfrb_match_create: a handle already plays in a live match");
   }
+  int rc = match_alloc(m, a, n_slots, n_games, seed);
+  if (rc) return rc;
+  cfrb::MatchDev& d = m->dev;
+  d.sampled = policy == CFRB_MATCH_SAMPLED;
+  d.iters[0] = ca.num_iters; d.iters[1] = cb.num_iters;
+  cfrb_handle* hs[2] = {a, b};
+  for (int k = 0; k < 2; ++k) {
+    cfrb_handle* h = hs[k];
+    d.wave[k] = h->d_wave.p; d.sg_tmpl[k] = h->d_sg_tmpl.p; d.sg_player[k] = h->d_sg_player.p; d.sg_row_off[k] = h->d_sg_row_off.p;
+    d.sg_act[k] = h->d_sg_act.p; d.steps[k] = h->d_steps.p;
+  }
+  cfrb::match_launch_deal(d, a->own_stream);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(a->own_stream));
+  m->h[0] = a; m->h[1] = b;
+  a->in_match = b->in_match = true;
+  return CFRB_OK;
+}
+
+// Slots, games, streams and trace buffers of a match played with agent a's game (the part shared by both kinds of match).
+static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed) {
+  const auto& ca = a->cfg;
   CK(cudaSetDevice(ca.device));
   CK(cudaDeviceSynchronize());
   const int S = n_slots, G = n_games, H = a->g.H, A = a->g.A, T = std::min(G, (int)CFRB_MATCH_TRACE_GAMES);
@@ -1741,8 +1800,7 @@ static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int3
   CK(cudaMallocHost((void**)&m->pin_left, sizeof(int)));
   CK(cudaEventCreateWithFlags(&m->ev_left, cudaEventDisableTiming));
   cfrb::MatchDev& d = m->dev;
-  d.S = S; d.G = G; d.A = A; d.H = H; d.F = a->g.F; d.max_depth = ca.max_depth; d.sampled = policy == CFRB_MATCH_SAMPLED;
-  d.iters[0] = ca.num_iters; d.iters[1] = cb.num_iters; d.seed = seed;
+  d.S = S; d.G = G; d.A = A; d.H = H; d.F = a->g.F; d.max_depth = ca.max_depth; d.seed = seed;
   d.game = m->game.p; d.last_bid = m->last_bid.p; d.player = m->player.p; d.hands = m->hands.p; d.ply = m->ply.p; d.round = m->round.p;
   d.widx = m->widx.p; d.act = m->act.p; d.bel = m->bel.p; d.mt = m->mt.p; d.mt_idx = m->mt_idx.p; d.running = m->running.p;
   d.left = m->left.p;
@@ -1751,17 +1809,6 @@ static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int3
   d.tr_bel = m->tr_bel.p; d.tr_rounds = m->tr_rounds.p;
   d.tmpl = a->d_tmpl.p; d.child_begin = a->d_child_begin.p; d.nchild = a->d_nchild.p; d.matches = a->d_matches.p;
   d.table_stride = a->table_stride;
-  cfrb_handle* hs[2] = {a, b};
-  for (int k = 0; k < 2; ++k) {
-    cfrb_handle* h = hs[k];
-    d.wave[k] = h->d_wave.p; d.sg_tmpl[k] = h->d_sg_tmpl.p; d.sg_player[k] = h->d_sg_player.p; d.sg_row_off[k] = h->d_sg_row_off.p;
-    d.sg_act[k] = h->d_sg_act.p; d.steps[k] = h->d_steps.p;
-  }
-  cfrb::match_launch_deal(d, a->own_stream);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(a->own_stream));
-  m->h[0] = a; m->h[1] = b;
-  a->in_match = b->in_match = true;
   return CFRB_OK;
 }
 
@@ -1779,6 +1826,96 @@ int cfrb_match_create(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n
   return CFRB_OK;
 }
 
+static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed) {
+  if (!a) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: null handle");
+  if (n_slots < 1) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: n_slots must be >= 1");
+  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: n_games must be even and >= 2 (seat-swapped pairs)");
+  if (a->sp.ready) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: the handle has a live self-play session");
+  if (a->in_match) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: the handle already plays in a live match");
+  const int A = a->g.A;
+  if (a->cfg.max_subgames < A - 1)
+    return fail(CFRB_EINVAL, "cfrb_match_create_lbr: the handle's capacity (max_subgames " + std::to_string(a->cfg.max_subgames) +
+                                 ") must hold the A - 1 = " + std::to_string(A - 1) + " what-if subgames of one LBR decision");
+  int rc = match_alloc(m, a, n_slots, n_games, seed);
+  if (rc) return rc;
+  const int S = n_slots, G = n_games, H = a->g.H, T = m->T;
+  cfrb::MatchDev& d = m->dev;
+  d.sampled = 0;
+  d.iters[0] = a->cfg.num_iters;
+  d.wave[0] = a->d_wave.p; d.sg_tmpl[0] = a->d_sg_tmpl.p; d.sg_player[0] = a->d_sg_player.p; d.sg_row_off[0] = a->d_sg_row_off.p;
+  d.sg_act[0] = a->d_sg_act.p; d.steps[0] = a->d_steps.p;
+  CK(m->nsg.alloc(S)); CK(m->pend.alloc(S)); CK(m->rr.alloc(1)); CK(m->deferred.alloc(1));
+  CK(m->solves_g.alloc(G)); CK(m->whatif_g.alloc(G));
+  CK(m->sigx.alloc((size_t)S * A * H));
+  CK(m->tr_val.alloc((size_t)T * A * A)); CK(m->tr_beta.alloc((size_t)T * A * H));
+  CK(cudaMemset(m->pend.p, 0, (size_t)S * sizeof(int)));
+  CK(cudaMemset(m->nsg.p, 0, (size_t)S * sizeof(int)));
+  CK(cudaMemset(m->rr.p, 0, sizeof(int)));
+  CK(cudaMemset(m->deferred.p, 0, sizeof(unsigned long long)));
+  CK(cudaMemset(m->solves_g.p, 0, (size_t)G * sizeof(int)));
+  CK(cudaMemset(m->whatif_g.p, 0, (size_t)G * sizeof(int)));
+  CK(cudaMemset(m->tr_bel.p, 0, (size_t)T * A * 4 * H * sizeof(double)));   // LBR's root beliefs stay zero
+  CK(cudaMemset(m->tr_beta.p, 0, (size_t)T * A * H * sizeof(double)));
+  const std::vector<double> nan((size_t)T * A * A, std::numeric_limits<double>::quiet_NaN());
+  CK(cudaMemcpy(m->tr_val.p, nan.data(), nan.size() * sizeof(double), cudaMemcpyHostToDevice));
+  cfrb::LbrDev& l = m->ldev;
+  l.K = a->cfg.max_subgames;
+  l.nsg = m->nsg.p; l.pend = m->pend.p; l.sigx = m->sigx.p; l.rr = m->rr.p; l.deferred = m->deferred.p;
+  l.solves = m->solves_g.p; l.whatif = m->whatif_g.p; l.tr_val = m->tr_val.p; l.tr_beta = m->tr_beta.p;
+  cfrb::match_launch_deal(d, a->own_stream);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(a->own_stream));
+  l.m = d;
+  m->lbr = true;
+  m->h[0] = a;
+  a->in_match = true;
+  return CFRB_OK;
+}
+
+int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out) {
+  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: null argument");
+  *out = nullptr;
+  cfrb_match* m = new cfrb_match();
+  const int rc = lbr_create_impl(m, agent, n_slots, n_games, seed);
+  if (rc != CFRB_OK) {
+    m->release();
+    delete m;
+    return rc;
+  }
+  *out = m;
+  return CFRB_OK;
+}
+
+int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* beliefs) {
+  if (!m || !m->lbr) return fail(CFRB_EINVAL, "cfrb_match_lbr_trace: not an LBR match");
+  if (game < 0 || game >= m->T) return fail(CFRB_EINVAL, "cfrb_match_lbr_trace: only games < min(n_games, CFRB_MATCH_TRACE_GAMES) are traced");
+  int rc = match_settle(m);
+  if (rc) return rc;
+  const size_t A = m->dev.A, H = m->dev.H;
+  int np = 0;
+  CK(cudaMemcpy(&np, m->tr_plies.p + game, sizeof(int), cudaMemcpyDeviceToHost));
+  if (values) CK(cudaMemcpy(values, m->tr_val.p + game * A * A, A * A * sizeof(double), cudaMemcpyDeviceToHost));
+  if (beliefs) CK(cudaMemcpy(beliefs, m->tr_beta.p + game * A * H, A * H * sizeof(double), cudaMemcpyDeviceToHost));
+  return np;
+}
+
+int cfrb_match_lbr_counts(cfrb_match* m, int64_t* whatif_solves, int64_t* deferred_slot_rounds) {
+  if (!m || !m->lbr) return fail(CFRB_EINVAL, "cfrb_match_lbr_counts: not an LBR match");
+  int rc = match_settle(m);
+  if (rc) return rc;
+  std::vector<int> w(m->G);
+  CK(cudaMemcpy(w.data(), m->whatif_g.p, (size_t)m->G * sizeof(int), cudaMemcpyDeviceToHost));
+  unsigned long long dr = 0;
+  CK(cudaMemcpy(&dr, m->deferred.p, sizeof(dr), cudaMemcpyDeviceToHost));
+  if (whatif_solves) {
+    int64_t s = 0;
+    for (int x : w) s += x;
+    *whatif_solves = s;
+  }
+  if (deferred_slot_rounds) *deferred_slot_rounds = (int64_t)dr;
+  return CFRB_OK;
+}
+
 int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
   if (!m || max_rounds < 1) return fail(CFRB_EINVAL, "cfrb_match_run: bad argument");
   CK(cudaSetDevice(m->h[0]->cfg.device));
@@ -1787,6 +1924,23 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
     if (*m->pin_left == 0) return 0;
   }
   cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->h[0]->own_stream;
+  if (m->lbr) {                       // one wave of at most max_subgames subgames of the agent, then the walk
+    cfrb_handle* h = m->h[0];
+    for (int r = 0; r < max_rounds; ++r) {
+      int rc = DISPATCH_REAL(h, lbr_begin_t, m, st);
+      if (rc) return rc;
+      h->n = h->cfg.max_subgames; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
+      if ((rc = DISPATCH_REAL(h, launch_init_t, h, st))) return rc;
+      if ((rc = cfrb_run(h, h->cfg.num_iters, st))) return rc;
+      CK(cudaMemsetAsync(m->left.p, 0, sizeof(int), st));
+      if ((rc = DISPATCH_REAL(h, lbr_advance_t, m, st))) return rc;
+      h->launches += 3;
+    }
+    CK(cudaMemcpyAsync(m->pin_left, m->left.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(m->ev_left, st));
+    m->ev_recorded = true;
+    return max_rounds;
+  }
   for (int r = 0; r < max_rounds; ++r) {
     int rc = DISPATCH_REAL(m->h[0], match_begin_t, m, st);
     if (rc) return rc;
@@ -1811,11 +1965,16 @@ int cfrb_match_results(cfrb_match* m, float* payoff_a, int32_t* plies, int64_t* 
   if (rc) return rc;
   const int G = m->G;
   std::vector<int> rounds(G);
-  CK(cudaMemcpy(rounds.data(), m->rounds.p, (size_t)G * sizeof(int), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(rounds.data(), m->lbr ? m->solves_g.p : m->rounds.p, (size_t)G * sizeof(int), cudaMemcpyDeviceToHost));
   if (payoff_a) CK(cudaMemcpy(payoff_a, m->payoff.p, (size_t)G * sizeof(float), cudaMemcpyDeviceToHost));
   if (plies) CK(cudaMemcpy(plies, m->plies.p, (size_t)G * sizeof(int), cudaMemcpyDeviceToHost));
   int64_t r = 0;
   for (int x : rounds) r += x;
+  if (m->lbr) {                       // every subgame the agent solved, the what-if ones included
+    if (solves) *solves = r;
+    if (subgame_iters) *subgame_iters = r * (int64_t)m->dev.iters[0];
+    return CFRB_OK;
+  }
   if (solves) *solves = 2 * r;
   if (subgame_iters) *subgame_iters = r * ((int64_t)m->dev.iters[0] + m->dev.iters[1]);
   return CFRB_OK;

@@ -2,6 +2,7 @@
 // value net; both re-solve subgames only along the path actually played, so the cost per game does not depend on the size of
 // the game tree and games the full-tree evaluators refuse (2x5f, 2x6f, 1x17f, ...) can be evaluated.
 #pragma once
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdint>
@@ -80,6 +81,60 @@ inline MatchResult play_match(const liars_dice::RecursiveSolvingParams& cfg_a, c
   r.payoff.resize(games);
   r.plies.resize(games);
   check(cfrb_match_results(m, r.payoff.data(), r.plies.data(), &r.solves, &r.subgame_iters), "cfrb_match_results");
+  r.seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  cleanup();
+  return r;
+}
+
+struct LbrResult : MatchResult {
+  int64_t whatif_solves = 0, deferred_slot_rounds = 0;
+  int capacity = 0;
+};
+
+// Default subgames per round of a local-best-response run: two per slot (a slot asks for one subgame at a game start or a
+// pseudo-leaf and for one per legal raise at an LBR decision on the edge of the agent's subgame), at least A - 1.
+inline int lbr_default_capacity(int slots, int num_actions) { return std::max(2 * slots, num_actions - 1); }
+
+// Local best response against one agent (cfrb_match_create_lbr): `games` games, `slots` at a time; payoff[] is the agent's.
+// max_subgames = 0 takes lbr_default_capacity.
+inline LbrResult play_lbr(const liars_dice::RecursiveSolvingParams& cfg, int device, int games, uint64_t seed, const std::vector<float>& w,
+                          int slots, int max_subgames) {
+  if (games < 2) throw std::runtime_error("play_lbr: games must be >= 2");
+  slots = std::max(1, std::min(slots, games));
+  cfrb_handle* h = nullptr;
+  cfrb_match* m = nullptr;
+  auto cleanup = [&]() {
+    if (m) cfrb_match_destroy(m);
+    if (h) cfrb_destroy(h);
+  };
+  auto check = [&](int rc, const char* what) {
+    if (rc < 0) {
+      const std::string err = std::string(what) + ": " + cfrb_last_error();
+      cleanup();
+      throw std::runtime_error(err);
+    }
+    return rc;
+  };
+  LbrResult r;
+  if (max_subgames <= 0) {                           // the game's number of actions, from a one-subgame handle
+    const cfrb_config c1 = liars_dice::solver_config(cfg, device, 1);
+    check(cfrb_create(&c1, &h), "cfrb_create");
+    max_subgames = lbr_default_capacity(slots, cfrb_num_actions(h));
+    cfrb_destroy(h);
+    h = nullptr;
+  }
+  r.capacity = max_subgames;
+  const cfrb_config c = liars_dice::solver_config(cfg, device, max_subgames);
+  check(cfrb_create(&c, &h), "cfrb_create");
+  if (!w.empty()) check(cfrb_set_weights(h, w.data(), w.size(), 1), "cfrb_set_weights");
+  check(cfrb_match_create_lbr(h, slots, games, seed, &m), "cfrb_match_create_lbr");
+  const auto t0 = std::chrono::steady_clock::now();
+  while (check(cfrb_match_run(m, 8, nullptr), "cfrb_match_run") > 0) {
+  }
+  r.payoff.resize(games);
+  r.plies.resize(games);
+  check(cfrb_match_results(m, r.payoff.data(), r.plies.data(), &r.solves, &r.subgame_iters), "cfrb_match_results");
+  check(cfrb_match_lbr_counts(m, &r.whatif_solves, &r.deferred_slot_rounds), "cfrb_match_lbr_counts");
   r.seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   cleanup();
   return r;

@@ -561,6 +561,30 @@ py::dict play_match_py(const RecursiveSolvingParams& cfg_a, const RecursiveSolvi
   return d;
 }
 
+py::dict play_lbr_py(const RecursiveSolvingParams& cfg, int device, int games, uint64_t seed, py::object flat_weights, int concurrent_games,
+                     int max_subgames) {
+  const std::vector<float> w = flat_of(flat_weights);
+  LbrResult r;
+  {
+    py::gil_scoped_release nogil;
+    r = play_lbr(cfg, device, games, seed, w, concurrent_games, max_subgames);
+  }
+  std::vector<float> lbr(r.payoff.size());
+  for (size_t i = 0; i < lbr.size(); ++i) lbr[i] = -r.payoff[i];
+  const MatchStats s = match_stats(lbr);
+  py::dict d;
+  d["mean"] = s.mean; d["stderr"] = s.stderr_;
+  d["seat_means"] = std::vector<double>{s.seat[1], s.seat[0]};   // LBR sits in seat 1 in even games, in seat 0 in odd ones
+  auto p = torch::empty({(int64_t)games}, torch::kFloat32);
+  std::copy(lbr.begin(), lbr.end(), p.data_ptr<float>());
+  auto pl = torch::empty({(int64_t)games}, torch::kInt32);
+  std::copy(r.plies.begin(), r.plies.end(), pl.data_ptr<int32_t>());
+  d["payoff_lbr"] = p; d["plies"] = pl; d["solves"] = r.solves; d["whatif_solves"] = r.whatif_solves;
+  d["deferred_slot_rounds"] = r.deferred_slot_rounds; d["max_subgames"] = r.capacity;
+  d["subgame_iters"] = r.subgame_iters; d["seconds"] = r.seconds;
+  return d;
+}
+
 py::dict match_stats_py(torch::Tensor payoff) {
   auto t = payoff.to(torch::kCPU, torch::kFloat32).contiguous();
   return stats_dict(std::vector<float>(t.data_ptr<float>(), t.data_ptr<float>() + t.numel()));
@@ -704,6 +728,13 @@ PYBIND11_MODULE(rela, m) {
         "each re-solving subgames along the path played with its recursive to-leaf policy ('average' or 'sampled').  dict: payoff_a "
         "[games] (to A), plies [games], mean, stderr (over pairs), seat_means [2] (A in seat 0 / seat 1), solves, subgame_iters, "
         "seconds.");
+  m.def("play_lbr", &play_lbr_py, py::arg("cfg"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
+        py::arg("flat_weights") = py::none(), py::arg("concurrent_games") = 8192, py::arg("max_subgames") = 0,
+        "rebel_b200 extension: local best response against one agent (cfg + net, average policy) on the GPU: `games` games "
+        "(seat-swapped pairs), concurrent_games at a time, at most max_subgames subgames solved per round (0: 2 x "
+        "concurrent_games, at least A - 1).  LBR's payoff is a lower bound on the agent's exploitability.  dict: payoff_lbr "
+        "[games], plies [games], mean, stderr (over pairs), seat_means [2] (LBR in seat 0 / seat 1), solves, whatif_solves, "
+        "deferred_slot_rounds, max_subgames, subgame_iters, seconds.");
   m.def("match_stats", &match_stats_py, py::arg("payoff_a"),
         "rebel_b200 extension: play_match's mean, stderr (over the pairs 2i, 2i+1) and seat_means of a payoff vector.");
   m.def("strategy_recursive_to_leaf", &strategy_recursive_to_leaf, py::arg("cfg"), py::arg("device") = 0,
