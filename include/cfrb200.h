@@ -261,7 +261,7 @@ int cfrb_selfplay_wait_examples(cfrb_handle* h);
 /* Game states (public state and beliefs [n][2][H]) copied to the host; any pointer may be NULL.  Synchronises.  Returns n_games. */
 int cfrb_selfplay_state(cfrb_handle* h, int32_t* last_bid, int32_t* player, double* beliefs);
 /* Test aid: the division-free quotient of the regret-matching step (reciprocal of the node's sum + two fused multiply-add
- * corrections, csrc/cfr_d2v2.cuh) against IEEE division on blocks x 256 x 4096 pseudo-random operand pairs. */
+ * corrections, csrc/cfr_kernels.cuh) against IEEE division on blocks x 256 x 4096 pseudo-random operand pairs. */
 int cfrb_debug_div_check(cfrb_handle* h, uint64_t seed, int32_t blocks, uint64_t* mismatches);
 /* Test aid: the packed-half GELU of the value-net epilogue on every fp16 input: out[i] = fp16 bits of f(fp16 with bit pattern i), i < 65536;
  * what 0 = tanh.approx.f16x2, 1 / 2 = GELU(2 x) computed from x = y / 2 the way the packed-half / fp32-tanh epilogue does (tests pin the arithmetic model of

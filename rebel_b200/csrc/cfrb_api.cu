@@ -106,8 +106,7 @@ struct cfrb_handle {
   int d2_groups_per_cta = 8;
   int d2_scratch_per_group = 0;
   size_t d2_smem = 0;      // dynamic shared memory of a depth-2 CTA
-  bool d2v2 = false;       // cfr_iter_d2v2_kernel (CFR solver, depth <= 2): one warp per CTA, inputs staged by cp.async.bulk
-  int d2v2_smem = 0, n1max = 0, d2v2_threads = 32;
+  int n1max = 0;           // bound on the level-1 nodes of a template (the depth-2 scratch layout)
   int table_stride = 0;
   int num_sms = 0;
   cudaStream_t own_stream = nullptr;
@@ -209,7 +208,7 @@ static int alloc_state(cfrb_handle* h, int max_optin) {
   const size_t rows_cap = (size_t)K * std::max(h->Lmax, 1);
   CK(s.beliefs.alloc((size_t)K * 2 * g.H)); CK(s.mu.alloc((size_t)K * 2 * g.H));
   CK(s.R.alloc(tab)); CK(s.Sg.alloc(tab)); CK(s.S.alloc(tab)); CK(s.Snap.alloc(tab));
-  const int vterm_stride = round_up(std::max(h->Tmax, 1) * g.H, 4);     // 16-byte aligned rows for the bulk copies
+  const int vterm_stride = round_up(std::max(h->Tmax, 1) * g.H, 4);     // 16-byte aligned rows
   CK(s.vterm.alloc((size_t)K * vterm_stride + 8)); CK(s.scaler.alloc(rows_cap + 8));
   CK(cudaMemset(s.vterm.p, 0, ((size_t)K * vterm_stride + 8) * sizeof(real)));
   CK(cudaMemset(s.scaler.p, 0, (rows_cap + 8) * sizeof(real)));
@@ -223,8 +222,7 @@ static int alloc_state(cfrb_handle* h, int max_optin) {
     h->groups_per_cta = (int)std::max<size_t>(1, std::min<size_t>(16, budget / per_group_bytes));
     const int smem_bytes = (int)(per_group_bytes * h->groups_per_cta);
     CK(cfrb::cfr_configure<real>(32, smem_bytes));
-    const char* no_d2 = std::getenv("CFRB_NO_D2");
-    if (h->max_levels <= 3 && h->tpk_stride > 0 && !(no_d2 && *no_d2 == '1')) {
+    if (h->max_levels <= 3 && h->tpk_stride > 0) {
       // 32 warps per SM (register file: 64 registers x 32 warps) as 8 CTAs of 4 warps: small CTAs even out the last round
       // (8192 subgames on the 4224 warp slots of a 132-SM H100 = 1.94 rounds); each CTA has 1 KB of shared memory reserved by the runtime
       h->d2 = true;
@@ -232,21 +230,8 @@ static int alloc_state(cfrb_handle* h, int max_optin) {
       const size_t d2_bytes = (size_t)h->d2_scratch_per_group * sizeof(real) + h->tpk_stride;
       const size_t cta_budget = ((size_t)228 * 1024 - 8 * 1024) / 8;
       h->d2_groups_per_cta = (int)std::max<size_t>(1, std::min<size_t>(4, cta_budget / d2_bytes));
-      if (const char* e = std::getenv("CFRB_D2_GROUPS")) h->d2_groups_per_cta = std::max(1, std::min(h->d2_groups_per_cta, std::atoi(e)));
       h->d2_smem = d2_bytes * h->d2_groups_per_cta;
-      // CFRB_D2_CTAS_PER_SM=n: pad the CTA's shared memory so that exactly n CTAs fit an SM (resident warps = n x warps per CTA);
-      // e.g. 7 x 4 = 28 warps per SM
-      if (const char* e = std::getenv("CFRB_D2_CTAS_PER_SM")) {
-        const int n = std::atoi(e);
-        if (n >= 1 && n <= 8) h->d2_smem = std::max(h->d2_smem, ((size_t)227 * 1024 - (size_t)n * 1024) / n / 16 * 16);
-      }
       CK(cfrb::cfr_configure_d2<real>((int)h->d2_smem));
-      const char* gen = std::getenv("CFRB_D2_GEN");
-      h->d2v2_smem = cfrb::cfr_d2v2_smem_bytes<real>(h->Nmax, g.H, h->Hout, std::max(h->Lmax, 1), std::max(h->Tmax, 1), h->n1max, h->table_stride);
-      // generation 2 (cfr_d2v2.cuh) is opt-in (CFRB_D2_GEN=2): measured slower than the 32-warps-per-SM kernel (see DESIGN.md)
-      h->d2v2 = h->cfg.solver == CFRB_SOLVER_CFR && h->cfg.max_depth == 2 && gen && *gen == '2' && h->d2v2_smem <= max_optin;
-      if (h->d2v2) CK(cfrb::cfr_configure_d2v2<real>(h->d2v2_smem));
-      if (const char* e = std::getenv("CFRB_D2V2_THREADS")) { const int v = std::atoi(e); if (v == 32 || v == 64 || v == 128) h->d2v2_threads = v; }
     }
   } else {
     h->group = 256;
@@ -291,9 +276,7 @@ template <typename real>
 static int launch_iter_t(cfrb_handle* h, cudaStream_t st, int iter, int do_b, int do_f) {
   auto& s = state_of<real>(h);
   const int nsg = h->capturing ? h->cfg.max_subgames : h->n;   // surplus groups return at once (k >= *wave_n)
-  if (h->d2 && h->d2v2) {
-    cfrb::cfr_launch_iter_d2v2<real>(s.dev, nsg, h->d2v2_threads, (size_t)h->d2v2_smem, st, iter, do_b, do_f, h->n1max);
-  } else if (h->d2) {
+  if (h->d2) {
     const int blocks = (nsg + h->d2_groups_per_cta - 1) / h->d2_groups_per_cta;
     const size_t smem = h->d2_smem;
     cfrb::cfr_launch_iter_d2<real>(s.dev, blocks, 32 * h->d2_groups_per_cta, smem, st, iter, do_b, do_f, h->d2_scratch_per_group);
@@ -659,7 +642,7 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   const int K = cfg->max_subgames;
   h->Qpad = round_up(g.Q + 1, 16);   // one spare column carries the constant 1 that feeds bias 1 through the tensor cores
   h->Hout = round_up(g.H, 4);                                     // value-net output rows padded to 16 bytes
-  h->table_stride = round_up(std::max(1, (h->Nmax - 1) * g.H), 4);   // every subgame's tables start 16-byte aligned (bulk copies)
+  h->table_stride = round_up(std::max(1, (h->Nmax - 1) * g.H), 4);   // every subgame's tables start 16-byte aligned
   h->n1max = g.A;
   h->scratch_per_group = cfrb::cfr_scratch_reals(h->Nmax, g.H, h->Lmax, h->Tmax);
   int max_optin = 0;
@@ -1563,8 +1546,9 @@ int cfrb_wave_roots(cfrb_handle* h, int32_t* last_bid, int32_t* player_id, int32
   return h->n;
 }
 
-// Development / test aid: div_by_rcp (reciprocal + two fused-multiply-add corrections, cfr_d2v2.cuh) against IEEE division on
-// `blocks` x 256 x 4096 pseudo-random operand pairs; *mismatches receives the number of differing quotients.
+// Development / test aid: div_by_rcp (reciprocal + two fused-multiply-add corrections, cfr_kernels.cuh; the regret matching of
+// cfr_iter_d2_kernel) against IEEE division on `blocks` x 256 x 4096 pseudo-random operand pairs; *mismatches receives the number
+// of differing quotients.
 int cfrb_debug_div_check(cfrb_handle* h, uint64_t seed, int32_t blocks, uint64_t* mismatches) {
   if (!h || !mismatches || blocks < 1) return fail(CFRB_EINVAL, "bad argument");
   CK(cudaSetDevice(h->cfg.device));

@@ -538,7 +538,7 @@ def test_snapshot_of_act_iteration_zero_needs_no_run(rb, port):
 
 
 def test_fast_division_is_correctly_rounded(rb):
-    """cfr_iter_d2v2_kernel obtains sigma = max(R, eps) / sum from the reciprocal of the sum (one true division per (node, hand))
+    """cfr_iter_d2_kernel obtains sigma = max(R, eps) / sum from the reciprocal of the sum (one true division per (node, hand))
     and two fused multiply-add correction steps instead of one IEEE division per action.  The quotients must be the correctly
     rounded ones — the bits `/` gives — or the solver would leave the reference's trajectory: 4.3e9 pseudo-random operand pairs
     (uniform mantissas, denominators next to 1 and 2, quotients within a few ulp of 1, the 1e-80 scale, small-integer multiples)."""
