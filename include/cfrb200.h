@@ -22,6 +22,8 @@
  *   cfrb_regrets_*                  <-  compute_immediate_regrets      (subgame_solving.cc:984-1050)
  *   cfrb_match_*                    <-  compute_[sampled_]strategy_recursive_to_leaf restricted to the path two agents play
  *                                       (recursive_solving.cc:76-134, 301-327); no counterpart in the reference
+ *   cfrb_agent_*                    <-  the same policies, one agent against external players, one action per call; no
+ *                                       counterpart in the reference
  *
  * Conventions: plain C, no exceptions across the boundary; every function returns 0 on success or a
  * negative CFRB_E* code (cfrb_last_error() gives the message for the calling thread); all buffers are
@@ -337,6 +339,50 @@ int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, 
 int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* beliefs);
 /* Synchronises.  what-if subgames solved, and running slots that waited a round for capacity (summed over rounds). */
 int cfrb_match_lbr_counts(cfrb_match* m, int64_t* whatif_solves, int64_t* deferred_slot_rounds);
+
+/* ---- A ReBeL agent played from outside: one handle's agent at n_tables independent tables, each a game against an external
+ * player (a person, another program's bot, a tournament harness), advanced one action per call.  At every table the agent plays
+ * as in a cfrb_match_* match: compute_strategy_recursive_to_leaf (policy CFRB_MATCH_AVERAGE) or
+ * compute_sampled_strategy_recursive_to_leaf without root_only (CFRB_MATCH_SAMPLED, recursive_solving.cc:76-134, 301-327)
+ * restricted to the path played.  It solves the subgame rooted at the current public node from its own beliefs at the game root
+ * and at every pseudo-leaf of its previous subgame, acts for its hand, and updates both players' beliefs with its own strategy,
+ * whoever acts (unnormalised inside a subgame, normalize_beliefs_inplace at its leaves, :41-44).  An opponent action the agent's
+ * strategy gives probability 0 is applied all the same: it zeroes that row's beliefs and the eps-normalisation at the next
+ * subgame root decides, as in the reference.
+ * Deals and seats belong to the caller: the agent only ever sees its own hand.  The payoff is the caller's business too.
+ * Table t's random draws (act_iteration, the agent's actions) come from mt19937(match_stream_seed(seed, key, 3)) where key is the
+ * game's key, so a game's draws depend only on (seed, key): not on the table, the batch, or the order of the calls.
+ * step / policy solve every listed table that stands at an unsolved subgame root in ONE wave of the handle (its CUDA graph of
+ * num_iters iterations), packed in list order.  Since wave positions change from call to call, each solved subgame's acting
+ * strategy (the normalised average of CFR, the average of FP, or the act_iteration snapshot) is copied into a per-table fp64
+ * cache right after the solve; everything later reads the cache only.
+ * Every call checks the whole batch on the host first and then synchronises; a table's error (id out of range or repeated, a hand
+ * outside [0, H), an action that is not above the last bid or a liar call before any bid, -1 on the opponent's turn, a table with
+ * no running game) returns CFRB_EINVAL with the table id in the message and leaves every table of the call unchanged.
+ * h: max_subgames >= n_tables, no live self-play session or match; while the agent lives the handle serves only it (it counts as
+ * in a live match).  The caller keeps the handle and destroys it after the agent. */
+typedef struct cfrb_agent cfrb_agent;
+int cfrb_agent_create(cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t policy, cfrb_agent** out);
+/* Start (or restart) a game at each listed table: the agent sits in seat seats[i] (0 moves first) with hand hands[i].  keys[i]
+ * keys the game's stream; keys NULL: the number of games this agent had started before, counted in list order. */
+int cfrb_agent_new_games(cfrb_agent* a, int32_t n, const int32_t* ids, const int32_t* seats, const int32_t* hands, const uint64_t* keys);
+/* One action at each listed table.  actions[i] in: the action to apply (normally the opponent's; on the agent's own turn it
+ * overrides the agent's choice, e.g. to replay a logged game), or -1 = the agent draws its action for its hand (its turn only);
+ * out: the action played.  probs [n][A] (may be NULL): on the agent's turns its probability row for its hand (0 on illegal
+ * actions), NaN on the opponent's.  done[i] = 1 when the action was the liar call (the table's game is over). */
+int cfrb_agent_step(cfrb_agent* a, int32_t n, const int32_t* ids, int32_t* actions, double* probs, int32_t* done);
+/* The agent's strategy for the player to move at each listed table, out [n][H][A] (0 on illegal actions). */
+int cfrb_agent_policy(cfrb_agent* a, int32_t n, const int32_t* ids, double* out);
+/* Any pointer may be NULL.  Public node (last bid, player to move, plies so far), subgames solved in the current game, the
+ * act_iteration of the current subgame (-1: AVERAGE), and its root beliefs [n][2][H] (fp64, before the conversion to the state
+ * dtype; at a table that waits for a solve, the beliefs of the subgame it will solve). */
+int cfrb_agent_state(cfrb_agent* a, int32_t n, const int32_t* ids, int32_t* last_bid, int32_t* player, int32_t* ply, int32_t* subgames,
+                     int32_t* act_iteration, double* root_beliefs);
+/* Subgames solved since creation and the iterations run for them. */
+int cfrb_agent_counts(cfrb_agent* a, int64_t* solves, int64_t* subgame_iters);
+/* Device time in ms of the solves (subgame initialisation and iterations, CUDA events) since creation. */
+int cfrb_agent_solve_ms(cfrb_agent* a, double* ms);
+int cfrb_agent_destroy(cfrb_agent* a);
 
 /* ---- Device-resident example rows: storage of the replay buffer (rela/prioritized_replay.h:224-506 keeps one pair of host
  * tensors per example; here the rows of the ring live in HBM as two [capacity][dim] fp32 matrices and never visit the host on

@@ -9,6 +9,7 @@
 #include "selfplay_kernels.cuh"
 #include "match_kernels.cuh"
 #include "lbr_kernels.cuh"
+#include "agent_kernels.cuh"
 
 namespace cfrb {
 
@@ -129,6 +130,20 @@ template <typename real>
 void lbr_launch_advance(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st) {
   lbr_advance_kernel<real><<<(p.m.S + 127) / 128, 128, 0, st>>>(p, t);
 }
+void agent_launch_new(const AgentDev& p, cudaStream_t st) { agent_new_kernel<<<(p.n + 127) / 128, 128, 0, st>>>(p); }
+template <typename real>
+void agent_launch_begin(const AgentDev& p, const MatchTabs<real>& t, cudaStream_t st) {
+  agent_scan_kernel<<<1, 1024, 0, st>>>(p);
+  agent_begin_kernel<real><<<(p.n + 127) / 128, 128, 0, st>>>(p, t);
+}
+template <typename real>
+void agent_launch_capture(const AgentDev& p, const MatchTabs<real>& t, cudaStream_t st) {
+  agent_capture_kernel<real><<<(p.n + 3) / 4, 128, 0, st>>>(p, t);
+}
+void agent_launch_step(const AgentDev& p, cudaStream_t st) { agent_step_kernel<<<(p.n + 127) / 128, 128, 0, st>>>(p); }
+void agent_launch_policy(const AgentDev& p, cudaStream_t st) {
+  agent_policy_kernel<<<(p.n * p.H + 127) / 128, 128, 0, st>>>(p);
+}
 __global__ void rows_gather_kernel(const float* __restrict__ src, int width, const int* __restrict__ ids, int n, float* __restrict__ out) {
   const size_t total = (size_t)n * width;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -180,7 +195,9 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void match_launch_begin<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                           \
   template void match_launch_advance<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                         \
   template void lbr_launch_begin<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                               \
-  template void lbr_launch_advance<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);
+  template void lbr_launch_advance<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                             \
+  template void agent_launch_begin<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);                           \
+  template void agent_launch_capture<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);
 CFRB_INSTANTIATE(float)
 CFRB_INSTANTIATE(double)
 

@@ -171,6 +171,40 @@ struct LbrDev {
 };
 template <typename real> void lbr_launch_begin(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st);
 template <typename real> void lbr_launch_advance(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st);
+// A ReBeL agent played from outside (agent_kernels.cuh): T independent tables, each a game between the agent (one handle) and an
+// external player.  A call lists n distinct tables; the kernels of that call index the per-table state through ids[0..n).
+struct AgentDev {
+  int T, A, H, max_depth, sampled, iters;
+  uint64_t seed;
+  // per table
+  int* seat; int* hand;               // [T] the agent's seat and hand
+  int* last_bid; int* player; int* ply;   // [T] public node
+  int* root_lb; int* root_player;     // [T] root of the current subgame
+  int* node; int* depth;              // [T] node of the subgame template, plies since its root
+  int* act; int* status; int* subgames;   // [T] act_iteration, 0 = no game / 1 = at an unsolved root / 2 = solved, subgames so far
+  double* root_bel; double* bel;      // [T][2][H] fp64 beliefs at the subgame root (normalised) and at the node (unnormalised)
+  uint32_t* mt; int* mt_idx;          // [624][T], [T]
+  double* cache; int stride;          // [T][stride] acting strategy of the solved subgame, entry (child - 1) * H + hand
+  // this call
+  int n;
+  const int* ids;                     // [n] tables of the call
+  int* io;                            // [n] step: action in (-1 = the agent draws) / action played out; new games: seats
+  const int* hands; const uint64_t* keys;   // [n] new games: hands and stream keys
+  int* widx;                          // [n] wave index of the table's solve, -1 = none
+  double* probs;                      // [n][A] step: the agent's row on its own turns, NaN on the opponent's (or nullptr)
+  int* flags;                         // [n] step: bit 0 game over, bit 1 at the root of a new subgame
+  double* pol;                        // [n][H][A] policy of the player to move
+  // tree templates and the handle's wave descriptors
+  const TemplateDev* tmpl; const int* child_begin; const int* nchild; const int* level_begin;
+  int table_stride;
+  int* wave; int* sg_tmpl; int* sg_player; int* sg_row_off; int* sg_act; const int* steps;
+};
+void agent_launch_new(const AgentDev& p, cudaStream_t st);
+// scan + subgame descriptors of the listed tables that stand at an unsolved root
+template <typename real> void agent_launch_begin(const AgentDev& p, const MatchTabs<real>& t, cudaStream_t st);
+template <typename real> void agent_launch_capture(const AgentDev& p, const MatchTabs<real>& t, cudaStream_t st);
+void agent_launch_step(const AgentDev& p, cudaStream_t st);
+void agent_launch_policy(const AgentDev& p, cudaStream_t st);
 // rows [ids[i]] of a [*, width] fp32 matrix -> out[i]  (replay sampling)
 void rows_launch_gather(const float* src, int width, const int* ids, int n, float* out, cudaStream_t st);
 

@@ -2354,3 +2354,317 @@ int cfrb_comm_reduce_sum(cfrb_comm* c, float* dev_buf, size_t n, int32_t root) {
 }
 
 }  // extern "C"
+
+// ============================================================================================ an agent against external players
+struct cfrb_agent {
+  cfrb_handle* h = nullptr;
+  int T = 0, sampled = 0;
+  uint64_t games_started = 0;
+  DevBuf<int> seat, hand, last_bid, player, ply, root_lb, root_player, node, depth, act, status, subgames, mt_idx;
+  DevBuf<int> ids, io, hands, widx, flags;
+  DevBuf<uint64_t> keys;
+  DevBuf<double> root_bel, bel, cache, probs, pol;
+  DevBuf<uint32_t> mt;
+  cfrb::AgentDev dev{};
+  // host mirror of each table's public state, updated from every call's outputs (all calls synchronise)
+  std::vector<char> running, need_solve;
+  std::vector<int> h_seat, h_last_bid, h_player;
+  std::vector<int64_t> stamp;         // call number that last listed the table (repeated ids)
+  int64_t calls = 0, solves = 0;
+  double solve_ms = 0;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  void release() {
+    for (auto* b : {&seat, &hand, &last_bid, &player, &ply, &root_lb, &root_player, &node, &depth, &act, &status, &subgames, &mt_idx,
+                    &ids, &io, &hands, &widx, &flags})
+      b->release();
+    for (auto* b : {&root_bel, &bel, &cache, &probs, &pol}) b->release();
+    keys.release(); mt.release();
+    for (auto& e : ev) if (e) cudaEventDestroy(e);
+    ev[0] = ev[1] = nullptr;
+  }
+};
+
+template <typename real>
+static cfrb::MatchTabs<real> agent_tabs(cfrb_agent* a) {
+  cfrb::MatchTabs<real> t{};
+  cfrb_handle* h = a->h;
+  auto& s = state_of<real>(h);
+  const bool fp = h->cfg.solver == CFRB_SOLVER_FP;
+  t.wave_beliefs[0] = s.beliefs.p;
+  t.table[0] = a->sampled ? s.Snap.p : fp ? s.Sg.p : s.S.p;
+  t.normalise[0] = !a->sampled && !fp;
+  return t;
+}
+template <typename real>
+static int agent_begin_t(cfrb_agent* a, const cfrb::AgentDev& d, cudaStream_t st) {
+  cfrb::agent_launch_begin<real>(d, agent_tabs<real>(a), st);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+template <typename real>
+static int agent_capture_t(cfrb_agent* a, const cfrb::AgentDev& d, cudaStream_t st) {
+  cfrb::agent_launch_capture<real>(d, agent_tabs<real>(a), st);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+
+static std::string agent_table(const char* who, int id) { return std::string(who) + ": table " + std::to_string(id) + ": "; }
+
+// Ids in range, distinct, and (running) holding a game.
+static int agent_check_ids(cfrb_agent* a, const char* who, int n, const int32_t* ids, bool running) {
+  ++a->calls;
+  for (int i = 0; i < n; ++i) {
+    const int t = ids[i];
+    if (t < 0 || t >= a->T) return fail(CFRB_EINVAL, agent_table(who, t) + "id out of range [0, " + std::to_string(a->T) + ")");
+    if (a->stamp[t] == a->calls) return fail(CFRB_EINVAL, agent_table(who, t) + "listed twice");
+    a->stamp[t] = a->calls;
+    if (running && !a->running[t]) return fail(CFRB_EINVAL, agent_table(who, t) + "no running game");
+  }
+  return CFRB_OK;
+}
+
+// Copies the call's ids to the device and returns the per-call view of the state.
+static int agent_call(cfrb_agent* a, int n, const int32_t* ids, cfrb::AgentDev* d) {
+  CK(cudaSetDevice(a->h->cfg.device));
+  CK(cudaMemcpyAsync(a->ids.p, ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, a->h->own_stream));
+  *d = a->dev;
+  d->n = n;
+  return CFRB_OK;
+}
+
+// One wave: every listed table at an unsolved root, packed in list order, solved and captured into the cache.
+static int agent_solve(cfrb_agent* a, const cfrb::AgentDev& d, int n, const int32_t* ids) {
+  int n_solve = 0;
+  for (int i = 0; i < n; ++i) n_solve += a->need_solve[ids[i]];
+  if (n_solve == 0) return CFRB_OK;
+  cfrb_handle* h = a->h;
+  cudaStream_t st = h->own_stream;
+  int rc = DISPATCH_REAL(h, agent_begin_t, a, d, st);
+  if (rc) return rc;
+  h->n = n_solve; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
+  CK(cudaEventRecord(a->ev[0], st));
+  if ((rc = DISPATCH_REAL(h, launch_init_t, h, st))) return rc;
+  if ((rc = cfrb_run(h, h->cfg.num_iters, st))) return rc;
+  CK(cudaEventRecord(a->ev[1], st));
+  if ((rc = DISPATCH_REAL(h, agent_capture_t, a, d, st))) return rc;
+  h->launches += 3;
+  CK(cudaEventSynchronize(a->ev[1]));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, a->ev[0], a->ev[1]));
+  a->solve_ms += ms;
+  a->solves += n_solve;
+  for (int i = 0; i < n; ++i) a->need_solve[ids[i]] = 0;
+  return CFRB_OK;
+}
+
+static int agent_create_impl(cfrb_agent* a, cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t policy) {
+  if (!h) return fail(CFRB_EINVAL, "cfrb_agent_create: null handle");
+  if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_SAMPLED) return fail(CFRB_EINVAL, "cfrb_agent_create: bad policy");
+  if (n_tables < 1) return fail(CFRB_EINVAL, "cfrb_agent_create: n_tables must be >= 1");
+  if (h->cfg.max_subgames < n_tables)
+    return fail(CFRB_EINVAL, "cfrb_agent_create: the handle's capacity (max_subgames " + std::to_string(h->cfg.max_subgames) +
+                                 ") is smaller than n_tables " + std::to_string(n_tables) + " (one wave solves every listed table)");
+  if (h->sp.ready) return fail(CFRB_EINVAL, "cfrb_agent_create: the handle has a live self-play session");
+  if (h->in_match) return fail(CFRB_EINVAL, "cfrb_agent_create: the handle already plays in a live match or agent");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());
+  const int T = n_tables, H = h->g.H, A = h->g.A;
+  a->T = T;
+  a->sampled = policy == CFRB_MATCH_SAMPLED;
+  for (auto* b : {&a->seat, &a->hand, &a->last_bid, &a->player, &a->ply, &a->root_lb, &a->root_player, &a->node, &a->depth, &a->act,
+                  &a->status, &a->subgames, &a->mt_idx, &a->ids, &a->io, &a->hands, &a->widx, &a->flags}) {
+    CK(b->alloc(T));
+    CK(cudaMemset(b->p, 0, (size_t)T * sizeof(int)));
+  }
+  CK(a->keys.alloc(T));
+  CK(a->root_bel.alloc((size_t)T * 2 * H)); CK(a->bel.alloc((size_t)T * 2 * H));
+  CK(cudaMemset(a->root_bel.p, 0, (size_t)T * 2 * H * sizeof(double)));
+  CK(a->cache.alloc((size_t)T * h->table_stride)); CK(a->probs.alloc((size_t)T * A)); CK(a->pol.alloc((size_t)T * H * A));
+  CK(a->mt.alloc((size_t)624 * T));
+  CK(cudaEventCreate(&a->ev[0])); CK(cudaEventCreate(&a->ev[1]));
+  a->running.assign(T, 0); a->need_solve.assign(T, 0);
+  a->h_seat.assign(T, 0); a->h_last_bid.assign(T, -1); a->h_player.assign(T, 0);
+  a->stamp.assign(T, 0);
+  cfrb::AgentDev& d = a->dev;
+  d.T = T; d.A = A; d.H = H; d.max_depth = h->cfg.max_depth; d.sampled = a->sampled; d.iters = h->cfg.num_iters; d.seed = seed;
+  d.seat = a->seat.p; d.hand = a->hand.p; d.last_bid = a->last_bid.p; d.player = a->player.p; d.ply = a->ply.p;
+  d.root_lb = a->root_lb.p; d.root_player = a->root_player.p; d.node = a->node.p; d.depth = a->depth.p;
+  d.act = a->act.p; d.status = a->status.p; d.subgames = a->subgames.p;
+  d.root_bel = a->root_bel.p; d.bel = a->bel.p; d.mt = a->mt.p; d.mt_idx = a->mt_idx.p;
+  d.cache = a->cache.p; d.stride = h->table_stride;
+  d.ids = a->ids.p; d.io = a->io.p; d.hands = a->hands.p; d.keys = a->keys.p; d.widx = a->widx.p; d.probs = a->probs.p;
+  d.flags = a->flags.p; d.pol = a->pol.p;
+  d.tmpl = h->d_tmpl.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p; d.level_begin = h->d_level_begin.p;
+  d.table_stride = h->table_stride;
+  d.wave = h->d_wave.p; d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_row_off = h->d_sg_row_off.p;
+  d.sg_act = h->d_sg_act.p; d.steps = h->d_steps.p;
+  a->h = h;
+  h->in_match = true;
+  return CFRB_OK;
+}
+
+extern "C" {
+
+int cfrb_agent_create(cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t policy, cfrb_agent** out) {
+  if (!out) return fail(CFRB_EINVAL, "cfrb_agent_create: null argument");
+  *out = nullptr;
+  cfrb_agent* a = new cfrb_agent();
+  const int rc = agent_create_impl(a, h, n_tables, seed, policy);
+  if (rc != CFRB_OK) {
+    a->release();
+    delete a;
+    return rc;
+  }
+  *out = a;
+  return CFRB_OK;
+}
+
+int cfrb_agent_destroy(cfrb_agent* a) {
+  if (!a) return CFRB_OK;
+  int rc = CFRB_OK;
+  if (cudaSetDevice(a->h->cfg.device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess)
+    rc = fail(CFRB_ECUDA, std::string("cfrb_agent_destroy: ") + cudaGetErrorString(cudaGetLastError()));
+  a->h->in_match = false;
+  a->release();
+  delete a;
+  return rc;
+}
+
+int cfrb_agent_new_games(cfrb_agent* a, int32_t n, const int32_t* ids, const int32_t* seats, const int32_t* hands, const uint64_t* keys) {
+  static const char* who = "cfrb_agent_new_games";
+  if (!a || n < 0 || n > (a ? a->T : 0)) return fail(CFRB_EINVAL, std::string(who) + ": bad argument");
+  if (n == 0) return CFRB_OK;
+  if (!ids || !seats || !hands) return fail(CFRB_EINVAL, std::string(who) + ": null argument");
+  int rc = agent_check_ids(a, who, n, ids, false);
+  if (rc) return rc;
+  for (int i = 0; i < n; ++i) {
+    if (seats[i] != 0 && seats[i] != 1) return fail(CFRB_EINVAL, agent_table(who, ids[i]) + "seat must be 0 or 1");
+    if (hands[i] < 0 || hands[i] >= a->dev.H)
+      return fail(CFRB_EINVAL, agent_table(who, ids[i]) + "hand " + std::to_string(hands[i]) + " outside [0, " + std::to_string(a->dev.H) + ")");
+  }
+  std::vector<uint64_t> k(n);
+  for (int i = 0; i < n; ++i) k[i] = keys ? keys[i] : a->games_started + (uint64_t)i;
+  cfrb::AgentDev d;
+  if ((rc = agent_call(a, n, ids, &d))) return rc;
+  cudaStream_t st = a->h->own_stream;
+  CK(cudaMemcpyAsync(a->io.p, seats, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(a->hands.p, hands, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(a->keys.p, k.data(), (size_t)n * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+  cfrb::agent_launch_new(d, st);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  a->games_started += n;
+  for (int i = 0; i < n; ++i) {
+    const int t = ids[i];
+    a->running[t] = 1; a->need_solve[t] = 1; a->h_seat[t] = seats[i]; a->h_last_bid[t] = -1; a->h_player[t] = 0;
+  }
+  return CFRB_OK;
+}
+
+int cfrb_agent_step(cfrb_agent* a, int32_t n, const int32_t* ids, int32_t* actions, double* probs, int32_t* done) {
+  static const char* who = "cfrb_agent_step";
+  if (!a || n < 0 || n > (a ? a->T : 0)) return fail(CFRB_EINVAL, std::string(who) + ": bad argument");
+  if (n == 0) return CFRB_OK;
+  if (!ids || !actions || !done) return fail(CFRB_EINVAL, std::string(who) + ": null argument");
+  int rc = agent_check_ids(a, who, n, ids, true);
+  if (rc) return rc;
+  const int A = a->dev.A;
+  for (int i = 0; i < n; ++i) {
+    const int t = ids[i], x = actions[i], lb = a->h_last_bid[t];
+    if (x == -1) {
+      if (a->h_player[t] != a->h_seat[t]) return fail(CFRB_EINVAL, agent_table(who, t) + "-1 (the agent plays) on the opponent's turn");
+    } else if (x < 0 || x >= A) {
+      return fail(CFRB_EINVAL, agent_table(who, t) + "action " + std::to_string(x) + " outside [-1, " + std::to_string(A) + ")");
+    } else if (x <= lb) {
+      return fail(CFRB_EINVAL, agent_table(who, t) + "illegal action " + std::to_string(x) + ": not above the last bid " + std::to_string(lb));
+    } else if (x == A - 1 && lb < 0) {
+      return fail(CFRB_EINVAL, agent_table(who, t) + "illegal action: liar call before any bid");
+    }
+  }
+  cfrb::AgentDev d;
+  if ((rc = agent_call(a, n, ids, &d))) return rc;
+  cudaStream_t st = a->h->own_stream;
+  CK(cudaMemcpyAsync(a->io.p, actions, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+  if ((rc = agent_solve(a, d, n, ids))) return rc;
+  if (!probs) d.probs = nullptr;
+  cfrb::agent_launch_step(d, st);
+  CK(cudaGetLastError());
+  a->h->launches += 1;
+  std::vector<int> flags(n);
+  CK(cudaMemcpyAsync(actions, a->io.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(flags.data(), a->flags.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (probs) CK(cudaMemcpyAsync(probs, a->probs.p, (size_t)n * A * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i) {
+    const int t = ids[i];
+    done[i] = flags[i] & 1;
+    a->running[t] = !done[i];
+    a->need_solve[t] = (flags[i] >> 1) & 1;
+    a->h_last_bid[t] = actions[i];
+    a->h_player[t] ^= 1;
+  }
+  return CFRB_OK;
+}
+
+int cfrb_agent_policy(cfrb_agent* a, int32_t n, const int32_t* ids, double* out) {
+  static const char* who = "cfrb_agent_policy";
+  if (!a || n < 0 || n > (a ? a->T : 0)) return fail(CFRB_EINVAL, std::string(who) + ": bad argument");
+  if (n == 0) return CFRB_OK;
+  if (!ids || !out) return fail(CFRB_EINVAL, std::string(who) + ": null argument");
+  int rc = agent_check_ids(a, who, n, ids, true);
+  if (rc) return rc;
+  cfrb::AgentDev d;
+  if ((rc = agent_call(a, n, ids, &d))) return rc;
+  cudaStream_t st = a->h->own_stream;
+  if ((rc = agent_solve(a, d, n, ids))) return rc;
+  cfrb::agent_launch_policy(d, st);
+  CK(cudaGetLastError());
+  a->h->launches += 1;
+  CK(cudaMemcpyAsync(out, a->pol.p, (size_t)n * d.H * d.A * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return CFRB_OK;
+}
+
+int cfrb_agent_state(cfrb_agent* a, int32_t n, const int32_t* ids, int32_t* last_bid, int32_t* player, int32_t* ply, int32_t* subgames,
+                     int32_t* act_iteration, double* root_beliefs) {
+  static const char* who = "cfrb_agent_state";
+  if (!a || n < 0 || n > (a ? a->T : 0)) return fail(CFRB_EINVAL, std::string(who) + ": bad argument");
+  if (n == 0) return CFRB_OK;
+  if (!ids) return fail(CFRB_EINVAL, std::string(who) + ": null argument");
+  int rc = agent_check_ids(a, who, n, ids, false);
+  if (rc) return rc;
+  CK(cudaSetDevice(a->h->cfg.device));
+  CK(cudaStreamSynchronize(a->h->own_stream));
+  const int T = a->T, H2 = 2 * a->dev.H;
+  auto gather = [&](const DevBuf<int>& src, int32_t* dst) -> int {
+    if (!dst) return CFRB_OK;
+    std::vector<int> all(T);
+    CK(cudaMemcpy(all.data(), src.p, (size_t)T * sizeof(int), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < n; ++i) dst[i] = all[ids[i]];
+    return CFRB_OK;
+  };
+  if ((rc = gather(a->last_bid, last_bid)) || (rc = gather(a->player, player)) || (rc = gather(a->ply, ply)) ||
+      (rc = gather(a->subgames, subgames)) || (rc = gather(a->act, act_iteration)))
+    return rc;
+  if (root_beliefs) {
+    std::vector<double> all((size_t)T * H2);
+    CK(cudaMemcpy(all.data(), a->root_bel.p, all.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < n; ++i) std::copy_n(all.data() + (size_t)ids[i] * H2, H2, root_beliefs + (size_t)i * H2);
+  }
+  return CFRB_OK;
+}
+
+int cfrb_agent_counts(cfrb_agent* a, int64_t* solves, int64_t* subgame_iters) {
+  if (!a) return fail(CFRB_EINVAL, "cfrb_agent_counts: null agent");
+  if (solves) *solves = a->solves;
+  if (subgame_iters) *subgame_iters = a->solves * (int64_t)a->dev.iters;
+  return CFRB_OK;
+}
+
+int cfrb_agent_solve_ms(cfrb_agent* a, double* ms) {
+  if (!a || !ms) return fail(CFRB_EINVAL, "cfrb_agent_solve_ms: null argument");
+  *ms = a->solve_ms;
+  return CFRB_OK;
+}
+
+}  // extern "C"

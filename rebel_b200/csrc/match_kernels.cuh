@@ -37,11 +37,15 @@ __device__ __forceinline__ uint32_t match_stream_seed(uint64_t seed, uint64_t ke
   return (uint32_t)z ^ (uint32_t)(z >> 32);
 }
 
+// std::mt19937(x) into an interleaved state whose words lie `stride` apart (word i at st[i * stride])
+__device__ __forceinline__ void mt_seed_strided(uint32_t* st, int stride, uint32_t x) {
+  st[0] = x;
+  for (int i = 1; i < 624; ++i) { x = 1812433253u * (x ^ (x >> 30)) + (uint32_t)i; st[(size_t)i * stride] = x; }
+}
+
 // std::mt19937(x) into the interleaved state of slot s
 __device__ __forceinline__ void match_mt_seed(const MatchDev& p, int s, uint32_t x) {
-  uint32_t* st = p.mt + s;
-  st[0] = x;
-  for (int i = 1; i < 624; ++i) { x = 1812433253u * (x ^ (x >> 30)) + (uint32_t)i; st[(size_t)i * p.S] = x; }
+  mt_seed_strided(p.mt + s, p.S, x);
   p.mt_idx[s] = 624;
 }
 

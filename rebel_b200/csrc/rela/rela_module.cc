@@ -8,6 +8,7 @@
 
 #include <chrono>
 
+#include "agent.h"
 #include "batched_runner.h"
 #include "model_locker.h"
 #include "params.h"
@@ -605,6 +606,75 @@ torch::Tensor strategy_recursive_to_leaf(const RecursiveSolvingParams& cfg, int 
   return f64_tensor(s, {N, H, A});
 }
 
+// rela.Agent: index lists and actions from anything torch.as_tensor accepts (lists, numpy arrays, tensors).
+std::vector<int32_t> i32_of(py::object o) {
+  auto t = py::module::import("torch").attr("as_tensor")(o).cast<torch::Tensor>().to(torch::kCPU, torch::kInt32).contiguous().view(-1);
+  return std::vector<int32_t>(t.data_ptr<int32_t>(), t.data_ptr<int32_t>() + t.numel());
+}
+torch::Tensor i32_tensor(const std::vector<int32_t>& v) {
+  auto t = torch::empty({(int64_t)v.size()}, torch::kInt32);
+  std::copy(v.begin(), v.end(), t.data_ptr<int32_t>());
+  return t;
+}
+
+std::shared_ptr<Agent> make_agent(const RecursiveSolvingParams& cfg, int device, int tables, const std::string& policy, uint64_t seed,
+                                  py::object flat_weights) {
+  if (policy != "sampled" && policy != "average") throw std::runtime_error("Agent: policy must be 'sampled' or 'average'");
+  const std::vector<float> w = flat_of(flat_weights);
+  py::gil_scoped_release nogil;
+  return std::make_shared<Agent>(cfg, device, tables, policy == "sampled" ? CFRB_MATCH_SAMPLED : CFRB_MATCH_AVERAGE, seed, w);
+}
+
+void agent_new_games(Agent& a, py::object ids, py::object seats, py::object hands, py::object keys) {
+  std::vector<uint64_t> k;
+  if (!keys.is_none()) {
+    auto t = py::module::import("torch").attr("as_tensor")(keys).cast<torch::Tensor>().to(torch::kCPU, torch::kInt64).contiguous().view(-1);
+    k.assign(reinterpret_cast<const uint64_t*>(t.data_ptr<int64_t>()), reinterpret_cast<const uint64_t*>(t.data_ptr<int64_t>()) + t.numel());
+  }
+  a.newGames(i32_of(ids), i32_of(seats), i32_of(hands), k);
+}
+
+py::tuple agent_step(Agent& a, py::object ids, py::object actions) {
+  const std::vector<int32_t> id = i32_of(ids);
+  std::vector<int32_t> act = i32_of(actions), done;
+  std::vector<double> probs;
+  {
+    py::gil_scoped_release nogil;
+    a.step(id, act, probs, done);
+  }
+  const int64_t n = (int64_t)id.size();
+  return py::make_tuple(i32_tensor(act), f64_tensor(probs, {n, (int64_t)a.numActions()}), i32_tensor(done).to(torch::kBool));
+}
+
+torch::Tensor agent_policy(Agent& a, py::object ids) {
+  const std::vector<int32_t> id = i32_of(ids);
+  std::vector<double> out;
+  {
+    py::gil_scoped_release nogil;
+    out = a.policy(id);
+  }
+  return f64_tensor(out, {(int64_t)id.size(), (int64_t)a.numHands(), (int64_t)a.numActions()});
+}
+
+py::dict agent_state(Agent& a, py::object ids) {
+  const std::vector<int32_t> id = i32_of(ids);
+  const Agent::State s = a.state(id);
+  py::dict d;
+  d["last_bid"] = i32_tensor(s.last_bid); d["player"] = i32_tensor(s.player); d["ply"] = i32_tensor(s.ply);
+  d["subgames"] = i32_tensor(s.subgames); d["act_iteration"] = i32_tensor(s.act_iteration);
+  d["root_beliefs"] = f64_tensor(s.root_beliefs, {(int64_t)id.size(), 2, (int64_t)a.numHands()});
+  return d;
+}
+
+py::dict agent_counts(Agent& a) {
+  int64_t solves = 0, iters = 0;
+  double ms = 0;
+  a.counts(&solves, &iters, &ms);
+  py::dict d;
+  d["solves"] = solves; d["subgame_iters"] = iters; d["solve_ms"] = ms;
+  return d;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(rela, m) {
@@ -737,6 +807,29 @@ PYBIND11_MODULE(rela, m) {
         "deferred_slot_rounds, max_subgames, subgame_iters, seconds.");
   m.def("match_stats", &match_stats_py, py::arg("payoff_a"),
         "rebel_b200 extension: play_match's mean, stderr (over the pairs 2i, 2i+1) and seat_means of a payoff vector.");
+  py::class_<Agent, std::shared_ptr<Agent>>(
+      m, "Agent",
+      "rebel_b200 extension: a ReBeL agent (cfg + net) at `tables` independent tables, each a game against an external player, "
+      "advanced one action per call on the GPU.  It plays its recursive to-leaf policy ('average' or 'sampled') along the path "
+      "played, re-solving from its own beliefs at the game root and at every pseudo-leaf; deals and seats belong to the caller.")
+      .def(py::init(&make_agent), py::arg("cfg"), py::arg("device") = 0, py::arg("tables") = 8192, py::arg("policy") = "sampled",
+           py::arg("seed") = 0, py::arg("flat_weights") = py::none())
+      .def("new_games", &agent_new_games, py::arg("ids"), py::arg("seats"), py::arg("hands"), py::arg("keys") = py::none(),
+           "start a game at each listed table: the agent in seat seats[i] (0 moves first) with hand hands[i]; keys[i] keys the "
+           "game's random stream (None: the number of games started before, in list order)")
+      .def("step", &agent_step, py::arg("ids"), py::arg("actions"),
+           "one action at each listed table: actions[i] is applied (normally the opponent's; on the agent's turn it overrides the "
+           "agent), -1 lets the agent play.  Returns (actions played int32 [n], probs float64 [n, A]: the agent's row for its hand "
+           "on its turns, NaN on the opponent's, done bool [n]: the liar call ended the game)")
+      .def("policy", &agent_policy, py::arg("ids"),
+           "the agent's strategy for the player to move at each listed table: float64 [n, H, A], 0 on illegal actions")
+      .def("state", &agent_state, py::arg("ids"),
+           "dict of last_bid, player, ply, subgames, act_iteration [n] and root_beliefs [n, 2, H] of the current subgame")
+      .def("counts", &agent_counts, "dict: solves, subgame_iters, solve_ms (device time of the solves) since creation")
+      .def("close", &Agent::close, "release the agent and its handle")
+      .def_property_readonly("num_actions", &Agent::numActions)
+      .def_property_readonly("num_hands", &Agent::numHands)
+      .def_property_readonly("tables", &Agent::tables);
   m.def("strategy_recursive_to_leaf", &strategy_recursive_to_leaf, py::arg("cfg"), py::arg("device") = 0,
         py::arg("flat_weights") = py::none(),
         "rebel_b200 extension: compute_strategy_recursive_to_leaf (every subgame solved for num_iters iterations, get_strategy) as a "
