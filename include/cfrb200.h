@@ -272,6 +272,16 @@ int cfrb_debug_gelu_table(cfrb_handle* h, int32_t what, uint16_t* out);
 /* Roots (last_bid, player_id) of the subgames of the current wave — also of a wave built on the device by cfrb_selfplay_wave
  * (synchronises then).  Writes min(n, cap) entries, returns n. */
 int cfrb_wave_roots(cfrb_handle* h, int32_t* last_bid, int32_t* player_id, int32_t cap);
+/* The order in which the depth <= 2 CFR kernel starts the current wave's subgames: wave positions, costliest subgame first
+ * (waves of cfrb_begin_wave and cfrb_selfplay_wave), else 0 .. n-1.  Synchronises.  Writes min(n, cap) entries, returns n. */
+int cfrb_wave_order(cfrb_handle* h, int32_t* order, int32_t cap);
+/* Host only: that order for n subgames rooted at last_bid[] of the game's depth-max_depth trees, and cost[k] (may be NULL), the
+ * schedule cost of subgame k: (nodes - 1) x hands table items + pseudo-leaves. */
+int cfrb_schedule_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t n, const int32_t* last_bid, int32_t* order,
+                        int64_t* cost);
+/* Test aid: run the depth <= 2 CFR kernel on at most max_ctas CTAs (0 = as many as are resident at once), so that every warp
+ * solves many subgames per launch.  Returns the number of CTAs resident at once. */
+int cfrb_debug_d2_grid(cfrb_handle* h, int32_t max_ctas);
 /* Block until the work enqueued on `cuda_stream` (NULL = the handle's stream) has finished. */
 int cfrb_stream_wait(cfrb_handle* h, void* cuda_stream);
 

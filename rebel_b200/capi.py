@@ -90,6 +90,9 @@ def lib():
     L.cfrb_debug_div_check.argtypes = [vp, C.c_uint64, C.c_int32, C.POINTER(C.c_uint64)]
     L.cfrb_debug_gelu_table.argtypes = [vp, C.c_int32, C.POINTER(C.c_uint16)]
     L.cfrb_wave_roots.argtypes = [vp, _ip, _ip, C.c_int32]
+    L.cfrb_wave_order.argtypes = [vp, _ip, C.c_int32]
+    L.cfrb_schedule_order.argtypes = [C.c_int32] * 4 + [_ip, _ip, C.POINTER(C.c_int64)]
+    L.cfrb_debug_d2_grid.argtypes = [vp, C.c_int32]
     L.cfrb_mark.argtypes = [vp, C.c_int32, vp]
     L.cfrb_mark_elapsed_ms.argtypes = [vp, C.c_int32, C.c_int32, _fp]
     L.cfrb_l2_flush.argtypes = [vp, C.c_size_t, vp]
@@ -130,6 +133,17 @@ def unroll_tree(num_dice, num_faces, last_bid=-1, player_id=0, max_depth=1000000
     out = np.zeros((cap, 6), np.int32)
     n = _check(lib().cfrb_unroll_tree(num_dice, num_faces, last_bid, player_id, max_depth, _p(out, _ip), cap))
     return out[:n].copy()
+
+
+def schedule_order(num_dice, num_faces, last_bid, max_depth=2):
+    """Host-only: (order, cost) — the order in which the depth-2 CFR kernel starts subgames rooted at last_bid (wave positions,
+    costliest first, stable) and each subgame's schedule cost."""
+    lb = np.ascontiguousarray(last_bid, np.int32)
+    order = np.zeros(lb.size, np.int32)
+    cost = np.zeros(lb.size, np.int64)
+    _check(lib().cfrb_schedule_order(num_dice, num_faces, max_depth, lb.size, _p(lb, _ip), _p(order, _ip),
+                                     cost.ctypes.data_as(C.POINTER(C.c_int64))))
+    return order, cost
 
 
 def tc_net_supported(num_dice, num_faces, hidden=256):
@@ -315,6 +329,16 @@ class WaveSolver:
         lb = np.zeros(self.n, np.int32); pl = np.zeros(self.n, np.int32)
         n = _check(lib().cfrb_wave_roots(self._h, _p(lb, _ip), _p(pl, _ip), self.n))
         return lb[:n], pl[:n]
+
+    def wave_order(self):
+        """The order in which the depth-2 CFR kernel starts the current wave's subgames (wave positions)."""
+        out = np.zeros(self.n, np.int32)
+        n = _check(lib().cfrb_wave_order(self._h, _p(out, _ip), self.n))
+        return out[:n]
+
+    def debug_d2_grid(self, max_ctas):
+        """Test aid: run the depth-2 CFR kernel on at most max_ctas CTAs (0 = no cap); returns the CTAs resident at once."""
+        return _check(lib().cfrb_debug_d2_grid(self._h, int(max_ctas)))
 
     def wait_examples(self):
         _check(lib().cfrb_selfplay_wait_examples(self._h))

@@ -68,12 +68,16 @@ void regret_launch(const RegretDev& r, const float* s32, const double* s64, int 
 }
 
 template <typename real>
-cudaError_t cfr_configure_d2(int smem_bytes) {
+cudaError_t cfr_configure_d2(int H, int threads, int smem_bytes, int* ctas_per_sm) {
   cudaError_t e = cudaSuccess;
 #define CFRB_CFG(HC)                                                                                                      \
   if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
   CFRB_CFG(0) CFRB_CFG(4) CFRB_CFG(5) CFRB_CFG(6) CFRB_CFG(9) CFRB_CFG(16)
 #undef CFRB_CFG
+  if (e != cudaSuccess) return e;
+#define CFRB_OCC(HC) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, cfr_iter_d2_kernel<real, HC>, threads, smem_bytes)
+  CFRB_DISPATCH_H(H, CFRB_OCC)
+#undef CFRB_OCC
   return e;
 }
 
@@ -188,7 +192,7 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template cudaError_t cfr_configure<real>(int, int);                                                                      \
   template void cfr_launch_init<real>(const CfrDev<real>&, int, int, int, size_t, cudaStream_t, int);                      \
   template void cfr_launch_iter<real>(const CfrDev<real>&, int, int, int, size_t, cudaStream_t, int, int, int, int);             \
-  template cudaError_t cfr_configure_d2<real>(int);                                                                        \
+  template cudaError_t cfr_configure_d2<real>(int, int, int, int*);                                                        \
   template void cfr_launch_iter_d2<real>(const CfrDev<real>&, int, int, size_t, cudaStream_t, int, int, int, int);                \
   template void sp_launch_begin<real>(const SpDev&, real*, cudaStream_t);                                                  \
   template void sp_launch_finish<real>(const SpDev&, const real*, const real*, float*, float*, cudaStream_t);              \

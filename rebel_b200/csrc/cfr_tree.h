@@ -11,6 +11,7 @@
 //   * every non-root node c has exactly one incoming edge, so per-(node,hand,action) tables
 //     [n][h][a] are stored compactly as [edge = c-1][h] with c = child(n, a).
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <vector>
 
@@ -78,6 +79,27 @@ inline TreeTemplate build_template(const GameShape& g, int root_bid, int max_dep
   t.level_begin.assign(t.levels + 1, t.N);
   for (int n = t.N - 1; n >= 0; --n) t.level_begin[t.depth[n]] = n;
   return t;
+}
+
+// Schedule of the depth <= 2 CFR kernel: a subgame's cost is its table items ((N - 1) edges x H hands) plus its value-net query
+// rows (L).  The cost is not monotone in the root bid for every game, so templates are ranked by it: rank 0 = the costliest,
+// ties by template index.
+inline int64_t schedule_cost(const TreeTemplate& t, int H) { return (int64_t)(t.N - 1) * H + t.L; }
+inline std::vector<int> schedule_ranks(const std::vector<TreeTemplate>& tmpl, int H) {
+  std::vector<int> by_cost(tmpl.size()), rank(tmpl.size());
+  for (size_t i = 0; i < tmpl.size(); ++i) by_cost[i] = (int)i;
+  std::stable_sort(by_cost.begin(), by_cost.end(),
+                   [&](int a, int b) { return schedule_cost(tmpl[a], H) > schedule_cost(tmpl[b], H); });
+  for (size_t r = 0; r < by_cost.size(); ++r) rank[by_cost[r]] = (int)r;
+  return rank;
+}
+// order[0..n) = the wave positions 0..n-1 of subgames with templates tm[], sorted by rank (stable counting sort); the same
+// permutation sp_scan_kernel builds on the device
+inline void schedule_order(const std::vector<int>& rank, const int* tm, int n, int* order) {
+  std::vector<int> start(rank.size() + 1, 0);
+  for (int k = 0; k < n; ++k) ++start[rank[tm[k]] + 1];
+  for (size_t r = 1; r < start.size(); ++r) start[r] += start[r - 1];
+  for (int k = 0; k < n; ++k) order[start[rank[tm[k]]]++] = k;
 }
 
 }  // namespace cfrb

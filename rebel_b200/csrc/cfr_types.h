@@ -26,6 +26,8 @@ struct CfrDev {
   // wave
   const int* wave_n;              // [1] number of live subgames
   const int* sg_tmpl; const int* sg_player; const int* sg_row_off; const int* sg_act_iter;
+  const int* sg_order;            // [K] wave positions largest template first (cfr_iter_d2_kernel's schedule) -- or nullptr = identity
+  int* ticket;                    // [1] cfr_iter_d2_kernel's subgame counter; zero between launches
   const real* beliefs;            // [K][2][H]
   real* mu;                       // [K][2][H] root_values_means
   int* steps;                     // [K][2]
@@ -109,6 +111,8 @@ struct SpDev {
   // wave descriptors
   int* wave;                          // [0] = number of subgames, [1] = value-net rows
   int* sg_tmpl; int* sg_player; int* sg_row_off; int* sg_act;
+  int* sg_order;                      // [K] wave positions sorted by tmpl_rank (stable)
+  const int* tmpl_rank;               // [A] schedule rank of each template, 0 = the costliest (schedule_ranks, cfr_tree.h)
   int table_stride;
 };
 void sp_launch_seed(const SpDev& p, const uint32_t* dev_seeds, cudaStream_t st);
@@ -219,8 +223,9 @@ template <typename real> void cfr_launch_init(const CfrDev<real>& p, int group, 
                                               int scratch_per_group);
 template <typename real> void cfr_launch_iter(const CfrDev<real>& p, int group, int blocks, int threads, size_t smem, cudaStream_t st,
                                               int iter, int do_b, int do_f, int scratch_per_group);
-// Depth <= 2 specialisation (warp per subgame, half the scratch); threads must be a multiple of 32 and <= 256.
-template <typename real> cudaError_t cfr_configure_d2(int smem_bytes);
+// Depth <= 2 specialisation (persistent warps, one subgame at a time, half the scratch); threads must be a multiple of 32 and
+// <= 256.  *ctas_per_sm receives how many CTAs of `threads` threads and `smem_bytes` bytes are resident per SM for H hands.
+template <typename real> cudaError_t cfr_configure_d2(int H, int threads, int smem_bytes, int* ctas_per_sm);
 template <typename real> void cfr_launch_iter_d2(const CfrDev<real>& p, int blocks, int threads, size_t smem, cudaStream_t st, int iter,
                                                  int do_b, int do_f, int scratch_per_group);
 

@@ -106,6 +106,10 @@ struct cfrb_handle {
   int d2_groups_per_cta = 8;
   int d2_scratch_per_group = 0;
   size_t d2_smem = 0;      // dynamic shared memory of a depth-2 CTA
+  int d2_ctas = 0;         // CTAs of the depth-2 kernel resident at once on the device: its persistent grid
+  int d2_grid_cap = 0;     // test aid (cfrb_debug_d2_grid): at most this many CTAs, 0 = no cap
+  std::vector<int> tmpl_rank;   // schedule rank of each template (schedule_ranks)
+  bool sorted = false;     // d_sg_order holds the current wave's schedule; otherwise the depth-2 kernel takes wave order
   int n1max = 0;           // bound on the level-1 nodes of a template (the depth-2 scratch layout)
   int table_stride = 0;
   int num_sms = 0;
@@ -116,9 +120,9 @@ struct cfrb_handle {
   std::vector<cudaEvent_t> net_ev;   // pairs around value-net launches (profiling mode)
   int net_ev_used = 0;
   // CUDA graphs of whole cfrb_run calls (2 launches per iteration would otherwise be enqueued one by one by the host)
-  struct GraphEntry { int first, count, prof, has_rows; cudaGraphExec_t exec; int launches, net_launches, ev_used; };
+  struct GraphEntry { int first, count, prof, has_rows, sorted; cudaGraphExec_t exec; int launches, net_launches, ev_used; };
   std::vector<GraphEntry> graphs;
-  std::vector<std::array<int, 4>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
+  std::vector<std::array<int, 5>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
   bool capturing = false;           // launch geometry independent of the wave size while a graph is being captured / replayed
   // device: templates
   DevBuf<cfrb::TemplateDev> d_tmpl;
@@ -146,6 +150,7 @@ struct cfrb_handle {
   // device: wave (untyped part)
   DevBuf<int> d_wave;      // [0] = n, [1] = rows
   DevBuf<int> d_sg_tmpl, d_sg_player, d_sg_row_off, d_sg_act, d_steps;
+  DevBuf<int> d_sg_order, d_tmpl_rank, d_ticket;   // the depth-2 kernel's schedule, template ranks, subgame counter
   DevBuf<float> d_X, d_out, d_dbg;
   long long* dbg_trace = nullptr;   // set only inside cfrb_debug_net_trace
   int x2_gelu = 2;                  // GELU variant of CFRB_NET_TC_F16X2 (leaf_mlp_tc.cuh kGelu): 2 = fp32 tanh, 1 = packed half
@@ -223,15 +228,17 @@ static int alloc_state(cfrb_handle* h, int max_optin) {
     const int smem_bytes = (int)(per_group_bytes * h->groups_per_cta);
     CK(cfrb::cfr_configure<real>(32, smem_bytes));
     if (h->max_levels <= 3 && h->tpk_stride > 0) {
-      // 32 warps per SM (register file: 64 registers x 32 warps) as 8 CTAs of 4 warps: small CTAs even out the last round
-      // (8192 subgames on the 4224 warp slots of a 132-SM H100 = 1.94 rounds); each CTA has 1 KB of shared memory reserved by the runtime
+      // 32 warps per SM (register file: 64 registers x 32 warps) as 8 CTAs of 4 warps; each CTA has 1 KB of shared memory reserved
+      // by the runtime.  The grid is at most the resident CTAs (d2_ctas): persistent warps, costliest subgame first
       h->d2 = true;
       h->d2_scratch_per_group = cfrb::cfr_scratch_reals_d2((int)sizeof(real), h->Nmax, h->g.H, h->Lmax, h->Tmax, h->n1max);
       const size_t d2_bytes = (size_t)h->d2_scratch_per_group * sizeof(real) + h->tpk_stride;
       const size_t cta_budget = ((size_t)228 * 1024 - 8 * 1024) / 8;
       h->d2_groups_per_cta = (int)std::max<size_t>(1, std::min<size_t>(4, cta_budget / d2_bytes));
       h->d2_smem = d2_bytes * h->d2_groups_per_cta;
-      CK(cfrb::cfr_configure_d2<real>((int)h->d2_smem));
+      int ctas_per_sm = 0;
+      CK(cfrb::cfr_configure_d2<real>(g.H, 32 * h->d2_groups_per_cta, (int)h->d2_smem, &ctas_per_sm));
+      h->d2_ctas = std::max(1, ctas_per_sm) * h->num_sms;
     }
   } else {
     h->group = 256;
@@ -246,6 +253,7 @@ static int alloc_state(cfrb_handle* h, int max_optin) {
   d.tpk = h->d_tpk.p; d.tpk_stride = h->tpk_stride;
   d.wave_n = h->d_wave.p; d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_row_off = h->d_sg_row_off.p;
   d.sg_act_iter = h->d_sg_act.p; d.beliefs = s.beliefs.p; d.mu = s.mu.p; d.steps = h->d_steps.p;
+  d.sg_order = nullptr; d.ticket = h->d_ticket.p;
   d.R = s.R.p; d.Sg = s.Sg.p; d.S = s.S.p; d.Snap = s.Snap.p; d.table_stride = h->table_stride;
   d.vterm = s.vterm.p; d.vterm_stride = vterm_stride;
   d.lmax = std::max(h->Lmax, 1); d.tmax = std::max(h->Tmax, 1); d.n1max = h->n1max;
@@ -277,9 +285,12 @@ static int launch_iter_t(cfrb_handle* h, cudaStream_t st, int iter, int do_b, in
   auto& s = state_of<real>(h);
   const int nsg = h->capturing ? h->cfg.max_subgames : h->n;   // surplus groups return at once (k >= *wave_n)
   if (h->d2) {
-    const int blocks = (nsg + h->d2_groups_per_cta - 1) / h->d2_groups_per_cta;
-    const size_t smem = h->d2_smem;
-    cfrb::cfr_launch_iter_d2<real>(s.dev, blocks, 32 * h->d2_groups_per_cta, smem, st, iter, do_b, do_f, h->d2_scratch_per_group);
+    // persistent warps: no more CTAs than are resident at once (the warps then take the wave's subgames from a counter)
+    int blocks = std::min((nsg + h->d2_groups_per_cta - 1) / h->d2_groups_per_cta, h->d2_ctas);
+    if (h->d2_grid_cap > 0) blocks = std::min(blocks, h->d2_grid_cap);
+    cfrb::CfrDev<real> d = s.dev;
+    d.sg_order = h->sorted ? h->d_sg_order.p : nullptr;
+    cfrb::cfr_launch_iter_d2<real>(d, blocks, 32 * h->d2_groups_per_cta, h->d2_smem, st, iter, do_b, do_f, h->d2_scratch_per_group);
   } else {
     const int blocks = (nsg + h->groups_per_cta - 1) / h->groups_per_cta;
     const size_t smem = h->group == 32 ? (size_t)h->scratch_per_group * sizeof(real) * h->groups_per_cta : 0;
@@ -522,6 +533,7 @@ int cfrb_destroy(cfrb_handle* h) {
   h->d_tpk.release();
   h->d_level_begin.release(); h->d_pleaf_node.release(); h->d_term_node.release(); h->d_matches.release(); h->d_qconst.release();
   h->d_wave.release(); h->d_sg_tmpl.release(); h->d_sg_player.release(); h->d_sg_row_off.release(); h->d_sg_act.release();
+  h->d_sg_order.release(); h->d_tmpl_rank.release(); h->d_ticket.release();
   h->d_steps.release(); h->d_X.release(); h->d_out.release(); h->d_dbg.release(); h->d_Xh.release();
   h->sf.release(); h->sd.release(); h->d_w.release(); h->d_blob.release();
   h->sp.last_bid.release(); h->sp.player.release(); h->sp.mt_idx.release(); h->sp.beliefs.release(); h->sp.mt.release();
@@ -637,6 +649,8 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   CK(up(h->d_tmpl, td)); CK(up(h->d_parent, parent)); CK(up(h->d_child_begin, child_begin)); CK(up(h->d_nchild, nchild));
   CK(up(h->d_last_bid, last_bid)); CK(up(h->d_level_begin, level_begin)); CK(up(h->d_pleaf_node, pleaf_node));
   CK(up(h->d_term_node, term_node)); CK(up(h->d_matches, matches)); CK(up(h->d_qconst, qconst));
+  h->tmpl_rank = cfrb::schedule_ranks(h->tmpl, g.H);
+  CK(up(h->d_tmpl_rank, h->tmpl_rank));
 
   // ---- sizes
   const int K = cfg->max_subgames;
@@ -651,6 +665,8 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   CK(h->d_wave.alloc(2));
   CK(h->d_sg_tmpl.alloc(K)); CK(h->d_sg_player.alloc(K)); CK(h->d_sg_row_off.alloc(K)); CK(h->d_sg_act.alloc(K));
   CK(h->d_steps.alloc((size_t)K * 2));
+  CK(h->d_sg_order.alloc(K)); CK(h->d_ticket.alloc(1));
+  CK(cudaMemset(h->d_ticket.p, 0, sizeof(int)));
   const size_t rows_cap = (size_t)K * std::max(h->Lmax, 1);
   CK(h->d_X.alloc(cfg->net_mode == CFRB_NET_FP32 ? rows_cap * h->Qpad : 1));
   CK(h->d_out.alloc(rows_cap * h->Hout));
@@ -865,7 +881,9 @@ int cfrb_begin_wave(cfrb_handle* h, int32_t n, const int32_t* last_bid, const in
     rows += h->tmpl[tm[k]].L;
     if (act_iteration) act[k] = act_iteration[k];
   }
-  h->n = n; h->rows = rows; h->iters_done = 0; h->rows_on_device = false; h->sp.pending = false;
+  std::vector<int> order(n);
+  cfrb::schedule_order(h->tmpl_rank, tm.data(), n, order.data());
+  h->n = n; h->rows = rows; h->iters_done = 0; h->rows_on_device = false; h->sp.pending = false; h->sorted = true;
   h->h_tmpl = tm; h->h_player = pl; h->h_row_off = ro;
   h->h_last_bid.assign(last_bid, last_bid + n);
   h->h_beliefs.assign(beliefs, beliefs + (size_t)n * 2 * H);
@@ -878,6 +896,7 @@ int cfrb_begin_wave(cfrb_handle* h, int32_t n, const int32_t* last_bid, const in
     CK(cudaMemcpyAsync(h->d_sg_player.p, pl.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(h->d_sg_row_off.p, ro.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(h->d_sg_act.p, act.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(h->d_sg_order.p, order.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
     int rc = DISPATCH_REAL(h, upload_beliefs_t, h, st);
     if (rc) return rc;
     rc = DISPATCH_REAL(h, launch_init_t, h, st);
@@ -983,19 +1002,19 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
   const int first = h->iters_done, last = first + iters;
   // Long runs are replayed from a CUDA graph: one host call instead of 2 * iters kernel launches, so a busy or slow host
   // thread cannot starve the GPU.  The graph bakes in the iteration indices and a wave-size-independent launch geometry; it
-  // is keyed by (first iteration, count, profiling period, "the wave has value-net rows").  The fp32 parity net sizes its grid
+  // is keyed by (first iteration, count, profiling period, "the wave has value-net rows", "the wave has a schedule").  The fp32 parity net sizes its grid
   // by the row count and stays on the eager path, like short runs.
   static const bool no_graph = [] { const char* e = std::getenv("CFRB_NO_GRAPH"); return e && *e == '1'; }();
   const bool graphable = !no_graph && iters >= 64 && h->cfg.net_mode != CFRB_NET_FP32;
   if (graphable) {
-    const int has_rows = h->rows > 0 || h->rows_on_device;
+    const int has_rows = h->rows > 0 || h->rows_on_device, sorted = h->sorted;
     cfrb_handle::GraphEntry* g = nullptr;
     for (auto& e : h->graphs)
-      if (e.first == first && e.count == iters && e.prof == h->profiling && e.has_rows == has_rows) { g = &e; break; }
+      if (e.first == first && e.count == iters && e.prof == h->profiling && e.has_rows == has_rows && e.sorted == sorted) { g = &e; break; }
     if (!g) {
       // capture + instantiation of ~2 * iters nodes costs ~0.1 s: only worth it for a key that repeats (waves of a self-play
       // loop, bench steps), not for one-off run lengths (e.g. the evaluator's per-chunk act_iteration maxima)
-      const std::array<int, 4> key{first, iters, h->profiling, has_rows};
+      const std::array<int, 5> key{first, iters, h->profiling, has_rows, sorted};
       bool seen = false;
       for (const auto& k : h->graph_seen) seen |= k == key;
       if (!seen) {
@@ -1026,7 +1045,7 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
       h->launches = l0;
       if (rc == CFRB_OK && ce == cudaSuccess && exec) {
         if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
-        h->graphs.push_back({first, iters, h->profiling, has_rows, exec, captured, h->net_launches_run, h->net_ev_used});
+        h->graphs.push_back({first, iters, h->profiling, has_rows, sorted, exec, captured, h->net_launches_run, h->net_ev_used});
         g = &h->graphs.back();
       } else {
         cudaGetLastError();   // the stream could not be captured (e.g. a legacy stream): run eagerly
@@ -1473,6 +1492,7 @@ int cfrb_selfplay_create(cfrb_handle* h, int32_t n_games, const uint32_t* seeds,
   d.tmpl = h->d_tmpl.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p; d.last_bid = h->d_last_bid.p;
   d.wave = h->d_wave.p; d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_row_off = h->d_sg_row_off.p;
   d.sg_act = h->d_sg_act.p; d.table_stride = h->table_stride;
+  d.sg_order = h->d_sg_order.p; d.tmpl_rank = h->d_tmpl_rank.p;
   CK(cudaStreamSynchronize(h->own_stream));
   CK(cudaMemcpyAsync(sp.seeds.p, seeds, (size_t)K * sizeof(uint32_t), cudaMemcpyHostToDevice, h->own_stream));
   cfrb::sp_launch_seed(d, sp.seeds.p, h->own_stream);
@@ -1504,7 +1524,7 @@ int cfrb_selfplay_wave(cfrb_handle* h, float* dev_ex_q, float* dev_ex_v, int32_t
   if (start_next) {
     int rc = DISPATCH_REAL(h, selfplay_begin_t, h, st);
     if (rc) return rc;
-    h->n = h->sp.K; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0;
+    h->n = h->sp.K; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sorted = true;
     rc = DISPATCH_REAL(h, launch_init_t, h, st);
     if (rc) return rc;
     rc = cfrb_run(h, h->cfg.num_iters, st);
@@ -1544,6 +1564,44 @@ int cfrb_wave_roots(cfrb_handle* h, int32_t* last_bid, int32_t* player_id, int32
     if (player_id) player_id[k] = h->h_player[k];
   }
   return h->n;
+}
+
+int cfrb_wave_order(cfrb_handle* h, int32_t* order, int32_t cap) {
+  if (!h || !order) return fail(CFRB_EINVAL, "null argument");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());
+  const int n = std::min(h->n, (int)std::max(cap, 0));
+  if (h->sorted) CK(cudaMemcpy(order, h->d_sg_order.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+  else for (int k = 0; k < n; ++k) order[k] = k;
+  return h->n;
+}
+
+int cfrb_schedule_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t n, const int32_t* last_bid, int32_t* order,
+                        int64_t* cost) {
+  if (num_dice < 1 || num_faces < 1 || max_depth < 1 || n < 0 || (n > 0 && (!last_bid || !order))) return fail(CFRB_EINVAL, "bad argument");
+  const cfrb::GameShape g(num_dice, num_faces);
+  std::vector<cfrb::TreeTemplate> tmpl;
+  for (int rb = -1; rb <= g.A - 2; ++rb) tmpl.push_back(cfrb::build_template(g, rb, max_depth));
+  std::vector<int> tm(n);
+  for (int k = 0; k < n; ++k) {
+    if (last_bid[k] < -1 || last_bid[k] > g.A - 2) return fail(CFRB_EINVAL, "subgame root bid out of range (terminal or invalid)");
+    tm[k] = last_bid[k] + 1;
+    if (cost) cost[k] = cfrb::schedule_cost(tmpl[tm[k]], g.H);
+  }
+  cfrb::schedule_order(cfrb::schedule_ranks(tmpl, g.H), tm.data(), n, order);
+  return CFRB_OK;
+}
+
+// Test aid: a persistent grid of at most max_ctas CTAs makes every warp of the depth-2 kernel solve many subgames per launch.
+// Graphs bake the grid in, so they are dropped.
+int cfrb_debug_d2_grid(cfrb_handle* h, int32_t max_ctas) {
+  if (!h || max_ctas < 0) return fail(CFRB_EINVAL, "bad argument");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());
+  for (auto& e : h->graphs) cudaGraphExecDestroy(e.exec);
+  h->graphs.clear(); h->graph_seen.clear();
+  h->d2_grid_cap = max_ctas;
+  return h->d2_ctas;
 }
 
 // Development / test aid: div_by_rcp (reciprocal + two fused-multiply-add corrections, cfr_kernels.cuh; the regret matching of
@@ -1914,6 +1972,7 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
       int rc = DISPATCH_REAL(h, lbr_begin_t, m, st);
       if (rc) return rc;
       h->n = h->cfg.max_subgames; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
+      h->sorted = false;
       if ((rc = DISPATCH_REAL(h, launch_init_t, h, st))) return rc;
       if ((rc = cfrb_run(h, h->cfg.num_iters, st))) return rc;
       CK(cudaMemsetAsync(m->left.p, 0, sizeof(int), st));
@@ -1930,6 +1989,7 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
     if (rc) return rc;
     for (cfrb_handle* h : m->h) {
       h->n = m->S; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
+      h->sorted = false;
       if ((rc = DISPATCH_REAL(h, launch_init_t, h, st))) return rc;
       if ((rc = cfrb_run(h, h->cfg.num_iters, st))) return rc;
     }
@@ -2442,6 +2502,7 @@ static int agent_solve(cfrb_agent* a, const cfrb::AgentDev& d, int n, const int3
   int rc = DISPATCH_REAL(h, agent_begin_t, a, d, st);
   if (rc) return rc;
   h->n = n_solve; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
+  h->sorted = false;
   CK(cudaEventRecord(a->ev[0], st));
   if ((rc = DISPATCH_REAL(h, launch_init_t, h, st))) return rc;
   if ((rc = cfrb_run(h, h->cfg.num_iters, st))) return rc;

@@ -10,7 +10,8 @@
 //   sp_advance    per game: br_sampler / eps / hand / action draws, sampling-belief and real-belief updates with
 //                 eps-normalisation, next public state (or a fresh game after a terminal state)
 //   sp_begin      per game: act_iteration ~ U{0..num_iters} and the descriptor of its next subgame (template, player, beliefs)
-//   sp_scan       prefix sum of the pseudo-leaf counts -> packed value-net row offsets, wave size, total rows
+//   sp_scan       prefix sum of the pseudo-leaf counts -> packed value-net row offsets, wave size, total rows; the CFR
+//                 kernel's schedule (wave positions, costliest template first)
 //
 // Every game owns a std::mt19937 stream (state words interleaved [624][K] so that the threads of a warp touch consecutive
 // addresses) and the libstdc++ distributions the reference uses are restated bit for bit (uniform_int_distribution = Lemire's
@@ -136,6 +137,26 @@ __global__ void __launch_bounds__(1024) sp_scan_kernel(SpDev p) {
   int off = part[t] - s;
   for (int g = b; g < e; ++g) { p.sg_row_off[g] = off; off += p.tmpl[p.sg_tmpl[g]].L; }
   if (t == 1023) { p.wave[0] = p.K; p.wave[1] = part[1023]; }
+  // The CFR kernel's schedule: the wave positions in template-rank order, a stable counting sort (schedule_order, cfr_tree.h)
+  // with one block-wide exclusive scan of the per-thread counts per rank.  part[] is reused for the 32 warp totals.
+  const int lane = t & 31, warp = t >> 5;
+  int base = 0;
+  for (int r = 0; r < p.A; ++r) {
+    int c = 0;
+    for (int g = b; g < e; ++g) c += p.tmpl_rank[p.sg_tmpl[g]] == r;
+    int x = c;                                   // inclusive scan within the warp
+    for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d) x += y; }
+    __syncthreads();                             // the previous rank's reads of part[] are done
+    if (lane == 31) part[warp] = x;
+    __syncthreads();
+    int wsum = part[lane];                       // inclusive scan of the warp totals, in every warp
+    for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(0xffffffffu, wsum, d); if (lane >= d) wsum += y; }
+    const int before = __shfl_sync(0xffffffffu, wsum, (warp + 31) & 31);
+    int pos = base + (warp ? before : 0) + x - c;
+    for (int g = b; g < e; ++g)
+      if (p.tmpl_rank[p.sg_tmpl[g]] == r) p.sg_order[pos++] = g;
+    base += __shfl_sync(0xffffffffu, wsum, 31);
+  }
 }
 
 // update_value_network (subgame_solving.cc:672-676, add_training_example :220-226) of every finished subgame: for traverser
