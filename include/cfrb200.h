@@ -256,7 +256,10 @@ int cfrb_selfplay_create(cfrb_handle* h, int32_t n_games, const uint32_t* seeds,
  *   1. if a wave is pending: its 2 * n_games training examples are written to the DEVICE buffers dev_ex_q [2n][Q] /
  *      dev_ex_v [2n][H] (both NULL = drop them) and every game samples its next public state (a finished game restarts);
  *   2. if start_next != 0: act_iteration draws, subgame descriptors, CFR constructor and num_iters iterations of the next wave.
- * Returns the number of example rows written (0 or 2 * n_games) or a negative error. */
+ * Returns the number of example rows written (0 or 2 * n_games) or a negative error.
+ * A CFR wave started here does not maintain the sum strategy, which the loop never reads.  The readers of it (cfrb_fetch's avg /
+ * sum, cfrb_fetch_compact 2 / 4, cfrb_load_state) first rebuild it bit for bit by solving the wave again on the handle's stream,
+ * which costs about one wave; they return CFRB_EINVAL instead when cfrb_set_weights has been called since the wave was solved. */
 int cfrb_selfplay_wave(cfrb_handle* h, float* dev_ex_q, float* dev_ex_v, int32_t start_next, void* cuda_stream);
 /* Block until the examples written by the most recent cfrb_selfplay_wave are complete (the wave it started keeps running). */
 int cfrb_selfplay_wait_examples(cfrb_handle* h);

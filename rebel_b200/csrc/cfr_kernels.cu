@@ -70,14 +70,20 @@ void regret_launch(const RegretDev& r, const float* s32, const double* s64, int 
 template <typename real>
 cudaError_t cfr_configure_d2(int H, int threads, int smem_bytes, int* ctas_per_sm) {
   cudaError_t e = cudaSuccess;
-#define CFRB_CFG(HC)                                                                                                      \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+#define CFRB_CFG(HC)                                                                                                                  \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
   CFRB_CFG(0) CFRB_CFG(4) CFRB_CFG(5) CFRB_CFG(6) CFRB_CFG(9) CFRB_CFG(16)
 #undef CFRB_CFG
   if (e != cudaSuccess) return e;
-#define CFRB_OCC(HC) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, cfr_iter_d2_kernel<real, HC>, threads, smem_bytes)
+  // the persistent grid of both variants (with and without the sum table): the smaller residency
+  int keep = 0, drop = 0;
+#define CFRB_OCC(HC)                                                                                                      \
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&keep, cfr_iter_d2_kernel<real, HC, true>, threads, smem_bytes);     \
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&drop, cfr_iter_d2_kernel<real, HC, false>, threads, smem_bytes);
   CFRB_DISPATCH_H(H, CFRB_OCC)
 #undef CFRB_OCC
+  *ctas_per_sm = std::min(keep, drop);
   return e;
 }
 
@@ -97,9 +103,15 @@ static void launch_pdl(void (*kernel)(KArgs...), int blocks, int threads, size_t
 template <typename real>
 void cfr_launch_iter_d2(const CfrDev<real>& p, int blocks, int threads, size_t smem, cudaStream_t st, int iter, int do_b, int do_f,
                         int scratch_per_group) {
-#define CFRB_CALL(HC) launch_pdl(cfr_iter_d2_kernel<real, HC>, blocks, threads, smem, st, p, iter, do_b, do_f, scratch_per_group)
-  CFRB_DISPATCH_H(p.H, CFRB_CALL)
-#undef CFRB_CALL
+#define CFRB_KEEP(HC) launch_pdl(cfr_iter_d2_kernel<real, HC, true>, blocks, threads, smem, st, p, iter, do_b, do_f, scratch_per_group)
+#define CFRB_DROP(HC) launch_pdl(cfr_iter_d2_kernel<real, HC, false>, blocks, threads, smem, st, p, iter, do_b, do_f, scratch_per_group)
+  if (p.keep_sum || p.fp) {
+    CFRB_DISPATCH_H(p.H, CFRB_KEEP)
+  } else {
+    CFRB_DISPATCH_H(p.H, CFRB_DROP)
+  }
+#undef CFRB_KEEP
+#undef CFRB_DROP
 }
 
 void sp_launch_seed(const SpDev& p, const uint32_t* dev_seeds, cudaStream_t st) {

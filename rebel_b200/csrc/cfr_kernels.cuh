@@ -313,7 +313,7 @@ __device__ void cfr_backward(const CfrDev<real>& p, int k, int trav, real* val, 
                                             : (sum > 0 ? rmax0(r) / sum : (real)1 / nchild[par]);
         Sg[e] = sg;
         R[e] = r * (r > 0 ? pos : neg);
-        S[e] = S[e] * strat + rn * sg;
+        if (p.keep_sum) S[e] = S[e] * strat + rn * sg;
         rt[c * H + h] = rn * sg;
       }
     } else {
@@ -515,7 +515,9 @@ __device__ __forceinline__ const real* d2_reach_row(const real* slot, const real
   return player == rp ? slot + parent[n] * H : slot + n * H;                    // level 2
 }
 
-template <typename real, int HC>
+// KEEP: maintain the sum table S (CfrDev::keep_sum, a compile-time copy: the kernel without it is a separate instantiation, and a
+// run-time test in the last loop costs the kernel spills)
+template <typename real, int HC, bool KEEP>
 __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2Levels& lv, int k, int trav, real* val, const real* bel, real* rcp, int lane) {
   constexpr int G = 32;
   const int H = HC > 0 ? HC : p.H;
@@ -620,13 +622,14 @@ __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2
   for (int it = lane; it < (ce - cb) * H; it += G) {
     const int c = cb + it / H, h = it % H;
     const int e = (c - 1) * H + h, par = parent[c];
-    const real s_old = __ldg(S + e);
+    real s_old = 0;
+    if constexpr (KEEP) s_old = __ldg(S + e);
     const real r = val[c * H + h], sum = val[par * H + h], rn = bt[h];
     const real sg = Eps<real>::kLiteral ? div_by_rcp(r > Eps<real>::v ? r : Eps<real>::v, sum, rcp[par * H + h])
                                         : (sum > 0 ? rmax0(r) / sum : (real)1 / nchild[par]);
     Sg[e] = sg;
     R[e] = r * (r > 0 ? pos : neg);
-    S[e] = s_old * strat + rn * sg;
+    if constexpr (KEEP) S[e] = s_old * strat + rn * sg;
     val[c * H + h] = rn * sg;
   }
   if (lane == 0) p.steps[2 * k + trav] = s + 1;
@@ -927,8 +930,8 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
 // Persistent warps: the grid holds at most the warps that are resident at once, and each warp solves subgames one after the
 // other until the wave is exhausted.  Warp w starts with ticket w and draws its later tickets from p.ticket; ticket i is the
 // subgame at wave position sg_order[i], so the costliest subgames start first and the cheapest fill the tail (longest
-// processing time first).  A subgame's results do not depend on which warp solves it or when.
-template <typename real, int HC>
+// processing time first).  A subgame's results do not depend on which warp solves it or when.  KEEP == p.keep_sum.
+template <typename real, int HC, bool KEEP>
 __global__ void __launch_bounds__(128, 8) cfr_iter_d2_kernel(CfrDev<real> p, int iter, int do_b, int do_f, int scratch_per_group) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // Programmatic dependent launch: the value-net kernel that follows may be scheduled as soon as every CTA of this grid has
@@ -965,7 +968,7 @@ __global__ void __launch_bounds__(128, 8) cfr_iter_d2_kernel(CfrDev<real> p, int
       const int lines = ((t.N - 1) * H * (int)sizeof(real) + 127) >> 7;
       const char* sg = reinterpret_cast<const char*>(p.Sg) + off;
       for (int i = lane; i < lines; i += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(sg + ((size_t)i << 7)));
-      if (do_b) {   // regrets and sum strategy: only the edges below the previous traverser's level are touched
+      if (do_b) {   // regrets and sum strategy (when kept): only the edges below the previous traverser's level are touched
         const bool root_acts = p.sg_player[k] == ((iter - 1) & 1);
         const int e0 = (root_acts ? lv.n1b : lv.n1e) - 1, e1 = (root_acts ? lv.n1e : lv.n2e) - 1;
         const size_t b0 = (size_t)e0 * H * sizeof(real) & ~(size_t)127, b1 = (size_t)e1 * H * sizeof(real);
@@ -973,7 +976,7 @@ __global__ void __launch_bounds__(128, 8) cfr_iter_d2_kernel(CfrDev<real> p, int
         const char* ss = reinterpret_cast<const char*>(p.S) + off;
         for (size_t o = b0 + ((size_t)lane << 7); o < b1; o += (size_t)32 << 7) {
           asm volatile("prefetch.global.L2 [%0];" ::"l"(rr + o));
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(ss + o));
+          if (KEEP) asm volatile("prefetch.global.L2 [%0];" ::"l"(ss + o));
         }
       }
     }
@@ -985,7 +988,7 @@ __global__ void __launch_bounds__(128, 8) cfr_iter_d2_kernel(CfrDev<real> p, int
     const int rp = p.sg_player[k];
     if (do_b) {
       if (p.fp) fp_backward_d2<real, HC>(p, t, lv, k, tb, slot, bel, lane);
-      else cfr_backward_d2<real, HC>(p, t, lv, k, tb, slot, bel, aux, lane);
+      else cfr_backward_d2<real, HC, KEEP>(p, t, lv, k, tb, slot, bel, aux, lane);
     }
     // sampling-strategy snapshot for RlRunner (recursive_solving.cc:168-174): state after `iter` iterations
     if (p.sg_act_iter[k] == iter) {
@@ -1048,7 +1051,7 @@ __global__ void __launch_bounds__(512) cfr_init_kernel(CfrDev<real> p, int scrat
       Sg[e] = u;
       if (snap0) Sn[e] = u;
       R[e] = p.fp ? u : (real)0;       // FP: last_strategies starts as the uniform strategy (subgame_solving.cc:375-377)
-      S[e] = u * (actor == 0 ? a0 : a1);
+      if (p.keep_sum) S[e] = u * (actor == 0 ? a0 : a1);
       reach0[c * H + h] = actor == 0 ? a0 * u : a0;
       reach1[c * H + h] = actor == 1 ? a1 * u : a1;
     }

@@ -45,6 +45,8 @@ struct CfrDev {
   int linear, dcfr; real dcfr_alpha, dcfr_beta, dcfr_gamma;
   int use_net;
   int fp, optimistic;             // fictitious play instead of CFR (FP, subgame_solving.cc:364-506)
+  int keep_sum;                   // CFR: 1 = maintain S (sum_strategies); 0 = neither read nor write it (a self-play wave, whose
+                                  // loop never reads it).  FP always keeps it: its average strategy is computed from S.
 };
 
 // Scratch of a group (reals): bufA[N*H] | bufB[N*H] | hist[10*T] | lsum[2*L]  (hist: per-terminal match-count histogram,

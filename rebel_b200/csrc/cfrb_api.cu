@@ -164,9 +164,9 @@ struct cfrb_handle {
   std::vector<Event> net_ev;   // pairs around value-net launches (profiling mode)
   int net_ev_used = 0;
   // CUDA graphs of whole cfrb_run calls (2 launches per iteration would otherwise be enqueued one by one by the host)
-  struct GraphEntry { int first, count, prof, has_rows, sorted; GraphExec exec; int launches, net_launches, ev_used; };
+  struct GraphEntry { int first, count, prof, has_rows, sorted, keep_sum; GraphExec exec; int launches, net_launches, ev_used; };
   std::vector<GraphEntry> graphs;
-  std::vector<std::array<int, 5>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
+  std::vector<std::array<int, 6>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
   bool capturing = false;           // launch geometry independent of the wave size while a graph is being captured / replayed
   // device: templates
   DevBuf<cfrb::TemplateDev> d_tmpl;
@@ -214,6 +214,11 @@ struct cfrb_handle {
   cfrb::NetDev net{};
   bool have_weights = false;
   uint64_t weights_version = 0;
+  uint64_t weight_uploads = 0;       // cfrb_set_weights calls so far
+  // The current wave is a CFR self-play wave, solved without the sum table S (the self-play loop never reads it).  Readers of S
+  // rebuild it first (materialise_sum), which needs the weights that wave was solved with: upload count sum_uploads.
+  bool sum_dropped = false;
+  uint64_t sum_uploads = 0;
   // host mirror of the wave
   int n = 0, rows = 0, iters_done = 0;
   std::vector<int> h_tmpl, h_player, h_row_off, h_last_bid;
@@ -283,6 +288,7 @@ static int alloc_state(cfrb_handle* h, WaveState<real>& s, int max_optin) {
   CK(cudaMemset(s.vterm.p, 0, ((size_t)K * vterm_stride + 8) * sizeof(real)));
   CK(cudaMemset(s.scaler.p, 0, (rows_cap + 8) * sizeof(real)));
   CK(cudaMemset(s.Snap.p, 0, tab * sizeof(real)));
+  CK(cudaMemset(s.S.p, 0, tab * sizeof(real)));   // self-play waves leave S alone: its entries outside a wave's trees stay defined
   const size_t per_group_bytes = (size_t)h->scratch_per_group * sizeof(real);
   if (per_group_bytes * 2 <= (size_t)max_optin) {
     h->group = 32;
@@ -331,7 +337,16 @@ static int alloc_state(cfrb_handle* h, WaveState<real>& s, int max_optin) {
   d.dcfr_alpha = (real)h->cfg.dcfr_alpha; d.dcfr_beta = (real)h->cfg.dcfr_beta; d.dcfr_gamma = (real)h->cfg.dcfr_gamma;
   d.use_net = h->cfg.net_mode != CFRB_NET_ZERO;
   d.fp = h->cfg.solver == CFRB_SOLVER_FP; d.optimistic = h->cfg.optimistic;
+  d.keep_sum = 1;
   return CFRB_OK;
+}
+
+// The kernel parameters of the current wave.
+template <typename real>
+static cfrb::CfrDev<real> wave_dev(const cfrb_handle* h, const WaveState<real>& s) {
+  cfrb::CfrDev<real> d = s.dev;
+  d.keep_sum = !h->sum_dropped;
+  return d;
 }
 
 static int launch_init(cfrb_handle* h, cudaStream_t st) {
@@ -339,7 +354,7 @@ static int launch_init(cfrb_handle* h, cudaStream_t st) {
   with_state(h, [&](auto& s) {
     using real = typename std::decay_t<decltype(s)>::real;
     const size_t smem = h->group == 32 ? (size_t)h->scratch_per_group * sizeof(real) * h->groups_per_cta : 0;
-    cfrb::cfr_launch_init<real>(s.dev, h->group, blocks, 32 * h->groups_per_cta, smem, st, h->scratch_per_group);
+    cfrb::cfr_launch_init<real>(wave_dev(h, s), h->group, blocks, 32 * h->groups_per_cta, smem, st, h->scratch_per_group);
   });
   ++h->launches;
   CK(cudaGetLastError());
@@ -349,17 +364,17 @@ static int launch_init(cfrb_handle* h, cudaStream_t st) {
 template <typename real>
 static int launch_iter(cfrb_handle* h, WaveState<real>& s, cudaStream_t st, int iter, int do_b, int do_f) {
   const int nsg = h->capturing ? h->cfg.max_subgames : h->n;   // surplus groups return at once (k >= *wave_n)
+  cfrb::CfrDev<real> d = wave_dev(h, s);
   if (h->d2) {
     // persistent warps: no more CTAs than are resident at once (the warps then take the wave's subgames from a counter)
     int blocks = std::min((nsg + h->d2_groups_per_cta - 1) / h->d2_groups_per_cta, h->d2_ctas);
     if (h->d2_grid_cap > 0) blocks = std::min(blocks, h->d2_grid_cap);
-    cfrb::CfrDev<real> d = s.dev;
     d.sg_order = h->sorted ? h->d_sg_order.p : nullptr;
     cfrb::cfr_launch_iter_d2<real>(d, blocks, 32 * h->d2_groups_per_cta, h->d2_smem, st, iter, do_b, do_f, h->d2_scratch_per_group);
   } else {
     const int blocks = (nsg + h->groups_per_cta - 1) / h->groups_per_cta;
     const size_t smem = h->group == 32 ? (size_t)h->scratch_per_group * sizeof(real) * h->groups_per_cta : 0;
-    cfrb::cfr_launch_iter<real>(s.dev, h->group, blocks, 32 * h->groups_per_cta, smem, st, iter, do_b, do_f, h->scratch_per_group);
+    cfrb::cfr_launch_iter<real>(d, h->group, blocks, 32 * h->groups_per_cta, smem, st, iter, do_b, do_f, h->scratch_per_group);
   }
   ++h->launches;
   CK(cudaGetLastError());
@@ -425,9 +440,33 @@ static int normalise_avg(cfrb_handle* h, double* tab) {
   return CFRB_OK;
 }
 
+// Rebuilds the sum table of a wave solved without it (sum_dropped): replays the wave from cfr_init with S kept, on the handle's
+// stream, from the wave's own descriptors (roots, players, beliefs, act_iterations, row offsets, schedule), which stay on the device
+// until the next wave is built.  The solve is deterministic, so R, Sg, Snap, mu and the step counters are rewritten with the bits
+// they hold, and S comes out as a wave that kept it would have left it.  Refused when the value-net weights have been replaced since
+// the wave was solved: the replay would solve a different wave.
+static int materialise_sum(cfrb_handle* h) {
+  if (!h->sum_dropped) return CFRB_OK;
+  if (h->weight_uploads != h->sum_uploads)
+    return fail(CFRB_EINVAL, "the sum strategy of this self-play wave was not kept, and it cannot be rebuilt: the value-net weights "
+                             "have been replaced (cfrb_set_weights) since the wave was solved");
+  const int iters = h->iters_done;
+  h->sum_dropped = false;
+  h->iters_done = 0;
+  int rc = launch_init(h, h->own_stream);
+  if (!rc) rc = cfrb_run(h, iters, h->own_stream);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(h->own_stream));
+  return CFRB_OK;
+}
+
 // The current wave's compact tables [n][table_stride] as doubles.  which: 0 = Snap, 1 = Sg, 2 = S, 3 = R, 4 = the average
 // strategy (avg_table, normalised where it is a sum).
 static int pull_table(cfrb_handle* h, int which, double* out) {
+  if (which == 2 || which == 4) {
+    const int rc = materialise_sum(h);
+    if (rc) return rc;
+  }
   bool normalise = false;
   int rc = with_state(h, [&](auto& s) {
     const auto avg = avg_table(h, s);
@@ -799,6 +838,7 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
   h->w_last = h->w_ev[slot];
   h->have_weights = true;
   h->weights_version = version;
+  ++h->weight_uploads;
   return CFRB_OK;
 }
 
@@ -824,6 +864,7 @@ int cfrb_begin_wave(cfrb_handle* h, int32_t n, const int32_t* last_bid, const in
   std::vector<int> order(n);
   cfrb::schedule_order(h->tmpl_rank, tm.data(), n, order.data());
   h->n = n; h->rows = rows; h->iters_done = 0; h->rows_on_device = false; h->sp.pending = false; h->sorted = true;
+  h->sum_dropped = false;
   h->h_tmpl = tm; h->h_player = pl; h->h_row_off = ro;
   h->h_last_bid.assign(last_bid, last_bid + n);
   h->h_beliefs.assign(beliefs, beliefs + (size_t)n * 2 * H);
@@ -913,6 +954,7 @@ int cfrb_reset_wave(cfrb_handle* h, void* cuda_stream) {
   if (!h) return fail(CFRB_EINVAL, "null handle");
   CK(cudaSetDevice(h->cfg.device));
   h->iters_done = 0;
+  h->sum_dropped = false;   // a wave the host runs again keeps its sum
   if (h->n == 0) return CFRB_OK;
   return launch_init(h, cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream);
 }
@@ -949,19 +991,20 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
   const int first = h->iters_done, last = first + iters;
   // Long runs are replayed from a CUDA graph: one host call instead of 2 * iters kernel launches, so a busy or slow host
   // thread cannot starve the GPU.  The graph bakes in the iteration indices and a wave-size-independent launch geometry; it
-  // is keyed by (first iteration, count, profiling period, "the wave has value-net rows", "the wave has a schedule").  The fp32 parity net sizes its grid
-  // by the row count and stays on the eager path, like short runs.
+  // is keyed by (first iteration, count, profiling period, "the wave has value-net rows", "the wave has a schedule", "the wave keeps
+  // the sum table").  The fp32 parity net sizes its grid by the row count and stays on the eager path, like short runs.
   static const bool no_graph = [] { const char* e = std::getenv("CFRB_NO_GRAPH"); return e && *e == '1'; }();
   const bool graphable = !no_graph && iters >= 64 && h->cfg.net_mode != CFRB_NET_FP32;
   if (graphable) {
-    const int has_rows = h->rows > 0 || h->rows_on_device, sorted = h->sorted;
+    const int has_rows = h->rows > 0 || h->rows_on_device, sorted = h->sorted, keep_sum = !h->sum_dropped;
     cfrb_handle::GraphEntry* g = nullptr;
     for (auto& e : h->graphs)
-      if (e.first == first && e.count == iters && e.prof == h->profiling && e.has_rows == has_rows && e.sorted == sorted) { g = &e; break; }
+      if (e.first == first && e.count == iters && e.prof == h->profiling && e.has_rows == has_rows && e.sorted == sorted &&
+          e.keep_sum == keep_sum) { g = &e; break; }
     if (!g) {
       // capture + instantiation of ~2 * iters nodes costs ~0.1 s: only worth it for a key that repeats (waves of a self-play
       // loop, bench steps), not for one-off run lengths (e.g. the evaluator's per-chunk act_iteration maxima)
-      const std::array<int, 5> key{first, iters, h->profiling, has_rows, sorted};
+      const std::array<int, 6> key{first, iters, h->profiling, has_rows, sorted, keep_sum};
       bool seen = false;
       for (const auto& k : h->graph_seen) seen |= k == key;
       if (!seen) {
@@ -989,7 +1032,8 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
       h->launches = l0;
       if (rc == CFRB_OK && ce == cudaSuccess && exec) {
         if (h->graphs.size() >= 8) h->graphs.erase(h->graphs.begin());
-        h->graphs.push_back({first, iters, h->profiling, has_rows, sorted, std::move(exec), captured, h->net_launches_run, h->net_ev_used});
+        h->graphs.push_back({first, iters, h->profiling, has_rows, sorted, keep_sum, std::move(exec), captured, h->net_launches_run,
+                             h->net_ev_used});
         g = &h->graphs.back();
       } else {
         cudaGetLastError();   // the stream could not be captured (e.g. a legacy stream): run eagerly
@@ -1096,6 +1140,7 @@ int cfrb_load_state(cfrb_handle* h, const double* regrets, const double* last_st
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaDeviceSynchronize());
   { int rc = sync_mirror(h); if (rc) return rc; }
+  { int rc = materialise_sum(h); if (rc) return rc; }   // the tables it does not replace, S among them, stay the wave's
   int rc = with_state(h, [&](auto& s) { return load_state_t(h, s, regrets, last_strategy, sum_strategy, root_value_means); });
   if (rc) return rc;
   if (num_steps) CK(cudaMemcpy(h->d_steps.p, num_steps, (size_t)h->n * 2 * sizeof(int), cudaMemcpyHostToDevice));
@@ -1433,10 +1478,14 @@ int cfrb_last_run_ms(cfrb_handle* h, float* total_ms, float* net_ms) {
 }
 
 // Starts a wave of n subgames built on the device (its leaf rows and roots exist only there) and runs num_iters on it.  sorted:
-// d_sg_order holds the wave's schedule; otherwise the depth-2 kernel takes wave order.
-static int solve_device_wave(cfrb_handle* h, int n, bool sorted, cudaStream_t st) {
+// d_sg_order holds the wave's schedule; otherwise the depth-2 kernel takes wave order.  drop_sum: a self-play wave, whose loop
+// reads the snapshots and root means only; CFR then leaves the sum table alone (materialise_sum rebuilds it for a reader).  Match,
+// LBR and agent waves keep it: they act with the average strategy of the wave they have just solved (act_slot).
+static int solve_device_wave(cfrb_handle* h, int n, bool sorted, bool drop_sum, cudaStream_t st) {
   h->n = n; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
   h->sorted = sorted;
+  h->sum_dropped = drop_sum && h->cfg.solver == CFRB_SOLVER_CFR;
+  h->sum_uploads = h->weight_uploads;
   const int rc = launch_init(h, st);
   return rc ? rc : cfrb_run(h, h->cfg.num_iters, st);
 }
@@ -1493,7 +1542,7 @@ int cfrb_selfplay_wave(cfrb_handle* h, float* dev_ex_q, float* dev_ex_v, int32_t
     with_state(h, [&](auto& s) { cfrb::sp_launch_begin(h->sp.dev, s.beliefs.p, st); });
     h->launches += 2;
     CK(cudaGetLastError());
-    const int rc = solve_device_wave(h, h->sp.K, true, st);
+    const int rc = solve_device_wave(h, h->sp.K, true, true, st);
     if (rc) return rc;
     h->sp.pending = true;
     ++h->sp.waves;
@@ -1894,7 +1943,7 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
     if (rc) return rc;
     // one wave per agent; LBR: one wave of at most max_subgames subgames of the agent
     for (cfrb_handle* h : m->h)
-      if (h && (rc = solve_device_wave(h, m->lbr ? h->cfg.max_subgames : m->S, false, st))) return rc;
+      if (h && (rc = solve_device_wave(h, m->lbr ? h->cfg.max_subgames : m->S, false, false, st))) return rc;
     CK(cudaMemsetAsync(m->left.p, 0, sizeof(int), st));
     if ((rc = match_kernels(m, false, st))) return rc;
     m->h[0]->launches += 3;
@@ -2356,7 +2405,7 @@ static int agent_solve(cfrb_agent* a, const cfrb::AgentDev& d, int n, const int3
   int rc = launch(true);
   if (rc) return rc;
   CK(cudaEventRecord(a->ev[0], st));
-  if ((rc = solve_device_wave(h, n_solve, false, st))) return rc;
+  if ((rc = solve_device_wave(h, n_solve, false, false, st))) return rc;
   CK(cudaEventRecord(a->ev[1], st));
   if ((rc = launch(false))) return rc;
   h->launches += 3;
