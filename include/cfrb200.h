@@ -419,6 +419,47 @@ int cfrb_dev_alloc(int32_t device, size_t bytes, void** out);
 int cfrb_dev_free(int32_t device, void* p);
 int cfrb_dev_to_host(int32_t device, void* dst, const void* src, size_t bytes);
 
+/* ---- Value-net training: one optimisation step of the reference trainer (cfvpy/selfplay.py:409-438) for the net the kernels
+ * evaluate, Net2(n_hidden=256, n_layers=2, use_layer_norm=True), on a batch of n <= max_batch examples: forward (Linear ->
+ * LayerNorm(eps 1e-5) -> erf GELU, twice, then Linear), the loss averaged over the H outputs and then over the batch
+ * (selfplay.py:135-149), backward through every parameter, clip_grad_norm_ (selfplay.py:636-651: total = 2-norm of the
+ * per-parameter 2-norms, gradients scaled by max_norm / (total + 1e-6) when that is < 1; max_norm <= 0 = no clipping) and
+ * torch.optim.Adam with its defaults (betas 0.9 / 0.999, eps 1e-8, no weight decay, bias correction).  fp32 operands and
+ * accumulation, no atomics: the same state and batch give the same bits on every run, eagerly or replayed from a CUDA graph.
+ * The trainer owns its parameters, gradients, Adam moments, step count and scratch on one device; a trainer is not thread-safe,
+ * and since steps and losses share its scratch, all calls on one trainer must be ordered: enqueue them on one stream, or order
+ * the streams (events) yourself.
+ * Parameters and moments cross the boundary as flat fp32 buffers in the cfrb_set_weights layout. */
+typedef struct cfrb_trainer cfrb_trainer;
+enum {
+  CFRB_LOSS_HUBER = 0,   /* (|x| > 1)(2|x| - 1) + (|x| <= 1) x^2 of x = values - net(query) */
+  CFRB_LOSS_MSE = 1      /* x^2 */
+};
+/* Parameters, moments and step count start at zero (cfrb_trainer_set_state installs a net). */
+int cfrb_trainer_create(int32_t device, int32_t num_dice, int32_t num_faces, int32_t max_batch, cfrb_trainer** out);
+int cfrb_trainer_destroy(cfrb_trainer* t);
+/* Number of floats of the flat parameter buffer (= of each Adam moment). */
+int64_t cfrb_trainer_num_params(const cfrb_trainer* t);
+/* Host buffers of cfrb_trainer_num_params floats; m / v NULL = zero moments.  step = Adam steps already taken.  Synchronises
+ * the device. */
+int cfrb_trainer_set_state(cfrb_trainer* t, const float* params, const float* m, const float* v, int64_t step);
+/* Any pointer may be NULL.  Synchronises the device. */
+int cfrb_trainer_get_state(cfrb_trainer* t, float* params, float* m, float* v, int64_t* step);
+/* One step on the batch dev_q [n][Q], dev_v [n][H] (row-major fp32, memory of the trainer's device), enqueued on `cuda_stream`
+ * (a cudaStream_t; NULL = the legacy default stream) with no host<->device copy and no synchronisation.  lr is the learning rate
+ * of this step (the host halves it on its schedule).  dev_out (device memory, may be NULL) receives {loss, pre-clip grad norm,
+ * loss of row 0, .., loss of row n-1} (row loss = mean over the H outputs) once the stream gets there.  Arguments are checked
+ * before anything is enqueued: a refused call leaves the trainer unchanged. */
+int cfrb_trainer_step(cfrb_trainer* t, const float* dev_q, const float* dev_v, int32_t n, double lr, double max_norm, int32_t loss_kind,
+                      void* cuda_stream, float* dev_out);
+/* Forward pass and loss only (validation sets), on `cuda_stream`: dev_out [2 + n] receives {loss, unused, row losses}. */
+int cfrb_trainer_loss(cfrb_trainer* t, const float* dev_q, const float* dev_v, int32_t n, int32_t loss_kind, void* cuda_stream,
+                      float* dev_out);
+/* Loss and pre-clip grad norm of the most recent cfrb_trainer_step.  Synchronises the device. */
+int cfrb_trainer_last(cfrb_trainer* t, float* loss, float* grad_norm);
+/* Test aid: the gradients of the most recent step after clipping, flat [cfrb_trainer_num_params].  Synchronises the device. */
+int cfrb_trainer_debug_grads(cfrb_trainer* t, float* out);
+
 /* ---- One process per GPU: the two hand-overs the reference performs through shared host memory inside ONE process become NCCL
  * collectives over NVLink, issued by this library on device buffers (no torch.distributed, no host bounce):
  *   ModelLocker::updateModel (rela/model_locker.h:69-79)         -> cfrb_comm_broadcast_weights

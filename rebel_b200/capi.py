@@ -113,6 +113,16 @@ def lib():
     L.cfrb_match_create_lbr.argtypes = [vp, C.c_int32, C.c_int32, C.c_uint64, C.POINTER(vp)]
     L.cfrb_match_lbr_trace.argtypes = [vp, C.c_int32, _dp, _dp]
     L.cfrb_match_lbr_counts.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    L.cfrb_trainer_create.argtypes = [C.c_int32] * 4 + [C.POINTER(vp)]
+    L.cfrb_trainer_destroy.argtypes = [vp]
+    L.cfrb_trainer_num_params.argtypes = [vp]
+    L.cfrb_trainer_num_params.restype = C.c_int64
+    L.cfrb_trainer_set_state.argtypes = [vp, _fp, _fp, _fp, C.c_int64]
+    L.cfrb_trainer_get_state.argtypes = [vp, _fp, _fp, _fp, C.POINTER(C.c_int64)]
+    L.cfrb_trainer_step.argtypes = [vp, vp, vp, C.c_int32, C.c_double, C.c_double, C.c_int32, vp, vp]
+    L.cfrb_trainer_loss.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, vp, vp]
+    L.cfrb_trainer_last.argtypes = [vp, _fp, _fp]
+    L.cfrb_trainer_debug_grads.argtypes = [vp, _fp]
     _lib = L
     return L
 

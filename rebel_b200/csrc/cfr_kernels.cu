@@ -24,16 +24,27 @@ namespace cfrb {
     default: { CALL(0); break; }          \
   }
 
+// The dynamic shared-memory limit is an attribute of the kernel, shared by every handle of the process: each handle raises it to
+// the device's opt-in maximum, so that a handle created later with a smaller need (another game or tree depth, e.g. an
+// exploitability evaluation beside running generator loops) cannot lower it under the launches of an earlier one.
+static int smem_limit(int smem_bytes) {
+  int dev = 0, optin = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
+    return smem_bytes;
+  return std::max(smem_bytes, optin);
+}
+
 template <typename real>
 cudaError_t cfr_configure(int group, int smem_bytes) {
   if (group != 32) return cudaSuccess;
   cudaError_t e = cudaSuccess;
+  const int limit = smem_limit(smem_bytes);
 #define CFRB_CFG(HC)                                                                                                      \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_kernel<real, 32, HC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_kernel<real, 32, HC>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit);
   CFRB_CFG(0) CFRB_CFG(4) CFRB_CFG(5) CFRB_CFG(6) CFRB_CFG(9) CFRB_CFG(16)
 #undef CFRB_CFG
   if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(cfr_init_kernel<real, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+  return cudaFuncSetAttribute(cfr_init_kernel<real, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit);
 }
 
 template <typename real>
@@ -70,9 +81,10 @@ void regret_launch(const RegretDev& r, const float* s32, const double* s64, int 
 template <typename real>
 cudaError_t cfr_configure_d2(int H, int threads, int smem_bytes, int* ctas_per_sm) {
   cudaError_t e = cudaSuccess;
+  const int limit = smem_limit(smem_bytes);
 #define CFRB_CFG(HC)                                                                                                                  \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit); \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit);
   CFRB_CFG(0) CFRB_CFG(4) CFRB_CFG(5) CFRB_CFG(6) CFRB_CFG(9) CFRB_CFG(16)
 #undef CFRB_CFG
   if (e != cudaSuccess) return e;

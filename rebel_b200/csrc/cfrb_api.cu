@@ -22,6 +22,7 @@
 #include "leaf_mlp_simt.cuh"
 #include "leaf_mlp_tc.cuh"
 #include "leaf_mlp_tc_wide.cuh"
+#include "train_kernels.cuh"
 
 namespace {
 inline bool is_tc(int net_mode) { return net_mode == CFRB_NET_TC_F16 || net_mode == CFRB_NET_TC_F16X2; }
@@ -667,10 +668,11 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
     CK(h->d_Xh.alloc(tiles * cfrb::tc::kTileM * h->Qpad));
     CK(cudaMemset(h->d_Xh.p, 0, tiles * cfrb::tc::kTileM * h->Qpad * sizeof(__half)));
     CK(h->d_dbg.alloc(2 * cfrb::tc::kTileM * cfrb::tc::kHid));
+    // the limit is per kernel and process-wide: raised to the device's opt-in maximum (see cfr_configure in cfr_kernels.cu)
+    const int sm = std::max(h->tc.smem_bytes, max_optin);
     if (h->tc.wide) {
-      CK(cfrb::tc::wide_configure(h->tc.nout, h->tc.smem_bytes));
+      CK(cfrb::tc::wide_configure(h->tc.nout, sm));
     } else {
-      const int sm = h->tc.smem_bytes;
       CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
       CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
       CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
@@ -2620,6 +2622,228 @@ int cfrb_agent_counts(cfrb_agent* a, int64_t* solves, int64_t* subgame_iters) {
 int cfrb_agent_solve_ms(cfrb_agent* a, double* ms) {
   if (!a || !ms) return fail(CFRB_EINVAL, "cfrb_agent_solve_ms: null argument");
   *ms = a->solve_ms;
+  return CFRB_OK;
+}
+
+// ============================================================================================ value-net trainer
+struct cfrb_trainer {
+  int device = 0, B = 0, Q = 0, H = 0;
+  cfrb::train::Layout L;
+  DevBuf<float> params, grads, m, v;
+  DevBuf<long long> step;
+  DevBuf<float> sq_norms, last;   // sq_norms [kParams]; last = {loss, pre-clip grad norm}
+  // activations and their gradients, [B][256] unless noted
+  DevBuf<float> z1, xh1, rs1, a1, z2, xh2, rs2, a2, pred, dpred, row_loss;   // rs* [B], pred / dpred [B][H], row_loss [B]
+  DevBuf<float> da2, dy2, dz2, da1, dy1, dz1;
+};
+
+int cfrb_trainer_create(int32_t device, int32_t num_dice, int32_t num_faces, int32_t max_batch, cfrb_trainer** out) {
+  static const char* who = "cfrb_trainer_create: ";
+  if (!out) return fail(CFRB_EINVAL, std::string(who) + "null argument");
+  if (num_dice < 1 || num_faces < 1) return fail(CFRB_EINVAL, std::string(who) + "num_dice and num_faces must be >= 1");
+  if (max_batch < 1) return fail(CFRB_EINVAL, std::string(who) + "max_batch must be >= 1");
+  const cfrb::GameShape g(num_dice, num_faces);
+  if (g.A > 1024 || g.H > 4096) return fail(CFRB_EINVAL, std::string(who) + "game too large");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    return fail(CFRB_ENODEV, "no CUDA device visible: libcfrb200 has no CPU fallback");
+  }
+  if (device < 0 || device >= ndev) return fail(CFRB_EINVAL, std::string(who) + "device ordinal out of range");
+  CK(cudaSetDevice(device));
+  auto t = std::make_unique<cfrb_trainer>();
+  t->device = device; t->B = max_batch; t->Q = g.Q; t->H = g.H;
+  t->L = cfrb::train::Layout(g.Q, g.H);
+  const size_t P = (size_t)t->L.total(), BH = (size_t)max_batch * cfrb::train::kHid, BO = (size_t)max_batch * g.H;
+  cudaError_t e = cudaSuccess;
+  for (auto* b : {&t->params, &t->grads, &t->m, &t->v})
+    if (e == cudaSuccess) e = b->alloc(P);
+  for (auto* b : {&t->z1, &t->xh1, &t->a1, &t->z2, &t->xh2, &t->a2, &t->da2, &t->dy2, &t->dz2, &t->da1, &t->dy1, &t->dz1})
+    if (e == cudaSuccess) e = b->alloc(BH);
+  for (auto* b : {&t->rs1, &t->rs2, &t->row_loss})
+    if (e == cudaSuccess) e = b->alloc(max_batch);
+  for (auto* b : {&t->pred, &t->dpred})
+    if (e == cudaSuccess) e = b->alloc(BO);
+  if (e == cudaSuccess) e = t->sq_norms.alloc(cfrb::train::kParams);
+  if (e == cudaSuccess) e = t->last.alloc(2);
+  if (e == cudaSuccess) e = t->step.alloc(1);
+  for (auto* b : {&t->params, &t->grads, &t->m, &t->v})
+    if (e == cudaSuccess) e = cudaMemset(b->p, 0, P * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemset(t->last.p, 0, 2 * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemset(t->step.p, 0, sizeof(long long));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) return fail(CFRB_ENOMEM, std::string(who) + cudaGetErrorString(e));
+  *out = t.release();
+  return CFRB_OK;
+}
+
+int cfrb_trainer_destroy(cfrb_trainer* t) {
+  if (!t) return CFRB_OK;
+  cudaSetDevice(t->device);
+  cudaDeviceSynchronize();
+  delete t;
+  return CFRB_OK;
+}
+
+int64_t cfrb_trainer_num_params(const cfrb_trainer* t) { return t ? t->L.total() : 0; }
+
+int cfrb_trainer_set_state(cfrb_trainer* t, const float* params, const float* m, const float* v, int64_t step) {
+  if (!t || !params) return fail(CFRB_EINVAL, "cfrb_trainer_set_state: null argument");
+  if (step < 0) return fail(CFRB_EINVAL, "cfrb_trainer_set_state: step must be >= 0");
+  const size_t bytes = (size_t)t->L.total() * sizeof(float);
+  const long long s = step;
+  CK(cudaSetDevice(t->device));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(t->params.p, params, bytes, cudaMemcpyHostToDevice));
+  if (m) CK(cudaMemcpy(t->m.p, m, bytes, cudaMemcpyHostToDevice));
+  else CK(cudaMemset(t->m.p, 0, bytes));
+  if (v) CK(cudaMemcpy(t->v.p, v, bytes, cudaMemcpyHostToDevice));
+  else CK(cudaMemset(t->v.p, 0, bytes));
+  CK(cudaMemcpy(t->step.p, &s, sizeof(s), cudaMemcpyHostToDevice));
+  CK(cudaDeviceSynchronize());
+  return CFRB_OK;
+}
+
+int cfrb_trainer_get_state(cfrb_trainer* t, float* params, float* m, float* v, int64_t* step) {
+  if (!t) return fail(CFRB_EINVAL, "cfrb_trainer_get_state: null trainer");
+  const size_t bytes = (size_t)t->L.total() * sizeof(float);
+  CK(cudaSetDevice(t->device));
+  CK(cudaDeviceSynchronize());
+  if (params) CK(cudaMemcpy(params, t->params.p, bytes, cudaMemcpyDeviceToHost));
+  if (m) CK(cudaMemcpy(m, t->m.p, bytes, cudaMemcpyDeviceToHost));
+  if (v) CK(cudaMemcpy(v, t->v.p, bytes, cudaMemcpyDeviceToHost));
+  if (step) {
+    long long s = 0;
+    CK(cudaMemcpy(&s, t->step.p, sizeof(s), cudaMemcpyDeviceToHost));
+    *step = s;
+  }
+  return CFRB_OK;
+}
+
+int cfrb_trainer_debug_grads(cfrb_trainer* t, float* out) {
+  if (!t || !out) return fail(CFRB_EINVAL, "cfrb_trainer_debug_grads: null argument");
+  CK(cudaSetDevice(t->device));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(out, t->grads.p, (size_t)t->L.total() * sizeof(float), cudaMemcpyDeviceToHost));
+  return CFRB_OK;
+}
+
+int cfrb_trainer_last(cfrb_trainer* t, float* loss, float* grad_norm) {
+  if (!t) return fail(CFRB_EINVAL, "cfrb_trainer_last: null trainer");
+  float h[2];
+  CK(cudaSetDevice(t->device));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(h, t->last.p, sizeof(h), cudaMemcpyDeviceToHost));
+  if (loss) *loss = h[0];
+  if (grad_norm) *grad_norm = h[1];
+  return CFRB_OK;
+}
+
+// A pointer the caller says is memory of the trainer's device.
+static int trainer_check_ptr(const cfrb_trainer* t, const void* p, const std::string& what) {
+  if (!p) return fail(CFRB_EINVAL, what + " is NULL");
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(CFRB_EINVAL, what + " is not CUDA memory");
+  }
+  if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != t->device)
+    return fail(CFRB_EINVAL, what + " must be device memory of cuda:" + std::to_string(t->device) +
+                                 (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged
+                                      ? " (it is on cuda:" + std::to_string(a.device) + ")" : " (it is host memory)"));
+  return CFRB_OK;
+}
+
+static int trainer_check_batch(const cfrb_trainer* t, const char* who, const float* q, const float* v, int32_t n, int32_t loss_kind,
+                               const float* out) {
+  if (!t) return fail(CFRB_EINVAL, std::string(who) + "null trainer");
+  if (n < 1 || n > t->B)
+    return fail(CFRB_EINVAL, std::string(who) + "batch of " + std::to_string(n) + " rows, must be 1 .. max_batch = " + std::to_string(t->B));
+  if (loss_kind != cfrb::train::LOSS_HUBER && loss_kind != cfrb::train::LOSS_MSE)
+    return fail(CFRB_EINVAL, std::string(who) + "loss_kind must be CFRB_LOSS_HUBER or CFRB_LOSS_MSE");
+  int rc;
+  if ((rc = trainer_check_ptr(t, q, std::string(who) + "queries")) || (rc = trainer_check_ptr(t, v, std::string(who) + "values")))
+    return rc;
+  if (out && (rc = trainer_check_ptr(t, out, std::string(who) + "out"))) return rc;
+  return CFRB_OK;
+}
+
+// Forward pass and loss of n rows: pred, row_loss and dpred in the trainer's scratch.
+static int trainer_forward(cfrb_trainer* t, const float* q, const float* vals, int n, int loss_kind, cudaStream_t st) {
+  using namespace cfrb::train;
+  const auto& L = t->L;
+  const float* P = t->params.p;
+  const int Q = t->Q, H = t->H, rb = (n + kRowsPerBlock - 1) / kRowsPerBlock;
+  Gemm f1{q, Q, 1, P + L.off[W1], 1, Q, t->z1.p, kHid, P + L.off[B1], n, kHid, Q};
+  CK(launch_gemm(&f1, 1, st));
+  ln_gelu_fwd<<<rb, 256, 0, st>>>(t->z1.p, P + L.off[G1], P + L.off[BE1], t->xh1.p, t->rs1.p, t->a1.p, n);
+  Gemm f2{t->a1.p, kHid, 1, P + L.off[W2], 1, kHid, t->z2.p, kHid, P + L.off[B2], n, kHid, kHid};
+  CK(launch_gemm(&f2, 1, st));
+  ln_gelu_fwd<<<rb, 256, 0, st>>>(t->z2.p, P + L.off[G2], P + L.off[BE2], t->xh2.p, t->rs2.p, t->a2.p, n);
+  Gemm f3{t->a2.p, kHid, 1, P + L.off[W3], 1, kHid, t->pred.p, H, P + L.off[B3], n, H, kHid};
+  CK(launch_gemm(&f3, 1, st));
+  loss_rows<<<rb, 256, 0, st>>>(t->pred.p, vals, n, H, loss_kind, t->row_loss.p, t->dpred.p);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+
+int cfrb_trainer_step(cfrb_trainer* t, const float* dev_q, const float* dev_v, int32_t n, double lr, double max_norm, int32_t loss_kind,
+                      void* cuda_stream, float* dev_out) {
+  using namespace cfrb::train;
+  static const char* who = "cfrb_trainer_step: ";
+  int rc = trainer_check_batch(t, who, dev_q, dev_v, n, loss_kind, dev_out);
+  if (rc) return rc;
+  if (!std::isfinite(lr) || lr < 0) return fail(CFRB_EINVAL, std::string(who) + "lr must be finite and >= 0");
+  if (std::isnan(max_norm)) return fail(CFRB_EINVAL, std::string(who) + "max_norm is NaN");
+  CK(cudaSetDevice(t->device));
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  if ((rc = trainer_forward(t, dev_q, dev_v, n, loss_kind, st))) return rc;
+  const auto& L = t->L;
+  float* P = t->params.p;
+  float* G = t->grads.p;
+  const int Q = t->Q, H = t->H, rb = (n + kRowsPerBlock - 1) / kRowsPerBlock;
+  // output layer: dW3 = dpred^T a2, da2 = dpred W3
+  const Gemm b3[2] = {{t->dpred.p, 1, H, t->a2.p, kHid, 1, G + L.off[W3], kHid, nullptr, H, kHid, n},
+                      {t->dpred.p, H, 1, P + L.off[W3], kHid, 1, t->da2.p, kHid, nullptr, n, kHid, H}};
+  CK(launch_gemm(b3, 2, st));
+  ln_gelu_bwd<<<rb, 256, 0, st>>>(t->da2.p, t->xh2.p, t->rs2.p, P + L.off[G2], P + L.off[BE2], t->dy2.p, t->dz2.p, n);
+  const ColJob c2[4] = {{t->dpred.p, nullptr, G + L.off[B3], H}, {t->dy2.p, t->xh2.p, G + L.off[G2], kHid},
+                        {t->dy2.p, nullptr, G + L.off[BE2], kHid}, {t->dz2.p, nullptr, G + L.off[B2], kHid}};
+  CK(launch_colsum(c2, 4, n, st));
+  // hidden layer 2: dW2 = dz2^T a1, da1 = dz2 W2
+  const Gemm b2[2] = {{t->dz2.p, 1, kHid, t->a1.p, kHid, 1, G + L.off[W2], kHid, nullptr, kHid, kHid, n},
+                      {t->dz2.p, kHid, 1, P + L.off[W2], kHid, 1, t->da1.p, kHid, nullptr, n, kHid, kHid}};
+  CK(launch_gemm(b2, 2, st));
+  ln_gelu_bwd<<<rb, 256, 0, st>>>(t->da1.p, t->xh1.p, t->rs1.p, P + L.off[G1], P + L.off[BE1], t->dy1.p, t->dz1.p, n);
+  const ColJob c1[3] = {{t->dy1.p, t->xh1.p, G + L.off[G1], kHid}, {t->dy1.p, nullptr, G + L.off[BE1], kHid},
+                        {t->dz1.p, nullptr, G + L.off[B1], kHid}};
+  CK(launch_colsum(c1, 3, n, st));
+  // hidden layer 1: dW1 = dz1^T q
+  const Gemm b1{t->dz1.p, 1, kHid, dev_q, Q, 1, G + L.off[W1], Q, nullptr, kHid, Q, n};
+  CK(launch_gemm(&b1, 1, st));
+  FinishArgs fa{G, L, t->sq_norms.p, t->step.p, t->row_loss.p, n, t->last.p, dev_out};
+  finish_kernel<<<kParams + 1, 256, 0, st>>>(fa);
+  CK(cudaGetLastError());
+  AdamArgs aa{P, G, t->m.p, t->v.p, L.total(), t->sq_norms.p, t->step.p, lr, (float)max_norm, t->last.p, dev_out};
+  const int blocks = (int)std::min<int64_t>((L.total() + 255) / 256, 1024);
+  adam_kernel<<<blocks, 256, 0, st>>>(aa);
+  CK(cudaGetLastError());
+  return CFRB_OK;
+}
+
+int cfrb_trainer_loss(cfrb_trainer* t, const float* dev_q, const float* dev_v, int32_t n, int32_t loss_kind, void* cuda_stream,
+                      float* dev_out) {
+  using namespace cfrb::train;
+  int rc = trainer_check_batch(t, "cfrb_trainer_loss: ", dev_q, dev_v, n, loss_kind, dev_out);
+  if (rc) return rc;
+  if (!dev_out) return fail(CFRB_EINVAL, "cfrb_trainer_loss: out is NULL");
+  CK(cudaSetDevice(t->device));
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  if ((rc = trainer_forward(t, dev_q, dev_v, n, loss_kind, st))) return rc;
+  // the loss block alone; cfrb_trainer_last keeps reporting the most recent training step
+  FinishArgs fa{t->grads.p, t->L, t->sq_norms.p, t->step.p, t->row_loss.p, n, nullptr, dev_out};
+  finish_kernel<<<1, 256, 0, st>>>(fa);
+  CK(cudaGetLastError());
   return CFRB_OK;
 }
 
