@@ -265,6 +265,19 @@ int cfrb_selfplay_wave(cfrb_handle* h, float* dev_ex_q, float* dev_ex_v, int32_t
 int cfrb_selfplay_wait_examples(cfrb_handle* h);
 /* Game states (public state and beliefs [n][2][H]) copied to the host; any pointer may be NULL.  Synchronises.  Returns n_games. */
 int cfrb_selfplay_state(cfrb_handle* h, int32_t* last_bid, int32_t* player, double* beliefs);
+/* Save and restore a self-play session, so that a stopped run continues bit for bit.  The image is a versioned header (magic,
+ * format version, num_dice, num_faces, n_games, num_hands, sample_leaf, the bits of random_action_prob, the wave count) followed by
+ * every game's beliefs, mt19937 state and index, last bid and player, in host byte order.
+ * cfrb_selfplay_export writes the image to `out` (cap bytes) and returns its size; out == NULL only reports the size.  It
+ * synchronises.  CFRB_ESTATE without a session or while a wave is pending: drain first with cfrb_selfplay_wave(..., start_next=0).
+ * cfrb_selfplay_import installs an image into the session of cfrb_selfplay_create with the same n_games.  The image is checked on
+ * the host before the device is touched; a header field that differs from the session (named in the message), a buffer of the
+ * wrong size, an mt index outside [0, 624], a player other than 0 / 1, a last bid the walk cannot produce, or a negative or
+ * non-finite belief returns CFRB_EINVAL and leaves the session unchanged.  An accepted image is installed between two device-wide
+ * synchronisations, so it is ordered after every wave drained on any stream and before the next one.  Afterwards no wave is pending and the handle holds no
+ * wave (as after cfrb_create), so readers of a solved wave find none until the next cfrb_selfplay_wave. */
+int64_t cfrb_selfplay_export(cfrb_handle* h, void* out, size_t cap);
+int cfrb_selfplay_import(cfrb_handle* h, const void* in, size_t bytes);
 /* Test aid: the division-free quotient of the regret-matching step (reciprocal of the node's sum + two fused multiply-add
  * corrections, csrc/cfr_kernels.cuh) against IEEE division on blocks x 256 x 4096 pseudo-random operand pairs. */
 int cfrb_debug_div_check(cfrb_handle* h, uint64_t seed, int32_t blocks, uint64_t* mismatches);

@@ -86,6 +86,9 @@ def lib():
     L.cfrb_selfplay_wave.argtypes = [vp, vp, vp, C.c_int32, vp]
     L.cfrb_selfplay_wait_examples.argtypes = [vp]
     L.cfrb_selfplay_state.argtypes = [vp, _ip, _ip, _dp]
+    L.cfrb_selfplay_export.argtypes = [vp, vp, C.c_size_t]
+    L.cfrb_selfplay_export.restype = C.c_int64
+    L.cfrb_selfplay_import.argtypes = [vp, C.c_char_p, C.c_size_t]
     L.cfrb_stream_wait.argtypes = [vp, vp]
     L.cfrb_debug_div_check.argtypes = [vp, C.c_uint64, C.c_int32, C.POINTER(C.c_uint64)]
     L.cfrb_debug_gelu_table.argtypes = [vp, C.c_int32, C.POINTER(C.c_uint16)]
@@ -322,6 +325,18 @@ class WaveSolver:
         lb = np.zeros(self.n, np.int32); pl = np.zeros(self.n, np.int32); b = np.zeros((self.n, 2, self.H), np.float64)
         _check(lib().cfrb_selfplay_state(self._h, _p(lb, _ip), _p(pl, _ip), _p(b, _dp)))
         return lb, pl, b
+
+    def selfplay_export(self):
+        """The session's image (bytes): every game's state and random stream.  Needs a drained session (no pending wave)."""
+        n = _check(lib().cfrb_selfplay_export(self._h, None, 0))
+        buf = C.create_string_buffer(n)
+        _check(lib().cfrb_selfplay_export(self._h, buf, n))
+        return buf.raw
+
+    def selfplay_import(self, image):
+        """Install an image of selfplay_export into this handle's session (same game, n_games, sampling parameters)."""
+        image = bytes(image)
+        _check(lib().cfrb_selfplay_import(self._h, image, len(image)))
 
     def gelu_table(self, what):
         """fp16 -> fp16 table of tanh.approx.f16x2 (what=0) / of the epilogue's GELU from hy = y/2, packed-half (what=1) or fp32-tanh

@@ -1571,6 +1571,120 @@ int cfrb_selfplay_state(cfrb_handle* h, int32_t* last_bid, int32_t* player, doub
   return K;
 }
 
+// Session image of cfrb_selfplay_export / _import: this header, then beliefs f64 [K][2][H], mt u32 [624][K], last_bid i32 [K],
+// player i32 [K], mt_idx i32 [K].  Host byte order.
+namespace {
+constexpr uint32_t kSpMagic = 0x50534643u;   // "CFSP"
+constexpr uint32_t kSpVersion = 1;
+struct SpImageHeader {
+  uint32_t magic, version;
+  int32_t num_dice, num_faces, n_games, num_hands, sample_leaf;
+  uint32_t random_action_prob_bits;
+  int64_t waves;
+};
+static_assert(sizeof(SpImageHeader) == 40, "session image header layout");
+
+size_t sp_image_bytes(int K, int H) {
+  return sizeof(SpImageHeader) + (size_t)K * 2 * H * sizeof(double) + (size_t)624 * K * sizeof(uint32_t) + (size_t)3 * K * sizeof(int32_t);
+}
+SpImageHeader sp_image_header(const cfrb_handle* h) {
+  SpImageHeader hd{kSpMagic, kSpVersion, h->cfg.num_dice, h->cfg.num_faces, h->sp.K, h->g.H, h->sp.dev.sample_leaf, 0, h->sp.waves};
+  std::memcpy(&hd.random_action_prob_bits, &h->sp.dev.random_action_prob, sizeof(float));
+  return hd;
+}
+}  // namespace
+
+int64_t cfrb_selfplay_export(cfrb_handle* h, void* out, size_t cap) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  if (!h->sp.ready) return fail(CFRB_ESTATE, "cfrb_selfplay_export: no self-play session (cfrb_selfplay_create)");
+  if (h->sp.pending)
+    return fail(CFRB_ESTATE, "cfrb_selfplay_export: a wave is pending; drain it first with cfrb_selfplay_wave(..., start_next=0)");
+  const int K = h->sp.K, H = h->g.H;
+  const size_t bytes = sp_image_bytes(K, H);
+  if (!out) return (int64_t)bytes;
+  if (cap < bytes) return fail(CFRB_EINVAL, "cfrb_selfplay_export: buffer of " + std::to_string(cap) + " bytes, the session needs " + std::to_string(bytes));
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());
+  const SpImageHeader hd = sp_image_header(h);
+  char* p = static_cast<char*>(out);
+  std::memcpy(p, &hd, sizeof hd); p += sizeof hd;
+  CK(cudaMemcpy(p, h->sp.beliefs.p, (size_t)K * 2 * H * sizeof(double), cudaMemcpyDeviceToHost)); p += (size_t)K * 2 * H * sizeof(double);
+  CK(cudaMemcpy(p, h->sp.mt.p, (size_t)624 * K * sizeof(uint32_t), cudaMemcpyDeviceToHost)); p += (size_t)624 * K * sizeof(uint32_t);
+  CK(cudaMemcpy(p, h->sp.last_bid.p, K * sizeof(int32_t), cudaMemcpyDeviceToHost)); p += K * sizeof(int32_t);
+  CK(cudaMemcpy(p, h->sp.player.p, K * sizeof(int32_t), cudaMemcpyDeviceToHost)); p += K * sizeof(int32_t);
+  CK(cudaMemcpy(p, h->sp.mt_idx.p, K * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return (int64_t)bytes;
+}
+
+int cfrb_selfplay_import(cfrb_handle* h, const void* in, size_t bytes) {
+  if (!h || !in) return fail(CFRB_EINVAL, "null argument");
+  if (!h->sp.ready) return fail(CFRB_ESTATE, "cfrb_selfplay_import: no self-play session (call cfrb_selfplay_create with the same n_games first)");
+  if (h->sp.pending)
+    return fail(CFRB_ESTATE, "cfrb_selfplay_import: a wave is pending; drain it first with cfrb_selfplay_wave(..., start_next=0)");
+  // Everything is checked on the host before the device is touched: a refused image leaves the session as it was.
+  const int K = h->sp.K, H = h->g.H, A = h->g.A;
+  if (bytes < sizeof(SpImageHeader)) return fail(CFRB_EINVAL, "cfrb_selfplay_import: " + std::to_string(bytes) + " bytes is shorter than the header");
+  SpImageHeader hd;
+  std::memcpy(&hd, in, sizeof hd);
+  const SpImageHeader want = sp_image_header(h);
+  auto field = [](const char* name, int64_t got, int64_t exp) {
+    return fail(CFRB_EINVAL, std::string("cfrb_selfplay_import: ") + name + " is " + std::to_string(got) + ", this session has " + std::to_string(exp));
+  };
+  if (hd.magic != kSpMagic) return fail(CFRB_EINVAL, "cfrb_selfplay_import: not a self-play session image (bad magic)");
+  if (hd.version != kSpVersion) return field("format version", hd.version, kSpVersion);
+  if (hd.num_dice != want.num_dice) return field("num_dice", hd.num_dice, want.num_dice);
+  if (hd.num_faces != want.num_faces) return field("num_faces", hd.num_faces, want.num_faces);
+  if (hd.n_games != want.n_games) return field("n_games", hd.n_games, want.n_games);
+  if (hd.num_hands != want.num_hands) return field("num_hands", hd.num_hands, want.num_hands);
+  if (hd.sample_leaf != want.sample_leaf) return field("sample_leaf", hd.sample_leaf, want.sample_leaf);
+  if (hd.random_action_prob_bits != want.random_action_prob_bits) {
+    float got, exp;
+    std::memcpy(&got, &hd.random_action_prob_bits, 4); std::memcpy(&exp, &want.random_action_prob_bits, 4);
+    return fail(CFRB_EINVAL, "cfrb_selfplay_import: random_action_prob is " + std::to_string(got) + ", this session has " + std::to_string(exp));
+  }
+  if (hd.waves < 0) return field("wave count", hd.waves, 0);
+  const size_t need = sp_image_bytes(K, H);
+  if (bytes != need) return fail(CFRB_EINVAL, "cfrb_selfplay_import: " + std::to_string(bytes) + " bytes, the image of this session has " + std::to_string(need));
+  const char* p = static_cast<const char*>(in) + sizeof hd;
+  std::vector<double> bel((size_t)K * 2 * H);
+  std::vector<uint32_t> mt((size_t)624 * K);
+  std::vector<int32_t> last_bid(K), player(K), mt_idx(K);
+  std::memcpy(bel.data(), p, bel.size() * sizeof(double)); p += bel.size() * sizeof(double);
+  std::memcpy(mt.data(), p, mt.size() * sizeof(uint32_t)); p += mt.size() * sizeof(uint32_t);
+  std::memcpy(last_bid.data(), p, K * sizeof(int32_t)); p += K * sizeof(int32_t);
+  std::memcpy(player.data(), p, K * sizeof(int32_t)); p += K * sizeof(int32_t);
+  std::memcpy(mt_idx.data(), p, K * sizeof(int32_t));
+  for (int g = 0; g < K; ++g) {
+    const std::string at = " of game " + std::to_string(g);
+    if (mt_idx[g] < 0 || mt_idx[g] > 624) return fail(CFRB_EINVAL, "cfrb_selfplay_import: mt_idx" + at + " is " + std::to_string(mt_idx[g]) + ", outside [0, 624]");
+    if (player[g] != 0 && player[g] != 1) return fail(CFRB_EINVAL, "cfrb_selfplay_import: player" + at + " is " + std::to_string(player[g]) + ", not 0 or 1");
+    // the walk leaves a game at the initial state (-1, player 0) or after a non-terminal bid; a liar call restarts the game
+    if (last_bid[g] < -1 || last_bid[g] > A - 2 || (last_bid[g] == -1 && player[g] != 0))
+      return fail(CFRB_EINVAL, "cfrb_selfplay_import: last_bid " + std::to_string(last_bid[g]) + " with player " + std::to_string(player[g]) + at +
+                                   " is not a state the walk produces (last_bid in [-1, " + std::to_string(A - 2) + "], player 0 at -1)");
+    for (int i = 0; i < 2 * H; ++i) {
+      const double b = bel[(size_t)g * 2 * H + i];
+      if (!std::isfinite(b) || b < 0) return fail(CFRB_EINVAL, "cfrb_selfplay_import: belief " + std::to_string(i) + at + " is " + std::to_string(b));
+    }
+  }
+  // Device-wide synchronisation on both sides: a finish kernel of the last wave may still be writing the session on a caller's
+  // stream, and copies from pageable memory may return before their DMA lands, while the next wave starts on the non-blocking
+  // own_stream.
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(h->sp.beliefs.p, bel.data(), bel.size() * sizeof(double), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->sp.mt.p, mt.data(), mt.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->sp.last_bid.p, last_bid.data(), K * sizeof(int32_t), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->sp.player.p, player.data(), K * sizeof(int32_t), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->sp.mt_idx.p, mt_idx.data(), K * sizeof(int32_t), cudaMemcpyHostToDevice));
+  CK(cudaDeviceSynchronize());
+  h->sp.waves = hd.waves;
+  h->sp.ev_recorded = false;
+  // The handle holds no wave, as after cfrb_create: the readers of a solved wave (cfrb_fetch, the sum rebuild, ...) find none.
+  h->n = 0; h->rows = 0; h->iters_done = 0; h->rows_on_device = false; h->mirror_stale = false; h->sum_dropped = false;
+  return CFRB_OK;
+}
+
 // Roots of the current wave (inspection; pulls the descriptors of a device-built wave).  Returns the number of subgames.
 int cfrb_wave_roots(cfrb_handle* h, int32_t* last_bid, int32_t* player_id, int32_t cap) {
   if (!h) return fail(CFRB_EINVAL, "null handle");

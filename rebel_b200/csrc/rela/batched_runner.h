@@ -22,6 +22,7 @@
 // rank * 1000 + i, so these never collide with another loop's games), and replays the reference's RlRunner(seed = s + 10^6 g)
 // exactly as long as the solver's strategies agree.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <functional>
 #include <memory>
@@ -151,6 +152,33 @@ class BatchedRlRunner {
     return sink(dev_q_[b], Q_, dev_v_[b], H_, rows, device_);
   }
 
+  // One wave delivered to `sink`, leaving the next one running (stepDevice) or, with keep_running false, no wave in flight.
+  bool waveDevice(const DeviceExampleSink& sink, bool keep_running) {
+    if (keep_running) return stepDevice(sink);
+    if (host_walk_) throw std::runtime_error("BatchedRlRunner::waveDevice needs the device walk");
+    if (!started_) {
+      check(cfrb_selfplay_wave(h_, nullptr, nullptr, 1, nullptr), "cfrb_selfplay_wave");
+      started_ = true;
+    }
+    return finishDevice(sink);
+  }
+  // No wave in flight: the games' states are final until the next wave, so the session can be exported or replaced.
+  bool drained() const { return !started_; }
+  // The session image of cfrb_selfplay_export / _import (every game's state and random stream).  A drained device walk only: the
+  // host-walk parity mode keeps its games on the host and has no device session to save.
+  std::string exportSession() {
+    requireDrainedSession("export");
+    const int64_t n = cfrb_selfplay_export(h_, nullptr, 0);
+    check((int)std::min<int64_t>(n, 0), "cfrb_selfplay_export");
+    std::string img((size_t)n, '\0');
+    check((int)std::min<int64_t>(cfrb_selfplay_export(h_, img.data(), img.size()), 0), "cfrb_selfplay_export");
+    return img;
+  }
+  void importSession(const std::string& img) {
+    requireDrainedSession("import");
+    check(cfrb_selfplay_import(h_, img.data(), img.size()), "cfrb_selfplay_import");
+  }
+
   // One wave, examples delivered in host memory.  Device walk: a synchronous wrapper around the pipeline (tests, tools).
   bool step(const ExampleSink& sink) {
     if (!host_walk_) {
@@ -202,6 +230,12 @@ class BatchedRlRunner {
 
   void check(int rc, const char* what) {
     if (rc < 0) throw std::runtime_error(std::string(what) + ": " + cfrb_last_error());
+  }
+  void requireDrainedSession(const char* what) const {
+    if (host_walk_)
+      throw std::runtime_error(std::string("self-play session ") + what + ": the host-walk parity mode (CFRB_HOST_WALK=1) has no device "
+                               "session to save or restore; use the device walk");
+    if (started_) throw std::runtime_error(std::string("self-play session ") + what + ": a wave is in flight; drain the runner first");
   }
   void resetGame(Game& G) {   // recursive_solving.cc:161-163
     G.last_bid = -1; G.player = 0;

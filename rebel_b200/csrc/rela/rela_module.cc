@@ -211,6 +211,95 @@ class DataThreadLoop : public ThreadLoop {
   std::atomic<double> w_sum_{0.0};
 };
 
+// A generator the caller drives: the BatchedRlRunner of a DataThreadLoop without the thread, so that a training loop can fix which
+// waves run with which weights and the order in which their examples reach the replay (train.py --deterministic).  Each run() call
+// delivers one wave; keep_running leaves the next wave running behind it (the loop's pipeline), otherwise nothing is in flight
+// afterwards, which set_weights, state and load_state require.
+class SelfPlayGenerator {
+ public:
+  SelfPlayGenerator(const RecursiveSolvingParams& cfg, int device, int seed) {
+    if (cfg.num_dice < 1 || cfg.num_faces < 1) throw std::runtime_error("SelfPlayGenerator: num_dice / num_faces not set");
+    if (cfg.subgame_params.max_depth < 1 || cfg.subgame_params.num_iters < 1)
+      throw std::runtime_error("SelfPlayGenerator: subgame_params.max_depth and num_iters must be >= 1");
+    if (cfg.concurrent_games < 1) throw std::runtime_error("SelfPlayGenerator: concurrent_games must be >= 1");
+    if (cfg.host_walk)
+      throw std::runtime_error("SelfPlayGenerator: the host-walk parity mode (CFRB_HOST_WALK=1) has no device session to drive, save or "
+                               "restore; use the device walk");
+    const int ndev = cfrb_device_count();
+    if (ndev <= 0) throw std::runtime_error("rebel_b200: no CUDA device (there is no CPU generation path)");
+    if (device < 0 || device >= ndev) throw std::runtime_error("SelfPlayGenerator: no CUDA device " + std::to_string(device));
+    py::gil_scoped_release nogil;
+    runner_ = std::make_unique<BatchedRlRunner>(cfg, device, seed);
+  }
+
+  void setWeights(torch::Tensor flat, uint64_t version) {
+    requireDrained("set_weights");
+    auto t = flat.to(torch::kCPU, torch::kFloat32).contiguous();
+    const std::vector<float> w(t.data_ptr<float>(), t.data_ptr<float>() + t.numel());
+    py::gil_scoped_release nogil;
+    runner_->setWeights(w, version);
+  }
+
+  // One wave's 2 x concurrent_games examples: appended to `replay` (returns the row count) or, without one, returned as host
+  // tensors (query [n, Q], values [n, H]).  A replay that cannot take the rows without blocking is an error: nothing else would
+  // ever make room.
+  py::object run(std::shared_ptr<ValuePrioritizedReplay> replay, bool keep_running) {
+    std::vector<float> q, v;
+    int rows = 0, qd = 0, vd = 0;
+    {
+      py::gil_scoped_release nogil;
+      bool full = false;
+      runner_->waveDevice([&](const float* dq, int q_dim, const float* dv, int v_dim, int n, int dev) {
+        rows = n; qd = q_dim; vd = v_dim;
+        if (replay) {
+          full = !replay->addRowsDevice(dq, q_dim, dv, v_dim, n, dev, [] { return true; });
+          return true;
+        }
+        q.resize((size_t)n * q_dim); v.resize((size_t)n * v_dim);
+        if (cfrb_dev_to_host(dev, q.data(), dq, q.size() * sizeof(float)) < 0 ||
+            cfrb_dev_to_host(dev, v.data(), dv, v.size() * sizeof(float)) < 0)
+          throw std::runtime_error(std::string("cfrb_dev_to_host: ") + cfrb_last_error());
+        return true;
+      }, keep_running);
+      if (full)
+        throw std::runtime_error("SelfPlayGenerator.run: the replay buffer has no room for the wave's " + std::to_string(rows) +
+                                 " rows (sample from it, or raise its capacity)");
+    }
+    if (replay) return py::int_(rows);
+    auto tq = torch::empty({rows, qd}), tv = torch::empty({rows, vd});
+    std::copy(q.begin(), q.end(), tq.data_ptr<float>());
+    std::copy(v.begin(), v.end(), tv.data_ptr<float>());
+    return py::make_tuple(tq, tv);
+  }
+
+  py::bytes state() {
+    requireDrained("state");
+    std::string img;
+    {
+      py::gil_scoped_release nogil;
+      img = runner_->exportSession();
+    }
+    return py::bytes(img);
+  }
+  void loadState(py::bytes image) {
+    requireDrained("load_state");
+    const std::string img = image;
+    py::gil_scoped_release nogil;
+    runner_->importSession(img);
+  }
+
+  bool drained() const { return runner_->drained(); }
+  uint64_t weightsVersion() const { return runner_->weightsVersion(); }
+  int games() const { return runner_->games(); }
+
+ private:
+  void requireDrained(const char* what) const {
+    if (!runner_->drained())
+      throw std::runtime_error(std::string("SelfPlayGenerator.") + what + ": a wave is in flight; finish it with run(keep_running=False) first");
+  }
+  std::unique_ptr<BatchedRlRunner> runner_;
+};
+
 std::shared_ptr<ThreadLoop> create_cfr_thread(std::shared_ptr<ModelLocker> locker, std::shared_ptr<ValuePrioritizedReplay> replay,
                                               const RecursiveSolvingParams& cfg, int seed) {
   return std::make_shared<DataThreadLoop>(std::move(locker), std::move(replay), cfg, seed);
@@ -696,7 +785,14 @@ PYBIND11_MODULE(rela, m) {
       .def("save", &ValuePrioritizedReplay::save)
       .def("extract", &ValuePrioritizedReplay::extract)
       .def("push", &ValuePrioritizedReplay::push, py::call_guard<py::gil_scoped_release>())
-      .def("update_priority", &ValuePrioritizedReplay::updatePriority);
+      .def("update_priority", &ValuePrioritizedReplay::updatePriority)
+      .def("save_state", &ValuePrioritizedReplay::saveState, py::arg("path"), py::call_guard<py::gil_scoped_release>(),
+           "rebel_b200 extension: write the whole state (live rows in order, weights, sum, num_add, sampler state, parameters) to "
+           "`path`; refused while sampled priorities are waiting for update_priority")
+      .def("load_state", &ValuePrioritizedReplay::loadState, py::arg("path"), py::arg("device") = 0,
+           py::call_guard<py::gil_scoped_release>(),
+           "rebel_b200 extension: restore save_state's file into this empty buffer of the same parameters (rows on CUDA `device` "
+           "when one exists); later samples, sizes, eviction and blocking are the saved buffer's");
 
   py::class_<ThreadLoop, std::shared_ptr<ThreadLoop>>(m, "ThreadLoop");
 
@@ -735,6 +831,24 @@ PYBIND11_MODULE(rela, m) {
       .def_property_readonly("weights_version", &DataThreadLoop::weightsVersion, "rebel_b200 extension: version of the weights this loop installed last")
       .def_property_readonly("weights_checksum", &DataThreadLoop::weightsChecksum, "rebel_b200 extension: plain sum of those flat weights")
       .def_property_readonly("concurrent_games", &DataThreadLoop::concurrentGames);
+
+  py::class_<SelfPlayGenerator, std::shared_ptr<SelfPlayGenerator>>(
+      m, "SelfPlayGenerator",
+      "rebel_b200 extension: the self-play of one generator loop (concurrent_games games on CUDA `device`, games seeded like "
+      "create_cfr_thread's loop `seed`) driven by the caller, one wave per run() call")
+      .def(py::init<const RecursiveSolvingParams&, int, int>(), py::arg("cfg"), py::arg("device"), py::arg("seed"))
+      .def("set_weights", &SelfPlayGenerator::setWeights, py::arg("flat"), py::arg("version"),
+           "install flat Net2 weights (FLAT_ORDER) for the waves started from now on; no wave may be in flight")
+      .def("run", &SelfPlayGenerator::run, py::arg("replay") = nullptr, py::arg("keep_running") = false,
+           "finish one wave (starting it first when none is in flight) and hand over its examples: appended to `replay` (returns the "
+           "rows), else returned as (query, values) host tensors.  keep_running: the next wave is started before the examples are "
+           "handed over and stays in flight")
+      .def("state", &SelfPlayGenerator::state, "the session image (bytes: every game's state and random stream); needs no wave in flight")
+      .def("load_state", &SelfPlayGenerator::loadState, py::arg("image"),
+           "continue from an image of state() taken with the same game, concurrent_games and sampling parameters")
+      .def_property_readonly("drained", &SelfPlayGenerator::drained, "no wave in flight")
+      .def_property_readonly("weights_version", &SelfPlayGenerator::weightsVersion)
+      .def_property_readonly("concurrent_games", &SelfPlayGenerator::games);
 
   py::class_<Context>(m, "Context")
       .def(py::init<>())

@@ -21,8 +21,10 @@
 #include <condition_variable>
 #include <cstdio>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <random>
+#include <sstream>
 #include <stdexcept>
 #include <string>
 #include <tuple>
@@ -116,7 +118,7 @@ class RowStore {
 class ValuePrioritizedReplay {
  public:
   ValuePrioritizedReplay(int capacity, int seed, float alpha, float beta, int prefetch, bool use_priority, bool compressed_values)
-      : alpha_(alpha), beta_(beta), prefetch_(prefetch), capacity_(capacity), ring_(int(1.25 * capacity)),
+      : alpha_(alpha), beta_(beta), prefetch_(prefetch), capacity_(capacity), ring_(int(1.25 * capacity)), seed_(seed),
         use_priority_(use_priority), weights_(ring_, 0.f), evicted_(ring_, 0) {
     if (compressed_values) throw std::runtime_error("ValuePrioritizedReplay: compressed_values is not supported by rebel_b200");
     if (capacity <= 0) throw std::runtime_error("ValuePrioritizedReplay: capacity must be positive");
@@ -286,6 +288,92 @@ class ValuePrioritizedReplay {
     std::fclose(f);
   }
 
+  // rebel_b200 extension: the whole observable state, so that a stopped training run continues bit for bit.  Binary file: a
+  // header (magic, format version, the constructor parameters, row widths, size, num_add, sum), the sampler's mt19937 state as
+  // text, then the live rows in order from head: weights [n] and rows (query, values) in blocks.  Host byte order.
+  void saveState(const std::string& path) {
+    std::lock_guard<std::mutex> lk(m_);
+    if (use_priority_ && !sampled_ids_.empty())
+      throw std::runtime_error("ValuePrioritizedReplay.save_state: the priorities of the last sample have not been updated");
+    FILE* f = std::fopen(path.c_str(), "wb");
+    if (!f) throw std::runtime_error("ValuePrioritizedReplay.save_state: cannot open " + path);
+    StateHeader hd = header();
+    hd.q_dim = store_.created() ? store_.qDim() : -1;
+    hd.v_dim = store_.created() ? store_.vDim() : -1;
+    hd.size = size_; hd.num_add = num_add_.load(); hd.sum = sum_;
+    std::ostringstream os;
+    os << rng_;
+    const std::string rng = os.str();
+    hd.rng_bytes = (int32_t)rng.size();
+    bool ok = std::fwrite(&hd, sizeof hd, 1, f) == 1 && std::fwrite(rng.data(), 1, rng.size(), f) == rng.size();
+    std::vector<float> w(size_);
+    for (int i = 0; i < size_; ++i) w[i] = weights_[(head_ + i) % ring_];
+    ok = ok && (int)std::fwrite(w.data(), sizeof(float), size_, f) == size_;
+    std::vector<float> q, v;
+    for (int i = 0; ok && i < size_; i += kStateBlock) {
+      const int n = std::min(kStateBlock, size_ - i);
+      q.resize((size_t)n * hd.q_dim); v.resize((size_t)n * hd.v_dim);
+      store_.read((head_ + i) % ring_, n, q.data(), v.data());
+      ok = std::fwrite(q.data(), sizeof(float), q.size(), f) == q.size() && std::fwrite(v.data(), sizeof(float), v.size(), f) == v.size();
+    }
+    ok = std::fclose(f) == 0 && ok;
+    if (!ok) throw std::runtime_error("ValuePrioritizedReplay.save_state: write to " + path + " failed");
+  }
+
+  // Restores saveState's file into this buffer, which must be empty (nothing ever added) and built with the same parameters.  The
+  // rows are laid out from slot 0; sample(), size(), num_add(), eviction and producer blocking behave as in the saved buffer.
+  // prefer_device: the CUDA ordinal of the rows when a device exists (CFRB_REPLAY_DEVICE overrides it, as for a first append).
+  void loadState(const std::string& path, int prefer_device) {
+    std::lock_guard<std::mutex> lk(m_);
+    const std::string who = "ValuePrioritizedReplay.load_state(" + path + "): ";
+    if (num_add_.load() != 0 || store_.created()) throw std::runtime_error(who + "the buffer is not empty");
+    FILE* f = std::fopen(path.c_str(), "rb");
+    if (!f) throw std::runtime_error(who + "cannot open the file");
+    std::unique_ptr<FILE, int (*)(FILE*)> closer(f, std::fclose);
+    StateHeader hd{};
+    if (std::fread(&hd, sizeof hd, 1, f) != 1) throw std::runtime_error(who + "truncated header");
+    const StateHeader want = header();
+    if (hd.magic != want.magic) throw std::runtime_error(who + "not a replay state file");
+    if (hd.version != want.version) throw std::runtime_error(who + "format version " + std::to_string(hd.version) + ", expected " + std::to_string(want.version));
+    auto differs = [&](const char* name, double got, double exp) {
+      return std::runtime_error(who + name + " is " + std::to_string(got) + " in the file and " + std::to_string(exp) + " in this buffer");
+    };
+    if (hd.capacity != want.capacity) throw differs("capacity", hd.capacity, want.capacity);
+    if (hd.seed != want.seed) throw differs("seed", hd.seed, want.seed);
+    if (hd.alpha != want.alpha) throw differs("alpha", hd.alpha, want.alpha);
+    if (hd.beta != want.beta) throw differs("beta", hd.beta, want.beta);
+    if (hd.prefetch != want.prefetch) throw differs("prefetch", hd.prefetch, want.prefetch);
+    if (hd.use_priority != want.use_priority) throw differs("use_priority", hd.use_priority, want.use_priority);
+    if (hd.size < 0 || hd.size > ring_ || hd.num_add < hd.size || hd.rng_bytes <= 0 || hd.rng_bytes > (1 << 16) ||
+        (hd.size > 0 && (hd.q_dim <= 0 || hd.v_dim <= 0)))
+      throw std::runtime_error(who + "inconsistent header");
+    std::string rng(hd.rng_bytes, '\0');
+    if (std::fread(rng.data(), 1, rng.size(), f) != rng.size()) throw std::runtime_error(who + "truncated sampler state");
+    std::mt19937 gen;
+    std::istringstream is(rng);
+    if (!(is >> gen)) throw std::runtime_error(who + "bad sampler state");
+    std::vector<float> w(hd.size);
+    if ((int)std::fread(w.data(), sizeof(float), hd.size, f) != hd.size) throw std::runtime_error(who + "truncated weights");
+    // read every row before the store exists, so that a truncated file leaves the buffer empty
+    std::vector<float> q((size_t)hd.size * std::max(hd.q_dim, 0)), v((size_t)hd.size * std::max(hd.v_dim, 0));
+    for (int i = 0; i < hd.size; i += kStateBlock) {
+      const int n = std::min(kStateBlock, hd.size - i);
+      if (std::fread(q.data() + (size_t)i * hd.q_dim, sizeof(float), (size_t)n * hd.q_dim, f) != (size_t)n * hd.q_dim ||
+          std::fread(v.data() + (size_t)i * hd.v_dim, sizeof(float), (size_t)n * hd.v_dim, f) != (size_t)n * hd.v_dim)
+        throw std::runtime_error(who + "truncated rows");
+    }
+    if (std::fgetc(f) != EOF) throw std::runtime_error(who + "trailing bytes after the rows");
+    if (hd.q_dim > 0) {
+      store_.create(ring_, hd.q_dim, hd.v_dim, prefer_device);
+      if (hd.size > 0) store_.write(0, hd.size, q.data(), v.data(), /*kind=*/0, -1);
+    }
+    std::copy(w.begin(), w.end(), weights_.begin());
+    std::fill(evicted_.begin(), evicted_.end(), 0);
+    head_ = 0; size_ = hd.size; sum_ = hd.sum; num_add_ = hd.num_add;
+    rng_ = gen;
+    sampled_ids_.clear();
+  }
+
   // Whole content as [queries [n,Q], values [n,H], weights [n]] and empty the buffer (prioritized_replay.h:338-345)
   std::vector<torch::Tensor> extract() {
     std::lock_guard<std::mutex> lk(m_);
@@ -304,6 +392,24 @@ class ValuePrioritizedReplay {
   }
 
  private:
+  struct StateHeader {
+    uint32_t magic, version;
+    int32_t capacity, seed, prefetch, use_priority;
+    float alpha, beta;
+    int32_t q_dim, v_dim, size, num_add;
+    double sum;
+    int32_t rng_bytes, pad;
+  };
+  static constexpr int kStateBlock = 65536;   // rows per host <-> store copy of save_state / load_state
+  StateHeader header() const {
+    StateHeader hd{};
+    hd.magic = 0x53525052u;   // "RPRS"
+    hd.version = 1;
+    hd.capacity = capacity_; hd.seed = seed_; hd.prefetch = prefetch_; hd.use_priority = use_priority_ ? 1 : 0;
+    hd.alpha = alpha_; hd.beta = beta_;
+    return hd;
+  }
+
   bool append(const float* q, int q_dim, const float* v, int v_dim, int n, const float* priority, int kind, int src_device,
               const std::function<bool()>& cancelled) {
     if (n <= 0) return true;
@@ -340,7 +446,7 @@ class ValuePrioritizedReplay {
   }
 
   const float alpha_, beta_;
-  const int prefetch_, capacity_, ring_;
+  const int prefetch_, capacity_, ring_, seed_;
   const bool use_priority_;
   mutable std::mutex m_;
   std::condition_variable cv_space_;
