@@ -216,6 +216,27 @@ int cfrb_ev2(cfrb_handle* h, const double* s1_dense, const double* s2_dense, dou
 /* Node count N_full of the full game tree (the tree cfrb_exploitability / cfrb_ev2 / cfrb_regrets_* index). */
 int cfrb_full_tree_nodes(cfrb_handle* h);
 
+/* Exploitability of the handle's recursive to-leaf average policy (compute_strategy_recursive_to_leaf, recursive_solving.cc:76-134:
+ * every subgame solved for num_iters iterations, get_strategy), with the handle's weights and solver settings, without a dense
+ * strategy: the subgames are solved level by level in waves of max_subgames (level l = the non-terminal nodes at depth
+ * l * max_depth), their roots and beliefs built on the device, their average strategies written into the handle's compact full-tree
+ * strategy, and both best responses taken on it (compute_exploitability2).  br_out2 = {br0, br1}; the exploitability is
+ * (br0 + br1) / 2.  subgames, subgame_iters (may be NULL): subgames solved and their CFR iterations; seconds2 (may be NULL): host
+ * wall time of the walk and of the best response.  Games with A > CFRB_TO_LEAF_MAX_ACTIONS are refused (CFRB_EINVAL), and so is
+ * any call whose cfrb_to_leaf_bytes exceed the device's free memory (CFRB_ENOMEM), before anything is allocated.  Replaces the
+ * handle's wave. */
+int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2);
+#define CFRB_TO_LEAF_MAX_ACTIONS 23   /* 1x11f; 2x6f (A = 25) would need more than 70 GB */
+/* Host-only: device bytes cfrb_to_leaf_exploitability needs beyond the handle of this game, max_depth and max_subgames: the full
+ * tree, its two compact strategies and the best-response scratch (none of which a handle that already holds its full tree
+ * allocates again), and the walk's template map and two largest levels of roots and beliefs.  Games with A > 26: CFRB_EINVAL. */
+int64_t cfrb_to_leaf_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t max_subgames);
+/* Test aid: the compact full-tree strategy [N_full - 1][H] (entry (child - 1) * H + hand) the last cfrb_to_leaf_exploitability
+ * filled. */
+int cfrb_to_leaf_strategy(cfrb_handle* h, double* compact);
+/* Test aid: cfrb_to_leaf_exploitability sees at most `bytes` free device bytes (0 = the device's own figure). */
+int cfrb_debug_to_leaf_free_cap(cfrb_handle* h, int64_t bytes);
+
 /* Immediate-regret accumulator on the handle's device, compute_immediate_regrets (subgame_solving.cc:984-1050) split so that a
  * list of strategies can be added in pieces: adding strategies in batches of any size gives the bits of one pass over the whole
  * list.  Reset zeroes the sums [N_full][H][A] and the count (and must precede the first add). */

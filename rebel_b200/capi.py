@@ -71,6 +71,11 @@ def lib():
     L.cfrb_exploitability.argtypes = [vp, _dp, _dp]
     L.cfrb_ev2.argtypes = [vp, _dp, _dp, _dp]
     L.cfrb_full_tree_nodes.argtypes = [vp]
+    L.cfrb_to_leaf_exploitability.argtypes = [vp, _dp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _dp]
+    L.cfrb_to_leaf_bytes.argtypes = [C.c_int32] * 4
+    L.cfrb_to_leaf_bytes.restype = C.c_int64
+    L.cfrb_to_leaf_strategy.argtypes = [vp, _dp]
+    L.cfrb_debug_to_leaf_free_cap.argtypes = [vp, C.c_int64]
     L.cfrb_regrets_reset.argtypes = [vp]
     L.cfrb_regrets_add.argtypes = [vp, _fp, C.c_int32]
     L.cfrb_regrets_add_current.argtypes = [vp]
@@ -157,6 +162,12 @@ def schedule_order(num_dice, num_faces, last_bid, max_depth=2):
     _check(lib().cfrb_schedule_order(num_dice, num_faces, max_depth, lb.size, _p(lb, _ip), _p(order, _ip),
                                      cost.ctypes.data_as(C.POINTER(C.c_int64))))
     return order, cost
+
+
+def to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames):
+    """Host-only: device bytes WaveSolver.to_leaf_exploitability needs beyond a handle of these sizes (full tree, best-response
+    scratch, the walk's largest levels)."""
+    return _check(lib().cfrb_to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames))
 
 
 def tc_net_supported(num_dice, num_faces, hidden=256):
@@ -284,6 +295,27 @@ class WaveSolver:
         out = np.zeros(2, np.float64)
         _check(lib().cfrb_exploitability(self._h, _p(s, _dp), _p(out, _dp)))
         return out
+
+    def to_leaf_exploitability(self):
+        """Exploitability of the recursive to-leaf average policy of this handle (its weights and solver settings), walked level by
+        level in waves of max_subgames on the device: dict of br [2], exploitability, subgames, subgame_iters, walk_seconds,
+        br_seconds.  Replaces the handle's wave."""
+        br, secs = np.zeros(2, np.float64), np.zeros(2, np.float64)
+        sg, it = C.c_int64(0), C.c_int64(0)
+        _check(lib().cfrb_to_leaf_exploitability(self._h, _p(br, _dp), C.byref(sg), C.byref(it), _p(secs, _dp)))
+        return {"br": br, "exploitability": (br[0] + br[1]) / 2, "subgames": sg.value, "subgame_iters": it.value,
+                "walk_seconds": float(secs[0]), "br_seconds": float(secs[1])}
+
+    def to_leaf_strategy(self):
+        """The compact full-tree strategy [N_full - 1, H] the last to_leaf_exploitability filled (entry [child - 1, hand])."""
+        n = (1 << self.A) - 1                    # the full Liar's Dice tree
+        out = np.zeros((max(n - 1, 1), self.H), np.float64)
+        _check(lib().cfrb_to_leaf_strategy(self._h, _p(out, _dp)))
+        return out
+
+    def debug_to_leaf_free_cap(self, nbytes):
+        """Test aid: to_leaf_exploitability sees at most nbytes free device bytes (0 = the device's own figure)."""
+        _check(lib().cfrb_debug_to_leaf_free_cap(self._h, int(nbytes)))
 
     @property
     def kernel_launches(self):

@@ -10,6 +10,7 @@
 #include "match_kernels.cuh"
 #include "lbr_kernels.cuh"
 #include "agent_kernels.cuh"
+#include "expl_kernels.cuh"
 
 namespace cfrb {
 
@@ -172,6 +173,16 @@ void agent_launch_step(const AgentDev& p, cudaStream_t st) { agent_step_kernel<<
 void agent_launch_policy(const AgentDev& p, cudaStream_t st) {
   agent_policy_kernel<<<(p.n * p.H + 127) / 128, 128, 0, st>>>(p);
 }
+template <typename real>
+void expl_launch_begin(const ExplDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st) {
+  expl_begin_kernel<real><<<(n + 127) / 128, 128, 0, st>>>(p, n, wave_beliefs);
+  sp_scan_kernel<<<1, 1024, 0, st>>>(scan);
+}
+template <typename real>
+void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st) {
+  expl_expand_kernel<real><<<n, 128, 0, st>>>(p, table, normalise);
+  expl_fill_kernel<<<1, 1, 0, st>>>(p);
+}
 __global__ void rows_gather_kernel(const float* __restrict__ src, int width, const int* __restrict__ ids, int n, float* __restrict__ out) {
   const size_t total = (size_t)n * width;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -225,7 +236,9 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void lbr_launch_begin<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                               \
   template void lbr_launch_advance<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                             \
   template void agent_launch_begin<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);                           \
-  template void agent_launch_capture<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);
+  template void agent_launch_capture<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);                         \
+  template void expl_launch_begin<real>(const ExplDev&, const SpDev&, int, real*, cudaStream_t);                           \
+  template void expl_launch_expand<real>(const ExplDev&, int, const real*, int, cudaStream_t);
 CFRB_INSTANTIATE(float)
 CFRB_INSTANTIATE(double)
 

@@ -211,6 +211,31 @@ template <typename real> void agent_launch_begin(const AgentDev& p, const MatchT
 template <typename real> void agent_launch_capture(const AgentDev& p, const MatchTabs<real>& t, cudaStream_t st);
 void agent_launch_step(const AgentDev& p, cudaStream_t st);
 void agent_launch_policy(const AgentDev& p, cudaStream_t st);
+// Recursive to-leaf walk (expl_kernels.cuh): one wave of a level of subgames, rooted at full-tree nodes, solved by one handle.
+struct ExplDev {
+  int H;
+  // the full tree (BrState of the handle) and the compact full-tree strategy [N_full - 1][H] the walk fills
+  const int* full_child_begin; const int* full_depth; const int* full_act_lo;
+  double* strategy;
+  // the handle's subgame templates
+  const TemplateDev* tmpl; const int* parent; const int* child_begin; const int* nchild; const int* level_begin;
+  const int* pleaf_node;
+  // the handle's wave descriptors and CFR step counters
+  int* sg_tmpl; int* sg_player; int* sg_act; const int* sg_row_off; const int* wave; const int* steps;
+  int table_stride;
+  // this level's roots [n_level] and fp64 beliefs [n_level][2][H]; the wave is entries off .. off + n - 1
+  const int* roots; const double* bel;
+  int off;
+  // the next level: cap entries, fill [1] of them written by the level's earlier waves
+  int* next_roots; double* next_bel;
+  int* fill;
+  int cap;
+  int* fid; int nmax;                 // [K][nmax] scratch: full-tree node of every template node of each subgame
+};
+// wave descriptors (template, player, root beliefs as `real`), row offsets and schedule of the level's subgames off .. off + n - 1
+template <typename real> void expl_launch_begin(const ExplDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st);
+// the solved wave's strategy into p.strategy, its pseudo-leaves onto the next level
+template <typename real> void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
 // rows [ids[i]] of a [*, width] fp32 matrix -> out[i]  (replay sampling)
 void rows_launch_gather(const float* src, int width, const int* ids, int n, float* out, cudaStream_t st);
 

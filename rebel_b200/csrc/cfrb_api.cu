@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <array>
@@ -243,6 +244,7 @@ struct cfrb_handle {
   bool rows_on_device = false;   // the wave was built on the device: its row count / roots exist only there
   bool mirror_stale = false;     // ... and the host mirror (h_tmpl, h_beliefs, rows) has not been pulled yet
   bool in_match = false;         // an agent of a live cfrb_match: its waves are built by the match
+  int64_t to_leaf_free_cap = 0;  // test aid (cfrb_debug_to_leaf_free_cap): cfrb_to_leaf_exploitability sees at most this many free bytes
 };
 
 // Calls f with the handle's typed (fp64 or fp32) solver state.
@@ -1490,6 +1492,145 @@ static int solve_device_wave(cfrb_handle* h, int n, bool sorted, bool drop_sum, 
   h->sum_uploads = h->weight_uploads;
   const int rc = launch_init(h, st);
   return rc ? rc : cfrb_run(h, h->cfg.num_iters, st);
+}
+
+// ============================================================================================ recursive to-leaf exploitability
+// Sizes of the device walk from the game alone.  The full tree has 2^A - 1 nodes, 2^(A-1) - 1 of them terminal (liar calls), and
+// C(A - 1, d) non-terminal nodes at depth d (d increasing bids out of the A - 1), so level l of the walk holds C(A - 1, l * max_depth)
+// subgames.  The largest subgame template, the game root's, has A - 1 nodes at depth 1 and C(A, d) at depth d >= 2.
+static int64_t binom(int n, int k) {
+  if (k < 0 || k > n) return 0;
+  int64_t r = 1;
+  for (int i = 1; i <= k; ++i) r = r * (n - k + i) / i;
+  return r;
+}
+struct ToLeafSizes { int64_t tree_bytes = 0, walk_bytes = 0, level_cap = 0; };
+static ToLeafSizes to_leaf_sizes(const cfrb::GameShape& g, int max_depth, int K) {
+  const int A = g.A;
+  const int64_t H = g.H, N = ((int64_t)1 << A) - 1, T = ((int64_t)1 << (A - 1)) - 1, levels = A + 1;
+  ToLeafSizes s;
+  // full_tree_setup: parent, child_begin, nchild, depth, act_lo [N], level_begin [levels + 1] and term_node [3][T] ints; two
+  // strategies [N - 1][H], the best-response scratch 2 x (3 N H + 10 T) and out [2] doubles
+  s.tree_bytes = (5 * N + levels + 1 + 3 * T) * 4 + (2 * (N - 1) * H + 2 * (3 * N * H + 10 * T) + 2) * 8;
+  int64_t nmax = 1;
+  for (int d = 1; d <= std::min(max_depth, A); ++d) nmax += d == 1 ? A - 1 : binom(A, d);
+  for (int d = 0; d <= A - 1; d += max_depth) s.level_cap = std::max(s.level_cap, binom(A - 1, d));
+  // the template-to-full-tree map [K][nmax], and two levels of roots and fp64 beliefs [2][H]
+  s.walk_bytes = (int64_t)K * nmax * 4 + 2 * s.level_cap * (4 + 2 * H * 8);
+  return s;
+}
+
+int64_t cfrb_to_leaf_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t max_subgames) {
+  if (num_dice < 1 || num_faces < 1 || max_depth < 1 || max_subgames < 1)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_bytes: num_dice, num_faces, max_depth, max_subgames must be >= 1");
+  if (2L * num_dice * num_faces + 1 > 26) return fail(CFRB_EINVAL, "cfrb_to_leaf_bytes: full tree too large (2^A - 1 nodes, A > 26)");
+  const auto s = to_leaf_sizes(cfrb::GameShape(num_dice, num_faces), max_depth, max_subgames);
+  return s.tree_bytes + s.walk_bytes;
+}
+
+int cfrb_debug_to_leaf_free_cap(cfrb_handle* h, int64_t bytes) {
+  if (!h || bytes < 0) return fail(CFRB_EINVAL, "cfrb_debug_to_leaf_free_cap: bad argument");
+  h->to_leaf_free_cap = bytes;
+  return CFRB_OK;
+}
+
+int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2) {
+  if (!h || !br_out2) return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: null argument");
+  const auto& g = h->g;
+  if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                                 " actions are not supported (A = " + std::to_string(g.A) + ": the full tree has 2^A - 1 nodes)");
+  if (h->in_match) return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: the handle plays in a live match or agent");
+  if (h->cfg.net_mode != CFRB_NET_ZERO && !h->have_weights && h->Lmax > 0)
+    return fail(CFRB_ESTATE, "cfrb_to_leaf_exploitability: value-net weights not set (cfrb_set_weights)");
+  CK(cudaSetDevice(h->cfg.device));
+  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H;
+  const auto sz = to_leaf_sizes(g, h->cfg.max_depth, K);
+  // refused before anything is allocated: on a shared device an allocation that fails late may starve other processes
+  const int64_t need = (h->br.ready ? 0 : sz.tree_bytes) + sz.walk_bytes;
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  int64_t avail = (int64_t)free_b;
+  if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
+  if (need > avail)
+    return fail(CFRB_ENOMEM, "cfrb_to_leaf_exploitability: needs " + std::to_string(need) + " bytes of device memory beyond the "
+                             "handle (full tree and best-response scratch " + std::to_string(h->br.ready ? 0 : sz.tree_bytes) +
+                             ", walk " + std::to_string(sz.walk_bytes) + "), " + std::to_string(avail) + " free");
+  int rc = full_tree_setup(h, "cfrb_to_leaf_exploitability");
+  if (rc) return rc;
+  cudaStream_t st = h->own_stream;
+  DevBuf<int> roots[2], fid, fill;
+  DevBuf<double> bel[2];
+  for (int i = 0; i < 2; ++i) { CK(roots[i].alloc(sz.level_cap)); CK(bel[i].alloc((size_t)sz.level_cap * W)); }
+  CK(fid.alloc((size_t)K * h->Nmax)); CK(fill.alloc(1));
+  const auto t0 = std::chrono::steady_clock::now();
+  const std::vector<double> uniform(W, 1.0 / H);   // level 0: the game root with uniform beliefs
+  const int root = 0;
+  CK(cudaMemcpyAsync(roots[0].p, &root, sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(bel[0].p, uniform.data(), W * sizeof(double), cudaMemcpyHostToDevice, st));
+  cfrb::ExplDev d{};
+  d.H = H;
+  d.full_child_begin = h->br.child_begin.p; d.full_depth = h->br.depth.p; d.full_act_lo = h->br.act_lo.p; d.strategy = h->br.strategy.p;
+  d.tmpl = h->d_tmpl.p; d.parent = h->d_parent.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p;
+  d.level_begin = h->d_level_begin.p; d.pleaf_node = h->d_pleaf_node.p;
+  d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_act = h->d_sg_act.p; d.sg_row_off = h->d_sg_row_off.p;
+  d.wave = h->d_wave.p; d.steps = h->d_steps.p; d.table_stride = h->table_stride;
+  d.fill = fill.p; d.cap = (int)sz.level_cap; d.fid = fid.p; d.nmax = h->Nmax;
+  cfrb::SpDev scan{};   // sp_scan_kernel's view of the wave
+  scan.A = g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
+  scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
+  int64_t solved = 0;
+  int cur = 0, n_level = 1;
+  for (int depth = 0; n_level > 0; depth += h->cfg.max_depth) {
+    d.roots = roots[cur].p; d.bel = bel[cur].p; d.next_roots = roots[cur ^ 1].p; d.next_bel = bel[cur ^ 1].p;
+    CK(cudaMemsetAsync(fill.p, 0, sizeof(int), st));
+    for (int off = 0; off < n_level; off += K) {
+      const int n = std::min(K, n_level - off);
+      d.off = off; scan.K = n;
+      with_state(h, [&](auto& s) { cfrb::expl_launch_begin(d, scan, n, s.beliefs.p, st); });
+      h->launches += 2;
+      CK(cudaGetLastError());
+      if ((rc = solve_device_wave(h, n, true, false, st))) return rc;
+      with_state(h, [&](auto& s) {
+        const auto avg = avg_table(h, s);
+        cfrb::expl_launch_expand(d, n, avg.p, avg.normalise ? 1 : 0, st);
+      });
+      h->launches += 2;
+      CK(cudaGetLastError());
+    }
+    solved += n_level;
+    int next = 0;
+    CK(cudaMemcpyAsync(&next, fill.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (next != binom(g.A - 1, depth + h->cfg.max_depth))
+      return fail(CFRB_ECUDA, "cfrb_to_leaf_exploitability: level at depth " + std::to_string(depth + h->cfg.max_depth) + " has " +
+                                  std::to_string(next) + " subgames, the tree " + std::to_string(binom(g.A - 1, depth + h->cfg.max_depth)));
+    n_level = next;
+    cur ^= 1;
+  }
+  const auto t1 = std::chrono::steady_clock::now();
+  cfrb::br_launch(full_tree_dev(h), st);
+  ++h->launches;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(br_out2, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const auto t2 = std::chrono::steady_clock::now();
+  if (subgames) *subgames = solved;
+  if (subgame_iters) *subgame_iters = solved * h->cfg.num_iters;
+  if (seconds2) {
+    seconds2[0] = std::chrono::duration<double>(t1 - t0).count();
+    seconds2[1] = std::chrono::duration<double>(t2 - t1).count();
+  }
+  return CFRB_OK;
+}
+
+int cfrb_to_leaf_strategy(cfrb_handle* h, double* compact) {
+  if (!h || !compact) return fail(CFRB_EINVAL, "cfrb_to_leaf_strategy: null argument");
+  if (!h->br.ready) return fail(CFRB_ESTATE, "cfrb_to_leaf_strategy: the handle holds no full-tree strategy (run cfrb_to_leaf_exploitability)");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->own_stream));
+  CK(cudaMemcpy(compact, h->br.strategy.p, h->br.strategy.n * sizeof(double), cudaMemcpyDeviceToHost));
+  return CFRB_OK;
 }
 
 // ============================================================================================ device-resident self-play

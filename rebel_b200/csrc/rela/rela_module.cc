@@ -695,6 +695,38 @@ torch::Tensor strategy_recursive_to_leaf(const RecursiveSolvingParams& cfg, int 
   return f64_tensor(s, {N, H, A});
 }
 
+// The exploitability of compute_strategy_recursive_to_leaf's policy, walked and best-responded on the device
+// (cfrb_to_leaf_exploitability): no dense strategy, so games up to A = 23 (2x5f, 5x2f, 1x10f, 1x11f) are accepted.
+py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity) {
+  const int A = 2 * cfg.num_dice * cfg.num_faces + 1;
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)   // the library's own refusal, before a device is touched
+    throw std::runtime_error("exploitability_to_leaf: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                             " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+  const std::vector<float> w = flat_of(flat_weights);
+  std::array<double, 2> br{};
+  double secs[2] = {0, 0}, total = 0;
+  int64_t subgames = 0, iters = 0;
+  int N = 0;
+  {
+    py::gil_scoped_release nogil;
+    const auto t0 = std::chrono::steady_clock::now();
+    const cfrb_config c = liars_dice::solver_config(cfg, device, std::max(1, wave_capacity));
+    cfrb_handle* raw = nullptr;
+    if (cfrb_create(&c, &raw) < 0) throw std::runtime_error(std::string("cfrb_create: ") + cfrb_last_error());
+    std::unique_ptr<cfrb_handle, int (*)(cfrb_handle*)> h(raw, cfrb_destroy);
+    if (!w.empty() && cfrb_set_weights(h.get(), w.data(), w.size(), 1) < 0) throw std::runtime_error(cfrb_last_error());
+    if (cfrb_to_leaf_exploitability(h.get(), br.data(), &subgames, &iters, secs) < 0) throw std::runtime_error(cfrb_last_error());
+    N = cfrb_full_tree_nodes(h.get());
+    total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  }
+  py::dict d;
+  d["exploitability"] = (br[0] + br[1]) / 2.;
+  d["br"] = std::vector<double>{br[0], br[1]};
+  d["num_nodes"] = N; d["subgames"] = subgames; d["subgame_iters"] = iters;
+  d["seconds"] = total; d["walk_seconds"] = secs[0]; d["br_seconds"] = secs[1];
+  return d;
+}
+
 // rela.Agent: index lists and actions from anything torch.as_tensor accepts (lists, numpy arrays, tensors).
 std::vector<int32_t> i32_of(py::object o) {
   auto t = py::module::import("torch").attr("as_tensor")(o).cast<torch::Tensor>().to(torch::kCPU, torch::kInt32).contiguous().view(-1);
@@ -919,6 +951,13 @@ PYBIND11_MODULE(rela, m) {
         "concurrent_games, at least A - 1).  LBR's payoff is a lower bound on the agent's exploitability.  dict: payoff_lbr "
         "[games], plies [games], mean, stderr (over pairs), seat_means [2] (LBR in seat 0 / seat 1), solves, whatif_solves, "
         "deferred_slot_rounds, max_subgames, subgame_iters, seconds.");
+  m.def("exploitability_to_leaf", &exploitability_to_leaf, py::arg("cfg"), py::arg("device") = 0, py::arg("flat_weights") = py::none(),
+        py::arg("wave_capacity") = 16384,
+        "rebel_b200 extension: exploitability of compute_strategy_recursive_to_leaf's policy (every subgame solved for num_iters "
+        "iterations, get_strategy; the policy play_match's 'average' plays and play_lbr bounds), the subgames walked level by level "
+        "in waves of wave_capacity and the best response taken on the GPU without a dense strategy (games with at most 23 actions "
+        "whose need fits the free device memory).  dict: exploitability = (br0 + br1) / 2, br [2], num_nodes, subgames, "
+        "subgame_iters, seconds, walk_seconds, br_seconds.");
   m.def("match_stats", &match_stats_py, py::arg("payoff_a"),
         "rebel_b200 extension: play_match's mean, stderr (over the pairs 2i, 2i+1) and seat_means of a payoff vector.");
   py::class_<Agent, std::shared_ptr<Agent>>(
