@@ -130,6 +130,10 @@ int cfrb_num_actions(const cfrb_handle* h);   /* A */
 int cfrb_num_hands(const cfrb_handle* h);     /* H */
 int cfrb_query_size(const cfrb_handle* h);    /* Q */
 int cfrb_max_nodes(const cfrb_handle* h);     /* Nmax over all root templates */
+/* Test aid: which CFR iteration kernel the handle runs, chosen by cfrb_create from the game, depth and state dtype:
+ * 0 = cfr_iter_d2_kernel (depth <= 2 templates in shared memory), 1 = cfr_iter_kernel with a warp per subgame and its scratch in
+ * shared memory, 2 = cfr_iter_kernel with a CTA per subgame and its scratch in global memory. */
+int cfrb_debug_kernel_path(const cfrb_handle* h);
 
 /* Host-only (no device needed): unroll_tree(game, {last_bid, player_id}, max_depth) (tree.h:51-70) through the same
  * template builder the kernels index with.  Returns the node count or a negative error; writes min(count, cap). */

@@ -50,7 +50,7 @@ def lib():
     L.cfrb_create.argtypes = [C.POINTER(Config), C.POINTER(vp)]
     L.cfrb_destroy.argtypes = [vp]
     for f in ("cfrb_num_actions", "cfrb_num_hands", "cfrb_query_size", "cfrb_max_nodes", "cfrb_iterations_done",
-              "cfrb_sync"):
+              "cfrb_sync", "cfrb_debug_kernel_path"):
         getattr(L, f).argtypes = [vp]
     L.cfrb_unroll_tree.argtypes = [C.c_int32] * 5 + [_ip, C.c_int32]
     L.cfrb_tc_net_supported.argtypes = [C.c_int32] * 3
@@ -392,6 +392,10 @@ class WaveSolver:
         out = np.zeros(self.n, np.int32)
         n = _check(lib().cfrb_wave_order(self._h, _p(out, _ip), self.n))
         return out[:n]
+
+    def kernel_path(self):
+        """Which CFR iteration kernel this handle runs: 0 = depth-2 kernel, 1 = warp per subgame, 2 = CTA per subgame."""
+        return _check(lib().cfrb_debug_kernel_path(self._h))
 
     def debug_d2_grid(self, max_ctas):
         """Test aid: run the depth-2 CFR kernel on at most max_ctas CTAs (0 = no cap); returns the CTAs resident at once."""

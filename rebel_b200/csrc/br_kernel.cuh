@@ -17,7 +17,8 @@ __global__ void __launch_bounds__(1024) br_kernel(BrDev p) {
   double* reach1 = reach0 + (size_t)N * H;
   double* val = reach1 + (size_t)N * H;
   double* hist = val + (size_t)N * H;
-  constexpr int kMaxBins = 9;
+  constexpr int kMaxBins = 9;            // match counts 0 .. 8; bin 8 stays empty for num_dice <= kMaxDice = 7 (cfr_types.h)
+  static_assert(kMaxBins >= kMaxDice + 2, "a clamped `left` must land on an empty bin");
   for (int h = tid; h < H; h += nt) { reach0[h] = 1. / H; reach1[h] = 1. / H; }   // uniform beliefs (:806-809)
   __syncthreads();
   for (int d = 1; d < p.levels; ++d) {

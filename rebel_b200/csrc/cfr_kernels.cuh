@@ -163,7 +163,8 @@ __device__ void cfr_forward(const CfrDev<real>& p, int k, int trav, real* reach0
   // Pass 1 (one lane per terminal): believed_counts[m] += reach (hand order), suffix sums from the top (:770-779) and the
   // belief sum — the reference's operation order, so the fp64 path is bit-identical.  Pass 2 (one lane per (terminal,
   // hand)) picks cum[max(0, quantity - matches(hand))], float-rounds it like :785 and forms the payoff.
-  constexpr int kMaxBins = 9;            // 2 * num_dice + 1 <= 9
+  constexpr int kMaxBins = 9;            // match counts 0 .. 8; bin 8 stays empty for num_dice <= kMaxDice = 7 (cfr_types.h)
+  static_assert(kMaxBins >= kMaxDice + 2, "a clamped `left` must land on an empty bin");
   real* __restrict__ vt = p.vterm + (size_t)k * p.vterm_stride;
   const real* ropp = trav == 0 ? reach1 : reach0;
   for (int z = lane; z < t.T; z += G) {
@@ -886,7 +887,8 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     }
   }
   // ---- terminals (compute_expected_terminal_values :80-98; win probability :765-789), as in cfr_forward
-  constexpr int kMaxBins = 9;
+  constexpr int kMaxBins = 9;            // num_dice <= kMaxDice = 7, as in cfr_forward
+  static_assert(kMaxBins >= kMaxDice + 2, "a clamped `left` must land on an empty bin");
   real* __restrict__ vt = p.vterm + (size_t)k * p.vterm_stride;
   __syncwarp();      // hist shares the aux region with the fp16 belief columns the query rows were assembled from
   for (int z = lane; z < t.T; z += G) {

@@ -6,6 +6,11 @@
 
 namespace cfrb {
 
+// Terminal payoffs (subgame_solving.cc:765-789) count the opponent's hands by match count.  The reference sizes that histogram
+// 2 * num_dice + 1; the CFR, best-response and regret kernels keep 9 bins (kMaxBins) and clamp the count a hand still needs to
+// bin 8.  That is exact only while bin 8 stays empty, i.e. for at most 7 dice per player: cfrb_create refuses larger games.
+constexpr int kMaxDice = 7;
+
 struct TemplateDev {
   int node_off, level_off, pleaf_off, term_off;
   int N, L, T, levels;

@@ -559,6 +559,9 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   h->g = cfrb::GameShape(cfg->num_dice, cfg->num_faces);
   const auto& g = h->g;
   if (g.A > 1024 || g.H > 4096) return fail(CFRB_EINVAL, "game too large");
+  if (cfg->num_dice > cfrb::kMaxDice)
+    return fail(CFRB_EINVAL, "game too large: " + std::to_string(cfg->num_dice) + " dice per player; the terminal payoff histogram "
+                             "holds 9 bins, so at most 7 dice per player");
   // ---- templates: root_bid in {-1, 0 .. A-2}
   std::vector<TemplateDev> td;
   std::vector<int> parent, child_begin, nchild, last_bid, level_begin, pleaf_node, term_node;
@@ -708,10 +711,15 @@ int cfrb_tc_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden) {
   if (num_dice < 1 || num_faces < 1 || hidden != 256) return 0;
   long hands = 1;
   for (int i = 0; i < num_dice && hands <= 4096; ++i) hands *= num_faces;
-  if (hands > 4096 || 2L * num_dice * num_faces + 1 > 1024) return 0;     // beyond what cfrb_create accepts at all
+  if (hands > 4096 || 2L * num_dice * num_faces + 1 > 1024 || num_dice > cfrb::kMaxDice) return 0;   // beyond what cfrb_create accepts at all
   const cfrb::GameShape g(num_dice, num_faces);
   TcPlan plan;
   return tc_plan(g.H, round_up(g.Q + 1, 16), cfrb::tc::kSmemOptinSm90, false, &plan, nullptr) ? 1 : 0;
+}
+
+int cfrb_debug_kernel_path(const cfrb_handle* h) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  return h->d2 ? 0 : h->group == 32 ? 1 : 2;
 }
 
 int cfrb_num_actions(const cfrb_handle* h) { return h->g.A; }

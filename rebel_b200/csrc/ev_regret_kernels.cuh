@@ -10,7 +10,8 @@
 namespace cfrb {
 
 namespace evr {
-constexpr int kMaxBins = 9;
+constexpr int kMaxBins = 9;            // match counts 0 .. 8; bin 8 stays empty for num_dice <= kMaxDice = 7 (cfr_types.h)
+static_assert(kMaxBins >= kMaxDice + 2, "a clamped `left` must land on an empty bin");
 
 // reach_out[c] = reach_out[parent] * strategy(parent -> c) at `player`'s nodes, a copy elsewhere (compute_reach_probabilities)
 template <typename S>

@@ -110,6 +110,16 @@ def test_teacher_forced_single_step(rb, port, net_weights, D, F, state_name, net
     if net_name in ("tc", "tcx2") and max_depth != 2:
         pytest.skip("tensor-core net is exercised on the data-generation depth")
     A, H, Q = game_dims(D, F)
+    teacher_forced_steps(rb, port, net_weights, D, F, max_depth, state_name, net_name, roots=[(-1, 0), (-1, 1), (1, 1), (A - 4, 0)],
+                         cps=[0, 1, 2, 3, 4, 5, 16, 17, 18, 101, 102, 103])
+
+
+def teacher_forced_steps(rb, port, net_weights, D, F, max_depth, state_name, net_name, roots, cps):
+    """P2: for every root and every pair of consecutive checkpoints c, c + 1 in cps, load the C port's state after c iterations
+    into a one-subgame wave, run one GPU step and compare with the port's state after c + 1 iterations: bit for bit with fp64
+    tables and no net, otherwise within the noise level of the configuration (regrets, root means, last and sum strategies where
+    regret matching is well conditioned, query rows and leaf values times the scaler)."""
+    A, H, Q = game_dims(D, F)
     state = {"f64": rb.STATE_F64, "f32": rb.STATE_F32}[state_name]
     net = NETS(rb)[net_name]
     noise = noise_level(rb, state, net)
@@ -119,8 +129,6 @@ def test_teacher_forced_single_step(rb, port, net_weights, D, F, state_name, net
     if state == rb.STATE_F32 and net != rb.NET_ZERO:
         noise = 2e-4
     w = net_weights(D, F) if net != rb.NET_ZERO else None
-    cps = [0, 1, 2, 3, 4, 5, 16, 17, 18, 101, 102, 103]
-    roots = [(-1, 0), (-1, 1), (1, 1), (A - 4, 0)]
     S = rb.WaveSolver(D, F, 1, max_depth=max_depth, net_mode=net, state_dtype=state)
     if w is not None:
         S.set_weights(w)
@@ -348,16 +356,17 @@ def test_long_horizon_within_reference_noise(rb, golden, net_weights, D, F, net_
     S.close()
 
 
-@pytest.mark.parametrize("D,F", [(1, 2), (1, 3), (1, 4), (1, 6), (2, 3)])
+@pytest.mark.parametrize("D,F", [(1, 2), (1, 3), (1, 4), (1, 6), (2, 3), (1, 5), (2, 2), (3, 2), (1, 7)])
 def test_gpu_best_response_bit_exact(rb, golden, port, D, F):
     """cfrb_exploitability (SURVEY 8f-1: BRSolver::compute_br + compute_exploitability2 on the GPU) against the golden
-    exploitabilities of the compiled reference and, on random strategies over the whole tree, against the oracle."""
+    exploitabilities of the compiled reference where the fixtures hold one and, on random strategies over the whole tree (up to
+    32 767 nodes at 1x7f), against the oracle."""
     A, H, Q = game_dims(D, F)
     S = rb.WaveSolver(D, F, 1, net_mode=rb.NET_ZERO)
     if (D, F) in ((1, 2), (1, 3), (1, 4)):
         g = golden("fulltree.npz")
         assert np.array_equal(S.exploitability(g[f"avg16_{D}x{F}"]), g[f"expl_{D}x{F}_nofma"][0])
-    else:
+    elif (D, F) in ((1, 6), (2, 3)):
         g = golden("recursive_eval_zero.npz")
         ss, sr = g[f"summed_strategy_{D}x{F}"], g[f"summed_reach_{D}x{F}"]
         assert np.array_equal(S.exploitability((ss / (sr + np.float32(1e-6))).astype(np.float64)), g[f"exploitability_{D}x{F}"][-1])
@@ -379,7 +388,8 @@ def test_gpu_best_response_bit_exact(rb, golden, port, D, F):
 
 @pytest.mark.parametrize("state_name", ["f64", "f32"])
 def test_full_tree_exploitability_1x4f(rb, golden, port, state_name):
-    """BASELINE config 0 on the GPU: full-depth 1x4f tree (511 nodes, CTA-per-subgame path), 1024 linear-CFR iterations,
+    """BASELINE config 0 on the GPU: full-depth 1x4f tree (511 nodes; with fp64 tables the warp-per-subgame path with HC = 4,
+    test_game_matrix), 1024 linear-CFR iterations,
     exploitability of the average strategy evaluated by the oracle's best response."""
     g = golden("fulltree.npz")
     D, F = 1, 4

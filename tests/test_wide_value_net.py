@@ -1,7 +1,7 @@
 """The tensor-core value net on games with more than 16 hands (leaf_mlp_tc_wide.cuh): 2x5f, 3x3f, 5x2f, 2x6f, 1x17f .. 1x32f.
 
 CPU: which games have a tensor-core net (cfrb_tc_net_supported, the rule cfrb_create and `rela` share).
-GPU: zero-net CFR at H > 16 against the C port, rows independent of their tile, the wide kernel bit-identical to the resident
+GPU: rows independent of their tile, the wide kernel bit-identical to the resident
 kernel where both apply (CFRB_TC_WIDE=1), layer taps against a host computation, one teacher-forced CFR step, and the `rela`
 data-generation loop running the tensor-core net at 2x5f with the example distribution of the fp32 net.
 """
@@ -54,37 +54,14 @@ def test_tc_net_supported():
         assert not capi.tc_net_supported(D, F), (D, F)
     assert not capi.tc_net_supported(2, 5, hidden=128)          # only n_hidden = 256 is built
     assert not capi.tc_net_supported(0, 5) and not capi.tc_net_supported(2, 0)
+    for D, F in [(8, 1), (9, 1), (8, 2)]:                       # more than 7 dice: cfrb_create refuses the game itself
+        assert not capi.tc_net_supported(D, F), (D, F)
 
 
 # ---------------------------------------------------------------------------------------------- GPU
 def _beliefs(rng, n, H):
     b = rng.rand(n, 2, H)
     return b / b.sum(-1, keepdims=True)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("D,F", [(2, 5), (3, 3)])
-def test_zero_net_cfr_bit_exact_above_16_hands(rb, port, D, F):
-    """fp64 tables, zero net, depth 2: 64-iteration trajectories of several roots in one wave are bit-identical to the C port
-    (the generic-H path of the CFR kernels at H = 25 / 27)."""
-    A, H, Q = game_dims(D, F)
-    roots = [(-1, 0), (-1, 1), (2, 1), (A - 6, 0), (A - 3, 1)]
-    cps = [1, 2, 16, 64]
-    rng = np.random.RandomState(11)
-    b = _beliefs(rng, len(roots), H)
-    S = rb.WaveSolver(D, F, len(roots), net_mode=rb.NET_ZERO)
-    S.begin([r[0] for r in roots], [r[1] for r in roots], b)
-    want = [port.cfr_solve(D, F, b[i], cps, lb, pl, num_iters=max(cps)) for i, (lb, pl) in enumerate(roots)]
-    done = 0
-    for ci, c in enumerate(cps):
-        S.run(c - done); done = c
-        f = S.fetch(("root_means", "last", "sum", "regrets", "avg"))
-        for i, o in enumerate(want):
-            N = o["tree"].shape[0]
-            for k in ("regrets", "last", "sum", "avg"):
-                assert np.array_equal(f[k][i, :N], o[k][ci]), (D, F, roots[i], c, k, np.abs(f[k][i, :N] - o[k][ci]).max())
-            assert np.array_equal(f["root_means"][i], o["root_means"][ci]), (D, F, roots[i], c)
-    S.close()
 
 
 @pytest.mark.gpu
