@@ -125,6 +125,12 @@ int cfrb_destroy(cfrb_handle* h);
  * game on an sm_90 device, else 0 (cfrb_create then fails with CFRB_EINVAL for those modes; CFRB_NET_FP32 serves every game). */
 int cfrb_tc_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden);
 
+/* Host-only: a bound B >= |output| of the tensor-core value net with these weights (cfrb_set_weights layout) over every query
+ * row, +inf when none holds (a weight that is not finite); -1 for a bad shape or weight count.  The depth-2 CFR kernel leaves out of
+ * the net's rows every pseudo-leaf whose opponent-reach scaler s has s * B <= 2^-151: its leaf values (float)(net * s) are +-0
+ * whatever the net returns. */
+double cfrb_net_output_bound(int32_t num_dice, int32_t num_faces, int32_t hidden, const float* flat, size_t n);
+
 /* Shape queries. */
 int cfrb_num_actions(const cfrb_handle* h);   /* A */
 int cfrb_num_hands(const cfrb_handle* h);     /* H */
@@ -258,6 +264,9 @@ int cfrb_regrets_fetch(cfrb_handle* h, double* immediate, double* sums, int64_t*
 /* Counters for bench.py: kernels launched by this handle since creation, and leaf rows of the wave. */
 int64_t cfrb_kernel_launches(const cfrb_handle* h);
 int64_t cfrb_wave_leaf_rows(const cfrb_handle* h);
+/* Value-net rows evaluated by this handle since creation (the wave's leaf rows minus those left out as dead, over all iterations);
+ * counted where the depth-2 kernel feeds a tensor-core net, CFRB_EINVAL elsewhere. */
+int64_t cfrb_net_rows_evaluated(const cfrb_handle* h);
 /* Timing marks (benchmarks): record CUDA event `slot` (0..7) on `cuda_stream` (NULL = the handle's stream); device time
  * between two recorded marks (waits for the second). */
 int cfrb_mark(cfrb_handle* h, int32_t slot, void* cuda_stream);
@@ -323,6 +332,8 @@ int cfrb_schedule_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, 
 /* Test aid: run the depth <= 2 CFR kernel on at most max_ctas CTAs (0 = as many as are resident at once), so that every warp
  * solves many subgames per launch.  Returns the number of CTAs resident at once. */
 int cfrb_debug_d2_grid(cfrb_handle* h, int32_t max_ctas);
+/* Test aid: skip = 0 makes the value net evaluate every pseudo-leaf row, dead or not, from the next cfrb_set_weights on. */
+int cfrb_debug_skip_dead_rows(cfrb_handle* h, int32_t skip);
 /* Block until the work enqueued on `cuda_stream` (NULL = the handle's stream) has finished. */
 int cfrb_stream_wait(cfrb_handle* h, void* cuda_stream);
 

@@ -86,6 +86,11 @@ def lib():
     L.cfrb_kernel_launches.restype = C.c_int64
     L.cfrb_wave_leaf_rows.argtypes = [vp]
     L.cfrb_wave_leaf_rows.restype = C.c_int64
+    L.cfrb_net_rows_evaluated.argtypes = [vp]
+    L.cfrb_net_rows_evaluated.restype = C.c_int64
+    L.cfrb_net_output_bound.argtypes = [C.c_int32] * 3 + [_fp, C.c_size_t]
+    L.cfrb_net_output_bound.restype = C.c_double
+    L.cfrb_debug_skip_dead_rows.argtypes = [vp, C.c_int32]
     L.cfrb_last_run_ms.argtypes = [vp, _fp, _fp]
     L.cfrb_selfplay_create.argtypes = [vp, C.c_int32, C.POINTER(C.c_uint32), C.c_float, C.c_int32]
     L.cfrb_selfplay_wave.argtypes = [vp, vp, vp, C.c_int32, vp]
@@ -168,6 +173,16 @@ def to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames):
     """Host-only: device bytes WaveSolver.to_leaf_exploitability needs beyond a handle of these sizes (full tree, best-response
     scratch, the walk's largest levels)."""
     return _check(lib().cfrb_to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames))
+
+
+def net_output_bound(num_dice, num_faces, flat, hidden=256):
+    """Host-only: the bound B >= |output| of the tensor-core value net with these weights over every query row (inf: none holds).
+    A pseudo-leaf whose opponent-reach scaler s has s * B <= 2^-151 is not evaluated: its leaf values are +-0 whatever the net returns."""
+    w = np.ascontiguousarray(flat, np.float32)
+    b = lib().cfrb_net_output_bound(num_dice, num_faces, hidden, _p(w, _fp), w.size)
+    if b < 0:
+        raise CfrbError("net_output_bound: bad game shape or weight count")
+    return b
 
 
 def tc_net_supported(num_dice, num_faces, hidden=256):
@@ -324,6 +339,16 @@ class WaveSolver:
     @property
     def leaf_rows(self):
         return lib().cfrb_wave_leaf_rows(self._h)
+
+    @property
+    def net_rows_evaluated(self):
+        """Value-net rows evaluated since the handle was created: the waves' leaf rows over all iterations, less the dead ones left
+        out (depth-2 kernel with a tensor-core net only)."""
+        return _check(lib().cfrb_net_rows_evaluated(self._h))
+
+    def debug_skip_dead_rows(self, skip):
+        """Test aid: skip=False makes the value net evaluate every row, dead or not, from the next set_weights on."""
+        _check(lib().cfrb_debug_skip_dead_rows(self._h, int(bool(skip))))
 
     # ---- device-resident self-play (cfrb_selfplay_*)
     def selfplay_create(self, seeds, random_action_prob=0.25, sample_leaf=True):

@@ -788,8 +788,17 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
   real* par_inv = aux + p.n1max;
   __half* qpar = reinterpret_cast<__half*>(reinterpret_cast<unsigned char*>(aux) + ((2 * p.n1max * (int)sizeof(real) + 15) & ~15));
   __half* qown = qpar + p.n1max * H;
+  int* rowpos = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(qpar) + (((p.n1max + p.lmax) * H * 2 + 3) & ~3));
   const int opp = 1 - trav;
   const bool have_l2 = lv.n2e > lv.n1e;
+  // Dead leaves (compacted tiles only): the backward half forms the leaf values (float)(net_out * scaler).  With |net_out| <= B
+  // (cfrb_set_weights) and scaler * B <= 2^-151 that product rounds to +-0 whatever the net returns, so the net need not see the
+  // row.  Bit i of live_bits: leaf lane + 32 i is live.
+  const double bound = p.row_src != nullptr ? *p.net_bound : 0.0;
+  unsigned live_bits = 0;
+  auto mark_live = [&](int r, real sc) {
+    if (!((double)sc * bound <= 0x1p-151)) live_bits |= 1u << (r >> 5);
+  };
   if (have_l2) {
     for (int i = lane; i < n1; i += G) {
       const real* r = slot + (1 + i) * H;
@@ -811,7 +820,9 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
       real s1 = 0, e1 = 0;
       for (int h = 0; h < H; ++h) { s1 += ro[h]; e1 += ro[h] + Eps<real>::v; }
       const real inv = (real)1 / e1;
-      p.scaler[row0 + r] = (opp == rp) ? par_sum[parent[n] - 1] : s1;                         // sum of the opponent's reach (:264-268)
+      const real sc = (opp == rp) ? par_sum[parent[n] - 1] : s1;                              // sum of the opponent's reach (:264-268)
+      p.scaler[row0 + r] = sc;
+      mark_live(r, sc);
       for (int h = 0; h < H; ++h) {
         float f;
         if (Eps<real>::kLiteral) f = (float)((ro[h] + Eps<real>::v) * inv);
@@ -830,6 +841,7 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
       for (int h = 0; h < H; ++h) { s0 += r0[h]; s1 += r1[h]; e0 += r0[h] + Eps<real>::v; e1 += r1[h] + Eps<real>::v; }
       const real i0 = (real)1 / e0, i1 = (real)1 / e1;
       p.scaler[row0 + r] = trav == 0 ? s1 : s0;
+      mark_live(r, trav == 0 ? s1 : s0);
       // qpar <- the root player's columns, qown <- the other player's, like on level 2 (one qpar row per leaf here)
       const real* rr = rp == 0 ? r0 : r1; const real* ro = rp == 0 ? r1 : r0;
       const real ir = rp == 0 ? i0 : i1, io_ = rp == 0 ? i1 : i0;
@@ -840,6 +852,37 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
         qpar[r * H + h] = __float2half_rn(fr);
         qown[r * H + h] = __float2half_rn(fo);
       }
+    }
+  }
+  if (p.row_src != nullptr && t.L > 0) {
+    // Query-tile rows of the leaves: the live ones packed from row 0 up, the dead ones from the last row down (their queries stay
+    // readable for the debug readers), each range taken with one atomic per subgame.  The net evaluates only rows < live[trav] and
+    // writes row i's outputs to net_out[row_src[i]]; a dead leaf's outputs are +0 here, so net_out and scaler keep the wave's row
+    // order and the backward half reads them as before.
+    const int rounds = (t.L + 31) >> 5;
+    const unsigned lt = (1u << lane) - 1u;
+    int nlive = 0;
+    for (int i = 0; i < rounds; ++i) nlive += __popc(__ballot_sync(0xffffffffu, (live_bits >> i) & 1u));
+    int base = 0;
+    if (lane == 0) base = atomicAdd(&p.net_rows->live[trav], nlive);
+    if (lane == 1) base = atomicAdd(&p.net_rows->dead[trav], t.L - nlive);
+    const int base_live = __shfl_sync(0xffffffffu, base, 0), base_dead = __shfl_sync(0xffffffffu, base, 1);
+    int before = 0;                                             // live leaves among 0 .. 32 i - 1
+    for (int i = 0; i < rounds; ++i) {
+      const unsigned b = __ballot_sync(0xffffffffu, (live_bits >> i) & 1u);
+      const int r = 32 * i + lane;
+      if (r < t.L) {
+        const int lr = before + __popc(b & lt);                 // live leaves before r
+        const bool live = (live_bits >> i) & 1u;
+        const int pos = live ? base_live + lr : p.xh_rows - 1 - (base_dead + r - lr);
+        rowpos[r] = pos;
+        p.row_src[pos] = row0 + r;
+        if (!live) {
+          float4* o = reinterpret_cast<float4*>(p.net_out + (size_t)(row0 + r) * p.Hout);
+          for (int c = 0; c < p.Hout / 4; ++c) o[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+      }
+      before += __popc(b);
     }
   }
   __syncwarp();
@@ -871,7 +914,7 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
           else if (q >= qb1 && q < qb2) c.h[j] = p1[q - qb1];
         }
       }
-      const int Rr = row0 + r, rr = Rr & 127;
+      const int Rr = p.row_src != nullptr ? rowpos[r] : row0 + r, rr = Rr & 127;
       *reinterpret_cast<int4*>(p.Xh + (size_t)(Rr >> 7) * 128 * Qp + k8 * 1024 + (rr >> 3) * 64 + (rr & 7) * 8) = c.v;
     }
   } else if (p.X != nullptr) {
@@ -985,6 +1028,13 @@ __global__ void __launch_bounds__(128, 8) cfr_iter_d2_kernel(CfrDev<real> p, int
     // ... and this grid, launched the same way behind the previous value-net kernel, must not touch that kernel's outputs (or
     // tables a still earlier CFR launch wrote) before the kernel has completed.  A no-op for ordinary launches.
     if (first) asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (p.net_rows != nullptr && ticket == 0 && lane == 0) {
+      // the value net of iteration iter - 1 has completed: account for its rows and clear its slot for the next launch's forward half
+      NetRows* c = p.net_rows;
+      const int s = (iter + 1) & 1;
+      if (do_b) { c->evaluated += (unsigned long long)c->live[s]; c->last_live = c->live[s]; }
+      c->live[s] = 0; c->dead[s] = 0;
+    }
     __syncwarp();
     const int tb = (iter - 1) & 1;
     const int rp = p.sg_player[k];

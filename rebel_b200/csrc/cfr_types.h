@@ -17,6 +17,17 @@ struct TemplateDev {
   int qconst_off, pad_[3];
 };
 
+// Row counters of the compacted query tiles (cfr_iter_d2_kernel with the tensor-core net).  The forward half of iteration i packs
+// the rows the value net must evaluate ("live") at the front of the tiles and the others ("dead") at the back, counting both in
+// slot i & 1; the value net of iteration i reads live[i & 1].  The CFR launch of iteration i + 1 adds live[i & 1] to `evaluated`
+// and clears slot i & 1 (its forward half fills the other slot), so both slots are zero between runs.
+struct NetRows {
+  int live[2], dead[2];
+  int last_live;                  // live rows of the last forward half of the most recent run
+  int pad_;
+  unsigned long long evaluated;   // rows the value net has evaluated, summed over the handle's runs
+};
+
 template <typename real>
 struct CfrDev {
   // game
@@ -41,8 +52,13 @@ struct CfrDev {
   real* vterm; int vterm_stride;  // [K][Tmax*H] terminal payoffs of the current iteration
   float* X;                       // [rows][Qpad] fp32 query rows (SIMT net) -- or nullptr
   __half* Xh;                     // fp16 query tiles in wgmma core-matrix order (tensor-core net) -- or nullptr
-  const float* net_out;           // [rows][Hout] raw net outputs
+  float* net_out;                 // [rows][Hout] raw net outputs
   real* scaler;                   // [rows] sum of opponent reach at the pseudo-leaf
+  // Compaction of the fp16 query tiles (depth-2 kernel, tensor-core net) -- or nullptr: every row at its wave position.
+  NetRows* net_rows;
+  int* row_src;                   // [xh_rows] wave row of each query-tile row
+  int xh_rows;                    // query-tile rows allocated (a multiple of 128)
+  const double* net_bound;        // [1] bound on |net output| of the current weights (cfrb_set_weights), +inf = none known
   real* scratch; size_t scratch_stride;   // global scratch (CTA groups), reals per subgame
   int nh_max, tmp_reals;                  // scratch layout: bufA[nh_max] | bufB[nh_max] | tmp[tmp_reals] | lsum[2*Lmax]
   int lmax, tmax, n1max;                  // largest pseudo-leaf / terminal / level-1 node count over the templates (depth <= 2 kernels' layouts)
@@ -61,9 +77,11 @@ __host__ __device__ inline int cfr_scratch_reals(int N, int H, int L, int T) { r
 
 // Depth <= 2 kernel (cfr_iter_d2_kernel): slot[N*H] | bel[2*H] | aux.  aux (bytes) serves the backward half as
 // rcp[(n1max + 1) * H] reals (reciprocals of the regret-matching sums) and the forward half first as par_sum[n1max] | par_inv[n1max]
-// reals followed by the fp16 belief columns qpar[n1max * H] | qown[L * H], then as the terminal histogram hist[10 * T] reals.
+// reals followed by the fp16 belief columns qpar[n1max * H] | qown[L * H] and the leaves' query-tile rows rowpos[L] (int), then as
+// the terminal histogram hist[10 * T] reals.
 __host__ __device__ inline int cfr_aux_bytes_d2(int sz, int H, int L, int T, int n1max) {
-  const int fwd = ((2 * n1max * sz + 15) & ~15) + (((n1max + (L > 0 ? L : 1)) * H * 2 + 15) & ~15);
+  const int l1 = L > 0 ? L : 1;
+  const int fwd = ((2 * n1max * sz + 15) & ~15) + (((n1max + l1) * H * 2 + 3) & ~3) + 4 * l1;
   const int bwd = (n1max + 1) * H * sz;
   const int hist = 10 * (T > 0 ? T : 1) * sz;
   int m = fwd > bwd ? fwd : bwd;

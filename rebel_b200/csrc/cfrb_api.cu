@@ -202,6 +202,12 @@ struct cfrb_handle {
   int x2_gelu = 2;                  // GELU variant of CFRB_NET_TC_F16X2 (leaf_mlp_tc.cuh kGelu): 2 = fp32 tanh, 1 = packed half
   TcPlan tc;                        // which tensor-core kernel serves the game (tc_plan)
   DevBuf<__half> d_Xh;
+  // Compacted query tiles (CfrDev::row_src): the depth-2 kernel feeding a tensor-core net packs the rows the net must evaluate
+  bool compact = false;
+  bool skip_dead = true;            // test aid (cfrb_debug_skip_dead_rows): false = the bound is +inf, so every row is evaluated
+  DevBuf<int> d_row_src;
+  DevBuf<cfrb::NetRows> d_net_rows;
+  DevBuf<double> d_net_bound;       // written by cfrb_set_weights on own_stream, behind the weights it bounds
   WaveState<float> sf;
   WaveState<double> sd;
   // device: weights
@@ -334,6 +340,11 @@ static int alloc_state(cfrb_handle* h, WaveState<real>& s, int max_optin) {
   d.X = h->cfg.net_mode == CFRB_NET_FP32 ? h->d_X.p : nullptr;
   d.Xh = is_tc(h->cfg.net_mode) ? h->d_Xh.p : nullptr;
   d.net_out = h->d_out.p; d.scaler = s.scaler.p;
+  h->compact = h->d2 && is_tc(h->cfg.net_mode);
+  d.net_rows = h->compact ? h->d_net_rows.p : nullptr;
+  d.row_src = h->compact ? h->d_row_src.p : nullptr;
+  d.xh_rows = (int)h->d_row_src.n;
+  d.net_bound = h->d_net_bound.p;
   d.scratch = h->group == 32 ? nullptr : s.scratch.p; d.scratch_stride = h->scratch_per_group;
   d.nh_max = h->Nmax * g.H; d.tmp_reals = cfrb::cfr_tmp_reals(h->Nmax, g.H, h->Lmax, h->Tmax);
   d.linear = h->cfg.linear_update; d.dcfr = h->cfg.dcfr;
@@ -522,7 +533,45 @@ static int sync_mirror(cfrb_handle* h) {
   return CFRB_OK;
 }
 
+// A bound B >= |out_h| of the tensor-core net for every query row and output h < H, from the parameters its kernels use (flat:
+// the cfrb_set_weights layout).  The mean-free LayerNorm divides the 256 features of layer 2 by their root mean square, so
+// |y_j * rstd| <= sqrt(256) = 16 and the affine gives |z_j| <= 16 |gamma_j| + |beta_j|; GELU(z) lies in [-0.17, max(z, 0)], and the
+// activation is rounded to fp16 (2^-11 relative), so |act_j| <= (16 |gamma_j| + |beta_j| + 0.2) (1 + 2^-10).  Then |out_h| <=
+// |b3_h| + sum_j |W3_hj| |act_j| with W3 rounded to fp16 as the kernels hold it; the factor 2 covers the fp32 accumulation and the
+// approximate rstd and GELU.  +inf where no bound holds: a parameter that is not finite, or an activation beyond fp16's range.
+static double net_output_bound(const float* flat, int Q, int H, int hid) {
+  const size_t n = (size_t)hid * Q + 3 * hid + (size_t)hid * hid + 3 * hid + (size_t)H * hid + H;
+  const double inf = std::numeric_limits<double>::infinity();
+  for (size_t i = 0; i < n; ++i)
+    if (!std::isfinite(flat[i])) return inf;
+  const float* g2 = flat + (size_t)hid * Q + 3 * hid + (size_t)hid * hid + hid;
+  const float* be2 = g2 + hid; const float* w3 = be2 + hid; const float* b3 = w3 + (size_t)H * hid;
+  std::vector<double> act(hid);
+  for (int j = 0; j < hid; ++j) {
+    act[j] = (16.0 * std::fabs((double)g2[j]) + std::fabs((double)be2[j]) + 0.2) * (1.0 + std::ldexp(1.0, -10));
+    if (act[j] > 65504.0) return inf;
+  }
+  double B = 0.0;
+  for (int o = 0; o < H; ++o) {
+    double s = std::fabs((double)b3[o]);
+    for (int j = 0; j < hid; ++j) s += std::fabs((double)__half2float(__float2half_rn(w3[(size_t)o * hid + j]))) * act[j];
+    B = std::max(B, s);
+  }
+  B *= 2.0;
+  return B < 1e30 ? B : inf;
+}
+
 extern "C" {
+
+double cfrb_net_output_bound(int32_t num_dice, int32_t num_faces, int32_t hidden, const float* flat, size_t n) {
+  if (num_dice < 1 || num_faces < 1 || num_dice > cfrb::kMaxDice || hidden < 1 || !flat) return -1.0;
+  long hands = 1;
+  for (int i = 0; i < num_dice && hands <= 4096; ++i) hands *= num_faces;
+  if (hands > 4096) return -1.0;
+  const cfrb::GameShape g(num_dice, num_faces);
+  if (n !=(size_t)hidden * g.Q + 3 * hidden + (size_t)hidden * hidden + 3 * hidden + (size_t)g.H * hidden + g.H) return -1.0;
+  return net_output_bound(flat, g.Q, g.H, hidden);
+}
 
 const char* cfrb_last_error(void) { return g_err.c_str(); }
 
@@ -672,6 +721,12 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
     const size_t tiles = (rows_cap + cfrb::tc::kTileM - 1) / cfrb::tc::kTileM;
     CK(h->d_Xh.alloc(tiles * cfrb::tc::kTileM * h->Qpad));
     CK(cudaMemset(h->d_Xh.p, 0, tiles * cfrb::tc::kTileM * h->Qpad * sizeof(__half)));
+    CK(h->d_row_src.alloc(tiles * cfrb::tc::kTileM));
+    CK(h->d_net_rows.alloc(1));
+    CK(cudaMemset(h->d_net_rows.p, 0, sizeof(cfrb::NetRows)));
+    CK(h->d_net_bound.alloc(1));
+    const double no_bound = std::numeric_limits<double>::infinity();
+    CK(cudaMemcpy(h->d_net_bound.p, &no_bound, sizeof(double), cudaMemcpyHostToDevice));
     CK(h->d_dbg.alloc(2 * cfrb::tc::kTileM * cfrb::tc::kHid));
     // the limit is per kernel and process-wide: raised to the device's opt-in maximum (see cfr_configure in cfr_kernels.cu)
     const int sm = std::max(h->tc.smem_bytes, max_optin);
@@ -772,7 +827,8 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
   const size_t total_fp32 = (size_t)Qp * hid + 3 * hid + (size_t)hid * hid + 3 * hid + (size_t)hid * h->Hout + h->Hout;
   // tensor-core blob: the resident kernel's layout, or the wide kernel's (W3 with tc.nout rows); with 16 outputs the two agree
   const cfrb::tc::WideLayout L(Qp, h->tc.nout);
-  const size_t need = is_tc(h->cfg.net_mode) ? (size_t)L.blob_bytes : total_fp32 * sizeof(float);
+  const size_t bound_off = ((size_t)L.blob_bytes + 7) / 8 * 8;     // the output bound is staged behind the blob
+  const size_t need = is_tc(h->cfg.net_mode) ? bound_off + sizeof(double) : total_fp32 * sizeof(float);
   if (h->w_stage_bytes < need) {
     CK(cudaStreamSynchronize(h->own_stream));
     for (int i = 0; i < 2; ++i) {
@@ -820,6 +876,9 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
     std::copy(b3, b3 + H, reinterpret_cast<float*>(blob.data() + L.off_b3));
     if (!h->d_blob.p) CK(h->d_blob.alloc(L.blob_bytes));
     CK(cudaMemcpyAsync(h->d_blob.p, blob.data(), L.blob_bytes, cudaMemcpyHostToDevice, h->own_stream));
+    double* bound = reinterpret_cast<double*>(blob.data() + bound_off);
+    *bound = h->skip_dead ? net_output_bound(flat, Q, H, hid) : std::numeric_limits<double>::infinity();
+    CK(cudaMemcpyAsync(h->d_net_bound.p, bound, sizeof(double), cudaMemcpyHostToDevice, h->own_stream));
   } else {
     // transposed k-major fp32 weights for the SIMT kernel
     const size_t total = (size_t)Qp * hid + 3 * hid + (size_t)hid * hid + 3 * hid + (size_t)hid * h->Hout + h->Hout;
@@ -915,7 +974,15 @@ static int reserve_net_events(cfrb_handle* h, int count) {
   return CFRB_OK;
 }
 
-static int launch_net(cfrb_handle* h, cudaStream_t st, float* dbg1, float* dbg2) {
+// Query tiles, row count, row map and outputs of a tensor-core value-net launch.
+struct NetIo { const __half* xh; const int* rows; const int* row_src; float* out; };
+// What the forward half of iteration `iter` left for the net: compacted tiles and that iteration's live-row count, or the wave's rows.
+static NetIo wave_net_io(const cfrb_handle* h, int iter) {
+  if (h->compact) return {h->d_Xh.p, h->d_net_rows.p->live + (iter & 1), h->d_row_src.p, h->d_out.p};
+  return {h->d_Xh.p, h->d_wave.p + 1, nullptr, h->d_out.p};
+}
+
+static int launch_net(cfrb_handle* h, cudaStream_t st, const NetIo& io, float* dbg1, float* dbg2) {
   if (h->cfg.net_mode == CFRB_NET_ZERO || (h->rows == 0 && !h->rows_on_device)) return CFRB_OK;
   const bool sample = h->profiling > 0 && (h->net_launch_idx % h->profiling) == 0;
   ++h->net_launch_idx;
@@ -925,7 +992,7 @@ static int launch_net(cfrb_handle* h, cudaStream_t st, float* dbg1, float* dbg2)
     CK(record_event(h, h->net_ev[h->net_ev_used], st));
   }
   if (is_tc(h->cfg.net_mode)) {
-    cfrb::tc::TcArgs a{h->d_blob.p, h->d_Xh.p, h->d_wave.p + 1, h->d_out.p, h->Qpad, h->g.H, h->Hout, dbg1, dbg2, nullptr};
+    cfrb::tc::TcArgs a{h->d_blob.p, io.xh, io.rows, io.row_src, io.out, h->Qpad, h->g.H, h->Hout, dbg1, dbg2, nullptr};
     const int tiles = (h->rows + cfrb::tc::kTileM - 1) / cfrb::tc::kTileM;
     const int grid = (h->capturing || h->rows_on_device) ? h->num_sms : std::min(tiles, h->num_sms);   // surplus CTAs return at once
     const bool x2 = h->cfg.net_mode == CFRB_NET_TC_F16X2;
@@ -985,7 +1052,7 @@ static int enqueue_run(cfrb_handle* h, cudaStream_t st, int first, int last) {
     const int do_b = i > first, do_f = i < last;
     int rc = with_state(h, [&](auto& s) { return launch_iter(h, s, st, i, do_b, do_f); });
     if (rc) return rc;
-    if (do_f) { rc = launch_net(h, st, nullptr, nullptr); if (rc) return rc; }
+    if (do_f) { rc = launch_net(h, st, wave_net_io(h, i), nullptr, nullptr); if (rc) return rc; }
   }
   CK(record_event(h, h->ev_b, st));
   h->net_launches_run = h->net_launch_idx;
@@ -1160,16 +1227,64 @@ int cfrb_load_state(cfrb_handle* h, const double* regrets, const double* last_st
   return CFRB_OK;
 }
 
+// The query tiles of the last forward half in wave row order (row r in tile r / 128), on the host.  Compacted tiles hold the
+// rows the net evaluated at the front and the others at the back (CfrDev::row_src); they are put back in place here.
+static int dense_tiles(cfrb_handle* h, std::vector<__half>& x) {
+  const size_t pos = h->d_row_src.n > 0 ? h->d_row_src.n : h->d_Xh.n / h->Qpad;   // query-tile rows allocated
+  const size_t Qp = h->Qpad, R = cfrb::tc::kTileM;
+  x.assign(pos * Qp, __float2half_rn(0.f));
+  CK(cudaMemcpy(x.data(), h->d_Xh.p, x.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+  if (!h->compact) return CFRB_OK;
+  std::vector<int> src(pos);
+  CK(cudaMemcpy(src.data(), h->d_row_src.p, pos * sizeof(int), cudaMemcpyDeviceToHost));
+  cfrb::NetRows c{};
+  CK(cudaMemcpy(&c, h->d_net_rows.p, sizeof(c), cudaMemcpyDeviceToHost));
+  const size_t rows = (size_t)h->rows, live = std::min<size_t>((size_t)std::max(c.last_live, 0), rows);
+  std::vector<__half> d(x.size(), __float2half_rn(0.f));
+  auto place = [&](size_t p) {
+    const int r = src[p];
+    if (r < 0 || (size_t)r >= rows) return;
+    for (size_t q = 0; q < Qp; ++q)
+      d[(size_t)(r / R) * R * Qp + cfrb::tc::umma_kmajor_offset_halves(r % R, (int)q, (int)R)] =
+          x[(p / R) * R * Qp + cfrb::tc::umma_kmajor_offset_halves((int)(p % R), (int)q, (int)R)];
+  };
+  for (size_t p = 0; p < live; ++p) place(p);
+  for (size_t p = pos - (rows - live); p < pos; ++p) place(p);
+  x.swap(d);
+  return CFRB_OK;
+}
+
+// Inputs of a debug launch of the tensor-core net (taps, trace): the tiles in wave row order, so that tile 0 holds rows 0 .. 127, and
+// an output buffer of its own (the wave's net_out keeps the +0 rows of a compacting forward half).
+struct DenseNet {
+  DevBuf<__half> xh;
+  DevBuf<float> out;
+  NetIo io{};
+};
+static int dense_net(cfrb_handle* h, DenseNet* d, std::vector<__half>* tiles = nullptr) {
+  if (!h->compact) { d->io = wave_net_io(h, 0); return CFRB_OK; }
+  int rc = sync_mirror(h);
+  if (rc) return rc;
+  std::vector<__half> own;
+  std::vector<__half>& x = tiles ? *tiles : own;
+  if (x.empty() && (rc = dense_tiles(h, x))) return rc;
+  CK(d->xh.alloc(x.size()));
+  CK(cudaMemcpy(d->xh.p, x.data(), x.size() * sizeof(__half), cudaMemcpyHostToDevice));
+  CK(d->out.alloc(h->d_out.n));
+  d->io = {d->xh.p, h->d_wave.p + 1, nullptr, d->out.p};
+  return CFRB_OK;
+}
+
 int cfrb_debug_leaf_io(cfrb_handle* h, float* queries, float* net_out, double* scalers, int32_t cap_rows) {
   if (!h) return fail(CFRB_EINVAL, "null handle");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaDeviceSynchronize());
   { int rc = sync_mirror(h); if (rc) return rc; }
   const int rows = std::min<int>(h->rows, cap_rows), Q = h->g.Q;
+  std::vector<__half> x;
   if (rows > 0 && queries && is_tc(h->cfg.net_mode)) {
-    const int tiles = (rows + cfrb::tc::kTileM - 1) / cfrb::tc::kTileM;
-    std::vector<__half> x((size_t)tiles * cfrb::tc::kTileM * h->Qpad);
-    CK(cudaMemcpy(x.data(), h->d_Xh.p, x.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+    const int rc = dense_tiles(h, x);
+    if (rc) return rc;
     for (int r = 0; r < rows; ++r)
       for (int q = 0; q < Q; ++q)
         queries[(size_t)r * Q + q] = __half2float(x[(size_t)(r >> 7) * cfrb::tc::kTileM * h->Qpad +
@@ -1180,8 +1295,21 @@ int cfrb_debug_leaf_io(cfrb_handle* h, float* queries, float* net_out, double* s
     for (int r = 0; r < rows; ++r) std::memcpy(queries + (size_t)r * Q, x.data() + (size_t)r * h->Qpad, Q * sizeof(float));
   }
   if (rows > 0 && net_out) {
+    // compacted tiles: the net's outputs of every row, the left-out ones included, from a launch on the tiles in wave row order
+    DenseNet dn;
+    const float* src = h->d_out.p;
+    if (h->compact && h->have_weights) {
+      const int prof = h->profiling;
+      h->profiling = 0;
+      int rc = dense_net(h, &dn, &x);
+      if (!rc) rc = launch_net(h, h->own_stream, dn.io, nullptr, nullptr);
+      h->profiling = prof;
+      if (rc) return rc;
+      CK(cudaStreamSynchronize(h->own_stream));
+      src = dn.out.p;
+    }
     std::vector<float> o((size_t)rows * h->Hout);
-    CK(cudaMemcpy(o.data(), h->d_out.p, o.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(o.data(), src, o.size() * sizeof(float), cudaMemcpyDeviceToHost));
     for (int r = 0; r < rows; ++r) std::memcpy(net_out + (size_t)r * h->g.H, o.data() + (size_t)r * h->Hout, h->g.H * sizeof(float));
   }
   if (rows > 0 && scalers) {
@@ -1202,8 +1330,11 @@ int cfrb_debug_net_trace(cfrb_handle* h, long long* out, int n) {
   CK(cudaMemset(d.p, 0, 2048 * sizeof(long long)));
   const int prof = h->profiling;
   h->profiling = 0;
+  DenseNet dn;
+  int rc = dense_net(h, &dn);
+  if (rc) return rc;
   h->dbg_trace = d.p;
-  int rc = launch_net(h, h->own_stream, nullptr, nullptr);
+  rc = launch_net(h, h->own_stream, dn.io, nullptr, nullptr);
   h->dbg_trace = nullptr;
   h->profiling = prof;
   if (!rc && cudaStreamSynchronize(h->own_stream) != cudaSuccess) rc = fail(CFRB_ECUDA, "trace launch failed");
@@ -1219,7 +1350,9 @@ int cfrb_debug_net_taps(cfrb_handle* h, float* d1, float* d2) {
   const size_t n = (size_t)cfrb::tc::kTileM * cfrb::tc::kHid;
   const int prof = h->profiling;
   h->profiling = 0;
-  int rc = launch_net(h, h->own_stream, h->d_dbg.p, h->d_dbg.p + n);
+  DenseNet dn;
+  int rc = dense_net(h, &dn);
+  if (!rc) rc = launch_net(h, h->own_stream, dn.io, h->d_dbg.p, h->d_dbg.p + n);
   h->profiling = prof;
   if (rc) return rc;
   CK(cudaStreamSynchronize(h->own_stream));
@@ -1435,6 +1568,25 @@ int64_t cfrb_wave_leaf_rows(const cfrb_handle* h) {
     return wave[1];
   }
   return h->rows;
+}
+
+int64_t cfrb_net_rows_evaluated(const cfrb_handle* h) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  if (!h->compact) return fail(CFRB_EINVAL, "evaluated rows are counted only where the depth-2 kernel feeds a tensor-core net");
+  cfrb::NetRows c{};
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+      cudaMemcpy(&c, h->d_net_rows.p, sizeof(c), cudaMemcpyDeviceToHost) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(CFRB_ECUDA, "cfrb_net_rows_evaluated: device read failed");
+  }
+  return (int64_t)c.evaluated;
+}
+
+// Test aid: skip = 0 makes the next cfrb_set_weights upload an infinite output bound, so the value net evaluates every row.
+int cfrb_debug_skip_dead_rows(cfrb_handle* h, int32_t skip) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  h->skip_dead = skip != 0;
+  return CFRB_OK;
 }
 
 // Timing marks: CUDA events recorded on the launching stream (NULL = the handle's stream); elapsed device time between two.

@@ -76,10 +76,6 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_wide_kernel(TcArgs a)
   const WideLayout L(a.Kp, kNo);
   // warp-uniform through a shuffle, as in leaf_mlp_tc_kernel: branches on wg do not serialise the wgmmas
   const int tid = threadIdx.x, wg = __shfl_sync(0xffffffffu, tid >> 7, 0), lt = tid & 127, warp = lt >> 5, lane = tid & 31;
-  const int rows = __shfl_sync(0xffffffffu, *a.rows_ptr, 0);
-  const int ntiles = (rows + kTileM - 1) / kTileM;
-  if ((int)blockIdx.x >= ntiles) return;
-  const int J = (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1;      // tiles of this CTA: blockIdx.x + j * gridDim.x
   const int ksteps = a.Kp / 16;
 
   const uint32_t bar_w = smem_u32(smem + L.off_bar);
@@ -97,6 +93,15 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_wide_kernel(TcArgs a)
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;");
+  // the row count may come from the CFR kernel before this launch (compacted query tiles): read only after the wait.  A CTA
+  // without tiles lets its weight copy land before it exits.
+  const int rows = __shfl_sync(0xffffffffu, *a.rows_ptr, 0);
+  const int ntiles = (rows + kTileM - 1) / kTileM;
+  if ((int)blockIdx.x >= ntiles) {
+    mbar_wait(bar_w, 0);
+    return;
+  }
+  const int J = (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1;      // tiles of this CTA: blockIdx.x + j * gridDim.x
   mbar_wait(bar_w, 0);
 
   const uint32_t sw1 = smem_u32(smem + L.off_w1), sw2 = smem_u32(smem + L.off_w2), sw3 = smem_u32(smem + L.off_w3);
@@ -186,6 +191,12 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_wide_kernel(TcArgs a)
     wgmma_commit();
     if (wg == 0 || j + 1 < J) pass_turn();
     CFRB_TRACE(4);
+    int dst[2];                                 // output rows of this thread's two rows (row_src: compacted tiles), -1 = none
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int row = tile * kTileM + wg * kWgRows + r_lo + 8 * e;
+      dst[e] = row < rows ? (a.row_src != nullptr ? __ldg(a.row_src + row) : row) : -1;
+    }
     wgmma_wait_all();
     fence_regs(acc[0]); fence_regs(acc[1]); fence_regs(act);
     tap(a.dbg_d2, tile);
@@ -205,9 +216,8 @@ __global__ void __launch_bounds__(kThreads, 1) leaf_mlp_tc_wide_kernel(TcArgs a)
     fence_regs(o); fence_regs(act);
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      const int row = tile * kTileM + wg * kWgRows + r_lo + 8 * e;
-      if (row < rows) {                         // rows are Hout floats apart, Hout a multiple of 4
-        float* orow = a.out + (size_t)row * a.Hout;
+      if (dst[e] >= 0) {                        // rows are Hout floats apart, Hout a multiple of 4
+        float* orow = a.out + (size_t)dst[e] * a.Hout;
 #pragma unroll
         for (int i = 0; i < kNo / 8; ++i) {
           const int c = i * 8 + 2 * q;
