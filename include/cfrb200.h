@@ -244,8 +244,42 @@ int64_t cfrb_to_leaf_bytes(int32_t num_dice, int32_t num_faces, int32_t max_dept
 /* Test aid: the compact full-tree strategy [N_full - 1][H] (entry (child - 1) * H + hand) the last cfrb_to_leaf_exploitability
  * filled. */
 int cfrb_to_leaf_strategy(cfrb_handle* h, double* compact);
-/* Test aid: cfrb_to_leaf_exploitability sees at most `bytes` free device bytes (0 = the device's own figure). */
+/* Test aid: cfrb_to_leaf_exploitability and cfrb_to_leaf_sampled see at most `bytes` free device bytes (0 = the device's own
+ * figure). */
 int cfrb_debug_to_leaf_free_cap(cfrb_handle* h, int64_t bytes);
+/* recursive_eval's sampled evaluation on the device, for games up to CFRB_TO_LEAF_MAX_ACTIONS: the float32 reach-weighted average
+ * of num_repeats sampled recursive strategies (strategy ids seed0 .. seed0 + num_repeats - 1) and its exploitability at every
+ * power of two and at num_repeats.  Replaces RecursiveEvaluator::run (recursive_eval.cc:331-369): each repeat is
+ * compute_sampled_strategy_recursive_to_leaf (recursive_solving.cc:76-134, 301-327), every subgame solved up to its act_iteration,
+ * the k-th draw of std::mt19937(strategy id) for the k-th subgame root in the reference's recursion order, its sampling strategy
+ * at that iteration acting; summed_strategy += float(s) * float(reach) and summed_reach += float(reach) in strategy-id order
+ * (:138-148, 349-355); final = summed_strategy / (summed_reach + 1e-6) (:362-363); both best responses of it
+ * (compute_exploitability2, subgame_solving.cc:802-816).  The subgames of batch_repeats repeats (in [1, max_subgames]) are walked
+ * level by level together, in waves of max_subgames rounded down to whole batches.  checkpoints [cap] receives the repeat counts
+ * and br_out [cap][2] both best-response values at each.  ev_full (may be null): a dense full-tree strategy [N_full][H][A]; then
+ * ev_out [cap][2] receives compute_ev2(ev_full, final) at each checkpoint (:368), and its compact copy ((N_full - 1) H doubles)
+ * adds to the device need.  subgames the subgames solved, subgame_iters the sum of their
+ * act_iterations, seconds3 the wall time of the draws, the walk and the best responses.  Returns the number of checkpoints.
+ * Refused like cfrb_to_leaf_exploitability: A > CFRB_TO_LEAF_MAX_ACTIONS (CFRB_EINVAL), or a cfrb_to_leaf_sampled_bytes need above
+ * the free device memory (CFRB_ENOMEM), before anything is allocated.  Replaces the handle's wave and full-tree strategy. */
+int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int32_t batch_repeats, int32_t cap, int32_t* checkpoints,
+                         double* br_out, const double* ev_full, double* ev_out, int64_t* subgames, int64_t* subgame_iters,
+                         double* seconds3);
+/* Host-only: device bytes cfrb_to_leaf_sampled needs beyond the handle: cfrb_to_leaf_bytes' full tree, best-response scratch and
+ * template map, two levels of roots, fp64 beliefs and fp64 reach for each of batch_repeats repeats, the two float32 accumulators
+ * ([N_full - 1][H] and [N_full][H]) and the act_iterations of a batch.  Games with A > 26: CFRB_EINVAL. */
+int64_t cfrb_to_leaf_sampled_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t max_subgames, int32_t batch_repeats);
+/* Host-only: the subgame roots of a to-leaf walk (non-terminal nodes of depth l * max_depth), R of them.  level_pos [R] (written
+ * when cap >= R) gets, for the k-th root in the reference's recursion order (the order of its act_iteration draws), its position
+ * in the device walk's level order over all levels; level_begin [A + 1] (may be null) gets the start of every level, R past the
+ * last.  Returns R. */
+int cfrb_to_leaf_recursion_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t* level_pos, int32_t* level_begin,
+                                 int32_t cap);
+/* Test aids of the last cfrb_to_leaf_sampled: its accumulators, summed_strategy [N_full - 1][H] (entry (child - 1) * H + hand)
+ * and summed_reach [N_full][H]; the last repeat's sampled strategy [N_full - 1][H] (fp64) and the act_iteration of every subgame
+ * root of that repeat, [N_full] by full-tree node (-1 where no subgame is rooted). */
+int cfrb_to_leaf_sampled_sums(cfrb_handle* h, float* summed_strategy, float* summed_reach);
+int cfrb_to_leaf_sampled_last(cfrb_handle* h, double* compact, int32_t* act_iteration);
 
 /* Immediate-regret accumulator on the handle's device, compute_immediate_regrets (subgame_solving.cc:984-1050) split so that a
  * list of strategies can be added in pieces: adding strategies in batches of any size gives the bits of one pass over the whole

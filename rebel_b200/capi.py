@@ -76,6 +76,12 @@ def lib():
     L.cfrb_to_leaf_bytes.restype = C.c_int64
     L.cfrb_to_leaf_strategy.argtypes = [vp, _dp]
     L.cfrb_debug_to_leaf_free_cap.argtypes = [vp, C.c_int64]
+    L.cfrb_to_leaf_sampled.argtypes = [vp] + [C.c_int32] * 4 + [_ip, _dp, _dp, _dp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _dp]
+    L.cfrb_to_leaf_sampled_bytes.argtypes = [C.c_int32] * 5
+    L.cfrb_to_leaf_sampled_bytes.restype = C.c_int64
+    L.cfrb_to_leaf_recursion_order.argtypes = [C.c_int32] * 3 + [_ip, _ip, C.c_int32]
+    L.cfrb_to_leaf_sampled_sums.argtypes = [vp, _fp, _fp]
+    L.cfrb_to_leaf_sampled_last.argtypes = [vp, _dp, _ip]
     L.cfrb_regrets_reset.argtypes = [vp]
     L.cfrb_regrets_add.argtypes = [vp, _fp, C.c_int32]
     L.cfrb_regrets_add_current.argtypes = [vp]
@@ -173,6 +179,23 @@ def to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames):
     """Host-only: device bytes WaveSolver.to_leaf_exploitability needs beyond a handle of these sizes (full tree, best-response
     scratch, the walk's largest levels)."""
     return _check(lib().cfrb_to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames))
+
+
+def to_leaf_sampled_bytes(num_dice, num_faces, max_depth, max_subgames, batch_repeats):
+    """Host-only: device bytes WaveSolver.to_leaf_sampled needs beyond a handle of these sizes (full tree, best-response scratch,
+    template map, the largest levels of batch_repeats repeats, the float32 accumulators, the draws of a batch)."""
+    return _check(lib().cfrb_to_leaf_sampled_bytes(num_dice, num_faces, max_depth, max_subgames, batch_repeats))
+
+
+def to_leaf_recursion_order(num_dice, num_faces, max_depth):
+    """Host-only: (level_pos [R], level_begin [A + 1]) of the R subgame roots of a to-leaf walk: level_pos[k] is the position in
+    the walk's level order of the k-th root in the reference's recursion order (the order of its act_iteration draws)."""
+    A = 2 * num_dice * num_faces + 1
+    begin = np.zeros(A + 1, np.int32)
+    n = _check(lib().cfrb_to_leaf_recursion_order(num_dice, num_faces, max_depth, None, _p(begin, _ip), 0))
+    pos = np.zeros(n, np.int32)
+    _check(lib().cfrb_to_leaf_recursion_order(num_dice, num_faces, max_depth, _p(pos, _ip), None, n))
+    return pos, begin
 
 
 def net_output_bound(num_dice, num_faces, flat, hidden=256):
@@ -328,8 +351,36 @@ class WaveSolver:
         _check(lib().cfrb_to_leaf_strategy(self._h, _p(out, _dp)))
         return out
 
+    def to_leaf_sampled(self, num_repeats, seed=0, batch_repeats=1):
+        """recursive_eval's sampled evaluation of this handle's policy (its weights and solver settings) on the device: the float32
+        reach-weighted average of num_repeats sampled recursive strategies (ids seed ..) and its best responses at every power of
+        two and at num_repeats.  dict of checkpoints, br [C, 2], subgames, subgame_iters, draw_seconds, walk_seconds,
+        br_seconds.  Replaces the handle's wave."""
+        cap = 64
+        cps, br, secs = np.zeros(cap, np.int32), np.zeros((cap, 2), np.float64), np.zeros(3, np.float64)
+        sg, it = C.c_int64(0), C.c_int64(0)
+        n = _check(lib().cfrb_to_leaf_sampled(self._h, seed, num_repeats, batch_repeats, cap, _p(cps, _ip), _p(br, _dp), None, None,
+                                              C.byref(sg), C.byref(it), _p(secs, _dp)))
+        return {"checkpoints": cps[:n].tolist(), "br": br[:n].copy(), "subgames": sg.value, "subgame_iters": it.value,
+                "draw_seconds": float(secs[0]), "walk_seconds": float(secs[1]), "br_seconds": float(secs[2])}
+
+    def to_leaf_sampled_sums(self):
+        """The last to_leaf_sampled's float32 accumulators: summed_strategy [N_full - 1, H] (row child - 1), summed_reach [N_full, H]."""
+        n = (1 << self.A) - 1
+        ss, sr = np.zeros((n - 1, self.H), np.float32), np.zeros((n, self.H), np.float32)
+        _check(lib().cfrb_to_leaf_sampled_sums(self._h, _p(ss, _fp), _p(sr, _fp)))
+        return ss, sr
+
+    def to_leaf_sampled_last(self):
+        """The last to_leaf_sampled's last repeat: its sampled strategy [N_full - 1, H] (fp64) and the act_iteration of every subgame
+        root [N_full] (-1 where none is rooted)."""
+        n = (1 << self.A) - 1
+        s, act = np.zeros((n - 1, self.H), np.float64), np.zeros(n, np.int32)
+        _check(lib().cfrb_to_leaf_sampled_last(self._h, _p(s, _dp), _p(act, _ip)))
+        return s, act
+
     def debug_to_leaf_free_cap(self, nbytes):
-        """Test aid: to_leaf_exploitability sees at most nbytes free device bytes (0 = the device's own figure)."""
+        """Test aid: to_leaf_exploitability and to_leaf_sampled see at most nbytes free device bytes (0 = the device's own figure)."""
         _check(lib().cfrb_debug_to_leaf_free_cap(self._h, int(nbytes)))
 
     @property

@@ -11,6 +11,7 @@
 #include "lbr_kernels.cuh"
 #include "agent_kernels.cuh"
 #include "expl_kernels.cuh"
+#include "expl_sampled_kernels.cuh"
 
 namespace cfrb {
 
@@ -183,6 +184,21 @@ void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalis
   expl_expand_kernel<real><<<n, 128, 0, st>>>(p, table, normalise);
   expl_fill_kernel<<<1, 1, 0, st>>>(p);
 }
+template <typename real>
+void expl_sampled_launch_begin(const ExplSampledDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st) {
+  expl_sampled_begin_kernel<real><<<(n + 127) / 128, 128, 0, st>>>(p, n, wave_beliefs);
+  sp_scan_kernel<<<1, 1024, 0, st>>>(scan);
+}
+template <typename real>
+void expl_sampled_launch_expand(const ExplSampledDev& p, int n, const real* snap, cudaStream_t st) {
+  expl_sampled_expand_kernel<real><<<n / p.b, 128, 0, st>>>(p, snap);
+  expl_sampled_fill_kernel<<<1, 1, 0, st>>>(p);
+}
+void expl_sampled_launch_finalize(const ExplSampledDev& p, cudaStream_t st) {
+  const size_t total = (size_t)(p.full_nodes - 1) * p.H;
+  const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 8);
+  expl_sampled_finalize_kernel<<<std::max(blocks, 1), 256, 0, st>>>(p);
+}
 __global__ void rows_gather_kernel(const float* __restrict__ src, int width, const int* __restrict__ ids, int n, float* __restrict__ out) {
   const size_t total = (size_t)n * width;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -238,7 +254,9 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void agent_launch_begin<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);                           \
   template void agent_launch_capture<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);                         \
   template void expl_launch_begin<real>(const ExplDev&, const SpDev&, int, real*, cudaStream_t);                           \
-  template void expl_launch_expand<real>(const ExplDev&, int, const real*, int, cudaStream_t);
+  template void expl_launch_expand<real>(const ExplDev&, int, const real*, int, cudaStream_t);                              \
+  template void expl_sampled_launch_begin<real>(const ExplSampledDev&, const SpDev&, int, real*, cudaStream_t);           \
+  template void expl_sampled_launch_expand<real>(const ExplSampledDev&, int, const real*, cudaStream_t);
 CFRB_INSTANTIATE(float)
 CFRB_INSTANTIATE(double)
 

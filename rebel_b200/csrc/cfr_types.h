@@ -259,6 +259,43 @@ struct ExplDev {
 template <typename real> void expl_launch_begin(const ExplDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st);
 // the solved wave's strategy into p.strategy, its pseudo-leaves onto the next level
 template <typename real> void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
+// Sampled recursive to-leaf walk (expl_sampled_kernels.cuh): the waves of one level of a batch of b repeats.  A level lists its
+// root groups in full-tree node order, each group the b repeats of one root in repeat order, so level position pos is repeat
+// pos % b of group pos / b.
+struct ExplSampledDev {
+  int H, A, b;
+  // the full tree (BrState of the handle): the accumulators, the final strategy and the last repeat's sampled strategy index it
+  const int* full_child_begin; const int* full_depth; const int* full_act_lo; const int* full_parent;
+  int full_nodes;
+  // the handle's subgame templates
+  const TemplateDev* tmpl; const int* parent; const int* child_begin; const int* nchild; const int* level_begin;
+  const int* pleaf_node;
+  // the handle's wave descriptors
+  int* sg_tmpl; int* sg_player; int* sg_act; const int* sg_row_off; const int* wave;
+  int table_stride;
+  // act_iteration of (repeat j, global level position g of its root group) = draws[j * draws_stride + level_base + g]
+  const int* draws; long long draws_stride; int level_base;
+  // this level's roots [n_level], fp64 beliefs and reach [n_level][2][H]; the wave is positions off .. off + n - 1 (whole groups)
+  const int* roots; const double* bel; const double* rch;
+  int off;
+  // the next level: cap positions, fill [1] of them written by the level's earlier waves
+  int* next_roots; double* next_bel; double* next_rch;
+  int* fill;
+  long long cap;
+  int* fid; int nmax;                 // [groups][nmax] scratch: full-tree node of every template node of each root group
+  // float32 accumulators, compact: summed_strategy [N_full - 1][H] (entry (child - 1) * H + hand), summed_reach [N_full][H]
+  float* sum_s; float* sum_r;
+  // repeat last_j of the batch (-1: none) writes its sampled strategy into last [N_full - 1][H]
+  double* last; int last_j;
+  double* strategy;                   // the compact full-tree strategy the best response reads [N_full - 1][H]
+};
+// wave descriptors (template, player, act_iteration, root beliefs as `real`), row offsets and schedule of positions off .. off + n - 1
+template <typename real> void expl_sampled_launch_begin(const ExplSampledDev& p, const SpDev& scan, int n, real* wave_beliefs,
+                                                        cudaStream_t st);
+// the solved wave's snapshot strategies into the accumulators, its pseudo-leaves (beliefs and reach) onto the next level
+template <typename real> void expl_sampled_launch_expand(const ExplSampledDev& p, int n, const real* snap, cudaStream_t st);
+// strategy = (double)(sum_s / (sum_r[parent] + 1e-6f)), the final strategy of a checkpoint
+void expl_sampled_launch_finalize(const ExplSampledDev& p, cudaStream_t st);
 // rows [ids[i]] of a [*, width] fp32 matrix -> out[i]  (replay sampling)
 void rows_launch_gather(const float* src, int width, const int* ids, int n, float* out, cudaStream_t st);
 

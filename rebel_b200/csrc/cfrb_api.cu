@@ -13,6 +13,7 @@
 #include <cstring>
 #include <limits>
 #include <memory>
+#include <random>
 #include <string>
 #include <type_traits>
 #include <utility>
@@ -250,7 +251,14 @@ struct cfrb_handle {
   bool rows_on_device = false;   // the wave was built on the device: its row count / roots exist only there
   bool mirror_stale = false;     // ... and the host mirror (h_tmpl, h_beliefs, rows) has not been pulled yet
   bool in_match = false;         // an agent of a live cfrb_match: its waves are built by the match
-  int64_t to_leaf_free_cap = 0;  // test aid (cfrb_debug_to_leaf_free_cap): cfrb_to_leaf_exploitability sees at most this many free bytes
+  int64_t to_leaf_free_cap = 0;  // test aid (cfrb_debug_to_leaf_free_cap): the to-leaf walks see at most this many free bytes
+  // the last cfrb_to_leaf_sampled call: its float32 accumulators and the act_iteration of every subgame root of its last repeat
+  // (its sampled strategy is br.strategy2)
+  struct SampledState {
+    bool ready = false;
+    DevBuf<float> sum_s, sum_r;
+    std::vector<int> last_act;
+  } smp;
 };
 
 // Calls f with the handle's typed (fp64 or fp32) solver state.
@@ -1645,13 +1653,13 @@ int cfrb_last_run_ms(cfrb_handle* h, float* total_ms, float* net_ms) {
 // d_sg_order holds the wave's schedule; otherwise the depth-2 kernel takes wave order.  drop_sum: a self-play wave, whose loop
 // reads the snapshots and root means only; CFR then leaves the sum table alone (materialise_sum rebuilds it for a reader).  Match,
 // LBR and agent waves keep it: they act with the average strategy of the wave they have just solved (act_slot).
-static int solve_device_wave(cfrb_handle* h, int n, bool sorted, bool drop_sum, cudaStream_t st) {
+static int solve_device_wave(cfrb_handle* h, int n, bool sorted, bool drop_sum, cudaStream_t st, int iters = -1) {
   h->n = n; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
   h->sorted = sorted;
   h->sum_dropped = drop_sum && h->cfg.solver == CFRB_SOLVER_CFR;
   h->sum_uploads = h->weight_uploads;
   const int rc = launch_init(h, st);
-  return rc ? rc : cfrb_run(h, h->cfg.num_iters, st);
+  return rc ? rc : cfrb_run(h, iters < 0 ? h->cfg.num_iters : iters, st);
 }
 
 // ============================================================================================ recursive to-leaf exploitability
@@ -1664,7 +1672,7 @@ static int64_t binom(int n, int k) {
   for (int i = 1; i <= k; ++i) r = r * (n - k + i) / i;
   return r;
 }
-struct ToLeafSizes { int64_t tree_bytes = 0, walk_bytes = 0, level_cap = 0; };
+struct ToLeafSizes { int64_t tree_bytes = 0, walk_bytes = 0, level_cap = 0, nmax = 0; };
 static ToLeafSizes to_leaf_sizes(const cfrb::GameShape& g, int max_depth, int K) {
   const int A = g.A;
   const int64_t H = g.H, N = ((int64_t)1 << A) - 1, T = ((int64_t)1 << (A - 1)) - 1, levels = A + 1;
@@ -1674,6 +1682,7 @@ static ToLeafSizes to_leaf_sizes(const cfrb::GameShape& g, int max_depth, int K)
   s.tree_bytes = (5 * N + levels + 1 + 3 * T) * 4 + (2 * (N - 1) * H + 2 * (3 * N * H + 10 * T) + 2) * 8;
   int64_t nmax = 1;
   for (int d = 1; d <= std::min(max_depth, A); ++d) nmax += d == 1 ? A - 1 : binom(A, d);
+  s.nmax = nmax;
   for (int d = 0; d <= A - 1; d += max_depth) s.level_cap = std::max(s.level_cap, binom(A - 1, d));
   // the template-to-full-tree map [K][nmax], and two levels of roots and fp64 beliefs [2][H]
   s.walk_bytes = (int64_t)K * nmax * 4 + 2 * s.level_cap * (4 + 2 * H * 8);
@@ -1790,6 +1799,291 @@ int cfrb_to_leaf_strategy(cfrb_handle* h, double* compact) {
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->own_stream));
   CK(cudaMemcpy(compact, h->br.strategy.p, h->br.strategy.n * sizeof(double), cudaMemcpyDeviceToHost));
+  return CFRB_OK;
+}
+
+// ============================================================================================ sampled recursive to-leaf evaluation
+// The subgame roots of a to-leaf walk (the non-terminal full-tree nodes of depth l * max_depth) form a tree: a root's children are
+// the non-terminal pseudo-leaves of its subgame, in BFS order.  The device walk lists them level by level, each level in full-tree
+// node order; the reference's recursion (compute_sampled_strategy_recursive_to_leaf, recursive_solving.cc:76-134, 301-327, as
+// RecursiveEvaluator::visit orders it) creates their solvers, and so draws their act_iterations, depth-first in the same child
+// order.  rec_to_level[k] = the level position (over all levels) of the k-th root in recursion order.  The order depends on the
+// game and max_depth alone; the per-bid templates give it without the full tree.
+struct ToLeafOrder {
+  std::vector<int> rec_to_level;   // [roots]
+  std::vector<int> level_begin;    // [levels + 1]
+};
+static ToLeafOrder to_leaf_order(const cfrb::GameShape& g, int max_depth) {
+  std::vector<std::vector<int>> leaves(g.A);   // template (root bid + 1) -> last bids of its non-terminal pseudo-leaves, BFS order
+  for (int b = -1; b <= g.A - 2; ++b) {
+    const auto t = cfrb::build_template(g, b, max_depth);
+    for (int n : t.pleaf_node) leaves[b + 1].push_back(t.last_bid[n]);
+  }
+  ToLeafOrder o;
+  std::vector<int> bid{-1}, first;             // per level position: root bid, level position of its first child
+  o.level_begin = {0, 1};
+  for (size_t lo = 0; lo < bid.size();) {
+    const size_t hi = bid.size();
+    for (size_t p = lo; p < hi; ++p) {
+      first.push_back((int)bid.size());
+      for (int c : leaves[bid[p] + 1]) bid.push_back(c);
+    }
+    lo = hi;
+    if (bid.size() > hi) o.level_begin.push_back((int)bid.size());
+  }
+  o.rec_to_level.reserve(bid.size());
+  std::vector<int> stack{0};
+  while (!stack.empty()) {
+    const int p = stack.back();
+    stack.pop_back();
+    o.rec_to_level.push_back(p);
+    for (int c = (int)leaves[bid[p] + 1].size() - 1; c >= 0; --c) stack.push_back(first[p] + c);
+  }
+  return o;
+}
+
+int cfrb_to_leaf_recursion_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t* level_pos, int32_t* level_begin,
+                                 int32_t cap) {
+  if (num_dice < 1 || num_faces < 1 || max_depth < 1)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_recursion_order: num_dice, num_faces, max_depth must be >= 1");
+  const cfrb::GameShape g(num_dice, num_faces);
+  if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_recursion_order: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                                 " actions are not supported (A = " + std::to_string(g.A) + ")");
+  const auto o = to_leaf_order(g, max_depth);
+  const int R = (int)o.rec_to_level.size();
+  if (level_pos && cap >= R) std::copy(o.rec_to_level.begin(), o.rec_to_level.end(), level_pos);
+  if (level_begin) {   // [A + 1]: the level starts, then R up to the end
+    for (int l = 0; l <= g.A; ++l) level_begin[l] = l < (int)o.level_begin.size() ? o.level_begin[l] : R;
+  }
+  return R;
+}
+
+// Sizes of the sampled walk: the average walk's full tree, best-response scratch and template map (to_leaf_sizes), two levels of
+// roots, fp64 beliefs and fp64 reach for every repeat of a batch, the two float32 accumulators and the batch's act_iterations.
+struct SampledSizes { int64_t tree_bytes = 0, walk_bytes = 0, level_cap = 0, roots = 0; };
+static SampledSizes sampled_sizes(const cfrb::GameShape& g, int max_depth, int K, int B) {
+  const auto t = to_leaf_sizes(g, max_depth, K);
+  const int64_t A = g.A, H = g.H, N = ((int64_t)1 << A) - 1;
+  SampledSizes s;
+  s.tree_bytes = t.tree_bytes;
+  s.level_cap = t.level_cap * B;
+  for (int64_t d = 0; d <= A - 1; d += max_depth) s.roots += binom((int)A - 1, (int)d);
+  s.walk_bytes = (int64_t)K * t.nmax * 4 + 2 * s.level_cap * (4 + 2 * 2 * H * 8) + ((N - 1) * H + N * H) * 4 + (int64_t)B * s.roots * 4;
+  return s;
+}
+
+int64_t cfrb_to_leaf_sampled_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t max_subgames, int32_t batch_repeats) {
+  if (num_dice < 1 || num_faces < 1 || max_depth < 1 || max_subgames < 1 || batch_repeats < 1)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled_bytes: num_dice, num_faces, max_depth, max_subgames, batch_repeats must be >= 1");
+  if (2L * num_dice * num_faces + 1 > 26) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled_bytes: full tree too large (2^A - 1 nodes, A > 26)");
+  const auto s = sampled_sizes(cfrb::GameShape(num_dice, num_faces), max_depth, max_subgames, batch_repeats);
+  return s.tree_bytes + s.walk_bytes;
+}
+
+int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int32_t batch_repeats, int32_t cap, int32_t* checkpoints,
+                         double* br_out, const double* ev_full, double* ev_out, int64_t* subgames, int64_t* subgame_iters,
+                         double* seconds3) {
+  if (!h || !checkpoints || !br_out || (ev_full && !ev_out)) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: null argument");
+  const auto& g = h->g;
+  if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                                 " actions are not supported (A = " + std::to_string(g.A) + ": the full tree has 2^A - 1 nodes)");
+  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H, md = h->cfg.max_depth, iters = h->cfg.num_iters;
+  if (num_repeats < 1) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: num_repeats must be >= 1");
+  if (batch_repeats < 1 || batch_repeats > K)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: batch_repeats must be in [1, max_subgames = " + std::to_string(K) + "]");
+  // checkpoints: every power of two up to num_repeats, and num_repeats (recursive_eval.cc:364-369)
+  std::vector<int> cps;
+  for (int64_t c = 1; c <= num_repeats; c <<= 1) cps.push_back((int)c);
+  if (cps.back() != num_repeats) cps.push_back(num_repeats);
+  if (cap < (int)cps.size())
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: " + std::to_string(cps.size()) + " checkpoints, room for " + std::to_string(cap));
+  if (h->in_match) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: the handle plays in a live match or agent");
+  if (h->cfg.net_mode != CFRB_NET_ZERO && !h->have_weights && h->Lmax > 0)
+    return fail(CFRB_ESTATE, "cfrb_to_leaf_sampled: value-net weights not set (cfrb_set_weights)");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->own_stream));
+  h->smp.ready = false;                        // the previous call's results go first: their memory counts as free below
+  h->smp.sum_s = DevBuf<float>();
+  h->smp.sum_r = DevBuf<float>();
+  h->smp.last_act.clear();
+  const auto sz = sampled_sizes(g, md, K, batch_repeats);
+  // refused before anything is allocated: on a shared device an allocation that fails late may starve other processes
+  const int64_t ev_bytes = ev_full ? ((((int64_t)1 << g.A) - 2) * H) * 8 : 0;   // the compact ev_full
+  const int64_t need = (h->br.ready ? 0 : sz.tree_bytes) + sz.walk_bytes + ev_bytes;
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  int64_t avail = (int64_t)free_b;
+  if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
+  if (need > avail)
+    return fail(CFRB_ENOMEM, "cfrb_to_leaf_sampled: needs " + std::to_string(need) + " bytes of device memory beyond the handle "
+                             "(full tree and best-response scratch " + std::to_string(h->br.ready ? 0 : sz.tree_bytes) + ", walk " +
+                             std::to_string(sz.walk_bytes) + " at batch_repeats " + std::to_string(batch_repeats) + "), " +
+                             std::to_string(avail) + " free");
+  int rc = full_tree_setup(h, "cfrb_to_leaf_sampled");
+  if (rc) return rc;
+  const int N = h->br.t.N;
+  const auto ord = to_leaf_order(g, md);
+  const int R = (int)ord.rec_to_level.size();
+  if (R != sz.roots) return fail(CFRB_ECUDA, "cfrb_to_leaf_sampled: " + std::to_string(R) + " subgame roots, expected " + std::to_string(sz.roots));
+  cudaStream_t st = h->own_stream;
+  DevBuf<int> roots[2], fid, fill, draws;
+  DevBuf<double> bel[2], rch[2];
+  for (int i = 0; i < 2; ++i) {
+    CK(roots[i].alloc(sz.level_cap)); CK(bel[i].alloc((size_t)sz.level_cap * W)); CK(rch[i].alloc((size_t)sz.level_cap * W));
+  }
+  CK(fid.alloc((size_t)K * h->Nmax)); CK(fill.alloc(1)); CK(draws.alloc((size_t)batch_repeats * R));
+  CK(h->smp.sum_s.alloc((size_t)(N - 1) * H)); CK(h->smp.sum_r.alloc((size_t)N * H));
+  DevBuf<double> full;
+  if (ev_full) {
+    CK(full.alloc((size_t)(N - 1) * H));
+    if ((rc = upload_compact(h, ev_full, full.p))) return rc;
+  }
+  CK(cudaMemsetAsync(h->smp.sum_s.p, 0, (size_t)(N - 1) * H * sizeof(float), st));
+  CK(cudaMemsetAsync(h->smp.sum_r.p, 0, (size_t)N * H * sizeof(float), st));
+  cfrb::ExplSampledDev d{};
+  d.H = H; d.A = g.A;
+  d.full_child_begin = h->br.child_begin.p; d.full_depth = h->br.depth.p; d.full_act_lo = h->br.act_lo.p; d.full_parent = h->br.parent.p;
+  d.full_nodes = N;
+  d.tmpl = h->d_tmpl.p; d.parent = h->d_parent.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p;
+  d.level_begin = h->d_level_begin.p; d.pleaf_node = h->d_pleaf_node.p;
+  d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_act = h->d_sg_act.p; d.sg_row_off = h->d_sg_row_off.p;
+  d.wave = h->d_wave.p; d.table_stride = h->table_stride;
+  d.draws = draws.p; d.draws_stride = R;
+  d.fill = fill.p; d.cap = sz.level_cap; d.fid = fid.p; d.nmax = h->Nmax;
+  d.sum_s = h->smp.sum_s.p; d.sum_r = h->smp.sum_r.p; d.last = h->br.strategy2.p; d.strategy = h->br.strategy.p;
+  cfrb::SpDev scan{};   // sp_scan_kernel's view of the wave
+  scan.A = g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
+  scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
+  // act_iteration ~ discrete distribution with weight i/2 + 1 on even i (recursive_solving.cc:304-309, 315-319); the distribution
+  // keeps no state between draws, so one object serves every root
+  std::vector<double> weights;
+  for (int i = 0; i < iters; ++i) weights.push_back(i % 2 ? 0.0 : (i / 2. + 1));
+  std::discrete_distribution<int> dist(weights.begin(), weights.end());
+  std::vector<int> draws_h, gmax(R), level_roots;
+  const std::vector<double> uniform(W, 1.0 / H);   // level 0: the game root with uniform beliefs and reach
+  std::vector<double> uniform_b;
+  double secs[3] = {0, 0, 0};
+  int64_t solved = 0, iters_sum = 0;
+  int done = 0, c = 0;
+  while (done < num_repeats) {
+    // batches end at the checkpoints, as RecursiveEvaluator::run's do
+    int next_cp = 1;
+    while (next_cp <= done) next_cp <<= 1;
+    const int b = std::min({num_repeats, done + batch_repeats, next_cp}) - done;
+    const bool last_batch = done + b == num_repeats;
+    const auto t0 = std::chrono::steady_clock::now();
+    // repeat r draws from std::mt19937(seed0 + r) once per subgame root, in recursion order (RecursiveEvaluator::runBatch)
+    draws_h.assign((size_t)b * R, 0);
+    std::fill(gmax.begin(), gmax.end(), 0);
+    for (int j = 0; j < b; ++j) {
+      std::mt19937 gen(seed0 + done + j);
+      int* dj = draws_h.data() + (size_t)j * R;
+      for (int k = 0; k < R; ++k) {
+        const int a = dist(gen), pos = ord.rec_to_level[k];
+        dj[pos] = a;
+        gmax[pos] = std::max(gmax[pos], a);
+        iters_sum += a;
+      }
+    }
+    CK(cudaMemcpyAsync(draws.p, draws_h.data(), draws_h.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    const auto t1 = std::chrono::steady_clock::now();
+    const std::vector<int> zeros(b, 0);
+    uniform_b.resize((size_t)b * W);
+    for (int j = 0; j < b; ++j) std::copy(uniform.begin(), uniform.end(), uniform_b.begin() + (size_t)j * W);
+    CK(cudaMemcpyAsync(roots[0].p, zeros.data(), b * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bel[0].p, uniform_b.data(), uniform_b.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(rch[0].p, uniform_b.data(), uniform_b.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    d.b = b; d.last_j = last_batch ? b - 1 : -1;
+    const int Kw = (K / b) * b;                   // a wave holds whole root groups
+    int cur = 0, n_level = b;
+    for (int depth = 0, l = 0; n_level > 0; depth += md, ++l) {
+      d.roots = roots[cur].p; d.bel = bel[cur].p; d.rch = rch[cur].p;
+      d.next_roots = roots[cur ^ 1].p; d.next_bel = bel[cur ^ 1].p; d.next_rch = rch[cur ^ 1].p;
+      d.level_base = ord.level_begin[l];
+      CK(cudaMemsetAsync(fill.p, 0, sizeof(int), st));
+      for (int off = 0; off < n_level; off += Kw) {
+        const int n = std::min(Kw, n_level - off);
+        int max_act = 0;   // the wave runs up to its largest act_iteration (RecursiveEvaluator::runBatch)
+        for (int gi = off / b; gi < (off + n) / b; ++gi) max_act = std::max(max_act, gmax[d.level_base + gi]);
+        d.off = off; scan.K = n;
+        with_state(h, [&](auto& s) { cfrb::expl_sampled_launch_begin(d, scan, n, s.beliefs.p, st); });
+        h->launches += 2;
+        CK(cudaGetLastError());
+        if ((rc = solve_device_wave(h, n, true, true, st, max_act))) return rc;   // the snapshot does not read the sum table
+        with_state(h, [&](auto& s) { cfrb::expl_sampled_launch_expand(d, n, s.Snap.p, st); });
+        h->launches += 2;
+        CK(cudaGetLastError());
+      }
+      solved += n_level;
+      if (last_batch) {   // the roots of this level, for the last repeat's act_iterations by node
+        level_roots.resize(n_level);
+        CK(cudaMemcpyAsync(level_roots.data(), roots[cur].p, n_level * sizeof(int), cudaMemcpyDeviceToHost, st));
+      }
+      int next = 0;
+      CK(cudaMemcpyAsync(&next, fill.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (last_batch) {
+        if (h->smp.last_act.empty()) h->smp.last_act.assign(N, -1);
+        for (int gi = 0; gi < n_level / b; ++gi)
+          h->smp.last_act[level_roots[(size_t)gi * b]] = draws_h[(size_t)(b - 1) * R + d.level_base + gi];
+      }
+      const int64_t want = binom(g.A - 1, depth + md) * b;
+      if (next != want)
+        return fail(CFRB_ECUDA, "cfrb_to_leaf_sampled: level at depth " + std::to_string(depth + md) + " has " +
+                                    std::to_string(next) + " subgames, the tree " + std::to_string(want));
+      n_level = next;
+      cur ^= 1;
+    }
+    const auto t2 = std::chrono::steady_clock::now();
+    done += b;
+    if (done == cps[c]) {
+      // the final strategy summed_strategy / (summed_reach + 1e-6) in float32 (recursive_eval.cc:362-363), widened, and both
+      // best responses of it (cfrb_exploitability = compute_exploitability2, subgame_solving.cc:802-816)
+      cfrb::expl_sampled_launch_finalize(d, st);
+      cfrb::br_launch(full_tree_dev(h), st);
+      h->launches += 2;
+      CK(cudaGetLastError());
+      CK(cudaMemcpyAsync(br_out + 2 * c, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+      if (ev_full) {   // compute_ev2(full_strategy, final_strategy) (recursive_eval.cc:368)
+        cfrb::ev_launch(full_tree_dev(h), full.p, h->br.strategy.p, st);
+        ++h->launches;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(ev_out + 2 * c, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+      }
+      CK(cudaStreamSynchronize(st));
+      checkpoints[c++] = done;
+    }
+    const auto t3 = std::chrono::steady_clock::now();
+    secs[0] += std::chrono::duration<double>(t1 - t0).count();
+    secs[1] += std::chrono::duration<double>(t2 - t1).count();
+    secs[2] += std::chrono::duration<double>(t3 - t2).count();
+  }
+  h->smp.ready = true;
+  if (subgames) *subgames = solved;
+  if (subgame_iters) *subgame_iters = iters_sum;
+  if (seconds3) std::copy(secs, secs + 3, seconds3);
+  return c;
+}
+
+int cfrb_to_leaf_sampled_sums(cfrb_handle* h, float* summed_strategy, float* summed_reach) {
+  if (!h || !summed_strategy || !summed_reach) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled_sums: null argument");
+  if (!h->smp.ready) return fail(CFRB_ESTATE, "cfrb_to_leaf_sampled_sums: no sampled walk has finished on this handle (cfrb_to_leaf_sampled)");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->own_stream));
+  CK(cudaMemcpy(summed_strategy, h->smp.sum_s.p, h->smp.sum_s.n * sizeof(float), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(summed_reach, h->smp.sum_r.p, h->smp.sum_r.n * sizeof(float), cudaMemcpyDeviceToHost));
+  return CFRB_OK;
+}
+
+int cfrb_to_leaf_sampled_last(cfrb_handle* h, double* compact, int32_t* act_iteration) {
+  if (!h || !compact || !act_iteration) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled_last: null argument");
+  if (!h->smp.ready) return fail(CFRB_ESTATE, "cfrb_to_leaf_sampled_last: no sampled walk has finished on this handle (cfrb_to_leaf_sampled)");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->own_stream));
+  CK(cudaMemcpy(compact, h->br.strategy2.p, h->br.strategy2.n * sizeof(double), cudaMemcpyDeviceToHost));
+  std::copy(h->smp.last_act.begin(), h->smp.last_act.end(), act_iteration);
   return CFRB_OK;
 }
 

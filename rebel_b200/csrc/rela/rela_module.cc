@@ -686,6 +686,75 @@ py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, p
   return d;
 }
 
+// recursive_eval's sampled evaluation (RecursiveEvaluator::run, recursive_eval.cc:331-369) walked on the device
+// (cfrb_to_leaf_sampled): no dense [N, H, A] sums, so games up to A = 23 are accepted.  batch_repeats <= 0: as many repeats per
+// batch as fill one wave with the largest level of subgames, between 1 and 64.
+int default_batch_repeats(int A, int max_depth, int wave_capacity) {
+  int64_t level = 1;
+  for (int d = 0; d <= A - 1; d += max_depth) {
+    int64_t c = 1;
+    for (int i = 1; i <= d; ++i) c = c * (A - 1 - d + i) / i;
+    level = std::max(level, c);
+  }
+  return (int)std::max<int64_t>(1, std::min<int64_t>(64, std::max(1, wave_capacity) / level));
+}
+py::dict recursive_eval_to_leaf(const RecursiveSolvingParams& cfg, int device, int num_repeats, int seed0, py::object flat_weights,
+                                int wave_capacity, int batch_repeats, bool return_sums, py::object full_strategy) {
+  const int A = 2 * cfg.num_dice * cfg.num_faces + 1;
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)   // the library's own refusal, before a device is touched
+    throw std::runtime_error("recursive_eval_to_leaf: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                             " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+  if (num_repeats < 1) throw std::runtime_error("recursive_eval_to_leaf: num_repeats must be >= 1");
+  const int K = std::max(1, wave_capacity);
+  const int B = batch_repeats > 0 ? batch_repeats : default_batch_repeats(A, cfg.subgame_params.max_depth, K);
+  const std::vector<float> w = flat_of(flat_weights);
+  std::vector<double> full;
+  if (!full_strategy.is_none()) {
+    auto t = full_strategy.cast<torch::Tensor>().to(torch::kCPU, torch::kFloat64).contiguous();
+    const int64_t want = (((int64_t)1 << A) - 1) * (int64_t)std::pow(cfg.num_faces, cfg.num_dice) * A;
+    if (t.numel() != want) throw std::runtime_error("recursive_eval_to_leaf: full_strategy must be [N_full][H][A]");
+    full.assign(t.data_ptr<double>(), t.data_ptr<double>() + t.numel());
+  }
+  std::vector<int> cps(64);
+  std::vector<double> br(128), ev(128);
+  std::vector<float> ss, sr;
+  double secs[3] = {0, 0, 0}, total = 0;
+  int64_t subgames = 0, iters = 0;
+  int N = 0, H = 0, C = 0;
+  {
+    py::gil_scoped_release nogil;
+    const auto t0 = std::chrono::steady_clock::now();
+    const HandlePtr h = open_handle(liars_dice::solver_config(cfg, device, K));
+    if (!w.empty()) check(cfrb_set_weights(h.get(), w.data(), w.size(), 1), "cfrb_set_weights");
+    C = check(cfrb_to_leaf_sampled(h.get(), seed0, num_repeats, B, (int)cps.size(), cps.data(), br.data(),
+                                   full.empty() ? nullptr : full.data(), ev.data(), &subgames, &iters, secs),
+              "cfrb_to_leaf_sampled");
+    N = cfrb_full_tree_nodes(h.get());
+    H = cfrb_num_hands(h.get());
+    if (return_sums) {
+      ss.resize((size_t)(N - 1) * H);
+      sr.resize((size_t)N * H);
+      check(cfrb_to_leaf_sampled_sums(h.get(), ss.data(), sr.data()), "cfrb_to_leaf_sampled_sums");
+    }
+    total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  }
+  std::vector<std::array<double, 2>> e(C), evs(C);
+  for (int c = 0; c < C; ++c) { e[c] = {br[2 * c], br[2 * c + 1]}; evs[c] = {ev[2 * c], ev[2 * c + 1]}; }
+  py::dict d;
+  d["checkpoints"] = std::vector<int>(cps.begin(), cps.begin() + C);
+  d["exploitability"] = pairs_tensor(e);
+  d["num_nodes"] = N; d["subgames"] = subgames; d["subgame_iters"] = iters; d["batch_repeats"] = B;
+  d["seconds"] = total; d["draw_seconds"] = secs[0]; d["walk_seconds"] = secs[1]; d["br_seconds"] = secs[2];
+  if (!full.empty()) d["ev_of_full"] = pairs_tensor(evs);
+  if (return_sums) {
+    auto tss = torch::empty({(int64_t)N - 1, (int64_t)H}), tsr = torch::empty({(int64_t)N, (int64_t)H});
+    std::copy(ss.begin(), ss.end(), tss.data_ptr<float>());
+    std::copy(sr.begin(), sr.end(), tsr.data_ptr<float>());
+    d["summed_strategy"] = tss; d["summed_reach"] = tsr;
+  }
+  return d;
+}
+
 // rela.Agent: index lists and actions from anything torch.as_tensor accepts (lists, numpy arrays, tensors).
 std::vector<int32_t> i32_of(py::object o) {
   auto t = py::module::import("torch").attr("as_tensor")(o).cast<torch::Tensor>().to(torch::kCPU, torch::kInt32).contiguous().view(-1);
@@ -917,6 +986,16 @@ PYBIND11_MODULE(rela, m) {
         "in waves of wave_capacity and the best response taken on the GPU without a dense strategy (games with at most 23 actions "
         "whose need fits the free device memory).  dict: exploitability = (br0 + br1) / 2, br [2], num_nodes, subgames, "
         "subgame_iters, seconds, walk_seconds, br_seconds.");
+  m.def("recursive_eval_to_leaf", &recursive_eval_to_leaf, py::arg("cfg"), py::arg("device") = 0, py::arg("num_repeats") = 1,
+        py::arg("seed") = 0, py::arg("flat_weights") = py::none(), py::arg("wave_capacity") = 16384, py::arg("batch_repeats") = 0,
+        py::arg("return_sums") = false, py::arg("full_strategy") = py::none(),
+        "rebel_b200 extension: recursive_eval_sampled's evaluation (the float32 reach-weighted average of num_repeats sampled "
+        "recursive strategies, strategy ids seed .. seed + num_repeats - 1, and its exploitability at every power of two and at "
+        "num_repeats) with the subgames walked level by level on the device and the best responses taken there, without dense "
+        "sums (games with at most 23 actions whose need fits the free device memory).  batch_repeats repeats are walked together "
+        "(<= 0: enough to fill a wave, at most 64).  dict: checkpoints, exploitability [C, 2], num_nodes, subgames, subgame_iters, "
+        "batch_repeats, seconds, draw_seconds, walk_seconds, br_seconds; return_sums adds the compact summed_strategy [N - 1, H] "
+        "(row child - 1) and summed_reach [N, H]; full_strategy (dense [N, H, A]) adds ev_of_full [C, 2] (compute_ev2 against it).");
   m.def("match_stats", &match_stats_py, py::arg("payoff_a"),
         "rebel_b200 extension: play_match's mean, stderr (over the pairs 2i, 2i+1) and seat_means of a payoff vector.");
   py::class_<Agent, std::shared_ptr<Agent>>(

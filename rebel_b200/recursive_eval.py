@@ -5,6 +5,11 @@ strategy against the full-tree solve, the immediate regrets (--print_regret / --
 
     python -m rebel_b200.recursive_eval --num_dice 2 --num_faces 3 --subgame_iters 1024 --cfr --mdp_depth 2 --num_repeats 4097 [--net model.ckpt]
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 -m rebel_b200.recursive_eval ...
+    python -m rebel_b200.recursive_eval --num_dice 2 --num_faces 5 --subgame_iters 1024 --cfr --mdp_depth 2 --num_repeats 4 --device_walk
+
+--device_walk walks the repeats' subgames level by level on the device (rela.recursive_eval_to_leaf) with the same numbers, and is
+taken on its own for games whose full tree has more than 2^20 nodes (2x5f, 5x2f, 1x10f, 1x11f), where the full-tree solve, the
+EVs against it and the regret reports are not available.
 
 Flags follow the reference binary (`--num_dice --num_faces --subgame_iters --mdp_depth --num_repeats --net --cfr --no_linear
 --optimistic --dcfr --num_threads --print_regret --print_regret_summary`).  One process per GPU: rank r solves the contiguous
@@ -121,15 +126,45 @@ def build_parser():
                     help="CFR: summed immediate regrets above mdp_depth / below, at every checkpoint")
     ap.add_argument("--no_full_tree", action="store_true",
                     help="skip the full-tree solve the reference binary always starts with (and the EVs against it)")
-    ap.add_argument("--batch_repeats", type=int, default=64)
+    ap.add_argument("--batch_repeats", type=int, default=None,
+                    help="repeats walked together (default: 64 on the host walk; enough to fill a wave, at most 64, on the device walk)")
     ap.add_argument("--wave_capacity", type=int, default=8192)
     ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast fp32-tanh GELU (default with --net)")
     ap.add_argument("--random_net_seed", type=int, default=None, help="use a random-init Net2 (benchmarks)")
+    ap.add_argument("--device_walk", action="store_true",
+                    help="walk the repeats' subgames level by level on the device and take the best responses there, without dense "
+                         "[N, H, A] sums (the same numbers; always on for games whose full tree has more than 2^20 nodes)")
     return ap
+
+
+DENSE_MAX_NODES = 1 << 20   # the host walk's dense [N, H, A] sums and the full-tree solve stop here (RecursiveEvaluator)
+
+
+def device_walk_plan(args, world):
+    """(device walk?, why the full-tree solve is skipped or None) for these flags; refuses what the device walk cannot report,
+    before any device work."""
+    A = 2 * args.num_dice * args.num_faces + 1
+    large = (1 << A) - 1 > DENSE_MAX_NODES
+    walk = args.device_walk or large
+    if walk and (args.print_regret or args.print_regret_summary):
+        n = (1 << A) - 1
+        raise SystemExit(f"recursive_eval: --print_regret / --print_regret_summary need the dense regret sums [N, H, A] of the "
+                         f"host walk ({n * args.num_faces ** args.num_dice * A * 8 / 1e9:.1f} GB at "
+                         f"{args.num_dice}x{args.num_faces}f); the device walk (--device_walk, or a game whose full tree has more "
+                         f"than 2^20 nodes) does not track regrets")
+    if walk and world > 1:
+        raise SystemExit("recursive_eval: the device walk runs on one GPU (WORLD_SIZE must be 1)")
+    skip = None
+    if args.no_full_tree:
+        skip = "--no_full_tree"
+    elif large:
+        skip = f"the full tree has {(1 << A) - 1} nodes, more than 2^20"
+    return walk, skip
 
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
+    walk, skip_full = device_walk_plan(args, int(os.environ.get("WORLD_SIZE", 1)))
 
     import rebel_b200.rela as rela
     from rebel_b200.models import flatten_state_dict, make_selfplay_net
@@ -160,7 +195,7 @@ def main(argv=None):
     depths = full_tree_depths(args.num_dice, args.num_faces) if want_regrets else None
     report = []        # (name, dense strategy, (expl0, expl1), (ev0, ev1) or None) of recursive_eval.cc:394-408
     full = None
-    if rank == 0 and not args.no_full_tree:
+    if rank == 0 and skip_full is None:
         # "Solving the game for the full tree" (recursive_eval.cc:264-309): exploitability curve at powers of two
         sp.max_depth = 100000
         f = rela.solve_full_tree(cfg, local, track_regrets=want_regrets)
@@ -173,11 +208,27 @@ def main(argv=None):
             print(regret_lines(f["immediate_regrets"], depths, args.mdp_depth, args.print_regret, args.print_regret_summary), flush=True)
         report.append(("full_tree", full, tuple(e), rela.ev_of_strategies(args.num_dice, args.num_faces, full, full)))
     elif rank == 0:
-        print("no full-tree solve (--no_full_tree): the full_tree entry and the EVs against it are not reported", flush=True)
-    if args.num_repeats > 0 and args.mdp_depth > 0:
+        print(f"no full-tree solve ({skip_full}): the full_tree entry and the EVs against it are not reported", flush=True)
+    if args.num_repeats > 0 and args.mdp_depth > 0 and walk:
+        t0 = time.time()
+        r = rela.recursive_eval_to_leaf(cfg, local, args.num_repeats, seed=0, flat_weights=weights, wave_capacity=args.wave_capacity,
+                                        batch_repeats=args.batch_repeats or 0, full_strategy=full)
+        wall = time.time() - t0
+        for i, (n, x) in enumerate(zip(r["checkpoints"], r["exploitability"].tolist())):
+            print(f"{n:5d}: {(x[0] + x[1]) / 2:.6e} ({x[0]:.6e},{x[1]:.6e})")
+            if full is not None:
+                ev = r["ev_of_full"][i].tolist()
+                print(f"\tEV of full: {(ev[0] + ev[1]) / 2:f} ({ev[0]:f},{ev[1]:f})")
+            report.append((f"repeated toleaf {n}", None, tuple(x), tuple(r["ev_of_full"][i].tolist()) if full is not None else None))
+        e = r["exploitability"][-1].tolist()
+        print(json.dumps({"game": f"{args.num_dice}x{args.num_faces}f", "num_repeats": args.num_repeats, "subgame_iters": args.subgame_iters,
+                          "n_gpus": world, "net_mode": net_mode, "exploitability": (e[0] + e[1]) / 2, "exploitability_p0_p1": list(e),
+                          "subgames_solved": int(r["subgames"]), "wall_s": wall, "solver_s_max_over_ranks": r["walk_seconds"],
+                          "repeats_per_s": args.num_repeats / wall}))
+    elif args.num_repeats > 0 and args.mdp_depth > 0:
         lo, hi = strategy_ids(rank, world, args.num_repeats)
         t0 = time.time()
-        r = rela.recursive_eval_sampled(cfg, local, hi - lo, seed=lo, batch_repeats=args.batch_repeats, wave_capacity=args.wave_capacity,
+        r = rela.recursive_eval_sampled(cfg, local, hi - lo, seed=lo, batch_repeats=args.batch_repeats or 64, wave_capacity=args.wave_capacity,
                                         flat_weights=weights, full_strategy=full if world == 1 else None, track_regrets=want_regrets)
         ss, sr = reduce_sums(r["summed_strategy"], r["summed_reach"], device)
         if want_regrets:
