@@ -281,6 +281,38 @@ int cfrb_to_leaf_recursion_order(int32_t num_dice, int32_t num_faces, int32_t ma
 int cfrb_to_leaf_sampled_sums(cfrb_handle* h, float* summed_strategy, float* summed_reach);
 int cfrb_to_leaf_sampled_last(cfrb_handle* h, double* compact, int32_t* act_iteration);
 
+/* ---- Full-game solver: CFR or fictitious play on the whole game tree from the initial state (build_solver(game, params) with an
+ * unlimited depth, subgame_solving.h:119-134), the same numbers as a handle whose one subgame is that tree (cfrb_begin_wave at the
+ * root with uniform beliefs, cfrb_run, the average strategy of cfrb_fetch, cfrb_exploitability) bit for bit, with the tree's
+ * (node, hand) entries spread over the whole device instead of one CTA and no dense [N][H][A] table anywhere, so games up to
+ * A = CFRB_TO_LEAF_MAX_ACTIONS (2x5f, 5x2f, 1x10f, 1x11f) fit.  The object owns its tables, the full tree and a stream.
+ * cfg: num_dice, num_faces, device, solver, linear_update, dcfr (+ alpha, beta, gamma), optimistic (FP) are read; state_dtype
+ * must be CFRB_STATE_F64; max_depth, num_iters, max_subgames, net_mode and hidden are ignored.  Refused before anything is
+ * allocated: A > CFRB_TO_LEAF_MAX_ACTIONS (CFRB_EINVAL, checked without a device), and a cfrb_full_game_bytes need above the
+ * device's free memory (CFRB_ENOMEM).  Starts at iteration 0 in the state of the CFR constructor (subgame_solving.cc:509-524). */
+typedef struct cfrb_full_game cfrb_full_game;
+int cfrb_full_game_create(const cfrb_config* cfg, cfrb_full_game** out);
+int cfrb_full_game_destroy(cfrb_full_game* g);
+/* Host-only: device bytes of a full-game object beyond its handle: the full tree, its compact strategy pair and best-response
+ * scratch (cfrb_to_leaf_bytes' tree part), the per-edge tables [N - 1][H] (CFR: regrets, current and sum strategy; FP: average and
+ * sum strategy), the per-node reach and values [N][H] and the iteration counter.  solver: CFRB_SOLVER_*.  A > 26: CFRB_EINVAL. */
+int64_t cfrb_full_game_bytes(int32_t num_dice, int32_t num_faces, int32_t solver);
+/* Run `iters` more iterations (iteration i has traverser i % 2), each one replayed from a CUDA graph of its level launches.
+ * Returns when they have finished. */
+int cfrb_full_game_step(cfrb_full_game* g, int32_t iters);
+/* Iterations done so far; full-tree node count N. */
+int cfrb_full_game_iterations(const cfrb_full_game* g);
+int cfrb_full_game_nodes(const cfrb_full_game* g);
+/* Best-response values {br0, br1} of the current average strategy (compute_exploitability2); the exploitability is their mean. */
+int cfrb_full_game_exploitability(cfrb_full_game* g, double* out2);
+/* The current average strategy (get_strategy), compact [N - 1][H] fp64 with entry (child - 1) * H + hand. */
+int cfrb_full_game_strategy(cfrb_full_game* g, double* compact);
+/* Device memory the object took when it was created (the drop of the device's free memory; cudaMalloc rounds up) and the part of
+ * it its handle took.  Either pointer may be NULL. */
+int cfrb_full_game_memory(const cfrb_full_game* g, int64_t* total_bytes, int64_t* handle_bytes);
+/* Test aid: cfrb_full_game_create sees at most `bytes` free device bytes (0 = the device's own figure); process-wide. */
+int cfrb_debug_full_game_free_cap(int64_t bytes);
+
 /* Immediate-regret accumulator on the handle's device, compute_immediate_regrets (subgame_solving.cc:984-1050) split so that a
  * list of strategies can be added in pieces: adding strategies in batches of any size gives the bits of one pass over the whole
  * list.  Reset zeroes the sums [N_full][H][A] and the count (and must precede the first add). */

@@ -82,6 +82,17 @@ def lib():
     L.cfrb_to_leaf_recursion_order.argtypes = [C.c_int32] * 3 + [_ip, _ip, C.c_int32]
     L.cfrb_to_leaf_sampled_sums.argtypes = [vp, _fp, _fp]
     L.cfrb_to_leaf_sampled_last.argtypes = [vp, _dp, _ip]
+    L.cfrb_full_game_create.argtypes = [C.POINTER(Config), C.POINTER(vp)]
+    L.cfrb_full_game_destroy.argtypes = [vp]
+    L.cfrb_full_game_bytes.argtypes = [C.c_int32] * 3
+    L.cfrb_full_game_bytes.restype = C.c_int64
+    L.cfrb_full_game_step.argtypes = [vp, C.c_int32]
+    L.cfrb_full_game_iterations.argtypes = [vp]
+    L.cfrb_full_game_nodes.argtypes = [vp]
+    L.cfrb_full_game_exploitability.argtypes = [vp, _dp]
+    L.cfrb_full_game_strategy.argtypes = [vp, _dp]
+    L.cfrb_full_game_memory.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    L.cfrb_debug_full_game_free_cap.argtypes = [C.c_int64]
     L.cfrb_regrets_reset.argtypes = [vp]
     L.cfrb_regrets_add.argtypes = [vp, _fp, C.c_int32]
     L.cfrb_regrets_add_current.argtypes = [vp]
@@ -187,6 +198,12 @@ def to_leaf_sampled_bytes(num_dice, num_faces, max_depth, max_subgames, batch_re
     return _check(lib().cfrb_to_leaf_sampled_bytes(num_dice, num_faces, max_depth, max_subgames, batch_repeats))
 
 
+def full_game_bytes(num_dice, num_faces, solver=SOLVER_CFR):
+    """Host-only: device bytes a FullGame of this game and solver needs beyond its handle (full tree, best-response scratch, the
+    solver's per-edge and per-node fp64 tables)."""
+    return _check(lib().cfrb_full_game_bytes(num_dice, num_faces, solver))
+
+
 def to_leaf_recursion_order(num_dice, num_faces, max_depth):
     """Host-only: (level_pos [R], level_begin [A + 1]) of the R subgame roots of a to-leaf walk: level_pos[k] is the position in
     the walk's level order of the k-th root in the reference's recursion order (the order of its act_iteration draws)."""
@@ -211,6 +228,56 @@ def net_output_bound(num_dice, num_faces, flat, hidden=256):
 def tc_net_supported(num_dice, num_faces, hidden=256):
     """Host-only: does a tensor-core value net (NET_TC_F16 / NET_TC_F16X2) fit this game?  Otherwise NET_FP32 serves it."""
     return bool(lib().cfrb_tc_net_supported(num_dice, num_faces, hidden))
+
+
+class FullGame:
+    """CFR or fictitious play on the whole game tree, spread over the GPU (cfrb_full_game_*): the numbers of a one-subgame
+    WaveSolver rooted at the initial state, for games of up to 23 actions.  strategy() is compact [N - 1, H] (entry
+    (child - 1) * H + hand)."""
+
+    def __init__(self, num_dice, num_faces, solver=SOLVER_CFR, linear_update=True, dcfr=False, dcfr_alpha=0.0, dcfr_beta=0.0,
+                 dcfr_gamma=0.0, optimistic=False, device=0):
+        L = lib()
+        self.cfg = Config(num_dice, num_faces, 1, 1, int(linear_update), int(dcfr), dcfr_alpha, dcfr_beta, dcfr_gamma, 1, device,
+                          NET_ZERO, 256, STATE_F64, int(solver), int(optimistic))
+        self._g = C.c_void_p()
+        _check(L.cfrb_full_game_create(C.byref(self.cfg), C.byref(self._g)))
+        self.H = num_faces ** num_dice
+        self.N = _check(L.cfrb_full_game_nodes(self._g))
+
+    def close(self):
+        if self._g:
+            lib().cfrb_full_game_destroy(self._g)
+            self._g = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def step(self, iters):
+        _check(lib().cfrb_full_game_step(self._g, iters))
+
+    @property
+    def iterations(self):
+        return _check(lib().cfrb_full_game_iterations(self._g))
+
+    def exploitability(self):
+        out = np.zeros(2)
+        _check(lib().cfrb_full_game_exploitability(self._g, _p(out, _dp)))
+        return out
+
+    def strategy(self):
+        out = np.zeros((self.N - 1, self.H))
+        _check(lib().cfrb_full_game_strategy(self._g, _p(out, _dp)))
+        return out
+
+    def memory(self):
+        """(bytes the object took on the device, the part its handle took)."""
+        tot, hnd = C.c_int64(), C.c_int64()
+        _check(lib().cfrb_full_game_memory(self._g, C.byref(tot), C.byref(hnd)))
+        return tot.value, hnd.value
 
 
 class WaveSolver:

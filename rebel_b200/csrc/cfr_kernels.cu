@@ -12,6 +12,7 @@
 #include "agent_kernels.cuh"
 #include "expl_kernels.cuh"
 #include "expl_sampled_kernels.cuh"
+#include "full_game_kernels.cuh"
 
 namespace cfrb {
 
@@ -199,6 +200,29 @@ void expl_sampled_launch_finalize(const ExplSampledDev& p, cudaStream_t st) {
   const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 8);
   expl_sampled_finalize_kernel<<<std::max(blocks, 1), 256, 0, st>>>(p);
 }
+// Full-game solver: level_begin is the host copy of the full tree's [levels + 1] level starts; grids are sized per level.
+static int fg_blocks(long long items, int max_blocks) {
+  return (int)std::max<long long>(1, std::min<long long>((items + 255) / 256, max_blocks));
+}
+void full_game_launch_init(const FullGameDev& p, const int* level_begin, int levels, int max_blocks, cudaStream_t st) {
+  for (int d = 1; d < levels; ++d) {
+    const int nb = level_begin[d], ne = level_begin[d + 1];
+    fg_init_kernel<<<fg_blocks((long long)(ne - nb) * p.H, max_blocks), 256, 0, st>>>(p, nb, ne, d);
+  }
+}
+void full_game_launch_iter(const FullGameDev& p, const int* level_begin, int levels, int max_blocks, cudaStream_t st) {
+  auto blocks = [&](int d) { return fg_blocks((long long)(level_begin[d + 1] - level_begin[d]) * p.H, max_blocks); };
+  if (p.fp)
+    for (int d = 1; d < levels; ++d) fg_reach_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
+  fg_terminal_kernel<<<fg_blocks(p.T, max_blocks), 256, 0, st>>>(p);
+  for (int d = levels - 2; d >= 0; --d) fg_up_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
+  for (int d = 0; d + 1 < levels; ++d) fg_down_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
+  fg_advance_kernel<<<1, 1, 0, st>>>(p.iter);
+}
+void full_game_launch_average(const FullGameDev& p, const int* depth, int untouched0, int untouched1, int max_blocks, cudaStream_t st) {
+  fg_average_kernel<<<fg_blocks((long long)p.N * p.H, max_blocks), 256, 0, st>>>(p, depth, untouched0, untouched1);
+}
+
 __global__ void rows_gather_kernel(const float* __restrict__ src, int width, const int* __restrict__ ids, int n, float* __restrict__ out) {
   const size_t total = (size_t)n * width;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {

@@ -296,6 +296,28 @@ template <typename real> void expl_sampled_launch_begin(const ExplSampledDev& p,
 template <typename real> void expl_sampled_launch_expand(const ExplSampledDev& p, int n, const real* snap, cudaStream_t st);
 // strategy = (double)(sum_s / (sum_r[parent] + 1e-6f)), the final strategy of a checkpoint
 void expl_sampled_launch_finalize(const ExplSampledDev& p, cudaStream_t st);
+// Full-game solver (full_game_kernels.cuh): CFR or FP on the full tree of the handle's game (BrState), fp64, one level per launch.
+struct FullGameDev {
+  int N, T, H, F;
+  int fp, linear, dcfr, optimistic;
+  double dcfr_alpha, dcfr_beta, dcfr_gamma;
+  double b0;                      // root belief of every hand, 1 / H
+  const int* parent; const int* child_begin; const int* nchild; const int* term_node;   // the full tree (BrDev's arrays)
+  const unsigned char* matches;   // [H][F]
+  double* R;                      // [N - 1][H] regrets (CFR; nullptr in FP)
+  double* Sg;                     // [N - 1][H] current strategy (FP: average strategy)
+  double* S;                      // [N - 1][H] sum strategy
+  double* reach;                  // [N][H] reach of one player (FP: also the best-response flags)
+  double* val;                    // [N][H] values (FP: also the traverser's beliefs)
+  double* avg;                    // [N - 1][H] the average strategy a checkpoint evaluates (BrDev::strategy)
+  int* iter;                      // [1] iterations done; the traverser of iteration i is i & 1
+};
+// CFR constructor on the full tree (iteration counter left alone)
+void full_game_launch_init(const FullGameDev& p, const int* level_begin, int levels, int max_blocks, cudaStream_t st);
+// one iteration: about 2 (CFR) or 3 (FP) launches per depth level, then the counter's increment
+void full_game_launch_iter(const FullGameDev& p, const int* level_begin, int levels, int max_blocks, cudaStream_t st);
+// CFR's normalised sum into p.avg (FP: the host copies Sg)
+void full_game_launch_average(const FullGameDev& p, const int* depth, int untouched0, int untouched1, int max_blocks, cudaStream_t st);
 // rows [ids[i]] of a [*, width] fp32 matrix -> out[i]  (replay sampling)
 void rows_launch_gather(const float* src, int width, const int* ids, int n, float* out, cudaStream_t st);
 

@@ -2087,6 +2087,185 @@ int cfrb_to_leaf_sampled_last(cfrb_handle* h, double* compact, int32_t* act_iter
   return CFRB_OK;
 }
 
+// ============================================================================================ full-game solver
+// A handle of the game with depth-1 templates and one subgame lends its full tree (full_tree_setup), best-response scratch, match
+// table and stream; the object adds the solver's tables and the CUDA graph of one iteration.
+struct cfrb_full_game {
+  cfrb_handle* h = nullptr;
+  bool fp = false;
+  int iters = 0;
+  DevBuf<double> R, Sg, S, reach, val;
+  DevBuf<int> iter;
+  cfrb::FullGameDev dev{};
+  GraphExec graph;
+  int64_t total_bytes = 0, handle_bytes = 0;
+  ~cfrb_full_game() {
+    if (h) cfrb_destroy(h);   // synchronises its stream, on which every kernel of the object ran
+  }
+};
+
+static int64_t g_full_game_free_cap = 0;
+
+static int64_t full_game_bytes(const cfrb::GameShape& g, bool fp) {
+  const int64_t H = g.H, N = ((int64_t)1 << g.A) - 1;
+  return to_leaf_sizes(g, 1, 1).tree_bytes + ((fp ? 2 : 3) * (N - 1) * H + 2 * N * H) * 8 + 4;
+}
+
+int64_t cfrb_full_game_bytes(int32_t num_dice, int32_t num_faces, int32_t solver) {
+  if (num_dice < 1 || num_faces < 1) return fail(CFRB_EINVAL, "cfrb_full_game_bytes: num_dice, num_faces must be >= 1");
+  if (solver != CFRB_SOLVER_CFR && solver != CFRB_SOLVER_FP) return fail(CFRB_EINVAL, "cfrb_full_game_bytes: bad solver");
+  if (2L * num_dice * num_faces + 1 > 26) return fail(CFRB_EINVAL, "cfrb_full_game_bytes: full tree too large (2^A - 1 nodes, A > 26)");
+  return full_game_bytes(cfrb::GameShape(num_dice, num_faces), solver == CFRB_SOLVER_FP);
+}
+
+int cfrb_debug_full_game_free_cap(int64_t bytes) {
+  if (bytes < 0) return fail(CFRB_EINVAL, "cfrb_debug_full_game_free_cap: bad argument");
+  g_full_game_free_cap = bytes;
+  return CFRB_OK;
+}
+
+static int full_game_create_impl(const cfrb_config* cfg, cfrb_full_game* fg) {
+  const int64_t A = 2L * cfg->num_dice * cfg->num_faces + 1;
+  if (cfg->num_dice < 1 || cfg->num_faces < 1) return fail(CFRB_EINVAL, "cfrb_full_game_create: num_dice, num_faces must be >= 1");
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, "cfrb_full_game_create: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                                 " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+  if (cfg->solver != CFRB_SOLVER_CFR && cfg->solver != CFRB_SOLVER_FP) return fail(CFRB_EINVAL, "cfrb_full_game_create: bad solver");
+  if (cfg->state_dtype != CFRB_STATE_F64) return fail(CFRB_EINVAL, "cfrb_full_game_create: the full-game solver keeps fp64 tables only");
+  if (cfrb_device_count() == 0) return fail(CFRB_ENODEV, "no CUDA device visible: libcfrb200 has no CPU fallback");
+  if (cfg->device < 0 || cfg->device >= cfrb_device_count()) return fail(CFRB_EINVAL, "device ordinal out of range");
+  CK(cudaSetDevice(cfg->device));
+  const cfrb::GameShape g(cfg->num_dice, cfg->num_faces);
+  fg->fp = cfg->solver == CFRB_SOLVER_FP;
+  // refused before anything is allocated: on a shared device an allocation that fails late may starve other processes
+  const int64_t need = full_game_bytes(g, fg->fp);
+  size_t free0 = 0, total = 0;
+  CK(cudaMemGetInfo(&free0, &total));
+  const int64_t avail = g_full_game_free_cap > 0 ? std::min<int64_t>((int64_t)free0, g_full_game_free_cap) : (int64_t)free0;
+  if (need > avail)
+    return fail(CFRB_ENOMEM, "cfrb_full_game_create: needs " + std::to_string(need) + " bytes of device memory beyond the handle, " +
+                                 std::to_string(avail) + " free");
+  cfrb_config c = *cfg;
+  c.max_depth = 1; c.num_iters = 1; c.max_subgames = 1; c.net_mode = CFRB_NET_ZERO; c.hidden = 256;
+  int rc = cfrb_create(&c, &fg->h);
+  if (rc) return rc;
+  cfrb_handle* h = fg->h;
+  size_t free1 = 0;
+  CK(cudaMemGetInfo(&free1, &total));
+  fg->handle_bytes = (int64_t)free0 - (int64_t)free1;
+  if ((rc = full_tree_setup(h, "cfrb_full_game_create"))) return rc;
+  const auto& t = h->br.t;
+  const size_t E = (size_t)(t.N - 1) * g.H, NH = (size_t)t.N * g.H;
+  if (!fg->fp) CK(fg->R.alloc(E));
+  CK(fg->Sg.alloc(E)); CK(fg->S.alloc(E)); CK(fg->reach.alloc(NH)); CK(fg->val.alloc(NH)); CK(fg->iter.alloc(1));
+  cfrb::FullGameDev& d = fg->dev;
+  d.N = t.N; d.T = t.T; d.H = g.H; d.F = g.F;
+  d.fp = fg->fp; d.linear = cfg->linear_update; d.dcfr = cfg->dcfr; d.optimistic = fg->fp && cfg->optimistic;
+  d.dcfr_alpha = cfg->dcfr_alpha; d.dcfr_beta = cfg->dcfr_beta; d.dcfr_gamma = cfg->dcfr_gamma;
+  d.b0 = 1.0 / g.H;   // the root beliefs of the full-tree solve (FullTreeSolver)
+  d.parent = h->br.parent.p; d.child_begin = h->br.child_begin.p; d.nchild = h->br.nchild.p; d.term_node = h->br.term_node.p;
+  d.matches = h->d_matches.p;
+  d.R = fg->fp ? nullptr : fg->R.p; d.Sg = fg->Sg.p; d.S = fg->S.p; d.reach = fg->reach.p; d.val = fg->val.p;
+  d.avg = h->br.strategy.p; d.iter = fg->iter.p;
+  cudaStream_t st = h->own_stream;
+  CK(cudaMemsetAsync(fg->iter.p, 0, sizeof(int), st));
+  cfrb::full_game_launch_init(d, t.level_begin.data(), t.levels, 8 * h->num_sms, st);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  size_t free2 = 0;
+  CK(cudaMemGetInfo(&free2, &total));
+  fg->total_bytes = (int64_t)free0 - (int64_t)free2;
+  return CFRB_OK;
+}
+
+int cfrb_full_game_create(const cfrb_config* cfg, cfrb_full_game** out) {
+  if (!cfg || !out) return fail(CFRB_EINVAL, "cfrb_full_game_create: null argument");
+  *out = nullptr;
+  auto fg = std::make_unique<cfrb_full_game>();
+  const int rc = full_game_create_impl(cfg, fg.get());
+  if (rc) return rc;
+  *out = fg.release();
+  return CFRB_OK;
+}
+
+int cfrb_full_game_destroy(cfrb_full_game* g) {
+  if (!g) return CFRB_OK;
+  cudaSetDevice(g->h ? g->h->cfg.device : 0);
+  delete g;
+  return CFRB_OK;
+}
+
+int cfrb_full_game_step(cfrb_full_game* g, int32_t iters) {
+  if (!g || iters < 0) return fail(CFRB_EINVAL, "cfrb_full_game_step: bad argument");
+  if (iters == 0) return CFRB_OK;
+  cfrb_handle* h = g->h;
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t st = h->own_stream;
+  const auto& t = h->br.t;
+  if (!g->graph) {   // one iteration, captured once: its level launches replay without host launch cost
+    CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    cfrb::full_game_launch_iter(g->dev, t.level_begin.data(), t.levels, 8 * h->num_sms, st);
+    Graph graph;
+    const cudaError_t launched = cudaGetLastError();
+    CK(cudaStreamEndCapture(st, graph.put()));
+    CK(launched);
+    CK(cudaGraphInstantiate(g->graph.put(), graph, 0));
+  }
+  for (int i = 0; i < iters; ++i) CK(cudaGraphLaunch(g->graph, st));
+  CK(cudaStreamSynchronize(st));
+  g->iters += iters;
+  return CFRB_OK;
+}
+
+int cfrb_full_game_iterations(const cfrb_full_game* g) { return g ? g->iters : fail(CFRB_EINVAL, "null full game"); }
+int cfrb_full_game_nodes(const cfrb_full_game* g) { return g ? g->h->br.t.N : fail(CFRB_EINVAL, "null full game"); }
+
+// The average strategy into the handle's compact full-tree strategy (the one br_kernel reads).
+static int full_game_average(cfrb_full_game* g) {
+  cfrb_handle* h = g->h;
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t st = h->own_stream;
+  if (g->fp) {
+    CK(cudaMemcpyAsync(h->br.strategy.p, g->Sg.p, g->Sg.n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  } else {
+    // a player whose strategy has not been updated yet keeps the uniform average (normalise_avg): player 0 updates in even
+    // iterations, player 1 in odd ones
+    const int steps0 = (g->iters + 1) / 2, steps1 = g->iters / 2;
+    cfrb::full_game_launch_average(g->dev, h->br.depth.p, steps0 == 0, steps1 == 0, 8 * h->num_sms, st);
+    CK(cudaGetLastError());
+  }
+  return CFRB_OK;
+}
+
+int cfrb_full_game_exploitability(cfrb_full_game* g, double* out2) {
+  if (!g || !out2) return fail(CFRB_EINVAL, "cfrb_full_game_exploitability: null argument");
+  int rc = full_game_average(g);
+  if (rc) return rc;
+  cfrb_handle* h = g->h;
+  cfrb::br_launch(full_tree_dev(h), h->own_stream);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out2, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  return CFRB_OK;
+}
+
+int cfrb_full_game_strategy(cfrb_full_game* g, double* compact) {
+  if (!g || !compact) return fail(CFRB_EINVAL, "cfrb_full_game_strategy: null argument");
+  int rc = full_game_average(g);
+  if (rc) return rc;
+  cfrb_handle* h = g->h;
+  CK(cudaMemcpyAsync(compact, h->br.strategy.p, g->Sg.n * sizeof(double), cudaMemcpyDeviceToHost, h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  return CFRB_OK;
+}
+
+int cfrb_full_game_memory(const cfrb_full_game* g, int64_t* total_bytes, int64_t* handle_bytes) {
+  if (!g) return fail(CFRB_EINVAL, "null full game");
+  if (total_bytes) *total_bytes = g->total_bytes;
+  if (handle_bytes) *handle_bytes = g->handle_bytes;
+  return CFRB_OK;
+}
+
 // ============================================================================================ device-resident self-play
 int cfrb_selfplay_create(cfrb_handle* h, int32_t n_games, const uint32_t* seeds, float random_action_prob, int32_t sample_leaf) {
   if (!h || !seeds) return fail(CFRB_EINVAL, "null argument");

@@ -578,6 +578,63 @@ py::dict solve_full_tree(RecursiveSolvingParams cfg, int device, bool track_regr
   return d;
 }
 
+// solve_full_tree's solve on the whole GPU (cfrb_full_game_*): the same checkpoints, exploitabilities and printed lines, bit for
+// bit, and the final average strategy in compact form [N - 1, H] (entry (child - 1) * H + hand), so that games of up to 23
+// actions fit.  Times: the iterations and the best responses, host wall time around calls that synchronise.
+py::dict solve_full_game(RecursiveSolvingParams cfg, int device) {
+  const int A = 2 * cfg.num_dice * cfg.num_faces + 1;
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)   // the library's own refusal, before a device is touched
+    throw std::runtime_error("solve_full_game: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                             " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+  std::vector<int> cps;
+  std::vector<std::array<double, 2>> expl;
+  std::vector<double> strategy;
+  int N = 0;
+  int64_t H = 1, total_bytes = 0, handle_bytes = 0;
+  for (int i = 0; i < cfg.num_dice; ++i) H *= cfg.num_faces;
+  double solve_s = 0, br_s = 0, total_s = 0;
+  const int iters = cfg.subgame_params.num_iters;
+  {
+    py::gil_scoped_release nogil;
+    const auto t0 = std::chrono::steady_clock::now();
+    cfrb_config c = liars_dice::solver_config(cfg, device, 1);
+    c.net_mode = CFRB_NET_ZERO;
+    cfrb_full_game* raw = nullptr;
+    check(cfrb_full_game_create(&c, &raw), "cfrb_full_game_create");
+    const FullGamePtr fg(raw);
+    N = check(cfrb_full_game_nodes(fg.get()), "cfrb_full_game_nodes");
+    check(cfrb_full_game_memory(fg.get(), &total_bytes, &handle_bytes), "cfrb_full_game_memory");
+    int done = 0;
+    for (int iter = 0; iter < iters; ++iter) {
+      if (((iter + 1) & iter) != 0 && iter + 1 != iters) continue;   // checkpoints at powers of two and at the end
+      const auto a = std::chrono::steady_clock::now();
+      check(cfrb_full_game_step(fg.get(), iter + 1 - done), "cfrb_full_game_step");
+      done = iter + 1;
+      const auto b = std::chrono::steady_clock::now();
+      std::array<double, 2> v{};
+      check(cfrb_full_game_exploitability(fg.get(), v.data()), "cfrb_full_game_exploitability");
+      const auto e = std::chrono::steady_clock::now();
+      solve_s += std::chrono::duration<double>(b - a).count();
+      br_s += std::chrono::duration<double>(e - b).count();
+      std::printf("Iter=%8d exploitabilities=(%.3e, %.3e) sum=%.3e\n", iter + 1, v[0], v[1], (v[0] + v[1]) / 2.);
+      std::fflush(stdout);
+      cps.push_back(iter + 1);
+      expl.push_back(v);
+    }
+    strategy.resize((size_t)(N - 1) * H);
+    check(cfrb_full_game_strategy(fg.get(), strategy.data()), "cfrb_full_game_strategy");
+    total_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  }
+  py::dict d;
+  d["checkpoints"] = cps;
+  d["exploitability"] = pairs_tensor(expl);
+  d["strategy"] = f64_tensor(strategy, {(int64_t)N - 1, H});
+  d["num_nodes"] = N;
+  d["seconds"] = total_s; d["solve_seconds"] = solve_s; d["br_seconds"] = br_s;
+  d["device_bytes"] = total_bytes; d["handle_bytes"] = handle_bytes;
+  return d;
+}
+
 // compute_exploitability2 (subgame_solving.cc:802-816) of a dense full-tree strategy [N][H][A] on the GPU best-response kernel.
 std::tuple<double, double> exploitability_of_strategy(int num_dice, int num_faces, torch::Tensor strategy) {
   FullTreeHandle f(num_dice, num_faces);
@@ -965,6 +1022,11 @@ PYBIND11_MODULE(rela, m) {
         "rebel_b200 extension: recursive_eval's full-tree solve — dict with checkpoints, exploitability [C, 2], the final "
         "get_strategy() [N, H, A] and, with track_regrets (CFR), the immediate regrets of the sampling strategies of the "
         "even iterations (immediate_regrets, regret_sums, regret_count).");
+  m.def("solve_full_game", &solve_full_game, py::arg("cfg"), py::arg("device") = 0,
+        "rebel_b200 extension: solve_full_tree's solve with the tree spread over the whole GPU, for games of up to 23 actions — "
+        "dict with checkpoints, exploitability [C, 2] (the same bits), the final average strategy in compact form [N - 1, H] "
+        "(entry (child - 1) * H + hand), num_nodes, seconds, solve_seconds, br_seconds, device_bytes and handle_bytes (device "
+        "memory the solver took, and the part its handle took).");
   m.def("play_match", &play_match_py, py::arg("cfg_a"), py::arg("cfg_b"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
         py::arg("policy") = "sampled", py::arg("flat_weights_a") = py::none(), py::arg("flat_weights_b") = py::none(),
         py::arg("concurrent_games") = 8192,
