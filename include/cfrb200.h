@@ -275,6 +275,24 @@ int64_t cfrb_to_leaf_sampled_bytes(int32_t num_dice, int32_t num_faces, int32_t 
  * last.  Returns R. */
 int cfrb_to_leaf_recursion_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t* level_pos, int32_t* level_begin,
                                  int32_t cap);
+/* cfrb_to_leaf_sampled with a compact baseline and immediate regrets, for games whose dense [N][H][A] tables do not fit.
+ * ev_full_compact (may be NULL): the full-tree strategy compact [N_full - 1][H] fp64 (entry (child - 1) * H + hand); ev_out as in
+ * cfrb_to_leaf_sampled.  track_regrets: every repeat's sampled strategy, as float32, goes into compact fp64 regret sums after its
+ * batch, in repeat order (RecursiveEvaluator::run's cfrb_regrets_add, bit for bit); at checkpoint c, regret_summary[2c .. 2c+1] =
+ * report_regrets' (sum of the immediate regrets of the nodes with depth < regret_depth, of the rest); at the last checkpoint
+ * immediate [N_full][H] (may be NULL) gets the immediate regrets, and after the call regret_sums [N_full - 1][H] (may be NULL) the
+ * raw sums and regret_count the number of strategies added.  The need check covers cfrb_to_leaf_sampled_regret_bytes more. */
+int cfrb_to_leaf_sampled_ev_regrets(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int32_t batch_repeats, int32_t cap,
+                                    int32_t* checkpoints, double* br_out, const double* ev_full_compact, double* ev_out,
+                                    int32_t track_regrets, int32_t regret_depth, double* regret_summary, double* immediate,
+                                    double* regret_sums, int64_t* regret_count, int64_t* subgames, int64_t* subgame_iters,
+                                    double* seconds3);
+/* Host-only: the device bytes track_regrets adds to a sampled walk: 8 (N - 1) H of sums and 4 (N - 1) H per repeat of a batch.
+ * A > CFRB_TO_LEAF_MAX_ACTIONS: CFRB_EINVAL. */
+int64_t cfrb_to_leaf_sampled_regret_bytes(int32_t num_dice, int32_t num_faces, int32_t batch_repeats);
+/* Host-only: compute_ev2 of two compact full-tree strategies [N_full - 1][H] on the handle's full tree (cfrb_ev2 without the dense
+ * tables). */
+int cfrb_ev2_compact(cfrb_handle* h, const double* s1, const double* s2, double* out2);
 /* Test aids of the last cfrb_to_leaf_sampled: its accumulators, summed_strategy [N_full - 1][H] (entry (child - 1) * H + hand)
  * and summed_reach [N_full][H]; the last repeat's sampled strategy [N_full - 1][H] (fp64) and the act_iteration of every subgame
  * root of that repeat, [N_full] by full-tree node (-1 where no subgame is rooted). */
@@ -312,6 +330,19 @@ int cfrb_full_game_strategy(cfrb_full_game* g, double* compact);
 int cfrb_full_game_memory(const cfrb_full_game* g, int64_t* total_bytes, int64_t* handle_bytes);
 /* Test aid: cfrb_full_game_create sees at most `bytes` free device bytes (0 = the device's own figure); process-wide. */
 int cfrb_debug_full_game_free_cap(int64_t bytes);
+/* Immediate regrets of the full-game solve (CFR only, as the reference's full-tree solve tracks them): after
+ * cfrb_full_game_track_regrets, cfrb_full_game_step adds the sampling strategy after every iteration with an even index to compact
+ * fp64 sums [N - 1][H] (entry (child - 1) * H + hand), computed over the whole device.  The sums, immediate regrets and count are
+ * bit-identical to cfrb_regrets_add_current after the same iterations of a one-subgame handle.  track_regrets refuses FP
+ * (CFRB_EINVAL), an object that has already stepped (CFRB_ESTATE) and a cfrb_full_game_regret_bytes need above the free device
+ * memory (CFRB_ENOMEM, before anything is allocated); a second call changes nothing. */
+int cfrb_full_game_track_regrets(cfrb_full_game* g);
+/* Host-only: the device bytes cfrb_full_game_track_regrets adds, 8 (N - 1) H.  A > CFRB_TO_LEAF_MAX_ACTIONS: CFRB_EINVAL. */
+int64_t cfrb_full_game_regret_bytes(int32_t num_dice, int32_t num_faces);
+/* immediate [N][H] = cfrb_regrets_fetch's max over the A action slots (0.0 for illegal ones) / count, 0 at leaves; sums [N - 1][H]
+ * compact raw; node_sums [N] = per node, the sum of immediate over hands in hand order (report_regrets' inner sum, so the host
+ * adds them in node order for its summary); count = strategies added.  Any pointer may be NULL.  Synchronises. */
+int cfrb_full_game_regrets(cfrb_full_game* g, double* immediate, double* sums, double* node_sums, int64_t* count);
 
 /* Immediate-regret accumulator on the handle's device, compute_immediate_regrets (subgame_solving.cc:984-1050) split so that a
  * list of strategies can be added in pieces: adding strategies in batches of any size gives the bits of one pass over the whole

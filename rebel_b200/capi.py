@@ -93,6 +93,15 @@ def lib():
     L.cfrb_full_game_strategy.argtypes = [vp, _dp]
     L.cfrb_full_game_memory.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.cfrb_debug_full_game_free_cap.argtypes = [C.c_int64]
+    L.cfrb_full_game_track_regrets.argtypes = [vp]
+    L.cfrb_to_leaf_sampled_ev_regrets.argtypes = ([vp] + [C.c_int32] * 4 + [_ip, _dp, _dp, _dp, C.c_int32, C.c_int32, _dp, _dp, _dp]
+                                                  + [C.POINTER(C.c_int64)] * 3 + [_dp])
+    L.cfrb_to_leaf_sampled_regret_bytes.argtypes = [C.c_int32] * 3
+    L.cfrb_to_leaf_sampled_regret_bytes.restype = C.c_int64
+    L.cfrb_ev2_compact.argtypes = [vp, _dp, _dp, _dp]
+    L.cfrb_full_game_regret_bytes.argtypes = [C.c_int32] * 2
+    L.cfrb_full_game_regret_bytes.restype = C.c_int64
+    L.cfrb_full_game_regrets.argtypes = [vp, _dp, _dp, _dp, C.POINTER(C.c_int64)]
     L.cfrb_regrets_reset.argtypes = [vp]
     L.cfrb_regrets_add.argtypes = [vp, _fp, C.c_int32]
     L.cfrb_regrets_add_current.argtypes = [vp]
@@ -198,10 +207,22 @@ def to_leaf_sampled_bytes(num_dice, num_faces, max_depth, max_subgames, batch_re
     return _check(lib().cfrb_to_leaf_sampled_bytes(num_dice, num_faces, max_depth, max_subgames, batch_repeats))
 
 
+def to_leaf_sampled_regret_bytes(num_dice, num_faces, batch_repeats):
+    """Host-only: device bytes WaveSolver.to_leaf_sampled_regrets adds for its regrets (the compact fp64 sums [N - 1, H] and the
+    float32 strategies of a batch); games above 23 actions are refused."""
+    return _check(lib().cfrb_to_leaf_sampled_regret_bytes(num_dice, num_faces, batch_repeats))
+
+
 def full_game_bytes(num_dice, num_faces, solver=SOLVER_CFR):
     """Host-only: device bytes a FullGame of this game and solver needs beyond its handle (full tree, best-response scratch, the
     solver's per-edge and per-node fp64 tables)."""
     return _check(lib().cfrb_full_game_bytes(num_dice, num_faces, solver))
+
+
+def full_game_regret_bytes(num_dice, num_faces):
+    """Host-only: device bytes FullGame.track_regrets adds (the compact fp64 regret sums [N - 1, H]); games above 23 actions are
+    refused."""
+    return _check(lib().cfrb_full_game_regret_bytes(num_dice, num_faces))
 
 
 def to_leaf_recursion_order(num_dice, num_faces, max_depth):
@@ -278,6 +299,18 @@ class FullGame:
         tot, hnd = C.c_int64(), C.c_int64()
         _check(lib().cfrb_full_game_memory(self._g, C.byref(tot), C.byref(hnd)))
         return tot.value, hnd.value
+
+    def track_regrets(self):
+        """CFR only, before the first step: from now on every iteration with an even index adds its sampling strategy to the
+        immediate-regret sums (full_game_regret_bytes more device memory)."""
+        _check(lib().cfrb_full_game_track_regrets(self._g))
+
+    def regrets(self):
+        """(immediate regrets [N, H], compact sums [N - 1, H], per-node sums of the immediate regrets over hands [N], count)."""
+        imm, sums, node = np.zeros((self.N, self.H)), np.zeros((self.N - 1, self.H)), np.zeros(self.N)
+        count = C.c_int64()
+        _check(lib().cfrb_full_game_regrets(self._g, _p(imm, _dp), _p(sums, _dp), _p(node, _dp), C.byref(count)))
+        return imm, sums, node, count.value
 
 
 class WaveSolver:
@@ -430,6 +463,33 @@ class WaveSolver:
                                               C.byref(sg), C.byref(it), _p(secs, _dp)))
         return {"checkpoints": cps[:n].tolist(), "br": br[:n].copy(), "subgames": sg.value, "subgame_iters": it.value,
                 "draw_seconds": float(secs[0]), "walk_seconds": float(secs[1]), "br_seconds": float(secs[2])}
+
+    def to_leaf_sampled_regrets(self, num_repeats, seed=0, batch_repeats=1, full_compact=None, regret_depth=2):
+        """to_leaf_sampled with the immediate regrets of the sampled strategies and, with full_compact (a compact [N - 1, H]
+        full-tree strategy), the EV against it at every checkpoint.  dict as to_leaf_sampled's plus regret_summary [C, 2] (depth
+        < regret_depth, rest), immediate_regrets [N, H], regret_sums [N - 1, H], regret_count and ev [C, 2]."""
+        cap = 64
+        cps, br, ev, summ = np.zeros(cap, np.int32), np.zeros((cap, 2)), np.zeros((cap, 2)), np.zeros((cap, 2))
+        secs = np.zeros(3)
+        N = (1 << lib().cfrb_num_actions(self._h)) - 1           # without building the full tree before the call's memory check
+        imm, sums = np.zeros((N, self.H)), np.zeros((N - 1, self.H))
+        full = None if full_compact is None else np.ascontiguousarray(full_compact, np.float64)
+        sg, it, cnt = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        n = _check(lib().cfrb_to_leaf_sampled_ev_regrets(self._h, seed, num_repeats, batch_repeats, cap, _p(cps, _ip), _p(br, _dp),
+                                                         _p(full, _dp), _p(ev, _dp), 1, regret_depth, _p(summ, _dp), _p(imm, _dp),
+                                                         _p(sums, _dp), C.byref(cnt), C.byref(sg), C.byref(it), _p(secs, _dp)))
+        r = {"checkpoints": cps[:n].tolist(), "br": br[:n].copy(), "subgames": sg.value, "subgame_iters": it.value,
+             "draw_seconds": float(secs[0]), "walk_seconds": float(secs[1]), "br_seconds": float(secs[2]),
+             "regret_summary": summ[:n].copy(), "immediate_regrets": imm, "regret_sums": sums, "regret_count": cnt.value}
+        if full is not None:
+            r["ev"] = ev[:n].copy()
+        return r
+
+    def ev2_compact(self, s1, s2):
+        """compute_ev2 of two compact full-tree strategies [N - 1, H]: (ev0, ev1)."""
+        a, b, out = np.ascontiguousarray(s1, np.float64), np.ascontiguousarray(s2, np.float64), np.zeros(2)
+        _check(lib().cfrb_ev2_compact(self._h, _p(a, _dp), _p(b, _dp), _p(out, _dp)))
+        return out
 
     def to_leaf_sampled_sums(self):
         """The last to_leaf_sampled's float32 accumulators: summed_strategy [N_full - 1, H] (row child - 1), summed_reach [N_full, H]."""

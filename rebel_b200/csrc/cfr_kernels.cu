@@ -13,6 +13,7 @@
 #include "expl_kernels.cuh"
 #include "expl_sampled_kernels.cuh"
 #include "full_game_kernels.cuh"
+#include "regret_grid_kernels.cuh"
 
 namespace cfrb {
 
@@ -218,6 +219,23 @@ void full_game_launch_iter(const FullGameDev& p, const int* level_begin, int lev
   for (int d = levels - 2; d >= 0; --d) fg_up_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
   for (int d = 0; d + 1 < levels; ++d) fg_down_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
   fg_advance_kernel<<<1, 1, 0, st>>>(p.iter);
+}
+// Grid-wide immediate regrets: the same level-by-level grid sizes as the full-game solver.
+template <typename S>
+static void regret_grid_launch_t(const RegretGridDev& p, const S* s, const int* level_begin, int levels, int max_blocks, cudaStream_t st) {
+  auto blocks = [&](int d) { return fg_blocks((long long)(level_begin[d + 1] - level_begin[d]) * p.H, max_blocks); };
+  for (int d = 1; d < levels; ++d) rg_reach_kernel<S><<<blocks(d), 256, 0, st>>>(p, s, level_begin[d], level_begin[d + 1], d);
+  rg_terminal_kernel<<<fg_blocks(p.T, max_blocks), 256, 0, st>>>(p);
+  for (int d = levels - 2; d >= 0; --d) rg_value_kernel<S><<<blocks(d), 256, 0, st>>>(p, s, level_begin[d], level_begin[d + 1], d);
+}
+void regret_grid_launch(const RegretGridDev& p, const float* s32, const double* s64, const int* level_begin, int levels, int max_blocks,
+                        cudaStream_t st) {
+  if (s32) regret_grid_launch_t(p, s32, level_begin, levels, max_blocks, st);
+  else regret_grid_launch_t(p, s64, level_begin, levels, max_blocks, st);
+}
+void regret_grid_launch_readout(const RegretGridDev& p, double count, double* immediate, double* node_sums, int max_blocks,
+                                cudaStream_t st) {
+  rg_readout_kernel<<<fg_blocks((long long)p.N * 32, max_blocks), 256, 0, st>>>(p, count, immediate, node_sums);
 }
 void full_game_launch_average(const FullGameDev& p, const int* depth, int untouched0, int untouched1, int max_blocks, cudaStream_t st) {
   fg_average_kernel<<<fg_blocks((long long)p.N * p.H, max_blocks), 256, 0, st>>>(p, depth, untouched0, untouched1);

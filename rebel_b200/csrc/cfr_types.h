@@ -287,6 +287,9 @@ struct ExplSampledDev {
   float* sum_s; float* sum_r;
   // repeat last_j of the batch (-1: none) writes its sampled strategy into last [N_full - 1][H]
   double* last; int last_j;
+  // with regrets tracked: every repeat j of the batch writes (float)s of its sampled strategy into rep_s + j * rep_stride,
+  // compact [N_full - 1][H] (nullptr: not tracked)
+  float* rep_s; size_t rep_stride;
   double* strategy;                   // the compact full-tree strategy the best response reads [N_full - 1][H]
 };
 // wave descriptors (template, player, act_iteration, root beliefs as `real`), row offsets and schedule of positions off .. off + n - 1
@@ -312,6 +315,21 @@ struct FullGameDev {
   double* avg;                    // [N - 1][H] the average strategy a checkpoint evaluates (BrDev::strategy)
   int* iter;                      // [1] iterations done; the traverser of iteration i is i & 1
 };
+// Immediate regrets of full-tree strategies over the whole GPU (regret_grid_kernels.cuh): the full tree's arrays, four [N][H]
+// tables in the handle's best-response scratch and the compact sums.
+struct RegretGridDev {
+  int N, T, H, F, A;
+  const int* parent; const int* child_begin; const int* nchild; const int* term_node; const int* act_lo;   // BrDev's arrays
+  const unsigned char* matches;   // [H][F]
+  double* reach0; double* reach1; double* val0; double* val1;   // [N][H] each
+  double* acc;                    // [N - 1][H] regret sums, entry (child - 1) * H + hand
+};
+// Adds one compact strategy [N - 1][H] (fp32 or fp64) to p.acc: about 2 launches per depth level and one for the terminals.
+void regret_grid_launch(const RegretGridDev& p, const float* s32, const double* s64, const int* level_begin, int levels, int max_blocks,
+                        cudaStream_t st);
+// immediate [N][H] and node_sums [N] (device pointers) of the sums of `count` strategies.
+void regret_grid_launch_readout(const RegretGridDev& p, double count, double* immediate, double* node_sums, int max_blocks,
+                                cudaStream_t st);
 // CFR constructor on the full tree (iteration counter left alone)
 void full_game_launch_init(const FullGameDev& p, const int* level_begin, int levels, int max_blocks, cudaStream_t st);
 // one iteration: about 2 (CFR) or 3 (FP) launches per depth level, then the counter's increment

@@ -1450,6 +1450,22 @@ int cfrb_ev2(cfrb_handle* h, const double* s1_dense, const double* s2_dense, dou
   return CFRB_OK;
 }
 
+int cfrb_ev2_compact(cfrb_handle* h, const double* s1, const double* s2, double* out2) {
+  if (!h || !s1 || !s2 || !out2) return fail(CFRB_EINVAL, "cfrb_ev2_compact: null argument");
+  CK(cudaSetDevice(h->cfg.device));
+  int rc = full_tree_setup(h, "cfrb_ev2_compact");
+  if (rc) return rc;
+  const size_t n = h->br.strategy.n * sizeof(double);
+  CK(cudaMemcpyAsync(h->br.strategy.p, s1, n, cudaMemcpyHostToDevice, h->own_stream));
+  CK(cudaMemcpyAsync(h->br.strategy2.p, s2, n, cudaMemcpyHostToDevice, h->own_stream));
+  cfrb::ev_launch(full_tree_dev(h), h->br.strategy.p, h->br.strategy2.p, h->own_stream);
+  ++h->launches;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out2, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  return CFRB_OK;
+}
+
 int cfrb_full_tree_nodes(cfrb_handle* h) {
   if (!h) return fail(CFRB_EINVAL, "null handle");
   CK(cudaSetDevice(h->cfg.device));
@@ -1881,9 +1897,89 @@ int64_t cfrb_to_leaf_sampled_bytes(int32_t num_dice, int32_t num_faces, int32_t 
   return s.tree_bytes + s.walk_bytes;
 }
 
+// The grid-wide regret pass over the handle's full tree: its four [N][H] tables are the first 4 N H doubles of the best-response
+// scratch (2 (3 N H + 10 T) doubles), which br_kernel and ev_kernel only use between passes on the same stream.
+static cfrb::RegretGridDev regret_grid_dev(cfrb_handle* h, double* acc) {
+  const auto& b = h->br;
+  const size_t NH = (size_t)b.t.N * h->g.H;
+  cfrb::RegretGridDev d{};
+  d.N = b.t.N; d.T = b.t.T; d.H = h->g.H; d.F = h->g.F; d.A = h->g.A;
+  d.parent = b.parent.p; d.child_begin = b.child_begin.p; d.nchild = b.nchild.p; d.term_node = b.term_node.p; d.act_lo = b.act_lo.p;
+  d.matches = h->d_matches.p;
+  d.reach0 = b.scratch.p; d.reach1 = d.reach0 + NH; d.val0 = d.reach1 + NH; d.val1 = d.val0 + NH;
+  d.acc = acc;
+  return d;
+}
+
+// Read-out of compact sums of `count` strategies (cfrb_regrets_fetch's max / count, then the per-node sums over hands), staged in
+// the best-response scratch: immediate [N][H] at its start, node_sums [N] behind it.  Any output may be NULL.  Synchronises.
+static int regret_grid_fetch(cfrb_handle* h, const DevBuf<double>& acc, int64_t count, double* immediate, double* sums, double* node_sums) {
+  const int N = h->br.t.N, H = h->g.H;
+  const size_t NH = (size_t)N * H;
+  cudaStream_t st = h->own_stream;
+  double* d_imm = h->br.scratch.p;
+  double* d_ns = d_imm + NH;
+  if (immediate || node_sums) {
+    cfrb::regret_grid_launch_readout(regret_grid_dev(h, acc.p), (double)count, d_imm, d_ns, 8 * h->num_sms, st);
+    CK(cudaGetLastError());
+  }
+  if (immediate) CK(cudaMemcpyAsync(immediate, d_imm, NH * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (node_sums) CK(cudaMemcpyAsync(node_sums, d_ns, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (sums) CK(cudaMemcpyAsync(sums, acc.p, acc.n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return CFRB_OK;
+}
+
+// Regret tracking of a sampled walk (cfrb_to_leaf_sampled_ev_regrets): where the outputs go; `on` false = not tracked.
+struct SampledRegretOut {
+  bool on = false;
+  int depth = 0;
+  double* summary = nullptr;    // [cap][2]
+  double* immediate = nullptr;  // [N][H], the last checkpoint's
+  double* sums = nullptr;       // [N - 1][H]
+  int64_t* count = nullptr;
+};
+static int64_t sampled_regret_bytes(const cfrb::GameShape& g, int B) {
+  const int64_t E = (((int64_t)1 << g.A) - 2) * g.H;
+  return E * 8 + (int64_t)B * E * 4;   // the compact fp64 sums and the batch's fp32 strategies
+}
+static int to_leaf_sampled_impl(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int32_t batch_repeats, int32_t cap, int32_t* checkpoints,
+                                double* br_out, const double* ev_full, bool ev_compact, double* ev_out, const SampledRegretOut& rg,
+                                int64_t* subgames, int64_t* subgame_iters, double* seconds3);
+
 int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int32_t batch_repeats, int32_t cap, int32_t* checkpoints,
                          double* br_out, const double* ev_full, double* ev_out, int64_t* subgames, int64_t* subgame_iters,
                          double* seconds3) {
+  return to_leaf_sampled_impl(h, seed0, num_repeats, batch_repeats, cap, checkpoints, br_out, ev_full, false, ev_out, SampledRegretOut(),
+                              subgames, subgame_iters, seconds3);
+}
+
+int64_t cfrb_to_leaf_sampled_regret_bytes(int32_t num_dice, int32_t num_faces, int32_t batch_repeats) {
+  if (num_dice < 1 || num_faces < 1 || batch_repeats < 1)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled_regret_bytes: num_dice, num_faces, batch_repeats must be >= 1");
+  const int64_t A = 2L * num_dice * num_faces + 1;
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled_regret_bytes: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                                 " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+  return sampled_regret_bytes(cfrb::GameShape(num_dice, num_faces), batch_repeats);
+}
+
+int cfrb_to_leaf_sampled_ev_regrets(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int32_t batch_repeats, int32_t cap,
+                                    int32_t* checkpoints, double* br_out, const double* ev_full_compact, double* ev_out,
+                                    int32_t track_regrets, int32_t regret_depth, double* regret_summary, double* immediate,
+                                    double* regret_sums, int64_t* regret_count, int64_t* subgames, int64_t* subgame_iters,
+                                    double* seconds3) {
+  if (track_regrets && !regret_summary) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: null argument");
+  SampledRegretOut rg;
+  rg.on = track_regrets != 0; rg.depth = regret_depth; rg.summary = regret_summary; rg.immediate = immediate; rg.sums = regret_sums;
+  rg.count = regret_count;
+  return to_leaf_sampled_impl(h, seed0, num_repeats, batch_repeats, cap, checkpoints, br_out, ev_full_compact, true, ev_out, rg,
+                              subgames, subgame_iters, seconds3);
+}
+
+static int to_leaf_sampled_impl(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int32_t batch_repeats, int32_t cap, int32_t* checkpoints,
+                                double* br_out, const double* ev_full, bool ev_compact, double* ev_out, const SampledRegretOut& rg,
+                                int64_t* subgames, int64_t* subgame_iters, double* seconds3) {
   if (!h || !checkpoints || !br_out || (ev_full && !ev_out)) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: null argument");
   const auto& g = h->g;
   if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
@@ -1911,7 +2007,8 @@ int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int
   const auto sz = sampled_sizes(g, md, K, batch_repeats);
   // refused before anything is allocated: on a shared device an allocation that fails late may starve other processes
   const int64_t ev_bytes = ev_full ? ((((int64_t)1 << g.A) - 2) * H) * 8 : 0;   // the compact ev_full
-  const int64_t need = (h->br.ready ? 0 : sz.tree_bytes) + sz.walk_bytes + ev_bytes;
+  const int64_t rg_bytes = rg.on ? sampled_regret_bytes(g, batch_repeats) : 0;   // the regret sums and the batch's strategies
+  const int64_t need = (h->br.ready ? 0 : sz.tree_bytes) + sz.walk_bytes + ev_bytes + rg_bytes;
   size_t free_b = 0, total_b = 0;
   CK(cudaMemGetInfo(&free_b, &total_b));
   int64_t avail = (int64_t)free_b;
@@ -1919,8 +2016,8 @@ int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int
   if (need > avail)
     return fail(CFRB_ENOMEM, "cfrb_to_leaf_sampled: needs " + std::to_string(need) + " bytes of device memory beyond the handle "
                              "(full tree and best-response scratch " + std::to_string(h->br.ready ? 0 : sz.tree_bytes) + ", walk " +
-                             std::to_string(sz.walk_bytes) + " at batch_repeats " + std::to_string(batch_repeats) + "), " +
-                             std::to_string(avail) + " free");
+                             std::to_string(sz.walk_bytes) + " at batch_repeats " + std::to_string(batch_repeats) +
+                             (rg.on ? ", regrets " + std::to_string(rg_bytes) : std::string()) + "), " + std::to_string(avail) + " free");
   int rc = full_tree_setup(h, "cfrb_to_leaf_sampled");
   if (rc) return rc;
   const int N = h->br.t.N;
@@ -1938,7 +2035,21 @@ int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int
   DevBuf<double> full;
   if (ev_full) {
     CK(full.alloc((size_t)(N - 1) * H));
-    if ((rc = upload_compact(h, ev_full, full.p))) return rc;
+    if (ev_compact) CK(cudaMemcpy(full.p, ev_full, full.n * sizeof(double), cudaMemcpyHostToDevice));
+    else if ((rc = upload_compact(h, ev_full, full.p))) return rc;
+  }
+  // regrets: compact fp64 sums, the batch's fp32 strategies, one CUDA graph of the grid pass per batch position
+  const size_t E = (size_t)(N - 1) * H;
+  DevBuf<double> racc;
+  DevBuf<float> rep;
+  std::vector<GraphExec> rgraphs;
+  std::vector<double> node_sums;
+  int64_t rcount = 0;
+  if (rg.on) {
+    CK(racc.alloc(E)); CK(rep.alloc((size_t)batch_repeats * E));
+    CK(cudaMemsetAsync(racc.p, 0, E * sizeof(double), st));
+    rgraphs.resize(batch_repeats);
+    node_sums.resize(N);
   }
   CK(cudaMemsetAsync(h->smp.sum_s.p, 0, (size_t)(N - 1) * H * sizeof(float), st));
   CK(cudaMemsetAsync(h->smp.sum_r.p, 0, (size_t)N * H * sizeof(float), st));
@@ -1953,6 +2064,7 @@ int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int
   d.draws = draws.p; d.draws_stride = R;
   d.fill = fill.p; d.cap = sz.level_cap; d.fid = fid.p; d.nmax = h->Nmax;
   d.sum_s = h->smp.sum_s.p; d.sum_r = h->smp.sum_r.p; d.last = h->br.strategy2.p; d.strategy = h->br.strategy.p;
+  d.rep_s = rg.on ? rep.p : nullptr; d.rep_stride = E;
   cfrb::SpDev scan{};   // sp_scan_kernel's view of the wave
   scan.A = g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
   scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
@@ -2036,6 +2148,23 @@ int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int
       n_level = next;
       cur ^= 1;
     }
+    if (rg.on) {   // the batch's sampled strategies into the regret sums in repeat order (RecursiveEvaluator::run)
+      const auto& t = h->br.t;
+      for (int j = 0; j < b; ++j) {
+        if (!rgraphs[j]) {
+          CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+          cfrb::regret_grid_launch(regret_grid_dev(h, racc.p), rep.p + (size_t)j * E, nullptr, t.level_begin.data(), t.levels,
+                                   8 * h->num_sms, st);
+          Graph graph;
+          const cudaError_t launched = cudaGetLastError();
+          CK(cudaStreamEndCapture(st, graph.put()));
+          CK(launched);
+          CK(cudaGraphInstantiate(rgraphs[j].put(), graph, 0));
+        }
+        CK(cudaGraphLaunch(rgraphs[j], st));
+      }
+      rcount += b;
+    }
     const auto t2 = std::chrono::steady_clock::now();
     done += b;
     if (done == cps[c]) {
@@ -2053,6 +2182,13 @@ int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int
         CK(cudaMemcpyAsync(ev_out + 2 * c, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
       }
       CK(cudaStreamSynchronize(st));
+      if (rg.on) {   // report_regrets' summary: the per-node sums over hands added in node order, depth < regret_depth or not
+        if ((rc = regret_grid_fetch(h, racc, rcount, done == num_repeats ? rg.immediate : nullptr, nullptr, node_sums.data()))) return rc;
+        double top = 0, rest = 0;
+        for (int n = 0; n < N; ++n) (h->br.t.depth[n] < rg.depth ? top : rest) += node_sums[n];
+        rg.summary[2 * c] = top;
+        rg.summary[2 * c + 1] = rest;
+      }
       checkpoints[c++] = done;
     }
     const auto t3 = std::chrono::steady_clock::now();
@@ -2061,6 +2197,10 @@ int cfrb_to_leaf_sampled(cfrb_handle* h, int32_t seed0, int32_t num_repeats, int
     secs[2] += std::chrono::duration<double>(t3 - t2).count();
   }
   h->smp.ready = true;
+  if (rg.on) {
+    if (rg.sums) CK(cudaMemcpy(rg.sums, racc.p, E * sizeof(double), cudaMemcpyDeviceToHost));
+    if (rg.count) *rg.count = rcount;
+  }
   if (subgames) *subgames = solved;
   if (subgame_iters) *subgame_iters = iters_sum;
   if (seconds3) std::copy(secs, secs + 3, seconds3);
@@ -2099,6 +2239,11 @@ struct cfrb_full_game {
   cfrb::FullGameDev dev{};
   GraphExec graph;
   int64_t total_bytes = 0, handle_bytes = 0;
+  // cfrb_full_game_track_regrets: the compact regret sums of the sampling strategies of the even iterations, their count and the
+  // CUDA graph of one strategy's pass
+  DevBuf<double> acc;
+  int64_t regret_count = 0;
+  GraphExec regret_graph;
   ~cfrb_full_game() {
     if (h) cfrb_destroy(h);   // synchronises its stream, on which every kernel of the object ran
   }
@@ -2195,6 +2340,50 @@ int cfrb_full_game_destroy(cfrb_full_game* g) {
   return CFRB_OK;
 }
 
+static int64_t full_game_regret_bytes(const cfrb::GameShape& g) {
+  return ((((int64_t)1 << g.A) - 2) * g.H) * 8;
+}
+
+int64_t cfrb_full_game_regret_bytes(int32_t num_dice, int32_t num_faces) {
+  if (num_dice < 1 || num_faces < 1) return fail(CFRB_EINVAL, "cfrb_full_game_regret_bytes: num_dice, num_faces must be >= 1");
+  const int64_t A = 2L * num_dice * num_faces + 1;
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, "cfrb_full_game_regret_bytes: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                                 " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+  return full_game_regret_bytes(cfrb::GameShape(num_dice, num_faces));
+}
+
+int cfrb_full_game_track_regrets(cfrb_full_game* g) {
+  if (!g) return fail(CFRB_EINVAL, "null full game");
+  if (g->fp) return fail(CFRB_EINVAL, "cfrb_full_game_track_regrets: immediate regrets are tracked for CFR only");
+  if (g->acc.p) return CFRB_OK;
+  if (g->iters > 0)
+    return fail(CFRB_ESTATE, "cfrb_full_game_track_regrets: the solver has already run " + std::to_string(g->iters) + " iterations");
+  cfrb_handle* h = g->h;
+  CK(cudaSetDevice(h->cfg.device));
+  // refused before anything is allocated, as cfrb_full_game_create is
+  const int64_t need = full_game_regret_bytes(h->g);
+  size_t free0 = 0, total = 0;
+  CK(cudaMemGetInfo(&free0, &total));
+  const int64_t avail = g_full_game_free_cap > 0 ? std::min<int64_t>((int64_t)free0, g_full_game_free_cap) : (int64_t)free0;
+  if (need > avail)
+    return fail(CFRB_ENOMEM, "cfrb_full_game_track_regrets: needs " + std::to_string(need) + " bytes of device memory, " +
+                                 std::to_string(avail) + " free");
+  CK(g->acc.alloc((size_t)(h->br.t.N - 1) * h->g.H));
+  CK(cudaMemsetAsync(g->acc.p, 0, g->acc.n * sizeof(double), h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  g->regret_count = 0;
+  return CFRB_OK;
+}
+
+int cfrb_full_game_regrets(cfrb_full_game* g, double* immediate, double* sums, double* node_sums, int64_t* count) {
+  if (!g) return fail(CFRB_EINVAL, "null full game");
+  if (!g->acc.p) return fail(CFRB_ESTATE, "cfrb_full_game_regrets: cfrb_full_game_track_regrets has not been called");
+  CK(cudaSetDevice(g->h->cfg.device));
+  if (count) *count = g->regret_count;
+  return regret_grid_fetch(g->h, g->acc, g->regret_count, immediate, sums, node_sums);
+}
+
 int cfrb_full_game_step(cfrb_full_game* g, int32_t iters) {
   if (!g || iters < 0) return fail(CFRB_EINVAL, "cfrb_full_game_step: bad argument");
   if (iters == 0) return CFRB_OK;
@@ -2211,7 +2400,23 @@ int cfrb_full_game_step(cfrb_full_game* g, int32_t iters) {
     CK(launched);
     CK(cudaGraphInstantiate(g->graph.put(), graph, 0));
   }
-  for (int i = 0; i < iters; ++i) CK(cudaGraphLaunch(g->graph, st));
+  if (g->acc.p && !g->regret_graph) {   // one strategy's regret pass, reading Sg in place
+    CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    cfrb::regret_grid_launch(regret_grid_dev(h, g->acc.p), nullptr, g->Sg.p, t.level_begin.data(), t.levels, 8 * h->num_sms, st);
+    Graph graph;
+    const cudaError_t launched = cudaGetLastError();
+    CK(cudaStreamEndCapture(st, graph.put()));
+    CK(launched);
+    CK(cudaGraphInstantiate(g->regret_graph.put(), graph, 0));
+  }
+  for (int i = 0; i < iters; ++i) {
+    CK(cudaGraphLaunch(g->graph, st));
+    // the sampling strategy after every iteration with an even index (solve_full_tree's iter % 2 == 0 rule)
+    if (g->acc.p && (g->iters + i) % 2 == 0) {
+      CK(cudaGraphLaunch(g->regret_graph, st));
+      ++g->regret_count;
+    }
+  }
   CK(cudaStreamSynchronize(st));
   g->iters += iters;
   return CFRB_OK;

@@ -100,6 +100,7 @@ __global__ void __launch_bounds__(128) expl_sampled_expand_kernel(ExplSampledDev
         const size_t e = (size_t)(fcb + jj - 1) * H + hd;
         p.sum_s[e] += (float)s * (float)r;
         if (j == p.last_j) p.last[e] = s;
+        if (p.rep_s) p.rep_s[(size_t)j * p.rep_stride + e] = (float)s;   // the repeat's strategy as recursive_eval's float32 tensor
       }
     }
     // beliefs and reach of the pseudo-leaves, one thread per (leaf, player row)

@@ -495,6 +495,18 @@ struct FullTreeHandle {
   }
 };
 
+// compute_ev2 of two compact full-tree strategies [N - 1, H] (solve_full_game's form) on the GPU: (ev0, ev1).
+std::tuple<double, double> ev_of_compact_strategies(int num_dice, int num_faces, torch::Tensor s1, torch::Tensor s2) {
+  FullTreeHandle f(num_dice, num_faces);
+  auto a = s1.to(torch::kCPU, torch::kFloat64).contiguous(), b = s2.to(torch::kCPU, torch::kFloat64).contiguous();
+  for (auto* t : {&a, &b})
+    if (t->dim() != 2 || t->size(0) != f.N - 1 || t->size(1) != f.H)
+      throw std::runtime_error("ev_of_compact_strategies: strategy must be [num_full_tree_nodes - 1, H]");
+  std::array<double, 2> e{};
+  check(cfrb_ev2_compact(f.h.get(), a.data_ptr<double>(), b.data_ptr<double>(), e.data()), "cfrb_ev2_compact");
+  return std::make_tuple(e[0], e[1]);
+}
+
 // compute_ev2 (subgame_solving.cc:975-982) of two dense full-tree strategies on the GPU: (ev0, ev1).
 std::tuple<double, double> ev_of_strategies(int num_dice, int num_faces, torch::Tensor s1, torch::Tensor s2) {
   FullTreeHandle f(num_dice, num_faces);
@@ -581,7 +593,18 @@ py::dict solve_full_tree(RecursiveSolvingParams cfg, int device, bool track_regr
 // solve_full_tree's solve on the whole GPU (cfrb_full_game_*): the same checkpoints, exploitabilities and printed lines, bit for
 // bit, and the final average strategy in compact form [N - 1, H] (entry (child - 1) * H + hand), so that games of up to 23
 // actions fit.  Times: the iterations and the best responses, host wall time around calls that synchronise.
-py::dict solve_full_game(RecursiveSolvingParams cfg, int device) {
+// Nodes of the full tree above `depth` (the first level_begin[depth] in BFS order): the root, its A - 1 bids (the root cannot call)
+// and C(A, d) strictly increasing action sequences of every length d >= 2.
+int64_t full_tree_nodes_above(int A, int depth) {
+  int64_t n = 0, c = 1;   // c = C(A, d)
+  for (int d = 0; d < depth && d <= A; ++d) {
+    n += d == 0 ? 1 : (d == 1 ? A - 1 : c);
+    c = c * (A - d) / (d + 1);
+  }
+  return n;
+}
+
+py::dict solve_full_game(RecursiveSolvingParams cfg, int device, bool track_regrets, int regret_depth) {
   const int A = 2 * cfg.num_dice * cfg.num_faces + 1;
   if (A > CFRB_TO_LEAF_MAX_ACTIONS)   // the library's own refusal, before a device is touched
     throw std::runtime_error("solve_full_game: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
@@ -594,6 +617,10 @@ py::dict solve_full_game(RecursiveSolvingParams cfg, int device) {
   for (int i = 0; i < cfg.num_dice; ++i) H *= cfg.num_faces;
   double solve_s = 0, br_s = 0, total_s = 0;
   const int iters = cfg.subgame_params.num_iters;
+  track_regrets = track_regrets && cfg.subgame_params.use_cfr;   // the reference tracks them for CFR only
+  std::vector<double> immediate, sums, node_sums;
+  int64_t regret_count = 0;
+  std::array<double, 2> summary{};
   {
     py::gil_scoped_release nogil;
     const auto t0 = std::chrono::steady_clock::now();
@@ -603,6 +630,7 @@ py::dict solve_full_game(RecursiveSolvingParams cfg, int device) {
     check(cfrb_full_game_create(&c, &raw), "cfrb_full_game_create");
     const FullGamePtr fg(raw);
     N = check(cfrb_full_game_nodes(fg.get()), "cfrb_full_game_nodes");
+    if (track_regrets) check(cfrb_full_game_track_regrets(fg.get()), "cfrb_full_game_track_regrets");
     check(cfrb_full_game_memory(fg.get(), &total_bytes, &handle_bytes), "cfrb_full_game_memory");
     int done = 0;
     for (int iter = 0; iter < iters; ++iter) {
@@ -623,6 +651,13 @@ py::dict solve_full_game(RecursiveSolvingParams cfg, int device) {
     }
     strategy.resize((size_t)(N - 1) * H);
     check(cfrb_full_game_strategy(fg.get(), strategy.data()), "cfrb_full_game_strategy");
+    if (track_regrets) {
+      immediate.resize((size_t)N * H); sums.resize((size_t)(N - 1) * H); node_sums.resize(N);
+      check(cfrb_full_game_regrets(fg.get(), immediate.data(), sums.data(), node_sums.data(), &regret_count), "cfrb_full_game_regrets");
+      // report_regrets' summary: the per-node sums over hands, added in node order (recursive_eval.h regret_summary)
+      const int64_t above = full_tree_nodes_above(2 * cfg.num_dice * cfg.num_faces + 1, regret_depth);
+      for (int64_t n = 0; n < N; ++n) summary[n < above ? 0 : 1] += node_sums[n];
+    }
     total_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   }
   py::dict d;
@@ -632,6 +667,12 @@ py::dict solve_full_game(RecursiveSolvingParams cfg, int device) {
   d["num_nodes"] = N;
   d["seconds"] = total_s; d["solve_seconds"] = solve_s; d["br_seconds"] = br_s;
   d["device_bytes"] = total_bytes; d["handle_bytes"] = handle_bytes;
+  if (track_regrets) {
+    d["immediate_regrets"] = f64_tensor(immediate, {(int64_t)N, H});
+    d["regret_sums_compact"] = f64_tensor(sums, {(int64_t)N - 1, H});
+    d["regret_count"] = regret_count;
+    d["regret_summary"] = py::make_tuple(summary[0], summary[1]);
+  }
   return d;
 }
 
@@ -756,7 +797,7 @@ int default_batch_repeats(int A, int max_depth, int wave_capacity) {
   return (int)std::max<int64_t>(1, std::min<int64_t>(64, std::max(1, wave_capacity) / level));
 }
 py::dict recursive_eval_to_leaf(const RecursiveSolvingParams& cfg, int device, int num_repeats, int seed0, py::object flat_weights,
-                                int wave_capacity, int batch_repeats, bool return_sums, py::object full_strategy) {
+                                int wave_capacity, int batch_repeats, bool return_sums, py::object full_strategy, bool track_regrets) {
   const int A = 2 * cfg.num_dice * cfg.num_faces + 1;
   if (A > CFRB_TO_LEAF_MAX_ACTIONS)   // the library's own refusal, before a device is touched
     throw std::runtime_error("recursive_eval_to_leaf: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
@@ -766,14 +807,20 @@ py::dict recursive_eval_to_leaf(const RecursiveSolvingParams& cfg, int device, i
   const int B = batch_repeats > 0 ? batch_repeats : default_batch_repeats(A, cfg.subgame_params.max_depth, K);
   const std::vector<float> w = flat_of(flat_weights);
   std::vector<double> full;
+  bool compact = false;   // full_strategy dense [N, H, A] or compact [N - 1, H], by shape
+  const int64_t Hg = (int64_t)std::pow(cfg.num_faces, cfg.num_dice), Ng = ((int64_t)1 << A) - 1;
   if (!full_strategy.is_none()) {
     auto t = full_strategy.cast<torch::Tensor>().to(torch::kCPU, torch::kFloat64).contiguous();
-    const int64_t want = (((int64_t)1 << A) - 1) * (int64_t)std::pow(cfg.num_faces, cfg.num_dice) * A;
-    if (t.numel() != want) throw std::runtime_error("recursive_eval_to_leaf: full_strategy must be [N_full][H][A]");
+    compact = t.dim() == 2 && t.size(0) == Ng - 1 && t.size(1) == Hg;
+    if (!compact && !(t.dim() == 3 && t.size(0) == Ng && t.size(1) == Hg && t.size(2) == A))
+      throw std::runtime_error("recursive_eval_to_leaf: full_strategy must be [N_full][H][A] or compact [N_full - 1][H]");
     full.assign(t.data_ptr<double>(), t.data_ptr<double>() + t.numel());
   }
+  track_regrets = track_regrets && cfg.subgame_params.use_cfr;   // the reference tracks them for CFR only
   std::vector<int> cps(64);
-  std::vector<double> br(128), ev(128);
+  std::vector<double> br(128), ev(128), summary(128), immediate, rsums;
+  int64_t rcount = 0;
+  if (track_regrets) { immediate.resize((size_t)Ng * Hg); rsums.resize((size_t)(Ng - 1) * Hg); }
   std::vector<float> ss, sr;
   double secs[3] = {0, 0, 0}, total = 0;
   int64_t subgames = 0, iters = 0;
@@ -783,9 +830,18 @@ py::dict recursive_eval_to_leaf(const RecursiveSolvingParams& cfg, int device, i
     const auto t0 = std::chrono::steady_clock::now();
     const HandlePtr h = open_handle(liars_dice::solver_config(cfg, device, K));
     if (!w.empty()) check(cfrb_set_weights(h.get(), w.data(), w.size(), 1), "cfrb_set_weights");
-    C = check(cfrb_to_leaf_sampled(h.get(), seed0, num_repeats, B, (int)cps.size(), cps.data(), br.data(),
-                                   full.empty() ? nullptr : full.data(), ev.data(), &subgames, &iters, secs),
-              "cfrb_to_leaf_sampled");
+    if (compact || track_regrets)
+      C = check(cfrb_to_leaf_sampled_ev_regrets(h.get(), seed0, num_repeats, B, (int)cps.size(), cps.data(), br.data(),
+                                                compact ? full.data() : nullptr, ev.data(), track_regrets, cfg.subgame_params.max_depth,
+                                                summary.data(), track_regrets ? immediate.data() : nullptr,
+                                                track_regrets ? rsums.data() : nullptr, &rcount, &subgames, &iters, secs),
+                "cfrb_to_leaf_sampled_ev_regrets");
+    if (!compact && track_regrets && !full.empty())
+      throw std::runtime_error("recursive_eval_to_leaf: track_regrets takes a compact full_strategy [N_full - 1][H]");
+    if (!compact && !track_regrets)
+      C = check(cfrb_to_leaf_sampled(h.get(), seed0, num_repeats, B, (int)cps.size(), cps.data(), br.data(),
+                                     full.empty() ? nullptr : full.data(), ev.data(), &subgames, &iters, secs),
+                "cfrb_to_leaf_sampled");
     N = cfrb_full_tree_nodes(h.get());
     H = cfrb_num_hands(h.get());
     if (return_sums) {
@@ -803,6 +859,14 @@ py::dict recursive_eval_to_leaf(const RecursiveSolvingParams& cfg, int device, i
   d["num_nodes"] = N; d["subgames"] = subgames; d["subgame_iters"] = iters; d["batch_repeats"] = B;
   d["seconds"] = total; d["draw_seconds"] = secs[0]; d["walk_seconds"] = secs[1]; d["br_seconds"] = secs[2];
   if (!full.empty()) d["ev_of_full"] = pairs_tensor(evs);
+  if (track_regrets) {
+    std::vector<std::array<double, 2>> rs(C);
+    for (int c = 0; c < C; ++c) rs[c] = {summary[2 * c], summary[2 * c + 1]};
+    d["regret_summary"] = pairs_tensor(rs);
+    d["immediate_regrets"] = f64_tensor(immediate, {Ng, Hg});
+    d["regret_sums_compact"] = f64_tensor(rsums, {Ng - 1, Hg});
+    d["regret_count"] = rcount;
+  }
   if (return_sums) {
     auto tss = torch::empty({(int64_t)N - 1, (int64_t)H}), tsr = torch::empty({(int64_t)N, (int64_t)H});
     std::copy(ss.begin(), ss.end(), tss.data_ptr<float>());
@@ -1014,6 +1078,8 @@ PYBIND11_MODULE(rela, m) {
         "regret_count.");
   m.def("ev_of_strategies", &ev_of_strategies, py::arg("num_dice"), py::arg("num_faces"), py::arg("s1"), py::arg("s2"),
         "rebel_b200 extension: compute_ev2 of two dense full-tree strategies (GPU kernel): (ev0, ev1).");
+  m.def("ev_of_compact_strategies", &ev_of_compact_strategies, py::arg("num_dice"), py::arg("num_faces"), py::arg("s1"), py::arg("s2"),
+        "rebel_b200 extension: compute_ev2(s1, s2) of two compact full-tree strategies [N - 1, H] on the GPU: (ev0, ev1).");
   m.def("immediate_regrets", &immediate_regrets, py::arg("num_dice"), py::arg("num_faces"), py::arg("strategies"),
         py::arg("batch") = 64,
         "rebel_b200 extension: compute_immediate_regrets of dense full-tree strategies [S, N, H, A] read as float32 (GPU "
@@ -1022,11 +1088,15 @@ PYBIND11_MODULE(rela, m) {
         "rebel_b200 extension: recursive_eval's full-tree solve — dict with checkpoints, exploitability [C, 2], the final "
         "get_strategy() [N, H, A] and, with track_regrets (CFR), the immediate regrets of the sampling strategies of the "
         "even iterations (immediate_regrets, regret_sums, regret_count).");
-  m.def("solve_full_game", &solve_full_game, py::arg("cfg"), py::arg("device") = 0,
+  m.def("solve_full_game", &solve_full_game, py::arg("cfg"), py::arg("device") = 0, py::arg("track_regrets") = false,
+        py::arg("regret_depth") = 2,
         "rebel_b200 extension: solve_full_tree's solve with the tree spread over the whole GPU, for games of up to 23 actions — "
         "dict with checkpoints, exploitability [C, 2] (the same bits), the final average strategy in compact form [N - 1, H] "
         "(entry (child - 1) * H + hand), num_nodes, seconds, solve_seconds, br_seconds, device_bytes and handle_bytes (device "
-        "memory the solver took, and the part its handle took).");
+        "memory the solver took, and the part its handle took).  track_regrets (CFR only; ignored for FP) adds the immediate "
+        "regrets of the sampling strategies of the even iterations, solve_full_tree's bits: immediate_regrets [N, H], "
+        "regret_sums_compact [N - 1, H], regret_count and regret_summary (top, rest), the summed immediate regrets of the nodes "
+        "above regret_depth and of the rest (report_regrets' summary).");
   m.def("play_match", &play_match_py, py::arg("cfg_a"), py::arg("cfg_b"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
         py::arg("policy") = "sampled", py::arg("flat_weights_a") = py::none(), py::arg("flat_weights_b") = py::none(),
         py::arg("concurrent_games") = 8192,
@@ -1050,14 +1120,17 @@ PYBIND11_MODULE(rela, m) {
         "subgame_iters, seconds, walk_seconds, br_seconds.");
   m.def("recursive_eval_to_leaf", &recursive_eval_to_leaf, py::arg("cfg"), py::arg("device") = 0, py::arg("num_repeats") = 1,
         py::arg("seed") = 0, py::arg("flat_weights") = py::none(), py::arg("wave_capacity") = 16384, py::arg("batch_repeats") = 0,
-        py::arg("return_sums") = false, py::arg("full_strategy") = py::none(),
+        py::arg("return_sums") = false, py::arg("full_strategy") = py::none(), py::arg("track_regrets") = false,
         "rebel_b200 extension: recursive_eval_sampled's evaluation (the float32 reach-weighted average of num_repeats sampled "
         "recursive strategies, strategy ids seed .. seed + num_repeats - 1, and its exploitability at every power of two and at "
         "num_repeats) with the subgames walked level by level on the device and the best responses taken there, without dense "
         "sums (games with at most 23 actions whose need fits the free device memory).  batch_repeats repeats are walked together "
         "(<= 0: enough to fill a wave, at most 64).  dict: checkpoints, exploitability [C, 2], num_nodes, subgames, subgame_iters, "
         "batch_repeats, seconds, draw_seconds, walk_seconds, br_seconds; return_sums adds the compact summed_strategy [N - 1, H] "
-        "(row child - 1) and summed_reach [N, H]; full_strategy (dense [N, H, A]) adds ev_of_full [C, 2] (compute_ev2 against it).");
+        "(row child - 1) and summed_reach [N, H]; full_strategy (dense [N, H, A], or compact [N - 1, H] by shape) adds ev_of_full "
+        "[C, 2] (compute_ev2 against it); track_regrets (CFR only; with a compact or no full_strategy) adds the immediate regrets "
+        "of the sampled strategies, recursive_eval_sampled's bits: regret_summary [C, 2] (depth < max_depth, rest), "
+        "immediate_regrets [N, H], regret_sums_compact [N - 1, H] and regret_count.");
   m.def("match_stats", &match_stats_py, py::arg("payoff_a"),
         "rebel_b200 extension: play_match's mean, stderr (over the pairs 2i, 2i+1) and seat_means of a payoff vector.");
   py::class_<Agent, std::shared_ptr<Agent>>(

@@ -9,7 +9,8 @@ strategy against the full-tree solve, the immediate regrets (--print_regret / --
 
 --device_walk walks the repeats' subgames level by level on the device (rela.recursive_eval_to_leaf) with the same numbers, and is
 taken on its own for games whose full tree has more than 2^20 nodes (2x5f, 5x2f, 1x10f, 1x11f), where the full-tree solve, the
-EVs against it and the regret reports are not available.
+EVs against it and the regret reports are not available.  --full_game (implies --device_walk) solves the full game over the whole
+GPU (rela.solve_full_game) instead, so those games get the full-tree solve, EV of full, YYY and --print_regret* too.
 
 Flags follow the reference binary (`--num_dice --num_faces --subgame_iters --mdp_depth --num_repeats --net --cfr --no_linear
 --optimistic --dcfr --num_threads --print_regret --print_regret_summary`).  One process per GPU: rank r solves the contiguous
@@ -79,11 +80,18 @@ def regret_summary(depths, immediate, mdp_depth):
 
 def regret_lines(immediate, depths, mdp_depth, print_regret, print_regret_summary):
     """The text report_regrets prints (recursive_eval.cc:33-52), numbers like std::cout in fixed mode (%f)."""
+    summary = regret_summary(depths, immediate, mdp_depth) if print_regret_summary else None
+    return regret_text(immediate[:min(20, len(depths))], summary, mdp_depth, print_regret, print_regret_summary)
+
+
+def regret_text(first_rows, summary, mdp_depth, print_regret, print_regret_summary):
+    """regret_lines' text from the immediate regrets of the first (up to 20) nodes and the (top, rest) summary, which the device
+    computes on games too large for a host loop over every node."""
     out = ""
     if print_regret:
-        out += "\tRegrets: " + "".join("".join(f"{v:f} " for v in immediate[n].tolist()) + "| " for n in range(min(20, len(depths)))) + "\n"
+        out += "\tRegrets: " + "".join("".join(f"{v:f} " for v in first_rows[n].tolist()) + "| " for n in range(len(first_rows))) + "\n"
     if print_regret_summary:
-        top, bottom = regret_summary(depths, immediate, mdp_depth)
+        top, bottom = summary
         out += f"\tRegrets (depth<={mdp_depth})/rest: {top:f}/{bottom:f}"
     return out
 
@@ -131,6 +139,9 @@ def build_parser():
     ap.add_argument("--wave_capacity", type=int, default=8192)
     ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast fp32-tanh GELU (default with --net)")
     ap.add_argument("--random_net_seed", type=int, default=None, help="use a random-init Net2 (benchmarks)")
+    ap.add_argument("--full_game", action="store_true",
+                    help="solve the full game over the whole GPU (rela.solve_full_game) and walk the repeats on the device (implies "
+                         "--device_walk), with EV of full, YYY and --print_regret* on games of up to 23 actions")
     ap.add_argument("--device_walk", action="store_true",
                     help="walk the repeats' subgames level by level on the device and take the best responses there, without dense "
                          "[N, H, A] sums (the same numbers; always on for games whose full tree has more than 2^20 nodes)")
@@ -138,6 +149,7 @@ def build_parser():
 
 
 DENSE_MAX_NODES = 1 << 20   # the host walk's dense [N, H, A] sums and the full-tree solve stop here (RecursiveEvaluator)
+FULL_GAME_MAX_ACTIONS = 23  # the full-game solver and the device walk (CFRB_TO_LEAF_MAX_ACTIONS)
 
 
 def device_walk_plan(args, world):
@@ -145,19 +157,24 @@ def device_walk_plan(args, world):
     before any device work."""
     A = 2 * args.num_dice * args.num_faces + 1
     large = (1 << A) - 1 > DENSE_MAX_NODES
-    walk = args.device_walk or large
-    if walk and (args.print_regret or args.print_regret_summary):
+    if args.full_game and args.no_full_tree:
+        raise SystemExit("recursive_eval: --full_game solves the full game; it does not go with --no_full_tree")
+    if args.full_game and A > FULL_GAME_MAX_ACTIONS:
+        raise SystemExit(f"recursive_eval: --full_game supports games of up to {FULL_GAME_MAX_ACTIONS} actions "
+                         f"(A = {A} at {args.num_dice}x{args.num_faces}f)")
+    walk = args.device_walk or large or args.full_game
+    if walk and not args.full_game and (args.print_regret or args.print_regret_summary):
         n = (1 << A) - 1
         raise SystemExit(f"recursive_eval: --print_regret / --print_regret_summary need the dense regret sums [N, H, A] of the "
                          f"host walk ({n * args.num_faces ** args.num_dice * A * 8 / 1e9:.1f} GB at "
                          f"{args.num_dice}x{args.num_faces}f); the device walk (--device_walk, or a game whose full tree has more "
-                         f"than 2^20 nodes) does not track regrets")
+                         f"than 2^20 nodes) does not track regrets; --full_game does")
     if walk and world > 1:
         raise SystemExit("recursive_eval: the device walk runs on one GPU (WORLD_SIZE must be 1)")
     skip = None
     if args.no_full_tree:
         skip = "--no_full_tree"
-    elif large:
+    elif large and not args.full_game:
         skip = f"the full tree has {(1 << A) - 1} nodes, more than 2^20"
     return walk, skip
 
@@ -192,10 +209,23 @@ def main(argv=None):
     if args.dcfr is not None:
         sp.dcfr, (sp.dcfr_alpha, sp.dcfr_beta, sp.dcfr_gamma) = True, args.dcfr
 
-    depths = full_tree_depths(args.num_dice, args.num_faces) if want_regrets else None
+    depths = full_tree_depths(args.num_dice, args.num_faces) if want_regrets and not args.full_game else None
     report = []        # (name, dense strategy, (expl0, expl1), (ev0, ev1) or None) of recursive_eval.cc:394-408
     full = None
-    if rank == 0 and skip_full is None:
+    if rank == 0 and args.full_game:
+        # the same solve over the whole GPU, its strategy compact [N - 1, H]; its object is freed before the walk starts
+        sp.max_depth = 100000
+        f = rela.solve_full_game(cfg, local, track_regrets=want_regrets, regret_depth=args.mdp_depth)
+        sp.max_depth = args.mdp_depth
+        full = f["strategy"]
+        e = f["exploitability"][-1].tolist()
+        total = float(np.float32(e[0] + e[1]))
+        print(f"Full {'CFR' if args.cfr else 'FP'} exploitability: {total / 2:.6e}", flush=True)
+        if want_regrets:
+            print(regret_text(f["immediate_regrets"][:20], f["regret_summary"], args.mdp_depth, args.print_regret,
+                              args.print_regret_summary), flush=True)
+        report.append(("full_tree", None, tuple(e), rela.ev_of_compact_strategies(args.num_dice, args.num_faces, full, full)))
+    elif rank == 0 and skip_full is None:
         # "Solving the game for the full tree" (recursive_eval.cc:264-309): exploitability curve at powers of two
         sp.max_depth = 100000
         f = rela.solve_full_tree(cfg, local, track_regrets=want_regrets)
@@ -211,15 +241,24 @@ def main(argv=None):
         print(f"no full-tree solve ({skip_full}): the full_tree entry and the EVs against it are not reported", flush=True)
     if args.num_repeats > 0 and args.mdp_depth > 0 and walk:
         t0 = time.time()
+        walk_regrets = want_regrets and args.full_game
         r = rela.recursive_eval_to_leaf(cfg, local, args.num_repeats, seed=0, flat_weights=weights, wave_capacity=args.wave_capacity,
-                                        batch_repeats=args.batch_repeats or 0, full_strategy=full)
+                                        batch_repeats=args.batch_repeats or 0, full_strategy=full, track_regrets=walk_regrets)
         wall = time.time() - t0
         for i, (n, x) in enumerate(zip(r["checkpoints"], r["exploitability"].tolist())):
             print(f"{n:5d}: {(x[0] + x[1]) / 2:.6e} ({x[0]:.6e},{x[1]:.6e})")
+            extra = ""
             if full is not None:
                 ev = r["ev_of_full"][i].tolist()
-                print(f"\tEV of full: {(ev[0] + ev[1]) / 2:f} ({ev[0]:f},{ev[1]:f})")
+                extra += f"\tEV of full: {(ev[0] + ev[1]) / 2:f} ({ev[0]:f},{ev[1]:f})"
+            if walk_regrets and args.print_regret_summary:
+                top, bottom = r["regret_summary"][i].tolist()
+                extra += f"\tRegrets (depth<={args.mdp_depth})/rest: {top:f}/{bottom:f}"
+            if extra:
+                print(extra)
             report.append((f"repeated toleaf {n}", None, tuple(x), tuple(r["ev_of_full"][i].tolist()) if full is not None else None))
+        if walk_regrets and args.print_regret:
+            print(regret_text(r["immediate_regrets"][:20], None, args.mdp_depth, True, False), end="")
         e = r["exploitability"][-1].tolist()
         print(json.dumps({"game": f"{args.num_dice}x{args.num_faces}f", "num_repeats": args.num_repeats, "subgame_iters": args.subgame_iters,
                           "n_gpus": world, "net_mode": net_mode, "exploitability": (e[0] + e[1]) / 2, "exploitability_p0_p1": list(e),
