@@ -24,12 +24,14 @@ constexpr int kMlpRows = 32;   // rows per CTA
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
 // One dense layer for a 32-row tile: thread j owns output feature j for all rows.
-// xs: [K][32] (k-major), wt: [K][HID] global.  Result left in acc[].
+// xs: [K][32] (k-major), wt: [K][HID] global.  Result left in acc[].  The bias is added after the dot product, as libtorch's
+// addmm does: started from a large bias (a common offset of every feature, which LayerNorm removes) the sum would be rounded at
+// the bias's ulp K times.
 template <int HID>
 __device__ __forceinline__ void dense_tile(const float* __restrict__ xs, const float* __restrict__ wt, int K, float bias,
                                            float (&acc)[kMlpRows], int j) {
 #pragma unroll
-  for (int r = 0; r < kMlpRows; ++r) acc[r] = bias;
+  for (int r = 0; r < kMlpRows; ++r) acc[r] = 0.f;
   for (int k = 0; k < K; ++k) {
     const float w = __ldg(wt + (size_t)k * HID + j);
     const float4* xv = reinterpret_cast<const float4*>(xs + k * kMlpRows);
@@ -39,6 +41,8 @@ __device__ __forceinline__ void dense_tile(const float* __restrict__ xs, const f
       acc[4 * i + 0] += x.x * w; acc[4 * i + 1] += x.y * w; acc[4 * i + 2] += x.z * w; acc[4 * i + 3] += x.w * w;
     }
   }
+#pragma unroll
+  for (int r = 0; r < kMlpRows; ++r) acc[r] += bias;
 }
 
 // LayerNorm(eps 1e-5, biased variance, affine) + GELU over ys[r][0..HID) for the 32 rows; writes xs[j][r].

@@ -5,7 +5,8 @@ is +-0 for such a leaf whatever the net returns, so nothing the solver computes 
 CPU: the bound against the net on random rows, and a weight that is not finite turns it off.
 GPU: every table, root value mean, leaf row, self-play example and match / local-best-response result byte for byte against the
 same run with every row evaluated, on a resident-kernel game (1x6f, 2x3f) and a wide-kernel game (2x5f), in both tensor-core
-modes, with fp64 and fp32 tables, and on a capped persistent grid whose warps take many subgames per launch.
+modes, with fp64 and fp32 tables, and on a capped persistent grid whose warps take many subgames per launch; the wave test also
+with weights away from the initialisation (the `distinct` and `trained` families of test_value_net_accuracy.py).
 """
 import numpy as np
 import pytest
@@ -88,16 +89,22 @@ def _same(a, b, what):
         (what, int((a != b).sum()), float(np.nanmax(np.abs(a.astype(np.float64) - b.astype(np.float64)))))
 
 
+# weight families of test_value_net_accuracy.py: the initialisation, every LayerNorm parameter distinct with the output layer x30,
+# and the trainer's weights after 400 steps (on the games that generate training data)
+GAME_FAMILIES = [(D, F, fam) for D, F in GAMES for fam in ("init", "distinct", "trained") if fam != "trained" or (D, F) != (2, 3)]
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("cap", [0, 3])
 @pytest.mark.parametrize("dtype", ["STATE_F64", "STATE_F32"])
 @pytest.mark.parametrize("mode", MODES)
-@pytest.mark.parametrize("D,F", GAMES)
-def test_wave_bit_identical_without_dead_rows(net_weights, D, F, mode, dtype, cap):
+@pytest.mark.parametrize("D,F,family", GAME_FAMILIES)
+def test_wave_bit_identical_without_dead_rows(D, F, family, mode, dtype, cap):
     """A wave of mixed roots, 90 iterations in two runs (the second replayed from a CUDA graph on its second call): regrets, last
     and sum strategies, snapshot, root value means and the leaf rows (queries, net outputs, scalers) byte for byte with and without
     the dead rows; the evaluated-row counter adds up."""
     import rebel_b200 as rb
+    from test_value_net_accuracy import family_weights
     A, H, Q = game_dims(D, F)
     K = 600
     rng = np.random.RandomState(D * 10 + F)
@@ -106,7 +113,7 @@ def test_wave_bit_identical_without_dead_rows(net_weights, D, F, mode, dtype, ca
     lb = rng.randint(-1, A - 2, size=K).astype(np.int32); lb[:8] = -1
     pl = rng.randint(0, 2, size=K).astype(np.int32)
     act = rng.randint(0, 90, size=K).astype(np.int32)
-    w = net_weights(D, F)
+    w = family_weights(family, D, F)
     got = []
     for skip in (True, False):
         S = _solver(rb, D, F, K, mode, getattr(rb, dtype), skip, w, cap)
@@ -126,7 +133,7 @@ def test_wave_bit_identical_without_dead_rows(net_weights, D, F, mode, dtype, ca
     (on, ev_on, rows), (off, ev_off, rows_off) = got
     assert rows == rows_off and ev_off == 2 * 90 * rows, (ev_off, rows)
     dead_frac = 1 - ev_on / ev_off
-    print(f"[dead-rows] {D}x{F}f {mode} {dtype} cap {cap}: {100 * dead_frac:.1f} % of the rows dead")
+    print(f"[dead-rows] {D}x{F}f {family} {mode} {dtype} cap {cap}: {100 * dead_frac:.1f} % of the rows dead")
     assert 0 < dead_frac < 1
     for k in ("snapshot", "last", "sum", "regrets", "mu", "q", "out", "sc"):
         _same(on[k], off[k], k)

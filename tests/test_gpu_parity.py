@@ -473,10 +473,10 @@ def test_full_size_properties_1x6f(rb, port, net_weights, net_name):
 
 @pytest.mark.parametrize("net_name", ["tc_f16x2", "tc_f16"])
 @pytest.mark.parametrize("D,F", [(1, 6), (2, 3)])
-def test_value_net_rows_do_not_depend_on_their_tile(rb, port, net_weights, D, F, net_name):
+def test_value_net_rows_do_not_depend_on_their_tile(rb, net_weights, D, F, net_name):
     """The persistent wgmma kernel (leaf_mlp_tc.cuh) evaluates every query row on its own: the outputs of a subgame's rows are
     bit-identical whether the wave has 1, 2, 3, 149 or 1300 subgames (CTAs with a single tile, an odd / even number of tiles,
-    both query buffers and both warpgroups, partial last tile), and match the fp32 oracle net within fp16 tolerance."""
+    both query buffers and both warpgroups, partial last tile).  Their accuracy is checked in test_value_net_accuracy.py."""
     A, H, Q = game_dims(D, F)
     Kmax = 1300
     rng = np.random.RandomState(5)
@@ -496,9 +496,6 @@ def test_value_net_rows_do_not_depend_on_their_tile(rb, port, net_weights, D, F,
         S.close()
         if ref is None:
             ref = (q, o, mu)
-            want = port.net2_forward(w, Q, 256, H, q)
-            err = np.abs(o - want)
-            assert err.max() < 4e-3 * max(1.0, np.abs(want).max()) and err.mean() < 4e-4, (err.max(), err.mean())
         else:
             n = len(q)
             assert np.array_equal(q, ref[0][:n]) and np.array_equal(o, ref[1][:n]) and np.array_equal(mu, ref[2][:K]), K

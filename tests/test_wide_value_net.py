@@ -67,10 +67,10 @@ def _beliefs(rng, n, H):
 @pytest.mark.gpu
 @pytest.mark.parametrize("net_name", ["tc_f16x2", "tc_f16"])
 @pytest.mark.parametrize("D,F", WIDE)
-def test_wide_net_rows_do_not_depend_on_their_tile(rb, port, net_weights, D, F, net_name):
+def test_wide_net_rows_do_not_depend_on_their_tile(rb, net_weights, D, F, net_name):
     """Every query row is evaluated on its own: bit-identical outputs whether the wave has 1, 2, 3, 149 or 1300 subgames (one
-    tile, odd / even tile counts per CTA, both warpgroups, partial last tile), and the outputs match the fp32 oracle net within
-    the fp16 tolerance of test_value_net_rows_do_not_depend_on_their_tile (max <= 4e-3 relative, mean <= 4e-4)."""
+    tile, odd / even tile counts per CTA, both warpgroups, partial last tile).  Their accuracy is checked in
+    test_value_net_accuracy.py."""
     A, H, Q = game_dims(D, F)
     Kmax = 1300
     rng = np.random.RandomState(5)
@@ -90,11 +90,6 @@ def test_wide_net_rows_do_not_depend_on_their_tile(rb, port, net_weights, D, F, 
         S.close()
         if ref is None:
             ref = (q, o, mu)
-            n = min(len(q), 8192)
-            want = port.net2_forward(w, Q, 256, H, q[:n])
-            err = np.abs(o[:n] - want)
-            _note(f"{D}x{F}f {net_name}: {len(q)} rows, max |out - fp32 net| {err.max():.2e}, mean {err.mean():.2e}")
-            assert err.max() < 4e-3 * max(1.0, np.abs(want).max()) and err.mean() < 4e-4, (err.max(), err.mean())
         else:
             n = len(q)
             assert np.array_equal(q, ref[0][:n]) and np.array_equal(o, ref[1][:n]) and np.array_equal(mu, ref[2][:K]), K
