@@ -205,7 +205,8 @@ int cfrb_load_state(cfrb_handle* h, const double* regrets, const double* last_st
 
 /* Debug/parity taps of the most recent iteration: query rows [rows][Q] and the (unscaled) net outputs
  * [rows][H] for all pseudo-leaves of the wave in (subgame, leaf) order; returns the number of rows,
- * writes at most cap_rows. */
+ * writes at most cap_rows.  After a self-play wave whose initial-state games shared one solve (cfrb_wave_solved < n), the rows of
+ * the games that took the shared results were never written: their entries are not those of the wave (zero queries). */
 int cfrb_debug_leaf_io(cfrb_handle* h, float* queries, float* net_out, double* scalers, int32_t cap_rows);
 
 /* Debug taps of the tensor-core value net (either tensor-core mode, either kernel): re-runs it on the current query tiles and returns
@@ -429,6 +430,13 @@ int cfrb_schedule_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, 
 /* Test aid: run the depth <= 2 CFR kernel on at most max_ctas CTAs (0 = as many as are resident at once), so that every warp
  * solves many subgames per launch.  Returns the number of CTAs resident at once. */
 int cfrb_debug_d2_grid(cfrb_handle* h, int32_t max_ctas);
+/* Test aid: share = 0 makes the next self-play waves solve every game on its own, instead of solving the games at the initial
+ * state (no bid yet, player 0, every belief bitwise 1 / num_hands) once and giving every other one the results (default 1). */
+int cfrb_debug_selfplay_share(cfrb_handle* h, int32_t share);
+/* The number of subgames the current wave's last solve ran: its size, less all but one of its initial-state games when it is a
+ * self-play wave whose initial-state games shared one solve.  A rerun of the wave (cfrb_reset_wave, the rebuild of its sum
+ * strategy) solves every game.  Synchronises then. */
+int cfrb_wave_solved(cfrb_handle* h);
 /* Test aid: skip = 0 makes the value net evaluate every pseudo-leaf row, dead or not, from the next cfrb_set_weights on. */
 int cfrb_debug_skip_dead_rows(cfrb_handle* h, int32_t skip);
 /* Block until the work enqueued on `cuda_stream` (NULL = the handle's stream) has finished. */

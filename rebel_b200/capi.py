@@ -132,6 +132,8 @@ def lib():
     L.cfrb_wave_order.argtypes = [vp, _ip, C.c_int32]
     L.cfrb_schedule_order.argtypes = [C.c_int32] * 4 + [_ip, _ip, C.POINTER(C.c_int64)]
     L.cfrb_debug_d2_grid.argtypes = [vp, C.c_int32]
+    L.cfrb_debug_selfplay_share.argtypes = [vp, C.c_int32]
+    L.cfrb_wave_solved.argtypes = [vp]
     L.cfrb_mark.argtypes = [vp, C.c_int32, vp]
     L.cfrb_mark_elapsed_ms.argtypes = [vp, C.c_int32, C.c_int32, _fp]
     L.cfrb_l2_flush.argtypes = [vp, C.c_size_t, vp]
@@ -599,6 +601,17 @@ class WaveSolver:
     def kernel_path(self):
         """Which CFR iteration kernel this handle runs: 0 = depth-2 kernel, 1 = warp per subgame, 2 = CTA per subgame."""
         return _check(lib().cfrb_debug_kernel_path(self._h))
+
+    def debug_selfplay_share(self, share):
+        """Test aid: share=False makes the next self-play waves solve every game on its own, instead of solving the initial-state
+        games once and copying the results to the others."""
+        _check(lib().cfrb_debug_selfplay_share(self._h, int(bool(share))))
+
+    @property
+    def wave_solved(self):
+        """Subgames the current wave's solve ran: the wave's size, less the initial-state games of a self-play wave that took the
+        results of another one's solve."""
+        return _check(lib().cfrb_wave_solved(self._h))
 
     def debug_d2_grid(self, max_ctas):
         """Test aid: run the depth-2 CFR kernel on at most max_ctas CTAs (0 = no cap); returns the CTAs resident at once."""

@@ -143,6 +143,10 @@ void sp_launch_finish(const SpDev& p, const real* mu, const real* snap, float* e
   if (ex_q) sp_examples_kernel<real><<<(2 * p.K + 127) / 128, 128, 0, st>>>(p, mu, ex_q, ex_v);
   sp_advance_kernel<real><<<(p.K + 127) / 128, 128, 0, st>>>(p, snap);
 }
+template <typename real>
+void sp_launch_share(const SpDev& p, const CfrDev<real>& d, cudaStream_t st) {
+  sp_share_kernel<real><<<p.K, 128, 0, st>>>(p, d);
+}
 void match_launch_deal(const MatchDev& p, cudaStream_t st) { match_deal_kernel<<<(p.S + 127) / 128, 128, 0, st>>>(p); }
 template <typename real>
 void match_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
@@ -289,6 +293,7 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void cfr_launch_iter_d2<real>(const CfrDev<real>&, int, int, size_t, cudaStream_t, int, int, int, int);                \
   template void sp_launch_begin<real>(const SpDev&, real*, cudaStream_t);                                                  \
   template void sp_launch_finish<real>(const SpDev&, const real*, const real*, float*, float*, cudaStream_t);              \
+  template void sp_launch_share<real>(const SpDev&, const CfrDev<real>&, cudaStream_t);                                    \
   template void match_launch_begin<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                           \
   template void match_launch_advance<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                         \
   template void lbr_launch_begin<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                               \

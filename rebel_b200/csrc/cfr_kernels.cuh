@@ -1042,11 +1042,15 @@ __global__ void __launch_bounds__(128, 8) cfr_iter_d2_kernel(CfrDev<real> p, int
       if (p.fp) fp_backward_d2<real, HC>(p, t, lv, k, tb, slot, bel, lane);
       else cfr_backward_d2<real, HC, KEEP>(p, t, lv, k, tb, slot, bel, aux, lane);
     }
-    // sampling-strategy snapshot for RlRunner (recursive_solving.cc:168-174): state after `iter` iterations
-    if (p.sg_act_iter[k] == iter) {
-      const real* Sg = p.Sg + (size_t)k * p.table_stride;
-      real* __restrict__ Sn = p.Snap + (size_t)k * p.table_stride;
-      for (int i = lane; i < (t.N - 1) * H; i += 32) Sn[i] = Sg[i];
+    // sampling-strategy snapshot for RlRunner (recursive_solving.cc:168-174): state after `iter` iterations.  The representative of a
+    // shared wave keeps every iteration's instead, for the games that share its solve (sp_share_kernel).
+    {
+      real* Sn = p.sg_act_iter[k] == iter ? p.Snap + (size_t)k * p.table_stride : nullptr;
+      if (p.snap_hist != nullptr && k == *p.share_rep) Sn = p.snap_hist + (size_t)iter * p.table_stride;
+      if (Sn != nullptr) {
+        const real* Sg = p.Sg + (size_t)k * p.table_stride;
+        for (int i = lane; i < (t.N - 1) * H; i += 32) Sn[i] = Sg[i];
+      }
     }
     if (do_f) cfr_forward_d2<real, HC>(p, t, lv, k, iter & 1, slot, bel, do_b ? (tb == rp ? 0 : 1) : -1, aux, hist, lane);
     // The next ticket.  Every warp that started draws exactly once more than it has subgames left to take, so the counter is
@@ -1072,8 +1076,9 @@ __global__ void __launch_bounds__(512) cfr_init_kernel(CfrDev<real> p, int scrat
   real* smem = reinterpret_cast<real*>(smem_raw);
   const int groups_per_cta = blockDim.x / G;
   const int gid = threadIdx.x / G, lane = threadIdx.x % G;
-  const int k = blockIdx.x * groups_per_cta + gid;
-  if (k >= *p.wave_n) return;
+  const int i0 = blockIdx.x * groups_per_cta + gid;
+  if (i0 >= *p.wave_n) return;
+  const int k = p.sg_order ? p.sg_order[i0] : i0;   // the wave's subgames, or the solved set of a shared self-play wave
   const TemplateDev t = p.tmpl[p.sg_tmpl[k]];
   const int H = p.H;
   real* base = (G == 32) ? smem + (size_t)gid * scratch_per_group : p.scratch + (size_t)k * p.scratch_stride;
@@ -1090,6 +1095,7 @@ __global__ void __launch_bounds__(512) cfr_init_kernel(CfrDev<real> p, int scrat
   // taken here
   real* __restrict__ Sn = p.Snap + (size_t)k * p.table_stride;
   const bool snap0 = p.sg_act_iter[k] == 0;
+  real* __restrict__ hist0 = p.snap_hist != nullptr && k == *p.share_rep ? p.snap_hist : nullptr;   // row 0 of the shared history
   for (int h = lane; h < H; h += G) { reach0[h] = b[h]; reach1[h] = b[H + h]; }
   group_sync<G>();
   for (int d = 1; d < t.levels; ++d) {
@@ -1102,6 +1108,7 @@ __global__ void __launch_bounds__(512) cfr_init_kernel(CfrDev<real> p, int scrat
       const real a0 = reach0[par * H + h], a1 = reach1[par * H + h];
       Sg[e] = u;
       if (snap0) Sn[e] = u;
+      if (hist0) hist0[e] = u;
       R[e] = p.fp ? u : (real)0;       // FP: last_strategies starts as the uniform strategy (subgame_solving.cc:375-377)
       if (p.keep_sum) S[e] = u * (actor == 0 ? a0 : a1);
       reach0[c * H + h] = actor == 0 ? a0 * u : a0;

@@ -40,7 +40,7 @@ struct CfrDev {
   const unsigned char* tpk; int tpk_stride;   // packed byte templates (cfr_iter_d2_kernel): template i at tpk + i * tpk_stride
   const __half* qconst;           // per template [L][Qpad] fp16: constant part of the query rows (one-hot last bid, 1 at column Q)
   // wave
-  const int* wave_n;              // [1] number of live subgames
+  const int* wave_n;              // [1] number of live subgames (of the solved set, in a self-play wave whose initial-state games share one solve)
   const int* sg_tmpl; const int* sg_player; const int* sg_row_off; const int* sg_act_iter;
   const int* sg_order;            // [K] wave positions largest template first (cfr_iter_d2_kernel's schedule) -- or nullptr = identity
   int* ticket;                    // [1] cfr_iter_d2_kernel's subgame counter; zero between launches
@@ -68,6 +68,10 @@ struct CfrDev {
   int fp, optimistic;             // fictitious play instead of CFR (FP, subgame_solving.cc:364-506)
   int keep_sum;                   // CFR: 1 = maintain S (sum_strategies); 0 = neither read nor write it (a self-play wave, whose
                                   // loop never reads it).  FP always keeps it: its average strategy is computed from S.
+  // A self-play wave whose initial-state games share one solve (sp_scan_kernel) -- or nullptr: the representative (wave position
+  // *share_rep, -1 = none) leaves Sg after every iteration i in snap_hist [num_iters + 1][table_stride] at row i, from which
+  // sp_share_kernel takes every initial-state game's act_iteration snapshot.
+  real* snap_hist; const int* share_rep;
 };
 
 // Scratch of a group (reals): bufA[N*H] | bufB[N*H] | hist[10*T] | lsum[2*L]  (hist: per-terminal match-count histogram,
@@ -134,9 +138,16 @@ struct SpDev {
   // tree templates (read-only; the same arrays the CFR kernels index)
   const TemplateDev* tmpl; const int* child_begin; const int* nchild; const int* last_bid;
   // wave descriptors
-  int* wave;                          // [0] = number of subgames, [1] = value-net rows
+  int* wave;                          // [0] = number of subgames, [1] = value-net rows, [2] = subgames solved, [3] = representative
   int* sg_tmpl; int* sg_player; int* sg_row_off; int* sg_act;
-  int* sg_order;                      // [K] wave positions sorted by tmpl_rank (stable)
+  int* sg_order;                      // [K] wave positions sorted by tmpl_rank (stable); when share, [solved_off, solved_off + K) the
+                                      // solved ones alone (solved_off = the handle's max_subgames, so that a CUDA graph of a shared
+                                      // wave stays valid when the session is re-created with another K)
+  int solved_off;
+  // share: the initial-state games (no bid yet, player 0, every belief bitwise 1 / H) share one solve, the one of the lowest such
+  // wave position (the representative); the others are copies, which the CFR kernels skip and sp_share_kernel fills in
+  int share;
+  int* sg_init;                       // [K] 1 = the game is at the initial state (written only when share)
   const int* tmpl_rank;               // [A] schedule rank of each template, 0 = the costliest (schedule_ranks, cfr_tree.h)
   int table_stride;
 };
@@ -145,6 +156,8 @@ void sp_launch_seed(const SpDev& p, const uint32_t* dev_seeds, cudaStream_t st);
 template <typename real> void sp_launch_begin(const SpDev& p, real* wave_beliefs, cudaStream_t st);
 // training examples of the finished wave (skipped when ex_q == nullptr) and the sampling step of every game
 template <typename real> void sp_launch_finish(const SpDev& p, const real* mu, const real* snap, float* ex_q, float* ex_v, cudaStream_t st);
+// after the last iteration of a shared wave: the representative's results to every copy, and every initial-state game's snapshot
+template <typename real> void sp_launch_share(const SpDev& p, const CfrDev<real>& d, cudaStream_t st);
 // Head-to-head matches (match_kernels.cuh): S game slots playing G games between two handles (agent 0 = A, 1 = B).
 struct MatchDev {
   int S, G, A, H, F, max_depth, sampled, iters[2];

@@ -132,6 +132,7 @@ template <typename Real>
 struct WaveState {
   using real = Real;
   DevBuf<real> beliefs, mu, R, Sg, S, Snap, vterm, scaler, scratch;
+  DevBuf<real> snap_hist;   // [num_iters + 1][table_stride]: the shared initial-state solve's Sg after every iteration (self-play)
   cfrb::CfrDev<real> dev{};
 };
 
@@ -157,6 +158,10 @@ struct cfrb_handle {
   int d2_grid_cap = 0;     // test aid (cfrb_debug_d2_grid): at most this many CTAs, 0 = no cap
   std::vector<int> tmpl_rank;   // schedule rank of each template (schedule_ranks)
   bool sorted = false;     // d_sg_order holds the current wave's schedule; otherwise the depth-2 kernel takes wave order
+  // Self-play waves on the depth-2 kernel solve their initial-state games once (sp_scan_kernel, sp_share_kernel).  share_on: test
+  // aid (cfrb_debug_selfplay_share), false = every game is solved on its own.  sharing: the kernels being enqueued solve the solved
+  // set only.  wave_shared: the current wave was solved that way.
+  bool share_on = true, sharing = false, wave_shared = false;
   int n1max = 0;           // bound on the level-1 nodes of a template (the depth-2 scratch layout)
   int table_stride = 0;
   int num_sms = 0;
@@ -167,9 +172,9 @@ struct cfrb_handle {
   std::vector<Event> net_ev;   // pairs around value-net launches (profiling mode)
   int net_ev_used = 0;
   // CUDA graphs of whole cfrb_run calls (2 launches per iteration would otherwise be enqueued one by one by the host)
-  struct GraphEntry { int first, count, prof, has_rows, sorted, keep_sum; GraphExec exec; int launches, net_launches, ev_used; };
+  struct GraphEntry { int first, count, prof, has_rows, sorted, keep_sum, sharing; GraphExec exec; int launches, net_launches, ev_used; };
   std::vector<GraphEntry> graphs;
-  std::vector<std::array<int, 6>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
+  std::vector<std::array<int, 7>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
   bool capturing = false;           // launch geometry independent of the wave size while a graph is being captured / replayed
   // device: templates
   DevBuf<cfrb::TemplateDev> d_tmpl;
@@ -195,9 +200,9 @@ struct cfrb_handle {
   DevBuf<unsigned char> d_tpk;   // byte-packed templates for the depth <= 2 kernel
   int tpk_stride = 0;
   // device: wave (untyped part)
-  DevBuf<int> d_wave;      // [0] = n, [1] = rows
+  DevBuf<int> d_wave;      // [0] = n, [1] = rows, [2] = subgames solved, [3] = representative (a self-play wave, sp_scan_kernel)
   DevBuf<int> d_sg_tmpl, d_sg_player, d_sg_row_off, d_sg_act, d_steps;
-  DevBuf<int> d_sg_order, d_tmpl_rank, d_ticket;   // the depth-2 kernel's schedule, template ranks, subgame counter
+  DevBuf<int> d_sg_order, d_tmpl_rank, d_ticket;   // the depth-2 kernel's schedule [2 max_subgames] (SpDev::sg_order), template ranks, subgame counter
   DevBuf<float> d_X, d_out, d_dbg;
   long long* dbg_trace = nullptr;   // set only inside cfrb_debug_net_trace
   int x2_gelu = 2;                  // GELU variant of CFRB_NET_TC_F16X2 (leaf_mlp_tc.cuh kGelu): 2 = fp32 tanh, 1 = packed half
@@ -238,7 +243,7 @@ struct cfrb_handle {
   struct SelfPlay {
     bool ready = false, pending = false;    // pending: a wave has been run whose games have not been advanced yet
     int K = 0;
-    DevBuf<int> last_bid, player, mt_idx;
+    DevBuf<int> last_bid, player, mt_idx, init;
     DevBuf<double> beliefs;
     DevBuf<uint32_t> mt, seeds;
     cfrb::SpDev dev{};
@@ -368,6 +373,8 @@ template <typename real>
 static cfrb::CfrDev<real> wave_dev(const cfrb_handle* h, const WaveState<real>& s) {
   cfrb::CfrDev<real> d = s.dev;
   d.keep_sum = !h->sum_dropped;
+  if (h->sorted) d.sg_order = h->d_sg_order.p + (h->sharing ? h->cfg.max_subgames : 0);
+  if (h->sharing) { d.wave_n = h->d_wave.p + 2; d.snap_hist = s.snap_hist.p; d.share_rep = h->d_wave.p + 3; }
   return d;
 }
 
@@ -391,7 +398,6 @@ static int launch_iter(cfrb_handle* h, WaveState<real>& s, cudaStream_t st, int 
     // persistent warps: no more CTAs than are resident at once (the warps then take the wave's subgames from a counter)
     int blocks = std::min((nsg + h->d2_groups_per_cta - 1) / h->d2_groups_per_cta, h->d2_ctas);
     if (h->d2_grid_cap > 0) blocks = std::min(blocks, h->d2_grid_cap);
-    d.sg_order = h->sorted ? h->d_sg_order.p : nullptr;
     cfrb::cfr_launch_iter_d2<real>(d, blocks, 32 * h->d2_groups_per_cta, h->d2_smem, st, iter, do_b, do_f, h->d2_scratch_per_group);
   } else {
     const int blocks = (nsg + h->groups_per_cta - 1) / h->groups_per_cta;
@@ -475,6 +481,7 @@ static int materialise_sum(cfrb_handle* h) {
   const int iters = h->iters_done;
   h->sum_dropped = false;
   h->iters_done = 0;
+  h->wave_shared = false;   // the rerun solves every game
   int rc = launch_init(h, h->own_stream);
   if (!rc) rc = cfrb_run(h, iters, h->own_stream);
   if (rc) return rc;
@@ -711,15 +718,15 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   int max_optin = 0;
   CK(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, cfg->device));
   CK(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, cfg->device));
-  CK(h->d_wave.alloc(2));
+  CK(h->d_wave.alloc(4));
   CK(h->d_sg_tmpl.alloc(K)); CK(h->d_sg_player.alloc(K)); CK(h->d_sg_row_off.alloc(K)); CK(h->d_sg_act.alloc(K));
   CK(h->d_steps.alloc((size_t)K * 2));
-  CK(h->d_sg_order.alloc(K)); CK(h->d_ticket.alloc(1));
+  CK(h->d_sg_order.alloc(2 * (size_t)K)); CK(h->d_ticket.alloc(1));
   CK(cudaMemset(h->d_ticket.p, 0, sizeof(int)));
   const size_t rows_cap = (size_t)K * std::max(h->Lmax, 1);
   CK(h->d_X.alloc(cfg->net_mode == CFRB_NET_FP32 ? rows_cap * h->Qpad : 1));
   CK(h->d_out.alloc(rows_cap * h->Hout));
-  CK(cudaMemset(h->d_wave.p, 0, 2 * sizeof(int)));
+  CK(cudaMemset(h->d_wave.p, 0, 4 * sizeof(int)));
   CK(cudaMemset(h->d_out.p, 0, rows_cap * h->Hout * sizeof(float)));
   if (is_tc(cfg->net_mode)) {
     // CFRB_TC_WIDE=1: the wide kernel also on games the resident kernel serves (tests, measurements)
@@ -943,7 +950,7 @@ int cfrb_begin_wave(cfrb_handle* h, int32_t n, const int32_t* last_bid, const in
   std::vector<int> order(n);
   cfrb::schedule_order(h->tmpl_rank, tm.data(), n, order.data());
   h->n = n; h->rows = rows; h->iters_done = 0; h->rows_on_device = false; h->sp.pending = false; h->sorted = true;
-  h->sum_dropped = false;
+  h->sum_dropped = false; h->wave_shared = false;
   h->h_tmpl = tm; h->h_player = pl; h->h_row_off = ro;
   h->h_last_bid.assign(last_bid, last_bid + n);
   h->h_beliefs.assign(beliefs, beliefs + (size_t)n * 2 * H);
@@ -1042,6 +1049,7 @@ int cfrb_reset_wave(cfrb_handle* h, void* cuda_stream) {
   CK(cudaSetDevice(h->cfg.device));
   h->iters_done = 0;
   h->sum_dropped = false;   // a wave the host runs again keeps its sum
+  h->wave_shared = false;   // ... and solves every game
   if (h->n == 0) return CFRB_OK;
   return launch_init(h, cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream);
 }
@@ -1079,19 +1087,20 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
   // Long runs are replayed from a CUDA graph: one host call instead of 2 * iters kernel launches, so a busy or slow host
   // thread cannot starve the GPU.  The graph bakes in the iteration indices and a wave-size-independent launch geometry; it
   // is keyed by (first iteration, count, profiling period, "the wave has value-net rows", "the wave has a schedule", "the wave keeps
-  // the sum table").  The fp32 parity net sizes its grid by the row count and stays on the eager path, like short runs.
+  // the sum table", "the wave's initial-state games share a solve").  The fp32 parity net sizes its grid by the row count and stays
+  // on the eager path, like short runs.
   static const bool no_graph = [] { const char* e = std::getenv("CFRB_NO_GRAPH"); return e && *e == '1'; }();
   const bool graphable = !no_graph && iters >= 64 && h->cfg.net_mode != CFRB_NET_FP32;
   if (graphable) {
-    const int has_rows = h->rows > 0 || h->rows_on_device, sorted = h->sorted, keep_sum = !h->sum_dropped;
+    const int has_rows = h->rows > 0 || h->rows_on_device, sorted = h->sorted, keep_sum = !h->sum_dropped, sharing = h->sharing;
     cfrb_handle::GraphEntry* g = nullptr;
     for (auto& e : h->graphs)
       if (e.first == first && e.count == iters && e.prof == h->profiling && e.has_rows == has_rows && e.sorted == sorted &&
-          e.keep_sum == keep_sum) { g = &e; break; }
+          e.keep_sum == keep_sum && e.sharing == sharing) { g = &e; break; }
     if (!g) {
       // capture + instantiation of ~2 * iters nodes costs ~0.1 s: only worth it for a key that repeats (waves of a self-play
       // loop, bench steps), not for one-off run lengths (e.g. the evaluator's per-chunk act_iteration maxima)
-      const std::array<int, 6> key{first, iters, h->profiling, has_rows, sorted, keep_sum};
+      const std::array<int, 7> key{first, iters, h->profiling, has_rows, sorted, keep_sum, sharing};
       bool seen = false;
       for (const auto& k : h->graph_seen) seen |= k == key;
       if (!seen) {
@@ -1119,7 +1128,7 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
       h->launches = l0;
       if (rc == CFRB_OK && ce == cudaSuccess && exec) {
         if (h->graphs.size() >= 8) h->graphs.erase(h->graphs.begin());
-        h->graphs.push_back({first, iters, h->profiling, has_rows, sorted, keep_sum, std::move(exec), captured, h->net_launches_run,
+        h->graphs.push_back({first, iters, h->profiling, has_rows, sorted, keep_sum, sharing, std::move(exec), captured, h->net_launches_run,
                              h->net_ev_used});
         g = &h->graphs.back();
       } else {
@@ -1247,7 +1256,14 @@ static int dense_tiles(cfrb_handle* h, std::vector<__half>& x) {
   CK(cudaMemcpy(src.data(), h->d_row_src.p, pos * sizeof(int), cudaMemcpyDeviceToHost));
   cfrb::NetRows c{};
   CK(cudaMemcpy(&c, h->d_net_rows.p, sizeof(c), cudaMemcpyDeviceToHost));
-  const size_t rows = (size_t)h->rows, live = std::min<size_t>((size_t)std::max(c.last_live, 0), rows);
+  const size_t rows = (size_t)h->rows;
+  size_t written = rows;   // rows the last forward half wrote: the copies of a shared self-play wave keep theirs unwritten (sp_scan_kernel)
+  if (h->wave_shared) {
+    int solved = 0;
+    CK(cudaMemcpy(&solved, h->d_wave.p + 2, sizeof(int), cudaMemcpyDeviceToHost));
+    written -= (size_t)(h->n - solved) * h->tmpl[0].L;
+  }
+  const size_t live = std::min<size_t>((size_t)std::max(c.last_live, 0), written);
   std::vector<__half> d(x.size(), __float2half_rn(0.f));
   auto place = [&](size_t p) {
     const int r = src[p];
@@ -1257,7 +1273,7 @@ static int dense_tiles(cfrb_handle* h, std::vector<__half>& x) {
           x[(p / R) * R * Qp + cfrb::tc::umma_kmajor_offset_halves((int)(p % R), (int)q, (int)R)];
   };
   for (size_t p = 0; p < live; ++p) place(p);
-  for (size_t p = pos - (rows - live); p < pos; ++p) place(p);
+  for (size_t p = pos - (written - live); p < pos; ++p) place(p);
   x.swap(d);
   return CFRB_OK;
 }
@@ -1668,14 +1684,25 @@ int cfrb_last_run_ms(cfrb_handle* h, float* total_ms, float* net_ms) {
 // Starts a wave of n subgames built on the device (its leaf rows and roots exist only there) and runs num_iters on it.  sorted:
 // d_sg_order holds the wave's schedule; otherwise the depth-2 kernel takes wave order.  drop_sum: a self-play wave, whose loop
 // reads the snapshots and root means only; CFR then leaves the sum table alone (materialise_sum rebuilds it for a reader).  Match,
-// LBR and agent waves keep it: they act with the average strategy of the wave they have just solved (act_slot).
-static int solve_device_wave(cfrb_handle* h, int n, bool sorted, bool drop_sum, cudaStream_t st, int iters = -1) {
+// LBR and agent waves keep it: they act with the average strategy of the wave they have just solved (act_slot).  share: a
+// self-play wave whose descriptors sp_scan_kernel built with SpDev::share; only its solved set is solved, and sp_share_kernel then
+// gives the copies their results.  Afterwards the wave is like one solved in full: a rerun (materialise_sum, cfrb_reset_wave) solves
+// every game.
+static int solve_device_wave(cfrb_handle* h, int n, bool sorted, bool drop_sum, cudaStream_t st, int iters = -1, bool share = false) {
   h->n = n; h->rows = 0; h->rows_on_device = true; h->mirror_stale = true; h->iters_done = 0; h->sp.pending = false;
   h->sorted = sorted;
   h->sum_dropped = drop_sum && h->cfg.solver == CFRB_SOLVER_CFR;
   h->sum_uploads = h->weight_uploads;
-  const int rc = launch_init(h, st);
-  return rc ? rc : cfrb_run(h, iters < 0 ? h->cfg.num_iters : iters, st);
+  h->sharing = h->wave_shared = share;
+  int rc = launch_init(h, st);
+  if (!rc) rc = cfrb_run(h, iters < 0 ? h->cfg.num_iters : iters, st);
+  if (!rc && share) {
+    with_state(h, [&](auto& s) { cfrb::sp_launch_share(h->sp.dev, wave_dev(h, s), st); });
+    ++h->launches;
+    if (cudaGetLastError() != cudaSuccess) rc = fail(CFRB_ECUDA, "sp_share_kernel launch failed");
+  }
+  h->sharing = false;
+  return rc;
 }
 
 // ============================================================================================ recursive to-leaf exploitability
@@ -2481,7 +2508,12 @@ int cfrb_selfplay_create(cfrb_handle* h, int32_t n_games, const uint32_t* seeds,
   auto& sp = h->sp;
   const int K = n_games, H = h->g.H;
   CK(sp.last_bid.alloc(K)); CK(sp.player.alloc(K)); CK(sp.mt_idx.alloc(K)); CK(sp.beliefs.alloc((size_t)K * 2 * H));
-  CK(sp.mt.alloc((size_t)624 * K)); CK(sp.seeds.alloc(K));
+  CK(sp.mt.alloc((size_t)624 * K)); CK(sp.seeds.alloc(K)); CK(sp.init.alloc(K));
+  // once per handle (its size depends on the configuration alone): a CUDA graph of a shared wave keeps pointing at it when the
+  // session is re-created
+  if (h->d2) CK(with_state(h, [&](auto& s) {
+    return s.snap_hist.p ? cudaSuccess : s.snap_hist.alloc((size_t)(h->cfg.num_iters + 1) * h->table_stride);
+  }));
   cfrb::SpDev& d = sp.dev;
   d.K = K; d.A = h->g.A; d.H = H; d.Q = h->g.Q; d.iters = h->cfg.num_iters; d.sample_leaf = sample_leaf;
   d.random_action_prob = random_action_prob;
@@ -2490,6 +2522,7 @@ int cfrb_selfplay_create(cfrb_handle* h, int32_t n_games, const uint32_t* seeds,
   d.wave = h->d_wave.p; d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_row_off = h->d_sg_row_off.p;
   d.sg_act = h->d_sg_act.p; d.table_stride = h->table_stride;
   d.sg_order = h->d_sg_order.p; d.tmpl_rank = h->d_tmpl_rank.p;
+  d.sg_init = sp.init.p; d.solved_off = h->cfg.max_subgames;
   CK(cudaStreamSynchronize(h->own_stream));
   CK(cudaMemcpyAsync(sp.seeds.p, seeds, (size_t)K * sizeof(uint32_t), cudaMemcpyHostToDevice, h->own_stream));
   cfrb::sp_launch_seed(d, sp.seeds.p, h->own_stream);
@@ -2520,10 +2553,12 @@ int cfrb_selfplay_wave(cfrb_handle* h, float* dev_ex_q, float* dev_ex_v, int32_t
     h->sp.ev_recorded = true;
   }
   if (start_next) {
+    // the initial-state games share one solve on the depth-2 kernel (the only one that takes its subgames from a schedule)
+    h->sp.dev.share = h->d2 && h->share_on;
     with_state(h, [&](auto& s) { cfrb::sp_launch_begin(h->sp.dev, s.beliefs.p, st); });
     h->launches += 2;
     CK(cudaGetLastError());
-    const int rc = solve_device_wave(h, h->sp.K, true, true, st);
+    const int rc = solve_device_wave(h, h->sp.K, true, true, st, -1, h->sp.dev.share);
     if (rc) return rc;
     h->sp.pending = true;
     ++h->sp.waves;
@@ -2661,6 +2696,7 @@ int cfrb_selfplay_import(cfrb_handle* h, const void* in, size_t bytes) {
   h->sp.ev_recorded = false;
   // The handle holds no wave, as after cfrb_create: the readers of a solved wave (cfrb_fetch, the sum rebuild, ...) find none.
   h->n = 0; h->rows = 0; h->iters_done = 0; h->rows_on_device = false; h->mirror_stale = false; h->sum_dropped = false;
+  h->wave_shared = false;
   return CFRB_OK;
 }
 
@@ -2700,6 +2736,22 @@ int cfrb_schedule_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, 
   }
   cfrb::schedule_order(cfrb::schedule_ranks(tmpl, g.H), tm.data(), n, order);
   return CFRB_OK;
+}
+
+int cfrb_debug_selfplay_share(cfrb_handle* h, int32_t share) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  h->share_on = share != 0;
+  return CFRB_OK;
+}
+
+int cfrb_wave_solved(cfrb_handle* h) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  if (!h->wave_shared) return h->n;
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaDeviceSynchronize());
+  int n = 0;
+  CK(cudaMemcpy(&n, h->d_wave.p + 2, sizeof(int), cudaMemcpyDeviceToHost));
+  return n;
 }
 
 // Test aid: a persistent grid of at most max_ctas CTAs makes every warp of the depth-2 kernel solve many subgames per launch.

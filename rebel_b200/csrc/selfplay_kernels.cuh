@@ -12,6 +12,7 @@
 //   sp_begin      per game: act_iteration ~ U{0..num_iters} and the descriptor of its next subgame (template, player, beliefs)
 //   sp_scan       prefix sum of the pseudo-leaf counts -> packed value-net row offsets, wave size, total rows; the CFR
 //                 kernel's schedule (wave positions, costliest template first)
+//   sp_share      after the last iteration: the results of the wave's one initial-state solve to every game that shares it
 //
 // Every game owns a std::mt19937 stream (state words interleaved [624][K] so that the threads of a warp touch consecutive
 // addresses) and the libstdc++ distributions the reference uses are restated bit for bit (uniform_int_distribution = Lemire's
@@ -21,6 +22,7 @@
 // as long as the solver's strategies agree — which the tests check against the compiled reference with the zero net.
 #pragma once
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 
 #include "cfr_types.h"
@@ -116,7 +118,31 @@ __global__ void __launch_bounds__(128) sp_begin_kernel(SpDev p, real* __restrict
   p.mt_idx[g] = rng.idx;
   p.sg_tmpl[g] = p.g_last_bid[g] + 1;
   p.sg_player[g] = p.g_player[g];
-  for (int i = 0; i < 2 * p.H; ++i) wave_beliefs[(size_t)g * 2 * p.H + i] = (real)p.g_beliefs[(size_t)g * 2 * p.H + i];
+  // The initial state (sp_seed_kernel, the terminal reset of sp_advance_kernel), told by the belief bits: a game whose beliefs only
+  // compare equal to 1 / H (an imported session) is solved on its own
+  const double* gb = p.g_beliefs + (size_t)g * 2 * p.H;
+  const long long uniform = __double_as_longlong(1.0 / p.H);
+  bool init = p.g_last_bid[g] == -1 && p.g_player[g] == 0;
+  for (int i = 0; i < 2 * p.H; ++i) {
+    wave_beliefs[(size_t)g * 2 * p.H + i] = (real)gb[i];
+    init = init && __double_as_longlong(gb[i]) == uniform;
+  }
+  if (p.share) p.sg_init[g] = init;
+}
+
+// Inclusive sum of x over the 1024 threads of the CTA, through part[1024].
+__device__ int sp_block_scan(int* part, int x) {
+  const int t = threadIdx.x;
+  __syncthreads();                               // earlier readers of part[] are done
+  part[t] = x;
+  __syncthreads();
+  for (int d = 1; d < 1024; d <<= 1) {
+    const int v = t >= d ? part[t - d] : 0;
+    __syncthreads();
+    part[t] += v;
+    __syncthreads();
+  }
+  return part[t];
 }
 
 // Exclusive prefix sum of the pseudo-leaf counts of the wave's subgames (one CTA; K is at most a few 10^4).
@@ -126,17 +152,10 @@ __global__ void __launch_bounds__(1024) sp_scan_kernel(SpDev p) {
   const int b = t * per, e = min(p.K, b + per);
   int s = 0;
   for (int g = b; g < e; ++g) s += p.tmpl[p.sg_tmpl[g]].L;
-  part[t] = s;
-  __syncthreads();
-  for (int d = 1; d < 1024; d <<= 1) {
-    const int v = t >= d ? part[t - d] : 0;
-    __syncthreads();
-    part[t] += v;
-    __syncthreads();
-  }
-  int off = part[t] - s;
+  const int rows = sp_block_scan(part, s);
+  int off = rows - s;
   for (int g = b; g < e; ++g) { p.sg_row_off[g] = off; off += p.tmpl[p.sg_tmpl[g]].L; }
-  if (t == 1023) { p.wave[0] = p.K; p.wave[1] = part[1023]; }
+  if (t == 1023) { p.wave[0] = p.K; p.wave[1] = rows; }
   // The CFR kernel's schedule: the wave positions in template-rank order, a stable counting sort (schedule_order, cfr_tree.h)
   // with one block-wide exclusive scan of the per-thread counts per rank.  part[] is reused for the 32 warp totals.
   const int lane = t & 31, warp = t >> 5;
@@ -157,6 +176,54 @@ __global__ void __launch_bounds__(1024) sp_scan_kernel(SpDev p) {
       if (p.tmpl_rank[p.sg_tmpl[g]] == r) p.sg_order[pos++] = g;
     base += __shfl_sync(0xffffffffu, wsum, 31);
   }
+  // Every initial-state subgame solves the same thing bit for bit (its template, player and beliefs are the same, and so are the
+  // weights and num_iters), so a shared wave solves only the lowest one, the representative; the solved set -- every game but the
+  // copies -- keeps the schedule's order in sg_order[solved_off ..].  Every game keeps its rows, so that a rerun of the whole wave
+  // (materialise_sum) finds them; a copy's rows are simply never written.
+  if (!p.share) {
+    if (t == 1023) { p.wave[2] = p.K; p.wave[3] = -1; }
+    return;
+  }
+  __shared__ int rep_s;
+  if (t == 0) rep_s = INT_MAX;
+  int first = INT_MAX;
+  for (int g = e - 1; g >= b; --g) if (p.sg_init[g]) first = g;
+  __syncthreads();                               // rep_s is set, and the schedule above is visible to the whole CTA
+  if (first != INT_MAX) atomicMin(&rep_s, first);
+  __syncthreads();
+  const int rep = rep_s == INT_MAX ? -1 : rep_s;
+  auto solved = [&](int g) { return !p.sg_init[g] || g == rep; };
+  int c = 0;
+  for (int i = b; i < e; ++i) c += solved(p.sg_order[i]);
+  const int n_solved = sp_block_scan(part, c);
+  int pos = n_solved - c;
+  for (int i = b; i < e; ++i)
+    if (solved(p.sg_order[i])) p.sg_order[p.solved_off + pos++] = p.sg_order[i];
+  if (t == 1023) { p.wave[2] = n_solved; p.wave[3] = rep; }
+}
+
+// The copies of a shared wave (sp_scan_kernel) take the representative's tables, root means and step counters, and every
+// initial-state game takes the snapshot of its own act_iteration from the representative's history: what solving the copy
+// would have left, bit for bit.  Only the template's (N - 1) x H entries are copied, as a solve writes only those.
+template <typename real>
+__global__ void __launch_bounds__(128) sp_share_kernel(SpDev p, CfrDev<real> d) {
+  const int g = blockIdx.x;
+  if (!p.sg_init[g]) return;
+  const int rep = p.wave[3], E = (p.tmpl[0].N - 1) * p.H;
+  const size_t st = p.table_stride;
+  const real* __restrict__ hist = d.snap_hist + (size_t)d.sg_act_iter[g] * st;
+  real* __restrict__ snap = d.Snap + (size_t)g * st;
+  for (int i = threadIdx.x; i < E; i += blockDim.x) snap[i] = hist[i];
+  if (g == rep) return;
+  const size_t to = (size_t)g * st, from = (size_t)rep * st;
+  const bool keep = d.keep_sum || d.fp;          // as cfr_launch_iter_d2 chooses its instantiation
+  for (int i = threadIdx.x; i < E; i += blockDim.x) {
+    d.R[to + i] = d.R[from + i];
+    d.Sg[to + i] = d.Sg[from + i];
+    if (keep) d.S[to + i] = d.S[from + i];
+  }
+  for (int i = threadIdx.x; i < 2 * p.H; i += blockDim.x) d.mu[(size_t)g * 2 * p.H + i] = d.mu[(size_t)rep * 2 * p.H + i];
+  if (threadIdx.x < 2) d.steps[2 * g + threadIdx.x] = d.steps[2 * rep + threadIdx.x];
 }
 
 // update_value_network (subgame_solving.cc:672-676, add_training_example :220-226) of every finished subgame: for traverser
