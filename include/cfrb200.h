@@ -345,6 +345,36 @@ int64_t cfrb_full_game_regret_bytes(int32_t num_dice, int32_t num_faces);
  * adds them in node order for its summary); count = strategies added.  Any pointer may be NULL.  Synchronises. */
 int cfrb_full_game_regrets(cfrb_full_game* g, double* immediate, double* sums, double* node_sums, int64_t* count);
 
+/* ---- FP subtree forest: eval_net's full-depth solves (stats.cc:118-124) of one depth at once.  Linear fictitious play without a
+ * value net on every full-tree subtree rooted at the listed nodes of one depth, each root with its own beliefs: the root value means
+ * of a one-subgame wave rooted at that node (cfrb_begin_wave with its last_bid, player and beliefs; solver FP, linear_update,
+ * max_depth >= the subtree's depth, no net; cfrb_run(iters); cfrb_fetch's root_value_means) bit for bit, for games up to
+ * A = CFRB_TO_LEAF_MAX_ACTIONS.  The object owns an FP full-game solver's tables, the full tree, a stream, the roots' beliefs and
+ * means of the largest level and one CUDA graph of an iteration per root depth.  Refused before anything is allocated:
+ * A > CFRB_TO_LEAF_MAX_ACTIONS (CFRB_EINVAL, checked without a device) and a cfrb_fp_forest_bytes need above the device's free
+ * memory, under the cap of cfrb_debug_full_game_free_cap (CFRB_ENOMEM). */
+typedef struct cfrb_fp_forest cfrb_fp_forest;
+int cfrb_fp_forest_create(int32_t num_dice, int32_t num_faces, int32_t device, cfrb_fp_forest** out);
+int cfrb_fp_forest_destroy(cfrb_fp_forest* f);
+/* Host-only: device bytes of a forest beyond its handle: cfrb_full_game_bytes(FP) and the beliefs and means [level][2][H] of the
+ * largest depth level of the full tree.  A > CFRB_TO_LEAF_MAX_ACTIONS: CFRB_EINVAL. */
+int64_t cfrb_fp_forest_bytes(int32_t num_dice, int32_t num_faces);
+/* Host-only: the checks cfrb_fp_forest_solve makes before it touches the device: depth in [1, A - 1], n >= 1, nodes [n] full-tree
+ * node ids (BFS order) strictly ascending, all at `depth` and non-terminal; beliefs [n][2][H] finite, non-negative, every row with
+ * a positive sum; iters >= 1.  CFRB_EINVAL with the reason when one fails. */
+int cfrb_fp_forest_check(int32_t num_dice, int32_t num_faces, int32_t depth, int32_t n, const int32_t* nodes, const double* beliefs,
+                         int32_t iters);
+/* `iters` iterations (iteration i has traverser i % 2) from the FP constructor of every listed root; root_means [n][2][H] receives
+ * each root's root_value_means.  Unlisted nodes of the depth are solved with uniform beliefs and change no listed result. */
+int cfrb_fp_forest_solve(cfrb_fp_forest* f, int32_t depth, int32_t n, const int32_t* nodes, const double* beliefs, int32_t iters,
+                         double* root_means);
+/* Reach statistics of a compact full-tree strategy [N - 1][H] (entry (child - 1) * H + hand) from uniform root beliefs
+ * (compute_stategy_stats, subgame_solving.cc:823-846): for the strictly ascending node list nodes [n], node_reach [n] =
+ * (sum over hands of player 0's reach) x (the same of player 1's), each sum in hand order, and rows [n][2][H] both players' reach. */
+int cfrb_fp_forest_reach(cfrb_fp_forest* f, const double* strategy, int32_t n, const int32_t* nodes, double* node_reach, double* rows);
+/* Device memory the forest took when it was created and the part of it its handle took.  Either pointer may be NULL. */
+int cfrb_fp_forest_memory(const cfrb_fp_forest* f, int64_t* total_bytes, int64_t* handle_bytes);
+
 /* Immediate-regret accumulator on the handle's device, compute_immediate_regrets (subgame_solving.cc:984-1050) split so that a
  * list of strategies can be added in pieces: adding strategies in batches of any size gives the bits of one pass over the whole
  * list.  Reset zeroes the sums [N_full][H][A] and the count (and must precede the first add). */

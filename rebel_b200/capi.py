@@ -102,6 +102,14 @@ def lib():
     L.cfrb_full_game_regret_bytes.argtypes = [C.c_int32] * 2
     L.cfrb_full_game_regret_bytes.restype = C.c_int64
     L.cfrb_full_game_regrets.argtypes = [vp, _dp, _dp, _dp, C.POINTER(C.c_int64)]
+    L.cfrb_fp_forest_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(vp)]
+    L.cfrb_fp_forest_destroy.argtypes = [vp]
+    L.cfrb_fp_forest_bytes.argtypes = [C.c_int32] * 2
+    L.cfrb_fp_forest_bytes.restype = C.c_int64
+    L.cfrb_fp_forest_check.argtypes = [C.c_int32] * 4 + [_ip, _dp, C.c_int32]
+    L.cfrb_fp_forest_solve.argtypes = [vp, C.c_int32, C.c_int32, _ip, _dp, C.c_int32, _dp]
+    L.cfrb_fp_forest_reach.argtypes = [vp, _dp, C.c_int32, _ip, _dp, _dp]
+    L.cfrb_fp_forest_memory.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.cfrb_regrets_reset.argtypes = [vp]
     L.cfrb_regrets_add.argtypes = [vp, _fp, C.c_int32]
     L.cfrb_regrets_add_current.argtypes = [vp]
@@ -227,6 +235,26 @@ def full_game_regret_bytes(num_dice, num_faces):
     return _check(lib().cfrb_full_game_regret_bytes(num_dice, num_faces))
 
 
+def fp_forest_bytes(num_dice, num_faces):
+    """Host-only: device bytes an FpForest of this game needs beyond its handle (an FP FullGame's and the beliefs and means of
+    the largest depth level); games above 23 actions are refused."""
+    return _check(lib().cfrb_fp_forest_bytes(num_dice, num_faces))
+
+
+def _forest_args(nodes, beliefs, H):
+    nodes = np.ascontiguousarray(nodes, np.int32).reshape(-1)
+    beliefs = np.ascontiguousarray(beliefs, np.float64)
+    if beliefs.shape != (nodes.size, 2, H):
+        raise ValueError(f"beliefs must be [{nodes.size}, 2, {H}]")
+    return nodes, beliefs
+
+
+def fp_forest_check(num_dice, num_faces, depth, nodes, beliefs, iters):
+    """Host-only: the checks FpForest.solve makes before it touches the device (raises CfrbError with the reason)."""
+    nodes, beliefs = _forest_args(nodes, beliefs, num_faces ** num_dice)
+    _check(lib().cfrb_fp_forest_check(num_dice, num_faces, depth, nodes.size, _p(nodes, _ip), _p(beliefs, _dp), iters))
+
+
 def to_leaf_recursion_order(num_dice, num_faces, max_depth):
     """Host-only: (level_pos [R], level_begin [A + 1]) of the R subgame roots of a to-leaf walk: level_pos[k] is the position in
     the walk's level order of the k-th root in the reference's recursion order (the order of its act_iteration draws)."""
@@ -313,6 +341,50 @@ class FullGame:
         count = C.c_int64()
         _check(lib().cfrb_full_game_regrets(self._g, _p(imm, _dp), _p(sums, _dp), _p(node, _dp), C.byref(count)))
         return imm, sums, node, count.value
+
+
+class FpForest:
+    """Linear fictitious play without a value net on every full-tree subtree rooted at listed nodes of one depth, each root with
+    its own beliefs (cfrb_fp_forest_*): each root's root_value_means equal a one-subgame WaveSolver's rooted there, bit for bit,
+    for games of up to 23 actions.  Node ids are full-tree BFS ids (cfrb_unroll_tree's order)."""
+
+    def __init__(self, num_dice, num_faces, device=0):
+        self._f = C.c_void_p()
+        _check(lib().cfrb_fp_forest_create(num_dice, num_faces, device, C.byref(self._f)))
+        self.D, self.F, self.H = num_dice, num_faces, num_faces ** num_dice
+
+    def close(self):
+        if self._f:
+            lib().cfrb_fp_forest_destroy(self._f)
+            self._f = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def solve(self, depth, nodes, beliefs, iters):
+        """root_value_means [n, 2, H] of the roots `nodes` (strictly ascending, all at `depth`, non-terminal) with beliefs
+        [n, 2, H] after `iters` iterations."""
+        nodes, beliefs = _forest_args(nodes, beliefs, self.H)
+        out = np.zeros((nodes.size, 2, self.H))
+        _check(lib().cfrb_fp_forest_solve(self._f, depth, nodes.size, _p(nodes, _ip), _p(beliefs, _dp), iters, _p(out, _dp)))
+        return out
+
+    def reach(self, strategy, nodes):
+        """(node_reach [n], reach rows [n, 2, H]) of a compact full-tree strategy [N - 1, H] at the strictly ascending `nodes`."""
+        s = np.ascontiguousarray(strategy, np.float64)
+        nodes = np.ascontiguousarray(nodes, np.int32).reshape(-1)
+        nr, rows = np.zeros(nodes.size), np.zeros((nodes.size, 2, self.H))
+        _check(lib().cfrb_fp_forest_reach(self._f, _p(s, _dp), nodes.size, _p(nodes, _ip), _p(nr, _dp), _p(rows, _dp)))
+        return nr, rows
+
+    def memory(self):
+        """(bytes the object took on the device, the part its handle took)."""
+        tot, hnd = C.c_int64(), C.c_int64()
+        _check(lib().cfrb_fp_forest_memory(self._f, C.byref(tot), C.byref(hnd)))
+        return tot.value, hnd.value
 
 
 class WaveSolver:

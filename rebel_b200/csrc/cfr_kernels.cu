@@ -14,6 +14,7 @@
 #include "expl_sampled_kernels.cuh"
 #include "full_game_kernels.cuh"
 #include "regret_grid_kernels.cuh"
+#include "fp_forest_kernels.cuh"
 
 namespace cfrb {
 
@@ -223,6 +224,33 @@ void full_game_launch_iter(const FullGameDev& p, const int* level_begin, int lev
   for (int d = levels - 2; d >= 0; --d) fg_up_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
   for (int d = 0; d + 1 < levels; ++d) fg_down_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
   fg_advance_kernel<<<1, 1, 0, st>>>(p.iter);
+}
+// FP subtree forest from level d0 (fp_forest_kernels.cuh): the full-game solver's launches on levels d0 .. levels - 1.
+void fp_forest_launch_init(const FullGameDev& p, const double* bel, double* mu, const int* level_begin, int levels, int d0, int max_blocks,
+                           cudaStream_t st) {
+  const int nb = level_begin[d0], ne = level_begin[d0 + 1];
+  ff_root_init_kernel<<<fg_blocks((long long)(ne - nb) * p.H, max_blocks), 256, 0, st>>>(p, bel, mu, nb, ne);
+  for (int d = d0 + 1; d < levels; ++d)
+    fg_init_kernel<<<fg_blocks((long long)(level_begin[d + 1] - level_begin[d]) * p.H, max_blocks), 256, 0, st>>>(p, level_begin[d],
+                                                                                                               level_begin[d + 1], d);
+}
+void fp_forest_launch_iter(const FullGameDev& p, const double* bel, double* mu, const int* level_begin, int levels, int d0, int max_blocks,
+                           cudaStream_t st) {
+  auto blocks = [&](int d) { return fg_blocks((long long)(level_begin[d + 1] - level_begin[d]) * p.H, max_blocks); };
+  const int nb = level_begin[d0], ne = level_begin[d0 + 1];
+  ff_root_reach_kernel<<<blocks(d0), 256, 0, st>>>(p, bel, nb, ne);
+  for (int d = d0 + 1; d < levels; ++d) fg_reach_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
+  fg_terminal_kernel<<<fg_blocks(p.T, max_blocks), 256, 0, st>>>(p);
+  for (int d = levels - 2; d >= d0; --d) fg_up_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
+  ff_root_mean_kernel<<<blocks(d0), 256, 0, st>>>(p, bel, mu, nb, ne);
+  for (int d = d0; d + 1 < levels; ++d) fg_down_kernel<<<blocks(d), 256, 0, st>>>(p, level_begin[d], level_begin[d + 1], d);
+  fg_advance_kernel<<<1, 1, 0, st>>>(p.iter);
+}
+void fp_forest_launch_reach(const RegretGridDev& p, const double* strategy, const int* nodes, int n, double* node_reach, double* rows,
+                            const int* level_begin, int levels, int max_blocks, cudaStream_t st) {
+  auto blocks = [&](int d) { return fg_blocks((long long)(level_begin[d + 1] - level_begin[d]) * p.H, max_blocks); };
+  for (int d = 1; d < levels; ++d) rg_reach_kernel<double><<<blocks(d), 256, 0, st>>>(p, strategy, level_begin[d], level_begin[d + 1], d);
+  ff_gather_kernel<<<fg_blocks(n, max_blocks), 256, 0, st>>>(p, nodes, n, node_reach, rows);
 }
 // Grid-wide immediate regrets: the same level-by-level grid sizes as the full-game solver.
 template <typename S>

@@ -349,6 +349,17 @@ void full_game_launch_init(const FullGameDev& p, const int* level_begin, int lev
 void full_game_launch_iter(const FullGameDev& p, const int* level_begin, int levels, int max_blocks, cudaStream_t st);
 // CFR's normalised sum into p.avg (FP: the host copies Sg)
 void full_game_launch_average(const FullGameDev& p, const int* depth, int untouched0, int untouched1, int max_blocks, cudaStream_t st);
+// FP subtree forest (fp_forest_kernels.cuh): linear FP on every full-tree subtree rooted at level d0, roots' beliefs and root value
+// means bel / mu [level_begin[d0 + 1] - level_begin[d0]][2][H].  init: the FP constructor of levels d0 .. levels - 1 (iteration
+// counter left alone); iter: one iteration, about 3 launches per level from d0 on, then the counter's increment.
+void fp_forest_launch_init(const FullGameDev& p, const double* bel, double* mu, const int* level_begin, int levels, int d0, int max_blocks,
+                           cudaStream_t st);
+void fp_forest_launch_iter(const FullGameDev& p, const double* bel, double* mu, const int* level_begin, int levels, int d0, int max_blocks,
+                           cudaStream_t st);
+// both players' reach of a compact strategy [N - 1][H] into p.reach0 / p.reach1, then node_reach [n] and rows [n][2][H] of the
+// device node list nodes [n]
+void fp_forest_launch_reach(const RegretGridDev& p, const double* strategy, const int* nodes, int n, double* node_reach, double* rows,
+                            const int* level_begin, int levels, int max_blocks, cudaStream_t st);
 // rows [ids[i]] of a [*, width] fp32 matrix -> out[i]  (replay sampling)
 void rows_launch_gather(const float* src, int width, const int* ids, int n, float* out, cudaStream_t st);
 

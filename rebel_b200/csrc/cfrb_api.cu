@@ -2498,6 +2498,193 @@ int cfrb_full_game_memory(const cfrb_full_game* g, int64_t* total_bytes, int64_t
   return CFRB_OK;
 }
 
+// ============================================================================================ FP subtree forest
+// An FP full-game object (linear, its tables, full tree and stream) whose solves start at one level of the tree; the roots' beliefs
+// and running means of the largest level, and the CUDA graph of one iteration per root depth.
+struct cfrb_fp_forest {
+  cfrb_full_game fg;
+  DevBuf<double> bel, mu;
+  GraphExec graphs[CFRB_TO_LEAF_MAX_ACTIONS + 1];
+  int64_t total_bytes = 0;
+};
+
+// the most nodes one depth of the full tree holds: A - 1 at depth 1, C(A, d) at depth d >= 2
+static int64_t forest_level_cap(const cfrb::GameShape& g) {
+  int64_t cap = g.A - 1;
+  for (int d = 2; d <= g.A; ++d) cap = std::max(cap, binom(g.A, d));
+  return cap;
+}
+
+static int64_t fp_forest_bytes(const cfrb::GameShape& g) {
+  return full_game_bytes(g, true) + 2 * forest_level_cap(g) * 2 * g.H * 8;
+}
+
+static int forest_refuse_game(int32_t num_dice, int32_t num_faces, const char* who) {
+  if (num_dice < 1 || num_faces < 1) return fail(CFRB_EINVAL, std::string(who) + ": num_dice, num_faces must be >= 1");
+  const int64_t A = 2L * num_dice * num_faces + 1;
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, std::string(who) + ": games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                                 " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+  return CFRB_OK;
+}
+
+int64_t cfrb_fp_forest_bytes(int32_t num_dice, int32_t num_faces) {
+  if (int rc = forest_refuse_game(num_dice, num_faces, "cfrb_fp_forest_bytes")) return rc;
+  return fp_forest_bytes(cfrb::GameShape(num_dice, num_faces));
+}
+
+// The host checks of a forest solve, against the full tree t; nothing on a device is touched.
+static int forest_validate(const cfrb::TreeTemplate& t, const cfrb::GameShape& g, int32_t depth, int32_t n, const int32_t* nodes,
+                           const double* beliefs, int32_t iters, const char* who) {
+  const std::string w(who);
+  if (!nodes || !beliefs) return fail(CFRB_EINVAL, w + ": null argument");
+  if (depth < 1 || depth > g.A - 1) return fail(CFRB_EINVAL, w + ": depth must be in [1, A - 1] = [1, " + std::to_string(g.A - 1) + "]");
+  if (n < 1) return fail(CFRB_EINVAL, w + ": n must be >= 1");
+  if (iters < 1) return fail(CFRB_EINVAL, w + ": iters must be >= 1");
+  const int nb = t.level_begin[depth], ne = t.level_begin[depth + 1];
+  for (int i = 0; i < n; ++i) {
+    const int v = nodes[i];
+    if (v < 0 || v >= t.N) return fail(CFRB_EINVAL, w + ": node " + std::to_string(v) + " out of range");
+    if (i > 0 && v <= nodes[i - 1]) return fail(CFRB_EINVAL, w + ": nodes must be strictly ascending");
+    if (v < nb || v >= ne) return fail(CFRB_EINVAL, w + ": node " + std::to_string(v) + " is not at depth " + std::to_string(depth));
+    if (t.last_bid[v] == g.liar) return fail(CFRB_EINVAL, w + ": node " + std::to_string(v) + " is terminal");
+    for (int p = 0; p < 2; ++p) {
+      const double* b = beliefs + ((size_t)i * 2 + p) * g.H;
+      double sum = 0;
+      for (int h = 0; h < g.H; ++h) {
+        if (!std::isfinite(b[h]) || b[h] < 0)
+          return fail(CFRB_EINVAL, w + ": beliefs of node " + std::to_string(v) + " must be finite and non-negative");
+        sum += b[h];
+      }
+      if (!(sum > 0)) return fail(CFRB_EINVAL, w + ": a belief row of node " + std::to_string(v) + " sums to zero");
+    }
+  }
+  return CFRB_OK;
+}
+
+int cfrb_fp_forest_check(int32_t num_dice, int32_t num_faces, int32_t depth, int32_t n, const int32_t* nodes, const double* beliefs,
+                         int32_t iters) {
+  if (int rc = forest_refuse_game(num_dice, num_faces, "cfrb_fp_forest_check")) return rc;
+  const cfrb::GameShape g(num_dice, num_faces);
+  return forest_validate(cfrb::build_template(g, -1, 1 << 30), g, depth, n, nodes, beliefs, iters, "cfrb_fp_forest_check");
+}
+
+static int fp_forest_create_impl(int32_t num_dice, int32_t num_faces, int32_t device, cfrb_fp_forest* f) {
+  if (int rc = forest_refuse_game(num_dice, num_faces, "cfrb_fp_forest_create")) return rc;
+  if (cfrb_device_count() == 0) return fail(CFRB_ENODEV, "no CUDA device visible: libcfrb200 has no CPU fallback");
+  if (device < 0 || device >= cfrb_device_count()) return fail(CFRB_EINVAL, "device ordinal out of range");
+  CK(cudaSetDevice(device));
+  const cfrb::GameShape g(num_dice, num_faces);
+  // refused before anything is allocated, as cfrb_full_game_create is (and under the same test cap)
+  const int64_t need = fp_forest_bytes(g);
+  size_t free0 = 0, total = 0;
+  CK(cudaMemGetInfo(&free0, &total));
+  const int64_t avail = g_full_game_free_cap > 0 ? std::min<int64_t>((int64_t)free0, g_full_game_free_cap) : (int64_t)free0;
+  if (need > avail)
+    return fail(CFRB_ENOMEM, "cfrb_fp_forest_create: needs " + std::to_string(need) + " bytes of device memory beyond the handle, " +
+                                 std::to_string(avail) + " free");
+  cfrb_config c{};
+  c.num_dice = num_dice; c.num_faces = num_faces; c.device = device; c.solver = CFRB_SOLVER_FP; c.linear_update = 1;
+  c.state_dtype = CFRB_STATE_F64;   // eval_net's solves: linear FP, no value net (stats.cc:118-124)
+  if (int rc = full_game_create_impl(&c, &f->fg)) return rc;
+  const size_t cap = (size_t)forest_level_cap(g) * 2 * g.H;
+  CK(f->bel.alloc(cap)); CK(f->mu.alloc(cap));
+  size_t free1 = 0;
+  CK(cudaMemGetInfo(&free1, &total));
+  f->total_bytes = (int64_t)free0 - (int64_t)free1;
+  return CFRB_OK;
+}
+
+int cfrb_fp_forest_create(int32_t num_dice, int32_t num_faces, int32_t device, cfrb_fp_forest** out) {
+  if (!out) return fail(CFRB_EINVAL, "cfrb_fp_forest_create: null argument");
+  *out = nullptr;
+  auto f = std::make_unique<cfrb_fp_forest>();
+  const int rc = fp_forest_create_impl(num_dice, num_faces, device, f.get());
+  if (rc) return rc;
+  *out = f.release();
+  return CFRB_OK;
+}
+
+int cfrb_fp_forest_destroy(cfrb_fp_forest* f) {
+  if (!f) return CFRB_OK;
+  cudaSetDevice(f->fg.h ? f->fg.h->cfg.device : 0);
+  delete f;
+  return CFRB_OK;
+}
+
+int cfrb_fp_forest_memory(const cfrb_fp_forest* f, int64_t* total_bytes, int64_t* handle_bytes) {
+  if (!f) return fail(CFRB_EINVAL, "null forest");
+  if (total_bytes) *total_bytes = f->total_bytes;
+  if (handle_bytes) *handle_bytes = f->fg.handle_bytes;
+  return CFRB_OK;
+}
+
+int cfrb_fp_forest_solve(cfrb_fp_forest* f, int32_t depth, int32_t n, const int32_t* nodes, const double* beliefs, int32_t iters,
+                         double* root_means) {
+  if (!f || !root_means) return fail(CFRB_EINVAL, "cfrb_fp_forest_solve: null argument");
+  cfrb_handle* h = f->fg.h;
+  const auto& g = h->g;
+  const auto& t = h->br.t;
+  if (int rc = forest_validate(t, g, depth, n, nodes, beliefs, iters, "cfrb_fp_forest_solve")) return rc;
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t st = h->own_stream;
+  const int H = g.H, nb = t.level_begin[depth], ne = t.level_begin[depth + 1];
+  // every root of the level: the listed ones with their beliefs, the others uniform (finite and independent of the listed ones)
+  std::vector<double> bel((size_t)(ne - nb) * 2 * H, 1.0 / H);
+  for (int i = 0; i < n; ++i) std::copy(beliefs + (size_t)i * 2 * H, beliefs + (size_t)(i + 1) * 2 * H, bel.begin() + (size_t)(nodes[i] - nb) * 2 * H);
+  CK(cudaMemcpyAsync(f->bel.p, bel.data(), bel.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(f->fg.iter.p, 0, sizeof(int), st));
+  const int blocks = 8 * h->num_sms;
+  cfrb::fp_forest_launch_init(f->fg.dev, f->bel.p, f->mu.p, t.level_begin.data(), t.levels, depth, blocks, st);
+  CK(cudaGetLastError());
+  GraphExec& ge = f->graphs[depth];
+  if (!ge) {   // one iteration from this depth, captured once: its level launches replay without host launch cost
+    CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    cfrb::fp_forest_launch_iter(f->fg.dev, f->bel.p, f->mu.p, t.level_begin.data(), t.levels, depth, blocks, st);
+    Graph graph;
+    const cudaError_t launched = cudaGetLastError();
+    CK(cudaStreamEndCapture(st, graph.put()));
+    CK(launched);
+    CK(cudaGraphInstantiate(ge.put(), graph, 0));
+  }
+  for (int i = 0; i < iters; ++i) CK(cudaGraphLaunch(ge, st));
+  // the means of the listed roots' span of the level
+  const int lo = nodes[0] - nb, hi = nodes[n - 1] - nb + 1;
+  std::vector<double> mu((size_t)(hi - lo) * 2 * H);
+  CK(cudaMemcpyAsync(mu.data(), f->mu.p + (size_t)lo * 2 * H, mu.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i)
+    std::copy(mu.begin() + (size_t)(nodes[i] - nb - lo) * 2 * H, mu.begin() + (size_t)(nodes[i] - nb - lo + 1) * 2 * H,
+              root_means + (size_t)i * 2 * H);
+  return CFRB_OK;
+}
+
+int cfrb_fp_forest_reach(cfrb_fp_forest* f, const double* strategy, int32_t n, const int32_t* nodes, double* node_reach, double* rows) {
+  if (!f || !strategy || !nodes || !node_reach || !rows) return fail(CFRB_EINVAL, "cfrb_fp_forest_reach: null argument");
+  cfrb_handle* h = f->fg.h;
+  const auto& t = h->br.t;
+  const int H = h->g.H;
+  if (n < 1) return fail(CFRB_EINVAL, "cfrb_fp_forest_reach: n must be >= 1");
+  for (int i = 0; i < n; ++i) {
+    if (nodes[i] < 0 || nodes[i] >= t.N) return fail(CFRB_EINVAL, "cfrb_fp_forest_reach: node " + std::to_string(nodes[i]) + " out of range");
+    if (i > 0 && nodes[i] <= nodes[i - 1]) return fail(CFRB_EINVAL, "cfrb_fp_forest_reach: nodes must be strictly ascending");
+  }
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t st = h->own_stream;
+  DevBuf<int> dn;
+  DevBuf<double> out;
+  CK(dn.alloc(n)); CK(out.alloc((size_t)n * (1 + 2 * H)));
+  CK(cudaMemcpyAsync(h->br.strategy.p, strategy, (size_t)(t.N - 1) * H * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(dn.p, nodes, n * sizeof(int), cudaMemcpyHostToDevice, st));
+  cfrb::fp_forest_launch_reach(regret_grid_dev(h, nullptr), h->br.strategy.p, dn.p, n, out.p, out.p + n, t.level_begin.data(), t.levels,
+                               8 * h->num_sms, st);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(node_reach, out.p, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rows, out.p + n, (size_t)n * 2 * H * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return CFRB_OK;
+}
+
 // ============================================================================================ device-resident self-play
 int cfrb_selfplay_create(cfrb_handle* h, int32_t n_games, const uint32_t* seeds, float random_action_prob, int32_t sample_leaf) {
   if (!h || !seeds) return fail(CFRB_EINVAL, "null argument");

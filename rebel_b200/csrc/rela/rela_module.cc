@@ -352,8 +352,77 @@ float compute_exploitability_with_net(RecursiveSolvingParams params, const std::
 
 // compute_stats_with_net (pybind.cc:57-84): exploitability of compute_strategy_recursive_to_leaf with the net, and eval_net's MSE
 // of the net against full-depth solves, with the beliefs defined by the net strategy and by the full-tree strategy.
-std::tuple<float, float, float> compute_stats_with_net(RecursiveSolvingParams params, const std::string& model_path) {
+//
+// device_walk (None: above 2^20 full-tree nodes, where the dense [N][H][A] strategies are not built) takes the same numbers and
+// printed lines without a dense table, for games up to CFRB_TO_LEAF_MAX_ACTIONS actions: the to-leaf walk and its best response
+// on the device (cfrb_to_leaf_exploitability), the full-tree solve on the full-game solver, the candidates' reach statistics and
+// each depth's root solves on an FP forest (cfrb_fp_forest_*).  The phases run one after another, each freeing its device memory.
+std::tuple<float, float, float> compute_stats_device(RecursiveSolvingParams params, const std::string& model_path) {
+  params.net_mode = liars_dice::env_int("CFRB_EVAL_NET_MODE", CFRB_NET_FP32);   // the reference evaluates a checkpoint with an fp32 forward
+  const int device = eval_device(), A = 2 * params.num_dice * params.num_faces + 1;
+  PhaseTimer pt;
+  auto model = torch::jit::load(model_path, torch::kCPU);
+  model.eval();
+  pt.lap("load model");
+  int N = 0, H = 0;
+  std::vector<double> net_strategy, full_strategy;   // compact [N - 1][H]
+  float exploitability = 0;
+  {
+    const HandlePtr h = open_handle(liars_dice::solver_config(params, device, 8192));
+    const std::vector<float> w = flat_weights_of(model);
+    check(cfrb_set_weights(h.get(), w.data(), w.size(), 1), "cfrb_set_weights");
+    pt.lap("create evaluator");
+    std::array<double, 2> e{};
+    double secs[2] = {0, 0};
+    check(cfrb_to_leaf_exploitability(h.get(), e.data(), nullptr, nullptr, secs), "cfrb_to_leaf_exploitability");
+    exploitability = (float)((e[0] + e[1]) / 2.0);
+    N = check(cfrb_full_tree_nodes(h.get()), "cfrb_full_tree_nodes");
+    H = cfrb_num_hands(h.get());
+    net_strategy.resize((size_t)(N - 1) * H);
+    check(cfrb_to_leaf_strategy(h.get(), net_strategy.data()), "cfrb_to_leaf_strategy");
+    if (pt.on) std::fprintf(stderr, "[rebel_b200] %-28s %.3f s\n[rebel_b200] %-28s %.3f s\n", "  to-leaf walk", secs[0], "  best response", secs[1]);
+    pt.lap("strategy to leaf");
+  }
+  {
+    cfrb_config c = liars_dice::solver_config(params, device, 1);
+    c.net_mode = CFRB_NET_ZERO;
+    cfrb_full_game* raw = nullptr;
+    check(cfrb_full_game_create(&c, &raw), "cfrb_full_game_create");
+    const FullGamePtr fg(raw);
+    pt.lap("create full-game solver");
+    check(cfrb_full_game_step(fg.get(), params.subgame_params.num_iters), "cfrb_full_game_step");
+    full_strategy.resize((size_t)(N - 1) * H);
+    check(cfrb_full_game_strategy(fg.get(), full_strategy.data()), "cfrb_full_game_strategy");
+    pt.lap("full-game solve");
+  }
+  std::vector<cfrb_node> tree(N);
+  if (cfrb_unroll_tree(params.num_dice, params.num_faces, -1, 0, 1 << 30, tree.data(), N) != N) throw std::runtime_error(cfrb_last_error());
+  cfrb_fp_forest* raw = nullptr;
+  check(cfrb_fp_forest_create(params.num_dice, params.num_faces, device, &raw), "cfrb_fp_forest_create");
+  const FpForestPtr forest(raw);
+  pt.lap("create forest");
+  const EvalNetCandidates cand = forest_candidates(forest.get(), tree, A, H, params.subgame_params.max_depth, net_strategy, full_strategy);
+  pt.lap("reach statistics");
+  auto after = [&](int depth, size_t roots) {
+    pt.lap(("  forest depth " + std::to_string(depth) + ", " + std::to_string(roots) + " roots").c_str());
+  };
+  const RootSolve solve = forest_root_solve(forest.get(), tree, H, params.subgame_params.num_iters, after);
+  float mse[2];
+  for (int k = 0; k < 2; ++k) {
+    mse[k] = eval_net_scored(params, tree, cand, model, /*traverse_by_net=*/k == 0, /*verbose=*/true, solve);
+    pt.lap(k == 0 ? "eval_net rest (net beliefs)" : "eval_net rest (full beliefs)");
+  }
+  return std::make_tuple(exploitability, mse[0], mse[1]);
+}
+
+std::tuple<float, float, float> compute_stats_with_net(RecursiveSolvingParams params, const std::string& model_path, py::object device_walk) {
+  const int A = 2 * params.num_dice * params.num_faces + 1;
+  const bool on_device = device_walk.is_none() ? ((int64_t)1 << A) - 1 > ((int64_t)1 << 20) : device_walk.cast<bool>();
+  if (on_device && A > CFRB_TO_LEAF_MAX_ACTIONS)   // the library's own refusal, before a device is touched
+    throw std::runtime_error("compute_stats_with_net: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                             " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
   py::gil_scoped_release nogil;
+  if (on_device) return compute_stats_device(params, model_path);
   params.net_mode = liars_dice::env_int("CFRB_EVAL_NET_MODE", CFRB_NET_FP32);   // the reference evaluates a checkpoint with an fp32 forward
   PhaseTimer pt;
   auto model = torch::jit::load(model_path, torch::kCPU);
@@ -1061,7 +1130,7 @@ PYBIND11_MODULE(rela, m) {
 
   m.def("compute_exploitability_fp", &compute_exploitability_fp, py::arg("params"));
   m.def("compute_exploitability_with_net", &compute_exploitability_with_net, py::arg("params"), py::arg("model_path"));
-  m.def("compute_stats_with_net", &compute_stats_with_net, py::arg("params"), py::arg("model_path"));
+  m.def("compute_stats_with_net", &compute_stats_with_net, py::arg("params"), py::arg("model_path"), py::arg("device_walk") = py::none());
   m.def("create_cfr_thread", &create_cfr_thread, py::arg("model_locker"), py::arg("replay"), py::arg("cfg"), py::arg("seed"));
   m.def("run_selfplay_waves", &run_selfplay_waves, py::arg("cfg"), py::arg("device"), py::arg("seed"), py::arg("waves"),
         py::arg("flat_weights") = py::none(),

@@ -11,7 +11,9 @@ is updated every epoch.  An epoch waits until num_add * train_gen_ratio >= train
 train_epoch_size / batch steps on a stream of its own while generation continues; the learning rate halves every 400 epochs, at
 most twice.  Every 10 epochs the run writes epoch{N}.ckpt (state_dict), epoch{N}.torchscript and epoch{N}.optim (the
 torch.optim.Adam state_dict layout) under --out and evaluates the validation snapshots (one every 100 epochs, from epoch 0); every
---exploit_every epochs it runs rela.compute_stats_with_net on games whose full tree that accepts.
+--exploit_every epochs it runs rela.compute_stats_with_net (exploitability, mse_net_reach, mse_fp_reach): on games of up to 23
+actions (2x5f, 5x2f, 1x10f and 1x11f included, whose evaluation runs without dense full-tree tables); above that the run says
+so once and stops evaluating.
 
 --deterministic replaces the threads by a fixed schedule, so that two runs with the same arguments print the same TRAIN lines
 (but for the wall-clock fields minutes and *_per_s) and write the same checkpoints.  There is one rela.SelfPlayGenerator per
