@@ -72,10 +72,15 @@ enum {
                              whose weights and two query tiles fit shared memory run the resident kernel; larger ones
                              (2x5f, 3x3f, 5x2f, 2x6f, 1x17f .. 1x32f) a kernel with the weights alone in shared memory;
                              cfrb_tc_net_supported() tells which games have one (CFRB_TC_WIDE=1 forces the second) */
-  CFRB_NET_TC_F16X2 = 3   /* same kernel with the fast GELU: y/2 (1 + tanh(poly)) with packed f32x2 FMAs and tanh.approx.f32, one
+  CFRB_NET_TC_F16X2 = 3,  /* same kernel with the fast GELU: y/2 (1 + tanh(poly)) with packed f32x2 FMAs and tanh.approx.f32, one
                              rounding to fp16 at the end (same accuracy as mode 2, 1 instead of 2 MUFU operations per element).
                              CFRB_X2_GELU=half selects the packed-fp16 evaluation (HFMA2 + tanh.approx.f16x2): 6 % faster, but
                              that instruction truncates towards zero and biases every activation (see DESIGN.md "P5") */
+  CFRB_NET_TC_CLUSTER = 4 /* wgmma tensor-core kernel on a cluster of two CTAs that split Net2's 256 hidden features and exchange
+                             LayerNorm sums and activations through distributed shared memory; mode 3's arithmetic (fp32 tanh
+                             GELU).  Serves the games whose weights do not fit one SM (2x7f, 3x4f, 6x2f, 4x3f, 7x2f, 2x8f .. 2x11f,
+                             3x5f, 1x33f .. 1x96f) and every game modes 2 and 3 serve; cfrb_tc_cluster_net_supported() tells which.
+                             CFRB_X2_GELU and CFRB_TC_WIDE do not apply */
 };
 
 /* Subgame solver.  In FP mode cfrb_fetch's "last" is FP::last_strategies (belief x best response), "avg" is
@@ -124,6 +129,10 @@ int cfrb_destroy(cfrb_handle* h);
 /* Host-only (no device needed): 1 if a tensor-core value net (CFRB_NET_TC_F16 / CFRB_NET_TC_F16X2) with `hidden` units fits the
  * game on an sm_90 device, else 0 (cfrb_create then fails with CFRB_EINVAL for those modes; CFRB_NET_FP32 serves every game). */
 int cfrb_tc_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden);
+/* Host-only: 1 if the two-CTA cluster value net (CFRB_NET_TC_CLUSTER) with `hidden` units serves the game on an sm_90 device: hidden
+ * == 256, a game cfrb_create accepts, and one CTA's half of the weights plus its exchange buffers fit the 227 KB of shared memory
+ * a block may opt into.  Otherwise cfrb_create fails with CFRB_EINVAL for that mode. */
+int cfrb_tc_cluster_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden);
 
 /* Host-only: a bound B >= |output| of the tensor-core value net with these weights (cfrb_set_weights layout) over every query
  * row, +inf when none holds (a weight that is not finite); -1 for a bad shape or weight count.  The depth-2 CFR kernel leaves out of

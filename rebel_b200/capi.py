@@ -11,7 +11,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcfrb200.so")
 
-NET_ZERO, NET_FP32, NET_TC_F16, NET_TC_F16X2 = 0, 1, 2, 3
+NET_ZERO, NET_FP32, NET_TC_F16, NET_TC_F16X2, NET_TC_CLUSTER = 0, 1, 2, 3, 4
 SOLVER_CFR, SOLVER_FP = 0, 1
 STATE_F64, STATE_F32 = 0, 1
 
@@ -54,6 +54,7 @@ def lib():
         getattr(L, f).argtypes = [vp]
     L.cfrb_unroll_tree.argtypes = [C.c_int32] * 5 + [_ip, C.c_int32]
     L.cfrb_tc_net_supported.argtypes = [C.c_int32] * 3
+    L.cfrb_tc_cluster_net_supported.argtypes = [C.c_int32] * 3
     L.cfrb_tree_template.argtypes = [vp, C.c_int32, C.c_int32, _ip, C.c_int32]
     L.cfrb_set_weights.argtypes = [vp, _fp, C.c_size_t, C.c_uint64]
     L.cfrb_weights_version.argtypes = [vp]
@@ -279,6 +280,11 @@ def net_output_bound(num_dice, num_faces, flat, hidden=256):
 def tc_net_supported(num_dice, num_faces, hidden=256):
     """Host-only: does a tensor-core value net (NET_TC_F16 / NET_TC_F16X2) fit this game?  Otherwise NET_FP32 serves it."""
     return bool(lib().cfrb_tc_net_supported(num_dice, num_faces, hidden))
+
+
+def tc_cluster_net_supported(num_dice, num_faces, hidden=256):
+    """Host-only: does the two-CTA cluster value net (NET_TC_CLUSTER) serve this game?  Otherwise NET_FP32 serves it."""
+    return bool(lib().cfrb_tc_cluster_net_supported(num_dice, num_faces, hidden))
 
 
 class FullGame:

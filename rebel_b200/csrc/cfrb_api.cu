@@ -24,10 +24,13 @@
 #include "leaf_mlp_simt.cuh"
 #include "leaf_mlp_tc.cuh"
 #include "leaf_mlp_tc_wide.cuh"
+#include "leaf_mlp_tc_cluster.cuh"
 #include "train_kernels.cuh"
 
 namespace {
-inline bool is_tc(int net_mode) { return net_mode == CFRB_NET_TC_F16 || net_mode == CFRB_NET_TC_F16X2; }
+inline bool is_tc(int net_mode) {
+  return net_mode == CFRB_NET_TC_F16 || net_mode == CFRB_NET_TC_F16X2 || net_mode == CFRB_NET_TC_CLUSTER;
+}
 
 thread_local std::string g_err;
 
@@ -105,7 +108,9 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 // memory, at most 16 outputs) where it fits and is not overridden, else the wide kernel (leaf_mlp_tc_wide.cuh: weights only,
 // query fragments loaded from global memory, nout = roundup(H, 16) outputs).  Returns false when neither fits; `why` then
 // holds the byte arithmetic.  `smem_limit` is the device's opt-in shared memory per block.
-struct TcPlan { bool wide = false; int nout = cfrb::tc::kNout, smem_bytes = 0; };
+// cluster: the two-CTA kernel of CFRB_NET_TC_CLUSTER (leaf_mlp_tc_cluster.cuh) with nout = 2 nh outputs, smem_bytes per CTA and
+// at most max_clusters clusters resident at once (its persistent grid).
+struct TcPlan { bool wide = false, cluster = false; int nout = cfrb::tc::kNout, smem_bytes = 0, max_clusters = 0; };
 bool tc_plan(int H, int Qpad, int smem_limit, bool force_wide, TcPlan* plan, std::string* why) {
   const cfrb::tc::BlobLayout R(Qpad);
   if (!force_wide && H <= cfrb::tc::kNout && R.smem_bytes <= smem_limit) {
@@ -124,6 +129,25 @@ bool tc_plan(int H, int Qpad, int smem_limit, bool force_wide, TcPlan* plan, std
            std::to_string(Qpad) + " x 2 B + W2 131072 B + W3 " + std::to_string(nout) + " x 256 x 2 B + biases / LayerNorm " +
            std::to_string(W.blob_bytes - W.off_b2) + " B = " + std::to_string(W.smem_bytes) + " B of shared memory (with the "
            "mbarrier) > " + std::to_string(smem_limit) + " B per block; use CFRB_NET_FP32";
+  return false;
+}
+
+// The two-CTA cluster kernel (CFRB_NET_TC_CLUSTER): one CTA's half of the weights (ClusterLayout) and its exchange buffers must
+// fit `smem_limit`, with at most 64 output columns per CTA.  Returns false otherwise; `why` then holds the byte arithmetic.
+bool tc_cluster_plan(int H, int Qpad, int smem_limit, TcPlan* plan, std::string* why) {
+  const int nh = cfrb::tc::cluster_nh(H);
+  const cfrb::tc::ClusterLayout C(Qpad, nh);
+  if (nh <= 64 && C.smem_bytes <= smem_limit) {
+    plan->wide = false; plan->cluster = true; plan->nout = 2 * nh; plan->smem_bytes = C.smem_bytes;
+    return true;
+  }
+  if (why)
+    *why = "two-CTA cluster value net does not fit this game: num_hands " + std::to_string(H) + ", padded query width " +
+           std::to_string(Qpad) + ", output columns per CTA " + std::to_string(nh) + " (at most 64); per CTA W1 128 x " +
+           std::to_string(Qpad) + " x 2 B + W2 65536 B + W3 " + std::to_string(nh) + " x 256 x 2 B + biases / LayerNorm " +
+           std::to_string(C.blob_bytes - C.off_b2) + " B + exchange buffers " + std::to_string(C.off_bar - C.off_xa) + " B = " +
+           std::to_string(C.smem_bytes) + " B of shared memory (with the mbarriers) > " + std::to_string(smem_limit) +
+           " B per block; use CFRB_NET_FP32";
   return false;
 }
 
@@ -615,7 +639,7 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   CK(cudaSetDevice(cfg->device));
   if (cfg->num_dice < 1 || cfg->num_faces < 1 || cfg->max_depth < 1 || cfg->max_subgames < 1)
     return fail(CFRB_EINVAL, "num_dice, num_faces, max_depth, max_subgames must be >= 1");
-  if (cfg->net_mode < CFRB_NET_ZERO || cfg->net_mode > CFRB_NET_TC_F16X2) return fail(CFRB_EINVAL, "bad net_mode");
+  if (cfg->net_mode < CFRB_NET_ZERO || cfg->net_mode > CFRB_NET_TC_CLUSTER) return fail(CFRB_EINVAL, "bad net_mode");
   if (cfg->state_dtype != CFRB_STATE_F64 && cfg->state_dtype != CFRB_STATE_F32) return fail(CFRB_EINVAL, "bad state_dtype");
   if (cfg->solver != CFRB_SOLVER_CFR && cfg->solver != CFRB_SOLVER_FP) return fail(CFRB_EINVAL, "bad solver");
   if (cfg->net_mode != CFRB_NET_ZERO && cfg->hidden != 256) return fail(CFRB_EINVAL, "only hidden == 256 is built");
@@ -626,6 +650,11 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   if (cfg->num_dice > cfrb::kMaxDice)
     return fail(CFRB_EINVAL, "game too large: " + std::to_string(cfg->num_dice) + " dice per player; the terminal payoff histogram "
                              "holds 9 bins, so at most 7 dice per player");
+  if (cfg->net_mode == CFRB_NET_TC_CLUSTER) {   // refused before anything is allocated
+    std::string why;
+    TcPlan plan;
+    if (!tc_cluster_plan(g.H, round_up(g.Q + 1, 16), cfrb::tc::kSmemOptinSm90, &plan, &why)) return fail(CFRB_EINVAL, why);
+  }
   // ---- templates: root_bid in {-1, 0 .. A-2}
   std::vector<TemplateDev> td;
   std::vector<int> parent, child_begin, nchild, last_bid, level_begin, pleaf_node, term_node;
@@ -732,7 +761,11 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
     // CFRB_TC_WIDE=1: the wide kernel also on games the resident kernel serves (tests, measurements)
     const char* fw = std::getenv("CFRB_TC_WIDE");
     std::string why;
-    if (!tc_plan(g.H, h->Qpad, max_optin, fw && *fw == '1', &h->tc, &why)) return fail(CFRB_EINVAL, why);
+    if (cfg->net_mode == CFRB_NET_TC_CLUSTER) {
+      if (!tc_cluster_plan(g.H, h->Qpad, max_optin, &h->tc, &why)) return fail(CFRB_EINVAL, why);
+    } else if (!tc_plan(g.H, h->Qpad, max_optin, fw && *fw == '1', &h->tc, &why)) {
+      return fail(CFRB_EINVAL, why);
+    }
     const size_t tiles = (rows_cap + cfrb::tc::kTileM - 1) / cfrb::tc::kTileM;
     CK(h->d_Xh.alloc(tiles * cfrb::tc::kTileM * h->Qpad));
     CK(cudaMemset(h->d_Xh.p, 0, tiles * cfrb::tc::kTileM * h->Qpad * sizeof(__half)));
@@ -745,7 +778,11 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
     CK(h->d_dbg.alloc(2 * cfrb::tc::kTileM * cfrb::tc::kHid));
     // the limit is per kernel and process-wide: raised to the device's opt-in maximum (see cfr_configure in cfr_kernels.cu)
     const int sm = std::max(h->tc.smem_bytes, max_optin);
-    if (h->tc.wide) {
+    if (h->tc.cluster) {
+      CK(cfrb::tc::cluster_configure(h->tc.nout / 2, sm, &h->tc.max_clusters));
+      if (h->tc.max_clusters < 1) return fail(CFRB_ECUDA, "no cluster of two CTAs with " + std::to_string(h->tc.smem_bytes) +
+                                                          " B of shared memory each fits the device");
+    } else if (h->tc.wide) {
       CK(cfrb::tc::wide_configure(h->tc.nout, sm));
     } else {
       CK(cudaFuncSetAttribute(cfrb::tc::leaf_mlp_tc_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
@@ -785,6 +822,16 @@ int cfrb_tc_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden) {
   const cfrb::GameShape g(num_dice, num_faces);
   TcPlan plan;
   return tc_plan(g.H, round_up(g.Q + 1, 16), cfrb::tc::kSmemOptinSm90, false, &plan, nullptr) ? 1 : 0;
+}
+
+int cfrb_tc_cluster_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden) {
+  if (num_dice < 1 || num_faces < 1 || hidden != 256) return 0;
+  long hands = 1;
+  for (int i = 0; i < num_dice && hands <= 4096; ++i) hands *= num_faces;
+  if (hands > 4096 || 2L * num_dice * num_faces + 1 > 1024 || num_dice > cfrb::kMaxDice) return 0;   // beyond what cfrb_create accepts at all
+  const cfrb::GameShape g(num_dice, num_faces);
+  TcPlan plan;
+  return tc_cluster_plan(g.H, round_up(g.Q + 1, 16), cfrb::tc::kSmemOptinSm90, &plan, nullptr) ? 1 : 0;
 }
 
 int cfrb_debug_kernel_path(const cfrb_handle* h) {
@@ -842,7 +889,12 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
   const size_t total_fp32 = (size_t)Qp * hid + 3 * hid + (size_t)hid * hid + 3 * hid + (size_t)hid * h->Hout + h->Hout;
   // tensor-core blob: the resident kernel's layout, or the wide kernel's (W3 with tc.nout rows); with 16 outputs the two agree
   const cfrb::tc::WideLayout L(Qp, h->tc.nout);
-  const size_t bound_off = ((size_t)L.blob_bytes + 7) / 8 * 8;     // the output bound is staged behind the blob
+  // the cluster kernel's blob: CTA 0's half, then CTA 1's, each in ClusterLayout (hidden features / output columns split in two)
+  const bool cl = h->tc.cluster;
+  const int nh = h->tc.nout / 2;
+  const cfrb::tc::ClusterLayout C(Qp, nh);
+  const size_t blob_bytes = cl ? 2 * (size_t)C.blob_bytes : (size_t)L.blob_bytes;
+  const size_t bound_off = (blob_bytes + 7) / 8 * 8;     // the output bound is staged behind the blob
   const size_t need = is_tc(h->cfg.net_mode) ? bound_off + sizeof(double) : total_fp32 * sizeof(float);
   if (h->w_stage_bytes < need) {
     CK(cudaStreamSynchronize(h->own_stream));
@@ -862,6 +914,23 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
     __half* hw1 = reinterpret_cast<__half*>(blob.data() + L.off_w1);
     __half* hw2 = reinterpret_cast<__half*>(blob.data() + L.off_w2);
     __half* hw3 = reinterpret_cast<__half*>(blob.data() + L.off_w3);
+    // where hidden feature j / output column j and its parameters go: the one blob, or the half of the CTA that holds it
+    auto cta = [&](int j, int per) { return blob.data() + (size_t)(j / per) * C.blob_bytes; };
+    auto w1_at = [&](int j, int k) -> __half& {
+      if (cl) return reinterpret_cast<__half*>(cta(j, 128) + C.off_w1)[cfrb::tc::umma_kmajor_offset_halves(j % 128, k, 128)];
+      return hw1[cfrb::tc::umma_kmajor_offset_halves(j, k, hid)];
+    };
+    auto w2_at = [&](int j, int k) -> __half& {
+      if (cl) return reinterpret_cast<__half*>(cta(j, 128) + C.off_w2)[cfrb::tc::umma_kmajor_offset_halves(j % 128, k, 128)];
+      return hw2[cfrb::tc::umma_kmajor_offset_halves(j, k, hid)];
+    };
+    auto w3_at = [&](int j, int k) -> __half& {
+      if (cl) return reinterpret_cast<__half*>(cta(j, nh) + C.off_w3)[cfrb::tc::umma_kmajor_offset_halves(j % nh, k, nh)];
+      return hw3[cfrb::tc::umma_kmajor_offset_halves(j, k, h->tc.nout)];
+    };
+    auto param = [&](int j, int per, int off_cl, int off, int stride) -> float* {   // stride floats per feature
+      return cl ? reinterpret_cast<float*>(cta(j, per) + off_cl) + (j % per) * stride : reinterpret_cast<float*>(blob.data() + off) + j * stride;
+    };
     // LayerNorm without the mean (leaf_mlp_tc.cuh).  Subtracting from every column of W (and from the bias) its
     // mean over the 256 output features makes the features of y = W x + b sum to zero for every x, which is all the mean
     // subtraction of LayerNorm does; the epilogue then only needs sum y^2.  Done in double, before the fp16 rounding.
@@ -872,25 +941,26 @@ int cfrb_set_weights(cfrb_handle* h, const float* flat, size_t n, uint64_t versi
     for (int k = 0; k < hid; ++k) { for (int j = 0; j < hid; ++j) m2[k] += w2[(size_t)j * hid + k]; m2[k] /= hid; }
     for (int j = 0; j < hid; ++j) m2[hid] += b2[j];
     m2[hid] /= hid;
-    for (int j = 0; j < hid; ++j) for (int k = 0; k < Q; ++k) hw1[cfrb::tc::umma_kmajor_offset_halves(j, k, hid)] = __float2half_rn((float)(w1[(size_t)j * Q + k] - m1[k]));
-    for (int j = 0; j < hid; ++j) hw1[cfrb::tc::umma_kmajor_offset_halves(j, Q, hid)] = __float2half_rn((float)(b1[j] - m1[Q]));   // bias 1 x constant-1 column
-    float* fb2 = reinterpret_cast<float*>(blob.data() + L.off_b2);      // bias 2, rounded to fp16 like bias 1 in W1
-    for (int j = 0; j < hid; ++j) fb2[j] = __half2float(__float2half_rn((float)(b2[j] - m2[hid])));
-    for (int j = 0; j < hid; ++j) for (int k = 0; k < hid; ++k) hw2[cfrb::tc::umma_kmajor_offset_halves(j, k, hid)] = __float2half_rn((float)(w2[(size_t)j * hid + k] - m2[k]));
-    for (int j = 0; j < H; ++j) for (int k = 0; k < hid; ++k) hw3[cfrb::tc::umma_kmajor_offset_halves(j, k, h->tc.nout)] = __float2half_rn(w3[(size_t)j * hid + k]);
-    float* ln1 = reinterpret_cast<float*>(blob.data() + L.off_ln1);
-    float* ln2 = reinterpret_cast<float*>(blob.data() + L.off_ln2);
-    // the GELU of CFRB_NET_TC_F16X2 evaluates the activation from y / 2: gamma / 2 and beta / 2 are stored
-    const float lnscale = h->cfg.net_mode == CFRB_NET_TC_F16X2 ? 0.5f : 1.f;
-    for (int j = 0; j < hid; ++j) {
+    for (int j = 0; j < hid; ++j) for (int k = 0; k < Q; ++k) w1_at(j, k) = __float2half_rn((float)(w1[(size_t)j * Q + k] - m1[k]));
+    for (int j = 0; j < hid; ++j) w1_at(j, Q) = __float2half_rn((float)(b1[j] - m1[Q]));   // bias 1 x constant-1 column
+    // bias 2, rounded to fp16 like bias 1 in W1
+    for (int j = 0; j < hid; ++j) *param(j, 128, C.off_b2, L.off_b2, 1) = __half2float(__float2half_rn((float)(b2[j] - m2[hid])));
+    for (int j = 0; j < hid; ++j) for (int k = 0; k < hid; ++k) w2_at(j, k) = __float2half_rn((float)(w2[(size_t)j * hid + k] - m2[k]));
+    for (int j = 0; j < H; ++j) for (int k = 0; k < hid; ++k) w3_at(j, k) = __float2half_rn(w3[(size_t)j * hid + k]);
+    // the GELU of CFRB_NET_TC_F16X2 (and of CFRB_NET_TC_CLUSTER) evaluates the activation from y / 2: gamma / 2 and beta / 2 are stored
+    const float lnscale = h->cfg.net_mode == CFRB_NET_TC_F16X2 || cl ? 0.5f : 1.f;
+    for (int j = 0; j < hid; j += 2) {
       // per feature pair (j even): {gamma_j, gamma_j+1, beta_j, beta_j+1}: one 16-byte load per column pair of the epilogue
-      const int o = (j >> 1) * 4 + (j & 1);
-      ln1[o] = lnscale * g1[j]; ln1[o + 2] = lnscale * be1[j];
-      ln2[o] = lnscale * g2[j]; ln2[o + 2] = lnscale * be2[j];
+      float* ln1 = param(j, 128, C.off_ln1, L.off_ln1, 2);
+      float* ln2 = param(j, 128, C.off_ln2, L.off_ln2, 2);
+      for (int e = 0; e < 2; ++e) {
+        ln1[e] = lnscale * g1[j + e]; ln1[e + 2] = lnscale * be1[j + e];
+        ln2[e] = lnscale * g2[j + e]; ln2[e + 2] = lnscale * be2[j + e];
+      }
     }
-    std::copy(b3, b3 + H, reinterpret_cast<float*>(blob.data() + L.off_b3));
-    if (!h->d_blob.p) CK(h->d_blob.alloc(L.blob_bytes));
-    CK(cudaMemcpyAsync(h->d_blob.p, blob.data(), L.blob_bytes, cudaMemcpyHostToDevice, h->own_stream));
+    for (int j = 0; j < H; ++j) *param(j, cl ? nh : H, C.off_b3, L.off_b3, 1) = b3[j];
+    if (!h->d_blob.p) CK(h->d_blob.alloc(blob_bytes));
+    CK(cudaMemcpyAsync(h->d_blob.p, blob.data(), blob_bytes, cudaMemcpyHostToDevice, h->own_stream));
     double* bound = reinterpret_cast<double*>(blob.data() + bound_off);
     *bound = h->skip_dead ? net_output_bound(flat, Q, H, hid) : std::numeric_limits<double>::infinity();
     CK(cudaMemcpyAsync(h->d_net_bound.p, bound, sizeof(double), cudaMemcpyHostToDevice, h->own_stream));
@@ -1022,7 +1092,17 @@ static int launch_net(cfrb_handle* h, cudaStream_t st, const NetIo& io, float* d
     at[0].val.programmaticStreamSerializationAllowed = 1;
     lc.attrs = at; lc.numAttrs = dbg ? 0 : 1;
     const int gelu = x2 ? h->x2_gelu : 0;
-    if (h->tc.wide) CK(cfrb::tc::wide_launch(lc, a, h->tc.nout, gelu, dbg));
+    if (h->tc.cluster) {
+      // persistent grid of whole clusters (surplus clusters return as a pair); cluster i takes tiles i, i + clusters, ...
+      const int clusters = (h->capturing || h->rows_on_device) ? h->tc.max_clusters : std::min(tiles, h->tc.max_clusters);
+      lc.gridDim = dim3(cfrb::tc::kClusterCtas * std::max(clusters, 1));
+      cudaLaunchAttribute cat[2];
+      cat[0] = at[0];
+      cat[1].id = cudaLaunchAttributeClusterDimension;
+      cat[1].val.clusterDim.x = cfrb::tc::kClusterCtas; cat[1].val.clusterDim.y = 1; cat[1].val.clusterDim.z = 1;
+      lc.attrs = cat; lc.numAttrs = 2;
+      CK(cfrb::tc::cluster_launch(lc, a, h->tc.nout / 2));
+    } else if (h->tc.wide) CK(cfrb::tc::wide_launch(lc, a, h->tc.nout, gelu, dbg));
     else if (dbg && gelu == 1) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 1>, a));
     else if (dbg && gelu == 2) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 2>, a));
     else if (dbg) CK(cudaLaunchKernelEx(&lc, cfrb::tc::leaf_mlp_tc_kernel<true, 0>, a));
@@ -1345,6 +1425,7 @@ int cfrb_debug_leaf_io(cfrb_handle* h, float* queries, float* net_out, double* s
 
 int cfrb_debug_net_trace(cfrb_handle* h, long long* out, int n) {
   if (!h || !is_tc(h->cfg.net_mode)) return fail(CFRB_EINVAL, "trace exists only for the tensor-core value net");
+  if (h->tc.cluster) return fail(CFRB_EINVAL, "the cluster value net (CFRB_NET_TC_CLUSTER) has no trace build");
   if (!h->have_weights || h->rows == 0) return fail(CFRB_ESTATE, "no weights or no leaf rows");
   if (n < 2048) return fail(CFRB_EINVAL, "trace buffer must hold 2048 stamps");
   CK(cudaSetDevice(h->cfg.device));
@@ -1368,6 +1449,7 @@ int cfrb_debug_net_trace(cfrb_handle* h, long long* out, int n) {
 
 int cfrb_debug_net_taps(cfrb_handle* h, float* d1, float* d2) {
   if (!h || !is_tc(h->cfg.net_mode)) return fail(CFRB_EINVAL, "taps exist only for the tensor-core value net");
+  if (h->tc.cluster) return fail(CFRB_EINVAL, "the cluster value net (CFRB_NET_TC_CLUSTER) has no layer taps");
   if (!h->have_weights || h->rows == 0) return fail(CFRB_ESTATE, "no weights or no leaf rows");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaDeviceSynchronize());

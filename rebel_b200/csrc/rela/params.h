@@ -41,8 +41,10 @@ struct RecursiveSolvingParams {
 };
 
 // A tensor-core net mode falls back to the fp32 SIMT net only on games whose Net2 weights do not fit a tensor-core kernel
-// (cfrb_tc_net_supported: 2x7f, 3x4f, 6x2f, 2x8f, one-die games from 1x33f on, ...).
+// (cfrb_tc_net_supported: 2x7f, 3x4f, 6x2f, 2x8f, one-die games from 1x33f on, ...).  Mode 4 (CFRB_NET_TC_CLUSTER, opt-in) runs
+// the two-CTA cluster kernel wherever cfrb_tc_cluster_net_supported holds, which includes those games, and the fp32 net elsewhere.
 inline int effective_net_mode(const RecursiveSolvingParams& p) {
+  if (p.net_mode == CFRB_NET_TC_CLUSTER) return cfrb_tc_cluster_net_supported(p.num_dice, p.num_faces, 256) ? p.net_mode : 1;
   return (p.net_mode >= 2 && !cfrb_tc_net_supported(p.num_dice, p.num_faces, 256)) ? 1 : p.net_mode;
 }
 

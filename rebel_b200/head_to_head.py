@@ -33,7 +33,8 @@ def build_parser():
     ap.add_argument("--cfr_b", choices=("yes", "no"), default=None, help="agent B's solver (default: as agent A)")
     ap.add_argument("--no_linear", action="store_true")
     ap.add_argument("--dcfr", type=float, nargs=3, metavar=("ALPHA", "BETA", "GAMMA"), default=None)
-    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast GELU (default 3 with a net)")
+    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast GELU (default 3 with a net), "
+                    "4 wgmma on two-CTA clusters with mode 3's GELU (also games too large for modes 2 and 3; the fp32 net where it does not fit)")
     ap.add_argument("--concurrent_games", type=int, default=8192)
     ap.add_argument("--device", type=int, default=0)
     return ap

@@ -31,7 +31,8 @@ def build_parser():
     ap.add_argument("--cfr", action="store_true", help="the agent solves with CFR instead of fictitious play")
     ap.add_argument("--no_linear", action="store_true")
     ap.add_argument("--dcfr", type=float, nargs=3, metavar=("ALPHA", "BETA", "GAMMA"), default=None)
-    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast GELU (default 3 with a net)")
+    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast GELU (default 3 with a net), "
+                    "4 wgmma on two-CTA clusters with mode 3's GELU (also games too large for modes 2 and 3; the fp32 net where it does not fit)")
     ap.add_argument("--concurrent_games", type=int, default=8192)
     ap.add_argument("--max_subgames", type=int, default=0, help="subgames solved per round (0: 2 x concurrent_games, at least A - 1)")
     ap.add_argument("--device", type=int, default=0)

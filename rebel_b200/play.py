@@ -30,8 +30,11 @@ def build_parser():
                     help="sampled: ReBeL's random-iteration policy; average: the average strategy of all iterations")
     ap.add_argument("--games", type=int, default=1)
     ap.add_argument("--seed", type=int, default=0, help="seeds the deals and the agent's draws")
+    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast GELU (default 3 with a "
+                    "net), 4 wgmma on two-CTA clusters with mode 3's GELU (also games too large for modes 2 and 3; the fp32 net where it does "
+                    "not fit)")
     # agent_params' other settings, at head_to_head's defaults
-    ap.set_defaults(net_mode=None, no_linear=False, dcfr=None, device=0)
+    ap.set_defaults(no_linear=False, dcfr=None, device=0)
     return ap
 
 

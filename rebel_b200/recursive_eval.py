@@ -137,7 +137,8 @@ def build_parser():
     ap.add_argument("--batch_repeats", type=int, default=None,
                     help="repeats walked together (default: 64 on the host walk; enough to fill a wave, at most 64, on the device walk)")
     ap.add_argument("--wave_capacity", type=int, default=8192)
-    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast fp32-tanh GELU (default with --net)")
+    ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast fp32-tanh GELU (default with --net), "
+                    "4 wgmma on two-CTA clusters with mode 3's GELU (also games too large for modes 2 and 3; the fp32 net where it does not fit)")
     ap.add_argument("--random_net_seed", type=int, default=None, help="use a random-init Net2 (benchmarks)")
     ap.add_argument("--full_game", action="store_true",
                     help="solve the full game over the whole GPU (rela.solve_full_game) and walk the repeats on the device (implies "
