@@ -340,6 +340,11 @@ int cfrb_full_game_strategy(cfrb_full_game* g, double* compact);
 int cfrb_full_game_memory(const cfrb_full_game* g, int64_t* total_bytes, int64_t* handle_bytes);
 /* Test aid: cfrb_full_game_create sees at most `bytes` free device bytes (0 = the device's own figure); process-wide. */
 int cfrb_debug_full_game_free_cap(int64_t bytes);
+/* Test aid, process-wide: with byte in 0..255, every later floating-point device buffer (fp64, fp32, fp16) the library allocates
+ * for a handle or another object is filled with that byte (cudaMemset, then a device-wide synchronise) before it is used, so a
+ * result that depends on what fresh device memory held shows up as a difference.  Integer and struct buffers (indices, templates,
+ * counters) are never filled.  -1 = off (the default).  Any other value: CFRB_EINVAL, before any device work. */
+int cfrb_debug_fill_allocations(int32_t byte);
 /* Immediate regrets of the full-game solve (CFR only, as the reference's full-tree solve tracks them): after
  * cfrb_full_game_track_regrets, cfrb_full_game_step adds the sampling strategy after every iteration with an even index to compact
  * fp64 sums [N - 1][H] (entry (child - 1) * H + hand), computed over the whole device.  The sums, immediate regrets and count are

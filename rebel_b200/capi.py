@@ -94,6 +94,7 @@ def lib():
     L.cfrb_full_game_strategy.argtypes = [vp, _dp]
     L.cfrb_full_game_memory.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.cfrb_debug_full_game_free_cap.argtypes = [C.c_int64]
+    L.cfrb_debug_fill_allocations.argtypes = [C.c_int32]
     L.cfrb_full_game_track_regrets.argtypes = [vp]
     L.cfrb_to_leaf_sampled_ev_regrets.argtypes = ([vp] + [C.c_int32] * 4 + [_ip, _dp, _dp, _dp, C.c_int32, C.c_int32, _dp, _dp, _dp]
                                                   + [C.POINTER(C.c_int64)] * 3 + [_dp])

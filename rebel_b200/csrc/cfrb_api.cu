@@ -47,6 +47,10 @@ int fail(int code, const std::string& msg) {
                                   std::to_string(__LINE__));                                       \
   } while (0)
 
+// Test aid (cfrb_debug_fill_allocations), process-wide: -1 = off, 0..255 = the byte every floating-point DevBuf is filled with
+// when it is allocated.
+int g_fill_byte = -1;
+
 // Device memory of `n` elements, freed with its owner.  alloc() frees what the buffer held before.
 template <class T>
 struct DevBuf {
@@ -64,9 +68,18 @@ struct DevBuf {
   cudaError_t alloc(size_t count) {
     free();
     const cudaError_t e = cudaMalloc((void**)&p, std::max<size_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) n = count;
-    else p = nullptr;
-    return e;
+    if (e != cudaSuccess) { p = nullptr; return e; }
+    n = count;
+    // Only floating-point buffers: a garbage value there can change results, which is what the aid looks for; a garbage index or
+    // count could send a kernel out of bounds.  No DevBuf is allocated while a stream is captured (the captured regions only
+    // enqueue kernels), so the synchronise cannot break a capture.
+    if constexpr (std::is_same_v<T, float> || std::is_same_v<T, double> || std::is_same_v<T, __half>) {
+      if (g_fill_byte >= 0) {
+        const cudaError_t f = cudaMemset(p, g_fill_byte, std::max<size_t>(count, 1) * sizeof(T));
+        return f != cudaSuccess ? f : cudaDeviceSynchronize();
+      }
+    }
+    return cudaSuccess;
   }
 
  private:
@@ -801,6 +814,10 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   if (rc) return rc;
   CK(cudaStreamCreateWithFlags(h->own_stream.put(), cudaStreamNonBlocking));
   CK(cudaEventCreate(h->ev_a.put())); CK(cudaEventCreate(h->ev_b.put()));
+  // The memsets above (S, Snap, vterm, scaler, the net's buffers) run on the legacy default stream, which orders nothing on
+  // own_stream (non-blocking) or on a caller's stream.  Without this wait the first cfr_init_kernel can write S before the memset
+  // of S has zeroed it (gigabytes for large waves), and FP's normalisation then divides 0 by 0.
+  CK(cudaDeviceSynchronize());
   return CFRB_OK;
 }
 
@@ -2375,6 +2392,12 @@ int64_t cfrb_full_game_bytes(int32_t num_dice, int32_t num_faces, int32_t solver
 int cfrb_debug_full_game_free_cap(int64_t bytes) {
   if (bytes < 0) return fail(CFRB_EINVAL, "cfrb_debug_full_game_free_cap: bad argument");
   g_full_game_free_cap = bytes;
+  return CFRB_OK;
+}
+
+int cfrb_debug_fill_allocations(int32_t byte) {
+  if (byte < -1 || byte > 255) return fail(CFRB_EINVAL, "cfrb_debug_fill_allocations: byte must be -1 (off) or 0..255");
+  g_fill_byte = byte;
   return CFRB_OK;
 }
 
