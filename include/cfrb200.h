@@ -251,11 +251,26 @@ int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgam
  * tree, its two compact strategies and the best-response scratch (none of which a handle that already holds its full tree
  * allocates again), and the walk's template map and two largest levels of roots and beliefs.  Games with A > 26: CFRB_EINVAL. */
 int64_t cfrb_to_leaf_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t max_subgames);
-/* Test aid: the compact full-tree strategy [N_full - 1][H] (entry (child - 1) * H + hand) the last cfrb_to_leaf_exploitability
- * filled. */
+/* Exploitability of the handle's every-node policy (compute_strategy_recursive, recursive_solving.cc:46-74: a subgame of depth
+ * max_depth solved for num_iters iterations at every non-terminal node of the full tree, acting with the average strategy of its
+ * root), with the handle's weights and solver settings, without a dense strategy: the 2^(A-1) subgames are solved level by level
+ * in waves of max_subgames (level d = the C(A - 1, d) non-terminal nodes at depth d, in full-tree order), their root rows written
+ * into the handle's compact full-tree strategy, each child's beliefs built on the device (the acting player's row times the child's
+ * strategy, eps-normalised; the other row unchanged), and both best responses taken on the strategy (compute_exploitability2).
+ * Outputs as cfrb_to_leaf_exploitability's, and refused like it: A > CFRB_TO_LEAF_MAX_ACTIONS, a handle in a live match or agent
+ * and null arguments (CFRB_EINVAL), missing weights (CFRB_ESTATE), and a cfrb_recursive_bytes need above the device's free memory
+ * (CFRB_ENOMEM, before anything is allocated).  Replaces the handle's wave. */
+int cfrb_recursive_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2);
+/* Host-only: device bytes cfrb_recursive_exploitability needs beyond the handle of this game: cfrb_to_leaf_bytes' full-tree part
+ * (none of which a handle that already holds its full tree allocates again) plus the walk, 2 Lmax (4 + 16 H) + 4 (two levels of
+ * roots and fp64 beliefs [2][H], Lmax = C(A - 1, floor((A - 1) / 2)), and a level counter); max_subgames does not enter it.  Games
+ * with A > 26: CFRB_EINVAL. */
+int64_t cfrb_recursive_bytes(int32_t num_dice, int32_t num_faces, int32_t max_subgames);
+/* Test aid: the compact full-tree strategy [N_full - 1][H] (entry (child - 1) * H + hand) that the last cfrb_to_leaf_exploitability
+ * or cfrb_recursive_exploitability, whichever ran last, filled. */
 int cfrb_to_leaf_strategy(cfrb_handle* h, double* compact);
-/* Test aid: cfrb_to_leaf_exploitability and cfrb_to_leaf_sampled see at most `bytes` free device bytes (0 = the device's own
- * figure). */
+/* Test aid: cfrb_to_leaf_exploitability, cfrb_recursive_exploitability and cfrb_to_leaf_sampled see at most `bytes` free device
+ * bytes (0 = the device's own figure). */
 int cfrb_debug_to_leaf_free_cap(cfrb_handle* h, int64_t bytes);
 /* recursive_eval's sampled evaluation on the device, for games up to CFRB_TO_LEAF_MAX_ACTIONS: the float32 reach-weighted average
  * of num_repeats sampled recursive strategies (strategy ids seed0 .. seed0 + num_repeats - 1) and its exploitability at every

@@ -76,6 +76,9 @@ def lib():
     L.cfrb_to_leaf_bytes.argtypes = [C.c_int32] * 4
     L.cfrb_to_leaf_bytes.restype = C.c_int64
     L.cfrb_to_leaf_strategy.argtypes = [vp, _dp]
+    L.cfrb_recursive_exploitability.argtypes = [vp, _dp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _dp]
+    L.cfrb_recursive_bytes.argtypes = [C.c_int32] * 3
+    L.cfrb_recursive_bytes.restype = C.c_int64
     L.cfrb_debug_to_leaf_free_cap.argtypes = [vp, C.c_int64]
     L.cfrb_to_leaf_sampled.argtypes = [vp] + [C.c_int32] * 4 + [_ip, _dp, _dp, _dp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _dp]
     L.cfrb_to_leaf_sampled_bytes.argtypes = [C.c_int32] * 5
@@ -211,6 +214,12 @@ def to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames):
     """Host-only: device bytes WaveSolver.to_leaf_exploitability needs beyond a handle of these sizes (full tree, best-response
     scratch, the walk's largest levels)."""
     return _check(lib().cfrb_to_leaf_bytes(num_dice, num_faces, max_depth, max_subgames))
+
+
+def recursive_bytes(num_dice, num_faces, max_subgames):
+    """Host-only: device bytes WaveSolver.recursive_exploitability needs beyond a handle of these sizes (to_leaf_bytes' full tree
+    and best-response scratch, two of the largest depth levels of roots and beliefs, a level counter)."""
+    return _check(lib().cfrb_recursive_bytes(num_dice, num_faces, max_subgames))
 
 
 def to_leaf_sampled_bytes(num_dice, num_faces, max_depth, max_subgames, batch_repeats):
@@ -525,8 +534,19 @@ class WaveSolver:
         return {"br": br, "exploitability": (br[0] + br[1]) / 2, "subgames": sg.value, "subgame_iters": it.value,
                 "walk_seconds": float(secs[0]), "br_seconds": float(secs[1])}
 
+    def recursive_exploitability(self):
+        """Exploitability of the every-node policy of this handle (compute_strategy_recursive: a subgame solved at every
+        non-terminal node, acting with its root's average strategy), walked depth by depth in waves of max_subgames on the device:
+        dict as to_leaf_exploitability's.  Replaces the handle's wave."""
+        br, secs = np.zeros(2, np.float64), np.zeros(2, np.float64)
+        sg, it = C.c_int64(0), C.c_int64(0)
+        _check(lib().cfrb_recursive_exploitability(self._h, _p(br, _dp), C.byref(sg), C.byref(it), _p(secs, _dp)))
+        return {"br": br, "exploitability": (br[0] + br[1]) / 2, "subgames": sg.value, "subgame_iters": it.value,
+                "walk_seconds": float(secs[0]), "br_seconds": float(secs[1])}
+
     def to_leaf_strategy(self):
-        """The compact full-tree strategy [N_full - 1, H] the last to_leaf_exploitability filled (entry [child - 1, hand])."""
+        """The compact full-tree strategy [N_full - 1, H] (entry [child - 1, hand]) that the last to_leaf_exploitability or
+        recursive_exploitability, whichever ran last, filled."""
         n = (1 << self.A) - 1                    # the full Liar's Dice tree
         out = np.zeros((max(n - 1, 1), self.H), np.float64)
         _check(lib().cfrb_to_leaf_strategy(self._h, _p(out, _dp)))
@@ -588,7 +608,8 @@ class WaveSolver:
         return s, act
 
     def debug_to_leaf_free_cap(self, nbytes):
-        """Test aid: to_leaf_exploitability and to_leaf_sampled see at most nbytes free device bytes (0 = the device's own figure)."""
+        """Test aid: to_leaf_exploitability, recursive_exploitability and to_leaf_sampled see at most nbytes free device bytes (0 =
+        the device's own figure)."""
         _check(lib().cfrb_debug_to_leaf_free_cap(self._h, int(nbytes)))
 
     @property

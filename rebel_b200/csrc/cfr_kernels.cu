@@ -192,6 +192,10 @@ void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalis
   expl_fill_kernel<<<1, 1, 0, st>>>(p);
 }
 template <typename real>
+void rec_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st) {
+  rec_expand_kernel<real><<<(n + 3) / 4, 128, 0, st>>>(p, n, table, normalise);   // a warp per subgame
+}
+template <typename real>
 void expl_sampled_launch_begin(const ExplSampledDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st) {
   expl_sampled_begin_kernel<real><<<(n + 127) / 128, 128, 0, st>>>(p, n, wave_beliefs);
   sp_scan_kernel<<<1, 1024, 0, st>>>(scan);
@@ -330,6 +334,7 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void agent_launch_capture<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);                         \
   template void expl_launch_begin<real>(const ExplDev&, const SpDev&, int, real*, cudaStream_t);                           \
   template void expl_launch_expand<real>(const ExplDev&, int, const real*, int, cudaStream_t);                              \
+  template void rec_launch_expand<real>(const ExplDev&, int, const real*, int, cudaStream_t);                               \
   template void expl_sampled_launch_begin<real>(const ExplSampledDev&, const SpDev&, int, real*, cudaStream_t);           \
   template void expl_sampled_launch_expand<real>(const ExplSampledDev&, int, const real*, cudaStream_t);
 CFRB_INSTANTIATE(float)

@@ -267,11 +267,15 @@ struct ExplDev {
   int* fill;
   int cap;
   int* fid; int nmax;                 // [K][nmax] scratch: full-tree node of every template node of each subgame
+  // the every-node walk (rec_expand_kernel): the full tree's child counts [N] and depth levels [levels + 1]
+  const int* full_nchild; const int* full_level_begin;
 };
 // wave descriptors (template, player, root beliefs as `real`), row offsets and schedule of the level's subgames off .. off + n - 1
 template <typename real> void expl_launch_begin(const ExplDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st);
 // the solved wave's strategy into p.strategy, its pseudo-leaves onto the next level
 template <typename real> void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
+// every-node walk: the solved wave's root rows into p.strategy, their non-terminal children onto the next level
+template <typename real> void rec_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
 // Sampled recursive to-leaf walk (expl_sampled_kernels.cuh): the waves of one level of a batch of b repeats.  A level lists its
 // root groups in full-tree node order, each group the b repeats of one root in repeat order, so level position pos is repeat
 // pos % b of group pos / b.

@@ -1845,29 +1845,77 @@ int cfrb_debug_to_leaf_free_cap(cfrb_handle* h, int64_t bytes) {
   return CFRB_OK;
 }
 
-int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2) {
-  if (!h || !br_out2) return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: null argument");
+// Refusals shared by the device walks, in this order: more than CFRB_TO_LEAF_MAX_ACTIONS actions, a handle in a live match or
+// agent, a net without weights, and a need above the free bytes -- all before anything is allocated, since on a shared device an
+// allocation that fails late may starve other processes.  Then the full tree (full_tree_setup).
+static int walk_admit(cfrb_handle* h, const char* who, int64_t tree_bytes, int64_t walk_bytes) {
   const auto& g = h->g;
+  const std::string w(who);
   if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
-    return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+    return fail(CFRB_EINVAL, w + ": games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
                                  " actions are not supported (A = " + std::to_string(g.A) + ": the full tree has 2^A - 1 nodes)");
-  if (h->in_match) return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: the handle plays in a live match or agent");
+  if (h->in_match) return fail(CFRB_EINVAL, w + ": the handle plays in a live match or agent");
   if (h->cfg.net_mode != CFRB_NET_ZERO && !h->have_weights && h->Lmax > 0)
-    return fail(CFRB_ESTATE, "cfrb_to_leaf_exploitability: value-net weights not set (cfrb_set_weights)");
+    return fail(CFRB_ESTATE, w + ": value-net weights not set (cfrb_set_weights)");
   CK(cudaSetDevice(h->cfg.device));
-  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H;
-  const auto sz = to_leaf_sizes(g, h->cfg.max_depth, K);
-  // refused before anything is allocated: on a shared device an allocation that fails late may starve other processes
-  const int64_t need = (h->br.ready ? 0 : sz.tree_bytes) + sz.walk_bytes;
+  const int64_t tree = h->br.ready ? 0 : tree_bytes, need = tree + walk_bytes;
   size_t free_b = 0, total_b = 0;
   CK(cudaMemGetInfo(&free_b, &total_b));
   int64_t avail = (int64_t)free_b;
   if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
   if (need > avail)
-    return fail(CFRB_ENOMEM, "cfrb_to_leaf_exploitability: needs " + std::to_string(need) + " bytes of device memory beyond the "
-                             "handle (full tree and best-response scratch " + std::to_string(h->br.ready ? 0 : sz.tree_bytes) +
-                             ", walk " + std::to_string(sz.walk_bytes) + "), " + std::to_string(avail) + " free");
-  int rc = full_tree_setup(h, "cfrb_to_leaf_exploitability");
+    return fail(CFRB_ENOMEM, w + ": needs " + std::to_string(need) + " bytes of device memory beyond the handle (full tree and "
+                             "best-response scratch " + std::to_string(tree) + ", walk " + std::to_string(walk_bytes) + "), " +
+                             std::to_string(avail) + " free");
+  return full_tree_setup(h, who);
+}
+
+// The walks' view of the handle: its full tree, compact strategy, templates and wave descriptors (ExplDev), and sp_scan_kernel's
+// view of the wave.
+static cfrb::ExplDev walk_dev(cfrb_handle* h) {
+  cfrb::ExplDev d{};
+  d.H = h->g.H;
+  d.full_child_begin = h->br.child_begin.p; d.full_depth = h->br.depth.p; d.full_act_lo = h->br.act_lo.p; d.strategy = h->br.strategy.p;
+  d.full_nchild = h->br.nchild.p; d.full_level_begin = h->br.level_begin.p;
+  d.tmpl = h->d_tmpl.p; d.parent = h->d_parent.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p;
+  d.level_begin = h->d_level_begin.p; d.pleaf_node = h->d_pleaf_node.p;
+  d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_act = h->d_sg_act.p; d.sg_row_off = h->d_sg_row_off.p;
+  d.wave = h->d_wave.p; d.steps = h->d_steps.p; d.table_stride = h->table_stride;
+  return d;
+}
+static cfrb::SpDev walk_scan(cfrb_handle* h) {
+  cfrb::SpDev scan{};
+  scan.A = h->g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
+  scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
+  return scan;
+}
+
+// Both best responses on the walk's compact strategy, and the walks' outputs.  t0: the walk's start; the walk ends here.
+static int walk_finish(cfrb_handle* h, std::chrono::steady_clock::time_point t0, int64_t solved, double* br_out2, int64_t* subgames,
+                       int64_t* subgame_iters, double* seconds2) {
+  cudaStream_t st = h->own_stream;
+  const auto t1 = std::chrono::steady_clock::now();
+  cfrb::br_launch(full_tree_dev(h), st);
+  ++h->launches;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(br_out2, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const auto t2 = std::chrono::steady_clock::now();
+  if (subgames) *subgames = solved;
+  if (subgame_iters) *subgame_iters = solved * h->cfg.num_iters;
+  if (seconds2) {
+    seconds2[0] = std::chrono::duration<double>(t1 - t0).count();
+    seconds2[1] = std::chrono::duration<double>(t2 - t1).count();
+  }
+  return CFRB_OK;
+}
+
+int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2) {
+  if (!h || !br_out2) return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: null argument");
+  const auto& g = h->g;
+  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H;
+  const auto sz = to_leaf_sizes(g, h->cfg.max_depth, K);
+  int rc = walk_admit(h, "cfrb_to_leaf_exploitability", sz.tree_bytes, sz.walk_bytes);
   if (rc) return rc;
   cudaStream_t st = h->own_stream;
   DevBuf<int> roots[2], fid, fill;
@@ -1879,17 +1927,9 @@ int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgam
   const int root = 0;
   CK(cudaMemcpyAsync(roots[0].p, &root, sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(bel[0].p, uniform.data(), W * sizeof(double), cudaMemcpyHostToDevice, st));
-  cfrb::ExplDev d{};
-  d.H = H;
-  d.full_child_begin = h->br.child_begin.p; d.full_depth = h->br.depth.p; d.full_act_lo = h->br.act_lo.p; d.strategy = h->br.strategy.p;
-  d.tmpl = h->d_tmpl.p; d.parent = h->d_parent.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p;
-  d.level_begin = h->d_level_begin.p; d.pleaf_node = h->d_pleaf_node.p;
-  d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_act = h->d_sg_act.p; d.sg_row_off = h->d_sg_row_off.p;
-  d.wave = h->d_wave.p; d.steps = h->d_steps.p; d.table_stride = h->table_stride;
+  cfrb::ExplDev d = walk_dev(h);
   d.fill = fill.p; d.cap = (int)sz.level_cap; d.fid = fid.p; d.nmax = h->Nmax;
-  cfrb::SpDev scan{};   // sp_scan_kernel's view of the wave
-  scan.A = g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
-  scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
+  cfrb::SpDev scan = walk_scan(h);
   int64_t solved = 0;
   int cur = 0, n_level = 1;
   for (int depth = 0; n_level > 0; depth += h->cfg.max_depth) {
@@ -1919,25 +1959,80 @@ int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgam
     n_level = next;
     cur ^= 1;
   }
-  const auto t1 = std::chrono::steady_clock::now();
-  cfrb::br_launch(full_tree_dev(h), st);
-  ++h->launches;
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(br_out2, h->br.out.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  const auto t2 = std::chrono::steady_clock::now();
-  if (subgames) *subgames = solved;
-  if (subgame_iters) *subgame_iters = solved * h->cfg.num_iters;
-  if (seconds2) {
-    seconds2[0] = std::chrono::duration<double>(t1 - t0).count();
-    seconds2[1] = std::chrono::duration<double>(t2 - t1).count();
+  return walk_finish(h, t0, solved, br_out2, subgames, subgame_iters, seconds2);
+}
+
+// ============================================================================================ every-node exploitability
+// Sizes of the every-node walk: the to-leaf walk's full tree and best-response scratch, two levels of roots and fp64 beliefs [2][H]
+// as large as the largest depth level, C(A - 1, floor((A - 1) / 2)) non-terminal nodes, and the level counter.
+static int64_t recursive_walk_bytes(const cfrb::GameShape& g) {
+  const int64_t lmax = binom(g.A - 1, (g.A - 1) / 2);
+  return 2 * lmax * (4 + 16 * (int64_t)g.H) + 4;
+}
+
+int64_t cfrb_recursive_bytes(int32_t num_dice, int32_t num_faces, int32_t max_subgames) {
+  if (num_dice < 1 || num_faces < 1 || max_subgames < 1)
+    return fail(CFRB_EINVAL, "cfrb_recursive_bytes: num_dice, num_faces, max_subgames must be >= 1");
+  if (2L * num_dice * num_faces + 1 > 26) return fail(CFRB_EINVAL, "cfrb_recursive_bytes: full tree too large (2^A - 1 nodes, A > 26)");
+  const cfrb::GameShape g(num_dice, num_faces);
+  return to_leaf_sizes(g, 1, 1).tree_bytes + recursive_walk_bytes(g);
+}
+
+int cfrb_recursive_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2) {
+  if (!h || !br_out2) return fail(CFRB_EINVAL, "cfrb_recursive_exploitability: null argument");
+  const auto& g = h->g;
+  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H;
+  const int64_t lmax = binom(g.A - 1, (g.A - 1) / 2);
+  int rc = walk_admit(h, "cfrb_recursive_exploitability", to_leaf_sizes(g, 1, 1).tree_bytes, recursive_walk_bytes(g));
+  if (rc) return rc;
+  cudaStream_t st = h->own_stream;
+  DevBuf<int> roots[2], fill;
+  DevBuf<double> bel[2];
+  for (int i = 0; i < 2; ++i) { CK(roots[i].alloc(lmax)); CK(bel[i].alloc((size_t)lmax * W)); }
+  CK(fill.alloc(1));
+  const auto t0 = std::chrono::steady_clock::now();
+  const std::vector<double> uniform(W, 1.0 / H);   // level 0: the game root with uniform beliefs
+  const int root = 0;
+  CK(cudaMemcpyAsync(roots[0].p, &root, sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(bel[0].p, uniform.data(), W * sizeof(double), cudaMemcpyHostToDevice, st));
+  cfrb::ExplDev d = walk_dev(h);
+  d.fill = fill.p; d.cap = (int)lmax;
+  cfrb::SpDev scan = walk_scan(h);
+  int64_t solved = 0;
+  int cur = 0, n_level = 1;
+  for (int depth = 0; n_level > 0; ++depth) {
+    d.roots = roots[cur].p; d.bel = bel[cur].p; d.next_roots = roots[cur ^ 1].p; d.next_bel = bel[cur ^ 1].p;
+    CK(cudaMemsetAsync(fill.p, 0, sizeof(int), st));
+    for (int off = 0; off < n_level; off += K) {
+      const int n = std::min(K, n_level - off);
+      d.off = off; scan.K = n;
+      with_state(h, [&](auto& s) { cfrb::expl_launch_begin(d, scan, n, s.beliefs.p, st); });
+      h->launches += 2;
+      CK(cudaGetLastError());
+      if ((rc = solve_device_wave(h, n, true, false, st))) return rc;
+      with_state(h, [&](auto& s) {
+        const auto avg = avg_table(h, s);
+        cfrb::rec_launch_expand(d, n, avg.p, avg.normalise ? 1 : 0, st);
+      });
+      ++h->launches;
+      CK(cudaGetLastError());
+    }
+    solved += n_level;
+    int next = 0;
+    CK(cudaMemcpyAsync(&next, fill.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (next != binom(g.A - 1, depth + 1))
+      return fail(CFRB_ECUDA, "cfrb_recursive_exploitability: level at depth " + std::to_string(depth + 1) + " has " +
+                                  std::to_string(next) + " subgames, the tree " + std::to_string(binom(g.A - 1, depth + 1)));
+    n_level = next;
+    cur ^= 1;
   }
-  return CFRB_OK;
+  return walk_finish(h, t0, solved, br_out2, subgames, subgame_iters, seconds2);
 }
 
 int cfrb_to_leaf_strategy(cfrb_handle* h, double* compact) {
   if (!h || !compact) return fail(CFRB_EINVAL, "cfrb_to_leaf_strategy: null argument");
-  if (!h->br.ready) return fail(CFRB_ESTATE, "cfrb_to_leaf_strategy: the handle holds no full-tree strategy (run cfrb_to_leaf_exploitability)");
+  if (!h->br.ready) return fail(CFRB_ESTATE, "cfrb_to_leaf_strategy: the handle holds no full-tree strategy (run cfrb_to_leaf_exploitability or cfrb_recursive_exploitability)");
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaStreamSynchronize(h->own_stream));
   CK(cudaMemcpy(compact, h->br.strategy.p, h->br.strategy.n * sizeof(double), cudaMemcpyDeviceToHost));

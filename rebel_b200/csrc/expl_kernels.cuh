@@ -104,4 +104,58 @@ __global__ void __launch_bounds__(128) expl_expand_kernel(ExplDev p, const real*
 
 __global__ void expl_fill_kernel(ExplDev p) { *p.fill += p.wave[1]; }
 
+// Every-node walk (cfrb_recursive_exploitability): compute_strategy_recursive (recursive_solving.cc:46-74, as
+// RecursiveEvaluator::strategyRecursive runs it on the host).  Level d holds the non-terminal full-tree nodes of depth d, in full-tree
+// order; each roots a depth-max_depth subgame, solved by expl_begin / sp_scan / the handle's solver like a to-leaf wave, of whose
+// average strategy only the root row is kept.  One warp per subgame of the wave:
+//   - the root row (CFR: the sum normalised as expl_expand_kernel does it; FP: Sg as it is) goes to the root's edges of the compact
+//     full-tree strategy;
+//   - every non-terminal child goes to the next level with the root's beliefs, the acting player's row multiplied by the child's
+//     strategy and eps-normalised (normalize_beliefs_inplace), the other row unchanged.  Only the acting row is renormalised, unlike
+//     the to-leaf walk's pseudo-leaves.
+// Every node below the game root has the liar call, which is terminal, as its last child, and the root has no call.  So a depth-d
+// node at level position i follows i call children in the full tree's depth d + 1, and its child c takes next-level slot
+// c - level_begin[d + 1] - i (at the root i = 0 and level_begin[1] = 1): the next level comes out in full-tree order without atomics.
+// fill only counts the children written, for the host's check of the level's size.
+template <typename real>
+__global__ void __launch_bounds__(128) rec_expand_kernel(ExplDev p, int n, const real* __restrict__ table, int normalise) {
+  const int k = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31, H = p.H;
+  if (k >= n) return;                          // whole warps
+  const int i = p.off + k, node = p.roots[i];
+  const int nc = p.full_nchild[node], cb = p.full_child_begin[node], pl = p.full_depth[node] & 1;
+  const real* tk = table + (size_t)k * p.table_stride;   // the template root's edges are its first nc rows
+  double* s = p.strategy + (size_t)(cb - 1) * H;
+  for (int h = lane; h < H; h += 32) {
+    if (normalise) {
+      const bool untouched = p.steps[2 * k + pl] == 0;
+      double sum = 0;
+      for (int j = 0; j < nc; ++j) sum += (double)tk[(size_t)j * H + h];
+      for (int j = 0; j < nc; ++j) {
+        const double v = (double)tk[(size_t)j * H + h];
+        s[(size_t)j * H + h] = (sum > 0 && !untouched) ? v / sum : 1.0 / nc;
+      }
+    } else {
+      for (int j = 0; j < nc; ++j) s[(size_t)j * H + h] = (double)tk[(size_t)j * H + h];
+    }
+  }
+  __syncwarp();
+  const int kids = node == 0 ? nc : nc - 1;
+  const int first = p.full_level_begin[p.full_depth[node] + 1] + i;
+  const double* rb = p.bel + (size_t)i * 2 * H;
+  for (int j = lane; j < kids; j += 32) {
+    const int slot = cb + j - first;
+    if (slot < 0 || slot >= p.cap) continue;   // cannot happen for a level sized by the host; the host checks the count
+    p.next_roots[slot] = cb + j;
+    double* ob = p.next_bel + (size_t)slot * 2 * H;
+    for (int x = 0; x < 2 * H; ++x) ob[x] = rb[x];
+    double* a = ob + (size_t)pl * H;
+    const double* sj = s + (size_t)j * H;
+    for (int h = 0; h < H; ++h) a[h] *= sj[h];
+    double sum = 0;
+    for (int h = 0; h < H; ++h) sum += a[h] + 1e-80;
+    for (int h = 0; h < H; ++h) a[h] = (a[h] + 1e-80) / sum;
+  }
+  if (lane == 0) atomicAdd(p.fill, kids);
+}
+
 }  // namespace cfrb

@@ -316,37 +316,72 @@ int eval_device() {
   return e && *e ? std::atoi(e) : 0;
 }
 
+// Refusal of the device walks' game size, before a device is touched (the library refuses it too, on a handle).
+void refuse_above_walk_limit(const RecursiveSolvingParams& cfg, const char* who) {
+  const int A = 2 * cfg.num_dice * cfg.num_faces + 1;
+  if (A > CFRB_TO_LEAF_MAX_ACTIONS)
+    throw std::runtime_error(std::string(who) + ": games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
+                             " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+}
+
 // compute_exploitability_no_net (pybind.cc:86-104, exported as compute_exploitability_fp): the solver build_solver returns for
 // params.subgame_params at the initial state, without a value net (so the tree must be full depth), with the exploitability
 // printed at powers of two.  The reference never steps the solver inside its loop and returns a shadowed zero; this version
-// does what the loop is written to do and returns the sum of both players' exploitabilities after num_iters iterations.
+// does what the loop is written to do and returns the sum of both players' exploitabilities after num_iters iterations.  With
+// fp64 tables the solve runs on the full-game solver (cfrb_full_game_*), whose checkpoints are the one-CTA full-tree solver's bit
+// for bit, so games of up to CFRB_TO_LEAF_MAX_ACTIONS actions are accepted.
 float compute_exploitability_fp(RecursiveSolvingParams params) {
+  // unroll_tree(game, max_depth) has a leaf that is not a liar call exactly when max_depth < A: the deepest non-terminal node, the
+  // sequence of all A - 1 bids, sits at depth A - 1 (subgame_solving.cc:181-184)
+  const int A = 2 * params.num_dice * params.num_faces + 1;
+  if (params.subgame_params.max_depth < A) throw std::runtime_error("Found a non-final leaf node, but value_net is not provided");
   py::gil_scoped_release nogil;
-  FullTreeSolver solver(params, eval_device(), params.subgame_params.max_depth);
+  const int iters = params.subgame_params.num_iters;
   std::array<double, 2> v{};
-  int done = 0;
-  for (int iter = 0; iter < params.subgame_params.num_iters; ++iter) {
-    if (((iter + 1) & iter) == 0 || iter + 1 == params.subgame_params.num_iters) {
-      solver.step(iter + 1 - done);
+  auto checkpoints = [&](auto step, auto exploitability) {
+    int done = 0;
+    for (int iter = 0; iter < iters; ++iter) {
+      if (((iter + 1) & iter) != 0 && iter + 1 != iters) continue;
+      step(iter + 1 - done);
       done = iter + 1;
-      v = solver.exploitability(solver.strategy());
+      v = exploitability();
       std::printf("Iter=%8d exploitabilities=(%.3e, %.3e) sum=%.3e\n", iter + 1, v[0], v[1], (v[0] + v[1]) / 2.);
+      std::fflush(stdout);
     }
+  };
+  if (params.state_dtype == CFRB_STATE_F64) {
+    cfrb_config c = liars_dice::solver_config(params, eval_device(), 1);
+    c.net_mode = CFRB_NET_ZERO;
+    cfrb_full_game* raw = nullptr;
+    check(cfrb_full_game_create(&c, &raw), "cfrb_full_game_create");
+    const FullGamePtr fg(raw);
+    checkpoints([&](int n) { check(cfrb_full_game_step(fg.get(), n), "cfrb_full_game_step"); },
+                [&] {
+                  std::array<double, 2> e{};
+                  check(cfrb_full_game_exploitability(fg.get(), e.data()), "cfrb_full_game_exploitability");
+                  return e;
+                });
+  } else {   // fp32 tables: only the one-CTA full-tree solver keeps them (full trees up to 2^20 nodes)
+    FullTreeSolver solver(params, eval_device(), params.subgame_params.max_depth);
+    checkpoints([&](int n) { solver.step(n); }, [&] { return solver.exploitability(solver.strategy()); });
   }
   return (float)(v[0] + v[1]);
 }
 
 // compute_exploitability (pybind.cc:45-55, exported as compute_exploitability_with_net): compute_strategy_recursive with the
-// checkpoint's value net, then the exploitability of the assembled full-tree strategy.
+// checkpoint's value net, then the exploitability of the assembled full-tree strategy.  The walk and its best responses run on the
+// device (cfrb_recursive_exploitability), with the strategy and best responses of the dense host walk (strategy_recursive) bit for
+// bit, so games of up to CFRB_TO_LEAF_MAX_ACTIONS actions are accepted.
 float compute_exploitability_with_net(RecursiveSolvingParams params, const std::string& model_path) {
+  refuse_above_walk_limit(params, "compute_exploitability_with_net");
   py::gil_scoped_release nogil;
   params.net_mode = liars_dice::env_int("CFRB_EVAL_NET_MODE", CFRB_NET_FP32);   // the reference evaluates a checkpoint with an fp32 forward
   auto model = torch::jit::load(model_path, torch::kCPU);
-  RecursiveEvaluator ev(params, eval_device(), 8192);
-  ev.setWeights(flat_weights_of(model));
-  const auto strategy = ev.strategyRecursive();
+  const HandlePtr h = open_handle(liars_dice::solver_config(params, eval_device(), 8192));
+  const std::vector<float> w = flat_weights_of(model);
+  check(cfrb_set_weights(h.get(), w.data(), w.size(), 1), "cfrb_set_weights");
   std::array<double, 2> e{};
-  check(cfrb_exploitability(ev.handle(), strategy.data(), e.data()), "cfrb_exploitability");
+  check(cfrb_recursive_exploitability(h.get(), e.data(), nullptr, nullptr, nullptr), "cfrb_recursive_exploitability");
   return (float)((e[0] + e[1]) / 2.0);
 }
 
@@ -824,13 +859,28 @@ torch::Tensor strategy_recursive_to_leaf(const RecursiveSolvingParams& cfg, int 
   return f64_tensor(s, {N, H, A});
 }
 
-// The exploitability of compute_strategy_recursive_to_leaf's policy, walked and best-responded on the device
-// (cfrb_to_leaf_exploitability): no dense strategy, so games up to A = 23 (2x5f, 5x2f, 1x10f, 1x11f) are accepted.
-py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity) {
-  const int A = 2 * cfg.num_dice * cfg.num_faces + 1;
-  if (A > CFRB_TO_LEAF_MAX_ACTIONS)   // the library's own refusal, before a device is touched
-    throw std::runtime_error("exploitability_to_leaf: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
-                             " actions are not supported (A = " + std::to_string(A) + ": the full tree has 2^A - 1 nodes)");
+// compute_strategy_recursive (recursive_solving.cc:46-74) of one agent on the host walk (RecursiveEvaluator::strategyRecursive):
+// dense [N, H, A] fp64, so the full tree is capped at 2^20 nodes.  The reference the device walk is checked against.
+torch::Tensor strategy_recursive(const RecursiveSolvingParams& cfg, int device, py::object flat_weights) {
+  const std::vector<float> w = flat_of(flat_weights);
+  std::vector<double> s;
+  int64_t N = 0, H = 0, A = 0;
+  {
+    py::gil_scoped_release nogil;
+    RecursiveEvaluator ev(cfg, device, 8192);
+    if (!w.empty()) ev.setWeights(w);
+    s = ev.strategyRecursive();
+    N = ev.numNodes(); H = ev.numHands(); A = ev.numActions();
+  }
+  return f64_tensor(s, {N, H, A});
+}
+
+// The exploitability of a policy walked and best-responded on the device by `walk` (cfrb_to_leaf_exploitability or
+// cfrb_recursive_exploitability): no dense strategy, so games up to A = 23 (2x5f, 5x2f, 1x10f, 1x11f) are accepted.
+using DeviceWalk = int (*)(cfrb_handle*, double*, int64_t*, int64_t*, double*);
+py::dict exploitability_walk(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity, const char* who,
+                             DeviceWalk walk, const char* walk_name) {
+  refuse_above_walk_limit(cfg, who);
   const std::vector<float> w = flat_of(flat_weights);
   std::array<double, 2> br{};
   double secs[2] = {0, 0}, total = 0;
@@ -841,7 +891,7 @@ py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, p
     const auto t0 = std::chrono::steady_clock::now();
     const HandlePtr h = open_handle(liars_dice::solver_config(cfg, device, std::max(1, wave_capacity)));
     if (!w.empty()) check(cfrb_set_weights(h.get(), w.data(), w.size(), 1), "cfrb_set_weights");
-    check(cfrb_to_leaf_exploitability(h.get(), br.data(), &subgames, &iters, secs), "cfrb_to_leaf_exploitability");
+    check(walk(h.get(), br.data(), &subgames, &iters, secs), walk_name);
     N = cfrb_full_tree_nodes(h.get());
     total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   }
@@ -851,6 +901,18 @@ py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, p
   d["num_nodes"] = N; d["subgames"] = subgames; d["subgame_iters"] = iters;
   d["seconds"] = total; d["walk_seconds"] = secs[0]; d["br_seconds"] = secs[1];
   return d;
+}
+
+// The exploitability of compute_strategy_recursive_to_leaf's policy (cfrb_to_leaf_exploitability).
+py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity) {
+  return exploitability_walk(cfg, device, flat_weights, wave_capacity, "exploitability_to_leaf", cfrb_to_leaf_exploitability,
+                             "cfrb_to_leaf_exploitability");
+}
+
+// The exploitability of compute_strategy_recursive's every-node policy (cfrb_recursive_exploitability).
+py::dict exploitability_recursive(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity) {
+  return exploitability_walk(cfg, device, flat_weights, wave_capacity, "exploitability_recursive", cfrb_recursive_exploitability,
+                             "cfrb_recursive_exploitability");
 }
 
 // recursive_eval's sampled evaluation (RecursiveEvaluator::run, recursive_eval.cc:331-369) walked on the device
@@ -1187,6 +1249,13 @@ PYBIND11_MODULE(rela, m) {
         "in waves of wave_capacity and the best response taken on the GPU without a dense strategy (games with at most 23 actions "
         "whose need fits the free device memory).  dict: exploitability = (br0 + br1) / 2, br [2], num_nodes, subgames, "
         "subgame_iters, seconds, walk_seconds, br_seconds.");
+  m.def("exploitability_recursive", &exploitability_recursive, py::arg("cfg"), py::arg("device") = 0,
+        py::arg("flat_weights") = py::none(), py::arg("wave_capacity") = 16384,
+        "rebel_b200 extension: exploitability of compute_strategy_recursive's every-node policy (a subgame solved for num_iters "
+        "iterations at every non-terminal node, acting with its root's average strategy; what compute_exploitability_with_net "
+        "measures), the 2^(A-1) subgames walked depth by depth in waves of wave_capacity and the best response taken on the GPU "
+        "without a dense strategy (games with at most 23 actions whose need fits the free device memory).  dict as "
+        "exploitability_to_leaf's.");
   m.def("recursive_eval_to_leaf", &recursive_eval_to_leaf, py::arg("cfg"), py::arg("device") = 0, py::arg("num_repeats") = 1,
         py::arg("seed") = 0, py::arg("flat_weights") = py::none(), py::arg("wave_capacity") = 16384, py::arg("batch_repeats") = 0,
         py::arg("return_sums") = false, py::arg("full_strategy") = py::none(), py::arg("track_regrets") = false,
@@ -1229,4 +1298,8 @@ PYBIND11_MODULE(rela, m) {
         py::arg("flat_weights") = py::none(),
         "rebel_b200 extension: compute_strategy_recursive_to_leaf (every subgame solved for num_iters iterations, get_strategy) as a "
         "dense full-tree strategy [N, H, A] fp64 (games whose full tree has at most 2^20 nodes).");
+  m.def("strategy_recursive", &strategy_recursive, py::arg("cfg"), py::arg("device") = 0, py::arg("flat_weights") = py::none(),
+        "rebel_b200 extension: compute_strategy_recursive (a subgame solved for num_iters iterations at every non-terminal node, its "
+        "root row kept) on the host walk, as a dense full-tree strategy [N, H, A] fp64 (games whose full tree has at most 2^20 "
+        "nodes): the reference of exploitability_recursive.");
 }
