@@ -489,6 +489,12 @@ int cfrb_schedule_order(int32_t num_dice, int32_t num_faces, int32_t max_depth, 
 /* Test aid: run the depth <= 2 CFR kernel on at most max_ctas CTAs (0 = as many as are resident at once), so that every warp
  * solves many subgames per launch.  Returns the number of CTAs resident at once. */
 int cfrb_debug_d2_grid(cfrb_handle* h, int32_t max_ctas);
+/* Test aid: wide tickets of the depth <= 2 CFR kernel in the waves that start from now on, the schedule's first m subgames each
+ * solved by a whole CTA instead of one warp: -1 = the wave's own rule (default), 0 = none, m > 0 = m (at most the subgames the wave
+ * solves).  Waves without a schedule (matches, local best responses, agents) stay narrow. */
+int cfrb_debug_d2_wide(cfrb_handle* h, int32_t m);
+/* Test aid: the wide tickets the current wave's depth-2 kernel takes (0 when it takes none). */
+int cfrb_wave_wide(cfrb_handle* h);
 /* Test aid: share = 0 makes the next self-play waves solve every game on its own, instead of solving the games at the initial
  * state (no bid yet, player 0, every belief bitwise 1 / num_hands) once and giving every other one the results (default 1). */
 int cfrb_debug_selfplay_share(cfrb_handle* h, int32_t share);

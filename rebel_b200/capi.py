@@ -145,6 +145,8 @@ def lib():
     L.cfrb_wave_order.argtypes = [vp, _ip, C.c_int32]
     L.cfrb_schedule_order.argtypes = [C.c_int32] * 4 + [_ip, _ip, C.POINTER(C.c_int64)]
     L.cfrb_debug_d2_grid.argtypes = [vp, C.c_int32]
+    L.cfrb_debug_d2_wide.argtypes = [vp, C.c_int32]
+    L.cfrb_wave_wide.argtypes = [vp]
     L.cfrb_debug_selfplay_share.argtypes = [vp, C.c_int32]
     L.cfrb_wave_solved.argtypes = [vp]
     L.cfrb_mark.argtypes = [vp, C.c_int32, vp]
@@ -716,6 +718,16 @@ class WaveSolver:
     def debug_d2_grid(self, max_ctas):
         """Test aid: run the depth-2 CFR kernel on at most max_ctas CTAs (0 = no cap); returns the CTAs resident at once."""
         return _check(lib().cfrb_debug_d2_grid(self._h, int(max_ctas)))
+
+    def debug_d2_wide(self, m):
+        """Test aid: the depth-2 CFR kernel solves the schedule's first m subgames of the waves that start from now on on a whole CTA
+        each (-1 = the wave's own rule, the default; 0 = none; m > 0 = m, at most the subgames the wave solves)."""
+        _check(lib().cfrb_debug_d2_wide(self._h, int(m)))
+
+    @property
+    def wave_wide(self):
+        """Test aid: the wide tickets the current wave's depth-2 CFR kernel takes (0 when it takes none)."""
+        return _check(lib().cfrb_wave_wide(self._h))
 
     def wait_examples(self):
         _check(lib().cfrb_selfplay_wait_examples(self._h))

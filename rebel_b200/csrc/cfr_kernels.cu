@@ -2,6 +2,7 @@
 // operation is an individually rounded IEEE operation in the same order as the reference's scalar C++ (built without
 // contraction), which makes the CFRB_STATE_F64 path reproduce the reference bit for bit between value-net calls.
 #include <algorithm>
+#include <type_traits>
 
 #include "cfr_kernels.cuh"
 #include "br_kernel.cuh"
@@ -87,20 +88,23 @@ template <typename real>
 cudaError_t cfr_configure_d2(int H, int threads, int smem_bytes, int* ctas_per_sm) {
   cudaError_t e = cudaSuccess;
   const int limit = smem_limit(smem_bytes);
-#define CFRB_CFG(HC)                                                                                                                  \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit); \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit);
+#define CFRB_CFG1(HC, KEEP, WIDE)                                                                                                      \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(cfr_iter_d2_kernel<real, HC, KEEP, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit);
+#define CFRB_CFG(HC) CFRB_CFG1(HC, true, true) CFRB_CFG1(HC, false, true) CFRB_CFG1(HC, true, false) CFRB_CFG1(HC, false, false)
   CFRB_CFG(0) CFRB_CFG(4) CFRB_CFG(5) CFRB_CFG(6) CFRB_CFG(9) CFRB_CFG(16)
 #undef CFRB_CFG
+#undef CFRB_CFG1
   if (e != cudaSuccess) return e;
-  // the persistent grid of both variants (with and without the sum table): the smaller residency
-  int keep = 0, drop = 0;
-#define CFRB_OCC(HC)                                                                                                      \
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&keep, cfr_iter_d2_kernel<real, HC, true>, threads, smem_bytes);     \
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&drop, cfr_iter_d2_kernel<real, HC, false>, threads, smem_bytes);
+  // the persistent grid of every variant (with and without the sum table, with and without wide tickets): the smallest residency
+  int occ[4] = {0, 0, 0, 0};
+#define CFRB_OCC(HC)                                                                                                              \
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[0], cfr_iter_d2_kernel<real, HC, true, true>, threads, smem_bytes);         \
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[1], cfr_iter_d2_kernel<real, HC, false, true>, threads, smem_bytes);  \
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[2], cfr_iter_d2_kernel<real, HC, true, false>, threads, smem_bytes);  \
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[3], cfr_iter_d2_kernel<real, HC, false, false>, threads, smem_bytes);
   CFRB_DISPATCH_H(H, CFRB_OCC)
 #undef CFRB_OCC
-  *ctas_per_sm = std::min(keep, drop);
+  *ctas_per_sm = std::min(std::min(occ[0], occ[1]), std::min(occ[2], occ[3]));
   return e;
 }
 
@@ -120,13 +124,19 @@ static void launch_pdl(void (*kernel)(KArgs...), int blocks, int threads, size_t
 template <typename real>
 void cfr_launch_iter_d2(const CfrDev<real>& p, int blocks, int threads, size_t smem, cudaStream_t st, int iter, int do_b, int do_f,
                         int scratch_per_group) {
-#define CFRB_KEEP(HC) launch_pdl(cfr_iter_d2_kernel<real, HC, true>, blocks, threads, smem, st, p, iter, do_b, do_f, scratch_per_group)
-#define CFRB_DROP(HC) launch_pdl(cfr_iter_d2_kernel<real, HC, false>, blocks, threads, smem, st, p, iter, do_b, do_f, scratch_per_group)
-  if (p.keep_sum || p.fp) {
-    CFRB_DISPATCH_H(p.H, CFRB_KEEP)
-  } else {
-    CFRB_DISPATCH_H(p.H, CFRB_DROP)
-  }
+#define CFRB_KEEP(HC) launch_pdl(cfr_iter_d2_kernel<real, HC, true, W>, blocks, threads, smem, st, p, iter, do_b, do_f, scratch_per_group)
+#define CFRB_DROP(HC) launch_pdl(cfr_iter_d2_kernel<real, HC, false, W>, blocks, threads, smem, st, p, iter, do_b, do_f, scratch_per_group)
+  auto launch = [&](auto wide) {
+    constexpr bool W = decltype(wide)::value;
+    if (p.keep_sum || p.fp) {
+      CFRB_DISPATCH_H(p.H, CFRB_KEEP)
+    } else {
+      CFRB_DISPATCH_H(p.H, CFRB_DROP)
+    }
+  };
+  // waves that can take wide tickets get the kernel with them; the others keep the narrow loop's registers
+  if (p.wide != nullptr) launch(std::true_type{});
+  else launch(std::false_type{});
 #undef CFRB_KEEP
 #undef CFRB_DROP
 }

@@ -516,11 +516,24 @@ __device__ __forceinline__ const real* d2_reach_row(const real* slot, const real
   return player == rp ? slot + parent[n] * H : slot + n * H;                    // level 2
 }
 
+// Query-tile row of leaf r of a compacted wave (cfr_forward_d2): lr = live leaves of the subgame before r.  A live leaf goes to row
+// base_live + lr, a dead one to the rows counted down from the last; a dead leaf's outputs are +0.
+template <typename real>
+__device__ __forceinline__ void d2_place_row(const CfrDev<real>& p, int r, int lr, bool live, int base_live, int base_dead, int row0,
+                                             int* rowpos) {
+  const int pos = live ? base_live + lr : p.xh_rows - 1 - (base_dead + r - lr);
+  rowpos[r] = pos;
+  p.row_src[pos] = row0 + r;
+  if (!live) {
+    float4* o = reinterpret_cast<float4*>(p.net_out + (size_t)(row0 + r) * p.Hout);
+    for (int c = 0; c < p.Hout / 4; ++c) o[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
 // KEEP: maintain the sum table S (CfrDev::keep_sum, a compile-time copy: the kernel without it is a separate instantiation, and a
 // run-time test in the last loop costs the kernel spills)
-template <typename real, int HC, bool KEEP>
+template <typename real, int HC, bool KEEP, int G>
 __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2Levels& lv, int k, int trav, real* val, const real* bel, real* rcp, int lane) {
-  constexpr int G = 32;
   const int H = HC > 0 ? HC : p.H;
   const int rp = p.sg_player[k];
   real* R = p.R + (size_t)k * p.table_stride;
@@ -545,7 +558,7 @@ __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2
     const int z = it / H, h = it % H;
     val[t.term[z] * H + h] = __ldg(vt + z * H + h);
   }
-  __syncwarp();
+  group_sync<G>();
   // ---- bottom-up (update_regrets :538-575): level-1 node values, then the root
   if (lv.n2e > lv.n1e) {
     for (int it = lane; it < (lv.n1e - lv.n1b) * H; it += G) {
@@ -558,7 +571,7 @@ __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2
       else        { for (int j = 0; j < nc; ++j) v += val[(c0 + j) * H + h]; }
       val[n * H + h] = v;
     }
-    __syncwarp();
+    group_sync<G>();
     if (!mine0) {   // new regrets of the level-1 actions, kept in the child's slot
 #pragma unroll 4
       for (int it = lane; it < (lv.n2e - lv.n1e) * H; it += G) {
@@ -573,7 +586,7 @@ __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2
     else       { for (int n = lv.n1b; n < lv.n1e; ++n) v += val[n * H + h]; }
     val[h] = v;
   }
-  __syncwarp();
+  group_sync<G>();
   if (mine0) {
     for (int it = lane; it < (lv.n1e - lv.n1b) * H; it += G) {
       const int n = lv.n1b + it / H, h = it % H;
@@ -598,7 +611,7 @@ __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2
       strat = rpow(ns / (ns + 1), p.dcfr_gamma);
     }
   }
-  __syncwarp();
+  group_sync<G>();
   // ---- regret matching (:619-634), regret discount and sum-strategy update (:639-661) on the traverser's level.  The
   // traverser has not acted above that level, so its reach there is its root belief; the child's slot receives
   // belief * new strategy = the traverser's reach under the new strategy (:636-638), which the forward half reuses.
@@ -618,7 +631,7 @@ __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2
     val[n * H + h] = sum;
     rcp[n * H + h] = (real)1 / sum;      // one true division per (node, hand); the per-action quotients below are derived from it
   }
-  __syncwarp();
+  group_sync<G>();
 #pragma unroll 4
   for (int it = lane; it < (ce - cb) * H; it += G) {
     const int c = cb + it / H, h = it % H;
@@ -634,15 +647,14 @@ __device__ void cfr_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2
     val[c * H + h] = rn * sg;
   }
   if (lane == 0) p.steps[2 * k + trav] = s + 1;
-  __syncwarp();
+  group_sync<G>();
 }
 
 // Fictitious-play backward half for depth <= 2 templates: fp_backward's arithmetic with the one-buffer discipline of
 // cfr_backward_d2.  The best-response flags (1 / 0) replace the children's values in place, then give way to the discounted
 // sums, and finally to belief x new average strategy = the reach the forward half needs (same `have` protocol as CFR).
-template <typename real, int HC>
+template <typename real, int HC, int G>
 __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2Levels& lv, int k, int trav, real* val, const real* bel, int lane) {
-  constexpr int G = 32;
   const int H = HC > 0 ? HC : p.H;
   const int rp = p.sg_player[k];
   real* Last = p.R + (size_t)k * p.table_stride;
@@ -661,7 +673,7 @@ __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     const int z = it / H, h = it % H;
     val[t.term[z] * H + h] = vt[z * H + h];
   }
-  __syncwarp();
+  group_sync<G>();
   // ---- bottom-up best response (BRSolver::compute_br :316-358): level 1, then the root
   if (lv.n2e > lv.n1e) {
     for (int it = lane; it < (lv.n1e - lv.n1b) * H; it += G) {
@@ -683,7 +695,7 @@ __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
       }
       val[n * H + h] = v;
     }
-    __syncwarp();
+    group_sync<G>();
   }
   for (int h = lane; h < H; h += G) {
     real v = 0;
@@ -700,7 +712,7 @@ __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     }
     val[h] = v;
   }
-  __syncwarp();
+  group_sync<G>();
   const int s = p.steps[2 * k + trav];
   {
     const real alpha = p.linear ? (real)2 / (s + 2) : (real)1 / (s + 1);
@@ -708,7 +720,7 @@ __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     for (int h = lane; h < H; h += G) mu[h] += (val[h] - mu[h]) * alpha;
   }
   const real disc = (real)(s + 2) / (s + 3);
-  __syncwarp();
+  group_sync<G>();
   // ---- update_sum_strat (:391-421) on the traverser's level: its beliefs there are its root beliefs
   const real* bt = bel + trav * H;
   const int pb = mine0 ? 0 : lv.n1b, pe = mine0 ? 1 : lv.n1e;
@@ -722,7 +734,7 @@ __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     S[e] = sn; Last[e] = x;
     val[c * H + h] = sn;
   }
-  __syncwarp();
+  group_sync<G>();
   for (int it = lane; it < (pe - pb) * H; it += G) {     // normalize_probabilities (util.h:20-34 / 52-63)
     const int n = pb + it / H, h = it % H;
     const int nc = nchild[n];
@@ -737,7 +749,7 @@ __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     }
     val[n * H + h] = tot;
   }
-  __syncwarp();
+  group_sync<G>();
   for (int it = lane; it < (ce - cb) * H; it += G) {
     const int c = cb + it / H, h = it % H;
     const int e = (c - 1) * H + h;
@@ -747,15 +759,14 @@ __device__ void fp_backward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     val[c * H + h] = bt[h] * avg;                        // the traverser's reach under the new average strategy
   }
   if (lane == 0) p.steps[2 * k + trav] = s + 1;
-  __syncwarp();
+  group_sync<G>();
 }
 
 // have: level whose slots already hold the reach of the player acting above it (0: level-1 slots = reach_P0 valid,
 // 1: level-2 slots = reach_P1 valid, -1: neither).
-template <typename real, int HC>
+template <typename real, int HC, int G>
 __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2Levels& lv, int k, int trav, real* slot, const real* bel, int have,
-                               real* aux, real* hist, int lane) {
-  constexpr int G = 32;
+                               real* aux, real* hist, int* xch, int lane) {
   const int H = HC > 0 ? HC : p.H;
   const int rp = p.sg_player[k];
   const real* Sg = p.Sg + (size_t)k * p.table_stride;     // not __restrict__/const-cached: written earlier in this launch
@@ -777,7 +788,7 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
       slot[c * H + h] = b1[h] * __ldg(Sg + (c - 1) * H + h);
     }
   }
-  __syncwarp();
+  group_sync<G>();
   // ---- pseudo-leaves (subgame_solving.cc:257-265, write_query_to :104-123).  All pseudo-leaves of a depth-2 tree sit on level 2:
   // the root player's reach there is its parent's level-1 slot — the same row for every leaf under one level-1 node — so it is
   // summed / normalised once per level-1 node; the other player's reach is the leaf's own slot.  The normalised beliefs are kept
@@ -793,11 +804,11 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
   const bool have_l2 = lv.n2e > lv.n1e;
   // Dead leaves (compacted tiles only): the backward half forms the leaf values (float)(net_out * scaler).  With |net_out| <= B
   // (cfrb_set_weights) and scaler * B <= 2^-151 that product rounds to +-0 whatever the net returns, so the net need not see the
-  // row.  Bit i of live_bits: leaf lane + 32 i is live.
+  // row.  Bit i of live_bits: leaf lane + G i is live.
   const double bound = p.row_src != nullptr ? *p.net_bound : 0.0;
   unsigned live_bits = 0;
   auto mark_live = [&](int r, real sc) {
-    if (!((double)sc * bound <= 0x1p-151)) live_bits |= 1u << (r >> 5);
+    if (!((double)sc * bound <= 0x1p-151)) live_bits |= 1u << (r / G);
   };
   if (have_l2) {
     for (int i = lane; i < n1; i += G) {
@@ -813,7 +824,7 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
         qpar[i * H + h] = __float2half_rn(f);
       }
     }
-    __syncwarp();
+    group_sync<G>();
     for (int r = lane; r < t.L; r += G) {
       const int n = t.pleaf[r];
       const real* ro = slot + n * H;
@@ -859,33 +870,50 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     // readable for the debug readers), each range taken with one atomic per subgame.  The net evaluates only rows < live[trav] and
     // writes row i's outputs to net_out[row_src[i]]; a dead leaf's outputs are +0 here, so net_out and scaler keep the wave's row
     // order and the backward half reads them as before.
-    const int rounds = (t.L + 31) >> 5;
-    const unsigned lt = (1u << lane) - 1u;
-    int nlive = 0;
-    for (int i = 0; i < rounds; ++i) nlive += __popc(__ballot_sync(0xffffffffu, (live_bits >> i) & 1u));
-    int base = 0;
-    if (lane == 0) base = atomicAdd(&p.net_rows->live[trav], nlive);
-    if (lane == 1) base = atomicAdd(&p.net_rows->dead[trav], t.L - nlive);
-    const int base_live = __shfl_sync(0xffffffffu, base, 0), base_dead = __shfl_sync(0xffffffffu, base, 1);
-    int before = 0;                                             // live leaves among 0 .. 32 i - 1
-    for (int i = 0; i < rounds; ++i) {
-      const unsigned b = __ballot_sync(0xffffffffu, (live_bits >> i) & 1u);
-      const int r = 32 * i + lane;
-      if (r < t.L) {
-        const int lr = before + __popc(b & lt);                 // live leaves before r
-        const bool live = (live_bits >> i) & 1u;
-        const int pos = live ? base_live + lr : p.xh_rows - 1 - (base_dead + r - lr);
-        rowpos[r] = pos;
-        p.row_src[pos] = row0 + r;
-        if (!live) {
-          float4* o = reinterpret_cast<float4*>(p.net_out + (size_t)(row0 + r) * p.Hout);
-          for (int c = 0; c < p.Hout / 4; ++c) o[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
+    const int rounds = (t.L + G - 1) / G;
+    const unsigned lt = (1u << (lane & 31)) - 1u;
+    if constexpr (G == 32) {
+      int nlive = 0;
+      for (int i = 0; i < rounds; ++i) nlive += __popc(__ballot_sync(0xffffffffu, (live_bits >> i) & 1u));
+      int base = 0;
+      if (lane == 0) base = atomicAdd(&p.net_rows->live[trav], nlive);
+      if (lane == 1) base = atomicAdd(&p.net_rows->dead[trav], t.L - nlive);
+      const int base_live = __shfl_sync(0xffffffffu, base, 0), base_dead = __shfl_sync(0xffffffffu, base, 1);
+      int before = 0;                                             // live leaves among 0 .. 32 i - 1
+      for (int i = 0; i < rounds; ++i) {
+        const unsigned b = __ballot_sync(0xffffffffu, (live_bits >> i) & 1u);
+        const int r = 32 * i + lane;
+        if (r < t.L) d2_place_row(p, r, before + __popc(b & lt), (live_bits >> i) & 1u, base_live, base_dead, row0, rowpos);
+        before += __popc(b);
       }
-      before += __popc(b);
+    } else {
+      // A group of several warps: xch[i * W + w] = live leaves of warp w among the group's leaves G i .. G i + G - 1, so that the
+      // live leaves before a leaf are the counts of the (round, warp) pairs before its own plus its warp's lower lanes
+      constexpr int W = G / 32;
+      const int w = lane >> 5;
+      for (int i = 0; i < rounds; ++i) {
+        const int c = __popc(__ballot_sync(0xffffffffu, (live_bits >> i) & 1u));
+        if ((lane & 31) == 0) xch[i * W + w] = c;
+      }
+      group_sync<G>();
+      int nlive = 0;
+      for (int j = 0; j < rounds * W; ++j) nlive += xch[j];
+      if (lane == 0) xch[rounds * W] = atomicAdd(&p.net_rows->live[trav], nlive);
+      if (lane == 1) xch[rounds * W + 1] = atomicAdd(&p.net_rows->dead[trav], t.L - nlive);
+      group_sync<G>();
+      const int base_live = xch[rounds * W], base_dead = xch[rounds * W + 1];
+      int before = 0;                                             // live leaves of the (round, warp) pairs before (i, w)
+      for (int j = 0; j < w; ++j) before += xch[j];
+      for (int i = 0; i < rounds; ++i) {
+        const unsigned b = __ballot_sync(0xffffffffu, (live_bits >> i) & 1u);
+        const int r = G * i + lane;
+        if (r < t.L) d2_place_row(p, r, before + __popc(b & lt), (live_bits >> i) & 1u, base_live, base_dead, row0, rowpos);
+        if (i + 1 < rounds)
+          for (int j = 0; j < W; ++j) before += xch[i * W + w + j];   // pairs (i, w) .. (i + 1, w - 1)
+      }
     }
   }
-  __syncwarp();
+  group_sync<G>();
   // ---- query rows; all pseudo-leaves sit on the last level
   const int leaf_player = rp ^ ((t.levels - 1) & 1);
   const int Qp = p.Qpad;
@@ -933,7 +961,7 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
   constexpr int kMaxBins = 9;            // num_dice <= kMaxDice = 7, as in cfr_forward
   static_assert(kMaxBins >= kMaxDice + 2, "a clamped `left` must land on an empty bin");
   real* __restrict__ vt = p.vterm + (size_t)k * p.vterm_stride;
-  __syncwarp();      // hist shares the aux region with the fp16 belief columns the query rows were assembled from
+  group_sync<G>();      // hist shares the aux region with the fp16 belief columns the query rows were assembled from
   for (int z = lane; z < t.T; z += G) {
     const int n = t.term[z];
     const int face = t.term[t.T + z] % p.F;
@@ -955,7 +983,7 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
     for (int m = 0; m < kMaxBins; ++m) hist[z * (kMaxBins + 1) + m] = cnt[m];
     hist[z * (kMaxBins + 1) + kMaxBins] = tot;
   }
-  __syncwarp();
+  group_sync<G>();
   for (int it = lane; it < t.T * H; it += G) {
     const int z = it / H, h = it % H;
     const int pbid = t.term[t.T + z];
@@ -972,98 +1000,254 @@ __device__ void cfr_forward_d2(const CfrDev<real>& p, const D2Tmpl& t, const D2L
 
 // Scratch of a d2 group (reals): slot[nh_max] | bel[2*H] | hist[tmp_reals] | aux (cfr_aux_bytes_d2)
 //
-// Persistent warps: the grid holds at most the warps that are resident at once, and each warp solves subgames one after the
-// other until the wave is exhausted.  Warp w starts with ticket w and draws its later tickets from p.ticket; ticket i is the
-// subgame at wave position sg_order[i], so the costliest subgames start first and the cheapest fill the tail (longest
-// processing time first).  A subgame's results do not depend on which warp solves it or when.  KEEP == p.keep_sum.
+// One subgame (wave position sg_order[ticket]) on a group of G threads with shared memory at gbase: [ template bytes
+// (p.tpk_stride) | slot[nh_max] | bel[2*H] | aux ]; the terminal histogram of the forward half aliases aux (the fp16 belief columns
+// are dead once the query rows are written).  xch: a few ints of shared memory for the exchanges of a group of several warps.
+// wait: the group's first subgame of the launch, which passes griddepcontrol.wait.
+template <typename real, int HC, bool KEEP, int G>
+__device__ __forceinline__ void d2_subgame(const CfrDev<real>& p, int iter, int do_b, int do_f, int ticket, unsigned char* gbase, int* xch,
+                                           int lane, bool wait) {
+  const int H = HC > 0 ? HC : p.H;
+  unsigned char* tb_s = gbase;
+  real* slot = reinterpret_cast<real*>(gbase + p.tpk_stride);
+  real* bel = slot + p.nh_max; real* aux = bel + 2 * H; real* hist = aux;
+  const int k = p.sg_order ? p.sg_order[ticket] : ticket;
+  {   // the subgame's template: one coalesced 16-byte-per-lane copy
+    const int4* src = reinterpret_cast<const int4*>(p.tpk + (size_t)p.sg_tmpl[k] * p.tpk_stride);
+    int4* dst = reinterpret_cast<int4*>(tb_s);
+    for (int i = lane; i < p.tpk_stride / 16; i += G) dst[i] = __ldg(src + i);
+  }
+  for (int i = lane; i < 2 * H; i += G) bel[i] = p.beliefs[(size_t)k * 2 * H + i];
+  group_sync<G>();
+  const D2Tmpl t = d2_tmpl_view(tb_s, H * p.F);
+  const D2Levels lv = d2_levels(tb_s);
+  {
+    // The wave's tables (3 x K x 4.3 KB at 1x6f) do not fit in L2 next to the query tiles, so every launch streams them from
+    // HBM.  Ask for this subgame's lines now: the requests overlap the leaf-value phase instead of stalling the phases
+    // that consume them one DRAM round trip at a time.
+    const size_t off = (size_t)k * p.table_stride * sizeof(real);
+    const int lines = ((t.N - 1) * H * (int)sizeof(real) + 127) >> 7;
+    const char* sg = reinterpret_cast<const char*>(p.Sg) + off;
+    for (int i = lane; i < lines; i += G) asm volatile("prefetch.global.L2 [%0];" ::"l"(sg + ((size_t)i << 7)));
+    if (do_b) {   // regrets and sum strategy (when kept): only the edges below the previous traverser's level are touched
+      const bool root_acts = p.sg_player[k] == ((iter - 1) & 1);
+      const int e0 = (root_acts ? lv.n1b : lv.n1e) - 1, e1 = (root_acts ? lv.n1e : lv.n2e) - 1;
+      const size_t b0 = (size_t)e0 * H * sizeof(real) & ~(size_t)127, b1 = (size_t)e1 * H * sizeof(real);
+      const char* rr = reinterpret_cast<const char*>(p.R) + off;
+      const char* ss = reinterpret_cast<const char*>(p.S) + off;
+      for (size_t o = b0 + ((size_t)lane << 7); o < b1; o += (size_t)G << 7) {
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(rr + o));
+        if (KEEP) asm volatile("prefetch.global.L2 [%0];" ::"l"(ss + o));
+      }
+    }
+  }
+  // ... and this grid, launched the same way behind the previous value-net kernel, must not touch that kernel's outputs (or
+  // tables a still earlier CFR launch wrote) before the kernel has completed.  A no-op for ordinary launches.
+  if (wait) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (p.net_rows != nullptr && ticket == 0 && lane == 0) {
+    // the value net of iteration iter - 1 has completed: account for its rows and clear its slot for the next launch's forward half
+    NetRows* c = p.net_rows;
+    const int s = (iter + 1) & 1;
+    if (do_b) { c->evaluated += (unsigned long long)c->live[s]; c->last_live = c->live[s]; }
+    c->live[s] = 0; c->dead[s] = 0;
+  }
+  group_sync<G>();
+  const int tb = (iter - 1) & 1;
+  const int rp = p.sg_player[k];
+  if (do_b) {
+    if (p.fp) fp_backward_d2<real, HC, G>(p, t, lv, k, tb, slot, bel, lane);
+    else cfr_backward_d2<real, HC, KEEP, G>(p, t, lv, k, tb, slot, bel, aux, lane);
+  }
+  // sampling-strategy snapshot for RlRunner (recursive_solving.cc:168-174): state after `iter` iterations.  The representative of a
+  // shared wave keeps every iteration's instead, for the games that share its solve (sp_share_kernel).
+  {
+    real* Sn = p.sg_act_iter[k] == iter ? p.Snap + (size_t)k * p.table_stride : nullptr;
+    if (p.snap_hist != nullptr && k == *p.share_rep) Sn = p.snap_hist + (size_t)iter * p.table_stride;
+    if (Sn != nullptr) {
+      const real* Sg = p.Sg + (size_t)k * p.table_stride;
+      for (int i = lane; i < (t.N - 1) * H; i += G) Sn[i] = Sg[i];
+    }
+  }
+  if (do_f) cfr_forward_d2<real, HC, G>(p, t, lv, k, iter & 1, slot, bel, do_b ? (tb == rp ? 0 : 1) : -1, aux, hist, xch, lane);
+}
+
+// A CTA as one group, compiled apart from the kernel: inlined, its registers crowd the warps' loop into local memory.  ps: the
+// kernel's parameters, copied to shared memory (a pointer to the parameters themselves would copy them to local memory).
 template <typename real, int HC, bool KEEP>
+__device__ __noinline__ void d2_subgame_cta(const CfrDev<real>* ps, int iter, int do_b, int do_f, int ticket, unsigned char* smem, int* xch,
+                                            bool wait) {
+  d2_subgame<real, HC, KEEP, 128>(*ps, iter, do_b, do_f, ticket, smem, xch, threadIdx.x, wait);
+}
+
+// The ticket counts of a launch (see cfr_iter_d2_kernel), read again where they are needed rather than kept in registers
+struct D2Tickets {
+  int n, m, mb, warps0;   // subgames, wide tickets, CTAs that start with a wide ticket, warps that start with a narrow one
+  template <typename real>
+  __device__ __forceinline__ explicit D2Tickets(const CfrDev<real>& p) {
+    n = *p.wave_n;
+    m = p.wide != nullptr ? min(*p.wide, n) : 0;   // the host sets p.wide only for CTAs of four warps
+    mb = min(m, (int)gridDim.x);
+    warps0 = ((int)gridDim.x - mb) * (int)(blockDim.x / 32);
+  }
+  __device__ __forceinline__ int narrow_draws() const { return n - m + mb * (int)(blockDim.x / 32); }
+};
+
+// A warp's next narrow ticket
+template <typename real>
+__device__ __forceinline__ int d2_draw(const CfrDev<real>& p, int lane) {
+  const D2Tickets c(p);
+  int w = 0;
+  if (lane == 0) {
+    w = atomicAdd(p.ticket, 1);
+    if (w == c.narrow_draws() - 1) *p.ticket = 0;
+  }
+  return c.m + c.warps0 + __shfl_sync(0xffffffffu, w, 0);
+}
+
+// Persistent warps: the grid holds at most the CTAs that are resident at once, and each group solves subgames one after the other
+// until the wave is exhausted.  Ticket i is the subgame at wave position sg_order[i], so the costliest subgames start first and the
+// cheapest fill the tail (longest processing time first).  A subgame's results do not depend on which group solves it or when.
+//
+// Wide tickets: the first m = *p.wide tickets (0 when p.wide is null) go to whole CTAs (four warps, one group of 128 threads on
+// group 0's shared memory); a wave with little work would otherwise end when the last of its costliest subgames ends on one warp.
+// CTA b < mb = min(m, grid) starts with wide ticket b and draws its later ones from p.ticket[1]; once those run out, its warps draw
+// narrow tickets.  The narrow tickets m .. n - 1 go to single warps: warp w of the other CTAs starts with ticket m + w, and every
+// warp draws its later ones from p.ticket[0].
+//
+// Every counter ends the launch at zero: each group that starts draws exactly once more than it has tickets left to take, so
+// p.ticket[1] is drawn m times and p.ticket[0] n - m + 4 mb times (the warps of the wide CTAs join the narrow draws); the draw that
+// returns the last count puts the counter back.  Every draw follows the drawing group's griddepcontrol.wait (a group passes it before
+// its first backward half), so it follows the reset of the previous launch on the stream.  KEEP == p.keep_sum.  WIDE: the host
+// launches the instantiation without wide tickets for waves that cannot take any (p.wide null, or m = 0 known on the host).
+template <typename real, int HC, bool KEEP, bool WIDE>
 __global__ void __launch_bounds__(128, 8) cfr_iter_d2_kernel(CfrDev<real> p, int iter, int do_b, int do_f, int scratch_per_group) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // Programmatic dependent launch: the value-net kernel that follows may be scheduled as soon as every CTA of this grid has
   // started (its weight-staging prologue then overlaps this grid's tail) ...
   asm volatile("griddepcontrol.launch_dependents;");
-  const int groups_per_cta = blockDim.x / 32;
   const int gid = threadIdx.x / 32, lane = threadIdx.x % 32;
-  int ticket = blockIdx.x * groups_per_cta + gid;
-  if (ticket >= *p.wave_n) return;
-  const int H = HC > 0 ? HC : p.H;
-  // per-group shared memory: [ template bytes (p.tpk_stride) | slot[nh_max] | bel[2*H] | aux ] ; the terminal histogram of the
-  // forward half aliases aux (the fp16 belief columns are dead once the query rows are written)
-  unsigned char* gbase = smem_raw + (size_t)gid * ((size_t)scratch_per_group * sizeof(real) + p.tpk_stride);
-  unsigned char* tb_s = gbase;
-  real* slot = reinterpret_cast<real*>(gbase + p.tpk_stride);
-  real* bel = slot + p.nh_max; real* aux = bel + 2 * H; real* hist = aux;
-  for (;;) {
-    const bool first = ticket < gridDim.x * groups_per_cta;   // the warp's first subgame of the launch
-    const int k = p.sg_order ? p.sg_order[ticket] : ticket;
-    {   // the subgame's template: one coalesced 16-byte-per-lane copy
-      const int4* src = reinterpret_cast<const int4*>(p.tpk + (size_t)p.sg_tmpl[k] * p.tpk_stride);
-      int4* dst = reinterpret_cast<int4*>(tb_s);
-      for (int i = lane; i < p.tpk_stride / 16; i += 32) dst[i] = __ldg(src + i);
-    }
-    for (int i = lane; i < 2 * H; i += 32) bel[i] = p.beliefs[(size_t)k * 2 * H + i];
-    __syncwarp();
-    const D2Tmpl t = d2_tmpl_view(tb_s, H * p.F);
-    const D2Levels lv = d2_levels(tb_s);
-    {
-      // The wave's tables (3 x K x 4.3 KB at 1x6f) do not fit in L2 next to the query tiles, so every launch streams them from
-      // HBM.  Ask for this subgame's lines now: the requests overlap the leaf-value phase instead of stalling the phases
-      // that consume them one DRAM round trip at a time.
-      const size_t off = (size_t)k * p.table_stride * sizeof(real);
-      const int lines = ((t.N - 1) * H * (int)sizeof(real) + 127) >> 7;
-      const char* sg = reinterpret_cast<const char*>(p.Sg) + off;
-      for (int i = lane; i < lines; i += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(sg + ((size_t)i << 7)));
-      if (do_b) {   // regrets and sum strategy (when kept): only the edges below the previous traverser's level are touched
-        const bool root_acts = p.sg_player[k] == ((iter - 1) & 1);
-        const int e0 = (root_acts ? lv.n1b : lv.n1e) - 1, e1 = (root_acts ? lv.n1e : lv.n2e) - 1;
-        const size_t b0 = (size_t)e0 * H * sizeof(real) & ~(size_t)127, b1 = (size_t)e1 * H * sizeof(real);
-        const char* rr = reinterpret_cast<const char*>(p.R) + off;
-        const char* ss = reinterpret_cast<const char*>(p.S) + off;
-        for (size_t o = b0 + ((size_t)lane << 7); o < b1; o += (size_t)32 << 7) {
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(rr + o));
-          if (KEEP) asm volatile("prefetch.global.L2 [%0];" ::"l"(ss + o));
+  const size_t group_bytes = (size_t)scratch_per_group * sizeof(real) + p.tpk_stride;
+  if constexpr (!WIDE) {
+    // Narrow tickets only (p.wide is ignored): the loop of the kernel before wide tickets, whose registers it keeps
+    const int groups_per_cta = blockDim.x / 32;
+    int ticket = blockIdx.x * groups_per_cta + gid;
+    if (ticket >= *p.wave_n) return;
+    const int H = HC > 0 ? HC : p.H;
+    // per-group shared memory: [ template bytes (p.tpk_stride) | slot[nh_max] | bel[2*H] | aux ] ; the terminal histogram of the
+    // forward half aliases aux (the fp16 belief columns are dead once the query rows are written)
+    unsigned char* gbase = smem_raw + (size_t)gid * ((size_t)scratch_per_group * sizeof(real) + p.tpk_stride);
+    unsigned char* tb_s = gbase;
+    real* slot = reinterpret_cast<real*>(gbase + p.tpk_stride);
+    real* bel = slot + p.nh_max; real* aux = bel + 2 * H; real* hist = aux;
+    for (;;) {
+      const bool first = ticket < gridDim.x * groups_per_cta;   // the warp's first subgame of the launch
+      const int k = p.sg_order ? p.sg_order[ticket] : ticket;
+      {   // the subgame's template: one coalesced 16-byte-per-lane copy
+        const int4* src = reinterpret_cast<const int4*>(p.tpk + (size_t)p.sg_tmpl[k] * p.tpk_stride);
+        int4* dst = reinterpret_cast<int4*>(tb_s);
+        for (int i = lane; i < p.tpk_stride / 16; i += 32) dst[i] = __ldg(src + i);
+      }
+      for (int i = lane; i < 2 * H; i += 32) bel[i] = p.beliefs[(size_t)k * 2 * H + i];
+      __syncwarp();
+      const D2Tmpl t = d2_tmpl_view(tb_s, H * p.F);
+      const D2Levels lv = d2_levels(tb_s);
+      {
+        // The wave's tables (3 x K x 4.3 KB at 1x6f) do not fit in L2 next to the query tiles, so every launch streams them from
+        // HBM.  Ask for this subgame's lines now: the requests overlap the leaf-value phase instead of stalling the phases
+        // that consume them one DRAM round trip at a time.
+        const size_t off = (size_t)k * p.table_stride * sizeof(real);
+        const int lines = ((t.N - 1) * H * (int)sizeof(real) + 127) >> 7;
+        const char* sg = reinterpret_cast<const char*>(p.Sg) + off;
+        for (int i = lane; i < lines; i += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(sg + ((size_t)i << 7)));
+        if (do_b) {   // regrets and sum strategy (when kept): only the edges below the previous traverser's level are touched
+          const bool root_acts = p.sg_player[k] == ((iter - 1) & 1);
+          const int e0 = (root_acts ? lv.n1b : lv.n1e) - 1, e1 = (root_acts ? lv.n1e : lv.n2e) - 1;
+          const size_t b0 = (size_t)e0 * H * sizeof(real) & ~(size_t)127, b1 = (size_t)e1 * H * sizeof(real);
+          const char* rr = reinterpret_cast<const char*>(p.R) + off;
+          const char* ss = reinterpret_cast<const char*>(p.S) + off;
+          for (size_t o = b0 + ((size_t)lane << 7); o < b1; o += (size_t)32 << 7) {
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(rr + o));
+            if (KEEP) asm volatile("prefetch.global.L2 [%0];" ::"l"(ss + o));
+          }
         }
       }
-    }
-    // ... and this grid, launched the same way behind the previous value-net kernel, must not touch that kernel's outputs (or
-    // tables a still earlier CFR launch wrote) before the kernel has completed.  A no-op for ordinary launches.
-    if (first) asm volatile("griddepcontrol.wait;" ::: "memory");
-    if (p.net_rows != nullptr && ticket == 0 && lane == 0) {
-      // the value net of iteration iter - 1 has completed: account for its rows and clear its slot for the next launch's forward half
-      NetRows* c = p.net_rows;
-      const int s = (iter + 1) & 1;
-      if (do_b) { c->evaluated += (unsigned long long)c->live[s]; c->last_live = c->live[s]; }
-      c->live[s] = 0; c->dead[s] = 0;
-    }
-    __syncwarp();
-    const int tb = (iter - 1) & 1;
-    const int rp = p.sg_player[k];
-    if (do_b) {
-      if (p.fp) fp_backward_d2<real, HC>(p, t, lv, k, tb, slot, bel, lane);
-      else cfr_backward_d2<real, HC, KEEP>(p, t, lv, k, tb, slot, bel, aux, lane);
-    }
-    // sampling-strategy snapshot for RlRunner (recursive_solving.cc:168-174): state after `iter` iterations.  The representative of a
-    // shared wave keeps every iteration's instead, for the games that share its solve (sp_share_kernel).
-    {
-      real* Sn = p.sg_act_iter[k] == iter ? p.Snap + (size_t)k * p.table_stride : nullptr;
-      if (p.snap_hist != nullptr && k == *p.share_rep) Sn = p.snap_hist + (size_t)iter * p.table_stride;
-      if (Sn != nullptr) {
-        const real* Sg = p.Sg + (size_t)k * p.table_stride;
-        for (int i = lane; i < (t.N - 1) * H; i += 32) Sn[i] = Sg[i];
+      // ... and this grid, launched the same way behind the previous value-net kernel, must not touch that kernel's outputs (or
+      // tables a still earlier CFR launch wrote) before the kernel has completed.  A no-op for ordinary launches.
+      if (first) asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (p.net_rows != nullptr && ticket == 0 && lane == 0) {
+        // the value net of iteration iter - 1 has completed: account for its rows and clear its slot for the next launch's forward half
+        NetRows* c = p.net_rows;
+        const int s = (iter + 1) & 1;
+        if (do_b) { c->evaluated += (unsigned long long)c->live[s]; c->last_live = c->live[s]; }
+        c->live[s] = 0; c->dead[s] = 0;
       }
+      __syncwarp();
+      const int tb = (iter - 1) & 1;
+      const int rp = p.sg_player[k];
+      if (do_b) {
+        if (p.fp) fp_backward_d2<real, HC, 32>(p, t, lv, k, tb, slot, bel, lane);
+        else cfr_backward_d2<real, HC, KEEP, 32>(p, t, lv, k, tb, slot, bel, aux, lane);
+      }
+      // sampling-strategy snapshot for RlRunner (recursive_solving.cc:168-174): state after `iter` iterations.  The representative of a
+      // shared wave keeps every iteration's instead, for the games that share its solve (sp_share_kernel).
+      {
+        real* Sn = p.sg_act_iter[k] == iter ? p.Snap + (size_t)k * p.table_stride : nullptr;
+        if (p.snap_hist != nullptr && k == *p.share_rep) Sn = p.snap_hist + (size_t)iter * p.table_stride;
+        if (Sn != nullptr) {
+          const real* Sg = p.Sg + (size_t)k * p.table_stride;
+          for (int i = lane; i < (t.N - 1) * H; i += 32) Sn[i] = Sg[i];
+        }
+      }
+      if (do_f) cfr_forward_d2<real, HC, 32>(p, t, lv, k, iter & 1, slot, bel, do_b ? (tb == rp ? 0 : 1) : -1, aux, hist, nullptr, lane);
+      // The next ticket.  Every warp that started draws exactly once more than it has subgames left to take, so the counter is
+      // drawn n times in all and the draw that returns n - 1 is the launch's last: it puts the counter back to zero.  The draws
+      // follow griddepcontrol.wait, so they follow the reset of the previous launch on the stream.
+      const int n = *p.wave_n;
+      int c = 0;
+      if (lane == 0) {
+        c = atomicAdd(p.ticket, 1);
+        if (c == n - 1) *p.ticket = 0;
+      }
+      ticket = gridDim.x * groups_per_cta + __shfl_sync(0xffffffffu, c, 0);
+      if (ticket >= n) break;
+      __syncwarp();   // the next subgame's template and beliefs overwrite this one's shared memory
     }
-    if (do_f) cfr_forward_d2<real, HC>(p, t, lv, k, iter & 1, slot, bel, do_b ? (tb == rp ? 0 : 1) : -1, aux, hist, lane);
-    // The next ticket.  Every warp that started draws exactly once more than it has subgames left to take, so the counter is
-    // drawn n times in all and the draw that returns n - 1 is the launch's last: it puts the counter back to zero.  The draws
-    // follow griddepcontrol.wait, so they follow the reset of the previous launch on the stream.
-    const int n = *p.wave_n;
-    int c = 0;
-    if (lane == 0) {
-      c = atomicAdd(p.ticket, 1);
-      if (c == n - 1) *p.ticket = 0;
+    return;
+  }
+  int ticket;
+  if ((int)blockIdx.x < D2Tickets(p).mb) {
+    // group 1's shared memory is idle while the CTA is one group: the wide group's exchange ints, then the parameters
+    int* xch = reinterpret_cast<int*>(smem_raw + group_bytes);
+    CfrDev<real>* ps = reinterpret_cast<CfrDev<real>*>(smem_raw + group_bytes + kD2XchBytes);
+    if (threadIdx.x == 0) *ps = p;
+    __syncthreads();
+    ticket = blockIdx.x;
+    for (bool first = true;; first = false) {
+      d2_subgame_cta<real, HC, KEEP>(ps, iter, do_b, do_f, ticket, smem_raw, xch + 1, first);
+      const D2Tickets c(p);
+      if (threadIdx.x == 0) {
+        const int w = atomicAdd(p.ticket + 1, 1);
+        if (w == c.m - 1) p.ticket[1] = 0;
+        xch[0] = w;
+      }
+      __syncthreads();
+      ticket = c.mb + xch[0];
+      __syncthreads();   // every thread has read xch[0], and the subgame's shared memory is free
+      if (ticket >= c.m) break;
     }
-    ticket = gridDim.x * groups_per_cta + __shfl_sync(0xffffffffu, c, 0);
-    if (ticket >= n) break;
+    ticket = d2_draw(p, lane);   // the CTA's warps continue with the narrow tickets they draw
+  } else {
+    const D2Tickets c(p);
+    ticket = c.m + ((int)blockIdx.x - c.mb) * (int)(blockDim.x / 32) + gid;
+  }
+  if (ticket >= *p.wave_n) return;
+  unsigned char* gbase = smem_raw + (size_t)gid * group_bytes;
+  for (;;) {
+    bool first;   // the warp's first subgame of the launch: a ticket it started with (the wide CTAs' warps have passed the wait)
+    { const D2Tickets c(p); first = ticket < c.m + c.warps0; }
+    d2_subgame<real, HC, KEEP, 32>(p, iter, do_b, do_f, ticket, gbase, nullptr, lane, first);
+    ticket = d2_draw(p, lane);
+    if (ticket >= *p.wave_n) break;
     __syncwarp();   // the next subgame's template and beliefs overwrite this one's shared memory
   }
 }

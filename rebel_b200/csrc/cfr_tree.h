@@ -81,10 +81,35 @@ inline TreeTemplate build_template(const GameShape& g, int root_bid, int max_dep
   return t;
 }
 
+#if defined(__CUDACC__)
+#define CFRB_HD __host__ __device__
+#else
+#define CFRB_HD
+#endif
+
 // Schedule of the depth <= 2 CFR kernel: a subgame's cost is its table items ((N - 1) edges x H hands) plus its value-net query
 // rows (L).  The cost is not monotone in the root bid for every game, so templates are ranked by it: rank 0 = the costliest,
 // ties by template index.
-inline int64_t schedule_cost(const TreeTemplate& t, int H) { return (int64_t)(t.N - 1) * H + t.L; }
+CFRB_HD inline int64_t template_cost(int N, int L, int H) { return (int64_t)(N - 1) * H + L; }
+inline int64_t schedule_cost(const TreeTemplate& t, int H) { return template_cost(t.N, t.L, H); }
+
+// Wide tickets of the depth <= 2 CFR kernel: how many of the schedule's first subgames a whole CTA (four warps) solves instead of one
+// warp.  A wave whose solved set is small against the resident warps ends when the last of its costliest subgames ends on its one
+// warp, while most warps idle; four warps cut that chain.  A wave with more work than warps would only lose concurrency.
+//   big:   solved subgames whose template cost is at least kWideShare x max_cost (the costliest template's), the schedule's head
+//   total: the solved set's summed cost; n: its size; warps: the kernel's resident warps (0 = no wide groups)
+//   force: -1 = the rule; otherwise min(force, n) (a test aid)
+// The rule: none unless total <= kWideLoad x warps x max_cost; then the big subgames, at most as many as leave the other subgames
+// kWideRoom warps each (a wide subgame takes three warps more than a narrow one).  Set with scripts/d2_chain_bench.py (DESIGN §4 K1/K3).
+constexpr double kWideShare = 0.45, kWideLoad = 0.5, kWideRoom = 0.5;
+CFRB_HD inline int wide_count(int64_t big, int64_t total, int64_t max_cost, int n, int warps, int force) {
+  if (warps <= 0 || n <= 0) return 0;
+  if (force >= 0) return force < n ? force : n;
+  if ((double)total > kWideLoad * warps * (double)max_cost) return 0;
+  const int64_t room = (int64_t)((warps - kWideRoom * n) / 3);
+  const int64_t m = big < room ? big : room;
+  return m > 0 ? (int)m : 0;
+}
 inline std::vector<int> schedule_ranks(const std::vector<TreeTemplate>& tmpl, int H) {
   std::vector<int> by_cost(tmpl.size()), rank(tmpl.size());
   for (size_t i = 0; i < tmpl.size(); ++i) by_cost[i] = (int)i;

@@ -43,7 +43,8 @@ struct CfrDev {
   const int* wave_n;              // [1] number of live subgames (of the solved set, in a self-play wave whose initial-state games share one solve)
   const int* sg_tmpl; const int* sg_player; const int* sg_row_off; const int* sg_act_iter;
   const int* sg_order;            // [K] wave positions largest template first (cfr_iter_d2_kernel's schedule) -- or nullptr = identity
-  int* ticket;                    // [1] cfr_iter_d2_kernel's subgame counter; zero between launches
+  int* ticket;                    // [2] cfr_iter_d2_kernel's narrow and wide ticket counters; zero between launches
+  const int* wide;                // [1] wide tickets of the wave (cfr_iter_d2_kernel, wide_count in cfr_tree.h) -- or nullptr = none
   const real* beliefs;            // [K][2][H]
   real* mu;                       // [K][2][H] root_values_means
   int* steps;                     // [K][2]
@@ -73,6 +74,10 @@ struct CfrDev {
   // sp_share_kernel takes every initial-state game's act_iteration snapshot.
   real* snap_hist; const int* share_rep;
 };
+
+// cfr_iter_d2_kernel's wide groups use the shared memory of the CTA's second warp for kD2XchBytes of exchange ints and a copy of
+// the kernel's CfrDev: they need CTAs of four warps whose group regions hold both (the host checks both, wide_warps in cfrb_api.cu).
+constexpr int kD2XchBytes = 256;
 
 // Scratch of a group (reals): bufA[N*H] | bufB[N*H] | hist[10*T] | lsum[2*L]  (hist: per-terminal match-count histogram,
 // 9 bins + belief sum)
@@ -138,7 +143,8 @@ struct SpDev {
   // tree templates (read-only; the same arrays the CFR kernels index)
   const TemplateDev* tmpl; const int* child_begin; const int* nchild; const int* last_bid;
   // wave descriptors
-  int* wave;                          // [0] = number of subgames, [1] = value-net rows, [2] = subgames solved, [3] = representative
+  int* wave;                          // [0] = number of subgames, [1] = value-net rows, [2] = subgames solved, [3] = representative,
+                                      // [4] = the CFR kernel's wide tickets
   int* sg_tmpl; int* sg_player; int* sg_row_off; int* sg_act;
   int* sg_order;                      // [K] wave positions sorted by tmpl_rank (stable); when share, [solved_off, solved_off + K) the
                                       // solved ones alone (solved_off = the handle's max_subgames, so that a CUDA graph of a shared
@@ -150,6 +156,9 @@ struct SpDev {
   int* sg_init;                       // [K] 1 = the game is at the initial state (written only when share)
   const int* tmpl_rank;               // [A] schedule rank of each template, 0 = the costliest (schedule_ranks, cfr_tree.h)
   int table_stride;
+  // the CFR kernel's wide tickets (wide_count, cfr_tree.h), which sp_scan_kernel leaves in wave[4]: the warps of its largest grid
+  // (0 = none; a launch of K subgames has at most 4 ceil(K / 4)) and the test aid's setting (-1 = the rule)
+  int wide_warps, wide_force;
 };
 void sp_launch_seed(const SpDev& p, const uint32_t* dev_seeds, cudaStream_t st);
 // act_iteration draw + subgame descriptors + packed row offsets of the next wave

@@ -193,6 +193,8 @@ struct cfrb_handle {
   size_t d2_smem = 0;      // dynamic shared memory of a depth-2 CTA
   int d2_ctas = 0;         // CTAs of the depth-2 kernel resident at once on the device: its persistent grid
   int d2_grid_cap = 0;     // test aid (cfrb_debug_d2_grid): at most this many CTAs, 0 = no cap
+  int d2_wide = -1;        // test aid (cfrb_debug_d2_wide): wide tickets of the next waves, -1 = the rule (wide_count)
+  int host_wide = 0;       // wide tickets of the current host wave (cfrb_begin_wave); a device-built wave keeps its own in d_wave[4]
   std::vector<int> tmpl_rank;   // schedule rank of each template (schedule_ranks)
   bool sorted = false;     // d_sg_order holds the current wave's schedule; otherwise the depth-2 kernel takes wave order
   // Self-play waves on the depth-2 kernel solve their initial-state games once (sp_scan_kernel, sp_share_kernel).  share_on: test
@@ -209,9 +211,9 @@ struct cfrb_handle {
   std::vector<Event> net_ev;   // pairs around value-net launches (profiling mode)
   int net_ev_used = 0;
   // CUDA graphs of whole cfrb_run calls (2 launches per iteration would otherwise be enqueued one by one by the host)
-  struct GraphEntry { int first, count, prof, has_rows, sorted, keep_sum, sharing; GraphExec exec; int launches, net_launches, ev_used; };
+  struct GraphEntry { int first, count, prof, has_rows, sorted, keep_sum, sharing, wide; GraphExec exec; int launches, net_launches, ev_used; };
   std::vector<GraphEntry> graphs;
-  std::vector<std::array<int, 7>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
+  std::vector<std::array<int, 8>> graph_seen;   // keys requested once: a graph is only built for a key that comes back
   bool capturing = false;           // launch geometry independent of the wave size while a graph is being captured / replayed
   // device: templates
   DevBuf<cfrb::TemplateDev> d_tmpl;
@@ -237,9 +239,10 @@ struct cfrb_handle {
   DevBuf<unsigned char> d_tpk;   // byte-packed templates for the depth <= 2 kernel
   int tpk_stride = 0;
   // device: wave (untyped part)
-  DevBuf<int> d_wave;      // [0] = n, [1] = rows, [2] = subgames solved, [3] = representative (a self-play wave, sp_scan_kernel)
+  DevBuf<int> d_wave;      // [0] = n, [1] = rows, [2] = subgames solved, [3] = representative (a self-play wave, sp_scan_kernel),
+                           // [4] = the depth-2 kernel's wide tickets (CfrDev::wide)
   DevBuf<int> d_sg_tmpl, d_sg_player, d_sg_row_off, d_sg_act, d_steps;
-  DevBuf<int> d_sg_order, d_tmpl_rank, d_ticket;   // the depth-2 kernel's schedule [2 max_subgames] (SpDev::sg_order), template ranks, subgame counter
+  DevBuf<int> d_sg_order, d_tmpl_rank, d_ticket;   // the depth-2 kernel's schedule [2 max_subgames] (SpDev::sg_order), template ranks, ticket counters [2]
   DevBuf<float> d_X, d_out, d_dbg;
   long long* dbg_trace = nullptr;   // set only inside cfrb_debug_net_trace
   int x2_gelu = 2;                  // GELU variant of CFRB_NET_TC_F16X2 (leaf_mlp_tc.cuh kGelu): 2 = fp32 tanh, 1 = packed half
@@ -383,7 +386,7 @@ static int alloc_state(cfrb_handle* h, WaveState<real>& s, int max_optin) {
   d.tpk = h->d_tpk.p; d.tpk_stride = h->tpk_stride;
   d.wave_n = h->d_wave.p; d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_row_off = h->d_sg_row_off.p;
   d.sg_act_iter = h->d_sg_act.p; d.beliefs = s.beliefs.p; d.mu = s.mu.p; d.steps = h->d_steps.p;
-  d.sg_order = nullptr; d.ticket = h->d_ticket.p;
+  d.sg_order = nullptr; d.ticket = h->d_ticket.p; d.wide = nullptr;
   d.R = s.R.p; d.Sg = s.Sg.p; d.S = s.S.p; d.Snap = s.Snap.p; d.table_stride = h->table_stride;
   d.vterm = s.vterm.p; d.vterm_stride = vterm_stride;
   d.lmax = std::max(h->Lmax, 1); d.tmax = std::max(h->Tmax, 1); d.n1max = h->n1max;
@@ -405,12 +408,31 @@ static int alloc_state(cfrb_handle* h, WaveState<real>& s, int max_optin) {
   return CFRB_OK;
 }
 
+// Warps of the depth-2 kernel's largest grid that wide tickets (wide_count, cfr_tree.h) may use: CTAs of four warps whose group
+// regions hold the wide group's exchange area (kD2XchBytes: the ticket, the live-row counts of ceil(L / 128) rounds of four warps
+// and two bases, at most 32 rounds) and a copy of the parameters (cfr_iter_d2_kernel), else none.  A launch has at most
+// ceil(n / 4) CTAs of them (launch_iter), which the rule's callers apply for a wave of n subgames.
+static int wide_warps(const cfrb_handle* h) {
+  const int rounds = (std::max(h->Lmax, 1) + 127) / 128;
+  const bool fits = h->d2_smem / 4 >= (size_t)cfrb::kD2XchBytes + sizeof(cfrb::CfrDev<double>) &&
+                    (3 + 4 * rounds) * (int)sizeof(int) <= cfrb::kD2XchBytes && rounds <= 32;
+  const int ctas = h->d2_grid_cap > 0 ? std::min(h->d2_ctas, h->d2_grid_cap) : h->d2_ctas;
+  return h->d2 && h->d2_groups_per_cta == 4 && fits ? 4 * ctas : 0;
+}
+static int wide_warps(const cfrb_handle* h, int n) { return std::min(wide_warps(h), 4 * ((n + 3) / 4)); }
+// sp_scan_kernel's inputs of the wide-ticket rule (the kernel applies the wave size)
+static void scan_wide(const cfrb_handle* h, cfrb::SpDev& scan) {
+  scan.H = h->g.H; scan.wide_warps = wide_warps(h); scan.wide_force = h->d2_wide;
+}
+
 // The kernel parameters of the current wave.
 template <typename real>
 static cfrb::CfrDev<real> wave_dev(const cfrb_handle* h, const WaveState<real>& s) {
   cfrb::CfrDev<real> d = s.dev;
   d.keep_sum = !h->sum_dropped;
   if (h->sorted) d.sg_order = h->d_sg_order.p + (h->sharing ? h->cfg.max_subgames : 0);
+  // waves without a schedule stay narrow, and so do host waves whose rule gave no wide ticket (the narrow-only kernel)
+  if (h->sorted && wide_warps(h) > 0 && (h->rows_on_device || h->host_wide > 0)) d.wide = h->d_wave.p + 4;
   if (h->sharing) { d.wave_n = h->d_wave.p + 2; d.snap_hist = s.snap_hist.p; d.share_rep = h->d_wave.p + 3; }
   return d;
 }
@@ -760,15 +782,15 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
   int max_optin = 0;
   CK(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, cfg->device));
   CK(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, cfg->device));
-  CK(h->d_wave.alloc(4));
+  CK(h->d_wave.alloc(5));
   CK(h->d_sg_tmpl.alloc(K)); CK(h->d_sg_player.alloc(K)); CK(h->d_sg_row_off.alloc(K)); CK(h->d_sg_act.alloc(K));
   CK(h->d_steps.alloc((size_t)K * 2));
-  CK(h->d_sg_order.alloc(2 * (size_t)K)); CK(h->d_ticket.alloc(1));
-  CK(cudaMemset(h->d_ticket.p, 0, sizeof(int)));
+  CK(h->d_sg_order.alloc(2 * (size_t)K)); CK(h->d_ticket.alloc(2));
+  CK(cudaMemset(h->d_ticket.p, 0, 2 * sizeof(int)));
   const size_t rows_cap = (size_t)K * std::max(h->Lmax, 1);
   CK(h->d_X.alloc(cfg->net_mode == CFRB_NET_FP32 ? rows_cap * h->Qpad : 1));
   CK(h->d_out.alloc(rows_cap * h->Hout));
-  CK(cudaMemset(h->d_wave.p, 0, 4 * sizeof(int)));
+  CK(cudaMemset(h->d_wave.p, 0, 5 * sizeof(int)));
   CK(cudaMemset(h->d_out.p, 0, rows_cap * h->Hout * sizeof(float)));
   if (is_tc(cfg->net_mode)) {
     // CFRB_TC_WIDE=1: the wide kernel also on games the resident kernel serves (tests, measurements)
@@ -1036,8 +1058,16 @@ int cfrb_begin_wave(cfrb_handle* h, int32_t n, const int32_t* last_bid, const in
   }
   std::vector<int> order(n);
   cfrb::schedule_order(h->tmpl_rank, tm.data(), n, order.data());
+  int64_t max_cost = 0, total = 0, big = 0;   // the depth-2 kernel's wide tickets, as sp_scan_kernel computes them
+  for (const auto& t : h->tmpl) max_cost = std::max(max_cost, cfrb::schedule_cost(t, H));
+  for (int k = 0; k < n; ++k) {
+    const int64_t c = cfrb::schedule_cost(h->tmpl[tm[k]], H);
+    total += c;
+    big += (double)c >= cfrb::kWideShare * (double)max_cost;
+  }
+  const int wide = cfrb::wide_count(big, total, max_cost, n, wide_warps(h, n), h->d2_wide);
   h->n = n; h->rows = rows; h->iters_done = 0; h->rows_on_device = false; h->sp.pending = false; h->sorted = true;
-  h->sum_dropped = false; h->wave_shared = false;
+  h->sum_dropped = false; h->wave_shared = false; h->host_wide = wide;
   h->h_tmpl = tm; h->h_player = pl; h->h_row_off = ro;
   h->h_last_bid.assign(last_bid, last_bid + n);
   h->h_beliefs.assign(beliefs, beliefs + (size_t)n * 2 * H);
@@ -1045,6 +1075,7 @@ int cfrb_begin_wave(cfrb_handle* h, int32_t n, const int32_t* last_bid, const in
   CK(cudaStreamSynchronize(st));
   const int wave[2] = {n, rows};
   CK(cudaMemcpyAsync(h->d_wave.p, wave, sizeof(wave), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(h->d_wave.p + 4, &wide, sizeof(int), cudaMemcpyHostToDevice, st));
   if (n) {
     CK(cudaMemcpyAsync(h->d_sg_tmpl.p, tm.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(h->d_sg_player.p, pl.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -1190,14 +1221,15 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
   const bool graphable = !no_graph && iters >= 64 && h->cfg.net_mode != CFRB_NET_FP32;
   if (graphable) {
     const int has_rows = h->rows > 0 || h->rows_on_device, sorted = h->sorted, keep_sum = !h->sum_dropped, sharing = h->sharing;
+    const int wide = with_state(h, [&](auto& s) { return (int)(wave_dev(h, s).wide != nullptr); });   // which kernel the graph bakes in
     cfrb_handle::GraphEntry* g = nullptr;
     for (auto& e : h->graphs)
       if (e.first == first && e.count == iters && e.prof == h->profiling && e.has_rows == has_rows && e.sorted == sorted &&
-          e.keep_sum == keep_sum && e.sharing == sharing) { g = &e; break; }
+          e.keep_sum == keep_sum && e.sharing == sharing && e.wide == wide) { g = &e; break; }
     if (!g) {
       // capture + instantiation of ~2 * iters nodes costs ~0.1 s: only worth it for a key that repeats (waves of a self-play
       // loop, bench steps), not for one-off run lengths (e.g. the evaluator's per-chunk act_iteration maxima)
-      const std::array<int, 7> key{first, iters, h->profiling, has_rows, sorted, keep_sum, sharing};
+      const std::array<int, 8> key{first, iters, h->profiling, has_rows, sorted, keep_sum, sharing, wide};
       bool seen = false;
       for (const auto& k : h->graph_seen) seen |= k == key;
       if (!seen) {
@@ -1225,7 +1257,7 @@ int cfrb_run(cfrb_handle* h, int32_t iters, void* cuda_stream) {
       h->launches = l0;
       if (rc == CFRB_OK && ce == cudaSuccess && exec) {
         if (h->graphs.size() >= 8) h->graphs.erase(h->graphs.begin());
-        h->graphs.push_back({first, iters, h->profiling, has_rows, sorted, keep_sum, sharing, std::move(exec), captured, h->net_launches_run,
+        h->graphs.push_back({first, iters, h->profiling, has_rows, sorted, keep_sum, sharing, wide, std::move(exec), captured, h->net_launches_run,
                              h->net_ev_used});
         g = &h->graphs.back();
       } else {
@@ -1887,6 +1919,7 @@ static cfrb::SpDev walk_scan(cfrb_handle* h) {
   cfrb::SpDev scan{};
   scan.A = h->g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
   scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
+  scan_wide(h, scan);
   return scan;
 }
 
@@ -2289,6 +2322,7 @@ static int to_leaf_sampled_impl(cfrb_handle* h, int32_t seed0, int32_t num_repea
   cfrb::SpDev scan{};   // sp_scan_kernel's view of the wave
   scan.A = g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
   scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
+  scan_wide(h, scan);
   // act_iteration ~ discrete distribution with weight i/2 + 1 on even i (recursive_solving.cc:304-309, 315-319); the distribution
   // keeps no state between draws, so one object serves every root
   std::vector<double> weights;
@@ -2942,6 +2976,7 @@ int cfrb_selfplay_wave(cfrb_handle* h, float* dev_ex_q, float* dev_ex_v, int32_t
   if (start_next) {
     // the initial-state games share one solve on the depth-2 kernel (the only one that takes its subgames from a schedule)
     h->sp.dev.share = h->d2 && h->share_on;
+    scan_wide(h, h->sp.dev);
     with_state(h, [&](auto& s) { cfrb::sp_launch_begin(h->sp.dev, s.beliefs.p, st); });
     h->launches += 2;
     CK(cudaGetLastError());
@@ -3150,6 +3185,24 @@ int cfrb_debug_d2_grid(cfrb_handle* h, int32_t max_ctas) {
   h->graphs.clear(); h->graph_seen.clear();
   h->d2_grid_cap = max_ctas;
   return h->d2_ctas;
+}
+
+// Test aid: wide tickets of the depth-2 kernel in the waves that start from now on: -1 = the rule (wide_count, cfr_tree.h), 0 = none,
+// m > 0 = the schedule's first m subgames of every wave (at most the wave's solved set).  Waves without a schedule stay narrow.
+int cfrb_debug_d2_wide(cfrb_handle* h, int32_t m) {
+  if (!h || m < -1) return fail(CFRB_EINVAL, "bad argument");
+  h->d2_wide = m;
+  return CFRB_OK;
+}
+
+// Test aid: the wide tickets the current wave's depth-2 kernel takes (d_wave[4]; 0 for a wave the narrow-only kernel solves).
+int cfrb_wave_wide(cfrb_handle* h) {
+  if (!h) return fail(CFRB_EINVAL, "null handle");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->own_stream));
+  int m = 0;
+  CK(cudaMemcpy(&m, h->d_wave.p + 4, sizeof(int), cudaMemcpyDeviceToHost));
+  return m;
 }
 
 // Development / test aid: div_by_rcp (reciprocal + two fused-multiply-add corrections, cfr_kernels.cuh; the regret matching of

@@ -25,6 +25,7 @@
 #include <limits.h>
 #include <stdint.h>
 
+#include "cfr_tree.h"
 #include "cfr_types.h"
 
 namespace cfrb {
@@ -180,26 +181,48 @@ __global__ void __launch_bounds__(1024) sp_scan_kernel(SpDev p) {
   // weights and num_iters), so a shared wave solves only the lowest one, the representative; the solved set -- every game but the
   // copies -- keeps the schedule's order in sg_order[solved_off ..].  Every game keeps its rows, so that a rerun of the whole wave
   // (materialise_sum) finds them; a copy's rows are simply never written.
+  int n_solved = p.K, solved_at = 0;             // the solved set: sg_order[solved_at, solved_at + n_solved)
   if (!p.share) {
     if (t == 1023) { p.wave[2] = p.K; p.wave[3] = -1; }
-    return;
+  } else {
+    __shared__ int rep_s;
+    if (t == 0) rep_s = INT_MAX;
+    int first = INT_MAX;
+    for (int g = e - 1; g >= b; --g) if (p.sg_init[g]) first = g;
+    __syncthreads();                               // rep_s is set, and the schedule above is visible to the whole CTA
+    if (first != INT_MAX) atomicMin(&rep_s, first);
+    __syncthreads();
+    const int rep = rep_s == INT_MAX ? -1 : rep_s;
+    auto solved = [&](int g) { return !p.sg_init[g] || g == rep; };
+    int c = 0;
+    for (int i = b; i < e; ++i) c += solved(p.sg_order[i]);
+    n_solved = sp_block_scan(part, c);
+    int pos = n_solved - c;
+    for (int i = b; i < e; ++i)
+      if (solved(p.sg_order[i])) p.sg_order[p.solved_off + pos++] = p.sg_order[i];
+    if (t == 1023) { p.wave[2] = n_solved; p.wave[3] = rep; }
+    n_solved = part[1023];
+    solved_at = p.solved_off;
   }
-  __shared__ int rep_s;
-  if (t == 0) rep_s = INT_MAX;
-  int first = INT_MAX;
-  for (int g = e - 1; g >= b; --g) if (p.sg_init[g]) first = g;
-  __syncthreads();                               // rep_s is set, and the schedule above is visible to the whole CTA
-  if (first != INT_MAX) atomicMin(&rep_s, first);
+  // The CFR kernel's wide tickets (wide_count, cfr_tree.h) from the solved set's costs, in p.wave[4]
+  __shared__ unsigned long long wide_s[2];         // summed cost, subgames with at least kWideShare of the costliest template's
+  if (t == 0) { wide_s[0] = 0; wide_s[1] = 0; }
+  long long max_cost = 0;
+  for (int r = 0; r < p.A; ++r) max_cost = max(max_cost, (long long)template_cost(p.tmpl[r].N, p.tmpl[r].L, p.H));
+  __syncthreads();                                 // wide_s is set, and the solved set is visible to the whole CTA
+  const int per_s = (n_solved + 1023) / 1024, sb = t * per_s, se = min(n_solved, sb + per_s);
+  unsigned long long tot = 0, big = 0;
+  for (int i = sb; i < se; ++i) {
+    const int g = p.sg_order[solved_at + i];
+    const long long cost = template_cost(p.tmpl[p.sg_tmpl[g]].N, p.tmpl[p.sg_tmpl[g]].L, p.H);
+    tot += cost;
+    big += (double)cost >= kWideShare * (double)max_cost;
+  }
+  if (tot) atomicAdd(&wide_s[0], tot);
+  if (big) atomicAdd(&wide_s[1], big);
   __syncthreads();
-  const int rep = rep_s == INT_MAX ? -1 : rep_s;
-  auto solved = [&](int g) { return !p.sg_init[g] || g == rep; };
-  int c = 0;
-  for (int i = b; i < e; ++i) c += solved(p.sg_order[i]);
-  const int n_solved = sp_block_scan(part, c);
-  int pos = n_solved - c;
-  for (int i = b; i < e; ++i)
-    if (solved(p.sg_order[i])) p.sg_order[p.solved_off + pos++] = p.sg_order[i];
-  if (t == 1023) { p.wave[2] = n_solved; p.wave[3] = rep; }
+  const int warps = min(p.wide_warps, 4 * ((p.K + 3) / 4));   // a launch has at most ceil(K / 4) CTAs (launch_iter)
+  if (t == 0) p.wave[4] = wide_count((int64_t)wide_s[1], (int64_t)wide_s[0], max_cost, n_solved, warps, p.wide_force);
 }
 
 // The copies of a shared wave (sp_scan_kernel) take the representative's tables, root means and step counters, and every
