@@ -269,8 +269,8 @@ int64_t cfrb_recursive_bytes(int32_t num_dice, int32_t num_faces, int32_t max_su
 /* Test aid: the compact full-tree strategy [N_full - 1][H] (entry (child - 1) * H + hand) that the last cfrb_to_leaf_exploitability
  * or cfrb_recursive_exploitability, whichever ran last, filled. */
 int cfrb_to_leaf_strategy(cfrb_handle* h, double* compact);
-/* Test aid: cfrb_to_leaf_exploitability, cfrb_recursive_exploitability and cfrb_to_leaf_sampled see at most `bytes` free device
- * bytes (0 = the device's own figure). */
+/* Test aid: cfrb_to_leaf_exploitability, cfrb_recursive_exploitability, cfrb_to_leaf_sampled and the strategy-cache check of
+ * cfrb_match_create2 (either handle's cap) see at most `bytes` free device bytes (0 = the device's own figure). */
 int cfrb_debug_to_leaf_free_cap(cfrb_handle* h, int64_t bytes);
 /* recursive_eval's sampled evaluation on the device, for games up to CFRB_TO_LEAF_MAX_ACTIONS: the float32 reach-weighted average
  * of num_repeats sampled recursive strategies (strategy ids seed0 .. seed0 + num_repeats - 1) and its exploitability at every
@@ -524,13 +524,39 @@ int cfrb_stream_wait(cfrb_handle* h, void* cuda_stream);
  * ...) is the last wave the match enqueued, which is empty once every game had finished before it. */
 enum {
   CFRB_MATCH_AVERAGE = 0,
-  CFRB_MATCH_SAMPLED = 1
+  CFRB_MATCH_SAMPLED = 1,
+  /* compute_strategy_recursive (recursive_solving.cc:46-74; the policy compute_exploitability_with_net and
+   * cfrb_recursive_exploitability measure) restricted to the path played: at EVERY node the agent solves the subgame rooted
+   * there from its own beliefs (all num_iters iterations) and acts with the average strategy of that subgame's root.  After each
+   * action it multiplies the mover's belief row by its root row and eps-normalises that row (normalize_beliefs_inplace); the
+   * other row is unchanged.  Matches with it play one ply per round (cfrb_match_create2). */
+  CFRB_MATCH_EVERY_NODE = 2
 };
 enum { CFRB_MATCH_TRACE_GAMES = 256 };   /* games < min(n_games, this) are traced (cfrb_match_trace) */
 typedef struct cfrb_match cfrb_match;
 /* a, b: two distinct handles with the same game, max_depth, device and state dtype, max_subgames >= n_slots, no live self-play
  * session or match.  n_games even.  Each violation returns CFRB_EINVAL with a message. */
 int cfrb_match_create(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out);
+/* Agent a plays policy_a and agent b policy_b, any pair of the three policies (every-node against to-leaf, AVERAGE against
+ * SAMPLED, ...); cfrb_match_create(..., p, ...) is cfrb_match_create2(..., p, p, ...).  A pair of equal to-leaf policies plays
+ * the to-leaf walk above, bit for bit.  Any other pair plays the per-ply walk: a round is ONE ply of every running game.  In it
+ * each agent solves one wave of the slots where its policy needs a subgame (an every-node agent: every running slot; a to-leaf
+ * agent: the slots at the game root or at a pseudo-leaf of its previous subgame), then the mover's agent acts and both agents
+ * update their own beliefs.  A to-leaf agent's acting strategy of each solve is copied into a per-slot fp64 cache right after
+ * the solve: n_slots x E x H x 8 bytes per to-leaf agent (E: the edges of the largest depth-max_depth template; about 0.7 GB for
+ * 8192 slots at 2x6f), see cfrb_match_cache_bytes.  It is refused with CFRB_ENOMEM and its byte count when it exceeds the free
+ * device memory (or either handle's cfrb_debug_to_leaf_free_cap), before anything is allocated.  Draws of game g come from its
+ * (seed, g) streams in a fixed order per ply (agent a's act_iteration when it starts a SAMPLED subgame, then b's, then the
+ * action), so results do not depend on n_slots.  In a per-ply match cfrb_match_trace's rounds are plies: act_iterations[r][k] is
+ * -1 when agent k solved with AVERAGE or EVERY_NODE at ply r, its draw for a SAMPLED solve, and -2 when it did not solve (it
+ * plays on inside its to-leaf subgame); root_beliefs[r][k] are agent k's beliefs at ply r in every case.  cfrb_match_results'
+ * solves and subgame_iters count each agent's actual solves.  Validation as cfrb_match_create's, plus a bad policy value. */
+int cfrb_match_create2(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy_a,
+                       int32_t policy_b, cfrb_match** out);
+/* Host-only: device bytes of the strategy caches cfrb_match_create2 allocates for a match of this game, max_depth, n_slots and
+ * pair of policies (0 for the to-leaf walk and for two every-node agents). */
+int64_t cfrb_match_cache_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t n_slots, int32_t policy_a,
+                               int32_t policy_b);
 /* Enqueue max_rounds rounds on `cuda_stream` (NULL = a's stream); a round is one wave of num_iters iterations per agent (the
  * subgames of every running game, built on the device) and one walk.  Returns max_rounds, or 0 once every game has finished
  * (learned from the previous call's rounds, without further work). */
@@ -538,6 +564,8 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream);
 /* Synchronises.  payoff_a [n_games] (0 for a game not finished yet), plies [n_games]; solves = subgames solved by both agents;
  * subgame_iters = CFR / FP iterations run for them.  Any pointer may be NULL. */
 int cfrb_match_results(cfrb_match* m, float* payoff_a, int32_t* plies, int64_t* solves, int64_t* subgame_iters);
+/* Synchronises.  solves [2]: subgames agent a and agent b solved (an LBR match: the agent's, and 0 for LBR). */
+int cfrb_match_agent_solves(cfrb_match* m, int64_t* solves);
 /* Synchronises.  Trace of one game < min(n_games, CFRB_MATCH_TRACE_GAMES); returns its number of plies P (<= A).
  *   ply_records [A][6]  per ply: agent that acted (0 = a), last bid before the action, acting player (seat), its hand, action,
  *                       subgame (round) index within the game
@@ -574,9 +602,12 @@ int cfrb_match_lbr_counts(cfrb_match* m, int64_t* whatif_solves, int64_t* deferr
 
 /* ---- A ReBeL agent played from outside: one handle's agent at n_tables independent tables, each a game against an external
  * player (a person, another program's bot, a tournament harness), advanced one action per call.  At every table the agent plays
- * as in a cfrb_match_* match: compute_strategy_recursive_to_leaf (policy CFRB_MATCH_AVERAGE) or
- * compute_sampled_strategy_recursive_to_leaf without root_only (CFRB_MATCH_SAMPLED, recursive_solving.cc:76-134, 301-327)
- * restricted to the path played.  It solves the subgame rooted at the current public node from its own beliefs at the game root
+ * as in a cfrb_match_* match: compute_strategy_recursive_to_leaf (policy CFRB_MATCH_AVERAGE),
+ * compute_sampled_strategy_recursive_to_leaf without root_only (CFRB_MATCH_SAMPLED, recursive_solving.cc:76-134, 301-327) or
+ * compute_strategy_recursive (CFRB_MATCH_EVERY_NODE, :46-74) restricted to the path played.  An every-node agent stands at an
+ * unsolved subgame root at every node: each step or policy at a table first solves the subgame at the table's current node,
+ * whoever is to move, and the cache holds that root row; after every action (its own or an observed opponent's) the mover's row
+ * is multiplied by the agent's root row and eps-normalised.  The to-leaf policies:  It solves the subgame rooted at the current public node from its own beliefs at the game root
  * and at every pseudo-leaf of its previous subgame, acts for its hand, and updates both players' beliefs with its own strategy,
  * whoever acts (unnormalised inside a subgame, normalize_beliefs_inplace at its leaves, :41-44).  An opponent action the agent's
  * strategy gives probability 0 is applied all the same: it zeroes that row's beliefs and the eps-normalisation at the next

@@ -162,6 +162,10 @@ def lib():
     L.cfrb_rows_read.argtypes = [vp, C.c_int64, C.c_int32, _fp, _fp]
     L.cfrb_rows_gather.argtypes = [vp, _ip, C.c_int32, vp, vp, C.c_int32, vp]
     L.cfrb_match_create.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_uint64, C.c_int32, C.POINTER(vp)]
+    L.cfrb_match_create2.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_uint64, C.c_int32, C.c_int32, C.POINTER(vp)]
+    L.cfrb_match_cache_bytes.argtypes = [C.c_int32] * 6
+    L.cfrb_match_cache_bytes.restype = C.c_int64
+    L.cfrb_match_agent_solves.argtypes = [vp, C.POINTER(C.c_int64)]
     L.cfrb_match_run.argtypes = [vp, C.c_int32, vp]
     L.cfrb_match_results.argtypes = [vp, _fp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.cfrb_match_trace.argtypes = [vp, C.c_int32, _ip, _dp, _ip, _dp, _ip]
@@ -749,17 +753,29 @@ class WaveSolver:
         return a.value, b.value
 
 
-MATCH_AVERAGE, MATCH_SAMPLED = 0, 1
+MATCH_AVERAGE, MATCH_SAMPLED, MATCH_EVERY_NODE = 0, 1, 2
 MATCH_TRACE_GAMES = 256
 
 
-class Match:
-    """A head-to-head match between the agents of two WaveSolvers (cfrb_match_*): n_games games, n_slots at a time."""
+def match_cache_bytes(num_dice, num_faces, max_depth, n_slots, policy_a, policy_b=None):
+    """Host-only: device bytes of the strategy caches a match of these agents allocates (cfrb_match_cache_bytes): n_slots x E x H
+    fp64 per to-leaf agent of a per-ply match (every-node against anything, or two different to-leaf policies), else 0."""
+    pb = policy_a if policy_b is None else policy_b
+    return _check(lib().cfrb_match_cache_bytes(num_dice, num_faces, max_depth, n_slots, policy_a, pb))
 
-    def __init__(self, a, b, n_slots, n_games, seed=0, policy=MATCH_SAMPLED):
+
+class Match:
+    """A head-to-head match between the agents of two WaveSolvers (cfrb_match_*): n_games games, n_slots at a time.  Agent a
+    plays `policy`, agent b policy_b (None: the same); a pair of different policies, or MATCH_EVERY_NODE, plays the per-ply walk
+    (cfrb_match_create2), whose trace has one round per ply."""
+
+    def __init__(self, a, b, n_slots, n_games, seed=0, policy=MATCH_SAMPLED, policy_b=None):
         self.a, self.b, self.G = a, b, n_games
         self._m = C.c_void_p()
-        _check(lib().cfrb_match_create(a._h, b._h, n_slots, n_games, seed, policy, C.byref(self._m)))
+        if policy_b is None or policy_b == policy:
+            _check(lib().cfrb_match_create(a._h, b._h, n_slots, n_games, seed, policy, C.byref(self._m)))
+        else:
+            _check(lib().cfrb_match_create2(a._h, b._h, n_slots, n_games, seed, policy, policy_b, C.byref(self._m)))
 
     def close(self):
         if self._m:
@@ -786,7 +802,10 @@ class Match:
         plies = np.zeros(self.G, np.int32)
         solves, iters = C.c_int64(0), C.c_int64(0)
         _check(lib().cfrb_match_results(self._m, _p(pay, _fp), _p(plies, _ip), C.byref(solves), C.byref(iters)))
-        return {"payoff_a": pay, "plies": plies, "solves": solves.value, "subgame_iters": iters.value}
+        per = (C.c_int64 * 2)()
+        _check(lib().cfrb_match_agent_solves(self._m, per))
+        return {"payoff_a": pay, "plies": plies, "solves": solves.value, "subgame_iters": iters.value, "solves_a": per[0],
+                "solves_b": per[1]}
 
     def trace(self, game):
         """dict: plies [P, 6] (agent, last bid, player, hand, action, round), prob [P], act_iteration [R, 2], root_beliefs [R, 2, 2, H]."""

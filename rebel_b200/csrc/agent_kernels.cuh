@@ -20,6 +20,9 @@
 //                   strategy of that action, the next node; at a pseudo-leaf both rows eps-normalised and the table unsolved
 //   agent_policy    per (listed table, hand): the strategy of the player to move at the table's node
 //
+// An every-node agent (CFRB_MATCH_EVERY_NODE, compute_strategy_recursive) has an unsolved subgame root at every node: it caches the
+// root row only, and after every action eps-normalises the mover's row and stands at an unsolved root again.
+//
 // This header is compiled into the -fmad=false translation unit: the belief arithmetic is the match walk's, bit for bit.
 #pragma once
 #include <cuda_runtime.h>
@@ -115,7 +118,8 @@ __global__ void __launch_bounds__(128) agent_capture_kernel(AgentDev p, MatchTab
   double* __restrict__ c = p.cache + (size_t)t * p.stride;
   const bool normalise = tb.normalise[0];
   const int root_player = p.root_player[t];
-  for (int d = 0; d < tp.levels; ++d) {
+  const int levels = p.every_node ? 1 : tp.levels;   // every-node: the root row only
+  for (int d = 0; d < levels; ++d) {
     const int nb = level[d], ne = level[d + 1];
     const bool untouched = normalise && p.steps[2 * w + (root_player ^ (d & 1))] == 0;
     for (int e = nb * H + lane; e < ne * H; e += 32) {
@@ -169,6 +173,12 @@ __global__ void __launch_bounds__(128) agent_step_kernel(AgentDev p) {
   if (a == A - 1) {                                  // liar call: the game is over
     p.status[t] = 0;
     flags = 1;
+  } else if (p.every_node) {                         // every node roots the agent's next subgame: the mover's row eps-normalised
+    double* root = p.root_bel + (size_t)t * 2 * H;
+    sp_normalize(bel + actor * H, H);
+    for (int k = 0; k < 2 * H; ++k) root[k] = bel[k];
+    p.status[t] = 1;
+    flags = 2;
   } else if (depth >= p.max_depth) {                 // pseudo-leaf: root of the agent's next subgame
     double* root = p.root_bel + (size_t)t * 2 * H;
     for (int r = 0; r < 2; ++r) sp_normalize(bel + r * H, H);

@@ -11,6 +11,7 @@
 #include "match_kernels.cuh"
 #include "lbr_kernels.cuh"
 #include "agent_kernels.cuh"
+#include "ply_kernels.cuh"
 #include "expl_kernels.cuh"
 #include "expl_sampled_kernels.cuh"
 #include "full_game_kernels.cuh"
@@ -167,6 +168,17 @@ void match_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_
 template <typename real>
 void match_launch_advance(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
   match_advance_kernel<real><<<(p.S + 127) / 128, 128, 0, st>>>(p, t);
+}
+void ply_launch_deal(const MatchDev& p, cudaStream_t st) { ply_deal_kernel<<<(p.S + 127) / 128, 128, 0, st>>>(p); }
+template <typename real>
+void ply_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
+  ply_scan_kernel<<<1, 1024, 0, st>>>(p);
+  ply_begin_kernel<real><<<(p.S + 127) / 128, 128, 0, st>>>(p, t);
+}
+template <typename real>
+void ply_launch_advance(const MatchDev& p, const MatchTabs<real>& t, bool capture, cudaStream_t st) {
+  if (capture) ply_capture_kernel<real><<<(2 * p.S + 3) / 4, 128, 0, st>>>(p, t);
+  ply_advance_kernel<real><<<(p.S + 127) / 128, 128, 0, st>>>(p, t);
 }
 template <typename real>
 void lbr_launch_begin(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st) {
@@ -338,6 +350,8 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void sp_launch_share<real>(const SpDev&, const CfrDev<real>&, cudaStream_t);                                    \
   template void match_launch_begin<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                           \
   template void match_launch_advance<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                         \
+  template void ply_launch_begin<real>(const MatchDev&, const MatchTabs<real>&, cudaStream_t);                             \
+  template void ply_launch_advance<real>(const MatchDev&, const MatchTabs<real>&, bool, cudaStream_t);                     \
   template void lbr_launch_begin<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                               \
   template void lbr_launch_advance<real>(const LbrDev&, const MatchTabs<real>&, cudaStream_t);                             \
   template void agent_launch_begin<real>(const AgentDev&, const MatchTabs<real>&, cudaStream_t);                           \

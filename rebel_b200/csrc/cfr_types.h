@@ -195,6 +195,14 @@ struct MatchDev {
   int table_stride;
   // each agent's wave descriptors and CFR step counters
   int* wave[2]; int* sg_tmpl[2]; int* sg_player[2]; int* sg_row_off[2]; int* sg_act[2]; const int* steps[2];
+  // per-ply walk only (ply_kernels.cuh; the to-leaf walk leaves these unset)
+  int policy[2];                      // each agent's CFRB_MATCH_* policy
+  const int* level_begin;
+  int* awidx[2];                      // [S] agent k's wave index of the slot in this round (-1 = k does not solve there)
+  int* sub_lb[2]; int* sub_player[2]; // [S] to-leaf agent k: root of its current subgame
+  int* sub_node[2]; int* sub_depth[2];   // [S] its template node and plies since that root (sub_node -1 = no subgame solved)
+  double* cache[2];                   // [S][table_stride] to-leaf agent k's acting strategy in that subgame (null: every-node)
+  int* solves[2];                     // [G] subgames agent k solved for game g
 };
 template <typename real>
 struct MatchTabs {
@@ -206,6 +214,11 @@ void match_launch_deal(const MatchDev& p, cudaStream_t st);
 // scan + subgame descriptors of the next round
 template <typename real> void match_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st);
 template <typename real> void match_launch_advance(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st);
+// Per-ply matches (ply_kernels.cuh): one ply per round, each agent solving only where its policy needs a subgame.
+void ply_launch_deal(const MatchDev& p, cudaStream_t st);
+template <typename real> void ply_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st);
+// capture: the to-leaf agents' acting strategies of this round's solves into their caches, then the ply
+template <typename real> void ply_launch_advance(const MatchDev& p, const MatchTabs<real>& t, bool capture, cudaStream_t st);
 // Local best response against one agent (lbr_kernels.cuh): the match's slots and games with handle 0 as the agent; index 1 of
 // m's per-agent arrays is unused.  m.bel holds per slot the agent's beliefs [player][hand] (rows 0, 1) and LBR's belief over the
 // agent's hand (row 2).
@@ -226,6 +239,7 @@ template <typename real> void lbr_launch_advance(const LbrDev& p, const MatchTab
 // external player.  A call lists n distinct tables; the kernels of that call index the per-table state through ids[0..n).
 struct AgentDev {
   int T, A, H, max_depth, sampled, iters;
+  int every_node;                     // 1: a subgame is solved at every node (CFRB_MATCH_EVERY_NODE), only its root row cached
   uint64_t seed;
   // per table
   int* seat; int* hand;               // [T] the agent's seat and hand

@@ -3283,6 +3283,11 @@ struct cfrb_match {
   DevBuf<int> nsg, pend, rr, solves_g, whatif_g;
   DevBuf<double> sigx, tr_val, tr_beta;
   DevBuf<unsigned long long> deferred;
+  // per-ply walk (ply_kernels.cuh): a round is one ply; per agent [2][S] wave indices and subgame state, [2][G] solves, and a
+  // strategy cache per to-leaf agent
+  bool per_ply = false;
+  DevBuf<int> awidx, sub_lb, sub_player, sub_node, sub_depth, solves_k;
+  DevBuf<double> cache[2];
 };
 
 // Agent slot k of the tables a match, LBR or agent kernel reads: the handle's wave beliefs and the table it acts with, the
@@ -3304,6 +3309,11 @@ static int match_kernels(cfrb_match* m, bool begin, cudaStream_t st) {
       act_slot(t, 0, a, sa, false);
       if (begin) cfrb::lbr_launch_begin(m->ldev, t, st);
       else cfrb::lbr_launch_advance(m->ldev, t, st);
+    } else if (m->per_ply) {
+      act_slot(t, 0, a, sa, m->dev.policy[0] == CFRB_MATCH_SAMPLED);
+      act_slot(t, 1, m->h[1], sb, m->dev.policy[1] == CFRB_MATCH_SAMPLED);
+      if (begin) cfrb::ply_launch_begin(m->dev, t, st);
+      else cfrb::ply_launch_advance(m->dev, t, m->dev.cache[0] || m->dev.cache[1], st);
     } else {
       act_slot(t, 0, a, sa, m->dev.sampled);
       act_slot(t, 1, m->h[1], sb, m->dev.sampled);
@@ -3345,41 +3355,80 @@ int cfrb_match_destroy(cfrb_match* m) {
 
 static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed);
 
+static int ply_alloc(cfrb_match* m, const char* who);
+
+// Bytes of the per-ply walk's strategy caches: n_slots x table_stride fp64 per to-leaf agent (none when both play every-node).
+static int64_t cache_bytes(int64_t table_stride, int32_t n_slots, int32_t policy_a, int32_t policy_b) {
+  if (policy_a == policy_b && policy_a != CFRB_MATCH_EVERY_NODE) return 0;   // the to-leaf walk reads its tables in place
+  const int n = (policy_a != CFRB_MATCH_EVERY_NODE) + (policy_b != CFRB_MATCH_EVERY_NODE);
+  return (int64_t)n * n_slots * table_stride * (int64_t)sizeof(double);
+}
+static int64_t match_cache_bytes(const cfrb_handle* a, int32_t n_slots, int32_t policy_a, int32_t policy_b) {
+  return cache_bytes(a->table_stride, n_slots, policy_a, policy_b);
+}
+
+static bool valid_policy(int32_t p) { return p == CFRB_MATCH_AVERAGE || p == CFRB_MATCH_SAMPLED || p == CFRB_MATCH_EVERY_NODE; }
+
+// A pair of equal to-leaf policies plays the to-leaf walk (match_kernels.cuh); any other pair the per-ply walk (ply_kernels.cuh).
 static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed,
-                             int32_t policy) {
-  if (!a || !b) return fail(CFRB_EINVAL, "cfrb_match_create: null handle");
-  if (a == b) return fail(CFRB_EINVAL, "cfrb_match_create: the two agents need two handles (create a second one with the same config)");
-  if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_SAMPLED) return fail(CFRB_EINVAL, "cfrb_match_create: bad policy");
-  if (n_slots < 1) return fail(CFRB_EINVAL, "cfrb_match_create: n_slots must be >= 1");
-  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, "cfrb_match_create: n_games must be even and >= 2 (seat-swapped pairs)");
+                             int32_t policy, int32_t policy_b, const char* who) {
+  const std::string w(who);
+  if (!a || !b)
+    return fail(CFRB_EINVAL, w + ": null handle (local best response, which plays the to-leaf average policy only, is "
+                                 "cfrb_match_create_lbr)");
+  if (a == b) return fail(CFRB_EINVAL, w + ": the two agents need two handles (create a second one with the same config)");
+  if (!valid_policy(policy) || !valid_policy(policy_b))
+    return fail(CFRB_EINVAL, w + ": bad policy (" + std::to_string(policy) + ", " + std::to_string(policy_b) +
+                                 "): CFRB_MATCH_AVERAGE, CFRB_MATCH_SAMPLED or CFRB_MATCH_EVERY_NODE");
+  if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
+  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
   const auto &ca = a->cfg, &cb = b->cfg;
   if (ca.num_dice != cb.num_dice || ca.num_faces != cb.num_faces)
-    return fail(CFRB_EINVAL, "cfrb_match_create: the agents play different games (" + std::to_string(ca.num_dice) + "x" +
+    return fail(CFRB_EINVAL, w + ": the agents play different games (" + std::to_string(ca.num_dice) + "x" +
                                  std::to_string(ca.num_faces) + "f vs " + std::to_string(cb.num_dice) + "x" + std::to_string(cb.num_faces) + "f)");
   if (ca.max_depth != cb.max_depth)
-    return fail(CFRB_EINVAL, "cfrb_match_create: the agents have different max_depth (" + std::to_string(ca.max_depth) + " vs " +
+    return fail(CFRB_EINVAL, w + ": the agents have different max_depth (" + std::to_string(ca.max_depth) + " vs " +
                                  std::to_string(cb.max_depth) + ")");
-  if (ca.device != cb.device) return fail(CFRB_EINVAL, "cfrb_match_create: the agents are on different devices");
-  if (ca.state_dtype != cb.state_dtype) return fail(CFRB_EINVAL, "cfrb_match_create: the agents have different state dtypes");
+  if (ca.device != cb.device) return fail(CFRB_EINVAL, w + ": the agents are on different devices");
+  if (ca.state_dtype != cb.state_dtype) return fail(CFRB_EINVAL, w + ": the agents have different state dtypes");
   for (cfrb_handle* h : {a, b}) {
     if (h->cfg.max_subgames < n_slots)
-      return fail(CFRB_EINVAL, "cfrb_match_create: a handle's capacity (max_subgames " + std::to_string(h->cfg.max_subgames) +
+      return fail(CFRB_EINVAL, w + ": a handle's capacity (max_subgames " + std::to_string(h->cfg.max_subgames) +
                                    ") is smaller than n_slots " + std::to_string(n_slots));
-    if (h->sp.ready) return fail(CFRB_EINVAL, "cfrb_match_create: a handle has a live self-play session");
-    if (h->in_match) return fail(CFRB_EINVAL, "cfrb_match_create: a handle already plays in a live match");
+    if (h->sp.ready) return fail(CFRB_EINVAL, w + ": a handle has a live self-play session");
+    if (h->in_match) return fail(CFRB_EINVAL, w + ": a handle already plays in a live match");
+  }
+  m->per_ply = policy != policy_b || policy == CFRB_MATCH_EVERY_NODE;
+  if (m->per_ply) {   // the strategy caches of the to-leaf agents, refused before anything is allocated
+    const int64_t bytes = match_cache_bytes(a, n_slots, policy, policy_b);
+    CK(cudaSetDevice(ca.device));
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    int64_t avail = (int64_t)free_b;
+    for (cfrb_handle* h : {a, b})
+      if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
+    if (bytes > avail)
+      return fail(CFRB_ENOMEM, w + ": the to-leaf agents' strategy caches need " + std::to_string(bytes) + " bytes of device memory, " +
+                                   std::to_string(avail) + " free (fewer n_slots need less)");
   }
   int rc = match_alloc(m, a, n_slots, n_games, seed);
   if (rc) return rc;
   cfrb::MatchDev& d = m->dev;
   d.sampled = policy == CFRB_MATCH_SAMPLED;
   d.iters[0] = ca.num_iters; d.iters[1] = cb.num_iters;
+  d.policy[0] = policy; d.policy[1] = policy_b;
   cfrb_handle* hs[2] = {a, b};
   for (int k = 0; k < 2; ++k) {
     cfrb_handle* h = hs[k];
     d.wave[k] = h->d_wave.p; d.sg_tmpl[k] = h->d_sg_tmpl.p; d.sg_player[k] = h->d_sg_player.p; d.sg_row_off[k] = h->d_sg_row_off.p;
     d.sg_act[k] = h->d_sg_act.p; d.steps[k] = h->d_steps.p;
   }
-  cfrb::match_launch_deal(d, a->own_stream);
+  if (m->per_ply) {
+    if ((rc = ply_alloc(m, who))) return rc;
+    cfrb::ply_launch_deal(d, a->own_stream);
+  } else {
+    cfrb::match_launch_deal(d, a->own_stream);
+  }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(a->own_stream));
   m->h[0] = a; m->h[1] = b;
@@ -3417,7 +3466,29 @@ static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n
   d.trace_games = T; d.tr_ply = m->tr_ply.p; d.tr_prob = m->tr_prob.p; d.tr_plies = m->tr_plies.p; d.tr_act = m->tr_act.p;
   d.tr_bel = m->tr_bel.p; d.tr_rounds = m->tr_rounds.p;
   d.tmpl = a->d_tmpl.p; d.child_begin = a->d_child_begin.p; d.nchild = a->d_nchild.p; d.matches = a->d_matches.p;
+  d.level_begin = a->d_level_begin.p;
   d.table_stride = a->table_stride;
+  return CFRB_OK;
+}
+
+// The per-ply walk's per-agent state; the caches of the to-leaf agents only.
+static int ply_alloc(cfrb_match* m, const char* who) {
+  (void)who;
+  const int S = m->S, G = m->G;
+  for (auto* p : {&m->awidx, &m->sub_lb, &m->sub_player, &m->sub_node, &m->sub_depth}) CK(p->alloc((size_t)2 * S));
+  CK(m->solves_k.alloc((size_t)2 * G));
+  CK(cudaMemset(m->solves_k.p, 0, (size_t)2 * G * sizeof(int)));
+  cfrb::MatchDev& d = m->dev;
+  for (int k = 0; k < 2; ++k) {
+    d.awidx[k] = m->awidx.p + (size_t)k * S; d.sub_lb[k] = m->sub_lb.p + (size_t)k * S;
+    d.sub_player[k] = m->sub_player.p + (size_t)k * S; d.sub_node[k] = m->sub_node.p + (size_t)k * S;
+    d.sub_depth[k] = m->sub_depth.p + (size_t)k * S; d.solves[k] = m->solves_k.p + (size_t)k * G;
+    d.cache[k] = nullptr;
+    if (d.policy[k] != CFRB_MATCH_EVERY_NODE) {
+      CK(m->cache[k].alloc((size_t)S * d.table_stride));
+      d.cache[k] = m->cache[k].p;
+    }
+  }
   return CFRB_OK;
 }
 
@@ -3425,7 +3496,30 @@ int cfrb_match_create(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n
   if (!out) return fail(CFRB_EINVAL, "cfrb_match_create: null argument");
   *out = nullptr;
   auto m = std::make_unique<cfrb_match>();
-  const int rc = match_create_impl(m.get(), a, b, n_slots, n_games, seed, policy);
+  const int rc = match_create_impl(m.get(), a, b, n_slots, n_games, seed, policy, policy, "cfrb_match_create");
+  if (rc != CFRB_OK) return rc;
+  *out = m.release();
+  return CFRB_OK;
+}
+
+int64_t cfrb_match_cache_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t n_slots, int32_t policy_a,
+                               int32_t policy_b) {
+  if (num_dice < 1 || num_faces < 1 || max_depth < 1 || n_slots < 1)
+    return fail(CFRB_EINVAL, "cfrb_match_cache_bytes: num_dice, num_faces, max_depth, n_slots must be >= 1");
+  if (!valid_policy(policy_a) || !valid_policy(policy_b)) return fail(CFRB_EINVAL, "cfrb_match_cache_bytes: bad policy");
+  const cfrb::GameShape g(num_dice, num_faces);
+  // the game root's template is the largest: A - 1 nodes at depth 1 and C(A, d) at depth d >= 2 (to_leaf_sizes)
+  const int64_t nmax = to_leaf_sizes(g, max_depth, 1).nmax;
+  const int64_t stride = round_up((int)std::max<int64_t>(1, (nmax - 1) * g.H), 4);
+  return cache_bytes(stride, n_slots, policy_a, policy_b);
+}
+
+int cfrb_match_create2(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy_a,
+                       int32_t policy_b, cfrb_match** out) {
+  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create2: null argument");
+  *out = nullptr;
+  auto m = std::make_unique<cfrb_match>();
+  const int rc = match_create_impl(m.get(), a, b, n_slots, n_games, seed, policy_a, policy_b, "cfrb_match_create2");
   if (rc != CFRB_OK) return rc;
   *out = m.release();
   return CFRB_OK;
@@ -3533,12 +3627,23 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
       if (h && (rc = solve_device_wave(h, m->lbr ? h->cfg.max_subgames : m->S, false, false, st))) return rc;
     CK(cudaMemsetAsync(m->left.p, 0, sizeof(int), st));
     if ((rc = match_kernels(m, false, st))) return rc;
-    m->h[0]->launches += 3;
+    m->h[0]->launches += m->per_ply && (m->dev.cache[0] || m->dev.cache[1]) ? 4 : 3;
   }
   CK(cudaMemcpyAsync(m->pin_left, m->left.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   CK(cudaEventRecord(m->ev_left, st));
   m->ev_recorded = true;
   return max_rounds;
+}
+
+// Subgames agent 0 and agent 1 solved in a per-ply match (after match_settle).
+static int match_agent_solves(cfrb_match* m, int64_t* out) {
+  std::vector<int> n((size_t)2 * m->G);
+  CK(cudaMemcpy(n.data(), m->solves_k.p, n.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  for (int k = 0; k < 2; ++k) {
+    out[k] = 0;
+    for (int g = 0; g < m->G; ++g) out[k] += n[(size_t)k * m->G + g];
+  }
+  return CFRB_OK;
 }
 
 int cfrb_match_results(cfrb_match* m, float* payoff_a, int32_t* plies, int64_t* solves, int64_t* subgame_iters) {
@@ -3557,8 +3662,29 @@ int cfrb_match_results(cfrb_match* m, float* payoff_a, int32_t* plies, int64_t* 
     if (subgame_iters) *subgame_iters = r * (int64_t)m->dev.iters[0];
     return CFRB_OK;
   }
+  if (m->per_ply) {                       // each agent's own solves
+    int64_t n[2];
+    if ((rc = match_agent_solves(m, n))) return rc;
+    if (solves) *solves = n[0] + n[1];
+    if (subgame_iters) *subgame_iters = n[0] * (int64_t)m->dev.iters[0] + n[1] * (int64_t)m->dev.iters[1];
+    return CFRB_OK;
+  }
   if (solves) *solves = 2 * r;
   if (subgame_iters) *subgame_iters = r * ((int64_t)m->dev.iters[0] + m->dev.iters[1]);
+  return CFRB_OK;
+}
+
+int cfrb_match_agent_solves(cfrb_match* m, int64_t* solves) {
+  if (!m || !solves) return fail(CFRB_EINVAL, "cfrb_match_agent_solves: null argument");
+  int rc = match_settle(m);
+  if (rc) return rc;
+  if (m->per_ply) return match_agent_solves(m, solves);
+  std::vector<int> n(m->G);
+  CK(cudaMemcpy(n.data(), m->lbr ? m->solves_g.p : m->rounds.p, (size_t)m->G * sizeof(int), cudaMemcpyDeviceToHost));
+  int64_t r = 0;
+  for (int x : n) r += x;
+  solves[0] = r;                      // the to-leaf walk: both agents solve every round; LBR: the agent's solves, LBR none
+  solves[1] = m->lbr ? 0 : r;
   return CFRB_OK;
 }
 
@@ -4007,7 +4133,9 @@ static int agent_solve(cfrb_agent* a, const cfrb::AgentDev& d, int n, const int3
 
 static int agent_create_impl(cfrb_agent* a, cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t policy) {
   if (!h) return fail(CFRB_EINVAL, "cfrb_agent_create: null handle");
-  if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_SAMPLED) return fail(CFRB_EINVAL, "cfrb_agent_create: bad policy");
+  if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_SAMPLED && policy != CFRB_MATCH_EVERY_NODE)
+    return fail(CFRB_EINVAL, "cfrb_agent_create: bad policy " + std::to_string(policy) +
+                                 " (CFRB_MATCH_AVERAGE, CFRB_MATCH_SAMPLED or CFRB_MATCH_EVERY_NODE)");
   if (n_tables < 1) return fail(CFRB_EINVAL, "cfrb_agent_create: n_tables must be >= 1");
   if (h->cfg.max_subgames < n_tables)
     return fail(CFRB_EINVAL, "cfrb_agent_create: the handle's capacity (max_subgames " + std::to_string(h->cfg.max_subgames) +
@@ -4035,6 +4163,7 @@ static int agent_create_impl(cfrb_agent* a, cfrb_handle* h, int32_t n_tables, ui
   a->stamp.assign(T, 0);
   cfrb::AgentDev& d = a->dev;
   d.T = T; d.A = A; d.H = H; d.max_depth = h->cfg.max_depth; d.sampled = a->sampled; d.iters = h->cfg.num_iters; d.seed = seed;
+  d.every_node = policy == CFRB_MATCH_EVERY_NODE;
   d.seat = a->seat.p; d.hand = a->hand.p; d.last_bid = a->last_bid.p; d.player = a->player.p; d.ply = a->ply.p;
   d.root_lb = a->root_lb.p; d.root_player = a->root_player.p; d.node = a->node.p; d.depth = a->depth.p;
   d.act = a->act.p; d.status = a->status.p; d.subgames = a->subgames.p;

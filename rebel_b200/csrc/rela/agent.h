@@ -14,7 +14,7 @@ namespace rela {
 
 class Agent {
  public:
-  // policy: CFRB_MATCH_AVERAGE / CFRB_MATCH_SAMPLED; w: flat Net2 weights (empty: none installed)
+  // policy: CFRB_MATCH_AVERAGE / _SAMPLED / _EVERY_NODE; w: flat Net2 weights (empty: none installed)
   Agent(const liars_dice::RecursiveSolvingParams& cfg, int device, int tables, int policy, uint64_t seed, const std::vector<float>& w)
       : tables_(tables), h_(open_handle(liars_dice::solver_config(cfg, device, tables))) {
     A_ = cfrb_num_actions(h_.get());

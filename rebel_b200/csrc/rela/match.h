@@ -44,13 +44,15 @@ struct MatchResult {
   std::vector<float> payoff;   // [games] to agent A
   std::vector<int> plies;      // [games]
   int64_t solves = 0, subgame_iters = 0;
+  int64_t agent_solves[2] = {0, 0};   // subgames A and B solved
   double seconds = 0;
 };
 
-// One handle per agent; `games` games, `slots` of them at a time.  policy: CFRB_MATCH_AVERAGE / CFRB_MATCH_SAMPLED.
+// One handle per agent; `games` games, `slots` of them at a time.  policy (A's), policy_b: CFRB_MATCH_AVERAGE / _SAMPLED /
+// _EVERY_NODE; a pair of different policies goes through cfrb_match_create2.
 inline MatchResult play_match(const liars_dice::RecursiveSolvingParams& cfg_a, const liars_dice::RecursiveSolvingParams& cfg_b,
                               int device, int games, uint64_t seed, int policy, const std::vector<float>& w_a,
-                              const std::vector<float>& w_b, int slots) {
+                              const std::vector<float>& w_b, int slots, int policy_b) {
   if (games < 2) throw std::runtime_error("play_match: games must be >= 2");
   slots = std::max(1, std::min(slots, games));
   const liars_dice::RecursiveSolvingParams* cfgs[2] = {&cfg_a, &cfg_b};
@@ -61,7 +63,8 @@ inline MatchResult play_match(const liars_dice::RecursiveSolvingParams& cfg_a, c
     if (!ws[k]->empty()) check(cfrb_set_weights(h[k].get(), ws[k]->data(), ws[k]->size(), 1), "cfrb_set_weights");
   }
   cfrb_match* raw = nullptr;
-  check(cfrb_match_create(h[0].get(), h[1].get(), slots, games, seed, policy, &raw), "cfrb_match_create");
+  if (policy == policy_b) check(cfrb_match_create(h[0].get(), h[1].get(), slots, games, seed, policy, &raw), "cfrb_match_create");
+  else check(cfrb_match_create2(h[0].get(), h[1].get(), slots, games, seed, policy, policy_b, &raw), "cfrb_match_create2");
   const MatchPtr m(raw);   // released before the handles it reads
   MatchResult r;
   const auto t0 = std::chrono::steady_clock::now();
@@ -70,6 +73,7 @@ inline MatchResult play_match(const liars_dice::RecursiveSolvingParams& cfg_a, c
   r.payoff.resize(games);
   r.plies.resize(games);
   check(cfrb_match_results(m.get(), r.payoff.data(), r.plies.data(), &r.solves, &r.subgame_iters), "cfrb_match_results");
+  check(cfrb_match_agent_solves(m.get(), r.agent_solves), "cfrb_match_agent_solves");
   r.seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   return r;
 }

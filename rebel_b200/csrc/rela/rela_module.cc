@@ -796,15 +796,24 @@ py::dict stats_dict(const std::vector<float>& payoff) {
   return d;
 }
 
+// CFRB_MATCH_* of a policy name ('average', 'sampled', 'every_node').
+int match_policy(const std::string& policy, const char* who) {
+  if (policy == "average") return CFRB_MATCH_AVERAGE;
+  if (policy == "sampled") return CFRB_MATCH_SAMPLED;
+  if (policy == "every_node") return CFRB_MATCH_EVERY_NODE;
+  throw std::runtime_error(std::string(who) + ": policy must be 'sampled', 'average' or 'every_node' (got '" + policy + "')");
+}
+
 py::dict play_match_py(const RecursiveSolvingParams& cfg_a, const RecursiveSolvingParams& cfg_b, int device, int games, uint64_t seed,
-                       const std::string& policy, py::object flat_weights_a, py::object flat_weights_b, int concurrent_games) {
-  if (policy != "sampled" && policy != "average") throw std::runtime_error("play_match: policy must be 'sampled' or 'average'");
+                       const std::string& policy, py::object flat_weights_a, py::object flat_weights_b, int concurrent_games,
+                       py::object policy_b) {
+  const int pa = match_policy(policy, "play_match");
+  const int pb = policy_b.is_none() ? pa : match_policy(policy_b.cast<std::string>(), "play_match");
   const std::vector<float> wa = flat_of(flat_weights_a), wb = flat_of(flat_weights_b);
   MatchResult r;
   {
     py::gil_scoped_release nogil;
-    r = play_match(cfg_a, cfg_b, device, games, seed, policy == "sampled" ? CFRB_MATCH_SAMPLED : CFRB_MATCH_AVERAGE, wa, wb,
-                   concurrent_games);
+    r = play_match(cfg_a, cfg_b, device, games, seed, pa, wa, wb, concurrent_games, pb);
   }
   py::dict d = stats_dict(r.payoff);
   auto p = torch::empty({(int64_t)games}, torch::kFloat32);
@@ -812,6 +821,7 @@ py::dict play_match_py(const RecursiveSolvingParams& cfg_a, const RecursiveSolvi
   auto pl = torch::empty({(int64_t)games}, torch::kInt32);
   std::copy(r.plies.begin(), r.plies.end(), pl.data_ptr<int32_t>());
   d["payoff_a"] = p; d["plies"] = pl; d["solves"] = r.solves; d["subgame_iters"] = r.subgame_iters; d["seconds"] = r.seconds;
+  d["solves_a"] = r.agent_solves[0]; d["solves_b"] = r.agent_solves[1];
   return d;
 }
 
@@ -1020,10 +1030,10 @@ torch::Tensor i32_tensor(const std::vector<int32_t>& v) {
 
 std::shared_ptr<Agent> make_agent(const RecursiveSolvingParams& cfg, int device, int tables, const std::string& policy, uint64_t seed,
                                   py::object flat_weights) {
-  if (policy != "sampled" && policy != "average") throw std::runtime_error("Agent: policy must be 'sampled' or 'average'");
+  const int pol = match_policy(policy, "Agent");
   const std::vector<float> w = flat_of(flat_weights);
   py::gil_scoped_release nogil;
-  return std::make_shared<Agent>(cfg, device, tables, policy == "sampled" ? CFRB_MATCH_SAMPLED : CFRB_MATCH_AVERAGE, seed, w);
+  return std::make_shared<Agent>(cfg, device, tables, pol, seed, w);
 }
 
 void agent_new_games(Agent& a, py::object ids, py::object seats, py::object hands, py::object keys) {
@@ -1230,11 +1240,12 @@ PYBIND11_MODULE(rela, m) {
         "above regret_depth and of the rest (report_regrets' summary).");
   m.def("play_match", &play_match_py, py::arg("cfg_a"), py::arg("cfg_b"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
         py::arg("policy") = "sampled", py::arg("flat_weights_a") = py::none(), py::arg("flat_weights_b") = py::none(),
-        py::arg("concurrent_games") = 8192,
+        py::arg("concurrent_games") = 8192, py::arg("policy_b") = py::none(),
         "rebel_b200 extension: `games` head-to-head games (seat-swapped pairs) of agent A (cfg_a + net A) against agent B on the GPU, "
-        "each re-solving subgames along the path played with its recursive to-leaf policy ('average' or 'sampled').  dict: payoff_a "
-        "[games] (to A), plies [games], mean, stderr (over pairs), seat_means [2] (A in seat 0 / seat 1), solves, subgame_iters, "
-        "seconds.");
+        "each re-solving subgames along the path played: A with `policy`, B with policy_b (None: the same).  'average' and "
+        "'sampled' are the recursive to-leaf policies; 'every_node' re-solves at every decision (compute_strategy_recursive).  "
+        "dict: payoff_a [games] (to A), plies [games], mean, stderr (over pairs), seat_means [2] (A in seat 0 / seat 1), solves, "
+        "solves_a, solves_b (each agent's), subgame_iters, seconds.");
   m.def("play_lbr", &play_lbr_py, py::arg("cfg"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
         py::arg("flat_weights") = py::none(), py::arg("concurrent_games") = 8192, py::arg("max_subgames") = 0,
         "rebel_b200 extension: local best response against one agent (cfg + net, average policy) on the GPU: `games` games "
@@ -1275,7 +1286,8 @@ PYBIND11_MODULE(rela, m) {
       m, "Agent",
       "rebel_b200 extension: a ReBeL agent (cfg + net) at `tables` independent tables, each a game against an external player, "
       "advanced one action per call on the GPU.  It plays its recursive to-leaf policy ('average' or 'sampled') along the path "
-      "played, re-solving from its own beliefs at the game root and at every pseudo-leaf; deals and seats belong to the caller.")
+      "played, re-solving from its own beliefs at the game root and at every pseudo-leaf, or ('every_node') re-solves at every "
+      "node and acts with the subgame root's average strategy; deals and seats belong to the caller.")
       .def(py::init(&make_agent), py::arg("cfg"), py::arg("device") = 0, py::arg("tables") = 8192, py::arg("policy") = "sampled",
            py::arg("seed") = 0, py::arg("flat_weights") = py::none())
       .def("new_games", &agent_new_games, py::arg("ids"), py::arg("seats"), py::arg("hands"), py::arg("keys") = py::none(),

@@ -1,5 +1,6 @@
 """Head-to-head evaluation of two ReBeL agents on the GPU: each agent (a value net plus a solver configuration) re-solves
-subgames along the path actually played, with its recursive to-leaf policy, in seat-swapped pairs of games.  Works on every game
+subgames along the path actually played, in seat-swapped pairs of games: with its recursive to-leaf policy ('sampled' or
+'average'), or ('every_node') re-solving at every decision as compute_strategy_recursive does.  Works on every game
 the wave solver supports, including those whose full game tree the exploitability tools refuse (2x5f, 5x2f, 2x6f, 1x17f, ...).
 
     python -m rebel_b200.head_to_head --num_dice 2 --num_faces 5 --net_a ckpt_400.torchscript --net_b ckpt_200.torchscript \
@@ -7,11 +8,15 @@ the wave solver supports, including those whose full game tree the exploitabilit
 
 Prints a summary and one tagged line `H2H {"net_a": ..., "net_b": ..., "games": ..., "mean": ..., "stderr": ..., "ci95": [lo, hi],
 "seat0": ..., "seat1": ...}` whose text after the tag is JSON.  mean is agent A's expected payoff per game (+1 win, -1 loss);
-seat0 / seat1 are A's mean payoffs in seat 0 (even games) and seat 1 (odd games)."""
+seat0 / seat1 are A's mean payoffs in seat 0 (even games) and seat 1 (odd games).  When --policy_b is given or either agent plays
+every_node, the line also has "policy_a" and "policy_b"."""
 import argparse
 import json
 
 import torch
+
+
+POLICIES = ("sampled", "average", "every_node")
 
 
 def build_parser():
@@ -24,8 +29,10 @@ def build_parser():
     ap.add_argument("--random_net_seed_b", type=int, default=None, help="agent B plays a random-init Net2 of this seed")
     ap.add_argument("--games", type=int, default=8192, help="games to play (even: seat-swapped pairs)")
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--policy", choices=("sampled", "average"), default="sampled",
-                    help="sampled: ReBeL's random-iteration policy; average: the average strategy of all iterations")
+    ap.add_argument("--policy", choices=POLICIES, default="sampled",
+                    help="sampled: ReBeL's random-iteration policy; average: the average strategy of all iterations (both act to "
+                    "the subgame's leaves); every_node: a subgame re-solved at every decision, acting with its root's average")
+    ap.add_argument("--policy_b", choices=POLICIES, default=None, help="agent B's policy (default: --policy)")
     ap.add_argument("--subgame_iters", type=int, default=1024)
     ap.add_argument("--subgame_iters_b", type=int, default=None, help="agent B's iterations (default: --subgame_iters)")
     ap.add_argument("--mdp_depth", type=int, default=2)
@@ -72,10 +79,12 @@ def agent_name(net, random_seed):
     return f"random_net_seed={random_seed}" if random_seed is not None else "zero"
 
 
-def h2h_line(name_a, name_b, games, mean, stderr, seat_means):
-    """The tagged report line; ci95 = mean -/+ 1.96 stderr."""
+def h2h_line(name_a, name_b, games, mean, stderr, seat_means, policies=None):
+    """The tagged report line; ci95 = mean -/+ 1.96 stderr.  policies: (A's, B's) policy names, reported as policy_a / policy_b."""
     d = {"net_a": name_a, "net_b": name_b, "games": games, "mean": mean, "stderr": stderr,
          "ci95": [mean - 1.96 * stderr, mean + 1.96 * stderr], "seat0": seat_means[0], "seat1": seat_means[1]}
+    if policies is not None:
+        d["policy_a"], d["policy_b"] = policies
     return "H2H " + json.dumps(d)
 
 
@@ -92,17 +101,20 @@ def main(argv=None):
     cfr_b = args.cfr if args.cfr_b is None else args.cfr_b == "yes"
     cfg_a = agent_params(rela, args, wa, args.subgame_iters, args.cfr)
     cfg_b = agent_params(rela, args, wb, args.subgame_iters_b or args.subgame_iters, cfr_b)
+    policy_b = args.policy_b or args.policy
     r = rela.play_match(cfg_a, cfg_b, args.device, args.games, seed=args.seed, policy=args.policy, flat_weights_a=wa,
-                        flat_weights_b=wb, concurrent_games=args.concurrent_games)
+                        flat_weights_b=wb, concurrent_games=args.concurrent_games, policy_b=policy_b)
     na, nb = agent_name(args.net_a, args.random_net_seed_a), agent_name(args.net_b, args.random_net_seed_b)
     mean, se = r["mean"], r["stderr"]
-    print(f"{args.num_dice}x{args.num_faces}f, {args.games} games ({args.policy} policy, depth {args.mdp_depth}): "
+    named = args.policy_b is not None or "every_node" in (args.policy, policy_b)
+    pol = f"{args.policy} policy" if policy_b == args.policy else f"A {args.policy}, B {policy_b} policy"
+    print(f"{args.num_dice}x{args.num_faces}f, {args.games} games ({pol}, depth {args.mdp_depth}): "
           f"A = {na} vs B = {nb}", flush=True)
     print(f"  A's payoff per game {mean:+.4f} +- {se:.4f} (95% CI [{mean - 1.96 * se:+.4f}, {mean + 1.96 * se:+.4f}]); "
           f"in seat 0 {r['seat_means'][0]:+.4f}, in seat 1 {r['seat_means'][1]:+.4f}", flush=True)
-    print(f"  {r['solves']} subgame solves, {r['subgame_iters']} subgame iterations, {float(r['plies'].float().mean()):.2f} plies "
+    print(f"  {r['solves']} subgame solves (A {r['solves_a']}, B {r['solves_b']}), {r['subgame_iters']} subgame iterations, {float(r['plies'].float().mean()):.2f} plies "
           f"per game, {r['seconds']:.2f} s ({args.games / r['seconds']:.1f} games/s)", flush=True)
-    print(h2h_line(na, nb, args.games, mean, se, r["seat_means"]), flush=True)
+    print(h2h_line(na, nb, args.games, mean, se, r["seat_means"], (args.policy, policy_b) if named else None), flush=True)
     return r
 
 

@@ -1,5 +1,6 @@
 """Play Liar's Dice against a ReBeL agent in the terminal.  The agent (a value net plus a solver configuration) re-solves subgames
-on the GPU along the path played, with its recursive to-leaf policy, exactly as in head-to-head matches (rela.Agent).
+on the GPU along the path played, exactly as in head-to-head matches (rela.Agent): with its recursive to-leaf policy ('sampled' or
+'average'), or ('every_node') re-solving at every decision.
 
     python -m rebel_b200.play --num_dice 1 --num_faces 6 --net ckpt.torchscript --subgame_iters 1024 --cfr --mdp_depth 2 \
         --policy sampled --games 5 --seed 0
@@ -15,7 +16,7 @@ import sys
 
 import numpy as np
 
-from rebel_b200.head_to_head import agent_name, agent_params, agent_weights
+from rebel_b200.head_to_head import POLICIES, agent_name, agent_params, agent_weights
 
 
 def build_parser():
@@ -26,8 +27,9 @@ def build_parser():
     ap.add_argument("--subgame_iters", type=int, default=1024)
     ap.add_argument("--cfr", action="store_true", help="the agent solves with CFR instead of fictitious play")
     ap.add_argument("--mdp_depth", type=int, default=2)
-    ap.add_argument("--policy", choices=("sampled", "average"), default="sampled",
-                    help="sampled: ReBeL's random-iteration policy; average: the average strategy of all iterations")
+    ap.add_argument("--policy", choices=POLICIES, default="sampled",
+                    help="sampled: ReBeL's random-iteration policy; average: the average strategy of all iterations (both act to "
+                    "the subgame's leaves); every_node: a subgame re-solved at every decision, acting with its root's average")
     ap.add_argument("--games", type=int, default=1)
     ap.add_argument("--seed", type=int, default=0, help="seeds the deals and the agent's draws")
     ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast GELU (default 3 with a "
