@@ -592,8 +592,26 @@ int cfrb_match_destroy(cfrb_match* m);
  * for 1 subgame (game start, pseudo-leaf) or m (an LBR decision with m raises) and are admitted round-robin; the others wait.
  * cfrb_match_run / _results / _trace / _destroy apply: payoff_a is the agent's payoff (LBR's is its negative), solves counts
  * every subgame solved, what-if ones included; in the trace agent 1 is LBR (probability 1, act_iteration and root beliefs 0).
- * agent: max_subgames >= A - 1, no live self-play session or match; n_games even.  Each violation returns CFRB_EINVAL. */
+ * agent: max_subgames >= A - 1, no live self-play session or match; n_games even.  Each violation returns CFRB_EINVAL.
+ * cfrb_match_create_lbr(...) is cfrb_match_create_lbr2(..., CFRB_MATCH_AVERAGE, ...). */
 int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out);
+/* LBR against the agent playing `policy`: CFRB_MATCH_AVERAGE (the walk above, bit for bit) or CFRB_MATCH_EVERY_NODE.  The
+ * every-node agent plays as in a per-ply cfrb_match_create2 match: it solves at every node of the path, whoever moves, and acts
+ * and updates the mover's belief row with that subgame's root row.  The LBR rule is unchanged; sigma(child(a)) is always the
+ * root row of a what-if solve at child(a).  At an LBR decision at node X with m > 0 legal raises a slot takes two rounds:
+ *   phase 1   one subgame rooted at X from the agent's beliefs (its root row is how the agent updates LBR's row)
+ *   phase 2   m what-if subgames rooted at the children: the agent's own row, and LBR's row times X's root row for that raise,
+ *             eps-normalised
+ * then LBR decides.  After a raise the chosen what-if is the agent's subgame at child(a), not solved again: the agent acts from
+ * its root row, and the slot waits for phase 1 at LBR's next decision.  At bid A - 2 LBR has no raise and calls without a
+ * solve; an agent moving first solves at the game root and acts.  Counts: solves = phase 1 + what-if + game-root solves, i.e.
+ * per game the sum over LBR decisions with m > 0 of (1 + m), plus 1 where the agent moves first; whatif_solves (cfrb_match_lbr_counts)
+ * = the sum of m.  In cfrb_match_trace a round is a node of the path where the agent solved a subgame it acts or updates
+ * beliefs from (the game root when it moves first, each phase 1, each chosen what-if): root_beliefs are its beliefs there, and
+ * each ply carries the round of its node (LBR's call after bid A - 2: the round of the agent's ply before it).
+ * CFRB_MATCH_SAMPLED (LBR would respond to a drawn snapshot the agent's opponent cannot see, so the payoff bounds nothing) and
+ * unknown values return CFRB_EINVAL with a message; other validation as cfrb_match_create_lbr's. */
+int cfrb_match_create_lbr2(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out);
 /* Synchronises.  For a traced game: per ply where LBR acted, values [A][A] (fp64 value of every action, NaN where illegal and on
  * the agent's plies) and beliefs [A][H] (beta before the decision, 0 on the agent's plies).  Returns the number of plies. */
 int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* beliefs);

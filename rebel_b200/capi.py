@@ -171,6 +171,7 @@ def lib():
     L.cfrb_match_trace.argtypes = [vp, C.c_int32, _ip, _dp, _ip, _dp, _ip]
     L.cfrb_match_destroy.argtypes = [vp]
     L.cfrb_match_create_lbr.argtypes = [vp, C.c_int32, C.c_int32, C.c_uint64, C.POINTER(vp)]
+    L.cfrb_match_create_lbr2.argtypes = [vp, C.c_int32, C.c_int32, C.c_uint64, C.c_int32, C.POINTER(vp)]
     L.cfrb_match_lbr_trace.argtypes = [vp, C.c_int32, _dp, _dp]
     L.cfrb_match_lbr_counts.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.cfrb_trainer_create.argtypes = [C.c_int32] * 4 + [C.POINTER(vp)]
@@ -821,13 +822,18 @@ class Match:
 
 
 class LbrMatch(Match):
-    """Local best response against the agent of one WaveSolver (cfrb_match_create_lbr): n_games games, n_slots at a time, at
-    most the solver's max_subgames subgames per round.  results()["payoff_a"] is the agent's payoff; in trace() agent 1 is LBR."""
+    """Local best response against the agent of one WaveSolver (cfrb_match_create_lbr2): n_games games, n_slots at a time, at
+    most the solver's max_subgames subgames per round.  The agent plays `policy`, MATCH_AVERAGE or MATCH_EVERY_NODE (then a
+    trace round is a node where the agent solved a subgame it acts or updates beliefs from).  results()["payoff_a"] is the
+    agent's payoff; in trace() agent 1 is LBR."""
 
-    def __init__(self, agent, n_slots, n_games, seed=0):
+    def __init__(self, agent, n_slots, n_games, seed=0, policy=MATCH_AVERAGE):
         self.a, self.b, self.G = agent, None, n_games
         self._m = C.c_void_p()
-        _check(lib().cfrb_match_create_lbr(agent._h, n_slots, n_games, seed, C.byref(self._m)))
+        if policy == MATCH_AVERAGE:
+            _check(lib().cfrb_match_create_lbr(agent._h, n_slots, n_games, seed, C.byref(self._m)))
+        else:
+            _check(lib().cfrb_match_create_lbr2(agent._h, n_slots, n_games, seed, policy, C.byref(self._m)))
 
     def results(self):
         r = super().results()

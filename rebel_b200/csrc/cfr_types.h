@@ -225,9 +225,11 @@ template <typename real> void ply_launch_advance(const MatchDev& p, const MatchT
 struct LbrDev {
   MatchDev m;
   int K;                              // subgames per round (the agent's max_subgames)
+  int every_node;                     // the agent plays CFRB_MATCH_EVERY_NODE (else CFRB_MATCH_AVERAGE)
   int* nsg;                           // [S] subgames the slot holds in this round's wave (0 = waiting or done)
   int* pend;                          // [S] 1: LBR's decision at (last_bid, player) waits for the solves of its raises' children
-  double* sigx;                       // [S][A][H] the agent's strategy for LBR's seat at that node, per raise
+  double* sigx;                       // [S][A][H] the agent's strategy for LBR's seat at that node, per raise (every-node: from
+                                      // the what-if set-up on, the agent's belief row for LBR's seat after that raise)
   int* rr;                            // [1] rotated slot position where the next round's admission starts
   unsigned long long* deferred;       // [1] running slots left out of a round, summed over rounds
   int* solves; int* whatif;           // [G] subgames solved for game g, and how many of them were what-if solves

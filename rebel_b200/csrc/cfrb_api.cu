@@ -3305,7 +3305,7 @@ static int match_kernels(cfrb_match* m, bool begin, cudaStream_t st) {
   cfrb_handle* a = m->h[0];
   with_state(a, m->lbr ? a : m->h[1], [&](auto& sa, auto& sb) {
     cfrb::MatchTabs<typename std::decay_t<decltype(sa)>::real> t{};
-    if (m->lbr) {   // LBR reads the agent's table as in an AVERAGE match
+    if (m->lbr) {   // LBR reads the agent's table as in an AVERAGE (or per-ply EVERY_NODE) match
       act_slot(t, 0, a, sa, false);
       if (begin) cfrb::lbr_launch_begin(m->ldev, t, st);
       else cfrb::lbr_launch_advance(m->ldev, t, st);
@@ -3374,8 +3374,8 @@ static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int3
                              int32_t policy, int32_t policy_b, const char* who) {
   const std::string w(who);
   if (!a || !b)
-    return fail(CFRB_EINVAL, w + ": null handle (local best response, which plays the to-leaf average policy only, is "
-                                 "cfrb_match_create_lbr)");
+    return fail(CFRB_EINVAL, w + ": null handle (local best response against one agent is cfrb_match_create_lbr or "
+                                 "cfrb_match_create_lbr2)");
   if (a == b) return fail(CFRB_EINVAL, w + ": the two agents need two handles (create a second one with the same config)");
   if (!valid_policy(policy) || !valid_policy(policy_b))
     return fail(CFRB_EINVAL, w + ": bad policy (" + std::to_string(policy) + ", " + std::to_string(policy_b) +
@@ -3525,15 +3525,22 @@ int cfrb_match_create2(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t 
   return CFRB_OK;
 }
 
-static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed) {
-  if (!a) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: null handle");
-  if (n_slots < 1) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: n_slots must be >= 1");
-  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: n_games must be even and >= 2 (seat-swapped pairs)");
-  if (a->sp.ready) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: the handle has a live self-play session");
-  if (a->in_match) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: the handle already plays in a live match");
+static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy,
+                           const char* who) {
+  const std::string w(who);
+  if (!a) return fail(CFRB_EINVAL, w + ": null handle");
+  if (policy == CFRB_MATCH_SAMPLED)
+    return fail(CFRB_EINVAL, w + ": CFRB_MATCH_SAMPLED is not supported: LBR would have to respond to the expectation over the "
+                                 "agent's act_iteration draws, and the drawn snapshot is information the agent's opponent does not have");
+  if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_EVERY_NODE)
+    return fail(CFRB_EINVAL, w + ": bad policy (" + std::to_string(policy) + "): CFRB_MATCH_AVERAGE or CFRB_MATCH_EVERY_NODE");
+  if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
+  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
+  if (a->sp.ready) return fail(CFRB_EINVAL, w + ": the handle has a live self-play session");
+  if (a->in_match) return fail(CFRB_EINVAL, w + ": the handle already plays in a live match");
   const int A = a->g.A;
   if (a->cfg.max_subgames < A - 1)
-    return fail(CFRB_EINVAL, "cfrb_match_create_lbr: the handle's capacity (max_subgames " + std::to_string(a->cfg.max_subgames) +
+    return fail(CFRB_EINVAL, w + ": the handle's capacity (max_subgames " + std::to_string(a->cfg.max_subgames) +
                                  ") must hold the A - 1 = " + std::to_string(A - 1) + " what-if subgames of one LBR decision");
   int rc = match_alloc(m, a, n_slots, n_games, seed);
   if (rc) return rc;
@@ -3559,6 +3566,7 @@ static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32
   CK(cudaMemcpy(m->tr_val.p, nan.data(), nan.size() * sizeof(double), cudaMemcpyHostToDevice));
   cfrb::LbrDev& l = m->ldev;
   l.K = a->cfg.max_subgames;
+  l.every_node = policy == CFRB_MATCH_EVERY_NODE;
   l.nsg = m->nsg.p; l.pend = m->pend.p; l.sigx = m->sigx.p; l.rr = m->rr.p; l.deferred = m->deferred.p;
   l.solves = m->solves_g.p; l.whatif = m->whatif_g.p; l.tr_val = m->tr_val.p; l.tr_beta = m->tr_beta.p;
   cfrb::match_launch_deal(d, a->own_stream);
@@ -3571,14 +3579,23 @@ static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32
   return CFRB_OK;
 }
 
-int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out) {
-  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create_lbr: null argument");
+static int lbr_create(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out,
+                      const char* who) {
+  if (!out) return fail(CFRB_EINVAL, std::string(who) + ": null argument");
   *out = nullptr;
   auto m = std::make_unique<cfrb_match>();
-  const int rc = lbr_create_impl(m.get(), agent, n_slots, n_games, seed);
+  const int rc = lbr_create_impl(m.get(), agent, n_slots, n_games, seed, policy, who);
   if (rc != CFRB_OK) return rc;
   *out = m.release();
   return CFRB_OK;
+}
+
+int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out) {
+  return lbr_create(agent, n_slots, n_games, seed, CFRB_MATCH_AVERAGE, out, "cfrb_match_create_lbr");
+}
+
+int cfrb_match_create_lbr2(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out) {
+  return lbr_create(agent, n_slots, n_games, seed, policy, out, "cfrb_match_create_lbr2");
 }
 
 int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* beliefs) {

@@ -19,6 +19,19 @@
 //   lbr_advance   per admitted slot: resolves a pending decision, then walks up to max_depth plies; stops at a pseudo-leaf, at
 //                 an LBR decision whose raises lead to pseudo-leaves (pending), or at the liar call (payoff, next game)
 //
+// Against an EVERY_NODE agent (cfrb_match_create_lbr2) the agent plays as in a per-ply match (ply_kernels.cuh): it solves the
+// subgame rooted at every node of the path, whoever moves, and acts and updates the mover's belief row with that root's row
+// (en_root_sig, en_update_row).  The LBR rule is the same; sigma(child(a)) is always the root row of a what-if solve at child(a):
+//   phase 1       LBR to move at X with m > 0 legal raises: one subgame rooted at X from the agent's beliefs; its root row for
+//                 LBR's seat goes to sigx (what the agent would multiply LBR's row by after each raise)
+//   phase 2       m what-if subgames rooted at the children: the agent's own row as it is, LBR's row times sigx[a], eps-normalised
+//                 (the row the agent holds if LBR raises to a; kept in sigx[a])
+//   decide, act   LBR values its actions from the what-if roots and chooses.  After a raise the chosen what-if is the agent's
+//                 subgame at child(a): it acts for its hand from that root row, updates its own row with it, LBR updates beta,
+//                 and the slot waits for phase 1 at LBR's next decision.  At bid A - 2 LBR has no raise and calls at once.
+// The agent moving first solves at the game root and acts.  A slot still asks for 1 subgame (phase 1, root) or m (phase 2) a
+// round, so lbr_scan and its admission serve both walks unchanged.
+//
 // LBR draws no random numbers, so the agent's draws consume the match's (seed, g) streams exactly as in a match.  Compiled into
 // the -fmad=false translation unit: every sum runs in the order stated, in fp64, without contraction.
 #pragma once
@@ -27,6 +40,7 @@
 
 #include "cfr_types.h"
 #include "match_kernels.cuh"
+#include "ply_kernels.cuh"
 
 namespace cfrb {
 
@@ -130,6 +144,13 @@ __global__ void __launch_bounds__(128) lbr_begin_kernel(LbrDev p, MatchTabs<real
     for (int a = lo; a <= A - 2; ++a) {
       const int ws = w + a - lo;
       q.sg_tmpl[0][ws] = a + 1; q.sg_player[0][ws] = pl ^ 1; q.sg_act[0][ws] = -1;
+      if (p.every_node) {                            // sigx[a] becomes LBR's row times it, eps-normalised (the product commutes,
+        double* x = p.sigx + ((size_t)s * A + a) * H;   // so these are ply_advance's bits); the agent's own row as it is
+        en_update_row(x, H, [&](int h) { return b[pl * H + h]; });
+        for (int k = 0; k < 2; ++k)
+          for (int h = 0; h < H; ++h) wb[((size_t)ws * 2 + k) * H + h] = (real)(k == pl ? x[h] : b[k * H + h]);
+        continue;
+      }
       const double* sx = p.sigx + ((size_t)s * A + a) * H;
       for (int k = 0; k < 2; ++k) {                  // sp_normalize of row k (LBR's row times the agent's strategy)
         const double* bk = b + k * H;
@@ -225,8 +246,12 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
       terminal = true;
     } else {                                         // the chosen raise's what-if subgame is the agent's next subgame
       const double* sx = p.sigx + ((size_t)s * A + a) * H;
-      for (int h = 0; h < H; ++h) bel[actor * H + h] *= sx[h];
-      sp_normalize(bel, H); sp_normalize(bel + H, H);
+      if (p.every_node) {                            // lbr_begin left the agent's updated row for LBR's seat there
+        for (int h = 0; h < H; ++h) bel[actor * H + h] = sx[h];
+      } else {
+        for (int h = 0; h < H; ++h) bel[actor * H + h] *= sx[h];
+        sp_normalize(bel, H); sp_normalize(bel + H, H);
+      }
       w += a - lo; lb = a; root_player = actor ^ 1; ++round;
       if (traced) {
         const size_t rec = (size_t)g * A + round;
@@ -235,6 +260,38 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
         q.tr_rounds[g] = round + 1;
       }
     }
+  }
+  if (p.every_node && !terminal) {                   // the subgame in slot w is rooted at the slot's node (lb, root_player)
+    const int lo = lb < 0 ? 0 : lb + 1, nc = q.nchild[q.tmpl[lb + 1].node_off];
+    const real* T = tb.table[0] + (size_t)w * q.table_stride;
+    const bool norm = tb.normalise[0] != 0, untouched = norm && q.steps[0][2 * w + root_player] == 0;
+    auto sig = [&](int h, int j) { return en_root_sig(T, H, nc, norm, untouched, h, j); };
+    if (root_player != me) {                         // phase 1: the agent's root row for LBR's seat, per raise
+      for (int a = lo; a <= A - 2; ++a)
+        for (int h = 0; h < H; ++h) p.sigx[((size_t)s * A + a) * H + h] = sig(h, a - lo);
+      p.pend[s] = 1;
+      atomicAdd(q.left, 1);
+      return;
+    }
+    const int j = sp_discrete(rng, nc, [&](int i) { return sig(hand_a, i); });   // the agent acts at the root
+    trace_ply(0, lb, me, hand_a, lo + j, sig(hand_a, j));
+    en_update_row(bel + me * H, H, [&](int h) { return sig(h, j); });
+    for (int h = 0; h < H; ++h) beta[h] *= sig(h, j);
+    double sum = 0;
+    for (int h = 0; h < H; ++h) sum += beta[h];
+    for (int h = 0; h < H; ++h) beta[h] /= sum;
+    prev_bid = lb; caller = me; lb = lo + j; ++ply;
+    if (lb == A - 2) {                               // LBR has no raise: it calls
+      const int a = decide(lb, [](int, int&, int&, int&) {});
+      trace_ply(1, lb, me ^ 1, hand_l, a, 1.0);
+      prev_bid = lb; caller = me ^ 1; ++ply;
+    } else if (lb < A - 2) {                         // LBR's next decision waits for phase 1
+      q.last_bid[s] = lb; q.player[s] = me ^ 1; q.ply[s] = ply; q.round[s] = round + 1;
+      q.mt_idx[s] = rng.idx;
+      atomicAdd(q.left, 1);
+      return;
+    }
+    terminal = true;
   }
   int depth = 0;
   if (!terminal) {

@@ -32,6 +32,25 @@ namespace cfrb {
 
 constexpr int kPlySampled = 1, kPlyEveryNode = 2;   // CFRB_MATCH_SAMPLED, CFRB_MATCH_EVERY_NODE
 
+// An every-node agent's probability of edge j for hand h at the root of its subgame, whose table is T (row j = edge j): normalised
+// as rec_expand_kernel does it (uniform while `untouched`, before the mover's first update; FP: Sg as it is).  The LBR walk
+// (lbr_kernels.cuh) reads every-node rows through this too.
+template <typename real>
+__device__ __forceinline__ double en_root_sig(const real* T, int H, int nc, bool normalise, bool untouched, int h, int j) {
+  const double v = (double)T[(size_t)j * H + h];
+  if (!normalise) return v;
+  double sum = 0;
+  for (int i = 0; i < nc; ++i) sum += (double)T[(size_t)i * H + h];
+  return (sum > 0 && !untouched) ? v / sum : 1.0 / nc;
+}
+
+// An every-node agent's update of the mover's belief row after an action: times sig(h), then eps-normalised.
+template <typename Sig>
+__device__ __forceinline__ void en_update_row(double* row, int H, Sig sig) {
+  for (int h = 0; h < H; ++h) row[h] *= sig(h);
+  sp_normalize(row, H);
+}
+
 // Does agent k solve at slot s this round?  An every-node agent at every node, a to-leaf one when it has no solved subgame there.
 __device__ __forceinline__ bool ply_solves(const MatchDev& p, int k, int s) {
   return p.game[s] >= 0 && (p.policy[k] == kPlyEveryNode || p.sub_node[k][s] < 0);
@@ -192,15 +211,10 @@ __global__ void __launch_bounds__(128) ply_advance_kernel(MatchDev p, MatchTabs<
       c[k] = p.cache[k] + (size_t)s * p.table_stride + (size_t)(cb - 1) * H;
     }
   }
-  // agent k's probability of edge j for hand h: the every-node root row normalised as rec_expand_kernel does it (uniform until
-  // the mover's first update; FP: Sg as it is), or the cached entry
+  // agent k's probability of edge j for hand h: the every-node root row (en_root_sig), or the cached entry
   auto sig = [&](int k, int h, int j) -> double {
     if (c[k]) return c[k][(size_t)j * H + h];
-    const double v = (double)T[k][(size_t)j * H + h];
-    if (!tb.normalise[k]) return v;
-    double sum = 0;
-    for (int i = 0; i < nc; ++i) sum += (double)T[k][(size_t)i * H + h];
-    return (sum > 0 && !untouched[k]) ? v / sum : 1.0 / nc;
+    return en_root_sig(T[k], H, nc, tb.normalise[k] != 0, untouched[k], h, j);
   };
   const int j = sp_discrete(rng, nc, [&](int i) { return sig(agent, hand, i); });
   const int ply = p.ply[s], a = lo + j;
@@ -213,11 +227,11 @@ __global__ void __launch_bounds__(128) ply_advance_kernel(MatchDev p, MatchTabs<
   double* bel = p.bel + (size_t)s * 4 * H;           // [agent][player][hand]
   for (int k = 0; k < 2; ++k) {
     double* bk = bel + (k * 2 + actor) * H;
-    for (int h = 0; h < H; ++h) bk[h] *= sig(k, h, j);
     if (!c[k]) {
-      sp_normalize(bk, H);
+      en_update_row(bk, H, [&](int h) { return sig(k, h, j); });
       continue;
     }
+    for (int h = 0; h < H; ++h) bk[h] *= sig(k, h, j);
     const int node = p.sub_node[k][s], depth = p.sub_depth[k][s] + 1;
     p.sub_node[k][s] = p.child_begin[p.tmpl[p.sub_lb[k][s] + 1].node_off + node] + j;
     p.sub_depth[k][s] = depth;

@@ -87,10 +87,10 @@ struct LbrResult : MatchResult {
 // pseudo-leaf and for one per legal raise at an LBR decision on the edge of the agent's subgame), at least A - 1.
 inline int lbr_default_capacity(int slots, int num_actions) { return std::max(2 * slots, num_actions - 1); }
 
-// Local best response against one agent (cfrb_match_create_lbr): `games` games, `slots` at a time; payoff[] is the agent's.
-// max_subgames = 0 takes lbr_default_capacity.
+// Local best response against one agent playing `policy` (CFRB_MATCH_AVERAGE or CFRB_MATCH_EVERY_NODE; cfrb_match_create_lbr2):
+// `games` games, `slots` at a time; payoff[] is the agent's.  max_subgames = 0 takes lbr_default_capacity.
 inline LbrResult play_lbr(const liars_dice::RecursiveSolvingParams& cfg, int device, int games, uint64_t seed, const std::vector<float>& w,
-                          int slots, int max_subgames) {
+                          int slots, int max_subgames, int policy = CFRB_MATCH_AVERAGE) {
   if (games < 2) throw std::runtime_error("play_lbr: games must be >= 2");
   slots = std::max(1, std::min(slots, games));
   LbrResult r;
@@ -99,7 +99,7 @@ inline LbrResult play_lbr(const liars_dice::RecursiveSolvingParams& cfg, int dev
   const HandlePtr h = open_handle(liars_dice::solver_config(cfg, device, max_subgames));
   if (!w.empty()) check(cfrb_set_weights(h.get(), w.data(), w.size(), 1), "cfrb_set_weights");
   cfrb_match* raw = nullptr;
-  check(cfrb_match_create_lbr(h.get(), slots, games, seed, &raw), "cfrb_match_create_lbr");
+  check(cfrb_match_create_lbr2(h.get(), slots, games, seed, policy, &raw), "cfrb_match_create_lbr2");
   const MatchPtr m(raw);   // released before the handle it reads
   const auto t0 = std::chrono::steady_clock::now();
   while (check(cfrb_match_run(m.get(), 8, nullptr), "cfrb_match_run") > 0) {

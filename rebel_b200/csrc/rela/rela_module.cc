@@ -826,12 +826,16 @@ py::dict play_match_py(const RecursiveSolvingParams& cfg_a, const RecursiveSolvi
 }
 
 py::dict play_lbr_py(const RecursiveSolvingParams& cfg, int device, int games, uint64_t seed, py::object flat_weights, int concurrent_games,
-                     int max_subgames) {
+                     int max_subgames, const std::string& policy) {
+  const int pol = match_policy(policy, "play_lbr");
+  if (pol == CFRB_MATCH_SAMPLED)
+    throw std::runtime_error("play_lbr: policy must be 'average' or 'every_node' (LBR against the sampled policy bounds nothing: "
+                             "it would respond to a drawn snapshot the agent's opponent cannot see)");
   const std::vector<float> w = flat_of(flat_weights);
   LbrResult r;
   {
     py::gil_scoped_release nogil;
-    r = play_lbr(cfg, device, games, seed, w, concurrent_games, max_subgames);
+    r = play_lbr(cfg, device, games, seed, w, concurrent_games, max_subgames, pol);
   }
   std::vector<float> lbr(r.payoff.size());
   for (size_t i = 0; i < lbr.size(); ++i) lbr[i] = -r.payoff[i];
@@ -845,7 +849,7 @@ py::dict play_lbr_py(const RecursiveSolvingParams& cfg, int device, int games, u
   std::copy(r.plies.begin(), r.plies.end(), pl.data_ptr<int32_t>());
   d["payoff_lbr"] = p; d["plies"] = pl; d["solves"] = r.solves; d["whatif_solves"] = r.whatif_solves;
   d["deferred_slot_rounds"] = r.deferred_slot_rounds; d["max_subgames"] = r.capacity;
-  d["subgame_iters"] = r.subgame_iters; d["seconds"] = r.seconds;
+  d["subgame_iters"] = r.subgame_iters; d["seconds"] = r.seconds; d["policy"] = policy;
   return d;
 }
 
@@ -1248,11 +1252,14 @@ PYBIND11_MODULE(rela, m) {
         "solves_a, solves_b (each agent's), subgame_iters, seconds.");
   m.def("play_lbr", &play_lbr_py, py::arg("cfg"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
         py::arg("flat_weights") = py::none(), py::arg("concurrent_games") = 8192, py::arg("max_subgames") = 0,
-        "rebel_b200 extension: local best response against one agent (cfg + net, average policy) on the GPU: `games` games "
-        "(seat-swapped pairs), concurrent_games at a time, at most max_subgames subgames solved per round (0: 2 x "
-        "concurrent_games, at least A - 1).  LBR's payoff is a lower bound on the agent's exploitability.  dict: payoff_lbr "
-        "[games], plies [games], mean, stderr (over pairs), seat_means [2] (LBR in seat 0 / seat 1), solves, whatif_solves, "
-        "deferred_slot_rounds, max_subgames, subgame_iters, seconds.");
+        py::arg("policy") = "average",
+        "rebel_b200 extension: local best response against one agent (cfg + net) on the GPU: `games` games (seat-swapped pairs), "
+        "concurrent_games at a time, at most max_subgames subgames solved per round (0: 2 x concurrent_games, at least A - 1).  "
+        "The agent plays `policy`: 'average' (the recursive to-leaf policy) or 'every_node' (compute_strategy_recursive: a "
+        "subgame solved at every decision; each LBR decision with a legal raise then costs 1 + m solves); 'sampled' is refused.  "
+        "LBR's payoff is a lower bound on the agent's exploitability.  dict: payoff_lbr [games], plies [games], mean, stderr "
+        "(over pairs), seat_means [2] (LBR in seat 0 / seat 1), solves, whatif_solves, deferred_slot_rounds, max_subgames, "
+        "subgame_iters, seconds, policy.");
   m.def("exploitability_to_leaf", &exploitability_to_leaf, py::arg("cfg"), py::arg("device") = 0, py::arg("flat_weights") = py::none(),
         py::arg("wave_capacity") = 16384,
         "rebel_b200 extension: exploitability of compute_strategy_recursive_to_leaf's policy (every subgame solved for num_iters "
