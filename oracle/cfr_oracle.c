@@ -13,7 +13,7 @@
  * CFR trajectories when both are built with -ffp-contract=off — and against the committed
  * fixtures in tests/golden/ that were generated from oracle/_ref by oracle/make_golden.py.
  * Covered: game, tree, CFR (linear / vanilla / DCFR), fictitious play (linear / optimistic), terminal
- * payoffs, query rows, Net2 forward, best response / exploitability, the RlRunner walk, the
+ * payoffs, query rows, Net2 forward, best response / exploitability, the RlRunner walk (CFR or FP), the
  * sampled recursive strategies of recursive_eval and the evaluation entry points of rela/pybind.cc
  * (compute_strategy_recursive[_to_leaf], eval_net) — bit-identical to the compiled reference with
  * the zero net (eval_net's float32 mean: 1e-7 relative).
@@ -167,6 +167,7 @@ int orc_query(int D, int F, int traverser, int last_bid, int player_id, const do
 typedef struct {
   int Q, hidden, H;
   const float *w1, *b1, *g1, *be1, *w2, *b2, *g2, *be2, *w3, *b3;
+  int w3_zero;   /* every output weight is +-0: each output is exactly its bias, whatever the (finite) hidden features */
 } orc_net;
 
 static orc_net net_from_flat(const float* w, int Q, int hidden, int H) {
@@ -174,6 +175,8 @@ static orc_net net_from_flat(const float* w, int Q, int hidden, int H) {
   n.w1 = w; w += (size_t)hidden * Q; n.b1 = w; w += hidden; n.g1 = w; w += hidden; n.be1 = w; w += hidden;
   n.w2 = w; w += (size_t)hidden * hidden; n.b2 = w; w += hidden; n.g2 = w; w += hidden; n.be2 = w; w += hidden;
   n.w3 = w; w += (size_t)H * hidden; n.b3 = w;
+  n.w3_zero = 1;
+  for (size_t i = 0; i < (size_t)H * hidden; ++i) n.w3_zero &= n.w3[i] == 0.0f;
   return n;
 }
 static void linear_f(const float* x, const float* w, const float* b, int in, int out, float* y) {
@@ -198,6 +201,10 @@ static void ln_gelu_f(float* x, const float* g, const float* be, int n) {
   }
 }
 static void net_forward(const orc_net* n, const float* queries, int rows, float* out) {
+  if (n->w3_zero) {   /* acc = b3 + sum of +-0 products == b3 bit for bit: skip the hidden layers (a constant-output net) */
+    for (int r = 0; r < rows; ++r) memcpy(out + (size_t)r * n->H, n->b3, sizeof(float) * n->H);
+    return;
+  }
   float* a = (float*)malloc(sizeof(float) * n->hidden * 2);
   float* b = a + n->hidden;
   for (int r = 0; r < rows; ++r) {
@@ -680,8 +687,18 @@ static void sink_add(ex_sink* k, const float* q, const float* v) {
   ++k->n;
 }
 
+/* One iteration of the walk's solver: build_solver (subgame_solving.cc:1052-1063) returns CFR or FP. */
+static void walk_step(orc_cfr* s, int it, int use_cfr, int optimistic) {
+  if (use_cfr) orc_cfr_step(s, it % 2); else orc_fp_step(s, it % 2, optimistic);
+}
+
+/* RlRunner::step `n_games` times (stopping early after `max_subgames` solved subgames when it is > 0).  The solver is CFR
+ * (linear, plain or DCFR) with use_cfr, fictitious play otherwise.  trace (optional): one row per solved subgame, [trace_cap][5]
+ * int32 = game index, root last_bid, root player, act_iteration, br_sampler.  Returns the number of examples (two per subgame). */
 int orc_rl_runner(int D, int F, int num_iters, int max_depth, int linear_update, float random_action_prob, int sample_leaf,
-                  int seed, int n_games, const float* net_w, int hidden, float* q_out, float* v_out, int cap) {
+                  int seed, int n_games, const float* net_w, int hidden, float* q_out, float* v_out, int cap,
+                  int use_cfr, int optimistic, int dcfr, double dcfr_alpha, double dcfr_beta, double dcfr_gamma,
+                  int max_subgames, int32_t* trace, int trace_cap) {
   orc_game g = game_make(D, F);
   int H = g.H, A = g.A, Q = 2 + A + 2 * H;
   ex_sink sink = {q_out, v_out, 0, cap, Q, H};
@@ -689,17 +706,27 @@ int orc_rl_runner(int D, int F, int num_iters, int max_depth, int linear_update,
   double* beliefs = (double*)malloc(sizeof(double) * 2 * H);
   double* sb = (double*)malloc(sizeof(double) * 2 * H);
   float* qrow = (float*)malloc(sizeof(float) * Q); float* vrow = (float*)malloc(sizeof(float) * H);
-  for (int game_i = 0; game_i < n_games; ++game_i) {   /* RlRunner::step :160-182 */
+  if (!use_cfr) dcfr = 0;
+  int solved = 0;
+  for (int game_i = 0; game_i < n_games && !(max_subgames > 0 && solved >= max_subgames); ++game_i) {   /* RlRunner::step :160-182 */
     int last_bid = -1, player = 0;
     for (int i = 0; i < 2 * H; ++i) beliefs[i] = 1.0 / H;
-    while (!game_is_terminal(&g, last_bid)) {
-      orc_cfr* s = orc_cfr_create(D, F, last_bid, player, beliefs, num_iters, max_depth, linear_update, 0, 0, 0, 0, net_w, hidden);
+    while (!game_is_terminal(&g, last_bid) && !(max_subgames > 0 && solved >= max_subgames)) {
+      orc_cfr* s = orc_cfr_create(D, F, last_bid, player, beliefs, num_iters, max_depth, linear_update, dcfr, dcfr_alpha, dcfr_beta,
+                                  dcfr_gamma, net_w, hidden);
       int act_iteration = uniform_int(&gen, 0, num_iters);
-      for (int it = 0; it < act_iteration; ++it) orc_cfr_step(s, it % 2);
+      int32_t* tr = trace && solved < trace_cap ? trace + 5 * (size_t)solved : 0;
+      if (tr) { tr[0] = game_i; tr[1] = last_bid; tr[2] = player; tr[3] = act_iteration; tr[4] = -1; }
+      ++solved;
+      for (int it = 0; it < act_iteration; ++it) walk_step(s, it, use_cfr, optimistic);
+      /* get_sampling_strategy = get_belief_propogation_strategy: CFR's last strategies, FP's average strategies (the
+       * ISubgameSolver defaults, subgame_solving.h:76-83) */
+      const double* sigma = use_cfr ? s->last : s->avg;
       if (sample_leaf) {   /* sample_state_to_leaf :192-246 */
         int path_n[64], path_a[64], plen = 0;
         int node = 0;
         int br_sampler = uniform_int(&gen, 0, 1);
+        if (tr) tr[4] = br_sampler;
         memcpy(sb, beliefs, sizeof(double) * 2 * H);
         while (s->tree[node].children_end - s->tree[node].children_begin) {
           float eps = canonical_f(&gen);
@@ -709,36 +736,38 @@ int orc_rl_runner(int D, int F, int num_iters, int max_depth, int linear_update,
             action = uniform_int(&gen, lo, hi - 1);
           } else {
             int hand = discrete(&gen, sb + pid * H, H);
-            action = discrete(&gen, s->last + IDX3(s, node, hand, 0), A);
+            action = discrete(&gen, sigma + IDX3(s, node, hand, 0), A);
           }
-          for (int h = 0; h < H; ++h) sb[pid * H + h] *= s->last[IDX3(s, node, h, action)];
+          for (int h = 0; h < H; ++h) sb[pid * H + h] *= sigma[IDX3(s, node, h, action)];
           normalize_safe_d(sb + pid * H, H, 1e-80);
           path_n[plen] = node; path_a[plen] = action; ++plen;
           node = s->tree[node].children_begin + action - lo;
         }
         for (int i = 0; i < plen; ++i) {   /* second pass :235-245 */
           int lo, hi; game_bid_range(&g, last_bid, &lo, &hi);
-          for (int h = 0; h < H; ++h) beliefs[player * H + h] *= s->last[IDX3(s, path_n[i], h, path_a[i])];
+          for (int h = 0; h < H; ++h) beliefs[player * H + h] *= sigma[IDX3(s, path_n[i], h, path_a[i])];
           normalize_safe_d(beliefs + player * H, H, 1e-80);
           int child = s->tree[path_n[i]].children_begin + path_a[i] - lo;
           last_bid = s->tree[child].last_bid; player = s->tree[child].player_id;
         }
       } else {             /* sample_state_single :248-275 */
         int br_sampler = uniform_int(&gen, 0, 1);
+        if (tr) tr[4] = br_sampler;
         float eps = canonical_f(&gen);
         int lo, hi, action; game_bid_range(&g, last_bid, &lo, &hi);
         if (player == br_sampler && eps < random_action_prob) {
           action = uniform_int(&gen, lo, hi - 1);
         } else {
           int hand = discrete(&gen, beliefs + player * H, H);
-          action = discrete(&gen, s->last + IDX3(s, 0, hand, 0), A);
+          action = discrete(&gen, sigma + IDX3(s, 0, hand, 0), A);
         }
-        for (int h = 0; h < H; ++h) beliefs[player * H + h] *= s->last[IDX3(s, 0, h, action)];
+        for (int h = 0; h < H; ++h) beliefs[player * H + h] *= sigma[IDX3(s, 0, h, action)];
         normalize_safe_d(beliefs + player * H, H, 1e-80);
         last_bid = action; player = 1 - player;
       }
-      for (int it = act_iteration; it < num_iters; ++it) orc_cfr_step(s, it % 2);
-      /* update_value_network :672-676 -> add_training_example :220-226 */
+      for (int it = act_iteration; it < num_iters; ++it) walk_step(s, it, use_cfr, optimistic);
+      /* update_value_network (CFR :672-676, FP :471-474 through its BRSolver, whose reaches are those of the last step) ->
+       * add_training_example :220-226 */
       for (int t = 0; t < 2; ++t) {
         write_query(&g, t, s->tree[0].last_bid, s->tree[0].player_id, s->reach[0], s->reach[1], qrow);
         for (int h = 0; h < H; ++h) vrow[h] = (float)s->root_means[t][h];

@@ -197,16 +197,28 @@ class Oracle:
         f(int(model))
 
     def rl_runner(self, D, F, seed, n_games, num_iters=1024, max_depth=2, linear_update=True,
-                  random_action_prob=0.25, sample_leaf=True, net_w=None, hidden=256, cap=4096, use_cfr=True):
+                  random_action_prob=0.25, sample_leaf=True, net_w=None, hidden=256, cap=4096, use_cfr=True, optimistic=False,
+                  dcfr=False, dcfr_alpha=0.0, dcfr_beta=0.0, dcfr_gamma=0.0, max_subgames=0, trace=False):
+        """RlRunner::step n_games times (recursive_solving.cc:160-182): the training examples (q [n, Q], v [n, H]), two per solved
+        subgame.  use_cfr=False is fictitious play (optimistic applies), use_cfr with dcfr is DCFR(alpha, beta, gamma).
+        Port only: max_subgames > 0 stops after that many subgames, and trace=True also returns one int32 row per subgame:
+        (game index, root last_bid, root player, act_iteration, br_sampler)."""
         A, H, Q = game_dims(D, F)
         q = np.zeros((cap, Q), np.float32)
         v = np.zeros((cap, H), np.float32)
+        tr = np.zeros((cap // 2 + 1, 5), np.int32) if trace else None
         w = None if net_w is None else np.ascontiguousarray(net_w, np.float32)
-        f = self._f("rl_runner" if use_cfr else "rl_runner_fp")      # the FP walk exists in the reference builds only
-        f.argtypes = [C.c_int] * 5 + [C.c_float] + [C.c_int] * 3 + [_fp, C.c_int, _fp, _fp, C.c_int]
+        f = self._f("rl_runner")
+        f.argtypes = [C.c_int] * 5 + [C.c_float] + [C.c_int] * 3 + [_fp, C.c_int, _fp, _fp] + [C.c_int] * 4 + [C.c_double] * 3 + \
+            [C.c_int, _ip, C.c_int]
         n = f(D, F, num_iters, max_depth, int(linear_update), random_action_prob, int(sample_leaf), seed, n_games,
-              _ptr(w, _fp), hidden, _ptr(q, _fp), _ptr(v, _fp), cap)
-        assert 0 <= n <= cap, n
+              _ptr(w, _fp), hidden, _ptr(q, _fp), _ptr(v, _fp), cap, int(use_cfr), int(optimistic), int(dcfr), float(dcfr_alpha),
+              float(dcfr_beta), float(dcfr_gamma), int(max_subgames), _ptr(tr, _ip), 0 if tr is None else len(tr))
+        if n < 0:
+            raise RuntimeError(self._f("last_error")().decode())
+        assert n <= cap, (n, cap)
+        if trace:
+            return q[:n].copy(), v[:n].copy(), tr[:n // 2].copy()
         return q[:n].copy(), v[:n].copy()
 
     def sampled_strategy(self, D, F, seed, num_iters=1024, max_depth=2, linear_update=True, net_w=None, hidden=256):

@@ -433,27 +433,19 @@ int ref_exploitability(int D, int F, const double* strategy, double* out2) {
   }
 }
 
-// Runs RlRunner::step (recursive_solving.cc:160-182) `n_games` times with seed, recording every
-// training example.  net_w == nullptr -> zero net.  Returns #examples, fills up to cap.
-static int rl_runner_impl(int D, int F, int num_iters, int max_depth, int linear_update, float random_action_prob,
-                          int sample_leaf, int seed, int n_games, const float* net_w, int hidden, float* q_out, float* v_out,
-                          int cap, bool use_cfr);
-int ref_rl_runner(int D, int F, int num_iters, int max_depth, int linear_update,
-                  float random_action_prob, int sample_leaf, int seed, int n_games,
-                  const float* net_w, int hidden, float* q_out, float* v_out, int cap) {
-  return rl_runner_impl(D, F, num_iters, max_depth, linear_update, random_action_prob, sample_leaf, seed, n_games, net_w, hidden,
-                        q_out, v_out, cap, true);
-}
-// Same walk with the fictitious-play solver (SubgameSolvingParams::use_cfr = false, the YAML default).
-int ref_rl_runner_fp(int D, int F, int num_iters, int max_depth, int linear_update,
-                     float random_action_prob, int sample_leaf, int seed, int n_games,
-                     const float* net_w, int hidden, float* q_out, float* v_out, int cap) {
-  return rl_runner_impl(D, F, num_iters, max_depth, linear_update, random_action_prob, sample_leaf, seed, n_games, net_w, hidden,
-                        q_out, v_out, cap, false);
-}
-static int rl_runner_impl(int D, int F, int num_iters, int max_depth, int linear_update, float random_action_prob,
-                          int sample_leaf, int seed, int n_games, const float* net_w, int hidden, float* q_out, float* v_out,
-                          int cap, bool use_cfr) {
+// Runs RlRunner::step (recursive_solving.cc:160-182) `n_games` times with seed, recording every training example.  net_w ==
+// nullptr -> zero net.  use_cfr = false is the fictitious-play solver (SubgameSolvingParams::use_cfr = false, the YAML default).
+// Same signature as orc_rl_runner; the subgame limit and the per-subgame trace are the port's alone (max_subgames must be 0 and
+// trace null here).  Returns #examples, fills up to cap.
+int ref_rl_runner(int D, int F, int num_iters, int max_depth, int linear_update, float random_action_prob, int sample_leaf, int seed,
+                  int n_games, const float* net_w, int hidden, float* q_out, float* v_out, int cap, int use_cfr, int optimistic,
+                  int dcfr, double dcfr_alpha, double dcfr_beta, double dcfr_gamma, int max_subgames, int32_t* trace,
+                  int trace_cap) {
+  (void)trace_cap;
+  if (max_subgames != 0 || trace) {
+    g_err = "ref_rl_runner: max_subgames and trace are not available in the reference build";
+    return -1;
+  }
   try {
     Game game(D, F);
     const int H = game.num_hands(), A = game.num_actions(), Q = 2 + A + 2 * H;
@@ -462,8 +454,9 @@ static int rl_runner_impl(int D, int F, int num_iters, int max_depth, int linear
     cfg.num_faces = F;
     cfg.random_action_prob = random_action_prob;
     cfg.sample_leaf = sample_leaf != 0;
-    cfg.subgame_params = make_params(num_iters, max_depth, linear_update, 0, 0, 0, 0);
-    cfg.subgame_params.use_cfr = use_cfr;
+    cfg.subgame_params = make_params(num_iters, max_depth, linear_update, use_cfr ? dcfr : 0, dcfr_alpha, dcfr_beta, dcfr_gamma);
+    cfg.subgame_params.use_cfr = use_cfr != 0;
+    cfg.subgame_params.optimistic = optimistic != 0;
     std::vector<float>*eq, *ev;
     std::shared_ptr<IValueNet> net;
     if (net_w) {

@@ -193,6 +193,58 @@ def test_selfplay_walk_bit_exact_vs_golden(port, golden):
             assert np.array_equal(q, g[f"q_{D}x{F}_{sl}"]) and np.array_equal(v, g[f"v_{D}x{F}_{sl}"])
 
 
+@pytest.mark.parametrize("D,F", SHAPES)
+def test_selfplay_walk_fictitious_play_bit_exact_vs_golden(port, golden, D, F):
+    """The port's walk with the FP solver (use_cfr = False): sampling and belief propagation with FP's average strategies, the
+    examples from its best-response pass, bit-identical to the reference's RlRunner(seed = 7) stream."""
+    g = golden("selfplay_zero.npz")
+    q, v = port.rl_runner(D, F, seed=7, n_games=4, num_iters=32, sample_leaf=True, use_cfr=False)
+    assert np.array_equal(q, g[f"q_fp_{D}x{F}"]) and np.array_equal(v, g[f"v_fp_{D}x{F}"])
+
+
+def test_selfplay_walk_beyond_nine_hands_bit_exact_vs_golden(port, golden):
+    """The port's walk against the compiled reference's RlRunner at 7x1f, 2x6f, 1x17f, 3x4f and 4x3f (up to 81 hands and 35
+    actions): CFR linear, plain and DCFR, linear FP, sample_leaf on and off, the zero net and a constant-output Net2
+    (selfplay_large.npz, oracle/make_golden_r4.py)."""
+    from oracle import make_golden_r4 as r4
+    g = golden("selfplay_large.npz")
+    keys = set()
+    for c in r4.cases():
+        k = r4.case_key(*c)
+        q, v = r4.stream(port, *c)
+        assert len(q) >= 2 * r4.GAMES_PER_STREAM, (k, len(q))
+        assert np.array_equal(q, g["q_" + k]) and np.array_equal(v, g["v_" + k]), k
+        keys |= {"q_" + k, "v_" + k}
+    assert keys == set(g.files)
+
+
+def test_selfplay_walk_trace_and_subgame_limit(port):
+    """rl_runner(trace=True): one row per solved subgame, (game, root last_bid, root player, act_iteration, br_sampler), in the
+    order of the examples; max_subgames cuts the same stream short."""
+    D, F, iters = 2, 3, 3
+    A, H, Q = game_dims(D, F)
+    for sl in (True, False):
+        q, v, tr = port.rl_runner(D, F, seed=11, n_games=6, num_iters=iters, sample_leaf=sl, trace=True, cap=4096)
+        assert tr.shape == (len(q) // 2, 5) and len(q) % 2 == 0
+        assert np.array_equal(np.unique(tr[:, 0]), np.arange(6))
+        assert np.all(np.diff(tr[:, 0]) >= 0)
+        first = np.r_[True, np.diff(tr[:, 0]) > 0]                        # every game starts at the initial state
+        assert np.all(tr[first, 1] == -1) and np.all(tr[first, 2] == 0)
+        assert np.all((tr[:, 3] >= 0) & (tr[:, 3] <= iters)) and {0, iters} <= set(tr[:, 3].tolist())
+        assert set(tr[:, 4].tolist()) <= {0, 1}
+        # the trace's root is the root of the examples: player and the one-hot last bid of both queries of each subgame
+        for t in range(2):
+            assert np.array_equal(q[t::2, 0], tr[:, 2].astype(np.float32)) and np.all(q[t::2, 1] == t)
+            onehot = q[t::2, 2:2 + A]
+            assert np.array_equal(np.where(onehot.any(1), onehot.argmax(1), -1), tr[:, 1])
+        if not sl:                                                         # one action per subgame: the bids rise by player
+            same = ~first[1:]
+            assert np.all(tr[1:, 1][same] > tr[:-1, 1][same]) and np.all(tr[1:, 2][same] != tr[:-1, 2][same])
+        n = len(tr) // 2
+        q2, v2, tr2 = port.rl_runner(D, F, seed=11, n_games=6, num_iters=iters, sample_leaf=sl, trace=True, max_subgames=n)
+        assert np.array_equal(q2, q[:2 * n]) and np.array_equal(v2, v[:2 * n]) and np.array_equal(tr2, tr[:n])
+
+
 # ---------------------------------------------------------------- cross-check with the compiled reference's stored outputs
 def test_port_vs_compiled_reference_live(port, golden):
     """The port against the compiled reference (fixture reference_live.npz, oracle/make_golden.py live): synthetic beliefs,
