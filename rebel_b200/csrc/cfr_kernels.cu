@@ -13,7 +13,6 @@
 #include "agent_kernels.cuh"
 #include "ply_kernels.cuh"
 #include "expl_kernels.cuh"
-#include "expl_sampled_kernels.cuh"
 #include "full_game_kernels.cuh"
 #include "regret_grid_kernels.cuh"
 #include "fp_forest_kernels.cuh"
@@ -218,16 +217,11 @@ void rec_launch_expand(const ExplDev& p, int n, const real* table, int normalise
   rec_expand_kernel<real><<<(n + 3) / 4, 128, 0, st>>>(p, n, table, normalise);   // a warp per subgame
 }
 template <typename real>
-void expl_sampled_launch_begin(const ExplSampledDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st) {
-  expl_sampled_begin_kernel<real><<<(n + 127) / 128, 128, 0, st>>>(p, n, wave_beliefs);
-  sp_scan_kernel<<<1, 1024, 0, st>>>(scan);
-}
-template <typename real>
-void expl_sampled_launch_expand(const ExplSampledDev& p, int n, const real* snap, cudaStream_t st) {
+void expl_sampled_launch_expand(const ExplDev& p, int n, const real* snap, cudaStream_t st) {
   expl_sampled_expand_kernel<real><<<n / p.b, 128, 0, st>>>(p, snap);
-  expl_sampled_fill_kernel<<<1, 1, 0, st>>>(p);
+  expl_fill_kernel<<<1, 1, 0, st>>>(p);
 }
-void expl_sampled_launch_finalize(const ExplSampledDev& p, cudaStream_t st) {
+void expl_sampled_launch_finalize(const ExplDev& p, cudaStream_t st) {
   const size_t total = (size_t)(p.full_nodes - 1) * p.H;
   const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 8);
   expl_sampled_finalize_kernel<<<std::max(blocks, 1), 256, 0, st>>>(p);
@@ -359,8 +353,7 @@ void div_check_launch(unsigned long long seed, int blocks, unsigned long long* m
   template void expl_launch_begin<real>(const ExplDev&, const SpDev&, int, real*, cudaStream_t);                           \
   template void expl_launch_expand<real>(const ExplDev&, int, const real*, int, cudaStream_t);                              \
   template void rec_launch_expand<real>(const ExplDev&, int, const real*, int, cudaStream_t);                               \
-  template void expl_sampled_launch_begin<real>(const ExplSampledDev&, const SpDev&, int, real*, cudaStream_t);           \
-  template void expl_sampled_launch_expand<real>(const ExplSampledDev&, int, const real*, cudaStream_t);
+  template void expl_sampled_launch_expand<real>(const ExplDev&, int, const real*, cudaStream_t);
 CFRB_INSTANTIATE(float)
 CFRB_INSTANTIATE(double)
 

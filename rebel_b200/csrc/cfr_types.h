@@ -272,50 +272,22 @@ template <typename real> void agent_launch_begin(const AgentDev& p, const MatchT
 template <typename real> void agent_launch_capture(const AgentDev& p, const MatchTabs<real>& t, cudaStream_t st);
 void agent_launch_step(const AgentDev& p, cudaStream_t st);
 void agent_launch_policy(const AgentDev& p, cudaStream_t st);
-// Recursive to-leaf walk (expl_kernels.cuh): one wave of a level of subgames, rooted at full-tree nodes, solved by one handle.
+// Device walks (expl_kernels.cuh): one wave of a level of subgames, rooted at full-tree nodes, solved by
+// one handle.  The sampled walk walks b repeats: a level lists its root groups in full-tree node order, each the b repeats of one
+// root, so position pos is repeat pos % b of group pos / b.  The other walks leave its fields null / zero.  (In this field order
+// ptxas keeps expl_sampled_expand_kernel free of spills.)
 struct ExplDev {
-  int H;
-  // the full tree (BrState of the handle) and the compact full-tree strategy [N_full - 1][H] the walk fills
-  const int* full_child_begin; const int* full_depth; const int* full_act_lo;
-  double* strategy;
+  int H, A, b;
+  // the full tree (BrState of the handle); the sampled walk's accumulators and strategies index its parents and size
+  const int* full_child_begin; const int* full_depth; const int* full_act_lo; const int* full_parent;
+  int full_nodes;
   // the handle's subgame templates
   const TemplateDev* tmpl; const int* parent; const int* child_begin; const int* nchild; const int* level_begin;
   const int* pleaf_node;
   // the handle's wave descriptors and CFR step counters
   int* sg_tmpl; int* sg_player; int* sg_act; const int* sg_row_off; const int* wave; const int* steps;
   int table_stride;
-  // this level's roots [n_level] and fp64 beliefs [n_level][2][H]; the wave is entries off .. off + n - 1
-  const int* roots; const double* bel;
-  int off;
-  // the next level: cap entries, fill [1] of them written by the level's earlier waves
-  int* next_roots; double* next_bel;
-  int* fill;
-  int cap;
-  int* fid; int nmax;                 // [K][nmax] scratch: full-tree node of every template node of each subgame
-  // the every-node walk (rec_expand_kernel): the full tree's child counts [N] and depth levels [levels + 1]
-  const int* full_nchild; const int* full_level_begin;
-};
-// wave descriptors (template, player, root beliefs as `real`), row offsets and schedule of the level's subgames off .. off + n - 1
-template <typename real> void expl_launch_begin(const ExplDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st);
-// the solved wave's strategy into p.strategy, its pseudo-leaves onto the next level
-template <typename real> void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
-// every-node walk: the solved wave's root rows into p.strategy, their non-terminal children onto the next level
-template <typename real> void rec_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
-// Sampled recursive to-leaf walk (expl_sampled_kernels.cuh): the waves of one level of a batch of b repeats.  A level lists its
-// root groups in full-tree node order, each group the b repeats of one root in repeat order, so level position pos is repeat
-// pos % b of group pos / b.
-struct ExplSampledDev {
-  int H, A, b;
-  // the full tree (BrState of the handle): the accumulators, the final strategy and the last repeat's sampled strategy index it
-  const int* full_child_begin; const int* full_depth; const int* full_act_lo; const int* full_parent;
-  int full_nodes;
-  // the handle's subgame templates
-  const TemplateDev* tmpl; const int* parent; const int* child_begin; const int* nchild; const int* level_begin;
-  const int* pleaf_node;
-  // the handle's wave descriptors
-  int* sg_tmpl; int* sg_player; int* sg_act; const int* sg_row_off; const int* wave;
-  int table_stride;
-  // act_iteration of (repeat j, global level position g of its root group) = draws[j * draws_stride + level_base + g]
+  // act_iteration of (repeat j, global level position g of its root group) = draws[j * draws_stride + level_base + g], or -1
   const int* draws; long long draws_stride; int level_base;
   // this level's roots [n_level], fp64 beliefs and reach [n_level][2][H]; the wave is positions off .. off + n - 1 (whole groups)
   const int* roots; const double* bel; const double* rch;
@@ -332,15 +304,20 @@ struct ExplSampledDev {
   // with regrets tracked: every repeat j of the batch writes (float)s of its sampled strategy into rep_s + j * rep_stride,
   // compact [N_full - 1][H] (nullptr: not tracked)
   float* rep_s; size_t rep_stride;
-  double* strategy;                   // the compact full-tree strategy the best response reads [N_full - 1][H]
+  double* strategy;                   // the compact full-tree strategy the walk fills and the best response reads [N_full - 1][H]
+  // the every-node walk (rec_expand_kernel): the full tree's child counts [N] and depth levels [levels + 1]
+  const int* full_nchild; const int* full_level_begin;
 };
 // wave descriptors (template, player, act_iteration, root beliefs as `real`), row offsets and schedule of positions off .. off + n - 1
-template <typename real> void expl_sampled_launch_begin(const ExplSampledDev& p, const SpDev& scan, int n, real* wave_beliefs,
-                                                        cudaStream_t st);
-// the solved wave's snapshot strategies into the accumulators, its pseudo-leaves (beliefs and reach) onto the next level
-template <typename real> void expl_sampled_launch_expand(const ExplSampledDev& p, int n, const real* snap, cudaStream_t st);
+template <typename real> void expl_launch_begin(const ExplDev& p, const SpDev& scan, int n, real* wave_beliefs, cudaStream_t st);
+// the solved wave's strategy into p.strategy, its pseudo-leaves onto the next level
+template <typename real> void expl_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
+// every-node walk: the solved wave's root rows into p.strategy, their non-terminal children onto the next level
+template <typename real> void rec_launch_expand(const ExplDev& p, int n, const real* table, int normalise, cudaStream_t st);
+// sampled walk: the solved wave's snapshot strategies into the accumulators, its pseudo-leaves (beliefs and reach) onto the next level
+template <typename real> void expl_sampled_launch_expand(const ExplDev& p, int n, const real* snap, cudaStream_t st);
 // strategy = (double)(sum_s / (sum_r[parent] + 1e-6f)), the final strategy of a checkpoint
-void expl_sampled_launch_finalize(const ExplSampledDev& p, cudaStream_t st);
+void expl_sampled_launch_finalize(const ExplDev& p, cudaStream_t st);
 // Full-game solver (full_game_kernels.cuh): CFR or FP on the full tree of the handle's game (BrState), fp64, one level per launch.
 struct FullGameDev {
   int N, T, H, F;

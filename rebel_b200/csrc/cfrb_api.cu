@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <array>
 #include <cstring>
+#include <functional>
 #include <limits>
 #include <memory>
 #include <random>
@@ -1879,8 +1880,11 @@ int cfrb_debug_to_leaf_free_cap(cfrb_handle* h, int64_t bytes) {
 
 // Refusals shared by the device walks, in this order: more than CFRB_TO_LEAF_MAX_ACTIONS actions, a handle in a live match or
 // agent, a net without weights, and a need above the free bytes -- all before anything is allocated, since on a shared device an
-// allocation that fails late may starve other processes.  Then the full tree (full_tree_setup).
-static int walk_admit(cfrb_handle* h, const char* who, int64_t tree_bytes, int64_t walk_bytes) {
+// allocation that fails late may starve other processes.  Then the full tree (full_tree_setup).  extra_bytes: what the caller
+// allocates beside the walk, walk_note: their account in the refusal.  release_sampled frees the previous sampled walk's results
+// before the free bytes are read: the call replaces them.
+static int walk_admit(cfrb_handle* h, const char* who, int64_t tree_bytes, int64_t walk_bytes, int64_t extra_bytes = 0,
+                      const std::string& walk_note = std::string(), bool release_sampled = false) {
   const auto& g = h->g;
   const std::string w(who);
   if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
@@ -1890,20 +1894,21 @@ static int walk_admit(cfrb_handle* h, const char* who, int64_t tree_bytes, int64
   if (h->cfg.net_mode != CFRB_NET_ZERO && !h->have_weights && h->Lmax > 0)
     return fail(CFRB_ESTATE, w + ": value-net weights not set (cfrb_set_weights)");
   CK(cudaSetDevice(h->cfg.device));
-  const int64_t tree = h->br.ready ? 0 : tree_bytes, need = tree + walk_bytes;
+  CK(cudaStreamSynchronize(h->own_stream));
+  if (release_sampled) h->smp = cfrb_handle::SampledState();
+  const int64_t tree = h->br.ready ? 0 : tree_bytes, need = tree + walk_bytes + extra_bytes;
   size_t free_b = 0, total_b = 0;
   CK(cudaMemGetInfo(&free_b, &total_b));
   int64_t avail = (int64_t)free_b;
   if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
   if (need > avail)
     return fail(CFRB_ENOMEM, w + ": needs " + std::to_string(need) + " bytes of device memory beyond the handle (full tree and "
-                             "best-response scratch " + std::to_string(tree) + ", walk " + std::to_string(walk_bytes) + "), " +
-                             std::to_string(avail) + " free");
+                             "best-response scratch " + std::to_string(tree) + ", walk " + std::to_string(walk_bytes) + walk_note +
+                             "), " + std::to_string(avail) + " free");
   return full_tree_setup(h, who);
 }
 
-// The walks' view of the handle: its full tree, compact strategy, templates and wave descriptors (ExplDev), and sp_scan_kernel's
-// view of the wave.
+// The walks' view of the handle: its full tree, compact strategy, templates and wave descriptors.
 static cfrb::ExplDev walk_dev(cfrb_handle* h) {
   cfrb::ExplDev d{};
   d.H = h->g.H;
@@ -1915,13 +1920,79 @@ static cfrb::ExplDev walk_dev(cfrb_handle* h) {
   d.wave = h->d_wave.p; d.steps = h->d_steps.p; d.table_stride = h->table_stride;
   return d;
 }
-static cfrb::SpDev walk_scan(cfrb_handle* h) {
-  cfrb::SpDev scan{};
-  scan.A = h->g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
-  scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
-  scan_wide(h, scan);
-  return scan;
-}
+
+// The level walk of the device walks (K8, K8e, K8s): two levels of roots, fp64 beliefs and (sampled walk) reach.  run() walks b
+// repeats (b > 1 in the sampled walk only) from level 0, b copies of the game root with uniform beliefs and reach, in waves of
+// whole root groups, at most (K / b) * b subgames: expl_begin + sp_scan, solve_device_wave, then the walk's expand, which appends
+// the next level at fill.  Each level's size is checked against the tree's, C(A - 1, depth) * b.
+struct LevelWalk {
+  const char* who;
+  int step = 1;                 // full-tree depth from one level to the next: max_depth, or 1 for the every-node walk
+  bool drop_sum = false;        // solve_device_wave's: the expand does not read the sum table
+  int expand_launches = 2;
+  std::function<void(int n)> expand;   // the expand launch of a solved wave of n subgames
+  std::function<int(int off, int n)> iters;   // the iterations of the wave at positions off .. off + n - 1 (unset: num_iters)
+  std::function<int(const int* roots, int n)> level_done;   // after a level's check, with its n roots on the device (or unset)
+  DevBuf<int> roots[2], fill;
+  DevBuf<double> bel[2], rch[2];
+  int64_t cap = 0;
+
+  int alloc(int64_t level_cap, int W, bool reach) {
+    cap = level_cap;
+    for (int i = 0; i < 2; ++i) {
+      CK(roots[i].alloc(cap)); CK(bel[i].alloc((size_t)cap * W));
+      if (reach) CK(rch[i].alloc((size_t)cap * W));
+    }
+    CK(fill.alloc(1));
+    return CFRB_OK;
+  }
+
+  int run(cfrb_handle* h, cfrb::ExplDev& d, int b, int64_t& solved) {
+    cudaStream_t st = h->own_stream;
+    const int H = h->g.H, Kw = (h->cfg.max_subgames / b) * b;
+    const std::vector<int> zeros(b, 0);
+    const std::vector<double> uniform((size_t)b * 2 * H, 1.0 / H);
+    CK(cudaMemcpyAsync(roots[0].p, zeros.data(), b * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bel[0].p, uniform.data(), uniform.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    if (rch[0].p) CK(cudaMemcpyAsync(rch[0].p, uniform.data(), uniform.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    cfrb::SpDev scan{};   // sp_scan_kernel's view of the wave
+    scan.A = h->g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
+    scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
+    scan_wide(h, scan);
+    d.fill = fill.p; d.cap = cap; d.level_base = 0;
+    int rc = CFRB_OK, cur = 0, n_level = b;
+    for (int depth = 0; n_level > 0; depth += step) {
+      d.roots = roots[cur].p; d.bel = bel[cur].p; d.rch = rch[cur].p;
+      d.next_roots = roots[cur ^ 1].p; d.next_bel = bel[cur ^ 1].p; d.next_rch = rch[cur ^ 1].p;
+      CK(cudaMemsetAsync(fill.p, 0, sizeof(int), st));
+      for (int off = 0; off < n_level; off += Kw) {
+        const int n = std::min(Kw, n_level - off);
+        const int wave_iters = iters ? iters(off, n) : -1;
+        d.off = off; scan.K = n;
+        with_state(h, [&](auto& s) { cfrb::expl_launch_begin(d, scan, n, s.beliefs.p, st); });
+        h->launches += 2;
+        CK(cudaGetLastError());
+        if ((rc = solve_device_wave(h, n, true, drop_sum, st, wave_iters))) return rc;
+        expand(n);
+        h->launches += expand_launches;
+        CK(cudaGetLastError());
+      }
+      solved += n_level;
+      int next = 0;
+      CK(cudaMemcpyAsync(&next, fill.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      const int64_t want = binom(h->g.A - 1, depth + step) * b;
+      if (next != want)
+        return fail(CFRB_ECUDA, std::string(who) + ": level at depth " + std::to_string(depth + step) + " has " +
+                                    std::to_string(next) + " subgames, the tree " + std::to_string(want));
+      if (level_done && (rc = level_done(d.roots, n_level))) return rc;
+      d.level_base += n_level / b;   // the root groups of the levels walked so far
+      n_level = next;
+      cur ^= 1;
+    }
+    return CFRB_OK;
+  }
+};
 
 // Both best responses on the walk's compact strategy, and the walks' outputs.  t0: the walk's start; the walk ends here.
 static int walk_finish(cfrb_handle* h, std::chrono::steady_clock::time_point t0, int64_t solved, double* br_out2, int64_t* subgames,
@@ -1945,53 +2016,22 @@ static int walk_finish(cfrb_handle* h, std::chrono::steady_clock::time_point t0,
 
 int cfrb_to_leaf_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2) {
   if (!h || !br_out2) return fail(CFRB_EINVAL, "cfrb_to_leaf_exploitability: null argument");
-  const auto& g = h->g;
-  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H;
-  const auto sz = to_leaf_sizes(g, h->cfg.max_depth, K);
+  const int K = h->cfg.max_subgames;
+  const auto sz = to_leaf_sizes(h->g, h->cfg.max_depth, K);
   int rc = walk_admit(h, "cfrb_to_leaf_exploitability", sz.tree_bytes, sz.walk_bytes);
   if (rc) return rc;
-  cudaStream_t st = h->own_stream;
-  DevBuf<int> roots[2], fid, fill;
-  DevBuf<double> bel[2];
-  for (int i = 0; i < 2; ++i) { CK(roots[i].alloc(sz.level_cap)); CK(bel[i].alloc((size_t)sz.level_cap * W)); }
-  CK(fid.alloc((size_t)K * h->Nmax)); CK(fill.alloc(1));
+  LevelWalk w{"cfrb_to_leaf_exploitability", h->cfg.max_depth};
+  DevBuf<int> fid;
+  if ((rc = w.alloc(sz.level_cap, 2 * h->g.H, false))) return rc;
+  CK(fid.alloc((size_t)K * h->Nmax));
   const auto t0 = std::chrono::steady_clock::now();
-  const std::vector<double> uniform(W, 1.0 / H);   // level 0: the game root with uniform beliefs
-  const int root = 0;
-  CK(cudaMemcpyAsync(roots[0].p, &root, sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(bel[0].p, uniform.data(), W * sizeof(double), cudaMemcpyHostToDevice, st));
   cfrb::ExplDev d = walk_dev(h);
-  d.fill = fill.p; d.cap = (int)sz.level_cap; d.fid = fid.p; d.nmax = h->Nmax;
-  cfrb::SpDev scan = walk_scan(h);
+  d.fid = fid.p; d.nmax = h->Nmax;
+  w.expand = [&](int n) {
+    with_state(h, [&](auto& s) { const auto a = avg_table(h, s); cfrb::expl_launch_expand(d, n, a.p, a.normalise, h->own_stream); });
+  };
   int64_t solved = 0;
-  int cur = 0, n_level = 1;
-  for (int depth = 0; n_level > 0; depth += h->cfg.max_depth) {
-    d.roots = roots[cur].p; d.bel = bel[cur].p; d.next_roots = roots[cur ^ 1].p; d.next_bel = bel[cur ^ 1].p;
-    CK(cudaMemsetAsync(fill.p, 0, sizeof(int), st));
-    for (int off = 0; off < n_level; off += K) {
-      const int n = std::min(K, n_level - off);
-      d.off = off; scan.K = n;
-      with_state(h, [&](auto& s) { cfrb::expl_launch_begin(d, scan, n, s.beliefs.p, st); });
-      h->launches += 2;
-      CK(cudaGetLastError());
-      if ((rc = solve_device_wave(h, n, true, false, st))) return rc;
-      with_state(h, [&](auto& s) {
-        const auto avg = avg_table(h, s);
-        cfrb::expl_launch_expand(d, n, avg.p, avg.normalise ? 1 : 0, st);
-      });
-      h->launches += 2;
-      CK(cudaGetLastError());
-    }
-    solved += n_level;
-    int next = 0;
-    CK(cudaMemcpyAsync(&next, fill.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (next != binom(g.A - 1, depth + h->cfg.max_depth))
-      return fail(CFRB_ECUDA, "cfrb_to_leaf_exploitability: level at depth " + std::to_string(depth + h->cfg.max_depth) + " has " +
-                                  std::to_string(next) + " subgames, the tree " + std::to_string(binom(g.A - 1, depth + h->cfg.max_depth)));
-    n_level = next;
-    cur ^= 1;
-  }
+  if ((rc = w.run(h, d, 1, solved))) return rc;
   return walk_finish(h, t0, solved, br_out2, subgames, subgame_iters, seconds2);
 }
 
@@ -2014,52 +2054,18 @@ int64_t cfrb_recursive_bytes(int32_t num_dice, int32_t num_faces, int32_t max_su
 int cfrb_recursive_exploitability(cfrb_handle* h, double* br_out2, int64_t* subgames, int64_t* subgame_iters, double* seconds2) {
   if (!h || !br_out2) return fail(CFRB_EINVAL, "cfrb_recursive_exploitability: null argument");
   const auto& g = h->g;
-  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H;
-  const int64_t lmax = binom(g.A - 1, (g.A - 1) / 2);
   int rc = walk_admit(h, "cfrb_recursive_exploitability", to_leaf_sizes(g, 1, 1).tree_bytes, recursive_walk_bytes(g));
   if (rc) return rc;
-  cudaStream_t st = h->own_stream;
-  DevBuf<int> roots[2], fill;
-  DevBuf<double> bel[2];
-  for (int i = 0; i < 2; ++i) { CK(roots[i].alloc(lmax)); CK(bel[i].alloc((size_t)lmax * W)); }
-  CK(fill.alloc(1));
+  LevelWalk w{"cfrb_recursive_exploitability", 1};
+  if ((rc = w.alloc(binom(g.A - 1, (g.A - 1) / 2), 2 * g.H, false))) return rc;
   const auto t0 = std::chrono::steady_clock::now();
-  const std::vector<double> uniform(W, 1.0 / H);   // level 0: the game root with uniform beliefs
-  const int root = 0;
-  CK(cudaMemcpyAsync(roots[0].p, &root, sizeof(int), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(bel[0].p, uniform.data(), W * sizeof(double), cudaMemcpyHostToDevice, st));
   cfrb::ExplDev d = walk_dev(h);
-  d.fill = fill.p; d.cap = (int)lmax;
-  cfrb::SpDev scan = walk_scan(h);
+  w.expand_launches = 1;
+  w.expand = [&](int n) {
+    with_state(h, [&](auto& s) { const auto a = avg_table(h, s); cfrb::rec_launch_expand(d, n, a.p, a.normalise, h->own_stream); });
+  };
   int64_t solved = 0;
-  int cur = 0, n_level = 1;
-  for (int depth = 0; n_level > 0; ++depth) {
-    d.roots = roots[cur].p; d.bel = bel[cur].p; d.next_roots = roots[cur ^ 1].p; d.next_bel = bel[cur ^ 1].p;
-    CK(cudaMemsetAsync(fill.p, 0, sizeof(int), st));
-    for (int off = 0; off < n_level; off += K) {
-      const int n = std::min(K, n_level - off);
-      d.off = off; scan.K = n;
-      with_state(h, [&](auto& s) { cfrb::expl_launch_begin(d, scan, n, s.beliefs.p, st); });
-      h->launches += 2;
-      CK(cudaGetLastError());
-      if ((rc = solve_device_wave(h, n, true, false, st))) return rc;
-      with_state(h, [&](auto& s) {
-        const auto avg = avg_table(h, s);
-        cfrb::rec_launch_expand(d, n, avg.p, avg.normalise ? 1 : 0, st);
-      });
-      ++h->launches;
-      CK(cudaGetLastError());
-    }
-    solved += n_level;
-    int next = 0;
-    CK(cudaMemcpyAsync(&next, fill.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (next != binom(g.A - 1, depth + 1))
-      return fail(CFRB_ECUDA, "cfrb_recursive_exploitability: level at depth " + std::to_string(depth + 1) + " has " +
-                                  std::to_string(next) + " subgames, the tree " + std::to_string(binom(g.A - 1, depth + 1)));
-    n_level = next;
-    cur ^= 1;
-  }
+  if ((rc = w.run(h, d, 1, solved))) return rc;
   return walk_finish(h, t0, solved, br_out2, subgames, subgame_iters, seconds2);
 }
 
@@ -2236,10 +2242,7 @@ static int to_leaf_sampled_impl(cfrb_handle* h, int32_t seed0, int32_t num_repea
                                 int64_t* subgames, int64_t* subgame_iters, double* seconds3) {
   if (!h || !checkpoints || !br_out || (ev_full && !ev_out)) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: null argument");
   const auto& g = h->g;
-  if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
-    return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) +
-                                 " actions are not supported (A = " + std::to_string(g.A) + ": the full tree has 2^A - 1 nodes)");
-  const int K = h->cfg.max_subgames, H = g.H, W = 2 * H, md = h->cfg.max_depth, iters = h->cfg.num_iters;
+  const int K = h->cfg.max_subgames, H = g.H, md = h->cfg.max_depth, iters = h->cfg.num_iters;
   if (num_repeats < 1) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: num_repeats must be >= 1");
   if (batch_repeats < 1 || batch_repeats > K)
     return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: batch_repeats must be in [1, max_subgames = " + std::to_string(K) + "]");
@@ -2249,42 +2252,22 @@ static int to_leaf_sampled_impl(cfrb_handle* h, int32_t seed0, int32_t num_repea
   if (cps.back() != num_repeats) cps.push_back(num_repeats);
   if (cap < (int)cps.size())
     return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: " + std::to_string(cps.size()) + " checkpoints, room for " + std::to_string(cap));
-  if (h->in_match) return fail(CFRB_EINVAL, "cfrb_to_leaf_sampled: the handle plays in a live match or agent");
-  if (h->cfg.net_mode != CFRB_NET_ZERO && !h->have_weights && h->Lmax > 0)
-    return fail(CFRB_ESTATE, "cfrb_to_leaf_sampled: value-net weights not set (cfrb_set_weights)");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->own_stream));
-  h->smp.ready = false;                        // the previous call's results go first: their memory counts as free below
-  h->smp.sum_s = DevBuf<float>();
-  h->smp.sum_r = DevBuf<float>();
-  h->smp.last_act.clear();
   const auto sz = sampled_sizes(g, md, K, batch_repeats);
-  // refused before anything is allocated: on a shared device an allocation that fails late may starve other processes
   const int64_t ev_bytes = ev_full ? ((((int64_t)1 << g.A) - 2) * H) * 8 : 0;   // the compact ev_full
   const int64_t rg_bytes = rg.on ? sampled_regret_bytes(g, batch_repeats) : 0;   // the regret sums and the batch's strategies
-  const int64_t need = (h->br.ready ? 0 : sz.tree_bytes) + sz.walk_bytes + ev_bytes + rg_bytes;
-  size_t free_b = 0, total_b = 0;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  int64_t avail = (int64_t)free_b;
-  if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
-  if (need > avail)
-    return fail(CFRB_ENOMEM, "cfrb_to_leaf_sampled: needs " + std::to_string(need) + " bytes of device memory beyond the handle "
-                             "(full tree and best-response scratch " + std::to_string(h->br.ready ? 0 : sz.tree_bytes) + ", walk " +
-                             std::to_string(sz.walk_bytes) + " at batch_repeats " + std::to_string(batch_repeats) +
-                             (rg.on ? ", regrets " + std::to_string(rg_bytes) : std::string()) + "), " + std::to_string(avail) + " free");
-  int rc = full_tree_setup(h, "cfrb_to_leaf_sampled");
+  int rc = walk_admit(h, "cfrb_to_leaf_sampled", sz.tree_bytes, sz.walk_bytes, ev_bytes + rg_bytes,
+                      " at batch_repeats " + std::to_string(batch_repeats) + (rg.on ? ", regrets " + std::to_string(rg_bytes) : ""),
+                      true);
   if (rc) return rc;
   const int N = h->br.t.N;
   const auto ord = to_leaf_order(g, md);
   const int R = (int)ord.rec_to_level.size();
   if (R != sz.roots) return fail(CFRB_ECUDA, "cfrb_to_leaf_sampled: " + std::to_string(R) + " subgame roots, expected " + std::to_string(sz.roots));
   cudaStream_t st = h->own_stream;
-  DevBuf<int> roots[2], fid, fill, draws;
-  DevBuf<double> bel[2], rch[2];
-  for (int i = 0; i < 2; ++i) {
-    CK(roots[i].alloc(sz.level_cap)); CK(bel[i].alloc((size_t)sz.level_cap * W)); CK(rch[i].alloc((size_t)sz.level_cap * W));
-  }
-  CK(fid.alloc((size_t)K * h->Nmax)); CK(fill.alloc(1)); CK(draws.alloc((size_t)batch_repeats * R));
+  LevelWalk w{"cfrb_to_leaf_sampled", md, true};   // the snapshot does not read the sum table
+  DevBuf<int> fid, draws;
+  if ((rc = w.alloc(sz.level_cap, 2 * H, true))) return rc;
+  CK(fid.alloc((size_t)K * h->Nmax)); CK(draws.alloc((size_t)batch_repeats * R));
   CK(h->smp.sum_s.alloc((size_t)(N - 1) * H)); CK(h->smp.sum_r.alloc((size_t)N * H));
   DevBuf<double> full;
   if (ev_full) {
@@ -2307,38 +2290,32 @@ static int to_leaf_sampled_impl(cfrb_handle* h, int32_t seed0, int32_t num_repea
   }
   CK(cudaMemsetAsync(h->smp.sum_s.p, 0, (size_t)(N - 1) * H * sizeof(float), st));
   CK(cudaMemsetAsync(h->smp.sum_r.p, 0, (size_t)N * H * sizeof(float), st));
-  cfrb::ExplSampledDev d{};
-  d.H = H; d.A = g.A;
-  d.full_child_begin = h->br.child_begin.p; d.full_depth = h->br.depth.p; d.full_act_lo = h->br.act_lo.p; d.full_parent = h->br.parent.p;
-  d.full_nodes = N;
-  d.tmpl = h->d_tmpl.p; d.parent = h->d_parent.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p;
-  d.level_begin = h->d_level_begin.p; d.pleaf_node = h->d_pleaf_node.p;
-  d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_act = h->d_sg_act.p; d.sg_row_off = h->d_sg_row_off.p;
-  d.wave = h->d_wave.p; d.table_stride = h->table_stride;
+  cfrb::ExplDev d = walk_dev(h);
+  d.A = g.A; d.full_parent = h->br.parent.p; d.full_nodes = N;
   d.draws = draws.p; d.draws_stride = R;
-  d.fill = fill.p; d.cap = sz.level_cap; d.fid = fid.p; d.nmax = h->Nmax;
-  d.sum_s = h->smp.sum_s.p; d.sum_r = h->smp.sum_r.p; d.last = h->br.strategy2.p; d.strategy = h->br.strategy.p;
+  d.fid = fid.p; d.nmax = h->Nmax;
+  d.sum_s = h->smp.sum_s.p; d.sum_r = h->smp.sum_r.p; d.last = h->br.strategy2.p;
   d.rep_s = rg.on ? rep.p : nullptr; d.rep_stride = E;
-  cfrb::SpDev scan{};   // sp_scan_kernel's view of the wave
-  scan.A = g.A; scan.tmpl = h->d_tmpl.p; scan.wave = h->d_wave.p; scan.sg_tmpl = h->d_sg_tmpl.p; scan.sg_row_off = h->d_sg_row_off.p;
-  scan.sg_order = h->d_sg_order.p; scan.tmpl_rank = h->d_tmpl_rank.p;
-  scan_wide(h, scan);
   // act_iteration ~ discrete distribution with weight i/2 + 1 on even i (recursive_solving.cc:304-309, 315-319); the distribution
   // keeps no state between draws, so one object serves every root
   std::vector<double> weights;
   for (int i = 0; i < iters; ++i) weights.push_back(i % 2 ? 0.0 : (i / 2. + 1));
   std::discrete_distribution<int> dist(weights.begin(), weights.end());
   std::vector<int> draws_h, gmax(R), level_roots;
-  const std::vector<double> uniform(W, 1.0 / H);   // level 0: the game root with uniform beliefs and reach
-  std::vector<double> uniform_b;
   double secs[3] = {0, 0, 0};
   int64_t solved = 0, iters_sum = 0;
-  int done = 0, c = 0;
+  int done = 0, c = 0, b = 0;
+  w.expand = [&](int n) { with_state(h, [&](auto& s) { cfrb::expl_sampled_launch_expand(d, n, s.Snap.p, st); }); };
+  w.iters = [&](int off, int n) {   // the wave runs up to its largest act_iteration (RecursiveEvaluator::runBatch)
+    int max_act = 0;
+    for (int gi = off / b; gi < (off + n) / b; ++gi) max_act = std::max(max_act, gmax[d.level_base + gi]);
+    return max_act;
+  };
   while (done < num_repeats) {
     // batches end at the checkpoints, as RecursiveEvaluator::run's do
     int next_cp = 1;
     while (next_cp <= done) next_cp <<= 1;
-    const int b = std::min({num_repeats, done + batch_repeats, next_cp}) - done;
+    b = std::min({num_repeats, done + batch_repeats, next_cp}) - done;
     const bool last_batch = done + b == num_repeats;
     const auto t0 = std::chrono::steady_clock::now();
     // repeat r draws from std::mt19937(seed0 + r) once per subgame root, in recursion order (RecursiveEvaluator::runBatch)
@@ -2356,53 +2333,18 @@ static int to_leaf_sampled_impl(cfrb_handle* h, int32_t seed0, int32_t num_repea
     }
     CK(cudaMemcpyAsync(draws.p, draws_h.data(), draws_h.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     const auto t1 = std::chrono::steady_clock::now();
-    const std::vector<int> zeros(b, 0);
-    uniform_b.resize((size_t)b * W);
-    for (int j = 0; j < b; ++j) std::copy(uniform.begin(), uniform.end(), uniform_b.begin() + (size_t)j * W);
-    CK(cudaMemcpyAsync(roots[0].p, zeros.data(), b * sizeof(int), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bel[0].p, uniform_b.data(), uniform_b.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(rch[0].p, uniform_b.data(), uniform_b.size() * sizeof(double), cudaMemcpyHostToDevice, st));
     d.b = b; d.last_j = last_batch ? b - 1 : -1;
-    const int Kw = (K / b) * b;                   // a wave holds whole root groups
-    int cur = 0, n_level = b;
-    for (int depth = 0, l = 0; n_level > 0; depth += md, ++l) {
-      d.roots = roots[cur].p; d.bel = bel[cur].p; d.rch = rch[cur].p;
-      d.next_roots = roots[cur ^ 1].p; d.next_bel = bel[cur ^ 1].p; d.next_rch = rch[cur ^ 1].p;
-      d.level_base = ord.level_begin[l];
-      CK(cudaMemsetAsync(fill.p, 0, sizeof(int), st));
-      for (int off = 0; off < n_level; off += Kw) {
-        const int n = std::min(Kw, n_level - off);
-        int max_act = 0;   // the wave runs up to its largest act_iteration (RecursiveEvaluator::runBatch)
-        for (int gi = off / b; gi < (off + n) / b; ++gi) max_act = std::max(max_act, gmax[d.level_base + gi]);
-        d.off = off; scan.K = n;
-        with_state(h, [&](auto& s) { cfrb::expl_sampled_launch_begin(d, scan, n, s.beliefs.p, st); });
-        h->launches += 2;
-        CK(cudaGetLastError());
-        if ((rc = solve_device_wave(h, n, true, true, st, max_act))) return rc;   // the snapshot does not read the sum table
-        with_state(h, [&](auto& s) { cfrb::expl_sampled_launch_expand(d, n, s.Snap.p, st); });
-        h->launches += 2;
-        CK(cudaGetLastError());
-      }
-      solved += n_level;
-      if (last_batch) {   // the roots of this level, for the last repeat's act_iterations by node
-        level_roots.resize(n_level);
-        CK(cudaMemcpyAsync(level_roots.data(), roots[cur].p, n_level * sizeof(int), cudaMemcpyDeviceToHost, st));
-      }
-      int next = 0;
-      CK(cudaMemcpyAsync(&next, fill.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    w.level_done = nullptr;
+    if (last_batch) w.level_done = [&](const int* roots, int n_level) -> int {   // the last repeat's act_iterations by node
+      level_roots.resize(n_level);
+      CK(cudaMemcpyAsync(level_roots.data(), roots, n_level * sizeof(int), cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
-      if (last_batch) {
-        if (h->smp.last_act.empty()) h->smp.last_act.assign(N, -1);
-        for (int gi = 0; gi < n_level / b; ++gi)
-          h->smp.last_act[level_roots[(size_t)gi * b]] = draws_h[(size_t)(b - 1) * R + d.level_base + gi];
-      }
-      const int64_t want = binom(g.A - 1, depth + md) * b;
-      if (next != want)
-        return fail(CFRB_ECUDA, "cfrb_to_leaf_sampled: level at depth " + std::to_string(depth + md) + " has " +
-                                    std::to_string(next) + " subgames, the tree " + std::to_string(want));
-      n_level = next;
-      cur ^= 1;
-    }
+      if (h->smp.last_act.empty()) h->smp.last_act.assign(N, -1);
+      for (int gi = 0; gi < n_level / b; ++gi)
+        h->smp.last_act[level_roots[(size_t)gi * b]] = draws_h[(size_t)(b - 1) * R + d.level_base + gi];
+      return CFRB_OK;
+    };
+    if ((rc = w.run(h, d, b, solved))) return rc;
     if (rg.on) {   // the batch's sampled strategies into the regret sums in repeat order (RecursiveEvaluator::run)
       const auto& t = h->br.t;
       for (int j = 0; j < b; ++j) {

@@ -1,9 +1,10 @@
 // Recursive to-leaf walk on the device (cfrb_to_leaf_exploitability): compute_strategy_recursive_to_leaf with the average strategy
 // (recursive_solving.cc:76-134, as RecursiveEvaluator::strategyToLeaf runs it on the host) for games whose full tree is too large
 // for a dense [N][H][A] strategy.  Level l holds the subgames rooted at the non-terminal full-tree nodes of depth l * max_depth, in
-// full-tree node order; each wave of a level is solved by the handle's CFR / FP solver, then
+// full-tree node order; each wave of a level is solved by the handle's CFR / FP solver (LevelWalk in cfrb_api.cu), then
 //
-//   expl_begin    per subgame: template, player and (real) root beliefs of the wave, from the level's roots and fp64 beliefs
+//   expl_begin    per subgame: template, player, act_iteration (the sampled walk's draw, else -1) and (real) root beliefs of the
+//                 wave, from the level's roots and fp64 beliefs.  The every-node and sampled walks begin their waves with it too
 //   sp_scan       packed value-net row offsets, wave size, largest-first schedule (selfplay_kernels.cuh)
 //   expl_expand   per subgame: the average strategy of its inner nodes (get_strategy; CFR's sum normalised as cfrb_fetch_compact
 //                 kind 4 does it) written straight into the compact full-tree strategy, and the beliefs of its non-terminal
@@ -26,12 +27,30 @@ template <typename real>
 __global__ void __launch_bounds__(128) expl_begin_kernel(ExplDev p, int n, real* __restrict__ wave_beliefs) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
-  const int node = p.roots[p.off + k];
+  const int pos = p.off + k;
+  const int node = p.roots[pos];
   p.sg_tmpl[k] = p.full_act_lo[node];          // = last_bid + 1 (0 at the game root)
   p.sg_player[k] = p.full_depth[node] & 1;     // the game root is player 0's node
-  p.sg_act[k] = -1;
-  const double* b = p.bel + (size_t)(p.off + k) * 2 * p.H;
+  p.sg_act[k] = p.draws ? p.draws[(long long)(pos % p.b) * p.draws_stride + p.level_base + pos / p.b] : -1;
+  const double* b = p.bel + (size_t)pos * 2 * p.H;
   for (int i = 0; i < 2 * p.H; ++i) wave_beliefs[(size_t)k * 2 * p.H + i] = (real)b[i];
+}
+
+// The full-tree node of every template node of the subgame at level position pos, by the whole CTA: child j of n is child j of n's
+// full-tree node (same bid range, same order).
+__device__ __forceinline__ void template_fid(const ExplDev& p, const TemplateDev& t, int pos, int* fid) {
+  const int* __restrict__ parent = p.parent + t.node_off;
+  const int* __restrict__ child_begin = p.child_begin + t.node_off;
+  const int* __restrict__ level_begin = p.level_begin + t.level_off;
+  if (threadIdx.x == 0) fid[0] = p.roots[pos];
+  __syncthreads();
+  for (int d = 1; d < t.levels; ++d) {
+    for (int c = level_begin[d] + threadIdx.x; c < level_begin[d + 1]; c += blockDim.x) {
+      const int q = parent[c];
+      fid[c] = p.full_child_begin[fid[q]] + (c - child_begin[q]);
+    }
+    __syncthreads();
+  }
 }
 
 // One CTA per subgame of the wave.  table: the solver's average-strategy table (CFR: the sum S, normalised here; FP: Sg).
@@ -42,18 +61,8 @@ __global__ void __launch_bounds__(128) expl_expand_kernel(ExplDev p, const real*
   const int* __restrict__ parent = p.parent + t.node_off;
   const int* __restrict__ child_begin = p.child_begin + t.node_off;
   const int* __restrict__ nchild = p.nchild + t.node_off;
-  const int* __restrict__ level_begin = p.level_begin + t.level_off;
   int* fid = p.fid + (size_t)k * p.nmax;
-  // full-tree node of every template node: child j of n is child j of n's full-tree node (same bid range, same order)
-  if (tid == 0) fid[0] = p.roots[p.off + k];
-  __syncthreads();
-  for (int d = 1; d < t.levels; ++d) {
-    for (int c = level_begin[d] + tid; c < level_begin[d + 1]; c += nt) {
-      const int q = parent[c];
-      fid[c] = p.full_child_begin[fid[q]] + (c - child_begin[q]);
-    }
-    __syncthreads();
-  }
+  template_fid(p, t, p.off + k, fid);
   // the average strategy of the inner nodes (normalise_avg in cfrb_api.cu: uniform until the acting player's first update)
   const real* tk = table + (size_t)k * p.table_stride;
   for (int it = tid; it < t.N * H; it += nt) {
@@ -156,6 +165,111 @@ __global__ void __launch_bounds__(128) rec_expand_kernel(ExplDev p, int n, const
     for (int h = 0; h < H; ++h) a[h] = (a[h] + 1e-80) / sum;
   }
   if (lane == 0) atomicAdd(p.fill, kids);
+}
+
+// Sampled recursive to-leaf walk on the device (cfrb_to_leaf_sampled): recursive_eval's --num_repeats evaluation
+// (recursive_eval.cc:331-369: compute_sampled_strategy_recursive_to_leaf, recursive_solving.cc:301-327 with :76-134, and the
+// float32 reach-weighted sums of :138-148, 349-355, as RecursiveEvaluator::run does it on the host) for games whose full tree is
+// too large for dense [N][H][A] sums.  A batch of b repeats is walked level by level like the average policy; a level holds, for
+// each subgame root in full-tree node order, its b repeats next to each other in repeat order.  Each wave (whole root groups) is
+// begun by expl_begin, whose act_iteration is the repeat's mt19937 draw for that root, solved by the handle's CFR / FP solver up to
+// the largest act_iteration of the wave, and ended by expl_fill after
+//
+//   expl_sampled_expand   one CTA per root group, its repeats in order: summed_reach[node] += float(reach[player(node)]) at every
+//                         node of the subgame but its non-terminal pseudo-leaves, summed_strategy[edge] += float(s) * float(reach)
+//                         at every inner edge, s the repeat's snapshot strategy (the sampling strategy at act_iteration); then the
+//                         fp64 beliefs (unnormalised down the subgame, eps-normalised at the leaf) and reach (never normalised) of
+//                         its non-terminal pseudo-leaves, appended to the next level at fill + group row offset + leaf * b + repeat
+//
+// Every (node, hand) entry of the accumulators gets one contribution per repeat, and a root's repeats are added by one CTA in
+// repeat order, batches in order: the float32 sums are the host's bit for bit.  Every fp64 operation is the host walk's, in its
+// order.  At a checkpoint expl_sampled_finalize divides the sums in float32 (recursive_eval.cc:362-363) and widens the result into
+// the compact strategy the best response (br_kernel) reads.
+
+// v and w times the snapshot strategy of every edge on the path from the root to template node nn whose parent player pl acts
+// on, from the root down (the host's copy-then-multiply per child, recursive_eval.h expand)
+template <typename real>
+__device__ __forceinline__ void sampled_path(const ExplDev& p, const int* __restrict__ parent, const int* __restrict__ fid,
+                                             const real* __restrict__ tk, int nn, int h, int pl, double& v, double& w) {
+  int dep = 0;
+  for (int c = nn; parent[c] >= 0; c = parent[c]) ++dep;
+  for (int d = 1; d <= dep; ++d) {
+    int c = nn;                                // nn's ancestor at depth d, and its parent
+    for (int up = dep; up > d; --up) c = parent[c];
+    const int q = parent[c];
+    if ((p.full_depth[fid[q]] & 1) == pl) {
+      const double s = (double)tk[(size_t)(c - 1) * p.H + h];
+      v *= s;
+      w *= s;
+    }
+  }
+}
+
+// One CTA per root group of the wave: subgames g * b .. g * b + b - 1, the b repeats of one root.  snap: the solver's snapshot
+// table (the sampling strategy at each subgame's act_iteration).
+template <typename real>
+__global__ void __launch_bounds__(128) expl_sampled_expand_kernel(ExplDev p, const real* __restrict__ snap) {
+  const int g = blockIdx.x, tid = threadIdx.x, nt = blockDim.x, H = p.H, k0 = g * p.b;
+  const TemplateDev t = p.tmpl[p.sg_tmpl[k0]];
+  const int* __restrict__ parent = p.parent + t.node_off;
+  const int* __restrict__ child_begin = p.child_begin + t.node_off;
+  const int* __restrict__ nchild = p.nchild + t.node_off;
+  int* fid = p.fid + (size_t)g * p.nmax;
+  template_fid(p, t, p.off + k0, fid);
+  const int base = *p.fill + p.sg_row_off[k0];
+  for (int j = 0; j < p.b; ++j) {
+    const int k = k0 + j;
+    const real* tk = snap + (size_t)k * p.table_stride;
+    const double* rb = p.bel + (size_t)(p.off + k) * 2 * H;
+    const double* rr = p.rch + (size_t)(p.off + k) * 2 * H;
+    // the weights of the infosets (node, hand) (recursive_eval.cc:143-148) and the weighted sampled strategy (:349-355)
+    for (int it = tid; it < t.N * H; it += nt) {
+      const int nn = it / H, hd = it % H;
+      const int f = fid[nn], nc = nchild[nn];
+      if (nc == 0 && p.full_act_lo[f] < p.A) continue;   // non-terminal pseudo-leaf: the next level's subgame root
+      const int pid = p.full_depth[f] & 1;
+      double r = rr[pid * H + hd], unused = 0;
+      sampled_path(p, parent, fid, tk, nn, hd, pid, r, unused);
+      p.sum_r[(size_t)f * H + hd] += (float)r;
+      const int cb = child_begin[nn], fcb = p.full_child_begin[f];
+      for (int jj = 0; jj < nc; ++jj) {
+        const double s = (double)tk[(size_t)(cb + jj - 1) * H + hd];
+        const size_t e = (size_t)(fcb + jj - 1) * H + hd;
+        p.sum_s[e] += (float)s * (float)r;
+        if (j == p.last_j) p.last[e] = s;
+        if (p.rep_s) p.rep_s[(size_t)j * p.rep_stride + e] = (float)s;   // the repeat's strategy as recursive_eval's float32 tensor
+      }
+    }
+    // beliefs and reach of the pseudo-leaves, one thread per (leaf, player row)
+    for (int it = tid; it < 2 * t.L; it += nt) {
+      const int r = it >> 1, pl = it & 1;
+      const int leaf = p.pleaf_node[t.pleaf_off + r];
+      const long long slot = (long long)base + (long long)r * p.b + j;
+      if (slot >= p.cap) continue;             // cannot happen for a level sized by the host; the host checks the count
+      if (pl == 0) p.next_roots[slot] = fid[leaf];
+      double* ob = p.next_bel + (size_t)slot * 2 * H + (size_t)pl * H;
+      double* orch = p.next_rch + (size_t)slot * 2 * H + (size_t)pl * H;
+      for (int h = 0; h < H; ++h) {
+        double vb = rb[pl * H + h], vr = rr[pl * H + h];
+        sampled_path(p, parent, fid, tk, leaf, h, pl, vb, vr);
+        ob[h] = vb;
+        orch[h] = vr;
+      }
+      double sum = 0;
+      for (int h = 0; h < H; ++h) sum += ob[h] + 1e-80;
+      for (int h = 0; h < H; ++h) ob[h] = (ob[h] + 1e-80) / sum;
+    }
+    __syncthreads();                           // repeat j + 1 adds to the entries repeat j has just added to
+  }
+}
+
+__global__ void expl_sampled_finalize_kernel(ExplDev p) {
+  const size_t total = (size_t)(p.full_nodes - 1) * p.H;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i / p.H) + 1, hd = (int)(i % p.H);
+    const float den = p.sum_r[(size_t)p.full_parent[c] * p.H + hd] + 1e-6f;
+    p.strategy[i] = (double)(p.sum_s[i] / den);
+  }
 }
 
 }  // namespace cfrb
