@@ -13,9 +13,8 @@
 //   agent_scan      one CTA: wave index of every listed table that stands at an unsolved root and the packed value-net row offsets
 //   agent_begin     per listed table that needs a solve: subgame descriptor (template, player, fp64 -> real beliefs) and, in
 //                   sampled mode, act_iteration ~ weight i/2 + 1 on even i < num_iters drawn from the table's stream
-//   agent_capture   warp per solved table: the acting strategy into the cache, entry (child - 1) * H + hand; average mode =
-//                   normalise(S) with the operation order and uniform-until-first-update rule of match_advance's sig (CFR) or Sg
-//                   itself (FP); sampled mode = the act_iteration snapshot
+//   agent_capture   warp per solved table: the acting strategy into the cache (capture_levels), entry (child - 1) * H + hand;
+//                   average mode = avg_row of S (CFR) or Sg (FP); sampled mode = the act_iteration snapshot
 //   agent_step      per listed table: one action (given, or drawn for the agent's hand), the mover's belief row times the
 //                   strategy of that action, the next node; at a pseudo-leaf both rows eps-normalised and the table unsolved
 //   agent_policy    per (listed table, hand): the strategy of the player to move at the table's node
@@ -51,7 +50,7 @@ __global__ void __launch_bounds__(128) agent_new_kernel(AgentDev p) {
 
 // Wave index of every listed table at an unsolved root (list order) and the exclusive prefix sum of their pseudo-leaf counts.
 __global__ void __launch_bounds__(1024) agent_scan_kernel(AgentDev p) {
-  __shared__ int part_n[1024], part_r[1024];
+  __shared__ int part[2 * 1024];
   const int t = threadIdx.x, per = (p.n + 1023) / 1024;
   const int b = t * per, e = min(p.n, b + per);
   int n = 0, r = 0;
@@ -59,15 +58,9 @@ __global__ void __launch_bounds__(1024) agent_scan_kernel(AgentDev p) {
     const int id = p.ids[i];
     if (p.status[id] == 1) { ++n; r += p.tmpl[p.last_bid[id] + 1].L; }
   }
-  part_n[t] = n; part_r[t] = r;
-  __syncthreads();
-  for (int d = 1; d < 1024; d <<= 1) {
-    const int vn = t >= d ? part_n[t - d] : 0, vr = t >= d ? part_r[t - d] : 0;
-    __syncthreads();
-    part_n[t] += vn; part_r[t] += vr;
-    __syncthreads();
-  }
-  int w = part_n[t] - n, off = part_r[t] - r;
+  int x[2] = {n, r};                                 // tables to solve, rows
+  sp_block_scan(part, x);
+  int w = x[0] - n, off = x[1] - r;
   for (int i = b; i < e; ++i) {
     const int id = p.ids[i];
     if (p.status[id] != 1) { p.widx[i] = -1; continue; }
@@ -76,7 +69,7 @@ __global__ void __launch_bounds__(1024) agent_scan_kernel(AgentDev p) {
     ++w;
     off += p.tmpl[p.last_bid[id] + 1].L;
   }
-  if (t == 1023) { p.wave[0] = part_n[1023]; p.wave[1] = part_r[1023]; }
+  if (t == 1023) { p.wave[0] = x[0]; p.wave[1] = x[1]; }
 }
 
 template <typename real>
@@ -89,7 +82,7 @@ __global__ void __launch_bounds__(128) agent_begin_kernel(AgentDev p, MatchTabs<
   int act = -1;
   if (p.sampled) {
     SpRng rng{p.mt + t, p.T, p.mt_idx[t]};
-    act = sp_discrete(rng, p.iters, [](int k) { return k % 2 ? 0.0 : (k / 2. + 1); });
+    act = sp_act_iteration(rng, p.iters);
     p.mt_idx[t] = rng.idx;
   }
   p.sg_tmpl[w] = p.last_bid[t] + 1;
@@ -102,42 +95,18 @@ __global__ void __launch_bounds__(128) agent_begin_kernel(AgentDev p, MatchTabs<
   for (int k = 0; k < 2 * H; ++k) tb.wave_beliefs[0][(size_t)w * 2 * H + k] = (real)b[k];
 }
 
-// One warp per listed table; the lanes stride over the (node, hand) pairs of one level, hands innermost (coalesced reads).
+// One warp per listed table.
 template <typename real>
 __global__ void __launch_bounds__(128) agent_capture_kernel(AgentDev p, MatchTabs<real> tb) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (i >= p.n) return;
   const int w = p.widx[i];
   if (w < 0) return;
-  const int t = p.ids[i], H = p.H;
+  const int t = p.ids[i];
   const TemplateDev tp = p.tmpl[p.root_lb[t] + 1];
-  const int* __restrict__ child_begin = p.child_begin + tp.node_off;
-  const int* __restrict__ nchild = p.nchild + tp.node_off;
-  const int* __restrict__ level = p.level_begin + tp.level_off;
-  const real* __restrict__ T = tb.table[0] + (size_t)w * p.table_stride;
-  double* __restrict__ c = p.cache + (size_t)t * p.stride;
-  const bool normalise = tb.normalise[0];
-  const int root_player = p.root_player[t];
-  const int levels = p.every_node ? 1 : tp.levels;   // every-node: the root row only
-  for (int d = 0; d < levels; ++d) {
-    const int nb = level[d], ne = level[d + 1];
-    const bool untouched = normalise && p.steps[2 * w + (root_player ^ (d & 1))] == 0;
-    for (int e = nb * H + lane; e < ne * H; e += 32) {
-      const int node = e / H, hand = e - node * H;
-      const int cb = child_begin[node], nc = nchild[node];
-      if (nc == 0) continue;
-      const real* __restrict__ Te = T + (size_t)(cb - 1) * H + hand;
-      double* __restrict__ ce = c + (size_t)(cb - 1) * H + hand;
-      if (!normalise) {
-        for (int j = 0; j < nc; ++j) ce[j * H] = (double)Te[j * H];
-        continue;
-      }
-      double sum = 0;
-      for (int j = 0; j < nc; ++j) sum += (double)Te[j * H];
-      const bool uniform = untouched || !(sum > 0);
-      for (int j = 0; j < nc; ++j) ce[j * H] = uniform ? 1.0 / nc : (double)Te[j * H] / sum;
-    }
-  }
+  capture_levels(lane, tp, p.child_begin, p.nchild, p.level_begin, p.H, tb.table[0] + (size_t)w * p.table_stride,
+                 tb.normalise[0] != 0, p.steps + 2 * w, p.root_player[t], p.every_node ? 1 : tp.levels,   // every-node: the root row only
+                 p.cache + (size_t)t * p.stride);
   if (lane == 0) p.status[t] = 2;
 }
 

@@ -158,7 +158,7 @@ template <typename real>
 void sp_launch_share(const SpDev& p, const CfrDev<real>& d, cudaStream_t st) {
   sp_share_kernel<real><<<p.K, 128, 0, st>>>(p, d);
 }
-void match_launch_deal(const MatchDev& p, cudaStream_t st) { match_deal_kernel<<<(p.S + 127) / 128, 128, 0, st>>>(p); }
+void match_launch_deal(const MatchDev& p, cudaStream_t st) { match_deal_kernel<match_start><<<(p.S + 127) / 128, 128, 0, st>>>(p); }
 template <typename real>
 void match_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
   match_scan_kernel<<<1, 1024, 0, st>>>(p);
@@ -168,7 +168,7 @@ template <typename real>
 void match_launch_advance(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
   match_advance_kernel<real><<<(p.S + 127) / 128, 128, 0, st>>>(p, t);
 }
-void ply_launch_deal(const MatchDev& p, cudaStream_t st) { ply_deal_kernel<<<(p.S + 127) / 128, 128, 0, st>>>(p); }
+void ply_launch_deal(const MatchDev& p, cudaStream_t st) { match_deal_kernel<ply_start><<<(p.S + 127) / 128, 128, 0, st>>>(p); }
 template <typename real>
 void ply_launch_begin(const MatchDev& p, const MatchTabs<real>& t, cudaStream_t st) {
   ply_scan_kernel<<<1, 1024, 0, st>>>(p);

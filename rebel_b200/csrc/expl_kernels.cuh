@@ -63,25 +63,15 @@ __global__ void __launch_bounds__(128) expl_expand_kernel(ExplDev p, const real*
   const int* __restrict__ nchild = p.nchild + t.node_off;
   int* fid = p.fid + (size_t)k * p.nmax;
   template_fid(p, t, p.off + k, fid);
-  // the average strategy of the inner nodes (normalise_avg in cfrb_api.cu: uniform until the acting player's first update)
+  // the average strategy of the inner nodes (avg_row)
   const real* tk = table + (size_t)k * p.table_stride;
   for (int it = tid; it < t.N * H; it += nt) {
     const int nn = it / H, hd = it % H;
     const int nc = nchild[nn];
     if (!nc) continue;
     const int cb = child_begin[nn], f = fid[nn];
-    double* out = p.strategy + (size_t)(p.full_child_begin[f] - 1) * H + hd;
-    if (normalise) {
-      const bool untouched = p.steps[2 * k + (p.full_depth[f] & 1)] == 0;
-      double sum = 0;
-      for (int j = 0; j < nc; ++j) sum += (double)tk[(size_t)(cb + j - 1) * H + hd];
-      for (int j = 0; j < nc; ++j) {
-        const double v = (double)tk[(size_t)(cb + j - 1) * H + hd];
-        out[(size_t)j * H] = (sum > 0 && !untouched) ? v / sum : 1.0 / nc;
-      }
-    } else {
-      for (int j = 0; j < nc; ++j) out[(size_t)j * H] = (double)tk[(size_t)(cb + j - 1) * H + hd];
-    }
+    avg_row(p.strategy + (size_t)(p.full_child_begin[f] - 1) * H + hd, tk, cb - 1, hd, H, nc, normalise != 0,
+            normalise && p.steps[2 * k + (p.full_depth[f] & 1)] == 0);
   }
   __syncthreads();
   // beliefs of the pseudo-leaves, one thread per (leaf, player row): the root row times the strategy of every edge on the path
@@ -105,9 +95,7 @@ __global__ void __launch_bounds__(128) expl_expand_kernel(ExplDev p, const real*
       const double* s = p.strategy + (size_t)(fid[c] - 1) * H;
       for (int h = 0; h < H; ++h) ob[h] *= s[h];
     }
-    double sum = 0;
-    for (int h = 0; h < H; ++h) sum += ob[h] + 1e-80;
-    for (int h = 0; h < H; ++h) ob[h] = (ob[h] + 1e-80) / sum;
+    sp_normalize(ob, H);
   }
 }
 
@@ -117,8 +105,7 @@ __global__ void expl_fill_kernel(ExplDev p) { *p.fill += p.wave[1]; }
 // RecursiveEvaluator::strategyRecursive runs it on the host).  Level d holds the non-terminal full-tree nodes of depth d, in full-tree
 // order; each roots a depth-max_depth subgame, solved by expl_begin / sp_scan / the handle's solver like a to-leaf wave, of whose
 // average strategy only the root row is kept.  One warp per subgame of the wave:
-//   - the root row (CFR: the sum normalised as expl_expand_kernel does it; FP: Sg as it is) goes to the root's edges of the compact
-//     full-tree strategy;
+//   - the root row (avg_row: CFR's sum normalised, FP's Sg as it is) goes to the root's edges of the compact full-tree strategy;
 //   - every non-terminal child goes to the next level with the root's beliefs, the acting player's row multiplied by the child's
 //     strategy and eps-normalised (normalize_beliefs_inplace), the other row unchanged.  Only the acting row is renormalised, unlike
 //     the to-leaf walk's pseudo-leaves.
@@ -134,19 +121,7 @@ __global__ void __launch_bounds__(128) rec_expand_kernel(ExplDev p, int n, const
   const int nc = p.full_nchild[node], cb = p.full_child_begin[node], pl = p.full_depth[node] & 1;
   const real* tk = table + (size_t)k * p.table_stride;   // the template root's edges are its first nc rows
   double* s = p.strategy + (size_t)(cb - 1) * H;
-  for (int h = lane; h < H; h += 32) {
-    if (normalise) {
-      const bool untouched = p.steps[2 * k + pl] == 0;
-      double sum = 0;
-      for (int j = 0; j < nc; ++j) sum += (double)tk[(size_t)j * H + h];
-      for (int j = 0; j < nc; ++j) {
-        const double v = (double)tk[(size_t)j * H + h];
-        s[(size_t)j * H + h] = (sum > 0 && !untouched) ? v / sum : 1.0 / nc;
-      }
-    } else {
-      for (int j = 0; j < nc; ++j) s[(size_t)j * H + h] = (double)tk[(size_t)j * H + h];
-    }
-  }
+  for (int h = lane; h < H; h += 32) avg_row(s + h, tk, 0, h, H, nc, normalise != 0, normalise && p.steps[2 * k + pl] == 0);
   __syncwarp();
   const int kids = node == 0 ? nc : nc - 1;
   const int first = p.full_level_begin[p.full_depth[node] + 1] + i;
@@ -160,9 +135,7 @@ __global__ void __launch_bounds__(128) rec_expand_kernel(ExplDev p, int n, const
     double* a = ob + (size_t)pl * H;
     const double* sj = s + (size_t)j * H;
     for (int h = 0; h < H; ++h) a[h] *= sj[h];
-    double sum = 0;
-    for (int h = 0; h < H; ++h) sum += a[h] + 1e-80;
-    for (int h = 0; h < H; ++h) a[h] = (a[h] + 1e-80) / sum;
+    sp_normalize(a, H);
   }
   if (lane == 0) atomicAdd(p.fill, kids);
 }
@@ -255,9 +228,7 @@ __global__ void __launch_bounds__(128) expl_sampled_expand_kernel(ExplDev p, con
         ob[h] = vb;
         orch[h] = vr;
       }
-      double sum = 0;
-      for (int h = 0; h < H; ++h) sum += ob[h] + 1e-80;
-      for (int h = 0; h < H; ++h) ob[h] = (ob[h] + 1e-80) / sum;
+      sp_normalize(ob, H);
     }
     __syncthreads();                           // repeat j + 1 adds to the entries repeat j has just added to
   }

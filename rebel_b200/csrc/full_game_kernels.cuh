@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include "cfr_types.h"
+#include "selfplay_kernels.cuh"
 
 namespace cfrb {
 
@@ -194,8 +195,8 @@ __global__ void fg_down_kernel(FullGameDev p, int nb, int ne, int d) {
 
 __global__ void fg_advance_kernel(int* iter) { ++*iter; }
 
-// The average strategy (ISubgameSolver::get_strategy) into avg: CFR's normalised sum, as cfrb_fetch normalises it (sum in action
-// order, uniform where the sum is 0 or the acting player has not been updated yet).  FP's is Sg itself (copied by the host).
+// The average strategy (ISubgameSolver::get_strategy) into avg: CFR's normalised sum (avg_row).  FP's is Sg itself (copied by the
+// host).
 __global__ void fg_average_kernel(FullGameDev p, const int* depth, int untouched0, int untouched1) {
   const int H = p.H;
   const long long items = (long long)p.N * H;
@@ -205,12 +206,7 @@ __global__ void fg_average_kernel(FullGameDev p, const int* depth, int untouched
     if (!nc) continue;
     const bool untouched = (depth[n] & 1) ? untouched1 : untouched0;
     const size_t e0 = (size_t)(p.child_begin[n] - 1) * H + h;
-    double sum = 0;
-    for (int j = 0; j < nc; ++j) sum += p.S[e0 + (size_t)j * H];
-    for (int j = 0; j < nc; ++j) {
-      const size_t e = e0 + (size_t)j * H;
-      p.avg[e] = (sum > 0 && !untouched) ? p.S[e] / sum : 1.0 / nc;
-    }
+    avg_row(p.avg + e0, p.S + e0, 0, 0, H, nc, true, untouched);
   }
 }
 

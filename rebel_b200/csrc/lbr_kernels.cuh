@@ -21,7 +21,7 @@
 //
 // Against an EVERY_NODE agent (cfrb_match_create_lbr2) the agent plays as in a per-ply match (ply_kernels.cuh): it solves the
 // subgame rooted at every node of the path, whoever moves, and acts and updates the mover's belief row with that root's row
-// (en_root_sig, en_update_row).  The LBR rule is the same; sigma(child(a)) is always the root row of a what-if solve at child(a):
+// (avg_prob, en_update_row).  The LBR rule is the same; sigma(child(a)) is always the root row of a what-if solve at child(a):
 //   phase 1       LBR to move at X with m > 0 legal raises: one subgame rooted at X from the agent's beliefs; its root row for
 //                 LBR's seat goes to sigx (what the agent would multiply LBR's row by after each raise)
 //   phase 2       m what-if subgames rooted at the children: the agent's own row as it is, LBR's row times sigx[a], eps-normalised
@@ -44,19 +44,6 @@
 
 namespace cfrb {
 
-// The agent's strategy at (node, hand, child j) of the subgame in wave slot w, read as match_advance's sig() reads it.
-template <typename real>
-__device__ __forceinline__ double lbr_sig(const LbrDev& p, const MatchTabs<real>& tb, int w, int cb, int nc, int actor, int hand, int j) {
-  const int H = p.m.H;
-  const real* T = tb.table[0] + (size_t)w * p.m.table_stride;
-  const double v = (double)T[(size_t)(cb + j - 1) * H + hand];
-  if (!tb.normalise[0]) return v;
-  if (p.m.steps[0][2 * w + actor] == 0) return 1.0 / nc;
-  double sum = 0;
-  for (int i = 0; i < nc; ++i) sum += (double)T[(size_t)(cb + i - 1) * H + hand];
-  return sum > 0 ? v / sum : 1.0 / nc;
-}
-
 // Subgames (n) and value-net rows (r) slot s asks for in this round.
 __device__ __forceinline__ void lbr_need(const LbrDev& p, int s, int& n, int& r) {
   n = 0; r = 0;
@@ -67,7 +54,7 @@ __device__ __forceinline__ void lbr_need(const LbrDev& p, int s, int& n, int& r)
 }
 
 __global__ void __launch_bounds__(1024) lbr_scan_kernel(LbrDev p) {
-  __shared__ int part_n[1024], part_r[1024];
+  __shared__ int part[2 * 1024];
   __shared__ int end_n, end_r, last_pos, deferred;
   const MatchDev& q = p.m;
   const int S = q.S, t = threadIdx.x, per = (S + 1023) / 1024, start = *p.rr;
@@ -79,16 +66,10 @@ __global__ void __launch_bounds__(1024) lbr_scan_kernel(LbrDev p) {
     lbr_need(p, (start + i) % S, ni, ri);
     n += ni; r += ri;
   }
-  part_n[t] = n; part_r[t] = r;
-  __syncthreads();
-  for (int d = 1; d < 1024; d <<= 1) {
-    const int vn = t >= d ? part_n[t - d] : 0, vr = t >= d ? part_r[t - d] : 0;
-    __syncthreads();
-    part_n[t] += vn; part_r[t] += vr;
-    __syncthreads();
-  }
+  int x[2] = {n, r};                                 // subgames, rows
+  sp_block_scan(part, x);
   // the needs are >= 0, so the admitted slots (exclusive prefix + need <= K) are a prefix of the rotated order
-  int w = part_n[t] - n, off = part_r[t] - r, dn = 0;
+  int w = x[0] - n, off = x[1] - r, dn = 0;
   for (int i = b; i < e; ++i) {
     const int s = (start + i) % S;
     int ni, ri;
@@ -203,19 +184,15 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
       int wc, cb, nc;
       child(a, wc, cb, nc);
       const real* T = tb.table[0] + (size_t)wc * q.table_stride;
-      const bool uniform = tb.normalise[0] && q.steps[0][2 * wc + me] == 0;   // the agent acts at child(a)
+      const bool norm = tb.normalise[0] != 0, untouched = norm && q.steps[0][2 * wc + me] == 0;   // the agent acts at child(a)
       double v = 0;
       for (int h = 0; h < H; ++h) {
         double sum = 0;
-        if (tb.normalise[0] && !uniform)
-          for (int i = 0; i < nc; ++i) sum += (double)T[(size_t)(cb + i - 1) * H + h];
+        if (norm && !untouched) sum = avg_row_sum(T, cb - 1, h, H, nc);   // once per hand, not per child
         const double ua = is_true(a, h) ? 1.0 : -1.0;
         double inner = 0;
         for (int i = 0; i < nc; ++i) {               // bids a + 1 .. A - 1, the liar call last
-          double sg;
-          if (!tb.normalise[0]) sg = (double)T[(size_t)(cb + i - 1) * H + h];
-          else if (uniform) sg = 1.0 / nc;
-          else sg = sum > 0 ? (double)T[(size_t)(cb + i - 1) * H + h] / sum : 1.0 / nc;
+          const double sg = avg_entry((double)T[(size_t)(cb - 1 + i) * H + h], sum, nc, norm, untouched);
           const int a2 = a + 1 + i;
           const double u = a2 == A - 1 ? ua : (is_true(a2, h) ? -1.0 : 1.0);
           inner += sg * u;
@@ -265,7 +242,7 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
     const int lo = lb < 0 ? 0 : lb + 1, nc = q.nchild[q.tmpl[lb + 1].node_off];
     const real* T = tb.table[0] + (size_t)w * q.table_stride;
     const bool norm = tb.normalise[0] != 0, untouched = norm && q.steps[0][2 * w + root_player] == 0;
-    auto sig = [&](int h, int j) { return en_root_sig(T, H, nc, norm, untouched, h, j); };
+    auto sig = [&](int h, int j) { return avg_prob(T, 0, h, H, nc, norm, untouched, j); };
     if (root_player != me) {                         // phase 1: the agent's root row for LBR's seat, per raise
       for (int a = lo; a <= A - 2; ++a)
         for (int h = 0; h < H; ++h) p.sigx[((size_t)s * A + a) * H + h] = sig(h, a - lo);
@@ -286,9 +263,7 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
       trace_ply(1, lb, me ^ 1, hand_l, a, 1.0);
       prev_bid = lb; caller = me ^ 1; ++ply;
     } else if (lb < A - 2) {                         // LBR's next decision waits for phase 1
-      q.last_bid[s] = lb; q.player[s] = me ^ 1; q.ply[s] = ply; q.round[s] = round + 1;
-      q.mt_idx[s] = rng.idx;
-      atomicAdd(q.left, 1);
+      match_continue(q, s, lb, me ^ 1, ply, round + 1, rng.idx);
       return;
     }
     terminal = true;
@@ -299,15 +274,20 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
     const int* __restrict__ child_begin = q.child_begin + t.node_off;
     const int* __restrict__ nchild = q.nchild + t.node_off;
     int node = 0;
+    // the agent's strategy at (node, hand, child j) of the subgame in wave slot w
+    auto sig = [&](int cb, int nc, int actor, int hand, int j) {
+      return avg_prob(tb.table[0] + (size_t)w * q.table_stride, cb - 1, hand, H, nc, tb.normalise[0] != 0,
+                      tb.normalise[0] && q.steps[0][2 * w + actor] == 0, j);
+    };
     while (depth < q.max_depth) {
       const int nc = nchild[node], cb = child_begin[node], lo = lb < 0 ? 0 : lb + 1;
       const int actor = root_player ^ (depth & 1);
       int j;
       if (actor == me) {
-        j = sp_discrete(rng, nc, [&](int i) { return lbr_sig(p, tb, w, cb, nc, actor, hand_a, i); });
-        trace_ply(0, lb, actor, hand_a, lo + j, lbr_sig(p, tb, w, cb, nc, actor, hand_a, j));
+        j = sp_discrete(rng, nc, [&](int i) { return sig(cb, nc, actor, hand_a, i); });
+        trace_ply(0, lb, actor, hand_a, lo + j, sig(cb, nc, actor, hand_a, j));
         for (int h = 0; h < H; ++h) {
-          const double sg = lbr_sig(p, tb, w, cb, nc, actor, h, j);
+          const double sg = sig(cb, nc, actor, h, j);
           bel[actor * H + h] *= sg;
           beta[h] *= sg;
         }
@@ -317,11 +297,9 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
       } else {
         if (depth + 1 == q.max_depth && lo <= A - 2) {   // the raises lead to pseudo-leaves: what-if solves first
           for (int a = lo; a <= A - 2; ++a)
-            for (int h = 0; h < H; ++h) p.sigx[((size_t)s * A + a) * H + h] = lbr_sig(p, tb, w, cb, nc, actor, h, a - lo);
+            for (int h = 0; h < H; ++h) p.sigx[((size_t)s * A + a) * H + h] = sig(cb, nc, actor, h, a - lo);
           p.pend[s] = 1;
-          q.last_bid[s] = lb; q.player[s] = actor; q.ply[s] = ply; q.round[s] = round;
-          q.mt_idx[s] = rng.idx;
-          atomicAdd(q.left, 1);
+          match_continue(q, s, lb, actor, ply, round, rng.idx);
           return;
         }
         const int a = decide(lb, [&](int a, int& wc, int& cb2, int& nc2) {
@@ -330,7 +308,7 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
         });
         j = a - lo;
         trace_ply(1, lb, actor, hand_l, a, 1.0);
-        for (int h = 0; h < H; ++h) bel[actor * H + h] *= lbr_sig(p, tb, w, cb, nc, actor, h, j);
+        for (int h = 0; h < H; ++h) bel[actor * H + h] *= sig(cb, nc, actor, h, j);
       }
       prev_bid = lb; caller = actor;
       node = cb + j;
@@ -341,25 +319,10 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
   }
   if (!terminal) {                                   // pseudo-leaf: root of the agent's next subgame (beta stays as it is)
     sp_normalize(bel, H); sp_normalize(bel + H, H);
-    q.last_bid[s] = lb; q.player[s] = root_player ^ (depth & 1); q.ply[s] = ply; q.round[s] = round + 1;
-    q.mt_idx[s] = rng.idx;
-    atomicAdd(q.left, 1);
+    match_continue(q, s, lb, root_player ^ (depth & 1), ply, round + 1, rng.idx);
     return;
   }
-  const int quantity = 1 + prev_bid / F, face = prev_bid % F;
-  const int count = (int)q.matches[q.hands[2 * s] * F + face] + (int)q.matches[q.hands[2 * s + 1] * F + face];
-  const int winner = count >= quantity ? caller ^ 1 : caller;
-  q.payoff[g] = winner == me ? 1.f : -1.f;
-  q.plies[g] = ply;
-  q.rounds[g] = round + 1;
-  if (traced) q.tr_plies[g] = ply;
-  const int next = g + q.S;
-  if (next < q.G) {
-    match_start(q, s, next);
-    atomicAdd(q.left, 1);
-  } else {
-    q.game[s] = -1;
-  }
+  match_settle<match_start>(q, s, g, prev_bid, caller, ply, round + 1);   // the agent is agent 0: its payoff
 }
 
 }  // namespace cfrb

@@ -37,12 +37,6 @@ __device__ __forceinline__ uint32_t match_stream_seed(uint64_t seed, uint64_t ke
   return (uint32_t)z ^ (uint32_t)(z >> 32);
 }
 
-// std::mt19937(x) into an interleaved state whose words lie `stride` apart (word i at st[i * stride])
-__device__ __forceinline__ void mt_seed_strided(uint32_t* st, int stride, uint32_t x) {
-  st[0] = x;
-  for (int i = 1; i < 624; ++i) { x = 1812433253u * (x ^ (x >> 30)) + (uint32_t)i; st[(size_t)i * stride] = x; }
-}
-
 // std::mt19937(x) into the interleaved state of slot s
 __device__ __forceinline__ void match_mt_seed(const MatchDev& p, int s, uint32_t x) {
   mt_seed_strided(p.mt + s, p.S, x);
@@ -61,30 +55,81 @@ __device__ void match_start(const MatchDev& p, int s, int g) {
   for (int i = 0; i < 4 * p.H; ++i) b[i] = 1.0 / p.H;
 }
 
+// The start of a game in a slot: match_start, or ply_start for the per-ply walk (ply_kernels.cuh).
+using MatchStart = void (*)(const MatchDev&, int, int);
+
+// Game s in slot s, or the slot retired when there are fewer games than slots.
+template <MatchStart start>
 __global__ void __launch_bounds__(128) match_deal_kernel(MatchDev p) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= p.S) return;
-  if (s < p.G) match_start(p, s, s);
+  if (s < p.G) start(p, s, s);
   else p.game[s] = -1;
+}
+
+// Slot s stops at the root of its next subgame: public node (last_bid, player), plies and rounds so far, and its stream position.
+__device__ __forceinline__ void match_continue(const MatchDev& p, int s, int last_bid, int player, int ply, int round, int mt_idx) {
+  p.last_bid[s] = last_bid; p.player[s] = player; p.ply[s] = ply; p.round[s] = round;
+  p.mt_idx[s] = mt_idx;
+  atomicAdd(p.left, 1);
+}
+
+// The liar call of seat `caller` on bid `bid` ends game g in slot s after `plies` plies and `rounds` rounds: the bidder wins iff
+// both hands together hold at least `quantity` dice of `face`, and the payoff is agent 0's (seat 0 in even games).  The slot then
+// starts its next game, or retires when its quota is done.
+template <MatchStart start>
+__device__ __forceinline__ void match_settle(const MatchDev& p, int s, int g, int bid, int caller, int plies, int rounds) {
+  const int quantity = 1 + bid / p.F, face = bid % p.F;
+  const int count = (int)p.matches[p.hands[2 * s] * p.F + face] + (int)p.matches[p.hands[2 * s + 1] * p.F + face];
+  const int winner = count >= quantity ? caller ^ 1 : caller;
+  p.payoff[g] = (winner ^ (g & 1)) == 0 ? 1.f : -1.f;
+  p.plies[g] = plies;
+  p.rounds[g] = rounds;
+  if (g < p.trace_games) p.tr_plies[g] = plies;
+  const int next = g + p.S;
+  if (next < p.G) {
+    start(p, s, next);
+    atomicAdd(p.left, 1);
+  } else {
+    p.game[s] = -1;
+  }
+}
+
+// Levels [0, levels) of the acting strategy (avg_row) of the subgame with template tp solved in one wave slot, into a cache row c,
+// entry (child - 1) * H + hand; by one warp, whose lanes stride over the (node, hand) pairs of a level, hands innermost.  T is the
+// slot's table, steps its two step counters, root_player the player to move at the subgame's root.  The per-ply walk and the agent
+// (agent_kernels.cuh) cache their solves through this.
+template <typename real>
+__device__ __forceinline__ void capture_levels(int lane, const TemplateDev& tp, const int* __restrict__ child_begin,
+                                               const int* __restrict__ nchild, const int* __restrict__ level_begin, int H,
+                                               const real* __restrict__ T, bool normalise, const int* __restrict__ steps,
+                                               int root_player, int levels, double* __restrict__ c) {
+  child_begin += tp.node_off; nchild += tp.node_off;
+  const int* __restrict__ level = level_begin + tp.level_off;
+  for (int d = 0; d < levels; ++d) {
+    const int nb = level[d], ne = level[d + 1];
+    const bool untouched = normalise && steps[root_player ^ (d & 1)] == 0;
+    for (int e = nb * H + lane; e < ne * H; e += 32) {
+      const int node = e / H, hand = e - node * H;
+      const int cb = child_begin[node], nc = nchild[node];
+      if (nc == 0) continue;
+      const size_t at = (size_t)(cb - 1) * H + hand;
+      avg_row(c + at, T + at, 0, 0, H, nc, normalise, untouched);
+    }
+  }
 }
 
 // Wave index of every running slot (slot order) and the exclusive prefix sum of their pseudo-leaf counts; one CTA.
 __global__ void __launch_bounds__(1024) match_scan_kernel(MatchDev p) {
-  __shared__ int part_n[1024], part_r[1024];
+  __shared__ int part[2 * 1024];
   const int t = threadIdx.x, per = (p.S + 1023) / 1024;
   const int b = t * per, e = min(p.S, b + per);
   int n = 0, r = 0;
   for (int s = b; s < e; ++s)
     if (p.game[s] >= 0) { ++n; r += p.tmpl[p.last_bid[s] + 1].L; }
-  part_n[t] = n; part_r[t] = r;
-  __syncthreads();
-  for (int d = 1; d < 1024; d <<= 1) {
-    const int vn = t >= d ? part_n[t - d] : 0, vr = t >= d ? part_r[t - d] : 0;
-    __syncthreads();
-    part_n[t] += vn; part_r[t] += vr;
-    __syncthreads();
-  }
-  int w = part_n[t] - n, off = part_r[t] - r;
+  int x[2] = {n, r};                                 // running slots, rows
+  sp_block_scan(part, x);
+  int w = x[0] - n, off = x[1] - r;
   for (int s = b; s < e; ++s) {
     if (p.game[s] < 0) { p.widx[s] = -1; continue; }
     p.widx[s] = w;
@@ -93,8 +138,8 @@ __global__ void __launch_bounds__(1024) match_scan_kernel(MatchDev p) {
     off += p.tmpl[p.last_bid[s] + 1].L;
   }
   if (t == 1023) {
-    for (int k = 0; k < 2; ++k) { p.wave[k][0] = part_n[1023]; p.wave[k][1] = part_r[1023]; }
-    *p.running = part_n[1023];
+    for (int k = 0; k < 2; ++k) { p.wave[k][0] = x[0]; p.wave[k][1] = x[1]; }
+    *p.running = x[0];
   }
 }
 
@@ -110,11 +155,7 @@ __global__ void __launch_bounds__(128) match_begin_kernel(MatchDev p, MatchTabs<
   const int r = p.round[s];
   const bool traced = g < p.trace_games;
   for (int k = 0; k < 2; ++k) {
-    int act = -1;
-    if (p.sampled) {
-      const int n = p.iters[k];
-      act = sp_discrete(rng, n, [](int i) { return i % 2 ? 0.0 : (i / 2. + 1); });
-    }
+    const int act = p.sampled ? sp_act_iteration(rng, p.iters[k]) : -1;
     p.sg_tmpl[k][w] = p.last_bid[s] + 1;
     p.sg_player[k][w] = p.player[s];
     p.sg_act[k][w] = act;
@@ -145,17 +186,12 @@ __global__ void __launch_bounds__(128) match_advance_kernel(MatchDev p, MatchTab
   const int* __restrict__ nchild = p.nchild + t.node_off;
   double* bel = p.bel + (size_t)s * 4 * H;         // [agent][player][hand]
   const bool traced = g < p.trace_games;
-  // strategy of agent k at (node, hand, child j): average mode = normalise(S) with cfrb_fetch_compact(..., 4)'s operation order
-  // and uniform-until-first-update rule (CFR) or the average table itself (FP); sampled mode = the act_iteration snapshot
+  // strategy of agent k at (node, hand, child j): average mode = avg_prob of S (CFR) or Sg (FP); sampled mode = the act_iteration
+  // snapshot, as it is
   auto sig = [&](int k, int node, int actor, int hand, int j) -> double {
     const real* T = tb.table[k] + (size_t)w * p.table_stride;
-    const int cb = child_begin[node], nc = nchild[node];
-    const double v = (double)T[(size_t)(cb + j - 1) * H + hand];
-    if (!tb.normalise[k]) return v;
-    if (p.steps[k][2 * w + actor] == 0) return 1.0 / nc;
-    double sum = 0;
-    for (int i = 0; i < nc; ++i) sum += (double)T[(size_t)(cb + i - 1) * H + hand];
-    return sum > 0 ? v / sum : 1.0 / nc;
+    return avg_prob(T, child_begin[node] - 1, hand, H, nchild[node], tb.normalise[k] != 0,
+                    tb.normalise[k] && p.steps[k][2 * w + actor] == 0, j);
   };
   int node = 0, depth = 0, ply = p.ply[s], prev_bid = lb, caller = 0;
   bool terminal = false;
@@ -182,26 +218,10 @@ __global__ void __launch_bounds__(128) match_advance_kernel(MatchDev p, MatchTab
   }
   if (!terminal) {                                   // pseudo-leaf: root of both agents' next subgames
     for (int i = 0; i < 4; ++i) sp_normalize(bel + i * H, H);
-    p.last_bid[s] = lb; p.player[s] = root_player ^ (depth & 1); p.ply[s] = ply; p.round[s] += 1;
-    p.mt_idx[s] = rng.idx;
-    atomicAdd(p.left, 1);
+    match_continue(p, s, lb, root_player ^ (depth & 1), ply, p.round[s] + 1, rng.idx);
     return;
   }
-  // liar call on bid prev_bid: the bidder wins iff both hands together hold at least `quantity` dice of `face`
-  const int quantity = 1 + prev_bid / p.F, face = prev_bid % p.F;
-  const int count = (int)p.matches[p.hands[2 * s] * p.F + face] + (int)p.matches[p.hands[2 * s + 1] * p.F + face];
-  const int winner = count >= quantity ? caller ^ 1 : caller;
-  p.payoff[g] = (winner ^ (g & 1)) == 0 ? 1.f : -1.f;
-  p.plies[g] = ply;
-  p.rounds[g] = p.round[s] + 1;
-  if (traced) p.tr_plies[g] = ply;
-  const int next = g + p.S;
-  if (next < p.G) {
-    match_start(p, s, next);
-    atomicAdd(p.left, 1);
-  } else {
-    p.game[s] = -1;
-  }
+  match_settle<match_start>(p, s, g, prev_bid, caller, ply, p.round[s] + 1);
 }
 
 }  // namespace cfrb

@@ -13,7 +13,7 @@
 //
 //   ply_scan      one CTA: per agent, the wave index of every running slot where it solves and the packed value-net row offsets
 //   ply_begin     per slot: each solving agent's subgame descriptor (and, sampled, its act_iteration), the trace of the ply's beliefs
-//   ply_capture   warp per (to-leaf agent, solving slot): the acting strategy into the cache, agent_capture_kernel's operations
+//   ply_capture   warp per (to-leaf agent, solving slot): the acting strategy into the cache (capture_levels)
 //   ply_advance   per slot: one action of the mover's agent for the mover's hand, both agents' belief updates, and at a liar call
 //                 the payoff and the slot's next game (match_start)
 //
@@ -31,18 +31,6 @@
 namespace cfrb {
 
 constexpr int kPlySampled = 1, kPlyEveryNode = 2;   // CFRB_MATCH_SAMPLED, CFRB_MATCH_EVERY_NODE
-
-// An every-node agent's probability of edge j for hand h at the root of its subgame, whose table is T (row j = edge j): normalised
-// as rec_expand_kernel does it (uniform while `untouched`, before the mover's first update; FP: Sg as it is).  The LBR walk
-// (lbr_kernels.cuh) reads every-node rows through this too.
-template <typename real>
-__device__ __forceinline__ double en_root_sig(const real* T, int H, int nc, bool normalise, bool untouched, int h, int j) {
-  const double v = (double)T[(size_t)j * H + h];
-  if (!normalise) return v;
-  double sum = 0;
-  for (int i = 0; i < nc; ++i) sum += (double)T[(size_t)i * H + h];
-  return (sum > 0 && !untouched) ? v / sum : 1.0 / nc;
-}
 
 // An every-node agent's update of the mover's belief row after an action: times sig(h), then eps-normalised.
 template <typename Sig>
@@ -62,19 +50,12 @@ __device__ void ply_start(const MatchDev& p, int s, int g) {
   p.sub_node[0][s] = p.sub_node[1][s] = -1;
 }
 
-__global__ void __launch_bounds__(128) ply_deal_kernel(MatchDev p) {
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= p.S) return;
-  if (s < p.G) ply_start(p, s, s);
-  else p.game[s] = -1;
-}
-
 // Per agent: the wave index of every slot it solves (slot order) and the exclusive prefix sum of their pseudo-leaf counts; one CTA.
 __global__ void __launch_bounds__(1024) ply_scan_kernel(MatchDev p) {
-  __shared__ int part[5][1024];                      // agent 0 slots, rows; agent 1 slots, rows; running slots
+  __shared__ int part[5 * 1024];
   const int t = threadIdx.x, per = (p.S + 1023) / 1024;
   const int b = t * per, e = min(p.S, b + per);
-  int v[5] = {0, 0, 0, 0, 0};
+  int v[5] = {0, 0, 0, 0, 0};                        // agent 0 slots, rows; agent 1 slots, rows; running slots
   for (int s = b; s < e; ++s) {
     if (p.game[s] < 0) continue;
     const int L = p.tmpl[p.last_bid[s] + 1].L;
@@ -82,17 +63,10 @@ __global__ void __launch_bounds__(1024) ply_scan_kernel(MatchDev p) {
       if (ply_solves(p, k, s)) { v[2 * k] += 1; v[2 * k + 1] += L; }
     v[4] += 1;
   }
-  for (int i = 0; i < 5; ++i) part[i][t] = v[i];
-  __syncthreads();
-  for (int d = 1; d < 1024; d <<= 1) {
-    int u[5];
-    for (int i = 0; i < 5; ++i) u[i] = t >= d ? part[i][t - d] : 0;
-    __syncthreads();
-    for (int i = 0; i < 5; ++i) part[i][t] += u[i];
-    __syncthreads();
-  }
+  int x[5] = {v[0], v[1], v[2], v[3], v[4]};        // inclusive sums; v stays for the exclusive offsets
+  sp_block_scan(part, x);
   int w[2], off[2];
-  for (int k = 0; k < 2; ++k) { w[k] = part[2 * k][t] - v[2 * k]; off[k] = part[2 * k + 1][t] - v[2 * k + 1]; }
+  for (int k = 0; k < 2; ++k) { w[k] = x[2 * k] - v[2 * k]; off[k] = x[2 * k + 1] - v[2 * k + 1]; }
   for (int s = b; s < e; ++s) {
     const int L = p.game[s] >= 0 ? p.tmpl[p.last_bid[s] + 1].L : 0;
     for (int k = 0; k < 2; ++k) {
@@ -104,8 +78,8 @@ __global__ void __launch_bounds__(1024) ply_scan_kernel(MatchDev p) {
     }
   }
   if (t == 1023) {
-    for (int k = 0; k < 2; ++k) { p.wave[k][0] = part[2 * k][1023]; p.wave[k][1] = part[2 * k + 1][1023]; }
-    *p.running = part[4][1023];
+    for (int k = 0; k < 2; ++k) { p.wave[k][0] = x[2 * k]; p.wave[k][1] = x[2 * k + 1]; }
+    *p.running = x[4];
   }
 }
 
@@ -124,7 +98,7 @@ __global__ void __launch_bounds__(128) ply_begin_kernel(MatchDev p, MatchTabs<re
     int act = -2;                                    // -2: k plays on inside its to-leaf subgame
     if (w >= 0) {
       act = -1;
-      if (p.policy[k] == kPlySampled) act = sp_discrete(rng, p.iters[k], [](int i) { return i % 2 ? 0.0 : (i / 2. + 1); });
+      if (p.policy[k] == kPlySampled) act = sp_act_iteration(rng, p.iters[k]);
       p.sg_tmpl[k][w] = p.last_bid[s] + 1;
       p.sg_player[k][w] = p.player[s];
       p.sg_act[k][w] = act;
@@ -153,34 +127,9 @@ __global__ void __launch_bounds__(128) ply_capture_kernel(MatchDev p, MatchTabs<
   if (!p.cache[k]) return;                           // every-node agents read their tables in place
   const int w = p.awidx[k][s];
   if (w < 0) return;
-  const int H = p.H;
   const TemplateDev tp = p.tmpl[p.sub_lb[k][s] + 1];
-  const int* __restrict__ child_begin = p.child_begin + tp.node_off;
-  const int* __restrict__ nchild = p.nchild + tp.node_off;
-  const int* __restrict__ level = p.level_begin + tp.level_off;
-  const real* __restrict__ T = tb.table[k] + (size_t)w * p.table_stride;
-  double* __restrict__ c = p.cache[k] + (size_t)s * p.table_stride;
-  const bool normalise = tb.normalise[k];
-  const int root_player = p.sub_player[k][s];
-  for (int d = 0; d < tp.levels; ++d) {
-    const int nb = level[d], ne = level[d + 1];
-    const bool untouched = normalise && p.steps[k][2 * w + (root_player ^ (d & 1))] == 0;
-    for (int e = nb * H + lane; e < ne * H; e += 32) {
-      const int node = e / H, hand = e - node * H;
-      const int cb = child_begin[node], nc = nchild[node];
-      if (nc == 0) continue;
-      const real* __restrict__ Te = T + (size_t)(cb - 1) * H + hand;
-      double* __restrict__ ce = c + (size_t)(cb - 1) * H + hand;
-      if (!normalise) {
-        for (int j = 0; j < nc; ++j) ce[j * H] = (double)Te[j * H];
-        continue;
-      }
-      double sum = 0;
-      for (int j = 0; j < nc; ++j) sum += (double)Te[j * H];
-      const bool uniform = untouched || !(sum > 0);
-      for (int j = 0; j < nc; ++j) ce[j * H] = uniform ? 1.0 / nc : (double)Te[j * H] / sum;
-    }
-  }
+  capture_levels(lane, tp, p.child_begin, p.nchild, p.level_begin, p.H, tb.table[k] + (size_t)w * p.table_stride,
+                 tb.normalise[k] != 0, p.steps[k] + 2 * w, p.sub_player[k][s], tp.levels, p.cache[k] + (size_t)s * p.table_stride);
 }
 
 template <typename real>
@@ -211,10 +160,10 @@ __global__ void __launch_bounds__(128) ply_advance_kernel(MatchDev p, MatchTabs<
       c[k] = p.cache[k] + (size_t)s * p.table_stride + (size_t)(cb - 1) * H;
     }
   }
-  // agent k's probability of edge j for hand h: the every-node root row (en_root_sig), or the cached entry
+  // agent k's probability of edge j for hand h: the every-node root row, or the cached entry
   auto sig = [&](int k, int h, int j) -> double {
     if (c[k]) return c[k][(size_t)j * H + h];
-    return en_root_sig(T[k], H, nc, tb.normalise[k] != 0, untouched[k], h, j);
+    return avg_prob(T[k], 0, h, H, nc, tb.normalise[k] != 0, untouched[k], j);
   };
   const int j = sp_discrete(rng, nc, [&](int i) { return sig(agent, hand, i); });
   const int ply = p.ply[s], a = lo + j;
@@ -240,27 +189,8 @@ __global__ void __launch_bounds__(128) ply_advance_kernel(MatchDev p, MatchTabs<
       p.sub_node[k][s] = -1;
     }
   }
-  if (!terminal) {
-    p.last_bid[s] = a; p.player[s] = actor ^ 1; p.ply[s] = ply + 1; p.round[s] += 1;
-    p.mt_idx[s] = rng.idx;
-    atomicAdd(p.left, 1);
-    return;
-  }
-  // liar call on bid lb: the bidder wins iff both hands together hold at least `quantity` dice of `face`
-  const int quantity = 1 + lb / p.F, face = lb % p.F;
-  const int count = (int)p.matches[p.hands[2 * s] * p.F + face] + (int)p.matches[p.hands[2 * s + 1] * p.F + face];
-  const int winner = count >= quantity ? actor ^ 1 : actor;
-  p.payoff[g] = (winner ^ (g & 1)) == 0 ? 1.f : -1.f;
-  p.plies[g] = ply + 1;
-  p.rounds[g] = p.round[s] + 1;
-  if (g < p.trace_games) p.tr_plies[g] = ply + 1;
-  const int next = g + p.S;
-  if (next < p.G) {
-    ply_start(p, s, next);
-    atomicAdd(p.left, 1);
-  } else {
-    p.game[s] = -1;
-  }
+  if (!terminal) match_continue(p, s, a, actor ^ 1, ply + 1, p.round[s] + 1, rng.idx);
+  else match_settle<ply_start>(p, s, g, lb, actor, ply + 1, p.round[s] + 1);
 }
 
 }  // namespace cfrb

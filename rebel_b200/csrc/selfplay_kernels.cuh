@@ -74,6 +74,12 @@ struct SpRng {
   }
 };
 
+// std::mt19937(x) into an interleaved state whose words lie `stride` apart (word i at st[i * stride])
+__device__ __forceinline__ void mt_seed_strided(uint32_t* st, int stride, uint32_t x) {
+  st[0] = x;
+  for (int i = 1; i < 624; ++i) { x = 1812433253u * (x ^ (x >> 30)) + (uint32_t)i; st[(size_t)i * stride] = x; }
+}
+
 // std::discrete_distribution<int> over n weights w(0..n-1): probabilities w/sum, partial sums, last one forced to 1,
 // lower_bound of a canonical double.  (The linear scan returns the same index as the binary search: the sums never decrease.)
 template <typename W>
@@ -90,6 +96,12 @@ __device__ int sp_discrete(SpRng& rng, int n, W w) {
   return n - 1;
 }
 
+// The act_iteration of a sampled policy's subgame (compute_sampled_strategy_recursive_to_leaf, recursive_solving.cc:304-319):
+// weight i / 2 + 1 on even i < n, 0 on odd i.
+__device__ __forceinline__ int sp_act_iteration(SpRng& rng, int n) {
+  return sp_discrete(rng, n, [](int i) { return i % 2 ? 0.0 : (i / 2. + 1); });
+}
+
 // normalize_beliefs_inplace (recursive_solving.cc:41-44 -> normalize_probabilities_safe, util.h:68-78)
 __device__ __forceinline__ void sp_normalize(double* b, int H) {
   double s = 0;
@@ -97,13 +109,38 @@ __device__ __forceinline__ void sp_normalize(double* b, int H) {
   for (int h = 0; h < H; ++h) b[h] = (b[h] + 1e-80) / s;
 }
 
+// The average strategy an agent acts with, for one (node, hand) of a solved subgame's table T: child j of the node is entry
+// T[(r0 + j) * H + h], r0 = the node's first child - 1 and h the hand.  FP's average and the sampled snapshot are used as they are
+// (normalise false); CFR's sum is divided by its serial fp64 sum over the node's nc children, and is uniform while the acting
+// player has no update yet (untouched) or when that sum is not positive (cfrb_fetch_compact kind 4, normalise_avg in cfrb_api.cu).
+// Every play and exploitability walk reads average strategies through these, so they all agree bit for bit.
+template <typename real>
+__device__ __forceinline__ double avg_row_sum(const real* T, int r0, int h, int H, int nc) {
+  double sum = 0;
+  for (int j = 0; j < nc; ++j) sum += (double)T[(size_t)(r0 + j) * H + h];
+  return sum;
+}
+__device__ __forceinline__ double avg_entry(double v, double sum, int nc, bool normalise, bool untouched) {
+  return !normalise ? v : (sum > 0 && !untouched) ? v / sum : 1.0 / nc;
+}
+// child j alone
+template <typename real>
+__device__ __forceinline__ double avg_prob(const real* T, int r0, int h, int H, int nc, bool normalise, bool untouched, int j) {
+  const double v = (double)T[(size_t)(r0 + j) * H + h];
+  if (!normalise || untouched) return avg_entry(v, 0.0, nc, normalise, untouched);
+  return avg_entry(v, avg_row_sum(T, r0, h, H, nc), nc, true, false);
+}
+// every child, into out[j * H]
+template <typename real>
+__device__ __forceinline__ void avg_row(double* out, const real* T, int r0, int h, int H, int nc, bool normalise, bool untouched) {
+  const double sum = normalise ? avg_row_sum(T, r0, h, H, nc) : 0.0;
+  for (int j = 0; j < nc; ++j) out[j * H] = avg_entry((double)T[(size_t)(r0 + j) * H + h], sum, nc, normalise, untouched);
+}
+
 __global__ void __launch_bounds__(128) sp_seed_kernel(SpDev p, const uint32_t* __restrict__ seeds) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= p.K) return;
-  uint32_t* s = p.mt + g;
-  uint32_t x = seeds[g];
-  s[0] = x;
-  for (int i = 1; i < 624; ++i) { x = 1812433253u * (x ^ (x >> 30)) + (uint32_t)i; s[(size_t)i * p.K] = x; }
+  mt_seed_strided(p.mt + g, p.K, seeds[g]);
   p.mt_idx[g] = 624;
   p.g_last_bid[g] = -1; p.g_player[g] = 0;                       // RlRunner::step :161-163
   for (int i = 0; i < 2 * p.H; ++i) p.g_beliefs[(size_t)g * 2 * p.H + i] = 1.0 / p.H;
@@ -131,19 +168,27 @@ __global__ void __launch_bounds__(128) sp_begin_kernel(SpDev p, real* __restrict
   if (p.share) p.sg_init[g] = init;
 }
 
-// Inclusive sum of x over the 1024 threads of the CTA, through part[1024].
-__device__ int sp_block_scan(int* part, int x) {
+// Inclusive sums of a thread's V values over the 1024 threads of the CTA, through part[V * 1024]: x[i] becomes the sum of x[i]
+// over threads 0 .. threadIdx.x, so thread 1023 holds the totals (and so does part[i * 1024 + 1023]).
+template <int V>
+__device__ void sp_block_scan(int* part, int (&x)[V]) {
   const int t = threadIdx.x;
   __syncthreads();                               // earlier readers of part[] are done
-  part[t] = x;
+  for (int i = 0; i < V; ++i) part[i * 1024 + t] = x[i];
   __syncthreads();
   for (int d = 1; d < 1024; d <<= 1) {
-    const int v = t >= d ? part[t - d] : 0;
+    int u[V];
+    for (int i = 0; i < V; ++i) u[i] = t >= d ? part[i * 1024 + t - d] : 0;
     __syncthreads();
-    part[t] += v;
+    for (int i = 0; i < V; ++i) part[i * 1024 + t] += u[i];
     __syncthreads();
   }
-  return part[t];
+  for (int i = 0; i < V; ++i) x[i] = part[i * 1024 + t];
+}
+__device__ __forceinline__ int sp_block_scan(int* part, int x) {
+  int v[1] = {x};
+  sp_block_scan(part, v);
+  return v[0];
 }
 
 // Exclusive prefix sum of the pseudo-leaf counts of the wave's subgames (one CTA; K is at most a few 10^4).
