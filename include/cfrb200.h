@@ -577,6 +577,57 @@ int cfrb_match_trace(cfrb_match* m, int32_t game, int32_t* ply_records, double* 
                      int32_t* n_rounds);
 int cfrb_match_destroy(cfrb_match* m);
 
+/* ---- Blueprints: fixed full-tree strategies as players.  A blueprint is a compact fp64 table [N - 1][H] over the full game
+ * tree (entry (child - 1) * H + hand, the layout of cfrb_full_game_strategy, cfrb_to_leaf_strategy and cfrb_ev2_compact) held on
+ * one device with the full tree's child_begin [N] and the game's match counts [H][F].  It never solves: at a public node it acts
+ * with the row of that node's edges for its hand.  Games with A > CFRB_TO_LEAF_MAX_ACTIONS have none (CFRB_EINVAL, checked
+ * without a device).  A blueprint is read-only; it must outlive every match that plays it, and any number of matches may. */
+typedef struct cfrb_blueprint cfrb_blueprint;
+/* Host-only: device bytes of a blueprint, 8 (N - 1) H + 4 N + H F with N = 2^A - 1 full-tree nodes (2x4f: 17 MB, 2x5f: 0.43 GB,
+ * 5x2f: 0.55 GB, 1x11f: 0.77 GB). */
+int64_t cfrb_blueprint_bytes(int32_t num_dice, int32_t num_faces);
+/* Host-only: the checks of cfrb_blueprint_create on a host table, each refused with CFRB_EINVAL and a message naming the first
+ * bad node and hand (full-tree BFS order, hands innermost): a non-finite or negative entry, or a (node, hand) row whose sum over
+ * the node's children is more than 1e-6 away from 1. */
+int cfrb_blueprint_check(int32_t num_dice, int32_t num_faces, const double* compact);
+/* Upload a host table to `device` after cfrb_blueprint_check's checks.  A cfrb_blueprint_bytes need above the device's free
+ * memory is refused with CFRB_ENOMEM before anything is allocated. */
+int cfrb_blueprint_create(int32_t device, int32_t num_dice, int32_t num_faces, const double* compact, cfrb_blueprint** out);
+/* The solver's current average strategy, copied on its device: bit for bit what cfrb_full_game_strategy returns. */
+int cfrb_blueprint_from_full_game(cfrb_full_game* g, cfrb_blueprint** out);
+/* The full-tree strategy the handle's last to-leaf or every-node walk filled, copied on its device: bit for bit what
+ * cfrb_to_leaf_strategy returns.  CFRB_ESTATE when the handle holds none. */
+int cfrb_blueprint_from_handle(cfrb_handle* h, cfrb_blueprint** out);
+/* Synchronises.  The table, compact [N - 1][H]. */
+int cfrb_blueprint_strategy(const cfrb_blueprint* b, double* compact);
+int cfrb_blueprint_destroy(cfrb_blueprint* b);
+
+/* One seat of cfrb_match_create3: a handle playing `policy` (CFRB_MATCH_*), or a blueprint (h NULL; policy is not read). */
+typedef struct cfrb_match_agent {
+  cfrb_handle* h;
+  cfrb_blueprint* bp;
+  int32_t policy;
+} cfrb_match_agent;
+/* A match in which either seat, or both, may be a blueprint.  Without a blueprint it is cfrb_match_create2(a.h, b.h, ...,
+ * a.policy, b.policy).  With one it plays the per-ply walk of cfrb_match_create2: a blueprint solves nothing and keeps no beliefs;
+ * it holds the full-tree node of each game (the root at the deal, child_begin[node] + j after action j) and acts there with its
+ * table's row.  Its draws are the action draws of the game's (seed, g) stream at the point where any other policy draws, and it
+ * draws no act_iteration, so a blueprint holding the table an AVERAGE or EVERY_NODE agent acts with plays that agent's games bit
+ * for bit.  A match of two blueprints needs no handle: it runs walk kernels only, on a stream of its own.  The agents must play
+ * the same game on the same device; a handle agent is refused as in cfrb_match_create2 (capacity, live session or match, bad
+ * policy, its strategy cache above the free memory: CFRB_ENOMEM).  cfrb_match_run / _results / _agent_solves / _trace /
+ * _destroy apply: a blueprint's solves are 0, its act_iterations trace entry is -2 on every ply and its traced beliefs stay
+ * uniform. */
+int cfrb_match_create3(const cfrb_match_agent* a, const cfrb_match_agent* b, int32_t n_slots, int32_t n_games, uint64_t seed,
+                       cfrb_match** out);
+/* Local best response against a blueprint: LBR's rule is exactly cfrb_match_create_lbr's, with sigma(child(a)) and every update of
+ * beta read from the blueprint's table, so there are no what-if solves and no solves at all.  A round plays every running slot's
+ * game to its end (walk kernels only, on a stream of the match's own).  Seats, deals and the agent's draws are a match's; a
+ * blueprint holding the table of an AVERAGE or EVERY_NODE agent's walked policy gives cfrb_match_create_lbr2's payoffs and LBR
+ * trace for that agent bit for bit.  cfrb_match_run / _results / _trace / _lbr_trace / _lbr_counts / _destroy apply: solves and
+ * whatif_solves are 0, and every traced ply has round 0. */
+int cfrb_match_create_lbr_blueprint(cfrb_blueprint* bp, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out);
+
 /* ---- Local best response (Lisy & Bowling, 2017): a lower bound on one agent's exploitability on any game.  The agent (one
  * handle) plays as in a CFRB_MATCH_AVERAGE match against LBR, which best-responds one decision at a time: with its fp64 belief
  * beta over the agent's hand (uniform, times the agent's strategy after every agent action, renormalised) it plays the argmax
@@ -644,6 +695,11 @@ int cfrb_match_lbr_counts(cfrb_match* m, int64_t* whatif_solves, int64_t* deferr
  * in a live match).  The caller keeps the handle and destroys it after the agent. */
 typedef struct cfrb_agent cfrb_agent;
 int cfrb_agent_create(cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t policy, cfrb_agent** out);
+/* An agent that plays a blueprint: step, policy and state answer from its table at the full-tree node of each table, its draws
+ * are the (seed, key) streams of cfrb_agent_create's agents, and it never solves (subgames 0, act_iteration -1, root beliefs
+ * uniform, counts 0).  A blueprint holding an AVERAGE agent's walked to-leaf policy answers as that agent, bit for bit.  It has
+ * no handle and runs on a stream of its own; the blueprint must outlive it. */
+int cfrb_agent_create_blueprint(cfrb_blueprint* bp, int32_t n_tables, uint64_t seed, cfrb_agent** out);
 /* Start (or restart) a game at each listed table: the agent sits in seat seats[i] (0 moves first) with hand hands[i].  keys[i]
  * keys the game's stream; keys NULL: the number of games this agent had started before, counted in list order. */
 int cfrb_agent_new_games(cfrb_agent* a, int32_t n, const int32_t* ids, const int32_t* seats, const int32_t* hands, const uint64_t* keys);

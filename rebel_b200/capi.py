@@ -16,6 +16,10 @@ SOLVER_CFR, SOLVER_FP = 0, 1
 STATE_F64, STATE_F32 = 0, 1
 
 
+class MatchAgent(C.Structure):
+    _fields_ = [("h", C.c_void_p), ("bp", C.c_void_p), ("policy", C.c_int32)]
+
+
 class CfrbError(RuntimeError):
     pass
 
@@ -170,6 +174,16 @@ def lib():
     L.cfrb_match_results.argtypes = [vp, _fp, _ip, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.cfrb_match_trace.argtypes = [vp, C.c_int32, _ip, _dp, _ip, _dp, _ip]
     L.cfrb_match_destroy.argtypes = [vp]
+    L.cfrb_match_create3.argtypes = [C.POINTER(MatchAgent), C.POINTER(MatchAgent), C.c_int32, C.c_int32, C.c_uint64, C.POINTER(vp)]
+    L.cfrb_match_create_lbr_blueprint.argtypes = [vp, C.c_int32, C.c_int32, C.c_uint64, C.POINTER(vp)]
+    L.cfrb_blueprint_bytes.argtypes = [C.c_int32] * 2
+    L.cfrb_blueprint_bytes.restype = C.c_int64
+    L.cfrb_blueprint_check.argtypes = [C.c_int32, C.c_int32, _dp]
+    L.cfrb_blueprint_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, _dp, C.POINTER(vp)]
+    L.cfrb_blueprint_from_full_game.argtypes = [vp, C.POINTER(vp)]
+    L.cfrb_blueprint_from_handle.argtypes = [vp, C.POINTER(vp)]
+    L.cfrb_blueprint_strategy.argtypes = [vp, _dp]
+    L.cfrb_blueprint_destroy.argtypes = [vp]
     L.cfrb_match_create_lbr.argtypes = [vp, C.c_int32, C.c_int32, C.c_uint64, C.POINTER(vp)]
     L.cfrb_match_create_lbr2.argtypes = [vp, C.c_int32, C.c_int32, C.c_uint64, C.c_int32, C.POINTER(vp)]
     L.cfrb_match_lbr_trace.argtypes = [vp, C.c_int32, _dp, _dp]
@@ -765,15 +779,83 @@ def match_cache_bytes(num_dice, num_faces, max_depth, n_slots, policy_a, policy_
     return _check(lib().cfrb_match_cache_bytes(num_dice, num_faces, max_depth, n_slots, policy_a, pb))
 
 
+class Blueprint:
+    """A fixed full-tree strategy on one device (cfrb_blueprint_*): the compact table [N - 1, H] (entry (child - 1) * H + hand)
+    that FullGame.strategy(), WaveSolver.to_leaf_strategy() and ev2_compact use.  It plays in a Match in place of a WaveSolver
+    and never solves.  Build it from a host table (checked row by row), from a FullGame, or from a WaveSolver's last to-leaf or
+    every-node walk; the last two copy on the device, bit for bit the table their own fetches return."""
+
+    def __init__(self, num_dice, num_faces, strategy=None, device=0, _from=None):
+        self._b = C.c_void_p()
+        self.D, self.F = num_dice, num_faces
+        self.H, self.A = num_faces ** num_dice, 1 + 2 * num_dice * num_faces
+        self.N = (1 << self.A) - 1
+        if _from is not None:
+            _check(_from(C.byref(self._b)))
+            return
+        s = _blueprint_table(num_dice, num_faces, strategy)
+        _check(lib().cfrb_blueprint_create(device, num_dice, num_faces, _p(s, _dp), C.byref(self._b)))
+
+    @classmethod
+    def from_full_game(cls, fg):
+        return cls(fg.cfg.num_dice, fg.cfg.num_faces, _from=lambda out: lib().cfrb_blueprint_from_full_game(fg._g, out))
+
+    @classmethod
+    def from_solver(cls, solver):
+        return cls(solver.cfg.num_dice, solver.cfg.num_faces, _from=lambda out: lib().cfrb_blueprint_from_handle(solver._h, out))
+
+    def strategy(self):
+        out = np.zeros((self.N - 1, self.H))
+        _check(lib().cfrb_blueprint_strategy(self._b, _p(out, _dp)))
+        return out
+
+    def close(self):
+        if self._b:
+            lib().cfrb_blueprint_destroy(self._b)
+            self._b = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def blueprint_bytes(num_dice, num_faces):
+    """Host-only: device bytes of a blueprint of this game, 8 (N - 1) H + 4 N + H F with N = 2^A - 1."""
+    return _check(lib().cfrb_blueprint_bytes(num_dice, num_faces))
+
+
+def _blueprint_table(num_dice, num_faces, strategy):
+    """The table as contiguous fp64 [N - 1, H]; a game above 23 actions (CfrbError) or another shape (ValueError) is refused."""
+    blueprint_bytes(num_dice, num_faces)
+    H, N = num_faces ** num_dice, (1 << (1 + 2 * num_dice * num_faces)) - 1
+    s = np.ascontiguousarray(strategy, dtype=np.float64)
+    if s.shape != (N - 1, H):
+        raise ValueError(f"blueprint of {num_dice}x{num_faces}f: strategy must be [{N - 1}, {H}], got {list(s.shape)}")
+    return s
+
+
+def blueprint_check(num_dice, num_faces, strategy):
+    """Host-only: cfrb_blueprint_create's checks of a table (CfrbError naming the first bad node and hand)."""
+    s = _blueprint_table(num_dice, num_faces, strategy)
+    _check(lib().cfrb_blueprint_check(num_dice, num_faces, _p(s, _dp)))
+
+
 class Match:
     """A head-to-head match between the agents of two WaveSolvers (cfrb_match_*): n_games games, n_slots at a time.  Agent a
     plays `policy`, agent b policy_b (None: the same); a pair of different policies, or MATCH_EVERY_NODE, plays the per-ply walk
-    (cfrb_match_create2), whose trace has one round per ply."""
+    (cfrb_match_create2), whose trace has one round per ply.  Either agent may be a Blueprint instead (cfrb_match_create3, the
+    per-ply walk; its policy is not read)."""
 
     def __init__(self, a, b, n_slots, n_games, seed=0, policy=MATCH_SAMPLED, policy_b=None):
         self.a, self.b, self.G = a, b, n_games
         self._m = C.c_void_p()
-        if policy_b is None or policy_b == policy:
+        if isinstance(a, Blueprint) or isinstance(b, Blueprint):
+            pb = policy if policy_b is None else policy_b
+            ag = [MatchAgent(None, x._b, 0) if isinstance(x, Blueprint) else MatchAgent(x._h, None, p) for x, p in ((a, policy), (b, pb))]
+            _check(lib().cfrb_match_create3(C.byref(ag[0]), C.byref(ag[1]), n_slots, n_games, seed, C.byref(self._m)))
+        elif policy_b is None or policy_b == policy:
             _check(lib().cfrb_match_create(a._h, b._h, n_slots, n_games, seed, policy, C.byref(self._m)))
         else:
             _check(lib().cfrb_match_create2(a._h, b._h, n_slots, n_games, seed, policy, policy_b, C.byref(self._m)))
@@ -825,12 +907,15 @@ class LbrMatch(Match):
     """Local best response against the agent of one WaveSolver (cfrb_match_create_lbr2): n_games games, n_slots at a time, at
     most the solver's max_subgames subgames per round.  The agent plays `policy`, MATCH_AVERAGE or MATCH_EVERY_NODE (then a
     trace round is a node where the agent solved a subgame it acts or updates beliefs from).  results()["payoff_a"] is the
-    agent's payoff; in trace() agent 1 is LBR."""
+    agent's payoff; in trace() agent 1 is LBR.  The agent may be a Blueprint (cfrb_match_create_lbr_blueprint: no solves; policy
+    is not read)."""
 
     def __init__(self, agent, n_slots, n_games, seed=0, policy=MATCH_AVERAGE):
         self.a, self.b, self.G = agent, None, n_games
         self._m = C.c_void_p()
-        if policy == MATCH_AVERAGE:
+        if isinstance(agent, Blueprint):
+            _check(lib().cfrb_match_create_lbr_blueprint(agent._b, n_slots, n_games, seed, C.byref(self._m)))
+        elif policy == MATCH_AVERAGE:
             _check(lib().cfrb_match_create_lbr(agent._h, n_slots, n_games, seed, C.byref(self._m)))
         else:
             _check(lib().cfrb_match_create_lbr2(agent._h, n_slots, n_games, seed, policy, C.byref(self._m)))

@@ -22,6 +22,9 @@
 // An every-node agent (CFRB_MATCH_EVERY_NODE, compute_strategy_recursive) has an unsolved subgame root at every node: it caches the
 // root row only, and after every action eps-normalises the mover's row and stands at an unsolved root again.
 //
+// A blueprint agent (cfrb_agent_create_blueprint) never solves: `cache` is the blueprint's full-tree table (stride 0), `node` a
+// full-tree node (bp_child_begin non-null), and no node is a pseudo-leaf, so step and policy read the table at every node.
+//
 // This header is compiled into the -fmad=false translation unit: the belief arithmetic is the match walk's, bit for bit.
 #pragma once
 #include <cuda_runtime.h>
@@ -110,13 +113,25 @@ __global__ void __launch_bounds__(128) agent_capture_kernel(AgentDev p, MatchTab
   if (lane == 0) p.status[t] = 2;
 }
 
+// The first child and the child count of table t's node: in its subgame template, or in the blueprint's full tree.
+__device__ __forceinline__ void agent_node(const AgentDev& p, int t, int& cb, int& nc) {
+  const int node = p.node[t];
+  if (p.bp_child_begin) {
+    const int lb = p.last_bid[t];
+    cb = p.bp_child_begin[node]; nc = lb < 0 ? p.A - 1 : p.A - 1 - lb;   // bids lo .. A - 1, no liar call at the game root
+    return;
+  }
+  const TemplateDev tp = p.tmpl[p.root_lb[t] + 1];
+  cb = p.child_begin[tp.node_off + node]; nc = p.nchild[tp.node_off + node];
+}
+
 __global__ void __launch_bounds__(128) agent_step_kernel(AgentDev p) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p.n) return;
   const int t = p.ids[i], H = p.H, A = p.A;
-  const TemplateDev tp = p.tmpl[p.root_lb[t] + 1];
-  const int node = p.node[t], lb = p.last_bid[t], actor = p.player[t];
-  const int cb = p.child_begin[tp.node_off + node], nc = p.nchild[tp.node_off + node];
+  const int lb = p.last_bid[t], actor = p.player[t];
+  int cb, nc;
+  agent_node(p, t, cb, nc);
   const int lo = lb < 0 ? 0 : lb + 1;
   const double* __restrict__ c = p.cache + (size_t)t * p.stride + (size_t)(cb - 1) * H;   // c[j * H + hand]
   const bool mine = actor == p.seat[t];
@@ -163,9 +178,9 @@ __global__ void __launch_bounds__(128) agent_policy_kernel(AgentDev p) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= p.n * p.H) return;
   const int i = g / p.H, hand = g - i * p.H, t = p.ids[i], H = p.H, A = p.A;
-  const TemplateDev tp = p.tmpl[p.root_lb[t] + 1];
-  const int node = p.node[t], lb = p.last_bid[t];
-  const int cb = p.child_begin[tp.node_off + node], nc = p.nchild[tp.node_off + node];
+  const int lb = p.last_bid[t];
+  int cb, nc;
+  agent_node(p, t, cb, nc);
   const int lo = lb < 0 ? 0 : lb + 1;
   const double* __restrict__ c = p.cache + (size_t)t * p.stride + (size_t)(cb - 1) * H;
   double* out = p.pol + (size_t)g * A;

@@ -188,6 +188,7 @@ template <typename real>
 void lbr_launch_advance(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st) {
   lbr_advance_kernel<real><<<(p.m.S + 127) / 128, 128, 0, st>>>(p, t);
 }
+void lbr_launch_blueprint(const LbrDev& p, cudaStream_t st) { lbr_blueprint_kernel<<<(p.m.S + 127) / 128, 128, 0, st>>>(p); }
 void agent_launch_new(const AgentDev& p, cudaStream_t st) { agent_new_kernel<<<(p.n + 127) / 128, 128, 0, st>>>(p); }
 template <typename real>
 void agent_launch_begin(const AgentDev& p, const MatchTabs<real>& t, cudaStream_t st) {

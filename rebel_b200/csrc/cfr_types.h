@@ -168,6 +168,8 @@ template <typename real> void sp_launch_finish(const SpDev& p, const real* mu, c
 // after the last iteration of a shared wave: the representative's results to every copy, and every initial-state game's snapshot
 template <typename real> void sp_launch_share(const SpDev& p, const CfrDev<real>& d, cudaStream_t st);
 // Head-to-head matches (match_kernels.cuh): S game slots playing G games between two handles (agent 0 = A, 1 = B).
+// MatchDev::policy of a blueprint agent (no CFRB_MATCH_* value: only cfrb_match_create3 seats one)
+constexpr int kPlyBlueprint = 3;
 struct MatchDev {
   int S, G, A, H, F, max_depth, sampled, iters[2];
   uint64_t seed;
@@ -189,7 +191,7 @@ struct MatchDev {
   int trace_games;
   int* tr_ply; double* tr_prob; int* tr_plies;             // [T][A][6], [T][A], [T]
   int* tr_act; double* tr_bel; int* tr_rounds;             // [T][A][2], [T][A][2][2][H], [T]
-  // tree templates (read-only; both handles index the same ones)
+  // tree templates (read-only; both handles index the same ones; null in a match between two blueprints)
   const TemplateDev* tmpl; const int* child_begin; const int* nchild;
   const unsigned char* matches;       // [H][F]
   int table_stride;
@@ -203,6 +205,10 @@ struct MatchDev {
   int* sub_node[2]; int* sub_depth[2];   // [S] its template node and plies since that root (sub_node -1 = no subgame solved)
   double* cache[2];                   // [S][table_stride] to-leaf agent k's acting strategy in that subgame (null: every-node)
   int* solves[2];                     // [G] subgames agent k solved for game g
+  // blueprint agents (cfrb_match_create3): agent k's fixed full-tree table, entry (child - 1) * H + hand, the full tree's
+  // child_begin, and per slot the full-tree node the game stands at (all null for a solving agent)
+  const double* bp[2]; const int* bp_child_begin[2];
+  int* bp_node[2];                    // [S]
 };
 template <typename real>
 struct MatchTabs {
@@ -234,9 +240,13 @@ struct LbrDev {
   unsigned long long* deferred;       // [1] running slots left out of a round, summed over rounds
   int* solves; int* whatif;           // [G] subgames solved for game g, and how many of them were what-if solves
   double* tr_val; double* tr_beta;    // [T][A][A] LBR's action values (NaN = illegal / not LBR's ply), [T][A][H] its belief
+  // against a blueprint (cfrb_match_create_lbr_blueprint; null otherwise): its table and the full tree's child_begin
+  const double* bp; const int* bp_child_begin;
 };
 template <typename real> void lbr_launch_begin(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st);
 template <typename real> void lbr_launch_advance(const LbrDev& p, const MatchTabs<real>& t, cudaStream_t st);
+// against a blueprint: every running slot's game to its end, no solves
+void lbr_launch_blueprint(const LbrDev& p, cudaStream_t st);
 // A ReBeL agent played from outside (agent_kernels.cuh): T independent tables, each a game between the agent (one handle) and an
 // external player.  A call lists n distinct tables; the kernels of that call index the per-table state through ids[0..n).
 struct AgentDev {
@@ -265,6 +275,7 @@ struct AgentDev {
   const TemplateDev* tmpl; const int* child_begin; const int* nchild; const int* level_begin;
   int table_stride;
   int* wave; int* sg_tmpl; int* sg_player; int* sg_row_off; int* sg_act; const int* steps;
+  const int* bp_child_begin;          // a blueprint agent: the full tree's child_begin (then cache is its table, stride 0); else null
 };
 void agent_launch_new(const AgentDev& p, cudaStream_t st);
 // scan + subgame descriptors of the listed tables that stand at an unsolved root

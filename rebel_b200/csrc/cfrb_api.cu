@@ -3206,9 +3206,167 @@ int cfrb_stream_wait(cfrb_handle* h, void* cuda_stream) {
 
 }  // extern "C"
 
+// ============================================================================================ blueprints
+// A fixed full-tree strategy on one device: the compact table [N - 1][H] (entry (child - 1) * H + hand) of the full tree of
+// build_template(g, -1, ...), that tree's child_begin [N], and the game's matches [H][F].  Read-only once built.
+struct cfrb_blueprint {
+  int device = 0;
+  cfrb::GameShape g;
+  int64_t N = 0;
+  DevBuf<double> table;
+  DevBuf<int> child_begin;
+  DevBuf<unsigned char> matches;
+};
+
+// Nodes of the full tree: the root, every non-empty increasing sequence of the A - 1 bids, and each of those closed by the liar call.
+static int64_t full_tree_nodes(const cfrb::GameShape& g) { return ((int64_t)1 << g.A) - 1; }
+
+static int64_t blueprint_bytes(const cfrb::GameShape& g) {
+  const int64_t N = full_tree_nodes(g);
+  return 8 * (N - 1) * g.H + 4 * N + (int64_t)g.H * g.F;
+}
+
+static int blueprint_refuse_game(int32_t num_dice, int32_t num_faces, const std::string& w) {
+  if (num_dice < 1 || num_faces < 1) return fail(CFRB_EINVAL, w + ": num_dice and num_faces must be >= 1");
+  const cfrb::GameShape g(num_dice, num_faces);
+  if (g.A > CFRB_TO_LEAF_MAX_ACTIONS)
+    return fail(CFRB_EINVAL, w + ": games with more than " + std::to_string(CFRB_TO_LEAF_MAX_ACTIONS) + " actions have no blueprint (" +
+                                 std::to_string(num_dice) + "x" + std::to_string(num_faces) + "f has " + std::to_string(g.A) + ")");
+  return CFRB_OK;
+}
+
+// The device part of a blueprint of game g on `device`: refused with CFRB_ENOMEM before anything is allocated when it does not fit.
+// The table is left for the caller to fill.
+static int blueprint_alloc(cfrb_blueprint* b, int device, const cfrb::GameShape& g, const std::vector<int32_t>& child_begin,
+                           const std::string& w) {
+  CK(cudaSetDevice(device));
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const int64_t need = blueprint_bytes(g);
+  if (need > (int64_t)free_b)
+    return fail(CFRB_ENOMEM, w + ": the blueprint needs " + std::to_string(need) + " bytes of device memory, " + std::to_string(free_b) + " free");
+  b->device = device; b->g = g; b->N = full_tree_nodes(g);
+  std::vector<unsigned char> matches((size_t)g.H * g.F);
+  for (int hd = 0; hd < g.H; ++hd)
+    for (int f = 0; f < g.F; ++f) matches[(size_t)hd * g.F + f] = (unsigned char)g.num_matches(hd, f);
+  CK(b->table.alloc((size_t)(b->N - 1) * g.H));
+  CK(b->child_begin.alloc(child_begin.size()));
+  CK(b->matches.alloc(matches.size()));
+  CK(cudaMemcpy(b->child_begin.p, child_begin.data(), child_begin.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(b->matches.p, matches.data(), matches.size(), cudaMemcpyHostToDevice));
+  return CFRB_OK;
+}
+
+// A handle's full-tree strategy (br.strategy) and tree into a new blueprint, device to device.
+static int blueprint_from_br(cfrb_handle* h, cfrb_blueprint** out, const std::string& w) {
+  auto b = std::make_unique<cfrb_blueprint>();
+  int rc = blueprint_alloc(b.get(), h->cfg.device, h->g, h->br.t.child_begin, w);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(b->table.p, h->br.strategy.p, b->table.n * sizeof(double), cudaMemcpyDeviceToDevice, h->own_stream));
+  CK(cudaStreamSynchronize(h->own_stream));
+  *out = b.release();
+  return CFRB_OK;
+}
+
+extern "C" {
+
+int64_t cfrb_blueprint_bytes(int32_t num_dice, int32_t num_faces) {
+  const int rc = blueprint_refuse_game(num_dice, num_faces, "cfrb_blueprint_bytes");
+  return rc ? rc : blueprint_bytes(cfrb::GameShape(num_dice, num_faces));
+}
+
+}  // extern "C"
+
+// Every (node, hand) row of a host table over full tree t: finite, non-negative entries summing to 1 within 1e-6.
+static int blueprint_validate(const cfrb::GameShape& g, const cfrb::TreeTemplate& t, const double* compact, const std::string& w) {
+  for (int n = 0; n < t.N; ++n) {
+    const int cb = t.child_begin[n], nc = t.nchild[n];
+    if (nc == 0) continue;
+    for (int hd = 0; hd < g.H; ++hd) {
+      const std::string at = w + ": node " + std::to_string(n) + ", hand " + std::to_string(hd) + ": ";
+      double sum = 0;
+      for (int j = 0; j < nc; ++j) {
+        const double x = compact[(size_t)(cb + j - 1) * g.H + hd];
+        if (!std::isfinite(x)) return fail(CFRB_EINVAL, at + "non-finite entry for child " + std::to_string(j));
+        if (x < 0) return fail(CFRB_EINVAL, at + "negative entry for child " + std::to_string(j));
+        sum += x;
+      }
+      if (std::fabs(sum - 1.0) > 1e-6)
+        return fail(CFRB_EINVAL, at + "the row over the node's " + std::to_string(nc) + " children sums to " + std::to_string(sum));
+    }
+  }
+  return CFRB_OK;
+}
+
+extern "C" {
+
+int cfrb_blueprint_check(int32_t num_dice, int32_t num_faces, const double* compact) {
+  const std::string w = "cfrb_blueprint_check";
+  if (!compact) return fail(CFRB_EINVAL, w + ": null table");
+  const int rc = blueprint_refuse_game(num_dice, num_faces, w);
+  if (rc) return rc;
+  const cfrb::GameShape g(num_dice, num_faces);
+  return blueprint_validate(g, cfrb::build_template(g, -1, 1 << 30), compact, w);
+}
+
+int cfrb_blueprint_create(int32_t device, int32_t num_dice, int32_t num_faces, const double* compact, cfrb_blueprint** out) {
+  const std::string w = "cfrb_blueprint_create";
+  if (!out) return fail(CFRB_EINVAL, w + ": null argument");
+  *out = nullptr;
+  if (!compact) return fail(CFRB_EINVAL, w + ": null table");
+  int rc = blueprint_refuse_game(num_dice, num_faces, w);
+  if (rc) return rc;
+  const cfrb::GameShape g(num_dice, num_faces);
+  const cfrb::TreeTemplate t = cfrb::build_template(g, -1, 1 << 30);
+  if ((rc = blueprint_validate(g, t, compact, w))) return rc;
+  auto b = std::make_unique<cfrb_blueprint>();
+  if ((rc = blueprint_alloc(b.get(), device, g, t.child_begin, w))) return rc;
+  CK(cudaMemcpy(b->table.p, compact, b->table.n * sizeof(double), cudaMemcpyHostToDevice));
+  *out = b.release();
+  return CFRB_OK;
+}
+
+int cfrb_blueprint_from_full_game(cfrb_full_game* fg, cfrb_blueprint** out) {
+  const std::string w = "cfrb_blueprint_from_full_game";
+  if (!fg || !out) return fail(CFRB_EINVAL, w + ": null argument");
+  *out = nullptr;
+  const int rc = full_game_average(fg);   // the table cfrb_full_game_strategy returns
+  return rc ? rc : blueprint_from_br(fg->h, out, w);
+}
+
+int cfrb_blueprint_from_handle(cfrb_handle* h, cfrb_blueprint** out) {
+  const std::string w = "cfrb_blueprint_from_handle";
+  if (!h || !out) return fail(CFRB_EINVAL, w + ": null argument");
+  *out = nullptr;
+  if (!h->br.ready)
+    return fail(CFRB_ESTATE, w + ": the handle holds no full-tree strategy (run cfrb_to_leaf_exploitability or cfrb_recursive_exploitability)");
+  CK(cudaSetDevice(h->cfg.device));
+  return blueprint_from_br(h, out, w);
+}
+
+int cfrb_blueprint_strategy(const cfrb_blueprint* b, double* compact) {
+  if (!b || !compact) return fail(CFRB_EINVAL, "cfrb_blueprint_strategy: null argument");
+  CK(cudaSetDevice(b->device));
+  CK(cudaMemcpy(compact, b->table.p, b->table.n * sizeof(double), cudaMemcpyDeviceToHost));
+  return CFRB_OK;
+}
+
+int cfrb_blueprint_destroy(cfrb_blueprint* b) {
+  if (!b) return CFRB_OK;
+  cudaSetDevice(b->device);
+  delete b;
+  return CFRB_OK;
+}
+
+}  // extern "C"
+
 // ============================================================================================ head-to-head matches
 struct cfrb_match {
-  cfrb_handle* h[2] = {nullptr, nullptr};
+  cfrb_handle* h[2] = {nullptr, nullptr};   // null for a blueprint agent (cfrb_match_create3) and for LBR
+  int device = 0;
+  cudaStream_t stream = nullptr;            // the first handle's stream, or own_stream in a match between two blueprints
+  Stream own_stream;
+  bool live = false;                        // fully created: destroy settles it
   int S = 0, G = 0, T = 0;
   DevBuf<int> game, last_bid, player, hands, ply, round, widx, act, mt_idx, running, left, plies, rounds;
   DevBuf<int> tr_ply, tr_plies, tr_act, tr_rounds;
@@ -3230,6 +3388,7 @@ struct cfrb_match {
   bool per_ply = false;
   DevBuf<int> awidx, sub_lb, sub_player, sub_node, sub_depth, solves_k;
   DevBuf<double> cache[2];
+  DevBuf<int> bp_node;                // [2][S] blueprint agents' full-tree nodes (cfrb_match_create3)
 };
 
 // Agent slot k of the tables a match, LBR or agent kernel reads: the handle's wave beliefs and the table it acts with, the
@@ -3244,6 +3403,29 @@ static void act_slot(cfrb::MatchTabs<real>& t, int k, const cfrb_handle* h, Wave
 
 // The kernels of a round around the agents' solves: the scan that packs the round's subgames (begin), or the walk that plays it.
 static int match_kernels(cfrb_match* m, bool begin, cudaStream_t st) {
+  if (m->lbr && !m->h[0]) {   // LBR against a blueprint: nothing to solve, the whole round is the walk
+    if (!begin) cfrb::lbr_launch_blueprint(m->ldev, st);
+    CK(cudaGetLastError());
+    return CFRB_OK;
+  }
+  if (m->per_ply && (!m->h[0] || !m->h[1])) {   // a blueprint in one seat or both: only a handle's slot of the tables is read
+    auto launch = [&](const auto& t) {
+      if (begin) cfrb::ply_launch_begin(m->dev, t, st);
+      else cfrb::ply_launch_advance(m->dev, t, m->dev.cache[0] || m->dev.cache[1], st);
+    };
+    const int k = m->h[0] ? 0 : 1;
+    if (!m->h[k]) {
+      launch(cfrb::MatchTabs<double>{});
+    } else {
+      with_state(m->h[k], [&](auto& s) {
+        cfrb::MatchTabs<typename std::decay_t<decltype(s)>::real> t{};
+        act_slot(t, k, m->h[k], s, m->dev.policy[k] == CFRB_MATCH_SAMPLED);
+        launch(t);
+      });
+    }
+    CK(cudaGetLastError());
+    return CFRB_OK;
+  }
   cfrb_handle* a = m->h[0];
   with_state(a, m->lbr ? a : m->h[1], [&](auto& sa, auto& sb) {
     cfrb::MatchTabs<typename std::decay_t<decltype(sa)>::real> t{};
@@ -3269,7 +3451,7 @@ static int match_kernels(cfrb_match* m, bool begin, cudaStream_t st) {
 
 // Everything enqueued has finished: each handle's current wave becomes the match's last wave (its size lives on the device).
 static int match_settle(cfrb_match* m) {
-  CK(cudaSetDevice(m->h[0]->cfg.device));
+  CK(cudaSetDevice(m->device));
   CK(cudaDeviceSynchronize());
   for (cfrb_handle* h : m->h) {
     if (!h) continue;
@@ -3286,7 +3468,7 @@ extern "C" {
 int cfrb_match_destroy(cfrb_match* m) {
   if (!m) return CFRB_OK;
   int rc = CFRB_OK;
-  if (m->h[0]) {
+  if (m->live) {
     rc = match_settle(m);
     for (cfrb_handle* h : m->h)
       if (h) h->in_match = false;
@@ -3375,15 +3557,17 @@ static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int3
   CK(cudaStreamSynchronize(a->own_stream));
   m->h[0] = a; m->h[1] = b;
   a->in_match = b->in_match = true;
+  m->live = true;
   return CFRB_OK;
 }
 
-// Slots, games, streams and trace buffers of a match played with agent a's game (the part shared by both kinds of match).
-static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed) {
-  const auto& ca = a->cfg;
-  CK(cudaSetDevice(ca.device));
+// Slots, games, streams and trace buffers of a match of game g on `device` (the part shared by every kind of match).
+static int match_alloc_game(cfrb_match* m, int device, const cfrb::GameShape& g, int max_depth, const unsigned char* matches,
+                            int32_t n_slots, int32_t n_games, uint64_t seed) {
+  CK(cudaSetDevice(device));
   CK(cudaDeviceSynchronize());
-  const int S = n_slots, G = n_games, H = a->g.H, A = a->g.A, T = std::min(G, (int)CFRB_MATCH_TRACE_GAMES);
+  m->device = device;
+  const int S = n_slots, G = n_games, H = g.H, A = g.A, T = std::min(G, (int)CFRB_MATCH_TRACE_GAMES);
   m->S = S; m->G = G; m->T = T;
   for (auto* p : {&m->game, &m->last_bid, &m->player, &m->ply, &m->round, &m->widx, &m->mt_idx}) CK(p->alloc(S));
   CK(m->hands.alloc((size_t)2 * S)); CK(m->act.alloc((size_t)2 * S));
@@ -3400,14 +3584,24 @@ static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n
   CK(cudaMallocHost((void**)m->pin_left.put(), sizeof(int)));
   CK(cudaEventCreateWithFlags(m->ev_left.put(), cudaEventDisableTiming));
   cfrb::MatchDev& d = m->dev;
-  d.S = S; d.G = G; d.A = A; d.H = H; d.F = a->g.F; d.max_depth = ca.max_depth; d.seed = seed;
+  d.S = S; d.G = G; d.A = A; d.H = H; d.F = g.F; d.max_depth = max_depth; d.seed = seed;
   d.game = m->game.p; d.last_bid = m->last_bid.p; d.player = m->player.p; d.hands = m->hands.p; d.ply = m->ply.p; d.round = m->round.p;
   d.widx = m->widx.p; d.act = m->act.p; d.bel = m->bel.p; d.mt = m->mt.p; d.mt_idx = m->mt_idx.p; d.running = m->running.p;
   d.left = m->left.p;
   d.payoff = m->payoff.p; d.plies = m->plies.p; d.rounds = m->rounds.p;
   d.trace_games = T; d.tr_ply = m->tr_ply.p; d.tr_prob = m->tr_prob.p; d.tr_plies = m->tr_plies.p; d.tr_act = m->tr_act.p;
   d.tr_bel = m->tr_bel.p; d.tr_rounds = m->tr_rounds.p;
-  d.tmpl = a->d_tmpl.p; d.child_begin = a->d_child_begin.p; d.nchild = a->d_nchild.p; d.matches = a->d_matches.p;
+  d.matches = matches;
+  return CFRB_OK;
+}
+
+// match_alloc_game with agent a's game, stream and tree templates.
+static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed) {
+  const int rc = match_alloc_game(m, a->cfg.device, a->g, a->cfg.max_depth, a->d_matches.p, n_slots, n_games, seed);
+  if (rc) return rc;
+  m->stream = a->own_stream;
+  cfrb::MatchDev& d = m->dev;
+  d.tmpl = a->d_tmpl.p; d.child_begin = a->d_child_begin.p; d.nchild = a->d_nchild.p;
   d.level_begin = a->d_level_begin.p;
   d.table_stride = a->table_stride;
   return CFRB_OK;
@@ -3426,7 +3620,7 @@ static int ply_alloc(cfrb_match* m, const char* who) {
     d.sub_player[k] = m->sub_player.p + (size_t)k * S; d.sub_node[k] = m->sub_node.p + (size_t)k * S;
     d.sub_depth[k] = m->sub_depth.p + (size_t)k * S; d.solves[k] = m->solves_k.p + (size_t)k * G;
     d.cache[k] = nullptr;
-    if (d.policy[k] != CFRB_MATCH_EVERY_NODE) {
+    if (d.policy[k] == CFRB_MATCH_AVERAGE || d.policy[k] == CFRB_MATCH_SAMPLED) {
       CK(m->cache[k].alloc((size_t)S * d.table_stride));
       d.cache[k] = m->cache[k].p;
     }
@@ -3467,6 +3661,106 @@ int cfrb_match_create2(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t 
   return CFRB_OK;
 }
 
+// A per-ply match with a blueprint in one seat or both (cfrb_match_create3).  A handle agent plays as in cfrb_match_create2.
+static int match_create3_impl(cfrb_match* m, const cfrb_match_agent* ag, int32_t n_slots, int32_t n_games, uint64_t seed) {
+  const std::string w = "cfrb_match_create3";
+  int device = -1;
+  cfrb::GameShape g;
+  for (int k = 0; k < 2; ++k) {
+    const cfrb_match_agent& x = ag[k];
+    const std::string who = w + ": agent " + (k ? "b" : "a");
+    if (x.bp) {
+      if (x.h) return fail(CFRB_EINVAL, who + " has both a handle and a blueprint");
+    } else {
+      if (x.h->sp.ready) return fail(CFRB_EINVAL, who + "'s handle has a live self-play session");
+      if (x.h->in_match) return fail(CFRB_EINVAL, who + "'s handle already plays in a live match");
+      if (x.h->cfg.max_subgames < n_slots)
+        return fail(CFRB_EINVAL, who + "'s handle capacity (max_subgames " + std::to_string(x.h->cfg.max_subgames) +
+                                     ") is smaller than n_slots " + std::to_string(n_slots));
+    }
+    const int dev = x.bp ? x.bp->device : x.h->cfg.device;
+    const cfrb::GameShape gk = x.bp ? x.bp->g : x.h->g;
+    if (k == 0) { device = dev; g = gk; continue; }
+    if (gk.D != g.D || gk.F != g.F)
+      return fail(CFRB_EINVAL, w + ": the agents play different games (" + std::to_string(g.D) + "x" + std::to_string(g.F) + "f vs " +
+                                   std::to_string(gk.D) + "x" + std::to_string(gk.F) + "f)");
+    if (dev != device) return fail(CFRB_EINVAL, w + ": the agents are on different devices");
+  }
+  const int k = ag[0].h ? 0 : ag[1].h ? 1 : -1;   // the handle agent, if any
+  if (k >= 0 && ag[k].policy != CFRB_MATCH_EVERY_NODE) {   // its strategy cache, refused before anything is allocated
+    const int64_t bytes = cache_bytes(ag[k].h->table_stride, n_slots, ag[k].policy, CFRB_MATCH_EVERY_NODE);
+    CK(cudaSetDevice(device));
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    int64_t avail = (int64_t)free_b;
+    if (ag[k].h->to_leaf_free_cap > 0) avail = std::min(avail, ag[k].h->to_leaf_free_cap);
+    if (bytes > avail)
+      return fail(CFRB_ENOMEM, w + ": the to-leaf agent's strategy cache needs " + std::to_string(bytes) + " bytes of device memory, " +
+                                   std::to_string(avail) + " free (fewer n_slots need less)");
+  }
+  int rc;
+  if (k >= 0) {
+    rc = match_alloc(m, ag[k].h, n_slots, n_games, seed);
+  } else {
+    const cfrb_blueprint* b = ag[0].bp;
+    rc = match_alloc_game(m, device, b->g, 1 << 30, b->matches.p, n_slots, n_games, seed);
+    if (!rc) {
+      CK(cudaStreamCreateWithFlags(m->own_stream.put(), cudaStreamNonBlocking));
+      m->stream = m->own_stream;
+    }
+  }
+  if (rc) return rc;
+  cfrb::MatchDev& d = m->dev;
+  m->per_ply = true;
+  CK(m->bp_node.alloc((size_t)2 * n_slots));
+  for (int j = 0; j < 2; ++j) {
+    const cfrb_match_agent& x = ag[j];
+    if (x.bp) {
+      d.policy[j] = cfrb::kPlyBlueprint; d.iters[j] = 0;
+      d.bp[j] = x.bp->table.p; d.bp_child_begin[j] = x.bp->child_begin.p; d.bp_node[j] = m->bp_node.p + (size_t)j * n_slots;
+      continue;
+    }
+    cfrb_handle* h = x.h;
+    d.policy[j] = x.policy; d.iters[j] = h->cfg.num_iters;
+    d.wave[j] = h->d_wave.p; d.sg_tmpl[j] = h->d_sg_tmpl.p; d.sg_player[j] = h->d_sg_player.p; d.sg_row_off[j] = h->d_sg_row_off.p;
+    d.sg_act[j] = h->d_sg_act.p; d.steps[j] = h->d_steps.p;
+  }
+  if ((rc = ply_alloc(m, w.c_str()))) return rc;
+  cfrb::ply_launch_deal(d, m->stream);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(m->stream));
+  for (int j = 0; j < 2; ++j) {
+    m->h[j] = ag[j].h;
+    if (ag[j].h) ag[j].h->in_match = true;
+  }
+  m->live = true;
+  return CFRB_OK;
+}
+
+int cfrb_match_create3(const cfrb_match_agent* a, const cfrb_match_agent* b, int32_t n_slots, int32_t n_games, uint64_t seed,
+                       cfrb_match** out) {
+  const std::string w = "cfrb_match_create3";
+  if (!out || !a || !b) return fail(CFRB_EINVAL, w + ": null argument");
+  *out = nullptr;
+  for (const cfrb_match_agent* x : {a, b})
+    if (!x->h && !x->bp) return fail(CFRB_EINVAL, w + ": an agent needs a handle or a blueprint");
+  if (!a->bp && !b->bp) return cfrb_match_create2(a->h, b->h, n_slots, n_games, seed, a->policy, b->policy, out);
+  for (const cfrb_match_agent* x : {a, b})
+    if (x->h && !valid_policy(x->policy))
+      return fail(CFRB_EINVAL, w + ": bad policy (" + std::to_string(x->policy) + "): CFRB_MATCH_AVERAGE, CFRB_MATCH_SAMPLED or "
+                                   "CFRB_MATCH_EVERY_NODE");
+  if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
+  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
+  auto m = std::make_unique<cfrb_match>();
+  const cfrb_match_agent ag[2] = {*a, *b};
+  const int rc = match_create3_impl(m.get(), ag, n_slots, n_games, seed);
+  if (rc != CFRB_OK) return rc;
+  *out = m.release();
+  return CFRB_OK;
+}
+
+static int lbr_alloc(cfrb_match* m);
+
 static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy,
                            const char* who) {
   const std::string w(who);
@@ -3486,12 +3780,29 @@ static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32
                                  ") must hold the A - 1 = " + std::to_string(A - 1) + " what-if subgames of one LBR decision");
   int rc = match_alloc(m, a, n_slots, n_games, seed);
   if (rc) return rc;
-  const int S = n_slots, G = n_games, H = a->g.H, T = m->T;
   cfrb::MatchDev& d = m->dev;
   d.sampled = 0;
   d.iters[0] = a->cfg.num_iters;
   d.wave[0] = a->d_wave.p; d.sg_tmpl[0] = a->d_sg_tmpl.p; d.sg_player[0] = a->d_sg_player.p; d.sg_row_off[0] = a->d_sg_row_off.p;
   d.sg_act[0] = a->d_sg_act.p; d.steps[0] = a->d_steps.p;
+  if ((rc = lbr_alloc(m))) return rc;
+  cfrb::LbrDev& l = m->ldev;
+  l.K = a->cfg.max_subgames;
+  l.every_node = policy == CFRB_MATCH_EVERY_NODE;
+  cfrb::match_launch_deal(d, a->own_stream);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(a->own_stream));
+  l.m = d;
+  m->lbr = true;
+  m->h[0] = a;
+  a->in_match = true;
+  m->live = true;
+  return CFRB_OK;
+}
+
+// LBR's per-slot state, counters and traces, for a match whose slots match_alloc_game has set up.
+static int lbr_alloc(cfrb_match* m) {
+  const int S = m->S, G = m->G, H = m->dev.H, A = m->dev.A, T = m->T;
   CK(m->nsg.alloc(S)); CK(m->pend.alloc(S)); CK(m->rr.alloc(1)); CK(m->deferred.alloc(1));
   CK(m->solves_g.alloc(G)); CK(m->whatif_g.alloc(G));
   CK(m->sigx.alloc((size_t)S * A * H));
@@ -3507,17 +3818,30 @@ static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32
   const std::vector<double> nan((size_t)T * A * A, std::numeric_limits<double>::quiet_NaN());
   CK(cudaMemcpy(m->tr_val.p, nan.data(), nan.size() * sizeof(double), cudaMemcpyHostToDevice));
   cfrb::LbrDev& l = m->ldev;
-  l.K = a->cfg.max_subgames;
-  l.every_node = policy == CFRB_MATCH_EVERY_NODE;
   l.nsg = m->nsg.p; l.pend = m->pend.p; l.sigx = m->sigx.p; l.rr = m->rr.p; l.deferred = m->deferred.p;
   l.solves = m->solves_g.p; l.whatif = m->whatif_g.p; l.tr_val = m->tr_val.p; l.tr_beta = m->tr_beta.p;
-  cfrb::match_launch_deal(d, a->own_stream);
+  return CFRB_OK;
+}
+
+// LBR against a blueprint: no handle, a stream of the match's own, one game per slot and round (lbr_blueprint_kernel).
+static int lbr_blueprint_impl(cfrb_match* m, cfrb_blueprint* bp, int32_t n_slots, int32_t n_games, uint64_t seed) {
+  const std::string w = "cfrb_match_create_lbr_blueprint";
+  if (!bp) return fail(CFRB_EINVAL, w + ": null blueprint");
+  if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
+  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
+  int rc = match_alloc_game(m, bp->device, bp->g, 1 << 30, bp->matches.p, n_slots, n_games, seed);
+  if (rc) return rc;
+  CK(cudaStreamCreateWithFlags(m->own_stream.put(), cudaStreamNonBlocking));
+  m->stream = m->own_stream;
+  if ((rc = lbr_alloc(m))) return rc;
+  cfrb::LbrDev& l = m->ldev;
+  l.bp = bp->table.p; l.bp_child_begin = bp->child_begin.p;
+  cfrb::match_launch_deal(m->dev, m->stream);
   CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(a->own_stream));
-  l.m = d;
+  CK(cudaStreamSynchronize(m->stream));
+  l.m = m->dev;
   m->lbr = true;
-  m->h[0] = a;
-  a->in_match = true;
+  m->live = true;
   return CFRB_OK;
 }
 
@@ -3538,6 +3862,16 @@ int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, 
 
 int cfrb_match_create_lbr2(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out) {
   return lbr_create(agent, n_slots, n_games, seed, policy, out, "cfrb_match_create_lbr2");
+}
+
+int cfrb_match_create_lbr_blueprint(cfrb_blueprint* bp, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out) {
+  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create_lbr_blueprint: null argument");
+  *out = nullptr;
+  auto m = std::make_unique<cfrb_match>();
+  const int rc = lbr_blueprint_impl(m.get(), bp, n_slots, n_games, seed);
+  if (rc != CFRB_OK) return rc;
+  *out = m.release();
+  return CFRB_OK;
 }
 
 int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* beliefs) {
@@ -3572,12 +3906,13 @@ int cfrb_match_lbr_counts(cfrb_match* m, int64_t* whatif_solves, int64_t* deferr
 
 int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
   if (!m || max_rounds < 1) return fail(CFRB_EINVAL, "cfrb_match_run: bad argument");
-  CK(cudaSetDevice(m->h[0]->cfg.device));
+  CK(cudaSetDevice(m->device));
   if (m->ev_recorded) {
     CK(cudaEventSynchronize(m->ev_left));
     if (*m->pin_left == 0) return 0;
   }
-  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->h[0]->own_stream;
+  cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : m->stream;
+  cfrb_handle* counter = m->h[0] ? m->h[0] : m->h[1];   // kernel launches are counted on the first handle (none: no count)
   for (int r = 0; r < max_rounds; ++r) {
     int rc = match_kernels(m, true, st);
     if (rc) return rc;
@@ -3586,7 +3921,7 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
       if (h && (rc = solve_device_wave(h, m->lbr ? h->cfg.max_subgames : m->S, false, false, st))) return rc;
     CK(cudaMemsetAsync(m->left.p, 0, sizeof(int), st));
     if ((rc = match_kernels(m, false, st))) return rc;
-    m->h[0]->launches += m->per_ply && (m->dev.cache[0] || m->dev.cache[1]) ? 4 : 3;
+    if (counter) counter->launches += m->per_ply && (m->dev.cache[0] || m->dev.cache[1]) ? 4 : 3;
   }
   CK(cudaMemcpyAsync(m->pin_left, m->left.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   CK(cudaEventRecord(m->ev_left, st));
@@ -4015,7 +4350,10 @@ int cfrb_comm_reduce_sum(cfrb_comm* c, float* dev_buf, size_t n, int32_t root) {
 
 // ============================================================================================ an agent against external players
 struct cfrb_agent {
-  cfrb_handle* h = nullptr;
+  cfrb_handle* h = nullptr;           // null for a blueprint agent (cfrb_agent_create_blueprint)
+  int device = 0;
+  cudaStream_t stream = nullptr;      // the handle's stream, or own_stream for a blueprint agent
+  Stream own_stream;
   int T = 0, sampled = 0;
   uint64_t games_started = 0;
   DevBuf<int> seat, hand, last_bid, player, ply, root_lb, root_player, node, depth, act, status, subgames, mt_idx;
@@ -4050,8 +4388,8 @@ static int agent_check_ids(cfrb_agent* a, const char* who, int n, const int32_t*
 
 // Copies the call's ids to the device and returns the per-call view of the state.
 static int agent_call(cfrb_agent* a, int n, const int32_t* ids, cfrb::AgentDev* d) {
-  CK(cudaSetDevice(a->h->cfg.device));
-  CK(cudaMemcpyAsync(a->ids.p, ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, a->h->own_stream));
+  CK(cudaSetDevice(a->device));
+  CK(cudaMemcpyAsync(a->ids.p, ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, a->stream));
   *d = a->dev;
   d->n = n;
   return CFRB_OK;
@@ -4059,6 +4397,7 @@ static int agent_call(cfrb_agent* a, int n, const int32_t* ids, cfrb::AgentDev* 
 
 // One wave: every listed table at an unsolved root, packed in list order, solved and captured into the cache.
 static int agent_solve(cfrb_agent* a, const cfrb::AgentDev& d, int n, const int32_t* ids) {
+  if (!a->h) return CFRB_OK;          // a blueprint solves nothing
   int n_solve = 0;
   for (int i = 0; i < n; ++i) n_solve += a->need_solve[ids[i]];
   if (n_solve == 0) return CFRB_OK;
@@ -4090,6 +4429,8 @@ static int agent_solve(cfrb_agent* a, const cfrb::AgentDev& d, int n, const int3
   return CFRB_OK;
 }
 
+static int agent_alloc(cfrb_agent* a, int device, const cfrb::GameShape& g, int32_t n_tables, int stride);
+
 static int agent_create_impl(cfrb_agent* a, cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t policy) {
   if (!h) return fail(CFRB_EINVAL, "cfrb_agent_create: null handle");
   if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_SAMPLED && policy != CFRB_MATCH_EVERY_NODE)
@@ -4101,11 +4442,30 @@ static int agent_create_impl(cfrb_agent* a, cfrb_handle* h, int32_t n_tables, ui
                                  ") is smaller than n_tables " + std::to_string(n_tables) + " (one wave solves every listed table)");
   if (h->sp.ready) return fail(CFRB_EINVAL, "cfrb_agent_create: the handle has a live self-play session");
   if (h->in_match) return fail(CFRB_EINVAL, "cfrb_agent_create: the handle already plays in a live match or agent");
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaDeviceSynchronize());
-  const int T = n_tables, H = h->g.H, A = h->g.A;
-  a->T = T;
+  int rc = agent_alloc(a, h->cfg.device, h->g, n_tables, h->table_stride);
+  if (rc) return rc;
   a->sampled = policy == CFRB_MATCH_SAMPLED;
+  cfrb::AgentDev& d = a->dev;
+  d.max_depth = h->cfg.max_depth; d.sampled = a->sampled; d.iters = h->cfg.num_iters; d.seed = seed;
+  d.every_node = policy == CFRB_MATCH_EVERY_NODE;
+  d.stride = h->table_stride;
+  d.tmpl = h->d_tmpl.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p; d.level_begin = h->d_level_begin.p;
+  d.table_stride = h->table_stride;
+  d.wave = h->d_wave.p; d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_row_off = h->d_sg_row_off.p;
+  d.sg_act = h->d_sg_act.p; d.steps = h->d_steps.p;
+  a->h = h;
+  a->stream = h->own_stream;
+  h->in_match = true;
+  return CFRB_OK;
+}
+
+// An agent's per-table state for game g on `device`, with a strategy cache of `stride` doubles per table (0: one shared table).
+static int agent_alloc(cfrb_agent* a, int device, const cfrb::GameShape& g, int32_t n_tables, int stride) {
+  CK(cudaSetDevice(device));
+  CK(cudaDeviceSynchronize());
+  a->device = device;
+  const int T = n_tables, H = g.H, A = g.A;
+  a->T = T;
   for (auto* b : {&a->seat, &a->hand, &a->last_bid, &a->player, &a->ply, &a->root_lb, &a->root_player, &a->node, &a->depth, &a->act,
                   &a->status, &a->subgames, &a->mt_idx, &a->ids, &a->io, &a->hands, &a->widx, &a->flags}) {
     CK(b->alloc(T));
@@ -4114,28 +4474,37 @@ static int agent_create_impl(cfrb_agent* a, cfrb_handle* h, int32_t n_tables, ui
   CK(a->keys.alloc(T));
   CK(a->root_bel.alloc((size_t)T * 2 * H)); CK(a->bel.alloc((size_t)T * 2 * H));
   CK(cudaMemset(a->root_bel.p, 0, (size_t)T * 2 * H * sizeof(double)));
-  CK(a->cache.alloc((size_t)T * h->table_stride)); CK(a->probs.alloc((size_t)T * A)); CK(a->pol.alloc((size_t)T * H * A));
+  if (stride > 0) CK(a->cache.alloc((size_t)T * stride));
+  CK(a->probs.alloc((size_t)T * A)); CK(a->pol.alloc((size_t)T * H * A));
   CK(a->mt.alloc((size_t)624 * T));
   CK(cudaEventCreate(a->ev[0].put())); CK(cudaEventCreate(a->ev[1].put()));
   a->running.assign(T, 0); a->need_solve.assign(T, 0);
   a->h_seat.assign(T, 0); a->h_last_bid.assign(T, -1); a->h_player.assign(T, 0);
   a->stamp.assign(T, 0);
   cfrb::AgentDev& d = a->dev;
-  d.T = T; d.A = A; d.H = H; d.max_depth = h->cfg.max_depth; d.sampled = a->sampled; d.iters = h->cfg.num_iters; d.seed = seed;
-  d.every_node = policy == CFRB_MATCH_EVERY_NODE;
+  d.T = T; d.A = A; d.H = H;
   d.seat = a->seat.p; d.hand = a->hand.p; d.last_bid = a->last_bid.p; d.player = a->player.p; d.ply = a->ply.p;
   d.root_lb = a->root_lb.p; d.root_player = a->root_player.p; d.node = a->node.p; d.depth = a->depth.p;
   d.act = a->act.p; d.status = a->status.p; d.subgames = a->subgames.p;
   d.root_bel = a->root_bel.p; d.bel = a->bel.p; d.mt = a->mt.p; d.mt_idx = a->mt_idx.p;
-  d.cache = a->cache.p; d.stride = h->table_stride;
+  d.cache = a->cache.p;
   d.ids = a->ids.p; d.io = a->io.p; d.hands = a->hands.p; d.keys = a->keys.p; d.widx = a->widx.p; d.probs = a->probs.p;
   d.flags = a->flags.p; d.pol = a->pol.p;
-  d.tmpl = h->d_tmpl.p; d.child_begin = h->d_child_begin.p; d.nchild = h->d_nchild.p; d.level_begin = h->d_level_begin.p;
-  d.table_stride = h->table_stride;
-  d.wave = h->d_wave.p; d.sg_tmpl = h->d_sg_tmpl.p; d.sg_player = h->d_sg_player.p; d.sg_row_off = h->d_sg_row_off.p;
-  d.sg_act = h->d_sg_act.p; d.steps = h->d_steps.p;
-  a->h = h;
-  h->in_match = true;
+  return CFRB_OK;
+}
+
+// A blueprint agent: the table is its cache for every table (stride 0), read at full-tree nodes; it never reaches a pseudo-leaf.
+static int agent_blueprint_impl(cfrb_agent* a, const cfrb_blueprint* bp, int32_t n_tables, uint64_t seed) {
+  if (!bp) return fail(CFRB_EINVAL, "cfrb_agent_create_blueprint: null blueprint");
+  if (n_tables < 1) return fail(CFRB_EINVAL, "cfrb_agent_create_blueprint: n_tables must be >= 1");
+  int rc = agent_alloc(a, bp->device, bp->g, n_tables, 0);
+  if (rc) return rc;
+  CK(cudaStreamCreateWithFlags(a->own_stream.put(), cudaStreamNonBlocking));
+  a->stream = a->own_stream;
+  cfrb::AgentDev& d = a->dev;
+  d.max_depth = std::numeric_limits<int>::max(); d.seed = seed;
+  d.cache = bp->table.p; d.stride = 0;
+  d.bp_child_begin = bp->child_begin.p;
   return CFRB_OK;
 }
 
@@ -4151,12 +4520,22 @@ int cfrb_agent_create(cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t p
   return CFRB_OK;
 }
 
+int cfrb_agent_create_blueprint(cfrb_blueprint* bp, int32_t n_tables, uint64_t seed, cfrb_agent** out) {
+  if (!out) return fail(CFRB_EINVAL, "cfrb_agent_create_blueprint: null argument");
+  *out = nullptr;
+  auto a = std::make_unique<cfrb_agent>();
+  const int rc = agent_blueprint_impl(a.get(), bp, n_tables, seed);
+  if (rc != CFRB_OK) return rc;
+  *out = a.release();
+  return CFRB_OK;
+}
+
 int cfrb_agent_destroy(cfrb_agent* a) {
   if (!a) return CFRB_OK;
   int rc = CFRB_OK;
-  if (cudaSetDevice(a->h->cfg.device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess)
+  if (cudaSetDevice(a->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess)
     rc = fail(CFRB_ECUDA, std::string("cfrb_agent_destroy: ") + cudaGetErrorString(cudaGetLastError()));
-  a->h->in_match = false;
+  if (a->h) a->h->in_match = false;
   delete a;
   return rc;
 }
@@ -4177,7 +4556,7 @@ int cfrb_agent_new_games(cfrb_agent* a, int32_t n, const int32_t* ids, const int
   for (int i = 0; i < n; ++i) k[i] = keys ? keys[i] : a->games_started + (uint64_t)i;
   cfrb::AgentDev d;
   if ((rc = agent_call(a, n, ids, &d))) return rc;
-  cudaStream_t st = a->h->own_stream;
+  cudaStream_t st = a->stream;
   CK(cudaMemcpyAsync(a->io.p, seats, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(a->hands.p, hands, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(a->keys.p, k.data(), (size_t)n * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
@@ -4214,13 +4593,13 @@ int cfrb_agent_step(cfrb_agent* a, int32_t n, const int32_t* ids, int32_t* actio
   }
   cfrb::AgentDev d;
   if ((rc = agent_call(a, n, ids, &d))) return rc;
-  cudaStream_t st = a->h->own_stream;
+  cudaStream_t st = a->stream;
   CK(cudaMemcpyAsync(a->io.p, actions, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
   if ((rc = agent_solve(a, d, n, ids))) return rc;
   if (!probs) d.probs = nullptr;
   cfrb::agent_launch_step(d, st);
   CK(cudaGetLastError());
-  a->h->launches += 1;
+  if (a->h) a->h->launches += 1;
   std::vector<int> flags(n);
   CK(cudaMemcpyAsync(actions, a->io.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(flags.data(), a->flags.p, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -4246,11 +4625,11 @@ int cfrb_agent_policy(cfrb_agent* a, int32_t n, const int32_t* ids, double* out)
   if (rc) return rc;
   cfrb::AgentDev d;
   if ((rc = agent_call(a, n, ids, &d))) return rc;
-  cudaStream_t st = a->h->own_stream;
+  cudaStream_t st = a->stream;
   if ((rc = agent_solve(a, d, n, ids))) return rc;
   cfrb::agent_launch_policy(d, st);
   CK(cudaGetLastError());
-  a->h->launches += 1;
+  if (a->h) a->h->launches += 1;
   CK(cudaMemcpyAsync(out, a->pol.p, (size_t)n * d.H * d.A * sizeof(double), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return CFRB_OK;
@@ -4264,8 +4643,8 @@ int cfrb_agent_state(cfrb_agent* a, int32_t n, const int32_t* ids, int32_t* last
   if (!ids) return fail(CFRB_EINVAL, std::string(who) + ": null argument");
   int rc = agent_check_ids(a, who, n, ids, false);
   if (rc) return rc;
-  CK(cudaSetDevice(a->h->cfg.device));
-  CK(cudaStreamSynchronize(a->h->own_stream));
+  CK(cudaSetDevice(a->device));
+  CK(cudaStreamSynchronize(a->stream));
   const int T = a->T, H2 = 2 * a->dev.H;
   auto gather = [&](const DevBuf<int>& src, int32_t* dst) -> int {
     if (!dst) return CFRB_OK;

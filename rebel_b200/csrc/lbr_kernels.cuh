@@ -32,6 +32,12 @@
 // The agent moving first solves at the game root and acts.  A slot still asks for 1 subgame (phase 1, root) or m (phase 2) a
 // round, so lbr_scan and its admission serve both walks unchanged.
 //
+// Against a blueprint (cfrb_match_create_lbr_blueprint) nothing is solved: sigma is the blueprint's table everywhere, so
+//   lbr_blueprint plays a slot's whole game in one round (no scan, no begin, no wave): the agent acts from its row at the slot's
+//                 full-tree node, LBR's beta is updated with that row, and LBR values its actions from the rows at the children
+// in the order and arithmetic of lbr_advance; a blueprint holding an AVERAGE or EVERY_NODE agent's walked policy gives that
+// agent's LBR games bit for bit.
+//
 // LBR draws no random numbers, so the agent's draws consume the match's (seed, g) streams exactly as in a match.  Compiled into
 // the -fmad=false translation unit: every sum runs in the order stated, in fp64, without contraction.
 #pragma once
@@ -323,6 +329,84 @@ __global__ void __launch_bounds__(128) lbr_advance_kernel(LbrDev p, MatchTabs<re
     return;
   }
   match_settle<match_start>(q, s, g, prev_bid, caller, ply, round + 1);   // the agent is agent 0: its payoff
+}
+
+// One thread per slot: the slot's game to its end against the blueprint p.bp, then match_settle (its next game waits a round).
+__global__ void __launch_bounds__(128) lbr_blueprint_kernel(LbrDev p) {
+  const MatchDev& q = p.m;
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= q.S) return;
+  const int g = q.game[s];
+  if (g < 0) return;
+  const int H = q.H, A = q.A, F = q.F;
+  const int me = g & 1;                              // the agent sits in seat 0 in even games
+  const int hand_a = q.hands[2 * s + me], hand_l = q.hands[2 * s + (me ^ 1)];
+  const double* __restrict__ bp = p.bp;
+  const int* __restrict__ child_begin = p.bp_child_begin;
+  SpRng rng{q.mt + s, q.S, q.mt_idx[s]};
+  double* beta = q.bel + (size_t)s * 4 * H + 2 * H;  // LBR's belief over the agent's hand (the agent keeps none)
+  const bool traced = g < q.trace_games;
+  auto is_true = [&](int bid, int h) {
+    const int f = bid % F;
+    return (int)q.matches[hand_l * F + f] + (int)q.matches[h * F + f] >= 1 + bid / F;
+  };
+  int lb = -1, actor = 0, node = 0, ply = 0, prev_bid = -1, caller = 0;
+  for (;;) {
+    const int lo = lb < 0 ? 0 : lb + 1, nc = lb < 0 ? A - 1 : A - 1 - lb, cb = child_begin[node];
+    const double* row = bp + (size_t)(cb - 1) * H;   // row[j * H + hand]: the agent's strategy at this node
+    int a;
+    if (actor == me) {
+      const int j = sp_discrete(rng, nc, [&](int i) { return row[(size_t)i * H + hand_a]; });
+      a = lo + j;
+      if (traced && ply < A) {
+        int* rec = q.tr_ply + ((size_t)g * A + ply) * 6;
+        rec[0] = 0; rec[1] = lb; rec[2] = actor; rec[3] = hand_a; rec[4] = a; rec[5] = 0;
+        q.tr_prob[(size_t)g * A + ply] = row[(size_t)j * H + hand_a];
+      }
+      for (int h = 0; h < H; ++h) beta[h] *= row[(size_t)j * H + h];
+      double sum = 0;
+      for (int h = 0; h < H; ++h) sum += beta[h];
+      for (int h = 0; h < H; ++h) beta[h] /= sum;
+    } else {                                         // lbr_advance's decide, sigma(child(a)) from the table
+      double* tv = traced && ply < A ? p.tr_val + ((size_t)g * A + ply) * A : nullptr;
+      if (tv) for (int h = 0; h < H; ++h) p.tr_beta[((size_t)g * A + ply) * H + h] = beta[h];
+      int best = -1;
+      double bv = 0;
+      for (int r = lo; r <= A - 2; ++r) {
+        const int cb2 = child_begin[cb + r - lo], nc2 = A - 1 - r;
+        const double* row2 = bp + (size_t)(cb2 - 1) * H;
+        double v = 0;
+        for (int h = 0; h < H; ++h) {
+          const double ua = is_true(r, h) ? 1.0 : -1.0;
+          double inner = 0;
+          for (int i = 0; i < nc2; ++i) {            // bids r + 1 .. A - 1, the liar call last
+            const int a2 = r + 1 + i;
+            const double u = a2 == A - 1 ? ua : (is_true(a2, h) ? -1.0 : 1.0);
+            inner += row2[(size_t)i * H + h] * u;
+          }
+          v += beta[h] * inner;
+        }
+        if (tv) tv[r] = v;
+        if (best < 0 || v > bv) { best = r; bv = v; }
+      }
+      if (lb >= 0) {
+        double v = 0;
+        for (int h = 0; h < H; ++h) v += beta[h] * (is_true(lb, h) ? -1.0 : 1.0);
+        if (tv) tv[A - 1] = v;
+        if (best < 0 || v > bv) { best = A - 1; bv = v; }
+      }
+      a = best;
+      if (traced && ply < A) {
+        int* rec = q.tr_ply + ((size_t)g * A + ply) * 6;
+        rec[0] = 1; rec[1] = lb; rec[2] = actor; rec[3] = hand_l; rec[4] = a; rec[5] = 0;
+        q.tr_prob[(size_t)g * A + ply] = 1.0;
+      }
+    }
+    prev_bid = lb; caller = actor;
+    node = cb + a - lo; lb = a; actor ^= 1; ++ply;
+    if (a == A - 1) break;
+  }
+  match_settle<match_start>(q, s, g, prev_bid, caller, ply, 1);
 }
 
 }  // namespace cfrb

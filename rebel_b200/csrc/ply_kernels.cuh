@@ -10,6 +10,11 @@
 //                      the acting strategy of that solve (normalised CFR average, FP average or act_iteration snapshot) copied
 //                      into a per-slot fp64 cache right after it (the handle's tables are rebuilt every round), beliefs
 //                      multiplied unnormalised inside the subgame and both of its rows eps-normalised at its pseudo-leaf.
+//   blueprint agent    a fixed full-tree table (cfrb_blueprint, cfrb_match_create3): it never solves and keeps no beliefs; each
+//                      slot holds the full-tree node its game stands at (0 at the game root, child_begin[node] + j after action j),
+//                      and the agent acts with bp[(child_begin[node] + j - 1) * H + hand].  Its trace act_iteration is -2 on
+//                      every ply and its traced beliefs stay uniform.  A match between two blueprints has no handle and no
+//                      templates: scan and begin only pack empty waves and write the trace.
 //
 //   ply_scan      one CTA: per agent, the wave index of every running slot where it solves and the packed value-net row offsets
 //   ply_begin     per slot: each solving agent's subgame descriptor (and, sampled, its act_iteration), the trace of the ply's beliefs
@@ -41,13 +46,15 @@ __device__ __forceinline__ void en_update_row(double* row, int H, Sig sig) {
 
 // Does agent k solve at slot s this round?  An every-node agent at every node, a to-leaf one when it has no solved subgame there.
 __device__ __forceinline__ bool ply_solves(const MatchDev& p, int k, int s) {
-  return p.game[s] >= 0 && (p.policy[k] == kPlyEveryNode || p.sub_node[k][s] < 0);
+  return p.game[s] >= 0 && p.policy[k] != kPlyBlueprint && (p.policy[k] == kPlyEveryNode || p.sub_node[k][s] < 0);
 }
 
-// Game g in slot s (match_start), neither agent holding a subgame.
+// Game g in slot s (match_start), neither agent holding a subgame, a blueprint agent at the full tree's root.
 __device__ void ply_start(const MatchDev& p, int s, int g) {
   match_start(p, s, g);
   p.sub_node[0][s] = p.sub_node[1][s] = -1;
+  for (int k = 0; k < 2; ++k)
+    if (p.bp_node[k]) p.bp_node[k][s] = 0;
 }
 
 // Per agent: the wave index of every slot it solves (slot order) and the exclusive prefix sum of their pseudo-leaf counts; one CTA.
@@ -58,9 +65,8 @@ __global__ void __launch_bounds__(1024) ply_scan_kernel(MatchDev p) {
   int v[5] = {0, 0, 0, 0, 0};                        // agent 0 slots, rows; agent 1 slots, rows; running slots
   for (int s = b; s < e; ++s) {
     if (p.game[s] < 0) continue;
-    const int L = p.tmpl[p.last_bid[s] + 1].L;
     for (int k = 0; k < 2; ++k)
-      if (ply_solves(p, k, s)) { v[2 * k] += 1; v[2 * k + 1] += L; }
+      if (ply_solves(p, k, s)) { v[2 * k] += 1; v[2 * k + 1] += p.tmpl[p.last_bid[s] + 1].L; }
     v[4] += 1;
   }
   int x[5] = {v[0], v[1], v[2], v[3], v[4]};        // inclusive sums; v stays for the exclusive offsets
@@ -68,17 +74,17 @@ __global__ void __launch_bounds__(1024) ply_scan_kernel(MatchDev p) {
   int w[2], off[2];
   for (int k = 0; k < 2; ++k) { w[k] = x[2 * k] - v[2 * k]; off[k] = x[2 * k + 1] - v[2 * k + 1]; }
   for (int s = b; s < e; ++s) {
-    const int L = p.game[s] >= 0 ? p.tmpl[p.last_bid[s] + 1].L : 0;
     for (int k = 0; k < 2; ++k) {
       if (!ply_solves(p, k, s)) { p.awidx[k][s] = -1; continue; }
       p.awidx[k][s] = w[k];
       p.sg_row_off[k][w[k]] = off[k];
       ++w[k];
-      off[k] += L;
+      off[k] += p.tmpl[p.last_bid[s] + 1].L;
     }
   }
   if (t == 1023) {
-    for (int k = 0; k < 2; ++k) { p.wave[k][0] = x[2 * k]; p.wave[k][1] = x[2 * k + 1]; }
+    for (int k = 0; k < 2; ++k)
+      if (p.wave[k]) { p.wave[k][0] = x[2 * k]; p.wave[k][1] = x[2 * k + 1]; }   // a blueprint has no wave
     *p.running = x[4];
   }
 }
@@ -144,14 +150,19 @@ __global__ void __launch_bounds__(128) ply_advance_kernel(MatchDev p, MatchTabs<
   const int agent = actor ^ (g & 1);                 // agent A (0) sits in seat 0 in even games
   const int hand = p.hands[2 * s + actor];
   const int lo = lb < 0 ? 0 : lb + 1;
-  const int nc = p.nchild[p.tmpl[lb + 1].node_off];  // children of this public node (the root of a subgame rooted here)
+  // children of this public node (the root of a subgame rooted here; bids lo .. A - 1, no liar call at the game root)
+  const int nc = p.tmpl ? p.nchild[p.tmpl[lb + 1].node_off] : lb < 0 ? A - 1 : A - 1 - lb;
   // the edges of this node in each agent's strategy: an every-node agent's root row in this round's table (row j = edge j), a
-  // to-leaf agent's node in its cache
+  // to-leaf agent's node in its cache, a blueprint's node in its table
   const real* T[2] = {nullptr, nullptr};
   const double* c[2] = {nullptr, nullptr};
   bool untouched[2] = {false, false};
+  int bcb[2] = {0, 0};                               // a blueprint's first child of its node
   for (int k = 0; k < 2; ++k) {
-    if (p.policy[k] == kPlyEveryNode) {
+    if (p.policy[k] == kPlyBlueprint) {
+      bcb[k] = p.bp_child_begin[k][p.bp_node[k][s]];
+      c[k] = p.bp[k] + (size_t)(bcb[k] - 1) * H;
+    } else if (p.policy[k] == kPlyEveryNode) {
       const int w = p.awidx[k][s];
       T[k] = tb.table[k] + (size_t)w * p.table_stride;
       untouched[k] = tb.normalise[k] && p.steps[k][2 * w + actor] == 0;
@@ -175,6 +186,7 @@ __global__ void __launch_bounds__(128) ply_advance_kernel(MatchDev p, MatchTabs<
   }
   double* bel = p.bel + (size_t)s * 4 * H;           // [agent][player][hand]
   for (int k = 0; k < 2; ++k) {
+    if (p.policy[k] == kPlyBlueprint) { p.bp_node[k][s] = bcb[k] + j; continue; }   // no beliefs to update
     double* bk = bel + (k * 2 + actor) * H;
     if (!c[k]) {
       en_update_row(bk, H, [&](int h) { return sig(k, h, j); });

@@ -25,8 +25,23 @@ class Agent {
     a_.reset(a);
   }
 
-  void close() {   // the agent first: it reads its handle when it is destroyed
+  // A blueprint agent: the compact full-tree table `strategy` [N - 1][H] (its size checked by the caller) uploaded to `device`
+  // with cfrb_blueprint_create's checks plays at every table; it never solves and needs no handle.
+  Agent(int num_dice, int num_faces, const std::vector<double>& strategy, int device, int tables, uint64_t seed) : tables_(tables) {
+    A_ = 1 + 2 * num_dice * num_faces;
+    H_ = 1;
+    for (int i = 0; i < num_dice; ++i) H_ *= num_faces;
+    cfrb_blueprint* b = nullptr;
+    check(cfrb_blueprint_create(device, num_dice, num_faces, strategy.data(), &b), "cfrb_blueprint_create");
+    bp_.reset(b);
+    cfrb_agent* a = nullptr;
+    check(cfrb_agent_create_blueprint(bp_.get(), tables, seed, &a), "cfrb_agent_create_blueprint");
+    a_.reset(a);
+  }
+
+  void close() {   // the agent first: it reads its handle (or blueprint) when it is destroyed
     a_.reset();
+    bp_.reset();
     h_.reset();
   }
 
@@ -83,7 +98,8 @@ class Agent {
  private:
   int tables_ = 0, A_ = 0, H_ = 0;
   HandlePtr h_;
-  AgentPtr a_;   // declared after its handle: released first
+  BlueprintPtr bp_;
+  AgentPtr a_;   // declared after its handle and blueprint: released first
 
   cfrb_agent* live() {
     if (!a_) throw std::runtime_error("Agent: closed");

@@ -27,6 +27,7 @@ using AgentPtr = std::unique_ptr<cfrb_agent, Destroyer<cfrb_agent_destroy>>;
 using RowsPtr = std::unique_ptr<cfrb_rows, Destroyer<cfrb_rows_destroy>>;
 using CommPtr = std::unique_ptr<cfrb_comm, Destroyer<cfrb_comm_destroy>>;
 using FullGamePtr = std::unique_ptr<cfrb_full_game, Destroyer<cfrb_full_game_destroy>>;
+using BlueprintPtr = std::unique_ptr<cfrb_blueprint, Destroyer<cfrb_blueprint_destroy>>;
 
 // fp32 device memory of cfrb_dev_alloc, which cfrb_dev_free releases on the device it came from.
 struct DevFree {

@@ -804,16 +804,38 @@ int match_policy(const std::string& policy, const char* who) {
   throw std::runtime_error(std::string(who) + ": policy must be 'sampled', 'average' or 'every_node' (got '" + policy + "')");
 }
 
+// A blueprint table argument as fp64 [N - 1][H] of cfg's game: a game above 23 actions and any other shape are refused.
+std::vector<double> blueprint_of(py::object table, int num_dice, int num_faces, const char* who) {
+  const int64_t bytes = cfrb_blueprint_bytes(num_dice, num_faces);
+  if (bytes < 0) throw std::runtime_error(std::string(who) + ": " + cfrb_last_error());
+  const int64_t A = 1 + 2 * (int64_t)num_dice * num_faces;
+  int64_t H = 1;
+  for (int i = 0; i < num_dice; ++i) H *= num_faces;
+  auto t = py::module::import("torch").attr("as_tensor")(table).cast<torch::Tensor>().to(torch::kCPU, torch::kFloat64).contiguous();
+  if (t.dim() != 2 || t.size(0) != ((int64_t)1 << A) - 2 || t.size(1) != H)
+    throw std::runtime_error(std::string(who) + ": a blueprint of " + std::to_string(num_dice) + "x" + std::to_string(num_faces) +
+                             "f is a [" + std::to_string(((int64_t)1 << A) - 2) + ", " + std::to_string(H) + "] table");
+  return std::vector<double>(t.data_ptr<double>(), t.data_ptr<double>() + t.numel());
+}
+
 py::dict play_match_py(const RecursiveSolvingParams& cfg_a, const RecursiveSolvingParams& cfg_b, int device, int games, uint64_t seed,
                        const std::string& policy, py::object flat_weights_a, py::object flat_weights_b, int concurrent_games,
-                       py::object policy_b) {
+                       py::object policy_b, py::object blueprint_a, py::object blueprint_b) {
   const int pa = match_policy(policy, "play_match");
   const int pb = policy_b.is_none() ? pa : match_policy(policy_b.cast<std::string>(), "play_match");
+  if (!blueprint_a.is_none() && !flat_weights_a.is_none())
+    throw std::runtime_error("play_match: blueprint_a replaces agent A, which then has no net: flat_weights_a must be None");
+  if (!blueprint_b.is_none() && !flat_weights_b.is_none())
+    throw std::runtime_error("play_match: blueprint_b replaces agent B, which then has no net: flat_weights_b must be None");
   const std::vector<float> wa = flat_of(flat_weights_a), wb = flat_of(flat_weights_b);
+  std::vector<double> ta, tb;
+  if (!blueprint_a.is_none()) ta = blueprint_of(blueprint_a, cfg_a.num_dice, cfg_a.num_faces, "play_match");
+  if (!blueprint_b.is_none()) tb = blueprint_of(blueprint_b, cfg_b.num_dice, cfg_b.num_faces, "play_match");
   MatchResult r;
   {
     py::gil_scoped_release nogil;
-    r = play_match(cfg_a, cfg_b, device, games, seed, pa, wa, wb, concurrent_games, pb);
+    r = play_match(cfg_a, cfg_b, device, games, seed, pa, wa, wb, concurrent_games, pb, blueprint_a.is_none() ? nullptr : &ta,
+                   blueprint_b.is_none() ? nullptr : &tb);
   }
   py::dict d = stats_dict(r.payoff);
   auto p = torch::empty({(int64_t)games}, torch::kFloat32);
@@ -826,16 +848,20 @@ py::dict play_match_py(const RecursiveSolvingParams& cfg_a, const RecursiveSolvi
 }
 
 py::dict play_lbr_py(const RecursiveSolvingParams& cfg, int device, int games, uint64_t seed, py::object flat_weights, int concurrent_games,
-                     int max_subgames, const std::string& policy) {
+                     int max_subgames, const std::string& policy, py::object blueprint) {
   const int pol = match_policy(policy, "play_lbr");
   if (pol == CFRB_MATCH_SAMPLED)
     throw std::runtime_error("play_lbr: policy must be 'average' or 'every_node' (LBR against the sampled policy bounds nothing: "
                              "it would respond to a drawn snapshot the agent's opponent cannot see)");
+  if (!blueprint.is_none() && !flat_weights.is_none())
+    throw std::runtime_error("play_lbr: a blueprint replaces the agent, which then has no net: flat_weights must be None");
   const std::vector<float> w = flat_of(flat_weights);
+  std::vector<double> table;
+  if (!blueprint.is_none()) table = blueprint_of(blueprint, cfg.num_dice, cfg.num_faces, "play_lbr");
   LbrResult r;
   {
     py::gil_scoped_release nogil;
-    r = play_lbr(cfg, device, games, seed, w, concurrent_games, max_subgames, pol);
+    r = play_lbr(cfg, device, games, seed, w, concurrent_games, max_subgames, pol, blueprint.is_none() ? nullptr : &table);
   }
   std::vector<float> lbr(r.payoff.size());
   for (size_t i = 0; i < lbr.size(); ++i) lbr[i] = -r.payoff[i];
@@ -849,7 +875,7 @@ py::dict play_lbr_py(const RecursiveSolvingParams& cfg, int device, int games, u
   std::copy(r.plies.begin(), r.plies.end(), pl.data_ptr<int32_t>());
   d["payoff_lbr"] = p; d["plies"] = pl; d["solves"] = r.solves; d["whatif_solves"] = r.whatif_solves;
   d["deferred_slot_rounds"] = r.deferred_slot_rounds; d["max_subgames"] = r.capacity;
-  d["subgame_iters"] = r.subgame_iters; d["seconds"] = r.seconds; d["policy"] = policy;
+  d["subgame_iters"] = r.subgame_iters; d["seconds"] = r.seconds; d["policy"] = blueprint.is_none() ? policy : "blueprint";
   return d;
 }
 
@@ -892,14 +918,16 @@ torch::Tensor strategy_recursive(const RecursiveSolvingParams& cfg, int device, 
 // The exploitability of a policy walked and best-responded on the device by `walk` (cfrb_to_leaf_exploitability or
 // cfrb_recursive_exploitability): no dense strategy, so games up to A = 23 (2x5f, 5x2f, 1x10f, 1x11f) are accepted.
 using DeviceWalk = int (*)(cfrb_handle*, double*, int64_t*, int64_t*, double*);
+// return_strategy adds the walked policy as the compact table [N - 1, H] (cfrb_to_leaf_strategy), a blueprint's input.
 py::dict exploitability_walk(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity, const char* who,
-                             DeviceWalk walk, const char* walk_name) {
+                             DeviceWalk walk, const char* walk_name, bool return_strategy) {
   refuse_above_walk_limit(cfg, who);
   const std::vector<float> w = flat_of(flat_weights);
   std::array<double, 2> br{};
   double secs[2] = {0, 0}, total = 0;
   int64_t subgames = 0, iters = 0;
-  int N = 0;
+  int N = 0, H = 0;
+  std::vector<double> strategy;
   {
     py::gil_scoped_release nogil;
     const auto t0 = std::chrono::steady_clock::now();
@@ -907,26 +935,34 @@ py::dict exploitability_walk(const RecursiveSolvingParams& cfg, int device, py::
     if (!w.empty()) check(cfrb_set_weights(h.get(), w.data(), w.size(), 1), "cfrb_set_weights");
     check(walk(h.get(), br.data(), &subgames, &iters, secs), walk_name);
     N = cfrb_full_tree_nodes(h.get());
+    H = cfrb_num_hands(h.get());
     total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    if (return_strategy) {
+      strategy.resize((size_t)(N - 1) * H);
+      check(cfrb_to_leaf_strategy(h.get(), strategy.data()), "cfrb_to_leaf_strategy");
+    }
   }
   py::dict d;
   d["exploitability"] = (br[0] + br[1]) / 2.;
   d["br"] = std::vector<double>{br[0], br[1]};
   d["num_nodes"] = N; d["subgames"] = subgames; d["subgame_iters"] = iters;
   d["seconds"] = total; d["walk_seconds"] = secs[0]; d["br_seconds"] = secs[1];
+  if (return_strategy) d["strategy"] = f64_tensor(strategy, {(int64_t)N - 1, (int64_t)H});
   return d;
 }
 
 // The exploitability of compute_strategy_recursive_to_leaf's policy (cfrb_to_leaf_exploitability).
-py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity) {
+py::dict exploitability_to_leaf(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity,
+                                bool return_strategy) {
   return exploitability_walk(cfg, device, flat_weights, wave_capacity, "exploitability_to_leaf", cfrb_to_leaf_exploitability,
-                             "cfrb_to_leaf_exploitability");
+                             "cfrb_to_leaf_exploitability", return_strategy);
 }
 
 // The exploitability of compute_strategy_recursive's every-node policy (cfrb_recursive_exploitability).
-py::dict exploitability_recursive(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity) {
+py::dict exploitability_recursive(const RecursiveSolvingParams& cfg, int device, py::object flat_weights, int wave_capacity,
+                                  bool return_strategy) {
   return exploitability_walk(cfg, device, flat_weights, wave_capacity, "exploitability_recursive", cfrb_recursive_exploitability,
-                             "cfrb_recursive_exploitability");
+                             "cfrb_recursive_exploitability", return_strategy);
 }
 
 // recursive_eval's sampled evaluation (RecursiveEvaluator::run, recursive_eval.cc:331-369) walked on the device
@@ -1038,6 +1074,12 @@ std::shared_ptr<Agent> make_agent(const RecursiveSolvingParams& cfg, int device,
   const std::vector<float> w = flat_of(flat_weights);
   py::gil_scoped_release nogil;
   return std::make_shared<Agent>(cfg, device, tables, pol, seed, w);
+}
+
+std::shared_ptr<Agent> make_blueprint_agent(int num_dice, int num_faces, py::object strategy, int device, int tables, uint64_t seed) {
+  const std::vector<double> s = blueprint_of(strategy, num_dice, num_faces, "Agent.from_blueprint");
+  py::gil_scoped_release nogil;
+  return std::make_shared<Agent>(num_dice, num_faces, s, device, tables, seed);
 }
 
 void agent_new_games(Agent& a, py::object ids, py::object seats, py::object hands, py::object keys) {
@@ -1244,31 +1286,37 @@ PYBIND11_MODULE(rela, m) {
         "above regret_depth and of the rest (report_regrets' summary).");
   m.def("play_match", &play_match_py, py::arg("cfg_a"), py::arg("cfg_b"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
         py::arg("policy") = "sampled", py::arg("flat_weights_a") = py::none(), py::arg("flat_weights_b") = py::none(),
-        py::arg("concurrent_games") = 8192, py::arg("policy_b") = py::none(),
+        py::arg("concurrent_games") = 8192, py::arg("policy_b") = py::none(), py::arg("blueprint_a") = py::none(),
+        py::arg("blueprint_b") = py::none(),
         "rebel_b200 extension: `games` head-to-head games (seat-swapped pairs) of agent A (cfg_a + net A) against agent B on the GPU, "
         "each re-solving subgames along the path played: A with `policy`, B with policy_b (None: the same).  'average' and "
         "'sampled' are the recursive to-leaf policies; 'every_node' re-solves at every decision (compute_strategy_recursive).  "
         "dict: payoff_a [games] (to A), plies [games], mean, stderr (over pairs), seat_means [2] (A in seat 0 / seat 1), solves, "
-        "solves_a, solves_b (each agent's), subgame_iters, seconds.");
+        "solves_a, solves_b (each agent's), subgame_iters, seconds.  blueprint_a / blueprint_b (a compact full-tree table "
+        "[N - 1, H], e.g. FullGame.strategy() or exploitability_to_leaf(return_strategy=True)['strategy']) replaces that agent by "
+        "a blueprint: it acts with the table's row at every node, never solves, and takes no net (refused with one) and no solver "
+        "settings from its cfg.");
   m.def("play_lbr", &play_lbr_py, py::arg("cfg"), py::arg("device"), py::arg("games"), py::arg("seed") = 0,
         py::arg("flat_weights") = py::none(), py::arg("concurrent_games") = 8192, py::arg("max_subgames") = 0,
-        py::arg("policy") = "average",
+        py::arg("policy") = "average", py::arg("blueprint") = py::none(),
         "rebel_b200 extension: local best response against one agent (cfg + net) on the GPU: `games` games (seat-swapped pairs), "
         "concurrent_games at a time, at most max_subgames subgames solved per round (0: 2 x concurrent_games, at least A - 1).  "
         "The agent plays `policy`: 'average' (the recursive to-leaf policy) or 'every_node' (compute_strategy_recursive: a "
         "subgame solved at every decision; each LBR decision with a legal raise then costs 1 + m solves); 'sampled' is refused.  "
         "LBR's payoff is a lower bound on the agent's exploitability.  dict: payoff_lbr [games], plies [games], mean, stderr "
         "(over pairs), seat_means [2] (LBR in seat 0 / seat 1), solves, whatif_solves, deferred_slot_rounds, max_subgames, "
-        "subgame_iters, seconds, policy.");
+        "subgame_iters, seconds, policy.  blueprint (a compact full-tree table [N - 1, H]) plays LBR against that fixed "
+        "strategy instead: no solves, no net (refused with one), policy 'blueprint'.");
   m.def("exploitability_to_leaf", &exploitability_to_leaf, py::arg("cfg"), py::arg("device") = 0, py::arg("flat_weights") = py::none(),
-        py::arg("wave_capacity") = 16384,
+        py::arg("wave_capacity") = 16384, py::arg("return_strategy") = false,
         "rebel_b200 extension: exploitability of compute_strategy_recursive_to_leaf's policy (every subgame solved for num_iters "
         "iterations, get_strategy; the policy play_match's 'average' plays and play_lbr bounds), the subgames walked level by level "
         "in waves of wave_capacity and the best response taken on the GPU without a dense strategy (games with at most 23 actions "
         "whose need fits the free device memory).  dict: exploitability = (br0 + br1) / 2, br [2], num_nodes, subgames, "
-        "subgame_iters, seconds, walk_seconds, br_seconds.");
+        "subgame_iters, seconds, walk_seconds, br_seconds; return_strategy adds strategy, the walked policy as the compact "
+        "table [N - 1, H] a blueprint plays (Agent.from_blueprint, play_match's blueprint_a / blueprint_b, play_lbr's blueprint).");
   m.def("exploitability_recursive", &exploitability_recursive, py::arg("cfg"), py::arg("device") = 0,
-        py::arg("flat_weights") = py::none(), py::arg("wave_capacity") = 16384,
+        py::arg("flat_weights") = py::none(), py::arg("wave_capacity") = 16384, py::arg("return_strategy") = false,
         "rebel_b200 extension: exploitability of compute_strategy_recursive's every-node policy (a subgame solved for num_iters "
         "iterations at every non-terminal node, acting with its root's average strategy; what compute_exploitability_with_net "
         "measures), the 2^(A-1) subgames walked depth by depth in waves of wave_capacity and the best response taken on the GPU "
@@ -1297,6 +1345,12 @@ PYBIND11_MODULE(rela, m) {
       "node and acts with the subgame root's average strategy; deals and seats belong to the caller.")
       .def(py::init(&make_agent), py::arg("cfg"), py::arg("device") = 0, py::arg("tables") = 8192, py::arg("policy") = "sampled",
            py::arg("seed") = 0, py::arg("flat_weights") = py::none())
+      .def_static("from_blueprint", &make_blueprint_agent, py::arg("num_dice"), py::arg("num_faces"), py::arg("strategy"),
+                  py::arg("device") = 0, py::arg("tables") = 8192, py::arg("seed") = 0,
+                  "an agent that plays a fixed full-tree strategy: the compact table [N - 1, H] (entry [child - 1, hand]) of "
+                  "FullGame.strategy(), exploitability_to_leaf(return_strategy=True) or exploitability_recursive(...).  It never "
+                  "solves; its draws are the same (seed, key) streams as any Agent's, so the table of an 'average' agent's walked "
+                  "policy answers as that agent")
       .def("new_games", &agent_new_games, py::arg("ids"), py::arg("seats"), py::arg("hands"), py::arg("keys") = py::none(),
            "start a game at each listed table: the agent in seat seats[i] (0 moves first) with hand hands[i]; keys[i] keys the "
            "game's random stream (None: the number of games started before, in list order)")

@@ -9,7 +9,11 @@ the wave solver supports, including those whose full game tree the exploitabilit
 Prints a summary and one tagged line `H2H {"net_a": ..., "net_b": ..., "games": ..., "mean": ..., "stderr": ..., "ci95": [lo, hi],
 "seat0": ..., "seat1": ...}` whose text after the tag is JSON.  mean is agent A's expected payoff per game (+1 win, -1 loss);
 seat0 / seat1 are A's mean payoffs in seat 0 (even games) and seat 1 (odd games).  When --policy_b is given or either agent plays
-every_node, the line also has "policy_a" and "policy_b"."""
+every_node, the line also has "policy_a" and "policy_b".
+
+--blueprint_a PATH / --blueprint_b PATH replace that agent by a blueprint file (`solve_game --save`, `exploitability --save`): a
+fixed full-tree strategy that never solves.  That agent's --net_* and --random_net_seed_* are refused with it; the line names it
+"blueprint:PATH" and gives its policy as "blueprint"."""
 import argparse
 import json
 
@@ -44,7 +48,27 @@ def build_parser():
                     "4 wgmma on two-CTA clusters with mode 3's GELU (also games too large for modes 2 and 3; the fp32 net where it does not fit)")
     ap.add_argument("--concurrent_games", type=int, default=8192)
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--blueprint_a", type=str, default=None, metavar="PATH", help="agent A is this blueprint file (no net, no solves)")
+    ap.add_argument("--blueprint_b", type=str, default=None, metavar="PATH", help="agent B is this blueprint file (no net, no solves)")
     return ap
+
+
+def blueprint_conflicts(args):
+    """The flags given together with a blueprint that would configure the agent it replaces (empty: none)."""
+    bad = []
+    for k in ("a", "b"):
+        if getattr(args, "blueprint_" + k) is not None:
+            bad += [f"--{f}_{k}" for f in ("net", "random_net_seed") if getattr(args, f"{f}_{k}") is not None]
+    return bad
+
+
+def load_blueprint_arg(path, args, who):
+    """A blueprint file of the command's game; anything else ends the command with a message."""
+    from rebel_b200.blueprint import load_blueprint
+    try:
+        return load_blueprint(path, args.num_dice, args.num_faces)
+    except (ValueError, OSError) as e:
+        raise SystemExit(f"{who}: {e}")
 
 
 def agent_weights(num_dice, num_faces, net, random_seed):
@@ -94,7 +118,13 @@ def parse_h2h(line):
 
 
 def main(argv=None):
-    args = build_parser().parse_args(argv)
+    ap = build_parser()
+    args = ap.parse_args(argv)
+    bad = blueprint_conflicts(args)
+    if bad:
+        ap.error(f"{', '.join(bad)} configure an agent that a blueprint replaces")
+    bp = {k: load_blueprint_arg(getattr(args, "blueprint_" + k), args, "head_to_head")
+          for k in ("a", "b") if getattr(args, "blueprint_" + k) is not None}
     import rebel_b200.rela as rela
     wa = agent_weights(args.num_dice, args.num_faces, args.net_a, args.random_net_seed_a)
     wb = agent_weights(args.num_dice, args.num_faces, args.net_b, args.random_net_seed_b)
@@ -102,19 +132,26 @@ def main(argv=None):
     cfg_a = agent_params(rela, args, wa, args.subgame_iters, args.cfr)
     cfg_b = agent_params(rela, args, wb, args.subgame_iters_b or args.subgame_iters, cfr_b)
     policy_b = args.policy_b or args.policy
+    kw = {f"blueprint_{k}": torch.from_numpy(v["strategy"]) for k, v in bp.items()}
     r = rela.play_match(cfg_a, cfg_b, args.device, args.games, seed=args.seed, policy=args.policy, flat_weights_a=wa,
-                        flat_weights_b=wb, concurrent_games=args.concurrent_games, policy_b=policy_b)
+                        flat_weights_b=wb, concurrent_games=args.concurrent_games, policy_b=policy_b, **kw)
     na, nb = agent_name(args.net_a, args.random_net_seed_a), agent_name(args.net_b, args.random_net_seed_b)
+    if bp:
+        from rebel_b200.blueprint import blueprint_name
+        na = blueprint_name(args.blueprint_a) if "a" in bp else na
+        nb = blueprint_name(args.blueprint_b) if "b" in bp else nb
     mean, se = r["mean"], r["stderr"]
-    named = args.policy_b is not None or "every_node" in (args.policy, policy_b)
-    pol = f"{args.policy} policy" if policy_b == args.policy else f"A {args.policy}, B {policy_b} policy"
+    named = args.policy_b is not None or "every_node" in (args.policy, policy_b) or bool(bp)
+    pol_a = "blueprint" if "a" in bp else args.policy
+    pol_b = "blueprint" if "b" in bp else policy_b
+    pol = f"{pol_a} policy" if pol_b == pol_a else f"A {pol_a}, B {pol_b} policy"
     print(f"{args.num_dice}x{args.num_faces}f, {args.games} games ({pol}, depth {args.mdp_depth}): "
           f"A = {na} vs B = {nb}", flush=True)
     print(f"  A's payoff per game {mean:+.4f} +- {se:.4f} (95% CI [{mean - 1.96 * se:+.4f}, {mean + 1.96 * se:+.4f}]); "
           f"in seat 0 {r['seat_means'][0]:+.4f}, in seat 1 {r['seat_means'][1]:+.4f}", flush=True)
     print(f"  {r['solves']} subgame solves (A {r['solves_a']}, B {r['solves_b']}), {r['subgame_iters']} subgame iterations, {float(r['plies'].float().mean()):.2f} plies "
           f"per game, {r['seconds']:.2f} s ({args.games / r['seconds']:.1f} games/s)", flush=True)
-    print(h2h_line(na, nb, args.games, mean, se, r["seat_means"], (args.policy, policy_b) if named else None), flush=True)
+    print(h2h_line(na, nb, args.games, mean, se, r["seat_means"], (pol_a, pol_b) if named else None), flush=True)
     return r
 
 

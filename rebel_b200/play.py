@@ -9,7 +9,9 @@ Both hands are dealt on the host from --seed; seats alternate between games (you
 face F is wild: it counts for every face.  Enter a bid as `<quantity> <face>` (a bid must beat the last one: a higher quantity, or
 the same quantity of a higher face) or `liar` to call the last bid.  At the liar call the bidder wins if both hands together hold
 at least `quantity` dice showing `face` or the wild face.  The session ends with one tagged line `PLAY {"net": ..., "games": ...,
-"agent_wins": ..., "human_wins": ..., "agent_mean": ...}` whose text after the tag is JSON."""
+"agent_wins": ..., "human_wins": ..., "agent_mean": ...}` whose text after the tag is JSON.  --blueprint PATH plays against a
+blueprint file (`solve_game --save`, `exploitability --save`) instead: a fixed full-tree strategy that never solves (--net is
+refused with it), named "blueprint:PATH"."""
 import argparse
 import json
 import sys
@@ -35,6 +37,7 @@ def build_parser():
     ap.add_argument("--net_mode", type=int, default=None, help="0 zero, 1 fp32 SIMT, 2 wgmma fp16, 3 wgmma fp16 + fast GELU (default 3 with a "
                     "net), 4 wgmma on two-CTA clusters with mode 3's GELU (also games too large for modes 2 and 3; the fp32 net where it does "
                     "not fit)")
+    ap.add_argument("--blueprint", type=str, default=None, metavar="PATH", help="play against this blueprint file (no net, no solves)")
     # agent_params' other settings, at head_to_head's defaults
     ap.set_defaults(no_linear=False, dcfr=None, device=0)
     return ap
@@ -106,18 +109,31 @@ def show(dice):
 
 
 def main(argv=None, stdin=None):
-    args = build_parser().parse_args(argv)
+    ap = build_parser()
+    args = ap.parse_args(argv)
     stdin = stdin or sys.stdin
-    import rebel_b200.rela as rela
     D, F = args.num_dice, args.num_faces
-    w = agent_weights(D, F, args.net, None)
-    cfg = agent_params(rela, args, w, args.subgame_iters, args.cfr)
-    agent = rela.Agent(cfg, device=args.device, tables=1, policy=args.policy, seed=args.seed, flat_weights=w)
+    if args.blueprint is not None:
+        if args.net is not None:
+            ap.error("--net configures the agent that --blueprint replaces")
+        from rebel_b200.blueprint import blueprint_name
+        from rebel_b200.head_to_head import load_blueprint_arg
+        bp = load_blueprint_arg(args.blueprint, args, "play")
+    import rebel_b200.rela as rela
+    if args.blueprint is not None:
+        agent = rela.Agent.from_blueprint(D, F, bp["strategy"], device=args.device, tables=1, seed=args.seed)
+        name = blueprint_name(args.blueprint)
+        print(f"{D}x{F}f against {name} ({bp['source']} blueprint, exploitability {bp['exploitability']:.6f}); face {F} is wild",
+              flush=True)
+    else:
+        w = agent_weights(D, F, args.net, None)
+        cfg = agent_params(rela, args, w, args.subgame_iters, args.cfr)
+        agent = rela.Agent(cfg, device=args.device, tables=1, policy=args.policy, seed=args.seed, flat_weights=w)
+        name = agent_name(args.net, None)
+        print(f"{D}x{F}f against {name} ({args.policy} policy, {args.subgame_iters} iterations, depth {args.mdp_depth}); "
+              f"face {F} is wild", flush=True)
     H, A = agent.num_hands, agent.num_actions
     rng = np.random.RandomState(args.seed)
-    name = agent_name(args.net, None)
-    print(f"{D}x{F}f against {name} ({args.policy} policy, {args.subgame_iters} iterations, depth {args.mdp_depth}); "
-          f"face {F} is wild", flush=True)
     wins = [0, 0]                                     # agent, human
     played = 0
     for g in range(args.games):

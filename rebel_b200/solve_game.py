@@ -7,7 +7,9 @@
 Prints the reference's `Iter=... exploitabilities=(...) sum=...` line at every power of two and at the last iteration, then one
 `SOLVE {...}` JSON line: the game, the solver settings, the final best-response pair and exploitability, the time of the whole
 call, of the iterations and of the best responses, and the device memory the solver took.  Flags follow `recursive_eval`; the
-solver is fictitious play unless --cfr is given, linear unless --no_linear or --dcfr."""
+solver is fictitious play unless --cfr is given, linear unless --no_linear or --dcfr.  --save PATH writes the final average
+strategy as a blueprint file (rebel_b200.blueprint) for `head_to_head --blueprint_a / _b`, `local_br --blueprint` and
+`play --blueprint`, and the SOLVE line adds "saved": PATH."""
 import argparse
 import json
 
@@ -22,6 +24,7 @@ def build_parser():
     ap.add_argument("--optimistic", action="store_true")
     ap.add_argument("--dcfr", type=float, nargs=3, metavar=("ALPHA", "BETA", "GAMMA"), default=None)
     ap.add_argument("--device", type=int, default=0, help="CUDA ordinal")
+    ap.add_argument("--save", type=str, default=None, metavar="PATH", help="write the final average strategy as a blueprint file")
     return ap
 
 
@@ -47,14 +50,19 @@ def main(argv=None):
     r = rela.solve_full_game(cfg, args.device)
     sp = cfg.subgame_params
     br = r["exploitability"][-1].tolist() if len(r["checkpoints"]) else [float("nan")] * 2
-    print("SOLVE " + json.dumps({
+    line = {
         "game": f"{args.num_dice}x{args.num_faces}f", "num_dice": args.num_dice, "num_faces": args.num_faces,
         "num_nodes": r["num_nodes"], "iterations": args.subgame_iters, "solver": "cfr" if args.cfr else "fp",
         "linear": bool(sp.linear_update), "dcfr": list(args.dcfr) if args.dcfr is not None else None, "optimistic": args.optimistic,
         "br": br, "exploitability": (br[0] + br[1]) / 2,
         "seconds": r["seconds"], "solve_seconds": r["solve_seconds"], "br_seconds": r["br_seconds"],
         "peak_device_bytes": r["device_bytes"],
-    }), flush=True)
+    }
+    if args.save:
+        from rebel_b200.blueprint import save_blueprint
+        settings = {k: line[k] for k in ("solver", "iterations", "linear", "dcfr", "optimistic")}
+        line["saved"] = save_blueprint(args.save, args.num_dice, args.num_faces, r["strategy"].numpy(), "solve_game", settings, br)
+    print("SOLVE " + json.dumps(line), flush=True)
     return r
 
 
