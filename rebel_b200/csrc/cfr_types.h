@@ -168,7 +168,7 @@ template <typename real> void sp_launch_finish(const SpDev& p, const real* mu, c
 // after the last iteration of a shared wave: the representative's results to every copy, and every initial-state game's snapshot
 template <typename real> void sp_launch_share(const SpDev& p, const CfrDev<real>& d, cudaStream_t st);
 // Head-to-head matches (match_kernels.cuh): S game slots playing G games between two handles (agent 0 = A, 1 = B).
-// MatchDev::policy of a blueprint agent (no CFRB_MATCH_* value: only cfrb_match_create3 seats one)
+// MatchDev::policy of a blueprint seat (no CFRB_MATCH_* value, so no caller's policy can name it)
 constexpr int kPlyBlueprint = 3;
 struct MatchDev {
   int S, G, A, H, F, max_depth, sampled, iters[2];

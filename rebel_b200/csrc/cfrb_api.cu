@@ -48,6 +48,27 @@ int fail(int code, const std::string& msg) {
                                   std::to_string(__LINE__));                                       \
   } while (0)
 
+// A new T for entry point `who`: *out stays null unless init succeeds, and a T that init leaves half built is freed.
+template <class T, class Init>
+int make_object(T** out, const std::string& who, Init&& init) {
+  if (!out) return fail(CFRB_EINVAL, who + ": null argument");
+  *out = nullptr;
+  auto p = std::make_unique<T>();
+  if (const int rc = init(p.get())) return rc;
+  *out = p.release();
+  return CFRB_OK;
+}
+
+// Free bytes of the current device as an admission sees them: at most `cap` when a test aid set one (cap > 0).  *raw, when
+// given, is the unclipped figure.
+int free_device_bytes(int64_t cap, int64_t* avail, int64_t* raw = nullptr) {
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  if (raw) *raw = (int64_t)free_b;
+  *avail = cap > 0 ? std::min((int64_t)free_b, cap) : (int64_t)free_b;
+  return CFRB_OK;
+}
+
 // Test aid (cfrb_debug_fill_allocations), process-wide: -1 = off, 0..255 = the byte every floating-point DevBuf is filled with
 // when it is allocated.
 int g_fill_byte = -1;
@@ -846,12 +867,7 @@ static int create_impl(const cfrb_config* cfg, cfrb_handle* h) {
 
 int cfrb_create(const cfrb_config* cfg, cfrb_handle** out) {
   if (!cfg || !out) return fail(CFRB_EINVAL, "null argument");
-  *out = nullptr;
-  auto h = std::make_unique<cfrb_handle>();
-  const int rc = create_impl(cfg, h.get());
-  if (rc != CFRB_OK) return rc;
-  *out = h.release();
-  return CFRB_OK;
+  return make_object(out, "cfrb_create", [&](cfrb_handle* h) -> int { return create_impl(cfg, h); });
 }
 
 int cfrb_tc_net_supported(int32_t num_dice, int32_t num_faces, int32_t hidden) {
@@ -1897,10 +1913,8 @@ static int walk_admit(cfrb_handle* h, const char* who, int64_t tree_bytes, int64
   CK(cudaStreamSynchronize(h->own_stream));
   if (release_sampled) h->smp = cfrb_handle::SampledState();
   const int64_t tree = h->br.ready ? 0 : tree_bytes, need = tree + walk_bytes + extra_bytes;
-  size_t free_b = 0, total_b = 0;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  int64_t avail = (int64_t)free_b;
-  if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
+  int64_t avail = 0;
+  if (int rc = free_device_bytes(h->to_leaf_free_cap, &avail)) return rc;
   if (need > avail)
     return fail(CFRB_ENOMEM, w + ": needs " + std::to_string(need) + " bytes of device memory beyond the handle (full tree and "
                              "best-response scratch " + std::to_string(tree) + ", walk " + std::to_string(walk_bytes) + walk_note +
@@ -2487,9 +2501,8 @@ static int full_game_create_impl(const cfrb_config* cfg, cfrb_full_game* fg) {
   fg->fp = cfg->solver == CFRB_SOLVER_FP;
   // refused before anything is allocated: on a shared device an allocation that fails late may starve other processes
   const int64_t need = full_game_bytes(g, fg->fp);
-  size_t free0 = 0, total = 0;
-  CK(cudaMemGetInfo(&free0, &total));
-  const int64_t avail = g_full_game_free_cap > 0 ? std::min<int64_t>((int64_t)free0, g_full_game_free_cap) : (int64_t)free0;
+  int64_t avail = 0, free0 = 0;
+  if (int rc = free_device_bytes(g_full_game_free_cap, &avail, &free0)) return rc;
   if (need > avail)
     return fail(CFRB_ENOMEM, "cfrb_full_game_create: needs " + std::to_string(need) + " bytes of device memory beyond the handle, " +
                                  std::to_string(avail) + " free");
@@ -2498,9 +2511,9 @@ static int full_game_create_impl(const cfrb_config* cfg, cfrb_full_game* fg) {
   int rc = cfrb_create(&c, &fg->h);
   if (rc) return rc;
   cfrb_handle* h = fg->h;
-  size_t free1 = 0;
-  CK(cudaMemGetInfo(&free1, &total));
-  fg->handle_bytes = (int64_t)free0 - (int64_t)free1;
+  int64_t free1 = 0;
+  if ((rc = free_device_bytes(0, &free1))) return rc;
+  fg->handle_bytes = free0 - free1;
   if ((rc = full_tree_setup(h, "cfrb_full_game_create"))) return rc;
   const auto& t = h->br.t;
   const size_t E = (size_t)(t.N - 1) * g.H, NH = (size_t)t.N * g.H;
@@ -2520,20 +2533,16 @@ static int full_game_create_impl(const cfrb_config* cfg, cfrb_full_game* fg) {
   cfrb::full_game_launch_init(d, t.level_begin.data(), t.levels, 8 * h->num_sms, st);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(st));
-  size_t free2 = 0;
-  CK(cudaMemGetInfo(&free2, &total));
-  fg->total_bytes = (int64_t)free0 - (int64_t)free2;
+  int64_t free2 = 0;
+  if ((rc = free_device_bytes(0, &free2))) return rc;
+  fg->total_bytes = free0 - free2;
   return CFRB_OK;
 }
 
 int cfrb_full_game_create(const cfrb_config* cfg, cfrb_full_game** out) {
-  if (!cfg || !out) return fail(CFRB_EINVAL, "cfrb_full_game_create: null argument");
-  *out = nullptr;
-  auto fg = std::make_unique<cfrb_full_game>();
-  const int rc = full_game_create_impl(cfg, fg.get());
-  if (rc) return rc;
-  *out = fg.release();
-  return CFRB_OK;
+  if (!cfg) return fail(CFRB_EINVAL, "cfrb_full_game_create: null argument");
+  return make_object(out, "cfrb_full_game_create",
+                     [&](cfrb_full_game* fg) -> int { return full_game_create_impl(cfg, fg); });
 }
 
 int cfrb_full_game_destroy(cfrb_full_game* g) {
@@ -2566,9 +2575,8 @@ int cfrb_full_game_track_regrets(cfrb_full_game* g) {
   CK(cudaSetDevice(h->cfg.device));
   // refused before anything is allocated, as cfrb_full_game_create is
   const int64_t need = full_game_regret_bytes(h->g);
-  size_t free0 = 0, total = 0;
-  CK(cudaMemGetInfo(&free0, &total));
-  const int64_t avail = g_full_game_free_cap > 0 ? std::min<int64_t>((int64_t)free0, g_full_game_free_cap) : (int64_t)free0;
+  int64_t avail = 0;
+  if (int rc = free_device_bytes(g_full_game_free_cap, &avail)) return rc;
   if (need > avail)
     return fail(CFRB_ENOMEM, "cfrb_full_game_track_regrets: needs " + std::to_string(need) + " bytes of device memory, " +
                                  std::to_string(avail) + " free");
@@ -2753,9 +2761,8 @@ static int fp_forest_create_impl(int32_t num_dice, int32_t num_faces, int32_t de
   const cfrb::GameShape g(num_dice, num_faces);
   // refused before anything is allocated, as cfrb_full_game_create is (and under the same test cap)
   const int64_t need = fp_forest_bytes(g);
-  size_t free0 = 0, total = 0;
-  CK(cudaMemGetInfo(&free0, &total));
-  const int64_t avail = g_full_game_free_cap > 0 ? std::min<int64_t>((int64_t)free0, g_full_game_free_cap) : (int64_t)free0;
+  int64_t avail = 0, free0 = 0;
+  if (int rc = free_device_bytes(g_full_game_free_cap, &avail, &free0)) return rc;
   if (need > avail)
     return fail(CFRB_ENOMEM, "cfrb_fp_forest_create: needs " + std::to_string(need) + " bytes of device memory beyond the handle, " +
                                  std::to_string(avail) + " free");
@@ -2765,20 +2772,15 @@ static int fp_forest_create_impl(int32_t num_dice, int32_t num_faces, int32_t de
   if (int rc = full_game_create_impl(&c, &f->fg)) return rc;
   const size_t cap = (size_t)forest_level_cap(g) * 2 * g.H;
   CK(f->bel.alloc(cap)); CK(f->mu.alloc(cap));
-  size_t free1 = 0;
-  CK(cudaMemGetInfo(&free1, &total));
-  f->total_bytes = (int64_t)free0 - (int64_t)free1;
+  int64_t free1 = 0;
+  if (int rc = free_device_bytes(0, &free1)) return rc;
+  f->total_bytes = free0 - free1;
   return CFRB_OK;
 }
 
 int cfrb_fp_forest_create(int32_t num_dice, int32_t num_faces, int32_t device, cfrb_fp_forest** out) {
-  if (!out) return fail(CFRB_EINVAL, "cfrb_fp_forest_create: null argument");
-  *out = nullptr;
-  auto f = std::make_unique<cfrb_fp_forest>();
-  const int rc = fp_forest_create_impl(num_dice, num_faces, device, f.get());
-  if (rc) return rc;
-  *out = f.release();
-  return CFRB_OK;
+  return make_object(out, "cfrb_fp_forest_create",
+                     [&](cfrb_fp_forest* f) { return fp_forest_create_impl(num_dice, num_faces, device, f); });
 }
 
 int cfrb_fp_forest_destroy(cfrb_fp_forest* f) {
@@ -3259,13 +3261,12 @@ static int blueprint_alloc(cfrb_blueprint* b, int device, const cfrb::GameShape&
 
 // A handle's full-tree strategy (br.strategy) and tree into a new blueprint, device to device.
 static int blueprint_from_br(cfrb_handle* h, cfrb_blueprint** out, const std::string& w) {
-  auto b = std::make_unique<cfrb_blueprint>();
-  int rc = blueprint_alloc(b.get(), h->cfg.device, h->g, h->br.t.child_begin, w);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(b->table.p, h->br.strategy.p, b->table.n * sizeof(double), cudaMemcpyDeviceToDevice, h->own_stream));
-  CK(cudaStreamSynchronize(h->own_stream));
-  *out = b.release();
-  return CFRB_OK;
+  return make_object(out, w, [&](cfrb_blueprint* b) -> int {
+    if (int rc = blueprint_alloc(b, h->cfg.device, h->g, h->br.t.child_begin, w)) return rc;
+    CK(cudaMemcpyAsync(b->table.p, h->br.strategy.p, b->table.n * sizeof(double), cudaMemcpyDeviceToDevice, h->own_stream));
+    CK(cudaStreamSynchronize(h->own_stream));
+    return CFRB_OK;
+  });
 }
 
 extern "C" {
@@ -3311,19 +3312,17 @@ int cfrb_blueprint_check(int32_t num_dice, int32_t num_faces, const double* comp
 
 int cfrb_blueprint_create(int32_t device, int32_t num_dice, int32_t num_faces, const double* compact, cfrb_blueprint** out) {
   const std::string w = "cfrb_blueprint_create";
-  if (!out) return fail(CFRB_EINVAL, w + ": null argument");
-  *out = nullptr;
-  if (!compact) return fail(CFRB_EINVAL, w + ": null table");
-  int rc = blueprint_refuse_game(num_dice, num_faces, w);
-  if (rc) return rc;
-  const cfrb::GameShape g(num_dice, num_faces);
-  const cfrb::TreeTemplate t = cfrb::build_template(g, -1, 1 << 30);
-  if ((rc = blueprint_validate(g, t, compact, w))) return rc;
-  auto b = std::make_unique<cfrb_blueprint>();
-  if ((rc = blueprint_alloc(b.get(), device, g, t.child_begin, w))) return rc;
-  CK(cudaMemcpy(b->table.p, compact, b->table.n * sizeof(double), cudaMemcpyHostToDevice));
-  *out = b.release();
-  return CFRB_OK;
+  return make_object(out, w, [&](cfrb_blueprint* b) -> int {
+    if (!compact) return fail(CFRB_EINVAL, w + ": null table");
+    int rc = blueprint_refuse_game(num_dice, num_faces, w);
+    if (rc) return rc;
+    const cfrb::GameShape g(num_dice, num_faces);
+    const cfrb::TreeTemplate t = cfrb::build_template(g, -1, 1 << 30);
+    if ((rc = blueprint_validate(g, t, compact, w))) return rc;
+    if ((rc = blueprint_alloc(b, device, g, t.child_begin, w))) return rc;
+    CK(cudaMemcpy(b->table.p, compact, b->table.n * sizeof(double), cudaMemcpyHostToDevice));
+    return CFRB_OK;
+  });
 }
 
 int cfrb_blueprint_from_full_game(cfrb_full_game* fg, cfrb_blueprint** out) {
@@ -3361,12 +3360,19 @@ int cfrb_blueprint_destroy(cfrb_blueprint* b) {
 }  // extern "C"
 
 // ============================================================================================ head-to-head matches
+// The walk a match plays: two handles with one to-leaf policy play the to-leaf walk (match_kernels.cuh), any other pair of seats
+// one ply per round (ply_kernels.cuh); local best response plays against a handle or against a blueprint (lbr_kernels.cuh).
+enum class Walk { ToLeaf, PerPly, Lbr, LbrBlueprint };
+
+static bool is_lbr(Walk w) { return w == Walk::Lbr || w == Walk::LbrBlueprint; }
+
 struct cfrb_match {
-  cfrb_handle* h[2] = {nullptr, nullptr};   // null for a blueprint agent (cfrb_match_create3) and for LBR
+  cfrb_handle* h[2] = {nullptr, nullptr};   // each seat's handle: null for a blueprint seat and for LBR's seat (1)
   int device = 0;
-  cudaStream_t stream = nullptr;            // the first handle's stream, or own_stream in a match between two blueprints
+  cudaStream_t stream = nullptr;            // the first handle's stream, or own_stream in a match without a handle
   Stream own_stream;
   bool live = false;                        // fully created: destroy settles it
+  Walk walk = Walk::ToLeaf;
   int S = 0, G = 0, T = 0;
   DevBuf<int> game, last_bid, player, hands, ply, round, widx, act, mt_idx, running, left, plies, rounds;
   DevBuf<int> tr_ply, tr_plies, tr_act, tr_rounds;
@@ -3377,19 +3383,23 @@ struct cfrb_match {
   Pinned<int> pin_left;               // slots with a game left, copied behind the last round of every cfrb_match_run
   Event ev_left;
   bool ev_recorded = false;
-  // local best response (cfrb_match_create_lbr): h[1] is null, agent 1 is LBR
-  bool lbr = false;
+  // local best response: agent 1 is LBR
   cfrb::LbrDev ldev{};
   DevBuf<int> nsg, pend, rr, solves_g, whatif_g;
   DevBuf<double> sigx, tr_val, tr_beta;
   DevBuf<unsigned long long> deferred;
   // per-ply walk (ply_kernels.cuh): a round is one ply; per agent [2][S] wave indices and subgame state, [2][G] solves, and a
   // strategy cache per to-leaf agent
-  bool per_ply = false;
   DevBuf<int> awidx, sub_lb, sub_player, sub_node, sub_depth, solves_k;
   DevBuf<double> cache[2];
-  DevBuf<int> bp_node;                // [2][S] blueprint agents' full-tree nodes (cfrb_match_create3)
+  DevBuf<int> bp_node;                // [2][S] blueprint seats' full-tree nodes
 };
+
+template <typename real>
+static WaveState<real>& wave_state(cfrb_handle* h) {
+  if constexpr (std::is_same_v<real, double>) return h->sd;
+  else return h->sf;
+}
 
 // Agent slot k of the tables a match, LBR or agent kernel reads: the handle's wave beliefs and the table it acts with, the
 // sampled snapshot or its average strategy (avg_table).
@@ -3402,49 +3412,40 @@ static void act_slot(cfrb::MatchTabs<real>& t, int k, const cfrb_handle* h, Wave
 }
 
 // The kernels of a round around the agents' solves: the scan that packs the round's subgames (begin), or the walk that plays it.
+// Only a handle seat's slot of the tables is filled; a SAMPLED seat acts with its snapshot (LBR's agent never does).
 static int match_kernels(cfrb_match* m, bool begin, cudaStream_t st) {
-  if (m->lbr && !m->h[0]) {   // LBR against a blueprint: nothing to solve, the whole round is the walk
-    if (!begin) cfrb::lbr_launch_blueprint(m->ldev, st);
-    CK(cudaGetLastError());
-    return CFRB_OK;
-  }
-  if (m->per_ply && (!m->h[0] || !m->h[1])) {   // a blueprint in one seat or both: only a handle's slot of the tables is read
-    auto launch = [&](const auto& t) {
-      if (begin) cfrb::ply_launch_begin(m->dev, t, st);
-      else cfrb::ply_launch_advance(m->dev, t, m->dev.cache[0] || m->dev.cache[1], st);
-    };
-    const int k = m->h[0] ? 0 : 1;
-    if (!m->h[k]) {
-      launch(cfrb::MatchTabs<double>{});
-    } else {
-      with_state(m->h[k], [&](auto& s) {
-        cfrb::MatchTabs<typename std::decay_t<decltype(s)>::real> t{};
-        act_slot(t, k, m->h[k], s, m->dev.policy[k] == CFRB_MATCH_SAMPLED);
-        launch(t);
-      });
+  const cfrb::MatchDev& d = m->dev;
+  auto launch = [&](const auto& t) {
+    switch (m->walk) {
+      case Walk::ToLeaf:
+        if (begin) cfrb::match_launch_begin(d, t, st);
+        else cfrb::match_launch_advance(d, t, st);
+        break;
+      case Walk::PerPly:
+        if (begin) cfrb::ply_launch_begin(d, t, st);
+        else cfrb::ply_launch_advance(d, t, d.cache[0] || d.cache[1], st);
+        break;
+      case Walk::Lbr:
+        if (begin) cfrb::lbr_launch_begin(m->ldev, t, st);
+        else cfrb::lbr_launch_advance(m->ldev, t, st);
+        break;
+      case Walk::LbrBlueprint:   // nothing to solve: the whole round is the walk
+        if (!begin) cfrb::lbr_launch_blueprint(m->ldev, st);
+        break;
     }
-    CK(cudaGetLastError());
-    return CFRB_OK;
+  };
+  cfrb_handle* first = m->h[0] ? m->h[0] : m->h[1];
+  if (!first) {
+    launch(cfrb::MatchTabs<double>{});
+  } else {
+    with_state(first, [&](auto& s) {
+      using real = typename std::decay_t<decltype(s)>::real;
+      cfrb::MatchTabs<real> t{};
+      for (int k = 0; k < 2; ++k)
+        if (cfrb_handle* h = m->h[k]) act_slot(t, k, h, wave_state<real>(h), d.policy[k] == CFRB_MATCH_SAMPLED);
+      launch(t);
+    });
   }
-  cfrb_handle* a = m->h[0];
-  with_state(a, m->lbr ? a : m->h[1], [&](auto& sa, auto& sb) {
-    cfrb::MatchTabs<typename std::decay_t<decltype(sa)>::real> t{};
-    if (m->lbr) {   // LBR reads the agent's table as in an AVERAGE (or per-ply EVERY_NODE) match
-      act_slot(t, 0, a, sa, false);
-      if (begin) cfrb::lbr_launch_begin(m->ldev, t, st);
-      else cfrb::lbr_launch_advance(m->ldev, t, st);
-    } else if (m->per_ply) {
-      act_slot(t, 0, a, sa, m->dev.policy[0] == CFRB_MATCH_SAMPLED);
-      act_slot(t, 1, m->h[1], sb, m->dev.policy[1] == CFRB_MATCH_SAMPLED);
-      if (begin) cfrb::ply_launch_begin(m->dev, t, st);
-      else cfrb::ply_launch_advance(m->dev, t, m->dev.cache[0] || m->dev.cache[1], st);
-    } else {
-      act_slot(t, 0, a, sa, m->dev.sampled);
-      act_slot(t, 1, m->h[1], sb, m->dev.sampled);
-      if (begin) cfrb::match_launch_begin(m->dev, t, st);
-      else cfrb::match_launch_advance(m->dev, t, st);
-    }
-  });
   CK(cudaGetLastError());
   return CFRB_OK;
 }
@@ -3477,87 +3478,98 @@ int cfrb_match_destroy(cfrb_match* m) {
   return rc;
 }
 
-static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed);
-
-static int ply_alloc(cfrb_match* m, const char* who);
-
 // Bytes of the per-ply walk's strategy caches: n_slots x table_stride fp64 per to-leaf agent (none when both play every-node).
 static int64_t cache_bytes(int64_t table_stride, int32_t n_slots, int32_t policy_a, int32_t policy_b) {
   if (policy_a == policy_b && policy_a != CFRB_MATCH_EVERY_NODE) return 0;   // the to-leaf walk reads its tables in place
   const int n = (policy_a != CFRB_MATCH_EVERY_NODE) + (policy_b != CFRB_MATCH_EVERY_NODE);
   return (int64_t)n * n_slots * table_stride * (int64_t)sizeof(double);
 }
-static int64_t match_cache_bytes(const cfrb_handle* a, int32_t n_slots, int32_t policy_a, int32_t policy_b) {
-  return cache_bytes(a->table_stride, n_slots, policy_a, policy_b);
-}
 
 static bool valid_policy(int32_t p) { return p == CFRB_MATCH_AVERAGE || p == CFRB_MATCH_SAMPLED || p == CFRB_MATCH_EVERY_NODE; }
 
-// A pair of equal to-leaf policies plays the to-leaf walk (match_kernels.cuh); any other pair the per-ply walk (ply_kernels.cuh).
-static int match_create_impl(cfrb_match* m, cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed,
-                             int32_t policy, int32_t policy_b, const char* who) {
-  const std::string w(who);
-  if (!a || !b)
-    return fail(CFRB_EINVAL, w + ": null handle (local best response against one agent is cfrb_match_create_lbr or "
-                                 "cfrb_match_create_lbr2)");
-  if (a == b) return fail(CFRB_EINVAL, w + ": the two agents need two handles (create a second one with the same config)");
-  if (!valid_policy(policy) || !valid_policy(policy_b))
-    return fail(CFRB_EINVAL, w + ": bad policy (" + std::to_string(policy) + ", " + std::to_string(policy_b) +
-                                 "): CFRB_MATCH_AVERAGE, CFRB_MATCH_SAMPLED or CFRB_MATCH_EVERY_NODE");
+// Refusals of a handle that already serves someone: a live self-play session, a live match or agent.  `whose` names the handle.
+static int handle_free(const cfrb_handle* h, const std::string& w, const std::string& whose) {
+  if (h->sp.ready) return fail(CFRB_EINVAL, w + ": " + whose + " has a live self-play session");
+  if (h->in_match) return fail(CFRB_EINVAL, w + ": " + whose + " already plays in a live match or agent");
+  return CFRB_OK;
+}
+
+// The walk of n seats: two seats play a match, one seat is the agent LBR plays against (LBR is seat 1).
+static Walk match_walk(const cfrb_match_agent* seat, int n) {
+  if (n == 1) return seat[0].bp ? Walk::LbrBlueprint : Walk::Lbr;
+  if (seat[0].bp || seat[1].bp || seat[0].policy != seat[1].policy || seat[0].policy == CFRB_MATCH_EVERY_NODE) return Walk::PerPly;
+  return Walk::ToLeaf;
+}
+
+// Every refusal of a match creator `w`, before anything is allocated.  `empty`: the refusal of a seat with neither a handle
+// nor a blueprint, in the terms of the creator's arguments.
+static int match_check(const cfrb_match_agent* seat, int n, Walk walk, int32_t n_slots, int32_t n_games, const std::string& w,
+                       const char* empty) {
+  const bool lbr = is_lbr(walk);
+  auto name = [&](int k) { return std::string(lbr ? "the agent" : k ? "agent b" : "agent a"); };
+  for (int k = 0; k < n; ++k) {
+    if (!seat[k].h && !seat[k].bp) return fail(CFRB_EINVAL, w + ": " + empty);
+    if (seat[k].h && seat[k].bp) return fail(CFRB_EINVAL, w + ": " + name(k) + " has both a handle and a blueprint");
+  }
+  std::string policies;   // of the handle seats (a blueprint's is not read)
+  bool bad = false;
+  for (int k = 0; k < n; ++k) {
+    if (!seat[k].h) continue;
+    const int32_t p = seat[k].policy;
+    if (lbr && p == CFRB_MATCH_SAMPLED)
+      return fail(CFRB_EINVAL, w + ": CFRB_MATCH_SAMPLED is not supported: LBR would have to respond to the expectation over the "
+                                   "agent's act_iteration draws, and the drawn snapshot is information the agent's opponent does not have");
+    bad |= lbr ? p != CFRB_MATCH_AVERAGE && p != CFRB_MATCH_EVERY_NODE : !valid_policy(p);
+    policies += (policies.empty() ? "" : ", ") + std::to_string(p);
+  }
+  if (bad)
+    return fail(CFRB_EINVAL, w + ": bad policy (" + policies + "): " +
+                                 (lbr ? "CFRB_MATCH_AVERAGE or CFRB_MATCH_EVERY_NODE" : "CFRB_MATCH_AVERAGE, CFRB_MATCH_SAMPLED or CFRB_MATCH_EVERY_NODE"));
   if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
   if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
-  const auto &ca = a->cfg, &cb = b->cfg;
-  if (ca.num_dice != cb.num_dice || ca.num_faces != cb.num_faces)
-    return fail(CFRB_EINVAL, w + ": the agents play different games (" + std::to_string(ca.num_dice) + "x" +
-                                 std::to_string(ca.num_faces) + "f vs " + std::to_string(cb.num_dice) + "x" + std::to_string(cb.num_faces) + "f)");
-  if (ca.max_depth != cb.max_depth)
-    return fail(CFRB_EINVAL, w + ": the agents have different max_depth (" + std::to_string(ca.max_depth) + " vs " +
-                                 std::to_string(cb.max_depth) + ")");
-  if (ca.device != cb.device) return fail(CFRB_EINVAL, w + ": the agents are on different devices");
-  if (ca.state_dtype != cb.state_dtype) return fail(CFRB_EINVAL, w + ": the agents have different state dtypes");
-  for (cfrb_handle* h : {a, b}) {
-    if (h->cfg.max_subgames < n_slots)
-      return fail(CFRB_EINVAL, w + ": a handle's capacity (max_subgames " + std::to_string(h->cfg.max_subgames) +
-                                   ") is smaller than n_slots " + std::to_string(n_slots));
-    if (h->sp.ready) return fail(CFRB_EINVAL, w + ": a handle has a live self-play session");
-    if (h->in_match) return fail(CFRB_EINVAL, w + ": a handle already plays in a live match");
+  cfrb_handle* h[2] = {seat[0].h, n > 1 ? seat[1].h : nullptr};
+  if (n > 1) {
+    const cfrb::GameShape g0 = h[0] ? h[0]->g : seat[0].bp->g, g1 = h[1] ? h[1]->g : seat[1].bp->g;
+    if (g0.D != g1.D || g0.F != g1.F)
+      return fail(CFRB_EINVAL, w + ": the agents play different games (" + std::to_string(g0.D) + "x" + std::to_string(g0.F) + "f vs " +
+                                   std::to_string(g1.D) + "x" + std::to_string(g1.F) + "f)");
+    if ((h[0] ? h[0]->cfg.device : seat[0].bp->device) != (h[1] ? h[1]->cfg.device : seat[1].bp->device))
+      return fail(CFRB_EINVAL, w + ": the agents are on different devices");
+    if (h[0] && h[1]) {
+      const auto &ca = h[0]->cfg, &cb = h[1]->cfg;
+      if (ca.max_depth != cb.max_depth)
+        return fail(CFRB_EINVAL, w + ": the agents have different max_depth (" + std::to_string(ca.max_depth) + " vs " +
+                                     std::to_string(cb.max_depth) + ")");
+      if (ca.state_dtype != cb.state_dtype) return fail(CFRB_EINVAL, w + ": the agents have different state dtypes");
+      if (h[0] == h[1]) return fail(CFRB_EINVAL, w + ": the two agents need two handles (create a second one with the same config)");
+    }
   }
-  m->per_ply = policy != policy_b || policy == CFRB_MATCH_EVERY_NODE;
-  if (m->per_ply) {   // the strategy caches of the to-leaf agents, refused before anything is allocated
-    const int64_t bytes = match_cache_bytes(a, n_slots, policy, policy_b);
-    CK(cudaSetDevice(ca.device));
-    size_t free_b = 0, total_b = 0;
-    CK(cudaMemGetInfo(&free_b, &total_b));
-    int64_t avail = (int64_t)free_b;
-    for (cfrb_handle* h : {a, b})
-      if (h->to_leaf_free_cap > 0) avail = std::min(avail, h->to_leaf_free_cap);
-    if (bytes > avail)
-      return fail(CFRB_ENOMEM, w + ": the to-leaf agents' strategy caches need " + std::to_string(bytes) + " bytes of device memory, " +
-                                   std::to_string(avail) + " free (fewer n_slots need less)");
-  }
-  int rc = match_alloc(m, a, n_slots, n_games, seed);
-  if (rc) return rc;
-  cfrb::MatchDev& d = m->dev;
-  d.sampled = policy == CFRB_MATCH_SAMPLED;
-  d.iters[0] = ca.num_iters; d.iters[1] = cb.num_iters;
-  d.policy[0] = policy; d.policy[1] = policy_b;
-  cfrb_handle* hs[2] = {a, b};
+  const cfrb_handle* first = nullptr;
+  int64_t cap = 0;   // the smallest cfrb_debug_to_leaf_free_cap of the handles
   for (int k = 0; k < 2; ++k) {
-    cfrb_handle* h = hs[k];
-    d.wave[k] = h->d_wave.p; d.sg_tmpl[k] = h->d_sg_tmpl.p; d.sg_player[k] = h->d_sg_player.p; d.sg_row_off[k] = h->d_sg_row_off.p;
-    d.sg_act[k] = h->d_sg_act.p; d.steps[k] = h->d_steps.p;
+    if (!h[k]) continue;
+    const int room = h[k]->cfg.max_subgames;
+    if (lbr && room < h[k]->g.A - 1)
+      return fail(CFRB_EINVAL, w + ": the agent's handle capacity (max_subgames " + std::to_string(room) + ") must hold the A - 1 = " +
+                                   std::to_string(h[k]->g.A - 1) + " what-if subgames of one LBR decision");
+    if (!lbr && room < n_slots)
+      return fail(CFRB_EINVAL, w + ": " + name(k) + "'s handle capacity (max_subgames " + std::to_string(room) +
+                                   ") is smaller than n_slots " + std::to_string(n_slots));
+    if (int rc = handle_free(h[k], w, name(k) + "'s handle")) return rc;
+    if (!first) first = h[k];
+    if (h[k]->to_leaf_free_cap > 0) cap = cap > 0 ? std::min(cap, h[k]->to_leaf_free_cap) : h[k]->to_leaf_free_cap;
   }
-  if (m->per_ply) {
-    if ((rc = ply_alloc(m, who))) return rc;
-    cfrb::ply_launch_deal(d, a->own_stream);
-  } else {
-    cfrb::match_launch_deal(d, a->own_stream);
-  }
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(a->own_stream));
-  m->h[0] = a; m->h[1] = b;
-  a->in_match = b->in_match = true;
-  m->live = true;
+  if (walk != Walk::PerPly) return CFRB_OK;
+  // the per-ply walk's strategy caches of the to-leaf handle seats (a blueprint needs none)
+  auto policy = [&](int k) { return h[k] ? seat[k].policy : (int32_t)CFRB_MATCH_EVERY_NODE; };
+  const int64_t bytes = first ? cache_bytes(first->table_stride, n_slots, policy(0), policy(1)) : 0;
+  if (bytes == 0) return CFRB_OK;
+  CK(cudaSetDevice(first->cfg.device));
+  int64_t avail = 0;
+  if (int rc = free_device_bytes(cap, &avail)) return rc;
+  if (bytes > avail)
+    return fail(CFRB_ENOMEM, w + ": the to-leaf agents' strategy caches need " + std::to_string(bytes) + " bytes of device memory, " +
+                                 std::to_string(avail) + " free (fewer n_slots need less)");
   return CFRB_OK;
 }
 
@@ -3595,21 +3607,8 @@ static int match_alloc_game(cfrb_match* m, int device, const cfrb::GameShape& g,
   return CFRB_OK;
 }
 
-// match_alloc_game with agent a's game, stream and tree templates.
-static int match_alloc(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed) {
-  const int rc = match_alloc_game(m, a->cfg.device, a->g, a->cfg.max_depth, a->d_matches.p, n_slots, n_games, seed);
-  if (rc) return rc;
-  m->stream = a->own_stream;
-  cfrb::MatchDev& d = m->dev;
-  d.tmpl = a->d_tmpl.p; d.child_begin = a->d_child_begin.p; d.nchild = a->d_nchild.p;
-  d.level_begin = a->d_level_begin.p;
-  d.table_stride = a->table_stride;
-  return CFRB_OK;
-}
-
 // The per-ply walk's per-agent state; the caches of the to-leaf agents only.
-static int ply_alloc(cfrb_match* m, const char* who) {
-  (void)who;
+static int ply_alloc(cfrb_match* m) {
   const int S = m->S, G = m->G;
   for (auto* p : {&m->awidx, &m->sub_lb, &m->sub_player, &m->sub_node, &m->sub_depth}) CK(p->alloc((size_t)2 * S));
   CK(m->solves_k.alloc((size_t)2 * G));
@@ -3625,178 +3624,6 @@ static int ply_alloc(cfrb_match* m, const char* who) {
       d.cache[k] = m->cache[k].p;
     }
   }
-  return CFRB_OK;
-}
-
-int cfrb_match_create(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out) {
-  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create: null argument");
-  *out = nullptr;
-  auto m = std::make_unique<cfrb_match>();
-  const int rc = match_create_impl(m.get(), a, b, n_slots, n_games, seed, policy, policy, "cfrb_match_create");
-  if (rc != CFRB_OK) return rc;
-  *out = m.release();
-  return CFRB_OK;
-}
-
-int64_t cfrb_match_cache_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t n_slots, int32_t policy_a,
-                               int32_t policy_b) {
-  if (num_dice < 1 || num_faces < 1 || max_depth < 1 || n_slots < 1)
-    return fail(CFRB_EINVAL, "cfrb_match_cache_bytes: num_dice, num_faces, max_depth, n_slots must be >= 1");
-  if (!valid_policy(policy_a) || !valid_policy(policy_b)) return fail(CFRB_EINVAL, "cfrb_match_cache_bytes: bad policy");
-  const cfrb::GameShape g(num_dice, num_faces);
-  // the game root's template is the largest: A - 1 nodes at depth 1 and C(A, d) at depth d >= 2 (to_leaf_sizes)
-  const int64_t nmax = to_leaf_sizes(g, max_depth, 1).nmax;
-  const int64_t stride = round_up((int)std::max<int64_t>(1, (nmax - 1) * g.H), 4);
-  return cache_bytes(stride, n_slots, policy_a, policy_b);
-}
-
-int cfrb_match_create2(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy_a,
-                       int32_t policy_b, cfrb_match** out) {
-  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create2: null argument");
-  *out = nullptr;
-  auto m = std::make_unique<cfrb_match>();
-  const int rc = match_create_impl(m.get(), a, b, n_slots, n_games, seed, policy_a, policy_b, "cfrb_match_create2");
-  if (rc != CFRB_OK) return rc;
-  *out = m.release();
-  return CFRB_OK;
-}
-
-// A per-ply match with a blueprint in one seat or both (cfrb_match_create3).  A handle agent plays as in cfrb_match_create2.
-static int match_create3_impl(cfrb_match* m, const cfrb_match_agent* ag, int32_t n_slots, int32_t n_games, uint64_t seed) {
-  const std::string w = "cfrb_match_create3";
-  int device = -1;
-  cfrb::GameShape g;
-  for (int k = 0; k < 2; ++k) {
-    const cfrb_match_agent& x = ag[k];
-    const std::string who = w + ": agent " + (k ? "b" : "a");
-    if (x.bp) {
-      if (x.h) return fail(CFRB_EINVAL, who + " has both a handle and a blueprint");
-    } else {
-      if (x.h->sp.ready) return fail(CFRB_EINVAL, who + "'s handle has a live self-play session");
-      if (x.h->in_match) return fail(CFRB_EINVAL, who + "'s handle already plays in a live match");
-      if (x.h->cfg.max_subgames < n_slots)
-        return fail(CFRB_EINVAL, who + "'s handle capacity (max_subgames " + std::to_string(x.h->cfg.max_subgames) +
-                                     ") is smaller than n_slots " + std::to_string(n_slots));
-    }
-    const int dev = x.bp ? x.bp->device : x.h->cfg.device;
-    const cfrb::GameShape gk = x.bp ? x.bp->g : x.h->g;
-    if (k == 0) { device = dev; g = gk; continue; }
-    if (gk.D != g.D || gk.F != g.F)
-      return fail(CFRB_EINVAL, w + ": the agents play different games (" + std::to_string(g.D) + "x" + std::to_string(g.F) + "f vs " +
-                                   std::to_string(gk.D) + "x" + std::to_string(gk.F) + "f)");
-    if (dev != device) return fail(CFRB_EINVAL, w + ": the agents are on different devices");
-  }
-  const int k = ag[0].h ? 0 : ag[1].h ? 1 : -1;   // the handle agent, if any
-  if (k >= 0 && ag[k].policy != CFRB_MATCH_EVERY_NODE) {   // its strategy cache, refused before anything is allocated
-    const int64_t bytes = cache_bytes(ag[k].h->table_stride, n_slots, ag[k].policy, CFRB_MATCH_EVERY_NODE);
-    CK(cudaSetDevice(device));
-    size_t free_b = 0, total_b = 0;
-    CK(cudaMemGetInfo(&free_b, &total_b));
-    int64_t avail = (int64_t)free_b;
-    if (ag[k].h->to_leaf_free_cap > 0) avail = std::min(avail, ag[k].h->to_leaf_free_cap);
-    if (bytes > avail)
-      return fail(CFRB_ENOMEM, w + ": the to-leaf agent's strategy cache needs " + std::to_string(bytes) + " bytes of device memory, " +
-                                   std::to_string(avail) + " free (fewer n_slots need less)");
-  }
-  int rc;
-  if (k >= 0) {
-    rc = match_alloc(m, ag[k].h, n_slots, n_games, seed);
-  } else {
-    const cfrb_blueprint* b = ag[0].bp;
-    rc = match_alloc_game(m, device, b->g, 1 << 30, b->matches.p, n_slots, n_games, seed);
-    if (!rc) {
-      CK(cudaStreamCreateWithFlags(m->own_stream.put(), cudaStreamNonBlocking));
-      m->stream = m->own_stream;
-    }
-  }
-  if (rc) return rc;
-  cfrb::MatchDev& d = m->dev;
-  m->per_ply = true;
-  CK(m->bp_node.alloc((size_t)2 * n_slots));
-  for (int j = 0; j < 2; ++j) {
-    const cfrb_match_agent& x = ag[j];
-    if (x.bp) {
-      d.policy[j] = cfrb::kPlyBlueprint; d.iters[j] = 0;
-      d.bp[j] = x.bp->table.p; d.bp_child_begin[j] = x.bp->child_begin.p; d.bp_node[j] = m->bp_node.p + (size_t)j * n_slots;
-      continue;
-    }
-    cfrb_handle* h = x.h;
-    d.policy[j] = x.policy; d.iters[j] = h->cfg.num_iters;
-    d.wave[j] = h->d_wave.p; d.sg_tmpl[j] = h->d_sg_tmpl.p; d.sg_player[j] = h->d_sg_player.p; d.sg_row_off[j] = h->d_sg_row_off.p;
-    d.sg_act[j] = h->d_sg_act.p; d.steps[j] = h->d_steps.p;
-  }
-  if ((rc = ply_alloc(m, w.c_str()))) return rc;
-  cfrb::ply_launch_deal(d, m->stream);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(m->stream));
-  for (int j = 0; j < 2; ++j) {
-    m->h[j] = ag[j].h;
-    if (ag[j].h) ag[j].h->in_match = true;
-  }
-  m->live = true;
-  return CFRB_OK;
-}
-
-int cfrb_match_create3(const cfrb_match_agent* a, const cfrb_match_agent* b, int32_t n_slots, int32_t n_games, uint64_t seed,
-                       cfrb_match** out) {
-  const std::string w = "cfrb_match_create3";
-  if (!out || !a || !b) return fail(CFRB_EINVAL, w + ": null argument");
-  *out = nullptr;
-  for (const cfrb_match_agent* x : {a, b})
-    if (!x->h && !x->bp) return fail(CFRB_EINVAL, w + ": an agent needs a handle or a blueprint");
-  if (!a->bp && !b->bp) return cfrb_match_create2(a->h, b->h, n_slots, n_games, seed, a->policy, b->policy, out);
-  for (const cfrb_match_agent* x : {a, b})
-    if (x->h && !valid_policy(x->policy))
-      return fail(CFRB_EINVAL, w + ": bad policy (" + std::to_string(x->policy) + "): CFRB_MATCH_AVERAGE, CFRB_MATCH_SAMPLED or "
-                                   "CFRB_MATCH_EVERY_NODE");
-  if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
-  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
-  auto m = std::make_unique<cfrb_match>();
-  const cfrb_match_agent ag[2] = {*a, *b};
-  const int rc = match_create3_impl(m.get(), ag, n_slots, n_games, seed);
-  if (rc != CFRB_OK) return rc;
-  *out = m.release();
-  return CFRB_OK;
-}
-
-static int lbr_alloc(cfrb_match* m);
-
-static int lbr_create_impl(cfrb_match* m, cfrb_handle* a, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy,
-                           const char* who) {
-  const std::string w(who);
-  if (!a) return fail(CFRB_EINVAL, w + ": null handle");
-  if (policy == CFRB_MATCH_SAMPLED)
-    return fail(CFRB_EINVAL, w + ": CFRB_MATCH_SAMPLED is not supported: LBR would have to respond to the expectation over the "
-                                 "agent's act_iteration draws, and the drawn snapshot is information the agent's opponent does not have");
-  if (policy != CFRB_MATCH_AVERAGE && policy != CFRB_MATCH_EVERY_NODE)
-    return fail(CFRB_EINVAL, w + ": bad policy (" + std::to_string(policy) + "): CFRB_MATCH_AVERAGE or CFRB_MATCH_EVERY_NODE");
-  if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
-  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
-  if (a->sp.ready) return fail(CFRB_EINVAL, w + ": the handle has a live self-play session");
-  if (a->in_match) return fail(CFRB_EINVAL, w + ": the handle already plays in a live match");
-  const int A = a->g.A;
-  if (a->cfg.max_subgames < A - 1)
-    return fail(CFRB_EINVAL, w + ": the handle's capacity (max_subgames " + std::to_string(a->cfg.max_subgames) +
-                                 ") must hold the A - 1 = " + std::to_string(A - 1) + " what-if subgames of one LBR decision");
-  int rc = match_alloc(m, a, n_slots, n_games, seed);
-  if (rc) return rc;
-  cfrb::MatchDev& d = m->dev;
-  d.sampled = 0;
-  d.iters[0] = a->cfg.num_iters;
-  d.wave[0] = a->d_wave.p; d.sg_tmpl[0] = a->d_sg_tmpl.p; d.sg_player[0] = a->d_sg_player.p; d.sg_row_off[0] = a->d_sg_row_off.p;
-  d.sg_act[0] = a->d_sg_act.p; d.steps[0] = a->d_steps.p;
-  if ((rc = lbr_alloc(m))) return rc;
-  cfrb::LbrDev& l = m->ldev;
-  l.K = a->cfg.max_subgames;
-  l.every_node = policy == CFRB_MATCH_EVERY_NODE;
-  cfrb::match_launch_deal(d, a->own_stream);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(a->own_stream));
-  l.m = d;
-  m->lbr = true;
-  m->h[0] = a;
-  a->in_match = true;
-  m->live = true;
   return CFRB_OK;
 }
 
@@ -3823,59 +3650,132 @@ static int lbr_alloc(cfrb_match* m) {
   return CFRB_OK;
 }
 
-// LBR against a blueprint: no handle, a stream of the match's own, one game per slot and round (lbr_blueprint_kernel).
-static int lbr_blueprint_impl(cfrb_match* m, cfrb_blueprint* bp, int32_t n_slots, int32_t n_games, uint64_t seed) {
-  const std::string w = "cfrb_match_create_lbr_blueprint";
-  if (!bp) return fail(CFRB_EINVAL, w + ": null blueprint");
-  if (n_slots < 1) return fail(CFRB_EINVAL, w + ": n_slots must be >= 1");
-  if (n_games < 2 || n_games % 2) return fail(CFRB_EINVAL, w + ": n_games must be even and >= 2 (seat-swapped pairs)");
-  int rc = match_alloc_game(m, bp->device, bp->g, 1 << 30, bp->matches.p, n_slots, n_games, seed);
+// Seat k of the walk: handle h's wave descriptors, iterations and policy (LBR's agent leaves the policy 0: LbrDev::every_node
+// says how it plays).
+static void seat_handle(cfrb::MatchDev& d, int k, const cfrb_handle* h, int32_t policy) {
+  d.iters[k] = h->cfg.num_iters; d.policy[k] = policy;
+  d.wave[k] = h->d_wave.p; d.sg_tmpl[k] = h->d_sg_tmpl.p; d.sg_player[k] = h->d_sg_player.p; d.sg_row_off[k] = h->d_sg_row_off.p;
+  d.sg_act[k] = h->d_sg_act.p; d.steps[k] = h->d_steps.p;
+}
+
+// Seat k of the walk: blueprint bp's table and full tree (LBR reads them from LbrDev, the per-ply walk per seat).
+static void seat_blueprint(cfrb_match* m, int k, const cfrb_blueprint* bp) {
+  if (m->walk == Walk::LbrBlueprint) {
+    m->ldev.bp = bp->table.p; m->ldev.bp_child_begin = bp->child_begin.p;
+    return;
+  }
+  cfrb::MatchDev& d = m->dev;
+  d.policy[k] = cfrb::kPlyBlueprint;
+  d.bp[k] = bp->table.p; d.bp_child_begin[k] = bp->child_begin.p; d.bp_node[k] = m->bp_node.p + (size_t)k * m->S;
+}
+
+// A match of `walk` between seats match_check passed: the game, stream and templates of the first handle seat (of the first
+// blueprint and a stream of its own when there is no handle), the seats, the walk's state, and the deal.
+static int match_open(cfrb_match* m, const cfrb_match_agent* seat, int n, Walk walk, int32_t n_slots, int32_t n_games,
+                      uint64_t seed) {
+  const cfrb_handle* a = seat[0].h ? seat[0].h : n > 1 ? seat[1].h : nullptr;
+  int rc = a ? match_alloc_game(m, a->cfg.device, a->g, a->cfg.max_depth, a->d_matches.p, n_slots, n_games, seed)
+             : match_alloc_game(m, seat[0].bp->device, seat[0].bp->g, 1 << 30, seat[0].bp->matches.p, n_slots, n_games, seed);
   if (rc) return rc;
-  CK(cudaStreamCreateWithFlags(m->own_stream.put(), cudaStreamNonBlocking));
-  m->stream = m->own_stream;
-  if ((rc = lbr_alloc(m))) return rc;
-  cfrb::LbrDev& l = m->ldev;
-  l.bp = bp->table.p; l.bp_child_begin = bp->child_begin.p;
-  cfrb::match_launch_deal(m->dev, m->stream);
+  m->walk = walk;
+  cfrb::MatchDev& d = m->dev;
+  if (a) {
+    m->stream = a->own_stream;
+    d.tmpl = a->d_tmpl.p; d.child_begin = a->d_child_begin.p; d.nchild = a->d_nchild.p;
+    d.level_begin = a->d_level_begin.p;
+    d.table_stride = a->table_stride;
+  } else {
+    CK(cudaStreamCreateWithFlags(m->own_stream.put(), cudaStreamNonBlocking));
+    m->stream = m->own_stream;
+  }
+  const bool any_bp = seat[0].bp || (n > 1 && seat[1].bp);
+  d.sampled = !any_bp && seat[0].policy == CFRB_MATCH_SAMPLED;   // the to-leaf walk's shared policy
+  if (walk == Walk::PerPly && any_bp) CK(m->bp_node.alloc((size_t)2 * n_slots));
+  for (int k = 0; k < n; ++k) {
+    if (seat[k].h) seat_handle(d, k, seat[k].h, is_lbr(walk) ? 0 : seat[k].policy);
+    else seat_blueprint(m, k, seat[k].bp);
+  }
+  if (walk == Walk::PerPly) {
+    if ((rc = ply_alloc(m))) return rc;
+    cfrb::ply_launch_deal(d, m->stream);
+  } else {
+    if (is_lbr(walk) && (rc = lbr_alloc(m))) return rc;
+    if (walk == Walk::Lbr) {
+      m->ldev.K = a->cfg.max_subgames;
+      m->ldev.every_node = seat[0].policy == CFRB_MATCH_EVERY_NODE;
+    }
+    cfrb::match_launch_deal(d, m->stream);
+  }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(m->stream));
-  l.m = m->dev;
-  m->lbr = true;
+  if (is_lbr(walk)) m->ldev.m = d;
+  for (int k = 0; k < n; ++k) {
+    m->h[k] = seat[k].h;
+    if (seat[k].h) seat[k].h->in_match = true;
+  }
   m->live = true;
   return CFRB_OK;
 }
 
-static int lbr_create(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out,
-                      const char* who) {
-  if (!out) return fail(CFRB_EINVAL, std::string(who) + ": null argument");
-  *out = nullptr;
-  auto m = std::make_unique<cfrb_match>();
-  const int rc = lbr_create_impl(m.get(), agent, n_slots, n_games, seed, policy, who);
-  if (rc != CFRB_OK) return rc;
-  *out = m.release();
-  return CFRB_OK;
+// Every match creator: n = 2 seats play a match, n = 1 seat is the agent LBR plays against.
+static int match_create(const char* who, const char* empty, const cfrb_match_agent* seat, int n, int32_t n_slots, int32_t n_games,
+                        uint64_t seed, cfrb_match** out) {
+  return make_object(out, who, [&](cfrb_match* m) -> int {
+    const Walk walk = match_walk(seat, n);
+    const int rc = match_check(seat, n, walk, n_slots, n_games, who, empty);
+    return rc ? rc : match_open(m, seat, n, walk, n_slots, n_games, seed);
+  });
+}
+
+static const char* kNullHandles = "null handle (local best response against one agent is cfrb_match_create_lbr or cfrb_match_create_lbr2)";
+
+int cfrb_match_create(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out) {
+  const cfrb_match_agent seat[2] = {{a, nullptr, policy}, {b, nullptr, policy}};
+  return match_create("cfrb_match_create", kNullHandles, seat, 2, n_slots, n_games, seed, out);
+}
+
+int64_t cfrb_match_cache_bytes(int32_t num_dice, int32_t num_faces, int32_t max_depth, int32_t n_slots, int32_t policy_a,
+                               int32_t policy_b) {
+  if (num_dice < 1 || num_faces < 1 || max_depth < 1 || n_slots < 1)
+    return fail(CFRB_EINVAL, "cfrb_match_cache_bytes: num_dice, num_faces, max_depth, n_slots must be >= 1");
+  if (!valid_policy(policy_a) || !valid_policy(policy_b)) return fail(CFRB_EINVAL, "cfrb_match_cache_bytes: bad policy");
+  const cfrb::GameShape g(num_dice, num_faces);
+  // the game root's template is the largest: A - 1 nodes at depth 1 and C(A, d) at depth d >= 2 (to_leaf_sizes)
+  const int64_t nmax = to_leaf_sizes(g, max_depth, 1).nmax;
+  const int64_t stride = round_up((int)std::max<int64_t>(1, (nmax - 1) * g.H), 4);
+  return cache_bytes(stride, n_slots, policy_a, policy_b);
+}
+
+int cfrb_match_create2(cfrb_handle* a, cfrb_handle* b, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy_a,
+                       int32_t policy_b, cfrb_match** out) {
+  const cfrb_match_agent seat[2] = {{a, nullptr, policy_a}, {b, nullptr, policy_b}};
+  return match_create("cfrb_match_create2", kNullHandles, seat, 2, n_slots, n_games, seed, out);
+}
+
+int cfrb_match_create3(const cfrb_match_agent* a, const cfrb_match_agent* b, int32_t n_slots, int32_t n_games, uint64_t seed,
+                       cfrb_match** out) {
+  if (!a || !b) return fail(CFRB_EINVAL, "cfrb_match_create3: null argument");
+  const cfrb_match_agent seat[2] = {*a, *b};
+  return match_create("cfrb_match_create3", "an agent needs a handle or a blueprint", seat, 2, n_slots, n_games, seed, out);
 }
 
 int cfrb_match_create_lbr(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out) {
-  return lbr_create(agent, n_slots, n_games, seed, CFRB_MATCH_AVERAGE, out, "cfrb_match_create_lbr");
+  const cfrb_match_agent seat{agent, nullptr, CFRB_MATCH_AVERAGE};
+  return match_create("cfrb_match_create_lbr", "null handle", &seat, 1, n_slots, n_games, seed, out);
 }
 
 int cfrb_match_create_lbr2(cfrb_handle* agent, int32_t n_slots, int32_t n_games, uint64_t seed, int32_t policy, cfrb_match** out) {
-  return lbr_create(agent, n_slots, n_games, seed, policy, out, "cfrb_match_create_lbr2");
+  const cfrb_match_agent seat{agent, nullptr, policy};
+  return match_create("cfrb_match_create_lbr2", "null handle", &seat, 1, n_slots, n_games, seed, out);
 }
 
 int cfrb_match_create_lbr_blueprint(cfrb_blueprint* bp, int32_t n_slots, int32_t n_games, uint64_t seed, cfrb_match** out) {
-  if (!out) return fail(CFRB_EINVAL, "cfrb_match_create_lbr_blueprint: null argument");
-  *out = nullptr;
-  auto m = std::make_unique<cfrb_match>();
-  const int rc = lbr_blueprint_impl(m.get(), bp, n_slots, n_games, seed);
-  if (rc != CFRB_OK) return rc;
-  *out = m.release();
-  return CFRB_OK;
+  const cfrb_match_agent seat{nullptr, bp, CFRB_MATCH_AVERAGE};
+  return match_create("cfrb_match_create_lbr_blueprint", "null blueprint", &seat, 1, n_slots, n_games, seed, out);
 }
 
 int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* beliefs) {
-  if (!m || !m->lbr) return fail(CFRB_EINVAL, "cfrb_match_lbr_trace: not an LBR match");
+  if (!m || !is_lbr(m->walk)) return fail(CFRB_EINVAL, "cfrb_match_lbr_trace: not an LBR match");
   if (game < 0 || game >= m->T) return fail(CFRB_EINVAL, "cfrb_match_lbr_trace: only games < min(n_games, CFRB_MATCH_TRACE_GAMES) are traced");
   int rc = match_settle(m);
   if (rc) return rc;
@@ -3888,7 +3788,7 @@ int cfrb_match_lbr_trace(cfrb_match* m, int32_t game, double* values, double* be
 }
 
 int cfrb_match_lbr_counts(cfrb_match* m, int64_t* whatif_solves, int64_t* deferred_slot_rounds) {
-  if (!m || !m->lbr) return fail(CFRB_EINVAL, "cfrb_match_lbr_counts: not an LBR match");
+  if (!m || !is_lbr(m->walk)) return fail(CFRB_EINVAL, "cfrb_match_lbr_counts: not an LBR match");
   int rc = match_settle(m);
   if (rc) return rc;
   std::vector<int> w(m->G);
@@ -3918,10 +3818,10 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
     if (rc) return rc;
     // one wave per agent; LBR: one wave of at most max_subgames subgames of the agent
     for (cfrb_handle* h : m->h)
-      if (h && (rc = solve_device_wave(h, m->lbr ? h->cfg.max_subgames : m->S, false, false, st))) return rc;
+      if (h && (rc = solve_device_wave(h, m->walk == Walk::Lbr ? h->cfg.max_subgames : m->S, false, false, st))) return rc;
     CK(cudaMemsetAsync(m->left.p, 0, sizeof(int), st));
     if ((rc = match_kernels(m, false, st))) return rc;
-    if (counter) counter->launches += m->per_ply && (m->dev.cache[0] || m->dev.cache[1]) ? 4 : 3;
+    if (counter) counter->launches += m->walk == Walk::PerPly && (m->dev.cache[0] || m->dev.cache[1]) ? 4 : 3;
   }
   CK(cudaMemcpyAsync(m->pin_left, m->left.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   CK(cudaEventRecord(m->ev_left, st));
@@ -3929,14 +3829,17 @@ int cfrb_match_run(cfrb_match* m, int32_t max_rounds, void* cuda_stream) {
   return max_rounds;
 }
 
-// Subgames agent 0 and agent 1 solved in a per-ply match (after match_settle).
-static int match_agent_solves(cfrb_match* m, int64_t* out) {
-  std::vector<int> n((size_t)2 * m->G);
-  CK(cudaMemcpy(n.data(), m->solves_k.p, n.size() * sizeof(int), cudaMemcpyDeviceToHost));
-  for (int k = 0; k < 2; ++k) {
-    out[k] = 0;
-    for (int g = 0; g < m->G; ++g) out[k] += n[(size_t)k * m->G + g];
-  }
+// Subgames agent a and agent b solved (after match_settle): in the to-leaf walk both solve every round; LBR's agent solves every
+// subgame of its games, the what-if ones included, and LBR none; in the per-ply walk each agent counts its own.
+static int match_solves(cfrb_match* m, int64_t n[2]) {
+  const int G = m->G, rows = m->walk == Walk::PerPly ? 2 : 1;
+  const int* src = m->walk == Walk::PerPly ? m->solves_k.p : m->walk == Walk::ToLeaf ? m->rounds.p : m->solves_g.p;
+  std::vector<int> c((size_t)rows * G);
+  CK(cudaMemcpy(c.data(), src, c.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  n[0] = n[1] = 0;
+  for (int k = 0; k < rows; ++k)
+    for (int g = 0; g < G; ++g) n[k] += c[(size_t)k * G + g];
+  if (m->walk == Walk::ToLeaf) n[1] = n[0];
   return CFRB_OK;
 }
 
@@ -3945,41 +3848,19 @@ int cfrb_match_results(cfrb_match* m, float* payoff_a, int32_t* plies, int64_t* 
   int rc = match_settle(m);
   if (rc) return rc;
   const int G = m->G;
-  std::vector<int> rounds(G);
-  CK(cudaMemcpy(rounds.data(), m->lbr ? m->solves_g.p : m->rounds.p, (size_t)G * sizeof(int), cudaMemcpyDeviceToHost));
   if (payoff_a) CK(cudaMemcpy(payoff_a, m->payoff.p, (size_t)G * sizeof(float), cudaMemcpyDeviceToHost));
   if (plies) CK(cudaMemcpy(plies, m->plies.p, (size_t)G * sizeof(int), cudaMemcpyDeviceToHost));
-  int64_t r = 0;
-  for (int x : rounds) r += x;
-  if (m->lbr) {                       // every subgame the agent solved, the what-if ones included
-    if (solves) *solves = r;
-    if (subgame_iters) *subgame_iters = r * (int64_t)m->dev.iters[0];
-    return CFRB_OK;
-  }
-  if (m->per_ply) {                       // each agent's own solves
-    int64_t n[2];
-    if ((rc = match_agent_solves(m, n))) return rc;
-    if (solves) *solves = n[0] + n[1];
-    if (subgame_iters) *subgame_iters = n[0] * (int64_t)m->dev.iters[0] + n[1] * (int64_t)m->dev.iters[1];
-    return CFRB_OK;
-  }
-  if (solves) *solves = 2 * r;
-  if (subgame_iters) *subgame_iters = r * ((int64_t)m->dev.iters[0] + m->dev.iters[1]);
+  int64_t n[2];
+  if ((rc = match_solves(m, n))) return rc;
+  if (solves) *solves = n[0] + n[1];
+  if (subgame_iters) *subgame_iters = n[0] * (int64_t)m->dev.iters[0] + n[1] * (int64_t)m->dev.iters[1];
   return CFRB_OK;
 }
 
 int cfrb_match_agent_solves(cfrb_match* m, int64_t* solves) {
   if (!m || !solves) return fail(CFRB_EINVAL, "cfrb_match_agent_solves: null argument");
-  int rc = match_settle(m);
-  if (rc) return rc;
-  if (m->per_ply) return match_agent_solves(m, solves);
-  std::vector<int> n(m->G);
-  CK(cudaMemcpy(n.data(), m->lbr ? m->solves_g.p : m->rounds.p, (size_t)m->G * sizeof(int), cudaMemcpyDeviceToHost));
-  int64_t r = 0;
-  for (int x : n) r += x;
-  solves[0] = r;                      // the to-leaf walk: both agents solve every round; LBR: the agent's solves, LBR none
-  solves[1] = m->lbr ? 0 : r;
-  return CFRB_OK;
+  const int rc = match_settle(m);
+  return rc ? rc : match_solves(m, solves);
 }
 
 int cfrb_match_trace(cfrb_match* m, int32_t game, int32_t* ply_records, double* probs, int32_t* act_iterations, double* root_beliefs,
@@ -4024,36 +3905,36 @@ int cfrb_rows_destroy(cfrb_rows* r) {
 
 int cfrb_rows_create(int32_t device, int64_t capacity_rows, int32_t q_dim, int32_t v_dim, cfrb_rows** out) {
   if (!out || capacity_rows < 1 || q_dim < 1 || v_dim < 1) return fail(CFRB_EINVAL, "bad argument");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(CFRB_ENODEV, "no CUDA device"); }
-  if (device < 0 || device >= ndev) return fail(CFRB_EINVAL, "device ordinal out of range");
-  CK(cudaSetDevice(device));
-  auto r = std::make_unique<cfrb_rows>();
-  r->device = device; r->q_dim = q_dim; r->v_dim = v_dim; r->cap = capacity_rows;
-  cudaError_t e = r->q.alloc((size_t)capacity_rows * q_dim);
-  if (e == cudaSuccess) e = r->v.alloc((size_t)capacity_rows * v_dim);
-  // Highest stream priority: the store's gathers and copies run next to a generator that keeps every SM busy with back-to-back
-  // (programmatically chained) kernels; at equal priority their blocks waited tens of milliseconds for a slot (measured: 47 ms for a
-  // 32 768-row sample, whatever its size), at high priority they take the next slot a retiring CTA frees.
-  int prio_least = 0, prio_greatest = 0;
-  if (e == cudaSuccess) e = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(r->st.put(), cudaStreamNonBlocking, prio_greatest);
-  // gather scratch (row-id slots, staging rows of host-bound batches) for batches of up to min(capacity, 262 144) rows, allocated
-  // HERE: an allocation later, next to a generator that keeps the GPU busy with whole waves, waits for the end of a wave (measured:
-  // 47 ms per sample while the four slots were being created one call at a time)
-  const int64_t scratch_rows = std::min<int64_t>(capacity_rows, 1 << 18);
-  for (auto& s : r->ids) {
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(s.done.put(), cudaEventDisableTiming);
-    if (e == cudaSuccess) e = s.dev.alloc(scratch_rows);
-    if (e == cudaSuccess) e = cudaMallocHost((void**)s.pin.put(), (size_t)scratch_rows * sizeof(int));
-    if (e == cudaSuccess) s.cap = (int)scratch_rows;
-  }
-  if (e == cudaSuccess) e = r->stage_q.alloc((size_t)scratch_rows * q_dim);
-  if (e == cudaSuccess) e = r->stage_v.alloc((size_t)scratch_rows * v_dim);
-  if (e == cudaSuccess) r->stage_rows = (int)scratch_rows;
-  if (e != cudaSuccess) return fail(CFRB_ENOMEM, std::string("cfrb_rows_create: ") + cudaGetErrorString(e));
-  *out = r.release();
-  return CFRB_OK;
+  return make_object(out, "cfrb_rows_create", [&](cfrb_rows* r) -> int {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(CFRB_ENODEV, "no CUDA device"); }
+    if (device < 0 || device >= ndev) return fail(CFRB_EINVAL, "device ordinal out of range");
+    CK(cudaSetDevice(device));
+    r->device = device; r->q_dim = q_dim; r->v_dim = v_dim; r->cap = capacity_rows;
+    cudaError_t e = r->q.alloc((size_t)capacity_rows * q_dim);
+    if (e == cudaSuccess) e = r->v.alloc((size_t)capacity_rows * v_dim);
+    // Highest stream priority: the store's gathers and copies run next to a generator that keeps every SM busy with back-to-back
+    // (programmatically chained) kernels; at equal priority their blocks waited tens of milliseconds for a slot (measured: 47 ms for a
+    // 32 768-row sample, whatever its size), at high priority they take the next slot a retiring CTA frees.
+    int prio_least = 0, prio_greatest = 0;
+    if (e == cudaSuccess) e = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest);
+    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(r->st.put(), cudaStreamNonBlocking, prio_greatest);
+    // gather scratch (row-id slots, staging rows of host-bound batches) for batches of up to min(capacity, 262 144) rows, allocated
+    // HERE: an allocation later, next to a generator that keeps the GPU busy with whole waves, waits for the end of a wave (measured:
+    // 47 ms per sample while the four slots were being created one call at a time)
+    const int64_t scratch_rows = std::min<int64_t>(capacity_rows, 1 << 18);
+    for (auto& s : r->ids) {
+      if (e == cudaSuccess) e = cudaEventCreateWithFlags(s.done.put(), cudaEventDisableTiming);
+      if (e == cudaSuccess) e = s.dev.alloc(scratch_rows);
+      if (e == cudaSuccess) e = cudaMallocHost((void**)s.pin.put(), (size_t)scratch_rows * sizeof(int));
+      if (e == cudaSuccess) s.cap = (int)scratch_rows;
+    }
+    if (e == cudaSuccess) e = r->stage_q.alloc((size_t)scratch_rows * q_dim);
+    if (e == cudaSuccess) e = r->stage_v.alloc((size_t)scratch_rows * v_dim);
+    if (e == cudaSuccess) r->stage_rows = (int)scratch_rows;
+    if (e != cudaSuccess) return fail(CFRB_ENOMEM, std::string("cfrb_rows_create: ") + cudaGetErrorString(e));
+    return CFRB_OK;
+  });
 }
 
 int cfrb_rows_device(const cfrb_rows* r) { return r ? r->device : -1; }
@@ -4222,21 +4103,21 @@ int cfrb_comm_unique_id(uint8_t* out128) {
 
 int cfrb_comm_create(const uint8_t* id128, int32_t rank, int32_t world, int32_t device, cfrb_comm** out) {
   if (!id128 || !out || world < 1 || rank < 0 || rank >= world) return fail(CFRB_EINVAL, "cfrb_comm_create: bad argument");
-  CK(cudaSetDevice(device));
-  auto c = std::make_unique<cfrb_comm>();
-  c->rank = rank; c->world = world; c->device = device;
-  ncclUniqueId id;
-  std::memcpy(&id, id128, 128);
-  ncclComm_t comm = nullptr;
-  ncclResult_t r = ncclCommInitRank(&comm, world, id, rank);
-  if (r != ncclSuccess) return fail(CFRB_ECUDA, std::string("ncclCommInitRank: ") + ncclGetErrorString(r));
-  c->comm = decltype(c->comm)(comm);
-  cudaError_t e = cudaStreamCreateWithFlags(c->st.put(), cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMallocHost((void**)c->pin_vote.put(), 8 * sizeof(int));
-  if (e != cudaSuccess) return fail(CFRB_ECUDA, cudaGetErrorString(e));
-  c->pin_vote_out = c->pin_vote + 4;
-  *out = c.release();
-  return CFRB_OK;
+  return make_object(out, "cfrb_comm_create", [&](cfrb_comm* c) -> int {
+    CK(cudaSetDevice(device));
+    c->rank = rank; c->world = world; c->device = device;
+    ncclUniqueId id;
+    std::memcpy(&id, id128, 128);
+    ncclComm_t comm = nullptr;
+    ncclResult_t r = ncclCommInitRank(&comm, world, id, rank);
+    if (r != ncclSuccess) return fail(CFRB_ECUDA, std::string("ncclCommInitRank: ") + ncclGetErrorString(r));
+    c->comm = decltype(c->comm)(comm);
+    cudaError_t e = cudaStreamCreateWithFlags(c->st.put(), cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMallocHost((void**)c->pin_vote.put(), 8 * sizeof(int));
+    if (e != cudaSuccess) return fail(CFRB_ECUDA, cudaGetErrorString(e));
+    c->pin_vote_out = c->pin_vote + 4;
+    return CFRB_OK;
+  });
 }
 
 int cfrb_comm_destroy(cfrb_comm* c) {
@@ -4440,10 +4321,9 @@ static int agent_create_impl(cfrb_agent* a, cfrb_handle* h, int32_t n_tables, ui
   if (h->cfg.max_subgames < n_tables)
     return fail(CFRB_EINVAL, "cfrb_agent_create: the handle's capacity (max_subgames " + std::to_string(h->cfg.max_subgames) +
                                  ") is smaller than n_tables " + std::to_string(n_tables) + " (one wave solves every listed table)");
-  if (h->sp.ready) return fail(CFRB_EINVAL, "cfrb_agent_create: the handle has a live self-play session");
-  if (h->in_match) return fail(CFRB_EINVAL, "cfrb_agent_create: the handle already plays in a live match or agent");
-  int rc = agent_alloc(a, h->cfg.device, h->g, n_tables, h->table_stride);
+  int rc = handle_free(h, "cfrb_agent_create", "the handle");
   if (rc) return rc;
+  if ((rc = agent_alloc(a, h->cfg.device, h->g, n_tables, h->table_stride))) return rc;
   a->sampled = policy == CFRB_MATCH_SAMPLED;
   cfrb::AgentDev& d = a->dev;
   d.max_depth = h->cfg.max_depth; d.sampled = a->sampled; d.iters = h->cfg.num_iters; d.seed = seed;
@@ -4511,23 +4391,13 @@ static int agent_blueprint_impl(cfrb_agent* a, const cfrb_blueprint* bp, int32_t
 extern "C" {
 
 int cfrb_agent_create(cfrb_handle* h, int32_t n_tables, uint64_t seed, int32_t policy, cfrb_agent** out) {
-  if (!out) return fail(CFRB_EINVAL, "cfrb_agent_create: null argument");
-  *out = nullptr;
-  auto a = std::make_unique<cfrb_agent>();
-  const int rc = agent_create_impl(a.get(), h, n_tables, seed, policy);
-  if (rc != CFRB_OK) return rc;
-  *out = a.release();
-  return CFRB_OK;
+  return make_object(out, "cfrb_agent_create",
+                     [&](cfrb_agent* a) -> int { return agent_create_impl(a, h, n_tables, seed, policy); });
 }
 
 int cfrb_agent_create_blueprint(cfrb_blueprint* bp, int32_t n_tables, uint64_t seed, cfrb_agent** out) {
-  if (!out) return fail(CFRB_EINVAL, "cfrb_agent_create_blueprint: null argument");
-  *out = nullptr;
-  auto a = std::make_unique<cfrb_agent>();
-  const int rc = agent_blueprint_impl(a.get(), bp, n_tables, seed);
-  if (rc != CFRB_OK) return rc;
-  *out = a.release();
-  return CFRB_OK;
+  return make_object(out, "cfrb_agent_create_blueprint",
+                     [&](cfrb_agent* a) -> int { return agent_blueprint_impl(a, bp, n_tables, seed); });
 }
 
 int cfrb_agent_destroy(cfrb_agent* a) {
@@ -4691,42 +4561,41 @@ struct cfrb_trainer {
 
 int cfrb_trainer_create(int32_t device, int32_t num_dice, int32_t num_faces, int32_t max_batch, cfrb_trainer** out) {
   static const char* who = "cfrb_trainer_create: ";
-  if (!out) return fail(CFRB_EINVAL, std::string(who) + "null argument");
-  if (num_dice < 1 || num_faces < 1) return fail(CFRB_EINVAL, std::string(who) + "num_dice and num_faces must be >= 1");
-  if (max_batch < 1) return fail(CFRB_EINVAL, std::string(who) + "max_batch must be >= 1");
-  const cfrb::GameShape g(num_dice, num_faces);
-  if (g.A > 1024 || g.H > 4096) return fail(CFRB_EINVAL, std::string(who) + "game too large");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(CFRB_ENODEV, "no CUDA device visible: libcfrb200 has no CPU fallback");
-  }
-  if (device < 0 || device >= ndev) return fail(CFRB_EINVAL, std::string(who) + "device ordinal out of range");
-  CK(cudaSetDevice(device));
-  auto t = std::make_unique<cfrb_trainer>();
-  t->device = device; t->B = max_batch; t->Q = g.Q; t->H = g.H;
-  t->L = cfrb::train::Layout(g.Q, g.H);
-  const size_t P = (size_t)t->L.total(), BH = (size_t)max_batch * cfrb::train::kHid, BO = (size_t)max_batch * g.H;
-  cudaError_t e = cudaSuccess;
-  for (auto* b : {&t->params, &t->grads, &t->m, &t->v})
-    if (e == cudaSuccess) e = b->alloc(P);
-  for (auto* b : {&t->z1, &t->xh1, &t->a1, &t->z2, &t->xh2, &t->a2, &t->da2, &t->dy2, &t->dz2, &t->da1, &t->dy1, &t->dz1})
-    if (e == cudaSuccess) e = b->alloc(BH);
-  for (auto* b : {&t->rs1, &t->rs2, &t->row_loss})
-    if (e == cudaSuccess) e = b->alloc(max_batch);
-  for (auto* b : {&t->pred, &t->dpred})
-    if (e == cudaSuccess) e = b->alloc(BO);
-  if (e == cudaSuccess) e = t->sq_norms.alloc(cfrb::train::kParams);
-  if (e == cudaSuccess) e = t->last.alloc(2);
-  if (e == cudaSuccess) e = t->step.alloc(1);
-  for (auto* b : {&t->params, &t->grads, &t->m, &t->v})
-    if (e == cudaSuccess) e = cudaMemset(b->p, 0, P * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemset(t->last.p, 0, 2 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemset(t->step.p, 0, sizeof(long long));
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) return fail(CFRB_ENOMEM, std::string(who) + cudaGetErrorString(e));
-  *out = t.release();
-  return CFRB_OK;
+  return make_object(out, "cfrb_trainer_create", [&](cfrb_trainer* t) -> int {
+    if (num_dice < 1 || num_faces < 1) return fail(CFRB_EINVAL, std::string(who) + "num_dice and num_faces must be >= 1");
+    if (max_batch < 1) return fail(CFRB_EINVAL, std::string(who) + "max_batch must be >= 1");
+    const cfrb::GameShape g(num_dice, num_faces);
+    if (g.A > 1024 || g.H > 4096) return fail(CFRB_EINVAL, std::string(who) + "game too large");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+      cudaGetLastError();
+      return fail(CFRB_ENODEV, "no CUDA device visible: libcfrb200 has no CPU fallback");
+    }
+    if (device < 0 || device >= ndev) return fail(CFRB_EINVAL, std::string(who) + "device ordinal out of range");
+    CK(cudaSetDevice(device));
+    t->device = device; t->B = max_batch; t->Q = g.Q; t->H = g.H;
+    t->L = cfrb::train::Layout(g.Q, g.H);
+    const size_t P = (size_t)t->L.total(), BH = (size_t)max_batch * cfrb::train::kHid, BO = (size_t)max_batch * g.H;
+    cudaError_t e = cudaSuccess;
+    for (auto* b : {&t->params, &t->grads, &t->m, &t->v})
+      if (e == cudaSuccess) e = b->alloc(P);
+    for (auto* b : {&t->z1, &t->xh1, &t->a1, &t->z2, &t->xh2, &t->a2, &t->da2, &t->dy2, &t->dz2, &t->da1, &t->dy1, &t->dz1})
+      if (e == cudaSuccess) e = b->alloc(BH);
+    for (auto* b : {&t->rs1, &t->rs2, &t->row_loss})
+      if (e == cudaSuccess) e = b->alloc(max_batch);
+    for (auto* b : {&t->pred, &t->dpred})
+      if (e == cudaSuccess) e = b->alloc(BO);
+    if (e == cudaSuccess) e = t->sq_norms.alloc(cfrb::train::kParams);
+    if (e == cudaSuccess) e = t->last.alloc(2);
+    if (e == cudaSuccess) e = t->step.alloc(1);
+    for (auto* b : {&t->params, &t->grads, &t->m, &t->v})
+      if (e == cudaSuccess) e = cudaMemset(b->p, 0, P * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(t->last.p, 0, 2 * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(t->step.p, 0, sizeof(long long));
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) return fail(CFRB_ENOMEM, std::string(who) + cudaGetErrorString(e));
+    return CFRB_OK;
+  });
 }
 
 int cfrb_trainer_destroy(cfrb_trainer* t) {
